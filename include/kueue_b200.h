@@ -270,6 +270,9 @@ typedef struct kb_stats {
    * multi-column searches (GetTargets of k_nominate_walk),
    * [5..7] SM clock cycles summed over warps: column load / classification / greedy (diagnostics) */
   int64_t search_stat[8];
+  /* after a cycle run by the fused flat-cohort kernel (k_cycle_flat), over the first 1024 entries of the first root:
+   * [0] entries nominated by the group walk (one podset that cannot be reduced), [1] all entries */
+  int64_t flat_group_walk[2];
 } kb_stats;
 
 /* indices into kb_stats.kernel_ms */

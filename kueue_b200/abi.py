@@ -100,6 +100,7 @@ class kb_stats(C.Structure):
         ("last_cycle_gpu_ms", C.c_double), ("last_h2d_ms", C.c_double), ("last_d2h_ms", C.c_double),
         ("h2d_bytes", C.c_int64), ("d2h_bytes", C.c_int64), ("kernel_launches", C.c_int32), ("sm_count", C.c_int32),
         ("kernel_ms", C.c_float * 20), ("search_stat", C.c_int64 * 8),
+        ("flat_group_walk", C.c_int64 * 2),
     ]
 
 

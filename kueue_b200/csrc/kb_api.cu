@@ -1190,6 +1190,7 @@ static int32_t cycle_finish(kb_handle *h) {
     if (h->kev_id[i] >= 0) h->stats.kernel_ms[h->kev_id[i]] += kms;
   }
   memcpy(h->stats.search_stat, h->hdr_host + 8, 64);
+  memcpy(h->stats.flat_group_walk, h->hdr_host + 24, 16);  // DevSnap::sstat[8..9]
   uint32_t st = h->hdr_host[0];
   if (st & KBS_UNSUPPORTED_PREEMPTION) return fail(h, KB_ERR_UNSUPPORTED, "unsupported preemption configuration");
   if (st & KBS_TARGET_OVERFLOW) return fail(h, KB_ERR_CAPACITY, "per-entry usage cell / target pool capacity exceeded");

@@ -19,7 +19,7 @@
 
 struct FlatLay {  // byte offsets into the dynamic shared memory of k_cycle_flat (computed on the host, passed by value)
   uint32_t u, sub, lq, bl, av, pot, over, lend, blob, n_e, n_wl, n_ps0, n_psn, e_gid, e_cq, e_prio, e_ident, e_psn, e_wl, e_ps0, e_ts, e_lg, e_qr,
-      e_mode, e_borrow, e_rank, sorted, m_sorted, d_sorted, r_gid, r_count, r_min, r_mask, r_group, r_ok, r_req, r_last, o_fl, o_md, o_tr, o_cnt, key, misc, snap, rec, total;
+      e_fast, e_mode, e_borrow, e_rank, sorted, m_sorted, d_sorted, r_gid, r_count, r_min, r_mask, r_group, r_ok, r_req, r_last, o_fl, o_md, o_tr, o_cnt, key, misc, snap, rec, total;
 };
 __host__ __device__ inline FlatLay flat_layout(int ncap, int FR, int R, int rcap, int bcap) {
   FlatLay L;
@@ -33,6 +33,7 @@ __host__ __device__ inline FlatLay flat_layout(int ncap, int FR, int R, int rcap
   L.e_gid = take((size_t)ncap * 4); L.e_cq = take((size_t)ncap * 4); L.e_prio = take((size_t)ncap * 4); L.e_ident = take((size_t)ncap * 4);
   L.e_psn = take((size_t)(ncap + 1) * 4); L.e_wl = take((size_t)ncap * 4); L.e_ps0 = take((size_t)ncap * 4);
   L.e_ts = take((size_t)ncap * 8); L.e_lg = take((size_t)ncap * 8); L.e_qr = take((size_t)ncap);
+  L.e_fast = take((size_t)ncap);
   L.e_mode = take((size_t)ncap * 4); L.e_borrow = take((size_t)ncap * 4); L.e_rank = take((size_t)ncap * 4);
   L.sorted = take((size_t)ncap * 4); L.m_sorted = take((size_t)ncap * 4); L.d_sorted = take(((size_t)ncap / 32 + 2) * 4);
   L.r_gid = take((size_t)rcap * 4); L.r_count = take((size_t)rcap * 4); L.r_min = take((size_t)rcap * 4); L.r_mask = take((size_t)rcap * 4);
@@ -181,10 +182,167 @@ __device__ __forceinline__ int flat_decision(int mode, const uint32_t *ok_bits, 
   return mode == KB_MODE_PREEMPT ? KB_DEC_PREEMPT_NO_TARGETS : KB_DEC_NOFIT;
 }
 
+#ifndef KB_FLAT_THREADS
 #define KB_FLAT_THREADS 1024
-#ifndef KB_FLAT_NG
-#define KB_FLAT_NG 8  // lanes per entry in the nominate phase
 #endif
+#ifndef KB_FLAT_NG
+#define KB_FLAT_NG 4  // lanes per entry in the nominate walks
+#endif
+// Entries that do not take the group walk of phase 5 (flat_nominate_group) go through the shared device functions on the relocated snapshot.
+// They are out of line, so that their register needs do not constrain the rest of the kernel.
+__device__ __noinline__ int flat_nominate_general(const DevSnap &L, int i, int *borrowing, unsigned gmask, int gbase, int glane) {
+  bool need_search = false;  // stays false: no ClusterQueue of a relocated view has preemption candidates
+  return get_assignments_coop<KB_FLAT_NG>(L, &need_search, i, borrowing, gmask, gbase, glane);
+}
+__device__ __noinline__ void flat_key_general(const DevSnap &L, int i, u64 *k) { compute_entry_key(L, i, k); }
+__device__ __noinline__ void flat_expand_general(const DevSnap &L, int i, i64 *qrow, int FR) {
+  for (int c = 0; c < FR; c++) qrow[c] = -1;
+  expand_entry(L, i, qrow);
+}
+// Phase 5 of k_cycle_flat for an entry with one podset that cannot be reduced (the usual case): the group walk of
+// findFlavorForPodSets on the shared tables.  One group of NG lanes per entry (as in get_assignments_coop), lane =
+// flavor slot of the resource group being assigned, rounds of NG flavors; the lane evaluates fitsResourceQuota
+// (flavorassigner.go:1017-1047, what cell_eval computes) for each resource of its flavor, reading the shared tables
+// directly instead of through the relocated DevSnap.  On a flat tree every ClusterQueue hangs off the root, so
+// find_height gives 0 or the root's height and mayReclaim is "fits within nominal"; no ClusterQueue has preemption
+// candidates (candidates_possible), so SimulatePreemption is NoCandidates.  The flavors of a round are then taken in
+// order by flavor_take, the rule get_assignments_coop uses.  The group also writes the podset's assignment row, the
+// entry's mode / borrowing and its iterator key.  A group of one podset assigns like the podset alone.
+template <int NG>
+__device__ __forceinline__ void flat_nominate_group(const FlatLay &Y, int i, int R, int FR, unsigned flags, int pods, bool has_qr_table,
+                                                    unsigned gmask, int gbase, int glane) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];  // the kernel's
+  const i64 *s_u = (const i64 *)(smem_raw + Y.u), *s_sub = (const i64 *)(smem_raw + Y.sub), *s_av = (const i64 *)(smem_raw + Y.av),
+            *s_pot = (const i64 *)(smem_raw + Y.pot);
+  const unsigned char *s_blob = smem_raw + Y.blob;
+  const TreeBlobHdr *BH = (const TreeBlobHdr *)s_blob;
+  const int32_t *b_rgs = (const int32_t *)(s_blob + BH->rgs), *b_rgfl = (const int32_t *)(s_blob + BH->rgfl), *b_fl = (const int32_t *)(s_blob + BH->fl);
+  const uint32_t *b_rgmask = (const uint32_t *)(s_blob + BH->rgmask);
+  const i64 *r_req = (const i64 *)(smem_raw + Y.r_req);
+  int8_t *o_fl = (int8_t *)(smem_raw + Y.o_fl), *o_md = (int8_t *)(smem_raw + Y.o_md), *o_tr = (int8_t *)(smem_raw + Y.o_tr);
+  const bool fair = (flags & KB_F_FAIR_SHARING) != 0, fung = (flags & KB_F_FLAVOR_FUNGIBILITY) != 0;
+
+  const int hq = ((const int *)(smem_raw + Y.e_cq))[i], l = ((const int *)(smem_raw + Y.e_psn))[i];
+  const u64 ok = ((const u64 *)(smem_raw + Y.r_ok))[l];
+  const int cnt = ((const int *)(smem_raw + Y.r_count))[l];
+  const i64 lg = ((const i64 *)(smem_raw + Y.e_lg))[i];
+  const bool use_last = fung && lg >= 0 && !(((const i64 *)(s_blob + BH->gen))[hq] > lg);
+  const int pref = s_blob[BH->pref + hq], wcb = s_blob[BH->wcb + hq], wcp = s_blob[BH->wcp + hq];
+  const bool can_pwb = s_blob[BH->borrow_w + hq] != KB_POLICY_NEVER || (fair && s_blob[BH->reclaim + hq] != KB_POLICY_NEVER);  // :1049-1052
+  const int P = ((const int32_t *)(s_blob + BH->par))[hq];
+  const int hp = ((const int32_t *)(s_blob + BH->hgt))[P];  // borrow height of a cell above nominal
+  const int rg0 = b_rgs[hq], rg1 = b_rgs[hq + 1];
+  bool covers = false;  // pods resource flavorassigner.go:585-587
+  if (pods >= 0) for (int g = rg0; g < rg1; g++) if ((b_rgmask[g] >> pods) & 1) covers = true;
+  const uint32_t mask = ((const uint32_t *)(smem_raw + Y.r_mask))[l] | (covers ? 1u << pods : 0u);
+  auto request = [&](int r) { return covers && r == pods ? (i64)cnt : r_req[(size_t)l * R + r]; };  // full count: ps_request unscaled
+  // resource r of the row is written by lane r % NG only, so the row needs no synchronisation within the group
+  for (int r = glane; r < R; r += NG) { o_fl[(size_t)l * R + r] = -1; o_md[(size_t)l * R + r] = -1; o_tr[(size_t)l * R + r] = -1; }
+  uint32_t assigned = 0, ps_pmask = 0;
+  int ps_borrow = 0;
+  bool has_reasons = false, failed = false;
+  for (int r0 = 0; r0 < R; r0++) {  // resource groups in the order of their first requested resource
+    if (!((mask >> r0) & 1) || ((assigned >> r0) & 1)) continue;
+    int g = -1;
+    for (int k = rg0; k < rg1 && g < 0; k++) if ((b_rgmask[k] >> r0) & 1) g = k;
+    if (g < 0) {
+      if (request(r0) == 0) continue;
+      has_reasons = failed = true;
+      break;
+    }
+    const uint32_t rgm = b_rgmask[g] & mask;
+    const int fl0 = b_rgfl[g], nfl = b_rgfl[g + 1] - fl0;
+    int best_f = -1, best_pm = PM_NOFIT, best_rb = INT32_MAX, best_maxb = 0, attempted = -1;
+    uint32_t best_pmask = 0;
+    bool any_reason = false, done = false;
+    for (int base = use_last ? ((const int8_t *)(smem_raw + Y.r_last))[(size_t)l * R + r0] + 1 : 0; base < nfl && !done; base += NG) {
+      // ---- one flavor per lane: representative mode over its resources, as in assign_workload_coop ----
+      const int idx = base + glane;
+      u64 res = 0;  // [0..2] rpm [3..9] rb [10..16] maxb [17] any_reason [19] eligible [20..27] flavor [32..63] pmask
+      if (idx < nfl) {
+        const int f = b_fl[fl0 + idx];
+        if ((ok >> f) & 1) {  // ps_flavor_ok: checkFlavorForPodSets
+          int rpm = PM_FIT, rb = 0, maxb = 0; uint32_t pmask = 0; bool reason = false;
+          for (int r = 0; r < R; r++) {
+            if (!((rgm >> r) & 1)) continue;
+            const int c = hq * FR + f * R + r;
+            const i64 val = request(r);
+            int pm = PM_NOFIT, b = 0;
+            if (val <= s_pot[c]) {  // cell_eval: find_height on a flat tree is the root's height above nominal, mayReclaim below
+              const bool above = s_u[c] + val > s_sub[c];  // nominal == SubtreeQuota for a ClusterQueue
+              b = above ? hp : 0;
+              pm = fits_mode(val, s_av[c], s_sub[c], !above, [&] { return can_pwb; });
+              if (pm == PM_NEED) pm = PM_NOCAND;  // no candidates: what SimulatePreemption returns
+            }
+            if (pm != PM_FIT) reason = true;
+            if (gm_preferred(rpm, rb, pm, b, pref)) { rpm = pm; rb = b; }
+            if (rpm == PM_NOFIT) break;
+            if (fa_mode(pm) == KB_MODE_PREEMPT) pmask |= 1u << r;
+            if (b > maxb) maxb = b;
+          }
+          res = (u64)rpm | ((u64)(rb & 127) << 3) | ((u64)(maxb & 127) << 10) | ((u64)reason << 17) | (1ull << 19) | ((u64)f << 20) |
+                ((u64)pmask << 32);
+        }
+      }
+      // ---- ordered walk over the flavors of this round ----
+      for (int j = 0; j < NG && base + j < nfl; j++) {
+        const u64 rj = __shfl_sync(gmask, res, gbase + j);
+        attempted = base + j;
+        if (!((rj >> 19) & 1)) { any_reason = true; continue; }
+        const int rpm = (int)(rj & 7), rb = (int)((rj >> 3) & 127);
+        if ((rj >> 17) & 1) any_reason = true;
+        if (flavor_take(fung, wcb, wcp, pref, rpm, rb, best_pm, best_rb, &done)) {
+          best_f = (int)((rj >> 20) & 255); best_pm = rpm; best_rb = rb; best_maxb = (int)((rj >> 10) & 127); best_pmask = (uint32_t)(rj >> 32);
+        }
+        if (done) break;
+      }
+    }
+    if (best_f < 0) { has_reasons = failed = true; break; }
+    const int tried = fung ? (attempted == nfl - 1 ? -1 : attempted) : 0;
+    for (int r = glane; r < R; r += NG)
+      if ((rgm >> r) & 1) { o_fl[(size_t)l * R + r] = (int8_t)best_f; o_md[(size_t)l * R + r] = (best_pmask >> r) & 1 ? KB_MODE_PREEMPT : KB_MODE_FIT; o_tr[(size_t)l * R + r] = (int8_t)tried; }
+    assigned |= rgm;
+    ps_pmask |= best_pmask & rgm;
+    if (best_maxb > ps_borrow) ps_borrow = best_maxb;
+    if (best_pm != PM_FIT && any_reason) has_reasons = true;
+  }
+  int mode = KB_MODE_FIT, borrowing = 0;
+  if (failed) {
+    mode = KB_MODE_NOFIT;
+    for (int r = glane; r < R; r += NG) { o_fl[(size_t)l * R + r] = -1; o_md[(size_t)l * R + r] = -1; o_tr[(size_t)l * R + r] = -1; }
+  } else {
+    borrowing = ps_borrow;
+    if (has_reasons) mode = (assigned & mask) == 0 ? KB_MODE_NOFIT : ((ps_pmask & mask) ? KB_MODE_PREEMPT : KB_MODE_FIT);
+  }
+  // iterator key: max over the resources of the DominantResourceShare terms of entry_share_ratio
+  double best = 0.0;
+  if (fair) {
+    const i64 *s_over = (const i64 *)(smem_raw + Y.over), *s_lend = (const i64 *)(smem_raw + Y.lend);
+    for (int r = glane; r < R; r += NG) {
+      i64 bo = s_over[hq * R + r];
+      const int f = o_fl[(size_t)l * R + r];
+      if (f >= 0) {
+        const int c = hq * FR + f * R + r;
+        const i64 q = request(r), base = s_u[c] - s_sub[c];
+        bo += imax(0, base + (q > 0 ? q : 0)) - imax(0, base);
+      }
+      const i64 lend = s_lend[P * R + r];
+      const double ratio = (bo > 0 && lend > 0) ? (double)bo * 1000.0 / (double)lend : 0.0;
+      if (ratio > best) best = ratio;
+    }
+    for (int o = NG >> 1; o > 0; o >>= 1) { const double x = __shfl_xor_sync(gmask, best, o); if (x > best) best = x; }
+  }
+  if (glane == 0) {
+    ((int *)(smem_raw + Y.o_cnt))[l] = cnt;
+    ((int *)(smem_raw + Y.e_mode))[i] = mode; ((int *)(smem_raw + Y.e_borrow))[i] = borrowing;
+    (smem_raw + Y.e_fast)[i] = covers ? 3 : 1;
+    entry_key_pack(flags, fair, best, fair ? ((const double *)(s_blob + BH->wgt))[hq] : 0.0, ((const int *)(smem_raw + Y.e_prio))[i],
+                   ((const i64 *)(smem_raw + Y.e_ts))[i], has_qr_table && (smem_raw + Y.e_qr)[i], borrowing,
+                   fair ? (unsigned)((const int32_t *)(s_blob + BH->gid))[hq] : (unsigned)((const int *)(smem_raw + Y.e_gid))[i],
+                   (u64 *)(smem_raw + Y.key) + (size_t)i * 4);
+  }
+}
+
 __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_constant__ DevSnap D, const __grid_constant__ FlatLay Y) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int FR = D.FR, R = D.R;
@@ -207,6 +365,7 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
   int *e_gid = (int *)(smem_raw + Y.e_gid), *e_cq = (int *)(smem_raw + Y.e_cq), *e_prio = (int *)(smem_raw + Y.e_prio), *e_ident = (int *)(smem_raw + Y.e_ident);
   int *e_psn = (int *)(smem_raw + Y.e_psn), *e_wl = (int *)(smem_raw + Y.e_wl), *e_ps0 = (int *)(smem_raw + Y.e_ps0);
   i64 *e_ts = (i64 *)(smem_raw + Y.e_ts), *e_lg = (i64 *)(smem_raw + Y.e_lg); uint8_t *e_qr = smem_raw + Y.e_qr;
+  uint8_t *e_fast = smem_raw + Y.e_fast;  // bit 0: nominated by the group walk of phase 5, bit 1: its ClusterQueue covers the pods resource
   int *e_mode = (int *)(smem_raw + Y.e_mode), *e_borrow = (int *)(smem_raw + Y.e_borrow), *e_rank = (int *)(smem_raw + Y.e_rank);
   int *s_sorted = (int *)(smem_raw + Y.sorted), *m_sorted = (int *)(smem_raw + Y.m_sorted); uint32_t *ok_bits = (uint32_t *)(smem_raw + Y.d_sorted);
   int *r_gid = (int *)(smem_raw + Y.r_gid), *r_count = (int *)(smem_raw + Y.r_count), *r_min = (int *)(smem_raw + Y.r_min);
@@ -408,6 +567,7 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
     const int ps0 = e_ps0[i], l0 = e_psn[i], np = e_psn[i + 1] - l0;
     const int pr = __ldg(D.wl_priority + wl); const i64 ts = __ldg(D.wl_ts + wl), lg = __ldg(D.wl_last_gen + wl);
     const uint8_t qr = D.wl_has_qr ? __ldg(D.wl_has_qr + wl) : 0;
+    bool fast = np == 1;  // see phase 5
     for (int k = 0; k < np; k++) {
       const int row = ps0 + k, l = l0 + k;
       const int cnt = __ldg(D.ps_count + row), mn = __ldg(D.ps_min_count + row); const uint32_t msk = __ldg(D.ps_req_mask + row);
@@ -420,69 +580,82 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
         for (int j = 0; j < 4; j++) if (r0 + j < R) { r_req[(size_t)l * R + r0 + j] = q[j]; r_last[(size_t)l * R + r0 + j] = lt[j]; }
       }
       r_gid[l] = row; r_count[l] = cnt; r_min[l] = mn; r_mask[l] = msk; r_group[l] = grp; r_ok[l] = ok;
+      if ((D.flags & KB_F_PARTIAL_ADMISSION) && mn >= 0 && cnt > mn) fast = false;
     }
-    e_prio[i] = pr; e_ts[i] = ts; e_lg[i] = lg; e_qr[i] = qr;
+    e_prio[i] = pr; e_ts[i] = ts; e_lg[i] = lg; e_qr[i] = qr; e_fast[i] = fast;
   }
   KB_PP(1, 6);
-  for (int i = tid; i < tb; i += nthreads) {
-    const int fr = col_of(i);
-    const i64 sub = s_sub[i], u = s_u[i];
-    const i64 lq = local_quota(sub, s_lq[i]);
-    s_lq[i] = lq;
-    if (i < FR) { s_av[i] = sub - u; s_pot[i] = sub; }
-    else {
-      const i64 bl = s_bl[i];
-      i64 pa = s_sub[fr] - s_u[fr], pot = lq + s_sub[fr];
-      if (bl != KB_NO_LIMIT) { pa = imin((sub - lq) - imax(0, u - lq) + bl, pa); pot = imin(sub + bl, pot); }
-      s_av[i] = imax(0, lq - u) + pa;
+  // fair sharing inputs (k_fair_prep): over-usage per (ClusterQueue, resource), lendable per (node, resource).  When a
+  // row is one aligned segment of a warp they are summed over the flavors by shuffles in this sweep (phase 4 otherwise)
+  const bool fair = (D.flags & KB_F_FAIR_SHARING) != 0;  // every tree is flat here: all entries take the fair flat key
+  const bool fair_rows = fair && FR <= 32 && fr_p2 && (R & (R - 1)) == 0;
+  const int tb_sweep = fair_rows ? (tb + 31) & ~31 : tb;
+  for (int i = tid; i < tb_sweep; i += nthreads) {
+    i64 pot = 0, over = 0;
+    if (i < tb) {
+      const int fr = col_of(i);
+      const i64 sub = s_sub[i], u = s_u[i];
+      const i64 lq = local_quota(sub, s_lq[i]);
+      s_lq[i] = lq;
+      if (i < FR) { s_av[i] = sub - u; pot = sub; }
+      else {
+        const i64 bl = s_bl[i];
+        i64 pa = s_sub[fr] - s_u[fr];
+        pot = lq + s_sub[fr];
+        if (bl != KB_NO_LIMIT) { pa = imin((sub - lq) - imax(0, u - lq) + bl, pa); pot = imin(sub + bl, pot); }
+        s_av[i] = imax(0, lq - u) + pa;
+      }
       s_pot[i] = pot;
+      over = imax(0, u - sub);
+    }
+    if (fair_rows) {
+      i64 lend = pot;
+      for (int o = R; o < FR; o <<= 1) { lend += __shfl_xor_sync(0xffffffffu, lend, o); over += __shfl_xor_sync(0xffffffffu, over, o); }
+      if (i < tb && col_of(i) < R) { const int h = row_of(i); s_lend[h * R + col_of(i)] = lend; s_over[h * R + col_of(i)] = over; }
     }
   }
   KB_PP(1, 7);
-  __syncthreads();
+  {
+    const int walked = __syncthreads_count(tid < n && e_fast[tid]);  // e_fast of entry tid was written by this thread
+    if (blockIdx.x == 0 && tid == 0) { D.sstat[8] = (u64)walked; D.sstat[9] = (u64)min(n, nthreads); }  // CTA 0: group walk / entries, of the first nthreads
+  }
   KB_FPHASE(2);
   KB_PP(2, 0);
   const DevSnap &L = *(const DevSnap *)(smem_raw + Y.snap);
-  // ---- 4. fair sharing inputs (k_fair_prep): over-usage per (ClusterQueue, resource), lendable per (node, resource)
-  if (D.flags & KB_F_FAIR_SHARING) {
+  // ---- 4. fair sharing inputs of rows that do not fit a warp segment
+  if (fair && !fair_rows) {
     const int Fn = D.F;
-    const bool r_p2 = (R & (R - 1)) == 0;
-    if (FR <= 32 && fr_p2 && r_p2) {  // a row is one aligned segment of a warp: sum over the flavors by shuffles
-      const int tb32 = (tb + 31) & ~31;
-      for (int i = tid; i < tb32; i += nthreads) {
-        i64 lend = 0, over = 0;
-        if (i < tb) { lend = s_pot[i]; const i64 o = s_u[i] - s_sub[i]; over = o > 0 ? o : 0; }
-        for (int o = R; o < FR; o <<= 1) { lend += __shfl_xor_sync(0xffffffffu, lend, o); over += __shfl_xor_sync(0xffffffffu, over, o); }
-        if (i < tb && col_of(i) < R) { const int h = row_of(i); s_lend[h * R + col_of(i)] = lend; s_over[h * R + col_of(i)] = over; }
+    for (int i = tid; i < nn * R; i += nthreads) {
+      const int h = i / R, r = i % R;
+      i64 over = 0, lend = 0;
+      for (int f = 0; f < Fn; f++) {
+        const int c = h * FR + f * R + r;
+        lend += s_pot[c];
+        const i64 o = s_u[c] - s_sub[c];
+        if (o > 0) over += o;
       }
-    } else {
-      for (int i = tid; i < nn * R; i += nthreads) {
-        const int h = i / R, r = i % R;
-        i64 over = 0, lend = 0;
-        for (int f = 0; f < Fn; f++) {
-          const int c = h * FR + f * R + r;
-          lend += s_pot[c];
-          const i64 o = s_u[c] - s_sub[c];
-          if (o > 0) over += o;
-        }
-        s_lend[i] = lend; s_over[i] = over;
-      }
+      s_lend[i] = lend; s_over[i] = over;
     }
+    __syncthreads();  // the group walk below reads s_over / s_lend for the iterator key
   }
   KB_PP(2, 1);
-  // ---- 5. nominate: KB_FLAT_NG lanes per entry (get_assignments_coop) on the relocated tables.  A round evaluates
-  // KB_FLAT_NG flavors of a resource group at once; the walk usually stops in its first round, so fewer lanes per entry
-  // mean fewer warps competing for the SM's issue slots at the same chain length.
+  // ---- 5. nominate (getInitialAssignments, scheduler.go:584-625): KB_FLAT_NG lanes per entry.  Entries with one
+  // podset that cannot be reduced take the group walk on the shared tables (flat_nominate_group); every other entry
+  // (several podsets, or partial admission with a reducible podset) takes get_assignments_coop on the relocated
+  // snapshot L.  A round evaluates KB_FLAT_NG flavors of a resource group at once; the walk usually stops in its first
+  // round, so fewer lanes per entry mean fewer warps competing for the SM's issue slots at the same chain length.
   {
     const int glane = lane % KB_FLAT_NG, gbase = lane - glane;
     const unsigned gmask = (KB_FLAT_NG == 32 ? 0xffffffffu : ((1u << KB_FLAT_NG) - 1u)) << gbase;
     const int groups = nthreads / KB_FLAT_NG;
     for (int i0 = 0; i0 < n; i0 += groups) {
       const int i = i0 + tid / KB_FLAT_NG;
-      if (i < n) {  // whole lane groups take the branch together
-        bool need_search = false;
+      if (i >= n) continue;  // whole lane groups take the branches together
+      if (e_fast[i] & 1) {
+        flat_nominate_group<KB_FLAT_NG>(Y, i, R, FR, D.flags, D.pods_res, D.wl_has_qr != nullptr, gmask, gbase, glane);
+      } else {
         int borrowing;
-        const int mode = get_assignments_coop<KB_FLAT_NG>(L, &need_search, i, &borrowing, gmask, gbase, glane);
+        const int mode = flat_nominate_general(L, i, &borrowing, gmask, gbase, glane);
         if (glane == 0) { e_mode[i] = mode; e_borrow[i] = borrowing; }
       }
     }
@@ -491,35 +664,34 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
   __syncthreads();
   KB_FPHASE(3);
   KB_PP(2, 3);
-  // ---- 6. iterator keys (threads of the lower half) | dense request rows (upper half); avail / potential are dead
-  i64 *s_q = s_av;    // [n][FR] Assignment.Usage.Quota per entry, absent = -1
+  // ---- 6. dense request rows (Assignment.Usage.Quota per entry, absent = -1) and, for the entries of the general
+  // walk, iterator keys; avail / potential are dead from here on
+  i64 *s_q = s_av;    // [n][FR]
   i64 *s_lim = s_pot; // [n][FR] thresholds in iterator order
-  const bool fair = (D.flags & KB_F_FAIR_SHARING) != 0;  // every tree is flat here: all entries take the fair flat key
-  double *s_ratio = (double *)s_key;                     // [n][4] terms of the DominantResourceShare, in the entry's key slots
-  const bool split = fair && R <= 4;
-  for (int c = tid; c < n * FR; c += nthreads) s_q[c] = -1;  // row-major: a row per thread would hit one bank 32 ways
-  __syncthreads();
+  {
+    const bool r_p2 = (R & (R - 1)) == 0;
+    const int r_sh = 31 - __clz(R);
+    for (int c = tid; c < n * FR; c += nthreads) {  // the group walk's entries, cell-parallel (one podset: the row is its request)
+      const int i = row_of(c);
+      const int fb = e_fast[i];
+      if (!(fb & 1)) continue;
+      const int fr = col_of(c), f = r_p2 ? fr >> r_sh : fr / R, r = fr - f * R;
+      const int l = e_psn[i];
+      i64 q = -1;
+      if (o_fl[(size_t)l * R + r] == f) q = (fb & 2) && r == D.pods_res ? (i64)o_cnt[l] : r_req[(size_t)l * R + r];
+      s_q[c] = q;
+    }
+  }
   KB_PP(2, 4);
   {
     const int half = nthreads / 2;
-    if (tid < half) {
-      if (split) { for (int c = tid; c < n * R; c += half) s_ratio[(size_t)(c / R) * 4 + c % R] = entry_share_ratio(L, c / R, c % R); }  // one division per thread
-      else for (int i = tid; i < n; i += half) compute_entry_key(L, i, s_key + (size_t)i * 4);
-    } else {
-      for (int i = tid - half; i < n; i += half) {
-        expand_entry(L, i, s_q + (size_t)i * FR);
-      }
+    for (int i = tid < half ? tid : tid - half; i < n; i += half) {
+      if (e_fast[i] & 1) continue;
+      if (tid < half) flat_key_general(L, i, s_key + (size_t)i * 4);
+      else flat_expand_general(L, i, s_q + (size_t)i * FR, FR);
     }
   }
   KB_PP(2, 5);
-  if (split) {
-    __syncthreads();
-    for (int i = tid; i < n; i += nthreads) {
-      double best = 0.0;
-      for (int r = 0; r < R; r++) { const double ratio = s_ratio[(size_t)i * 4 + r]; if (ratio > best) best = ratio; }
-      entry_key_finish(L, i, true, best, s_key + (size_t)i * 4);  // overwrites the entry's own four slots
-    }
-  }
   KB_PP(2, 6);
   __syncthreads();
   KB_FPHASE(4);

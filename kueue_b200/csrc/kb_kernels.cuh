@@ -160,6 +160,20 @@ __device__ __forceinline__ bool gm_preferred(int apm, int ab, int bpm, int bb, i
 __device__ __forceinline__ int fa_mode(int pm) {  // flavorAssignmentMode :470-485
   return pm == PM_NOFIT ? KB_MODE_NOFIT : (pm == PM_FIT ? KB_MODE_FIT : KB_MODE_PREEMPT);
 }
+// One step of findFlavorForPodSets' ordered flavor walk: does the next flavor, with representative mode rpm and borrow
+// height rb over its resources, replace the best one so far, and does the walk stop there (*done)?  With fungibility
+// the walk stops at the first flavor whenCanBorrow / whenCanPreempt accept and otherwise keeps the preferred one
+// (isPreferred); without it the flavor with the better mode wins and a Fit stops the walk.
+__device__ __forceinline__ bool flavor_take(bool fung, int wcb, int wcp, int pref, int rpm, int rb, int best_pm, int best_rb, bool *done) {
+  if (fung) {
+    const bool try_next = rpm == PM_NOFIT || rpm == PM_NOCAND || ((rpm == PM_PREEMPT || rpm == PM_RECLAIM) && wcp == KB_FUNG_TRY_NEXT_FLAVOR) ||
+                          (rb != 0 && wcb == KB_FUNG_TRY_NEXT_FLAVOR);
+    if (!try_next) { *done = true; return true; }
+    return gm_preferred(rpm, rb, best_pm, best_rb, pref);
+  }
+  if (rpm > best_pm) { *done = rpm == PM_FIT; return true; }
+  return false;
+}
 __device__ __forceinline__ int rg_by_resource(const DevSnap &D, int cq, int r) {  // RGByResource clusterqueue_snapshot.go:67-74
   for (int g = D.cq_rg_start[cq]; g < D.cq_rg_start[cq + 1]; g++)
     if (D.rg_res_mask[g] & (1u << r)) return g;
@@ -420,20 +434,24 @@ __device__ inline int get_assignments(const DevSnap &D, Oracle &orc, int wl, int
 #define KB_NG 8
 enum { PM_NEED = 5 };
 
-// fitsResourceQuota :1017-1047 without the oracle call: PM_NEED where SimulatePreemption would run.
+// fitsResourceQuota :1017-1047 for a quantity val <= potentialAvailable: Fit within available, else PM_NEED where
+// SimulatePreemption would run (within nominal, the lowest fitting subtree is below the root, or preemption while
+// borrowing is allowed: can_pwb(), asked only then), else NoFit.
+template <typename PwbFn>
+__device__ __forceinline__ int fits_mode(i64 val, i64 avail, i64 nominal, bool may_reclaim, PwbFn can_pwb) {
+  if (val <= imax(0, avail)) return PM_FIT;
+  return (val <= nominal || may_reclaim || can_pwb()) ? PM_NEED : PM_NOFIT;
+}
+// fitsResourceQuota without the oracle call: PM_NEED where SimulatePreemption would run.
 __device__ __forceinline__ int cell_eval(const DevSnap &D, int cq, int fr, i64 assumed, i64 request, int *borrow) {
   size_t c = (size_t)nix(D, cq) * D.FR + fr;
-  i64 avail = imax(0, D.avail[c]);
   i64 val = assumed + request;
   if (val > D.potential[c]) { *borrow = 0; return PM_NOFIT; }
   bool may_reclaim;
-  int b = find_height(D, D.usage, cq, fr, val, &may_reclaim);
-  *borrow = b;
-  if (val <= avail) return PM_FIT;
-  bool can_pwb = D.cq_borrow_within[cq] != KB_POLICY_NEVER ||
-                 ((D.flags & KB_F_FAIR_SHARING) && D.cq_reclaim_within[cq] != KB_POLICY_NEVER);
-  if (val <= D.nominal[c] || may_reclaim || can_pwb) return PM_NEED;
-  return PM_NOFIT;
+  *borrow = find_height(D, D.usage, cq, fr, val, &may_reclaim);
+  return fits_mode(val, D.avail[c], D.nominal[c], may_reclaim, [&] {
+    return D.cq_borrow_within[cq] != KB_POLICY_NEVER || ((D.flags & KB_F_FAIR_SHARING) && D.cq_reclaim_within[cq] != KB_POLICY_NEVER);
+  });
 }
 
 template <int NG = KB_NG>  // lanes per entry (a power of two <= 32): NG flavors of a resource group are evaluated per round
@@ -533,18 +551,7 @@ __device__ inline int assign_workload_coop(const DevSnap &D, bool *need_search, 
           uint32_t pmask = (uint32_t)(rj >> 32) & 0xffffu;
           if ((rj >> 17) & 1) any_reason = true;
           if ((rj >> 18) & 1) *need_search = true;  // the sequential walk would have called SimulatePreemption here
-          bool take = false;
-          if (fung) {
-            bool try_next = rpm == PM_NOFIT || rpm == PM_NOCAND ||
-                            ((rpm == PM_PREEMPT || rpm == PM_RECLAIM) && wcp == KB_FUNG_TRY_NEXT_FLAVOR) ||
-                            (rb != 0 && wcb == KB_FUNG_TRY_NEXT_FLAVOR);
-            if (!try_next) { take = true; done = true; }
-            else if (gm_preferred(rpm, rb, best_pm, best_rb, pref)) take = true;
-          } else if (rpm > best_pm) {
-            take = true;
-            done = rpm == PM_FIT;
-          }
-          if (take) { best_f = fj; best_pm = rpm; best_rb = rb; best_maxb = maxb; best_pmask = pmask; }
+          if (flavor_take(fung, wcb, wcp, pref, rpm, rb, best_pm, best_rb, &done)) { best_f = fj; best_pm = rpm; best_rb = rb; best_maxb = maxb; best_pmask = pmask; }
           if (done) break;
         }
       }
@@ -1186,25 +1193,32 @@ __device__ __forceinline__ bool entry_key_is_fair_flat(const DevSnap &D, int e) 
   const int P = D.parent[nix(D, cq)];
   return (D.flags & KB_F_FAIR_SHARING) && P >= 0 && (D.tab_local == 2 ? D.local_flat != 0 : D.tree_flat[D.root_slot[cq] - D.nLone] != 0);
 }
-// The 4 x u64 key; `best` = max over the resources of entry_share_ratio (only read on the fair flat path).
+// The 4 x u64 key from the entry's fields: `best` = max over the resources of entry_share_ratio and `weight` the
+// ClusterQueue's fair weight (both only read on the fair flat path); `ident` = the ClusterQueue's node id on the fair
+// flat path, else the entry id.
+__device__ __forceinline__ void entry_key_pack(unsigned flags, bool fair_flat, double best, double weight, int priority, i64 wl_ts,
+                                               bool has_qr, int borrow, unsigned ident, u64 *k) {
+  unsigned prio = 0;
+  if (flags & KB_F_PRIORITY_SORTING_WITHIN_COHORT) prio = ~((unsigned)priority ^ 0x80000000u);  // signed priority, descending
+  const u64 ts = (u64)wl_ts ^ 0x8000000000000000ull;
+  if (!fair_flat) {
+    // workloads that already hold a quota reservation (second pass) first: scheduler.go:781-789
+    const u64 no_qr = has_qr ? 0ull : 1ull;
+    k[0] = (no_qr << 63) | ((u64)(unsigned)borrow << 32) | prio; k[1] = ts; k[2] = (u64)ident; k[3] = 0;
+    return;
+  }
+  const bool zwb = weight == 0 && best != 0;
+  const double value = zwb ? best : (best == 0 ? 0.0 : best / weight);
+  const u64 vb = (u64)__double_as_longlong(value);  // value >= 0: the bit pattern is monotone
+  const u64 kf = ((flags & KB_F_FS_PRIORITIZE_NON_BORROWING) && borrow > 0 ? 2 : 0) | (zwb ? 1 : 0);
+  k[0] = (kf << 32) | (vb >> 32); k[1] = (vb << 32) | prio; k[2] = ts; k[3] = (u64)ident;
+}
 __device__ inline void entry_key_finish(const DevSnap &D, int e, bool fair_flat, double best, u64 *k) {
   const int wl = D.heads[e];
   const int cq = D.wl_cq[wl];
-  unsigned prio = 0;
-  if (D.flags & KB_F_PRIORITY_SORTING_WITHIN_COHORT) prio = ~((unsigned)D.wl_priority[wl] ^ 0x80000000u);  // signed priority, descending
-  const u64 ts = (u64)D.wl_ts[wl] ^ 0x8000000000000000ull;
-  if (!fair_flat) {
-    // workloads that already hold a quota reservation (second pass) first: scheduler.go:781-789
-    const u64 no_qr = (D.wl_has_qr && D.wl_has_qr[wl]) ? 0ull : 1ull;
-    k[0] = (no_qr << 63) | ((u64)(unsigned)D.borrow[e] << 32) | prio; k[1] = ts; k[2] = (u64)(unsigned)(D.ent_gid ? D.ent_gid[e] : e); k[3] = 0;
-    return;
-  }
-  const double w = D.fair_weight[cq];
-  const bool zwb = w == 0 && best != 0;
-  const double value = zwb ? best : (best == 0 ? 0.0 : best / w);
-  const u64 vb = (u64)__double_as_longlong(value);  // value >= 0: the bit pattern is monotone
-  const u64 flags = ((D.flags & KB_F_FS_PRIORITIZE_NON_BORROWING) && D.borrow[e] > 0 ? 2 : 0) | (zwb ? 1 : 0);
-  k[0] = (flags << 32) | (vb >> 32); k[1] = (vb << 32) | prio; k[2] = ts; k[3] = (u64)(unsigned)(D.node_gid ? D.node_gid[cq] : cq);
+  const bool has_qr = D.wl_has_qr && D.wl_has_qr[wl];
+  const unsigned ident = fair_flat ? (unsigned)(D.node_gid ? D.node_gid[cq] : cq) : (unsigned)(D.ent_gid ? D.ent_gid[e] : e);
+  entry_key_pack(D.flags, fair_flat, best, fair_flat ? D.fair_weight[cq] : 0.0, D.wl_priority[wl], D.wl_ts[wl], has_qr, D.borrow[e], ident, k);
 }
 __device__ inline void compute_entry_key(const DevSnap &D, int e, u64 *k) {
   const bool fair_flat = entry_key_is_fair_flat(D, e);
