@@ -216,6 +216,43 @@ typedef struct kb_snapshot {
   int32_t n_usage_delta;            /* rows in the two tables below                                   */
   const int32_t *usage_delta_cq;    /* [n_usage_delta] ClusterQueue index, each at most once; NULL = cq_usage is the full table */
   const int64_t *usage_delta_rows;  /* [n_usage_delta][F*R] the rows' new values (same layout as a cq_usage row) */
+
+  /* ---- AdmissionFairSharing (optional; read by kb_run_drain).  wl_lq == NULL: AFS is off and every other table of
+     this block is ignored.  With afs.Enabled(cfg) (the AdmissionFairSharing gate on and the Configuration's
+     admissionFairSharing set), a ClusterQueue whose spec.admissionScope.admissionMode is UsageBasedAdmissionFairSharing
+     orders its queue by LocalQueue usage first (queueOrderingFunc, pkg/cache/queue/cluster_queue.go:636-685):
+       usage(lq) = sum_r afs_res_weight[r] * AsApproximateFloat64(consumed_r (+) penalty_r), then / lq_weight[lq]
+     (Info.CalcLocalQueueFSUsage, pkg/workload/workload.go:391-427), where (+) is Quantity.Add (int64Amount.Add,
+     apimachinery amount.go:162-199: a zero operand keeps the other's scale, otherwise the sum takes the smaller scale)
+     and AsApproximateFloat64 is value * Pow10(scale) (quantity.go:468-483; Pow10(-k) = 1 / 10^k).  Canonical choices:
+     Go sums over a map in random order, the library sums in resource-index order; after penalties the reference's Pop
+     (rebuildAll + heap.Fix per item in map order, cluster_queue.go:494-531) may return a workload that is not the
+     minimum, the library takes the true minimum of (usage, -priority, timestamp, UID) over the LocalQueue heads.  The
+     sticky workload is not modelled.  Every admitted workload of such a ClusterQueue adds its entry penalty to its
+     LocalQueue (scheduler.go:727-742,946-960; pkg/util/admissionfairsharing/admission_fair_sharing.go):
+       penalty_r += int64(float64(MilliValue(SumTotalRequests_r)) * afs_alpha)   (milli-units, truncated toward zero)
+     over the workload's full TotalRequests (ps_req where ps_req_mask has bit r, before partial admission).
+     Errors: KB_ERR_INVALID for an index out of range, lq_cq[wl_lq[w]] != wl_cq[w] or LocalQueues not numbered
+     ClusterQueue-major; KB_ERR_UNSUPPORTED for a scale outside [-22, 22] or a sum that overflows int64 (the reference
+     would leave the int64Amount form for inf.Dec).
+     Preemption guard: with AFS, CandidatesOrdering (preemption/common/ordering.go:41-100) compares LocalQueue usage only
+     between candidates of one ClusterQueue, which is not a transitive order across ClusterQueues, so the order
+     slices.SortFunc produces depends on the sort algorithm.  kb_run_cycle, kb_upload and kb_run_drain therefore return
+     KB_ERR_UNSUPPORTED when wl_lq != NULL, some cq_afs is set and some ClusterQueue has a preemption policy (a target
+     search is possible); the caller then runs the Go cycle.  Without a possible target search kb_run_cycle accepts the
+     tables and ignores them: the heads of a single cycle come from the caller's queue. ---- */
+  int32_t n_lq;                     /* LocalQueues                                                                  */
+  const int32_t *wl_lq;             /* [n_wl] LocalQueue of each pending workload (Spec.QueueName); NULL = AFS off  */
+  const int32_t *lq_cq;             /* [n_lq] ClusterQueue of each LocalQueue; non-decreasing (ClusterQueue-major)  */
+  const uint8_t *cq_afs;            /* [n_cq] afs.ResourceWeights(cq.Spec.AdmissionScope, cfg) enabled (admission_fair_sharing.go) */
+  const double  *lq_weight;         /* [n_lq] Spec.FairSharing.Weight.AsApproximateFloat64(), 1.0 when nil          */
+  const int64_t *lq_consumed;       /* [n_lq][R] AfsConsumedResources entry as int64Amount values (0 = absent)      */
+  const int32_t *lq_consumed_scale; /* [n_lq][R] their scales (resource.Scale: value * 10^scale)                    */
+  const int64_t *lq_penalty;        /* [n_lq][R] AfsEntryPenalties.Peek at the start, milli-units; NULL = none      */
+  const double  *afs_res_weight;    /* [R] AdmissionFairSharing.ResourceWeights, 1 for a resource not listed        */
+  const int64_t *afs_milli_mul;     /* [R] MilliValue factor of the library's unit: 1 for cpu (milli), else 1000   */
+  double afs_alpha;                 /* 1 - 0.5^(UsageSamplingInterval / UsageHalfLifeTime), 0 when the half-life is 0
+                                       (calculateAlphaRate); computed by the caller so the Go shim passes math.Pow's bits */
 } kb_snapshot;
 
 /* ------------------------------------------------------------------------
@@ -263,7 +300,8 @@ typedef struct kb_stats {
   int32_t kernel_launches;       /* kernels of this library launched by the last call    */
   int32_t sm_count;
   /* per-kernel device time of the last kb_cycle_resident when kb_set_profile(h, 1):
-   * CUDA events recorded on the launching stream around each kernel. */
+   * CUDA events recorded on the launching stream around each kernel.  After kb_run_drain: summed over its cycles,
+   * KB_K_DRAIN = the queue layer after every cycle (decisions applied, admissions, penalties, next heads). */
   float   kernel_ms[KB_N_KERNELS];
   /* target-search counters of the last cycle: [0] searches run, [1] candidate records classified (32 B each),
    * [2] candidates visited by the greedy loops, [3] workloads removed (incl. fill-back), [4] the part of [1] classified by
@@ -336,7 +374,13 @@ int32_t kb_download(kb_handle *h, kb_cycle_out *out);
  *                              becomes the head; a NoFit head with a known wl_sched_hash also sets aside every queued
  *                              workload of its class (handleInadmissibleHash, cluster_queue.go:408-425).
  * Evictions are asynchronous in the reference and are not replayed: the targets of a Preempting entry stay admitted.
- * Cycle c runs with now_ns + c.  Bit-exact with iterating kb_run_cycle under the same rules (kueue_b200/drain.py). */
+ * Cycle c runs with now_ns + c.  Bit-exact with iterating kb_run_cycle under the same rules (kueue_b200/drain.py).
+ * With the AdmissionFairSharing tables (kb_snapshot.wl_lq != NULL), the queue of a ClusterQueue with cq_afs set is one
+ * segment per LocalQueue, each in the order above; its head is the workload with the smallest (LocalQueue usage by
+ * cmp.Compare — NaN first —, -priority, timestamp, UID) among the segments' heads, and every admission adds its entry
+ * penalty to its LocalQueue before the next cycle.  StrictFIFO keeps the head (the next cycle picks the minimum again),
+ * BestEffortFIFO advances the head's own segment, the scheduling-hash move covers every segment of the ClusterQueue.
+ * Consumed usage does not decay inside a drain (CalculateDecayedConsumed is the LocalQueue reconciler's). */
 typedef struct kb_drain_out {
   int32_t max_cycles;        /* in */
   int32_t n_cycles;          /* out: cycles run */

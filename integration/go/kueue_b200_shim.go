@@ -21,6 +21,7 @@ import "C"
 
 import (
 	"fmt"
+	"math"
 	"runtime"
 	"slices"
 	"sort"
@@ -32,7 +33,9 @@ import (
 	schdcache "sigs.k8s.io/kueue/pkg/cache/scheduler"
 	"sigs.k8s.io/kueue/pkg/features"
 	"sigs.k8s.io/kueue/pkg/resources"
+	afs "sigs.k8s.io/kueue/pkg/util/admissionfairsharing"
 	"sigs.k8s.io/kueue/pkg/util/priority"
+	utilqueue "sigs.k8s.io/kueue/pkg/util/queue"
 	"sigs.k8s.io/kueue/pkg/workload"
 )
 
@@ -356,6 +359,70 @@ func (s *Scheduler) flatten(snap *schdcache.Snapshot, heads []workload.Info, gen
 	return f
 }
 
+// flattenAFS fills the AdmissionFairSharing tables of a drain snapshot (kb_snapshot.wl_lq ..., include/kueue_b200.h)
+// from the queue manager and the Configuration; wlQueue[w] is the LocalQueue key of pending workload w.  Without
+// afs.Enabled the tables stay NULL.  A consumed quantity in inf.Dec form has no (value, scale) pair: the caller runs the
+// Go path.
+func (s *Scheduler) flattenAFS(f *flat, wlQueue []utilqueue.LocalQueueReference) error {
+	if !afs.Enabled(s.admissionFairSharing) {
+		return nil
+	}
+	R := len(f.resources)
+	var lqKeys []utilqueue.LocalQueueReference // ClusterQueue-major
+	var lqCq []int32
+	var lqWeight []float64
+	for ci, cq := range f.cqs {
+		for _, key := range s.queues.LocalQueuesOf(cq.Name) { // sorted keys of the LocalQueues feeding cq
+			lqKeys, lqCq = append(lqKeys, key), append(lqCq, int32(ci))
+			lqWeight = append(lqWeight, s.queues.LocalQueueFairSharingWeight(key)) // Weight.AsApproximateFloat64(), 1.0 when nil
+		}
+	}
+	cqAfs := make([]uint8, len(f.cqs))
+	for ci, cq := range f.cqs {
+		on, _ := afs.ResourceWeights(cq.AdmissionScope, s.admissionFairSharing)
+		cqAfs[ci] = b2u(on)
+	}
+	consumed, scale, penalty := make([]int64, len(lqKeys)*R), make([]int32, len(lqKeys)*R), make([]int64, len(lqKeys)*R)
+	for l, key := range lqKeys {
+		if entry, ok := s.queues.AfsConsumedResources.Get(key); ok {
+			for r, q := range entry.Resources {
+				v, sc, ok := q.AsScaledInt64Pair() // (value, scale) of the int64Amount form; false for inf.Dec
+				if !ok {
+					return fmt.Errorf("afs: consumed %s of %s is not an int64Amount", r, key)
+				}
+				consumed[l*R+slices.Index(f.resources, r)], scale[l*R+slices.Index(f.resources, r)] = v, int32(sc)
+			}
+		}
+		for r, q := range s.queues.AfsEntryPenalties.Peek(key) {
+			penalty[l*R+slices.Index(f.resources, r)] = q.MilliValue()
+		}
+	}
+	resWeight, milliMul := make([]float64, R), make([]int64, R)
+	for ri, r := range f.resources {
+		resWeight[ri], milliMul[ri] = 1, 1000
+		if w, ok := s.admissionFairSharing.ResourceWeights[r]; ok {
+			resWeight[ri] = w
+		}
+		if r == corev1.ResourceCPU {
+			milliMul[ri] = 1 // the library keeps cpu in milli-units (pkg/resources/requests.go:104-109)
+		}
+	}
+	wlLq := make([]int32, len(wlQueue))
+	for w, key := range wlQueue {
+		wlLq[w] = int32(slices.Index(lqKeys, key))
+	}
+	cfg := s.admissionFairSharing
+	alpha := 0.0
+	if cfg.UsageHalfLifeTime.Seconds() != 0 { // calculateAlphaRate (admission_fair_sharing.go): Go's math.Pow bits
+		alpha = 1.0 - math.Pow(0.5, cfg.UsageSamplingInterval.Seconds()/cfg.UsageHalfLifeTime.Seconds())
+	}
+	c := &f.c
+	c.n_lq, c.wl_lq, c.lq_cq, c.cq_afs = C.int32_t(len(lqKeys)), cp32(wlLq), cp32(lqCq), cpU8(cqAfs)
+	c.lq_weight, c.lq_consumed, c.lq_consumed_scale = cpF64(lqWeight), cp64(consumed), cp32(scale)
+	c.lq_penalty, c.afs_res_weight, c.afs_milli_mul, c.afs_alpha = cp64(penalty), cpF64(resWeight), cp64(milliMul), C.double(alpha)
+	return nil
+}
+
 // scheduleKB replaces nominate + makeIterator + the decision part of the loop (scheduler.go:255-401) and replays
 // the side effects in the order the library committed the entries.
 func (s *Scheduler) scheduleKB(heads []workload.Info, snap *schdcache.Snapshot) ([]entry, error) {
@@ -434,6 +501,8 @@ func b2u(b bool) uint8 {
 }
 
 // Small helpers left to the integrator (each a few lines): fungibilityCodes, quotaReservedNs, uidRank / wlUIDRank,
-// cp32 / cp64 / cpU8 / cpI8 / cpU64 (copy a Go slice into pinned memory and return the C pointer),
+// cp32 / cp64 / cpU8 / cpI8 / cpU64 / cpF64 (copy a Go slice into pinned memory and return the C pointer),
+// LocalQueuesOf / LocalQueueFairSharingWeight (queue-manager lookups), Quantity.AsScaledInt64Pair (the int64Amount
+// fields of a resource.Quantity),
 // (*Scheduler).eligibleFlavors (checkFlavorForPodSets per flavor -> bitmask), kbFlags (feature gates -> KB_F_*),
 // assignmentFromRows and targetFrom (output rows -> flavorassigner.Assignment / preemption.Target).

@@ -73,6 +73,10 @@ class kb_snapshot(C.Structure):
         ("wl_has_quota_reservation", _P(C.c_uint8)), ("wl_sched_hash", _P(C.c_int64)), ("ps_group", _P(C.c_int32)),
         ("static_generation", C.c_int64),
         ("n_usage_delta", C.c_int32), ("usage_delta_cq", _P(C.c_int32)), ("usage_delta_rows", _P(C.c_int64)),
+        ("n_lq", C.c_int32), ("wl_lq", _P(C.c_int32)), ("lq_cq", _P(C.c_int32)), ("cq_afs", _P(C.c_uint8)),
+        ("lq_weight", _P(C.c_double)), ("lq_consumed", _P(C.c_int64)), ("lq_consumed_scale", _P(C.c_int32)),
+        ("lq_penalty", _P(C.c_int64)), ("afs_res_weight", _P(C.c_double)), ("afs_milli_mul", _P(C.c_int64)),
+        ("afs_alpha", C.c_double),
     ]
 
 
@@ -165,8 +169,13 @@ _DT = {
     "heads": np.int32,
     "wl_has_quota_reservation": np.uint8, "wl_sched_hash": np.int64, "ps_group": np.int32,
     "usage_delta_cq": np.int32, "usage_delta_rows": np.int64,
+    "wl_lq": np.int32, "lq_cq": np.int32, "cq_afs": np.uint8, "lq_weight": np.float64, "lq_consumed": np.int64,
+    "lq_consumed_scale": np.int32, "lq_penalty": np.int64, "afs_res_weight": np.float64, "afs_milli_mul": np.int64,
 }
-OPTIONAL_FIELDS = ("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows")  # NULL in kb_snapshot when absent
+# AdmissionFairSharing tables (include/kueue_b200.h): wl_lq absent = AFS off
+AFS_FIELDS = ("wl_lq", "lq_cq", "cq_afs", "lq_weight", "lq_consumed", "lq_consumed_scale", "lq_penalty", "afs_res_weight",
+              "afs_milli_mul")
+OPTIONAL_FIELDS = ("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows") + AFS_FIELDS  # NULL in kb_snapshot when absent
 ARRAY_FIELDS = list(_DT.keys())
 # tables the library keeps resident while kb_snapshot.static_generation is unchanged (include/kueue_b200.h)
 STATIC_FIELDS = ("parent", "fair_weight", "nominal", "borrow_limit", "lend_limit", "cq_within_cq", "cq_reclaim_within",
@@ -193,6 +202,7 @@ class FlatSnapshot:
     flags: int = FLAGS_DEFAULT
     now_ns: int = 0
     static_generation: int = 0
+    afs_alpha: float = 0.0  # kb_snapshot.afs_alpha: entry-penalty rate of AdmissionFairSharing
     arrays: dict = field(default_factory=dict)
 
     def __getattr__(self, name):
@@ -286,6 +296,7 @@ class FlatSnapshot:
         if cached and getattr(self, "_struct", None) is not None:
             s = self._struct
             s.flags, s.now_ns, s.static_generation = self.flags, self.now_ns, self.static_generation
+            s.afs_alpha = self.afs_alpha
             return s
         s = kb_snapshot()
         s.n_cq, s.n_cohort, s.n_flavor, s.n_resource = self.n_cq, self.n_cohort, self.n_flavor, self.n_resource
@@ -295,6 +306,8 @@ class FlatSnapshot:
         s.n_heads = self.n_heads
         s.pods_resource, s.flags, s.now_ns = self.pods_resource, self.flags, self.now_ns
         s.static_generation = self.static_generation
+        s.n_lq = len(self.arrays["lq_cq"]) if "lq_cq" in self.arrays else 0
+        s.afs_alpha = self.afs_alpha
         for name in ARRAY_FIELDS:
             if name in OPTIONAL_FIELDS and name not in self.arrays:
                 continue  # stays NULL

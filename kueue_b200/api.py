@@ -92,8 +92,14 @@ class MakeClusterQueue(_QuotaHolder):
         self.strategy = abi.QUEUE_BEST_EFFORT_FIFO
         self.fair_weight = 1.0
         self.generation = 0
+        self.admission_mode: Optional[str] = None  # Spec.AdmissionScope.AdmissionMode; None = no AdmissionScope
 
     def Cohort(self, c: str): self.cohort = c; return self
+
+    def AdmissionMode(self, mode: str):
+        assert mode in ("UsageBasedAdmissionFairSharing", "NoAdmissionFairSharing"), mode
+        self.admission_mode = mode
+        return self
 
     def Preemption(self, withinClusterQueue="Never", reclaimWithinCohort="Never", borrowWithinCohort=None,
                    maxPriorityThreshold=None):
@@ -121,6 +127,89 @@ class MakeClusterQueue(_QuotaHolder):
     def FairWeight(self, w): self.fair_weight = float(w); return self
     def Generation(self, g: int): self.generation = g; return self
     def Obj(self): return self
+
+
+class MakeLocalQueue:
+    """LocalQueue (wrappers.go MakeLocalQueue): the ClusterQueue it feeds and its Spec.FairSharing.Weight."""
+
+    def __init__(self, name: str, ns: str = "default"):
+        self.name, self.namespace = name, ns
+        self.cq: Optional[str] = None
+        self.weight = None  # Spec.FairSharing.Weight quantity; None = nil
+
+    def FairSharing(self, weight=None): self.weight = weight; return self
+    def ClusterQueue(self, cq: str): self.cq = cq; return self
+    def Obj(self): return self
+
+
+@dataclass
+class AdmissionFairSharing:
+    """config.AdmissionFairSharing (apis/config/v1beta2): the Configuration block that, with the feature gate on,
+    makes afs.Enabled true.  Durations in seconds; resource_weights = ResourceWeights (1 for a resource not listed)."""
+    usage_half_life_s: float = 0.0
+    usage_sampling_s: float = 0.0
+    resource_weights: Dict[str, float] = field(default_factory=dict)
+
+    @property
+    def alpha(self) -> float:
+        """calculateAlphaRate(sampling, halfLife) (admission_fair_sharing.go): 1 - 0.5^(sampling/halfLife), 0 without a
+        half-life."""
+        if self.usage_half_life_s == 0:
+            return 0.0
+        return 1.0 - 0.5 ** (self.usage_sampling_s / self.usage_half_life_s)
+
+
+_DEC_EXP = {"": 0, "n": -9, "u": -6, "m": -3, "k": 3, "M": 6, "G": 9, "T": 12, "P": 15, "E": 18}
+_BIN_EXP = {"Ki": 10, "Mi": 20, "Gi": 30, "Ti": 40, "Pi": 50, "Ei": 60}
+_PQRE = re.compile(r"^([+-]?)([0-9]*)(?:\.([0-9]*))?(Ki|Mi|Gi|Ti|Pi|Ei|[numkMGTPE]?)$")
+
+
+def parse_quantity(q) -> tuple:
+    """resource.MustParse(q) in the int64Amount form it keeps: (value, scale) with quantity = value * 10^scale
+    (apimachinery quantity.go ParseQuantity: a decimal suffix sets the scale, the fraction digits lower it; a binary
+    suffix multiplies the integer value, scale 0).  Forms that MustParse keeps as inf.Dec raise ValueError."""
+    m = _PQRE.match(str(q))
+    if not m or not (m.group(2) or m.group(3)):
+        raise ValueError(f"bad quantity {q!r}")
+    sign = -1 if m.group(1) == "-" else 1
+    num, frac, suf = m.group(2) or "0", m.group(3) or "", m.group(4)
+    if suf in _BIN_EXP:
+        if frac:
+            raise ValueError(f"{q!r}: a fractional binary quantity is not in the int64Amount form")
+        v, sc = sign * (int(num) << _BIN_EXP[suf]), 0
+    else:
+        v, sc = sign * int(num + frac), _DEC_EXP[suf] - len(frac)
+    if not -2**63 <= v < 2**63:
+        raise ValueError(f"{q!r} does not fit the int64Amount form")
+    return v, sc
+
+
+def _flatten_afs(snap, idx, cqs, pending, local_queues, afs_config, consumed, penalties):
+    """AdmissionFairSharing tables of `flatten` (include/kueue_b200.h), what the shim fills from
+    qManager.AfsConsumedResources / AfsEntryPenalties and the Configuration."""
+    from .drain import quantity_float
+    R = snap.n_resource
+    order = sorted(range(len(local_queues)), key=lambda i: idx.cqs.index(local_queues[i].cq))  # ClusterQueue-major
+    lqs = [local_queues[i] for i in order]
+    idx.lqs = [lq.name for lq in lqs]
+    snap.set("lq_cq", [idx.cqs.index(lq.cq) for lq in lqs])
+    snap.set("wl_lq", [idx.lqs.index(w.queue) for w in pending])
+    on = afs_config is not None
+    snap.set("cq_afs", [on and c.admission_mode == "UsageBasedAdmissionFairSharing" for c in cqs])
+    snap.set("lq_weight", [1.0 if lq.weight is None else quantity_float(*parse_quantity(lq.weight)) for lq in lqs])
+    val = np.zeros((len(lqs), R), np.int64); sc = np.zeros((len(lqs), R), np.int32); pen = np.zeros((len(lqs), R), np.int64)
+    for i, lq in enumerate(lqs):
+        for rname, q in (consumed or {}).get(lq.name, {}).items():
+            val[i, idx.resources.index(rname)], sc[i, idx.resources.index(rname)] = parse_quantity(q)
+        for rname, milli in (penalties or {}).get(lq.name, {}).items():
+            pen[i, idx.resources.index(rname)] = milli
+    snap.set("lq_consumed", val); snap.set("lq_consumed_scale", sc)
+    if penalties:
+        snap.set("lq_penalty", pen)
+    rw = (afs_config.resource_weights if on else {})
+    snap.set("afs_res_weight", [float(rw.get(r, 1.0)) for r in idx.resources])
+    snap.set("afs_milli_mul", [1 if r == "cpu" else 1000 for r in idx.resources])  # MilliValue in the library's units
+    snap.afs_alpha = afs_config.alpha if on else 0.0
 
 
 class MakeCohort(_QuotaHolder):
@@ -259,6 +348,7 @@ class Index:
     resources: List[str]
     pending: List[str] = field(default_factory=list)
     admitted: List[str] = field(default_factory=list)
+    lqs: List[str] = field(default_factory=list)  # LocalQueues in kb_snapshot order (AdmissionFairSharing)
 
     def node(self, name: str) -> int:
         return self.cqs.index(name) if name in self.cqs else len(self.cqs) + self.cohorts.index(name)
@@ -311,15 +401,25 @@ def flatten(cqs: Sequence[MakeClusterQueue], cohorts: Sequence[MakeCohort] = (),
             heads: Optional[Sequence[str]] = None, now_ns: int = 0,
             flavors: Optional[Sequence[str]] = None, extra_resources: Sequence[str] = (),
             resource_flavors: Optional[Sequence["MakeResourceFlavor"]] = None,
-            pods_ready_requeuing: str = "Eviction", reclaimable_pods: bool = True):
+            pods_ready_requeuing: str = "Eviction", reclaimable_pods: bool = True,
+            local_queues: Sequence[MakeLocalQueue] = (), afs_config: Optional[AdmissionFairSharing] = None,
+            consumed: Optional[Dict[str, Dict[str, str]]] = None, penalties: Optional[Dict[str, Dict[str, int]]] = None):
     """Build (FlatSnapshot, Index).
 
     `usage` optionally overrides ClusterQueue usage as {cq: {(flavor, resource): int64}}
     (already in int64 units, like resources.FlavorResourceQuantities literals in the
     reference tests); otherwise usage is the sum of `admitted` workloads' admissions
     (clusterqueue.go:535-563).
+
+    `local_queues` adds the AdmissionFairSharing tables: a pending workload's LocalQueue is its Queue() (its
+    ClusterQueue defaults to the LocalQueue's); `afs_config` None = afs.Enabled false; `consumed` =
+    AfsConsumedResources as {lq: {resource: quantity string}}; `penalties` = AfsEntryPenalties as {lq: {resource: milli}}.
     """
     cohorts = list(cohorts)
+    lq_of = {lq.name: lq for lq in local_queues}
+    for w in pending:  # the queue manager routes a workload to the ClusterQueue of its LocalQueue
+        if w.cq is None and w.queue in lq_of:
+            w.cq = lq_of[w.queue].cq
     known = {c.name for c in cohorts}
     # implicit cohorts (hierarchy.Manager creates them on reference, manager.go:80-100)
     for holder in list(cqs) + list(cohorts):
@@ -328,6 +428,8 @@ def flatten(cqs: Sequence[MakeClusterQueue], cohorts: Sequence[MakeCohort] = (),
             cohorts.append(MakeCohort(par)); known.add(par)
     fl: List[str] = list(flavors) if flavors else []
     res: set = set(extra_resources)
+    for m in (consumed or {}).values():
+        res.update(m.keys())
     for holder in list(cqs) + cohorts:
         for rg in holder.resource_groups:
             for fq in rg:
@@ -481,6 +583,8 @@ def flatten(cqs: Sequence[MakeClusterQueue], cohorts: Sequence[MakeCohort] = (),
         snap.set("heads", np.arange(len(w_cq)))
     else:
         snap.set("heads", [idx.pending.index(h) for h in heads])
+    if local_queues:
+        _flatten_afs(snap, idx, cqs, pending, list(local_queues), afs_config, consumed, penalties)
     snap.finalize()
     return snap, idx
 

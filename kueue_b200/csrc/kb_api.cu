@@ -539,6 +539,29 @@ static int32_t build_dynamic(kb_handle *h, const kb_snapshot *s) {
     // can any ClusterQueue ever have preemption candidates?  (candidates_possible, kb_kernels.cuh)
     h->preempt_possible = h->s_preempt_policy;
   }
+  if (s->wl_lq) {  // AdmissionFairSharing tables (include/kueue_b200.h)
+    const int L = s->n_lq;
+    if (L < 0 || !s->lq_cq || !s->cq_afs || !s->lq_weight || !s->lq_consumed || !s->lq_consumed_scale || !s->afs_res_weight || !s->afs_milli_mul)
+      return fail(h, KB_ERR_INVALID, "afs: wl_lq given without the LocalQueue tables");
+    for (int l = 0; l < L; l++) {
+      if (s->lq_cq[l] < 0 || s->lq_cq[l] >= Q) return fail(h, KB_ERR_INVALID, "afs: lq_cq out of range");
+      if (l && s->lq_cq[l] < s->lq_cq[l - 1]) return fail(h, KB_ERR_INVALID, "afs: LocalQueues must be numbered ClusterQueue-major");
+    }
+    for (int w = 0; w < s->n_wl; w++) {
+      const int l = s->wl_lq[w];
+      if (l < 0 || l >= L) return fail(h, KB_ERR_INVALID, "afs: wl_lq out of range");
+      if (s->lq_cq[l] != s->wl_cq[w]) return fail(h, KB_ERR_INVALID, "afs: the LocalQueue of a workload feeds another ClusterQueue");
+    }
+    for (int r = 0; r < s->n_resource; r++)
+      if (s->afs_milli_mul[r] < 1) return fail(h, KB_ERR_INVALID, "afs: afs_milli_mul must be positive");
+    for (size_t i = 0; i < (size_t)L * s->n_resource; i++)
+      if (s->lq_consumed_scale[i] < -AFS_MAX_SCALE || s->lq_consumed_scale[i] > AFS_MAX_SCALE)
+        return fail(h, KB_ERR_UNSUPPORTED, "afs: consumed quantity scale outside [-22, 22]");
+    bool any_afs = false;
+    for (int q = 0; q < Q; q++) any_afs |= s->cq_afs[q] != 0;
+    if (any_afs && h->preempt_possible)
+      return fail(h, KB_ERR_UNSUPPORTED, "afs: preemption candidate ordering with AdmissionFairSharing is not supported (not a transitive order across ClusterQueues)");
+  }
   return KB_OK;
 }
 
@@ -1339,8 +1362,36 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   if (rc != KB_OK) return rc;
   DevSnap &D = h->D;
   if (!h->ev_d) cudaEventCreate(&h->ev_d);
+  // ---- AdmissionFairSharing: queue segments, one per LocalQueue of a ClusterQueue with cq_afs set and one per other
+  // ClusterQueue, numbered ClusterQueue-major; the initial LocalQueue usage (kb_drain.cuh afs_lq_usage)
+  const bool afs = s->wl_lq != nullptr;
+  const int L = afs ? s->n_lq : 0;
+  std::vector<int32_t> seg_start, lq_seg, seg_lq, afs_cqs;
+  std::vector<double> lq_usage;
+  int S = Q;
+  if (afs) {
+    std::vector<int32_t> lq_first((size_t)Q + 1, 0);
+    for (int l = 0; l < L; l++) lq_first[s->lq_cq[l] + 1]++;
+    for (int q = 0; q < Q; q++) lq_first[q + 1] += lq_first[q];
+    seg_start.resize((size_t)Q + 1); lq_seg.assign((size_t)std::max(1, L), -1); lq_usage.assign((size_t)std::max(1, L), 0.0);
+    for (int q = 0; q < Q; q++) {
+      seg_start[q] = (int32_t)seg_lq.size();
+      if (!s->cq_afs[q]) { seg_lq.push_back(-1); continue; }
+      afs_cqs.push_back(q);
+      for (int l = lq_first[q]; l < lq_first[q + 1]; l++) {
+        lq_seg[l] = (int32_t)seg_lq.size(); seg_lq.push_back(l);
+        const size_t o = (size_t)l * R;
+        if (!afs_lq_usage((const i64 *)s->lq_consumed + o, s->lq_consumed_scale + o, s->lq_penalty ? (const i64 *)s->lq_penalty + o : nullptr, s->afs_res_weight,
+                          s->lq_weight[l], R, &lq_usage[l]))
+          return fail(h, KB_ERR_UNSUPPORTED, "afs: consumed usage + entry penalty of a LocalQueue overflows int64");
+      }
+    }
+    seg_start[Q] = (int32_t)seg_lq.size();
+    S = seg_start[Q];
+    if (seg_lq.empty()) seg_lq.push_back(-1);
+  }
   // ---- drain-only device buffers
-  const size_t Wz = (size_t)W, Hz = (size_t)Hcap;
+  const size_t Wz = (size_t)W, Hz = (size_t)Hcap, Sz = (size_t)S, Lz = (size_t)std::max(1, L), LR = Lz * R;
   size_t sort_bytes = 0;
   {
     cub::DoubleBuffer<u64> dk(nullptr, nullptr); cub::DoubleBuffer<int32_t> dv(nullptr, nullptr);
@@ -1351,9 +1402,13 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   size_t tot = 0;
   auto need = [&](size_t n, size_t sz) { tot += pad256(n * sz); };
   need(Wz, 8); need(Wz, 8); need(Wz, 4); need(Wz, 4); need(sort_bytes, 1);
-  need((size_t)Q + 2, 4); need((size_t)Q + 2, 4); need(Q, 4); need(Wz, 1); need((size_t)Q + 2, 4); need((size_t)Q + 2, 4);
+  need(Sz + 2, 4); need(Sz + 2, 4); need(Sz, 4); need(Wz, 1); need((size_t)Q + 2, 4); need((size_t)Q + 2, 4);
   for (int k = 0; k < 4; k++) need(Hz + 2, 4);
   need(16, 4); need(Wz, 4); need(Wz, 4); need(Wz, 1); need(trace_cap, 4); need(trace_cap, 1);
+  if (afs) {
+    need((size_t)Q + 1, 4); need(Lz, 4); need(seg_lq.size(), 4); need(afs_cqs.size() + 1, 4); need(Q, 4); need(Wz, 4); need(Q, 1);
+    need(Lz, 8); need(LR, 8); need(LR, 4); need(LR, 8); need(Lz, 8); need(R, 8); need(R, 8);
+  }
   if (tot > h->drain_buf_cap) {
     if (h->drain_buf) cudaFree(h->drain_buf);
   if (h->tas_buf) cudaFree(h->tas_buf);
@@ -1367,8 +1422,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   int32_t *vals[2] = {(int32_t *)take(Wz, 4), (int32_t *)take(Wz, 4)};
   void *sort_tmp = take(sort_bytes, 1);
   DrainDev X{};
-  int32_t *q_count = (int32_t *)take((size_t)Q + 2, 4);
-  X.q_start = (int32_t *)take((size_t)Q + 2, 4); X.cursor = (int32_t *)take(Q, 4); X.gone = (uint8_t *)take(Wz, 1);
+  int32_t *q_count = (int32_t *)take(Sz + 2, 4);
+  X.q_start = (int32_t *)take(Sz + 2, 4); X.cursor = (int32_t *)take(Sz, 4); X.gone = (uint8_t *)take(Wz, 1);
   X.flag = (int32_t *)take((size_t)Q + 2, 4); X.pos = (int32_t *)take((size_t)Q + 2, 4);
   X.e_assumed = (int32_t *)take(Hz + 2, 4); X.e_ncells = (int32_t *)take(Hz + 2, 4);
   X.e_adm_off = (int32_t *)take(Hz + 2, 4); X.e_cell_off = (int32_t *)take(Hz + 2, 4);
@@ -1381,9 +1436,37 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   X.adm_ts = const_cast<i64 *>(D.adm_ts); X.adm_qr_ts = const_cast<i64 *>(D.adm_qr_ts); X.adm_uid = const_cast<i64 *>(D.adm_uid);
   X.adm_evicted = const_cast<uint8_t *>(D.adm_evicted); X.adm_use_start = const_cast<int32_t *>(D.adm_use_start);
   X.adm_use_fr = const_cast<int32_t *>(D.adm_use_fr); X.adm_use_qty = const_cast<i64 *>(D.adm_use_qty);
+  if (afs) {
+    auto h2d = [&](const void *src, size_t n, size_t sz) {
+      char *p = take(n, sz);
+      if (n) { cudaError_t e = cudaMemcpyAsync(p, src, n * sz, cudaMemcpyHostToDevice, h->stream); if (e != cudaSuccess) return (char *)nullptr; }
+      return p;
+    };
+    X.seg_start = (const int32_t *)h2d(seg_start.data(), seg_start.size(), 4);
+    X.lq_seg = (const int32_t *)h2d(lq_seg.data(), lq_seg.size(), 4);
+    X.seg_lq = (const int32_t *)h2d(seg_lq.data(), seg_lq.size(), 4);
+    X.afs_cqs = (const int32_t *)h2d(afs_cqs.data(), afs_cqs.size(), 4);
+    X.head_seg = (int32_t *)take(Q, 4);
+    X.wl_lq = (const int32_t *)h2d(s->wl_lq, Wz, 4);
+    X.cq_afs = (const uint8_t *)h2d(s->cq_afs, Q, 1);
+    X.lq_weight = (const double *)h2d(s->lq_weight, L, 8);
+    X.lq_consumed = (const i64 *)h2d(s->lq_consumed, (size_t)L * R, 8);
+    X.lq_consumed_scale = (const int32_t *)h2d(s->lq_consumed_scale, (size_t)L * R, 4);
+    X.lq_penalty = (i64 *)take(LR, 8);
+    if (s->lq_penalty) CUDA_TRY(h, cudaMemcpyAsync(X.lq_penalty, s->lq_penalty, (size_t)L * R * 8, cudaMemcpyHostToDevice, h->stream));
+    else CUDA_TRY(h, cudaMemsetAsync(X.lq_penalty, 0, LR * 8, h->stream));
+    X.lq_usage = (double *)h2d(lq_usage.data(), Lz, 8);
+    X.res_weight = (const double *)h2d(s->afs_res_weight, R, 8);
+    X.milli_mul = (const i64 *)h2d(s->afs_milli_mul, R, 8);
+    X.alpha = s->afs_alpha;
+    X.n_afs_cq = (int)afs_cqs.size();
+    if (!X.seg_start || !X.lq_seg || !X.seg_lq || !X.afs_cqs || !X.wl_lq || !X.cq_afs || !X.lq_weight || !X.lq_consumed ||
+        !X.lq_consumed_scale || !X.lq_usage || !X.res_weight || !X.milli_mul)
+      return fail(h, KB_ERR_CUDA, "afs: upload of the LocalQueue tables failed");
+  }
   // ---- per-ClusterQueue order (queueOrderingFunc): stable LSD passes uid -> timestamp -> (ClusterQueue | priority desc)
   const int tb = 256, nbW = (W + tb - 1) / tb, nbQ = (Q + tb - 1) / tb;
-  CUDA_TRY(h, cudaMemsetAsync(q_count, 0, sizeof(int32_t) * ((size_t)Q + 2), h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(q_count, 0, sizeof(int32_t) * (Sz + 2), h->stream));
   {
     cub::DoubleBuffer<u64> dk(keys[0], keys[1]); cub::DoubleBuffer<int32_t> dv(vals[0], vals[1]);
     size_t bytes = sort_bytes;
@@ -1391,16 +1474,17 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 64, h->stream));
     k_drain_keys_ts<<<nbW, tb, 0, h->stream>>>(D, dv.Current(), dk.Current());
     CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 64, h->stream));
-    k_drain_keys_cq<<<nbW, tb, 0, h->stream>>>(D, dv.Current(), dk.Current(), q_count);
-    int cq_bits = 1; while ((1ll << cq_bits) < (long long)Q) cq_bits++;
+    k_drain_keys_cq<<<nbW, tb, 0, h->stream>>>(D, X, dv.Current(), dk.Current(), q_count);
+    int cq_bits = 1; while ((1ll << cq_bits) < (long long)S) cq_bits++;
     CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 32 + cq_bits, h->stream));
     X.q_order = dv.Current();
   }
-  k_scan_i32<<<1, 1024, 0, h->stream>>>(q_count, X.q_start, Q);
-  k_drain_init<<<std::max(nbW, nbQ), tb, 0, h->stream>>>(D, X);
+  k_scan_i32<<<1, 1024, 0, h->stream>>>(q_count, X.q_start, S);
+  k_drain_init<<<std::max(nbW, (S + tb - 1) / tb), tb, 0, h->stream>>>(D, X, S);
   int32_t *d_heads = const_cast<int32_t *>(D.heads);
   auto enqueue_heads = [&]() {
     k_drain_flag<<<nbQ, tb, 0, h->stream>>>(D, X);
+    if (X.n_afs_cq) k_drain_afs_heads<<<(X.n_afs_cq + 7) / 8, tb, 0, h->stream>>>(D, X);
     k_scan_i32<<<1, 1024, 0, h->stream>>>(X.flag, X.pos, Q);
     k_drain_heads<<<nbQ, tb, 0, h->stream>>>(D, X, d_heads);
   };
@@ -1411,6 +1495,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   int A_cur = s->n_adm, AU_cur = s->n_adm_use;
   const bool pre = h->preempt_possible;
   double gpu_ms = 0;
+  float kms[KB_N_KERNELS] = {};  // per-kernel times summed over the cycles (kb_set_profile)
   for (int cyc = 0; cyc < max_cycles && n_live > 0; cyc++) {
     D.H = n_live; D.now_ns = s->now_ns + cyc;
     D.A = pre ? A_cur : 0; D.AU = pre ? AU_cur : 0;  // without preemption policies the cycle never looks at the admitted tables
@@ -1418,18 +1503,23 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (rc != KB_OK) return rc;
     X.A = A_cur; X.AU = AU_cur; X.cycle = cyc; X.trace_off = (long long)out->n_decisions;
     const int nbH = (n_live + tb - 1) / tb;
+    kmark(h, KB_K_DRAIN);
     k_drain_apply<<<nbH, tb, 0, h->stream>>>(D, X);
     k_scan_i32<<<1, 1024, 0, h->stream>>>(X.e_assumed, X.e_adm_off, n_live);
     k_scan_i32<<<1, 1024, 0, h->stream>>>(X.e_ncells, X.e_cell_off, n_live);
     k_drain_admit<<<nbH, tb, 0, h->stream>>>(D, X, s->now_ns + cyc);
     enqueue_heads();
+    kmark(h, -1);
     CUDA_TRY(h, cudaEventRecord(h->ev_d, h->stream));
     CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[8], X.counters, 4, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[9], X.e_adm_off + n_live, 4, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[10], X.e_cell_off + n_live, 4, cudaMemcpyDeviceToHost, h->stream));
+    if (afs) CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[11], D.status, 4, cudaMemcpyDeviceToHost, h->stream));  // after k_drain_admit
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     rc = cycle_finish(h);
     if (rc != KB_OK) return rc;
+    if (afs && (h->host_words[11] & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: an entry penalty overflows int64");
+    for (int i = 0; i < KB_N_KERNELS; i++) kms[i] += h->stats.kernel_ms[i];
     { float ms = 0; cudaEventElapsedTime(&ms, h->ev2, h->ev_d); gpu_ms += ms; }
     int n_new = (int)h->host_words[9], n_cells = (int)h->host_words[10];
     if (out->cycle_heads) out->cycle_heads[cyc] = n_live;
@@ -1441,6 +1531,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   }
   out->gpu_ms = gpu_ms;
   h->stats.last_cycle_gpu_ms = gpu_ms;
+  memcpy(h->stats.kernel_ms, kms, sizeof(kms));
   // ---- results
   size_t PR = (size_t)D.P * D.R;
   if (out->wl_admit_cycle) CUDA_TRY(h, cudaMemcpyAsync(out->wl_admit_cycle, X.wl_admit_cycle, Wz * 4, cudaMemcpyDeviceToHost, h->stream));

@@ -10,9 +10,68 @@
 // to the inadmissible set".  Every cycle: pick the heads (ordered compaction over ClusterQueues), run the unchanged
 // cycle kernels on them, then apply the decisions — admissions extend the admitted tables and the ClusterQueue
 // usage on the device, the others keep their LastAssignment and move per the Strict / BestEffort FIFO rules.
+//
+// AdmissionFairSharing (kb_snapshot.wl_lq != NULL): the queue of a ClusterQueue with cq_afs set is one SEGMENT per
+// LocalQueue (each sorted as above, each with its own cursor); every other ClusterQueue is one segment.  Segments are
+// numbered ClusterQueue-major (seg_start[Q+1]).  The head of an AFS ClusterQueue is the minimum of (LocalQueue usage by
+// cmp.Compare, -priority, timestamp, UID) over the heads of its segments (one warp per ClusterQueue, k_drain_afs_heads);
+// an admission adds its entry penalty to its LocalQueue and recomputes that LocalQueue's usage (k_drain_admit).
 #pragma once
 
 #include "kb_device.cuh"
+
+// ---- resource.Quantity in the int64Amount form (value * 10^scale), as AdmissionFairSharing sums it -----------------
+// Pow10 for |n| <= 22: 10^n is exact in a double, and Go's math.Pow10(-n) is 1 / 10^n (not a multiplication by 1e-n).
+__host__ __device__ inline double afs_pow10(int n) {
+  double p = 1.0;
+  for (int i = 0; i < (n < 0 ? -n : n); i++) p *= 10.0;
+  return n < 0 ? 1.0 / p : p;
+}
+#define AFS_MAX_SCALE 22
+// positiveScaleInt64 (apimachinery math.go:140-165): v * 10^k, false on int64 overflow
+__host__ __device__ inline bool afs_scale_up(i64 v, int k, i64 *out) {
+  for (int i = 0; i < k; i++) {
+    if (v > 922337203685477580ll || v < -922337203685477580ll) return false;
+    v *= 10;
+  }
+  *out = v;
+  return true;
+}
+// int64Add (math.go): false when the sum leaves int64
+__host__ __device__ inline bool afs_add64(i64 a, i64 b, i64 *out) {
+  i64 c = (i64)((u64)a + (u64)b);
+  if ((a > 0 && b > 0 && c < 0) || (a < 0 && b < 0 && c >= 0)) return false;
+  *out = c;
+  return true;
+}
+// int64Amount.Add (amount.go:162-199): a zero operand keeps the other's scale, otherwise the smaller scale wins
+__host__ __device__ inline bool afs_qty_add(i64 av, int as, i64 bv, int bs, i64 *rv, int *rs) {
+  if (bv == 0) { *rv = av; *rs = as; return true; }
+  if (av == 0) { *rv = bv; *rs = bs; return true; }
+  i64 c;
+  if (as == bs) { if (!afs_add64(av, bv, &c)) return false; *rv = c; *rs = as; return true; }
+  if (as > bs) { if (!afs_scale_up(av, as - bs, &c) || !afs_add64(c, bv, &c)) return false; *rv = c; *rs = bs; return true; }
+  if (!afs_scale_up(bv, bs - as, &c) || !afs_add64(av, c, &c)) return false;
+  *rv = c; *rs = as;
+  return true;
+}
+// Quantity.AsApproximateFloat64 (quantity.go:468-483)
+__host__ __device__ inline double afs_qty_float(i64 v, int s) { return s == 0 ? (double)v : (double)v * afs_pow10(s); }
+// Info.CalcLocalQueueFSUsage (workload.go:391-427) for one LocalQueue, resources in index order (the reference sums over
+// a map: its order is random; this order is the library's canonical choice).  A zero quantity adds nothing, like an
+// absent key.  Built with -fmad=false: each product is rounded before the sum.  false = int64 overflow.
+__host__ __device__ inline bool afs_lq_usage(const i64 *consumed, const int32_t *scale, const i64 *penalty_milli,
+                                             const double *res_weight, double lq_weight, int R, double *out) {
+  double usage = 0.0;
+  for (int r = 0; r < R; r++) {
+    i64 v; int s;
+    if (!afs_qty_add(consumed[r], scale[r], penalty_milli ? penalty_milli[r] : 0, -3, &v, &s)) return false;
+    if (v == 0) continue;
+    usage += res_weight[r] * afs_qty_float(v, s);
+  }
+  *out = usage / lq_weight;
+  return true;
+}
 
 struct DrainDev {
   // queues
@@ -27,7 +86,21 @@ struct DrainDev {
   i64 *cq_usage, *wl_last_gen; int8_t *ps_last_tried;
   int32_t *adm_cq, *adm_priority; i64 *adm_ts, *adm_qr_ts, *adm_uid; uint8_t *adm_evicted; int32_t *adm_use_start, *adm_use_fr; i64 *adm_use_qty;
   int A, AU, cycle;  // admitted workloads / usage cells before this cycle's admissions
+  // AdmissionFairSharing; seg_start == nullptr: no AFS tables, segment = ClusterQueue
+  const int32_t *seg_start;   // [Q+1] first segment of every ClusterQueue
+  const int32_t *lq_seg;      // [n_lq] segment of a LocalQueue of an AFS ClusterQueue
+  const int32_t *seg_lq;      // [S] LocalQueue of a segment of an AFS ClusterQueue
+  const int32_t *afs_cqs;     // [n_afs_cq] ClusterQueues with cq_afs set
+  int32_t *head_seg;          // [Q] segment of this cycle's head
+  const int32_t *wl_lq, *lq_consumed_scale; const uint8_t *cq_afs; const double *lq_weight, *res_weight;
+  const i64 *lq_consumed, *milli_mul;
+  i64 *lq_penalty; double *lq_usage;
+  double alpha;
+  int n_afs_cq;
 };
+
+__device__ __forceinline__ int drain_seg0(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq] : cq; }
+__device__ __forceinline__ int drain_seg1(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq + 1] : cq + 1; }
 
 // sort keys of queueOrderingFunc (cluster_queue.go:636-685): LSD passes uid, timestamp, (ClusterQueue | priority desc)
 __global__ void k_drain_keys_uid(DevSnap D, u64 *keys, int32_t *vals) {
@@ -41,30 +114,75 @@ __global__ void k_drain_keys_ts(DevSnap D, const int32_t *vals, u64 *keys) {
   if (i >= D.W) return;
   keys[i] = (u64)D.wl_ts[vals[i]] ^ 0x8000000000000000ull;
 }
-__global__ void k_drain_keys_cq(DevSnap D, const int32_t *vals, u64 *keys, int32_t *q_count) {
+// third pass: (segment | priority desc); the segment is the ClusterQueue unless its queue is split by LocalQueue
+__global__ void k_drain_keys_cq(DevSnap D, DrainDev X, const int32_t *vals, u64 *keys, int32_t *q_count) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= D.W) return;
   int w = vals[i];
   int cq = D.wl_cq[w];
-  keys[i] = ((u64)cq << 32) | (u64)(~((unsigned)D.wl_priority[w] ^ 0x80000000u));  // higher priority first
-  atomicAdd(&q_count[cq], 1);
+  int seg = (X.seg_start && X.cq_afs[cq]) ? X.lq_seg[X.wl_lq[w]] : drain_seg0(X, cq);
+  keys[i] = ((u64)seg << 32) | (u64)(~((unsigned)D.wl_priority[w] ^ 0x80000000u));  // higher priority first
+  atomicAdd(&q_count[seg], 1);
 }
-__global__ void k_drain_init(DevSnap D, DrainDev X) {
+__global__ void k_drain_init(DevSnap D, DrainDev X, int S) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < D.W) { X.gone[i] = 0; X.wl_admit_cycle[i] = -1; X.wl_evals[i] = 0; X.wl_last_decision[i] = 0xff; }
-  if (i < D.Q) X.cursor[i] = 0;
+  if (i < S) X.cursor[i] = 0;
 }
 
-// heads of the next cycle (queues.Heads manager.go:770-794): one per ClusterQueue with work left, in ClusterQueue order
+// heads of the next cycle (queues.Heads manager.go:770-794): one per ClusterQueue with work left, in ClusterQueue order.
+// Thread per ClusterQueue of one segment; the AFS ClusterQueues are k_drain_afs_heads'.
 __global__ void k_drain_flag(DevSnap D, DrainDev X) {
   int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= D.Q) return;
-  X.flag[q] = X.cursor[q] < X.q_start[q + 1] - X.q_start[q];
+  if (X.seg_start && X.cq_afs[q]) return;
+  int s = drain_seg0(X, q);
+  X.flag[q] = X.cursor[s] < X.q_start[s + 1] - X.q_start[s];
+  if (X.head_seg) X.head_seg[q] = s;
 }
+
+// (usage, -priority, timestamp, UID) of a segment head; seg < 0 = no candidate
+struct AfsHead { double u; i64 ts, uid; int prio, seg; };
+__device__ __forceinline__ bool afs_before(const AfsHead &a, const AfsHead &b) {
+  if (a.seg < 0 || b.seg < 0) return a.seg >= 0 && b.seg < 0;
+  const bool an = isnan(a.u), bn = isnan(b.u);  // cmp.Compare: NaN sorts first, two NaNs are equal
+  if (an != bn) return an;
+  if (!an && a.u != b.u) return a.u < b.u;
+  if (a.prio != b.prio) return a.prio > b.prio;
+  if (a.ts != b.ts) return a.ts < b.ts;
+  if (a.uid != b.uid) return a.uid < b.uid;
+  return a.seg < b.seg;
+}
+// head of an AFS ClusterQueue (queueOrderingFunc with enableAdmissionFs, cluster_queue.go:636-685): one warp per
+// ClusterQueue, lanes stride its LocalQueue segments and reduce by shuffles
+__global__ void k_drain_afs_heads(DevSnap D, DrainDev X) {
+  const int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (wid >= X.n_afs_cq) return;
+  const int q = X.afs_cqs[wid];
+  AfsHead best{0.0, 0, 0, 0, -1};
+  for (int s = X.seg_start[q] + lane; s < X.seg_start[q + 1]; s += 32) {
+    const int c = X.cursor[s];
+    if (c >= X.q_start[s + 1] - X.q_start[s]) continue;
+    const int w = X.q_order[X.q_start[s] + c];
+    AfsHead h{X.lq_usage[X.seg_lq[s]], D.wl_ts[w], D.wl_uid[w], D.wl_priority[w], s};
+    if (afs_before(h, best)) best = h;
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    AfsHead h;
+    h.u = __shfl_xor_sync(0xffffffffu, best.u, o);
+    h.ts = __shfl_xor_sync(0xffffffffu, best.ts, o);
+    h.uid = __shfl_xor_sync(0xffffffffu, best.uid, o);
+    h.prio = __shfl_xor_sync(0xffffffffu, best.prio, o);
+    h.seg = __shfl_xor_sync(0xffffffffu, best.seg, o);
+    if (afs_before(h, best)) best = h;
+  }
+  if (lane == 0) { X.flag[q] = best.seg >= 0; X.head_seg[q] = best.seg; }
+}
+
 __global__ void k_drain_heads(DevSnap D, DrainDev X, int32_t *heads) {
   int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= D.Q) return;
-  if (X.flag[q]) heads[X.pos[q]] = X.q_order[X.q_start[q] + X.cursor[q]];
+  if (X.flag[q]) { int s = X.head_seg ? X.head_seg[q] : q; heads[X.pos[q]] = X.q_order[X.q_start[s] + X.cursor[s]]; }
   if (q == 0) X.counters[0] = X.pos[D.Q];
 }
 
@@ -115,16 +233,23 @@ __global__ void k_drain_apply(DevSnap D, DrainDev X) {
   // ---- queue movement (cluster_queue.go:362-425,609-633)
   const bool strict = D.cq_strategy[cq] == KB_QUEUE_STRICT_FIFO;
   const bool inadmissible = (dec == KB_DEC_NOFIT || dec == KB_DEC_PREEMPT_NO_TARGETS) && !pending_flavors;
-  const int qs = X.q_start[cq], qn = X.q_start[cq + 1] - qs;
-  int cur = X.cursor[cq];
-  if (dec == KB_DEC_NOFIT && !strict && D.wl_sched_hash) {  // handleInadmissibleHash :408-425
-    i64 hsh = D.wl_sched_hash[wl];
-    if (hsh != 0)
-      for (int p = cur + 1; p < qn; p++) { int w2 = X.q_order[qs + p]; if (D.wl_sched_hash[w2] == hsh) X.gone[w2] = 1; }
+  const int hs = X.head_seg ? X.head_seg[cq] : cq, s0 = drain_seg0(X, cq), s1 = drain_seg1(X, cq);
+  const bool bulk = dec == KB_DEC_NOFIT && !strict && D.wl_sched_hash && D.wl_sched_hash[wl] != 0;
+  if (bulk) {  // handleInadmissibleHash :408-425: every queued workload of the class, in every segment of the queue
+    const i64 hsh = D.wl_sched_hash[wl];
+    for (int s = s0; s < s1; s++) {
+      const int qs = X.q_start[s], qn = X.q_start[s + 1] - qs;
+      for (int p = X.cursor[s] + (s == hs); p < qn; p++) { int w2 = X.q_order[qs + p]; if (D.wl_sched_hash[w2] == hsh) X.gone[w2] = 1; }
+    }
   }
-  if (ok || (inadmissible && !strict)) cur++;
-  while (cur < qn && X.gone[X.q_order[qs + cur]]) cur++;
-  X.cursor[cq] = cur;
+  if (ok || (inadmissible && !strict)) X.cursor[hs]++;
+  for (int s = s0; s < s1; s++) {
+    if (s != hs && !bulk) continue;
+    const int qs = X.q_start[s], qn = X.q_start[s + 1] - qs;
+    int cur = X.cursor[s];
+    while (cur < qn && X.gone[X.q_order[qs + cur]]) cur++;
+    X.cursor[s] = cur;
+  }
 }
 
 // admitted entries join the admitted tables (cache.AssumeWorkload) and the ClusterQueue usage
@@ -154,4 +279,27 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
     }
   X.adm_use_start[a + 1] = c0 + n;
   for (int j = 0; j < n; j++) X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c0 + j]] += X.adm_use_qty[c0 + j];  // one entry per ClusterQueue
+  if (X.seg_start && X.cq_afs[cq]) {
+    // entry penalty (scheduler.go:727-742,946-960; CalculateEntryPenalty + MulByFloat): per resource of SumTotalRequests
+    // (the full TotalRequests, partial admission does not reduce it), int64(float64(MilliValue) * alpha) milli-units,
+    // pushed into the LocalQueue's penalties (AfsEntryPenalties.Push: Quantity.Add at scale -3).  A ClusterQueue admits
+    // one entry per cycle and a LocalQueue belongs to one ClusterQueue: one writer per LocalQueue, no atomics.
+    const int lq = X.wl_lq[wl];
+    i64 *pen = X.lq_penalty + (size_t)lq * R;
+    bool bad = false;
+    for (int r = 0; r < R; r++) {
+      i64 total = 0;
+      for (int row = ps0; row < ps1; row++)
+        if (D.ps_req_mask[row] & (1u << r)) bad |= !afs_add64(total, D.ps_req[(size_t)row * R + r], &total);
+      if (total == 0) continue;
+      const i64 mul = X.milli_mul[r];
+      if (total > INT64_MAX / mul || total < -INT64_MAX / mul) { bad = true; continue; }
+      const i64 delta = (i64)((double)(total * mul) * X.alpha);
+      bad |= !afs_add64(pen[r], delta, &pen[r]);
+    }
+    double u = 0.0;
+    bad |= !afs_lq_usage(X.lq_consumed + (size_t)lq * R, X.lq_consumed_scale + (size_t)lq * R, pen, X.res_weight, X.lq_weight[lq], R, &u);
+    X.lq_usage[lq] = u;
+    if (bad) atomicOr(D.status, KBS_AFS_OVERFLOW);
+  }
 }

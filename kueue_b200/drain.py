@@ -22,6 +22,19 @@ loop on the oracle and compares kb_run_drain with it cycle by cycle.
   * the drain ends with the first cycle that admits nothing (no cluster event can change the outcome after that;
     evictions are asynchronous in the reference and are not replayed: a Preempting entry keeps its place and its
     targets stay admitted).
+
+AdmissionFairSharing (the snapshot carries `wl_lq` and the LocalQueue tables, include/kueue_b200.h): the queue of a
+ClusterQueue with `cq_afs` set is one segment per LocalQueue, each in the static order above with its own cursor.
+  * the head is the minimum of (LocalQueue usage by cmp.Compare, -priority, timestamp, UID) over the segment heads
+    (queueOrderingFunc with enableAdmissionFs, cluster_queue.go:636-685; the sticky workload is not modelled).  After
+    penalties the reference's Pop re-heapifies in map order (rebuildAll, cluster_queue.go:494-531; heap.go:115-123,
+    166-172) and may return a workload that is not the minimum: the true minimum is this definition's canonical rule;
+  * LocalQueue usage is `lq_usage` (Info.CalcLocalQueueFSUsage, workload.go:391-427), summed in resource-index order
+    (the reference sums over a map, in random order: resource-index order is the canonical choice);
+  * every admission adds its entry penalty to its LocalQueue (`entry_penalty`; scheduler.go:727-742,946-960) before
+    the next cycle; consumed usage does not decay inside a drain;
+  * StrictFIFO keeps its head (the next cycle picks the minimum again), BestEffortFIFO advances the head's own segment,
+    handleInadmissibleHash sets aside the workloads of the class in every segment of the ClusterQueue.
 """
 from __future__ import annotations
 
@@ -86,21 +99,135 @@ def requeue_goes_inadmissible(strict_fifo: bool, reason: str, last_tried) -> boo
     return not (immediate or pending_flavors(last_tried))
 
 
+class AfsOverflow(ValueError):
+    """A quantity sum leaves int64: the reference would switch to inf.Dec (kb_run_drain: KB_ERR_UNSUPPORTED)."""
+
+
+AFS_MAX_SCALE = 22
+_I64 = 2**63
+
+
+def _int64(v: int) -> int:
+    if not -_I64 <= v < _I64:
+        raise AfsOverflow(v)
+    return v
+
+
+def quantity_add(a, b):
+    """int64Amount.Add (apimachinery amount.go:162-199) on (value, scale) pairs: a zero operand keeps the other's scale,
+    otherwise the sum is aligned to the smaller scale (positiveScaleInt64 + int64Add, AfsOverflow when they fail)."""
+    (av, as_), (bv, bs) = a, b
+    if bv == 0:
+        return av, as_
+    if av == 0:
+        return bv, bs
+    if as_ == bs:
+        return _int64(av + bv), as_
+    if as_ > bs:
+        return _int64(_int64(av * 10**(as_ - bs)) + bv), bs
+    return _int64(av + _int64(bv * 10**(bs - as_))), as_
+
+
+def pow10(n: int) -> float:
+    """math.Pow10 for |n| <= 22: 10^n exactly, and 1 / 10^-n (not a product with 1e-n) for negative n."""
+    return float(10**n) if n >= 0 else 1.0 / float(10**-n)
+
+
+def quantity_float(v: int, s: int) -> float:
+    """Quantity.AsApproximateFloat64 (quantity.go:468-483) of the int64Amount (v, s)."""
+    return float(v) if s == 0 else float(v) * pow10(s)
+
+
+def compare_usage(a: float, b: float) -> int:
+    """cmp.Compare on float64: NaN sorts before every other value, two NaNs are equal."""
+    an, bn = a != a, b != b
+    if an or bn:
+        return 0 if an and bn else (-1 if an else 1)
+    return -1 if a < b else (1 if a > b else 0)
+
+
+def lq_usage(consumed, scale, penalty_milli, res_weight, lq_weight) -> float:
+    """Info.CalcLocalQueueFSUsage (workload.go:391-427) of one LocalQueue: sum_r weight_r * AsApproximateFloat64(
+    consumed_r (+) penalty_r) in resource-index order, divided by the LocalQueue's fair-sharing weight (1.0 when nil).
+    `consumed` / `scale`: int64Amount per resource (0 = absent); `penalty_milli`: AfsEntryPenalties in milli-units."""
+    usage = 0.0
+    for r in range(len(consumed)):
+        v, s = quantity_add((int(consumed[r]), int(scale[r])), (int(penalty_milli[r]), -3))
+        if v == 0:
+            continue  # a zero quantity adds what an absent key adds: nothing
+        usage += float(res_weight[r]) * quantity_float(v, s)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return float(np.float64(usage) / np.float64(lq_weight))
+
+
+def entry_penalty(req_rows, mask_rows, milli_mul, alpha: float):
+    """CalculateEntryPenalty (admission_fair_sharing.go) of one workload in milli-units per resource:
+    int64(float64(MilliValue(SumTotalRequests_r)) * alpha), over the full TotalRequests (the keys of Requests only)."""
+    R = len(milli_mul)
+    out = []
+    for r in range(R):
+        total = sum(int(q) for q, m in zip(req_rows[:, r], mask_rows) if int(m) >> r & 1)
+        milli = _int64(_int64(total) * int(milli_mul[r]))
+        out.append(int(float(milli) * alpha))
+    return out
+
+
 def _queue_order(a, Q):
-    """Pending workloads of every ClusterQueue in queueOrderingFunc order: (order, start[Q+1])."""
+    """Pending workloads in queueOrderingFunc order per segment: (order, start[S+1], seg_start[Q+1], seg_lq[S]).  A
+    segment is a ClusterQueue, or one LocalQueue of a ClusterQueue with AdmissionFairSharing (numbered
+    ClusterQueue-major)."""
     cq = a["wl_cq"].astype(np.int64)
-    order = np.lexsort((a["wl_uid"], a["wl_ts"], -a["wl_priority"].astype(np.int64), cq))
-    start = np.zeros(Q + 1, np.int64)
-    np.add.at(start, cq + 1, 1)
-    return order, np.cumsum(start)
+    if "wl_lq" in a:
+        afs = a["cq_afs"].astype(bool)
+        n_lq_of = np.bincount(a["lq_cq"].astype(np.int64), minlength=Q)
+        nseg = np.where(afs, n_lq_of, 1)
+        seg_start = np.concatenate([[0], np.cumsum(nseg)])
+        lq_first = np.concatenate([[0], np.cumsum(n_lq_of)])
+        seg_lq = np.full(int(seg_start[-1]), -1, np.int64)
+        for q in np.flatnonzero(afs):
+            seg_lq[seg_start[q]:seg_start[q + 1]] = np.arange(lq_first[q], lq_first[q + 1])
+        lq = a["wl_lq"].astype(np.int64)
+        seg = np.where(afs[cq], seg_start[cq] + lq - lq_first[cq], seg_start[cq])
+    else:
+        seg_start, seg_lq, seg = np.arange(Q + 1), np.full(Q, -1, np.int64), cq
+    S = int(seg_start[-1])
+    order = np.lexsort((a["wl_uid"], a["wl_ts"], -a["wl_priority"].astype(np.int64), seg))
+    start = np.zeros(S + 1, np.int64)
+    np.add.at(start, seg + 1, 1)
+    return order, np.cumsum(start), seg_start, seg_lq
 
 
 def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.CycleOut], max_cycles: int = 10_000) -> DrainResult:
     a = snap.arrays
     Q, R, FR = snap.n_cq, snap.n_resource, snap.n_fr
-    order, qstart = _queue_order(a, Q)
+    order, qstart, seg_start, seg_lq = _queue_order(a, Q)
     qlen = np.diff(qstart)
-    cursor = np.zeros(Q, np.int64)
+    cursor = np.zeros(len(qlen), np.int64)
+    afs_cq = a["cq_afs"].astype(bool) if "wl_lq" in a else np.zeros(Q, bool)
+    if afs_cq.any():
+        L = len(a["lq_cq"])
+        penalty = (a["lq_penalty"].reshape(L, R).astype(object) if "lq_penalty" in a else np.zeros((L, R), object))
+        consumed, cscale = a["lq_consumed"].reshape(L, R), a["lq_consumed_scale"].reshape(L, R)
+        usage_of = lambda l: lq_usage(consumed[l], cscale[l], penalty[l], a["afs_res_weight"], a["lq_weight"][l])  # noqa: E731
+        lqu = {int(l): usage_of(l) for l in seg_lq if l >= 0}
+
+    first_seg = seg_start[:-1]
+
+    def afs_head_seg(q):
+        """segment of the head of AFS ClusterQueue q, -1 = nothing queued"""
+        s0, s1 = int(seg_start[q]), int(seg_start[q + 1])
+        best, bkey = -1, None
+        for s in range(s0, s1):
+            if cursor[s] >= qlen[s]:
+                continue
+            w = order[qstart[s] + cursor[s]]
+            key = (int(a["wl_priority"][w]), int(a["wl_ts"][w]), int(a["wl_uid"][w]))
+            if best >= 0:
+                c = compare_usage(lqu[int(seg_lq[s])], lqu[int(seg_lq[best])])
+                if c > 0 or (c == 0 and (-key[0], key[1], key[2]) >= (-bkey[0], bkey[1], bkey[2])):
+                    continue
+            best, bkey = s, key
+        return best
     strict = a["cq_strategy"].astype(bool)  # KB_QUEUE_STRICT_FIFO = 1
     usage = a["cq_usage"].reshape(Q, FR).astype(np.int64).copy()
     adm = {k: a[k].copy() for k in ("adm_cq", "adm_priority", "adm_ts", "adm_qr_ts", "adm_uid", "adm_evicted", "adm_use_start",
@@ -113,17 +240,21 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     shash = a.get("wl_sched_hash")
     has_qr = a.get("wl_has_quota_reservation")
     gone = np.zeros(snap.n_wl, bool)                              # moved to the inadmissible set by its scheduling hash
-    static = {k: v for k, v in a.items() if not (k.startswith(("wl_", "ps_", "adm_")) or k in ("heads", "cq_usage"))}
+    static = {k: v for k, v in a.items() if not (k.startswith(("wl_", "ps_", "adm_")) or k in ("heads", "cq_usage") + abi.AFS_FIELDS)}
     covers_pods = np.zeros(Q, bool)
     if snap.pods_resource >= 0:
         for q in range(Q):
             masks = a["rg_res_mask"][a["cq_rg_start"][q]:a["cq_rg_start"][q + 1]]
             covers_pods[q] = bool(np.any(masks & (1 << snap.pods_resource)))
-    for cyc in range(max_cycles):
-        live = np.flatnonzero(cursor < qlen)
+    for cyc in range(max_cycles if len(qlen) else 0):
+        hseg = np.where(cursor[np.minimum(first_seg, len(qlen) - 1)] < qlen[np.minimum(first_seg, len(qlen) - 1)], first_seg, -1)
+        for q in np.flatnonzero(afs_cq):
+            hseg[q] = afs_head_seg(q)
+        live = np.flatnonzero(hseg >= 0)
         if len(live) == 0:
             break
-        heads = order[qstart[live] + cursor[live]]  # global pending indices, one per ClusterQueue with work left
+        segs = hseg[live]
+        heads = order[qstart[segs] + cursor[segs]]  # global pending indices, one per ClusterQueue with work left
         cs = abi.FlatSnapshot(n_cq=Q, n_cohort=snap.n_cohort, n_flavor=snap.n_flavor, n_resource=R, pods_resource=snap.pods_resource,
                               flags=snap.flags, now_ns=snap.now_ns + cyc, static_generation=snap.static_generation)
         cs.arrays.update(static)
@@ -172,6 +303,12 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 usage[cqi, fr] += q
                 new_fr.append(fr); new_qty.append(q)
             new_start.append(new_start[-1] + len(cells))
+            if afs_cq[cqi]:  # AfsEntryPenalties.Push of the entry penalty, then the LocalQueue's usage again
+                w, lq = int(heads[e]), int(a["wl_lq"][heads[e]])
+                rows = slice(int(ps_start[w]), int(ps_start[w + 1]))
+                for r, d in enumerate(entry_penalty(ps_req[rows], a["ps_req_mask"][rows], a["afs_milli_mul"], snap.afs_alpha)):
+                    penalty[lq, r] = _int64(int(penalty[lq, r]) + d)
+                lqu[lq] = usage_of(lq)
         n_new = int(ok.sum())
         if n_new:
             g = heads[ok]
@@ -209,12 +346,14 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 if hsh == 0:
                     continue
                 q = int(cqs[e])
-                rest = order[qstart[q] + cursor[q] + 1:qstart[q + 1]]
-                gone[rest[shash[rest] == hsh]] = True
-        cursor[cqs[advance]] += 1
+                for s in range(int(seg_start[q]), int(seg_start[q + 1])):  # every segment of the ClusterQueue's queue
+                    rest = order[qstart[s] + cursor[s] + (s == segs[e]):qstart[s + 1]]
+                    gone[rest[shash[rest] == hsh]] = True
+        cursor[segs[advance]] += 1
         for q in cqs:  # the next head is the first queued workload that was not set aside
-            while cursor[q] < qlen[q] and gone[order[qstart[q] + cursor[q]]]:
-                cursor[q] += 1
+            for s in range(int(seg_start[q]), int(seg_start[q + 1])):
+                while cursor[s] < qlen[s] and gone[order[qstart[s] + cursor[s]]]:
+                    cursor[s] += 1
         if n_new == 0:
             break
     res.cq_usage = usage

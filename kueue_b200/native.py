@@ -86,6 +86,7 @@ def pin_snapshot(snap: abi.FlatSnapshot) -> abi.FlatSnapshot:
         off += pad(v.nbytes)
     out._pinned_block = block
     out.static_generation = snap.static_generation
+    out.afs_alpha = snap.afs_alpha
     return out
 
 

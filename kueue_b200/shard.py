@@ -125,6 +125,20 @@ def shard(snap: abi.FlatSnapshot, rank: int, world: int, node_rank: np.ndarray |
     us, ui = _csr_take(a["adm_use_start"].astype(np.int64), adms)
     out.set("adm_use_start", us)
     out.set("adm_use_fr", a["adm_use_fr"][ui]); out.set("adm_use_qty", a["adm_use_qty"][ui])
+    if "wl_lq" in a:  # AdmissionFairSharing: the LocalQueues travel with their ClusterQueues (still ClusterQueue-major)
+        L = len(a["lq_cq"])
+        lqs = np.flatnonzero(node_rank[a["lq_cq"]] == rank) if L else np.zeros(0, np.int64)
+        lq_remap = np.full(max(1, L), -1, np.int64)
+        lq_remap[lqs] = np.arange(len(lqs))
+        out.set("lq_cq", remap[a["lq_cq"][lqs]])
+        out.set("wl_lq", lq_remap[a["wl_lq"][wls]])
+        out.set("cq_afs", a["cq_afs"][cqs])
+        out.set("lq_weight", a["lq_weight"][lqs])
+        for nm in ("lq_consumed", "lq_consumed_scale", "lq_penalty"):
+            if nm in a:
+                out.set(nm, a[nm].reshape(L, R)[lqs])
+        out.set("afs_res_weight", a["afs_res_weight"]); out.set("afs_milli_mul", a["afs_milli_mul"])
+        out.afs_alpha = snap.afs_alpha
     out.finalize()
     return out, ShardMap(nodes=nodes, wls=wls, podsets=ps_rows, adms=adms, heads=hpos)
 

@@ -29,13 +29,14 @@ def _cohort_forest(n_root: int, fanouts, cqs_per_leaf: int):
 def make_snapshot(config: int = 2, W: int | None = None, Q: int | None = None, F: int | None = None,
                   R: int | None = None, seed: int | None = None, heads: str = "all",
                   podsets_max: int = 1, admitted: int | None = None, preemption: bool | None = None,
-                  partial: bool = False, tight: float = 1.0) -> abi.FlatSnapshot:
+                  partial: bool = False, tight: float = 1.0, afs: int = 0) -> abi.FlatSnapshot:
     """config 1: 100 wl x 10 CQ x 2 flavors x 3 resources, no cohort
        config 2: 100k x 1k x 8 x 4, StrictFIFO, no cohort, usage 60-90% of nominal
        config 3: 1M x 10k, 100 flat cohorts x 100 CQ, BestEffortFIFO, fair sharing
        config 4: 1M x 10k, depth-4 cohort forest (10 -> 5 -> 5 -> 4), classical
     heads: "all" (batched evaluator over every pending workload) | "one_per_cq"
-    (reference cycle: the best-ordered workload of each CQ)."""
+    (reference cycle: the best-ordered workload of each CQ).
+    afs: k > 0 gives every ClusterQueue k LocalQueues with UsageBasedAdmissionFairSharing (see `add_afs`)."""
     dflt = {1: (100, 10, 2, 3), 2: (100_000, 1_000, 8, 4), 3: (1_000_000, 10_000, 8, 4), 4: (1_000_000, 10_000, 8, 4)}[config]
     W = W or dflt[0]; Q = Q or dflt[1]; F = F or dflt[2]; R = R or dflt[3]
     rng = np.random.Generator(np.random.PCG64(config if seed is None else seed))
@@ -149,6 +150,8 @@ def make_snapshot(config: int = 2, W: int | None = None, Q: int | None = None, F
         snap.set("ps_min_count", mc)
     ok = rng.integers(0, 2**63, P, dtype=np.uint64) | rng.integers(0, 2**63, P, dtype=np.uint64) | np.uint64(1 << (F - 1))
     snap.set("ps_flavor_ok", ok)  # ~75% of flavors eligible, last flavor always
+    if afs:
+        add_afs(snap, afs, seed=(config if seed is None else seed) + 1000)
     if heads == "all":
         snap.set("heads", np.arange(W))
     else:
@@ -185,3 +188,30 @@ def compact_to_heads(snap: abi.FlatSnapshot) -> abi.FlatSnapshot:
             out.set(nm, a[nm][h])
     out.set("heads", np.arange(len(h)))
     return out.finalize()
+
+
+def add_afs(snap: abi.FlatSnapshot, k: int, seed: int = 0, half_life_s: float = 10.0, sampling_s: float = 1.0) -> abi.FlatSnapshot:
+    """AdmissionFairSharing tables (include/kueue_b200.h): k LocalQueues per ClusterQueue (numbered ClusterQueue-major),
+    every ClusterQueue in UsageBasedAdmissionFairSharing mode, every pending workload in a random LocalQueue of its
+    ClusterQueue.  Seeded LocalQueue weights, consumed usage (cpu as whole or milli quantities, the other resources
+    whole), initial entry penalties and ResourceWeights.  Resource 0 is cpu (milli units)."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    Q, R, W = snap.n_cq, snap.n_resource, snap.n_wl
+    L = Q * k
+    snap.set("lq_cq", np.repeat(np.arange(Q), k))
+    snap.set("wl_lq", snap.arrays["wl_cq"].astype(np.int64) * k + rng.integers(0, k, W))
+    snap.set("cq_afs", np.ones(Q))
+    snap.set("lq_weight", rng.choice([0.5, 1.0, 1.5, 2.0], L))
+    scale = np.array([2_000, 2**31, 4, 100_000, 50, 10, 1000, 64][:R], np.int64)
+    val = (rng.uniform(0, 8, (L, R)) * scale[None, :]).astype(np.int64)
+    sc = np.zeros((L, R), np.int64)
+    whole = rng.random(L) < 0.5  # cpu as "3" (scale 0) or "3500m" (scale -3)
+    val[whole, 0] //= 1000
+    sc[~whole, 0] = -3
+    val[rng.random((L, R)) < 0.1] = 0  # absent keys
+    snap.set("lq_consumed", val); snap.set("lq_consumed_scale", sc)
+    snap.set("lq_penalty", np.where(rng.random((L, R)) < 0.3, rng.integers(0, 5000, (L, R)), 0))
+    snap.set("afs_res_weight", rng.choice([0.5, 1.0, 2.0], R))
+    snap.set("afs_milli_mul", np.where(np.arange(R) == 0, 1, 1000))
+    snap.afs_alpha = 1.0 - 0.5 ** (sampling_s / half_life_s) if half_life_s else 0.0
+    return snap
