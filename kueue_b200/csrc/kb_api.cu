@@ -646,12 +646,13 @@ static int32_t upload_impl(kb_handle *h, const kb_snapshot *s, bool sync) {
     SUP(nd_tin, h->nd_tin.data(), h->nd_tin.size()); SUP(nd_tout, h->nd_tout.data(), h->nd_tout.size());
     SUP(cq_path, h->cq_path.data(), h->cq_path.size()); SUP(cq_plen, h->cq_plen.data(), h->cq_plen.size());
     SUP(tree_blob, h->tree_blob.data(), h->tree_blob.size()); SUP(tree_blob_off, h->tree_blob_off.data(), h->tree_blob_off.size());
-    D.tl_nominal = D.tl_blimit = D.tl_llimit = nullptr; D.tl_usage = nullptr;
+    D.tl_subtree = D.tl_blimit = D.tl_lquota = nullptr; D.tl_usage = nullptr;
     if (tl_cells && tl_cells < (size_t)INT32_MAX) {  // quota tables in tree-local row order (k_cycle_flat's bulk staging)
       i64 *tn = h->sarena.take<i64>(tl_cells), *tb_ = h->sarena.take<i64>(tl_cells), *tl_ = h->sarena.take<i64>(tl_cells);
       D.FR = FR; D.Q = Q;
       k_tl_static<<<(unsigned)((tl_cells + 255) / 256), 256, 0, h->stream>>>(D, tn, tb_, tl_, (int)tl_cells);
-      D.tl_nominal = tn; D.tl_blimit = tb_; D.tl_llimit = tl_;
+      k_tl_root<<<(unsigned)(((size_t)D.nTrees * FR + 255) / 256), 256, 0, h->stream>>>(D, tn, tl_);
+      D.tl_subtree = tn; D.tl_blimit = tb_; D.tl_lquota = tl_;
     }
     D.path_stride = h->path_stride;
 #undef SUP
@@ -884,12 +885,12 @@ static int32_t upload_impl(kb_handle *h, const kb_snapshot *s, bool sync) {
                   (!(s->flags & KB_F_FAIR_SHARING) || all_flat) && getenv("KB_NO_FUSED") == nullptr;
     // k_cycle_flat: every tree flat, FR <= 64, the relocated copy of the largest root fits shared memory
     h->d_cq_rec = h->arena.take<int4>(h->tree_nodes.size() + 1); D.cq_rec = h->d_cq_rec;
-    D.tl_usage = D.tl_nominal ? h->arena.take<i64>(h->tree_nodes.size() * (size_t)FR) : nullptr;
+    D.tl_usage = D.tl_subtree ? h->arena.take<i64>(h->tree_nodes.size() * (size_t)FR) : nullptr;
     h->flat_rcap = (int)std::min<size_t>((size_t)1 << 20, nnm * (size_t)std::max(1, h->max_head_podsets));
     h->flat_smem = flat_layout((int)nnm, FR, R, h->flat_rcap, h->max_blob_bytes).total;
     if (h->flat_static_smem == 0) { cudaFuncAttributes fa{}; cudaFuncGetAttributes(&fa, k_cycle_flat); h->flat_static_smem = std::max<size_t>(16, fa.sharedSizeBytes); }
     h->flat_on = h->fused_on && all_flat && FR <= 64 && h->flat_smem + h->flat_static_smem <= 227 * 1024 && getenv("KB_FUSED_V1") == nullptr;
-    h->flat_on = h->flat_on && h->max_head_podsets < 65536;
+    h->flat_on = h->flat_on && h->max_head_podsets < KB_REC_GENERAL && D.tl_subtree != nullptr;  // head record; staged from the tree-local tables only
     if (h->fused_on && !h->flat_on && !h->drain_mode) {
       CUDA_TRY(h, cudaMemsetAsync(h->d_cq_entry, 0xff, sizeof(int32_t) * (size_t)Q, h->stream));
       if (H) k_cq_entry<<<(unsigned)((H + 255) / 256), 256, 0, h->stream>>>(D, h->d_cq_entry);

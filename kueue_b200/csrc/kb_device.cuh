@@ -89,9 +89,10 @@ struct DevSnap {
   const int4 *cq_rec;          // [tree_start[nTrees]] head record per tree node (kb_flat.cuh: cq_rec_write), valid when stamped rec_stamp
   unsigned rec_stamp;
   // quota tables in tree-local row order (row = tree_start[t] + local handle): one root's rows are contiguous, so
-  // k_cycle_flat stages each table with ONE bulk copy (cp.async.bulk).  Static ones are permuted when the static tables
-  // are uploaded, the usage by k_flat_prep / k_cq_rec every cycle (zero rows for cohorts).
-  const i64 *tl_nominal, *tl_blimit, *tl_llimit; i64 *tl_usage;
+  // k_cycle_flat stages each table with ONE bulk copy (cp.async.bulk).  Static ones are built when the static tables
+  // are uploaded (k_tl_static / k_tl_root: SubtreeQuota and localQuota, final for every row of a flat tree), the usage
+  // by k_flat_prep / k_cq_rec every cycle (zero rows for cohorts).
+  const i64 *tl_subtree, *tl_blimit, *tl_lquota; i64 *tl_usage;
   // ---- derived, static per topology (host-built at upload) ----
   const int32_t *root_slot;   // [N] dense index of the node's root among all roots
   const int32_t *depth;       // [N] distance to the root

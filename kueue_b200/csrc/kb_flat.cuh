@@ -19,7 +19,7 @@
 
 struct FlatLay {  // byte offsets into the dynamic shared memory of k_cycle_flat (computed on the host, passed by value)
   uint32_t u, sub, lq, bl, av, pot, over, lend, blob, n_e, n_wl, n_ps0, n_psn, e_gid, e_cq, e_prio, e_ident, e_psn, e_wl, e_ps0, e_ts, e_lg, e_qr,
-      e_fast, e_mode, e_borrow, e_rank, sorted, m_sorted, d_sorted, r_gid, r_count, r_min, r_mask, r_group, r_ok, r_req, r_last, o_fl, o_md, o_tr, o_cnt, key, misc, snap, rec, total;
+      e_fast, e_mode, e_borrow, e_rank, m_sorted, d_sorted, r_gid, r_count, r_min, r_mask, r_group, r_ok, r_req, r_last, o_fl, o_md, o_tr, o_cnt, key, misc, snap, rec, total;
 };
 __host__ __device__ inline FlatLay flat_layout(int ncap, int FR, int R, int rcap, int bcap) {
   FlatLay L;
@@ -35,7 +35,7 @@ __host__ __device__ inline FlatLay flat_layout(int ncap, int FR, int R, int rcap
   L.e_ts = take((size_t)ncap * 8); L.e_lg = take((size_t)ncap * 8); L.e_qr = take((size_t)ncap);
   L.e_fast = take((size_t)ncap);
   L.e_mode = take((size_t)ncap * 4); L.e_borrow = take((size_t)ncap * 4); L.e_rank = take((size_t)ncap * 4);
-  L.sorted = take((size_t)ncap * 4); L.m_sorted = take((size_t)ncap * 4); L.d_sorted = take(((size_t)ncap / 32 + 2) * 4);
+  L.m_sorted = take((size_t)ncap * 4); L.d_sorted = take(((size_t)ncap / 32 + 2) * 4);
   L.r_gid = take((size_t)rcap * 4); L.r_count = take((size_t)rcap * 4); L.r_min = take((size_t)rcap * 4); L.r_mask = take((size_t)rcap * 4);
   L.r_group = take((size_t)rcap * 4); L.r_ok = take((size_t)rcap * 8); L.r_req = take((size_t)rcap * R * 8); L.r_last = take((size_t)rcap * R);
   L.o_fl = take((size_t)rcap * R); L.o_md = take((size_t)rcap * R); L.o_tr = take((size_t)rcap * R); L.o_cnt = take((size_t)rcap * 4);
@@ -60,16 +60,20 @@ struct TreeBlobHdr {
 };
 static_assert(sizeof(TreeBlobHdr) == 80, "TreeBlobHdr layout");
 
-// Head records: per tree node (tree-local order) {entry, workload, first podset row, podset count | stamp << 16} of the
-// ClusterQueue's head.  A record is valid only when its stamp is the current one (DevSnap::rec_stamp), so the table
-// is never cleared between cycles (the host clears it when it is (re)allocated or the 16-bit stamp wraps).
+// Head records: per tree node (tree-local order) {entry, workload, first podset row, podset count | KB_REC_GENERAL |
+// stamp << 16} of the ClusterQueue's head.  A record is valid only when its stamp is the current one
+// (DevSnap::rec_stamp), so the table is never cleared between cycles (the host clears it when it is (re)allocated or
+// the 16-bit stamp wraps).  KB_REC_GENERAL marks a head that k_cycle_flat nominates with the general walk: several
+// podsets (or none), or one that partial admission could reduce.
+#define KB_REC_GENERAL 0x8000
 __device__ __forceinline__ void cq_rec_write(const DevSnap &D, int4 *rec, int e) {
   const int wl = D.heads[e];
   const int cq = D.wl_cq[wl];
   const int slot = D.root_slot[cq] - D.nLone;
   if (slot < 0) return;
-  const int ps0 = D.wl_ps_start[wl];
-  rec[D.tree_start[slot] + D.local_idx[cq]] = make_int4(e, wl, ps0, (D.wl_ps_start[wl + 1] - ps0) | (int)(D.rec_stamp << 16));
+  const int ps0 = D.wl_ps_start[wl], np = D.wl_ps_start[wl + 1] - ps0;
+  const bool general = np != 1 || ((D.flags & KB_F_PARTIAL_ADMISSION) && D.ps_min_count[ps0] >= 0 && D.ps_count[ps0] > D.ps_min_count[ps0]);
+  rec[D.tree_start[slot] + D.local_idx[cq]] = make_int4(e, wl, ps0, np | (general ? KB_REC_GENERAL : 0) | (int)(D.rec_stamp << 16));
 }
 // usage rows into tree-local order (cohort rows zero): cell i of [tree nodes][FR]
 __device__ __forceinline__ void tl_usage_write(const DevSnap &D, int i) {
@@ -81,12 +85,29 @@ __global__ void k_cq_rec(DevSnap D, int4 *rec, int tl_cells) {
   if (i < D.H) cq_rec_write(D, rec, i);
   if (i < tl_cells) tl_usage_write(D, i);
 }
-// static quota tables into tree-local row order (once per static upload)
-__global__ void k_tl_static(DevSnap D, i64 *nominal, i64 *blimit, i64 *llimit, int tl_cells) {
+// static quota tables into tree-local row order (once per static upload), holding the quotas k_cycle_flat derives from
+// them: SubtreeQuota (a ClusterQueue's is its nominal quota, resource_node.go:160-166) and localQuota (:66-71) per cell.
+// A flat root's SubtreeQuota and localQuota depend on its ClusterQueues' rows and are written by k_tl_root.  Cohort
+// rows of hierarchical trees are left at nominal / local_quota(nominal) and never read: k_cycle_flat needs every tree flat.
+__global__ void k_tl_static(DevSnap D, i64 *subtree, i64 *blimit, i64 *lquota, int tl_cells) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= tl_cells) return;
   const size_t g = (size_t)D.tree_nodes[i / D.FR] * D.FR + i % D.FR;
-  nominal[i] = D.nominal[g]; blimit[i] = D.blimit[g]; llimit[i] = D.llimit[g];
+  subtree[i] = D.nominal[g]; blimit[i] = D.blimit[g]; lquota[i] = local_quota(D.nominal[g], D.llimit[g]);
+}
+// the root row of a flat tree: SubtreeQuota = nominal + sum of (SubtreeQuota - localQuota) over the ClusterQueues
+// (accumulateFromChild resource_node.go:210-217), then its localQuota.  One thread per (tree, column), after k_tl_static.
+__global__ void k_tl_root(DevSnap D, i64 *subtree, i64 *lquota) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= D.nTrees * D.FR) return;
+  const int t = k / D.FR, fr = k % D.FR;
+  if (!D.tree_flat[t]) return;
+  const size_t r0 = (size_t)D.tree_start[t] * D.FR + fr;
+  const int nn = D.tree_start[t + 1] - D.tree_start[t];
+  i64 sub = subtree[r0];
+  for (int h = 1; h < nn; h++) sub += subtree[r0 + (size_t)h * D.FR] - lquota[r0 + (size_t)h * D.FR];
+  subtree[r0] = sub;
+  lquota[r0] = local_quota(sub, D.llimit[(size_t)D.tree_nodes[D.tree_start[t]] * D.FR + fr]);
 }
 // Everything the cycle needs prepared on the device, in one launch: head records, result rows of workloads that are
 // not heads (-1 / 0), cleared cycle header.
@@ -208,12 +229,23 @@ __device__ __noinline__ void flat_expand_general(const DevSnap &L, int i, i64 *q
 // candidates (candidates_possible), so SimulatePreemption is NoCandidates.  The flavors of a round are then taken in
 // order by flavor_take, the rule get_assignments_coop uses.  The group also writes the podset's assignment row, the
 // entry's mode / borrowing and its iterator key.  A group of one podset assigns like the podset alone.
+// available / potentialAvailable (resource_node.go:104-133) of a ClusterQueue cell of a flat tree: sub, u, lq, bl of
+// the cell, srt / urt the root's SubtreeQuota and usage in the same column
+__device__ __forceinline__ void flat_cell_available(i64 sub, i64 u, i64 lq, i64 bl, i64 srt, i64 urt, i64 &av, i64 &pot) {
+  i64 pa = srt - urt;
+  pot = lq + srt;
+  if (bl != KB_NO_LIMIT) { pa = imin((sub - lq) - imax(0, u - lq) + bl, pa); pot = imin(sub + bl, pot); }
+  av = imax(0, lq - u) + pa;
+}
+// The lanes compute available / potentialAvailable of the cells they evaluate and the over-usage of the entry's own
+// row themselves (the root's lendable is in s_lend from the tree pass), so the walk needs no sweep over the tree.
+// With qrow set, the group also writes the entry's dense request row (Assignment.Usage.Quota, absent = -1).
 template <int NG>
 __device__ __forceinline__ void flat_nominate_group(const FlatLay &Y, int i, int R, int FR, unsigned flags, int pods, bool has_qr_table,
-                                                    unsigned gmask, int gbase, int glane) {
+                                                    unsigned gmask, int gbase, int glane, i64 *qrow) {
   extern __shared__ __align__(16) unsigned char smem_raw[];  // the kernel's
-  const i64 *s_u = (const i64 *)(smem_raw + Y.u), *s_sub = (const i64 *)(smem_raw + Y.sub), *s_av = (const i64 *)(smem_raw + Y.av),
-            *s_pot = (const i64 *)(smem_raw + Y.pot);
+  const i64 *s_u = (const i64 *)(smem_raw + Y.u), *s_sub = (const i64 *)(smem_raw + Y.sub), *s_lq = (const i64 *)(smem_raw + Y.lq),
+            *s_bl = (const i64 *)(smem_raw + Y.bl);
   const unsigned char *s_blob = smem_raw + Y.blob;
   const TreeBlobHdr *BH = (const TreeBlobHdr *)s_blob;
   const int32_t *b_rgs = (const int32_t *)(s_blob + BH->rgs), *b_rgfl = (const int32_t *)(s_blob + BH->rgfl), *b_fl = (const int32_t *)(s_blob + BH->fl);
@@ -265,13 +297,15 @@ __device__ __forceinline__ void flat_nominate_group(const FlatLay &Y, int i, int
           int rpm = PM_FIT, rb = 0, maxb = 0; uint32_t pmask = 0; bool reason = false;
           for (int r = 0; r < R; r++) {
             if (!((rgm >> r) & 1)) continue;
-            const int c = hq * FR + f * R + r;
-            const i64 val = request(r);
+            const int fr = f * R + r, c = hq * FR + fr;
+            const i64 val = request(r), sub = s_sub[c], u = s_u[c];
+            i64 av, pot;
+            flat_cell_available(sub, u, s_lq[c], s_bl[c], s_sub[fr], s_u[fr], av, pot);
             int pm = PM_NOFIT, b = 0;
-            if (val <= s_pot[c]) {  // cell_eval: find_height on a flat tree is the root's height above nominal, mayReclaim below
-              const bool above = s_u[c] + val > s_sub[c];  // nominal == SubtreeQuota for a ClusterQueue
+            if (val <= pot) {  // cell_eval: find_height on a flat tree is the root's height above nominal, mayReclaim below
+              const bool above = u + val > sub;  // nominal == SubtreeQuota for a ClusterQueue
               b = above ? hp : 0;
-              pm = fits_mode(val, s_av[c], s_sub[c], !above, [&] { return can_pwb; });
+              pm = fits_mode(val, av, sub, !above, [&] { return can_pwb; });
               if (pm == PM_NEED) pm = PM_NOCAND;  // no candidates: what SimulatePreemption returns
             }
             if (pm != PM_FIT) reason = true;
@@ -317,9 +351,10 @@ __device__ __forceinline__ void flat_nominate_group(const FlatLay &Y, int i, int
   // iterator key: max over the resources of the DominantResourceShare terms of entry_share_ratio
   double best = 0.0;
   if (fair) {
-    const i64 *s_over = (const i64 *)(smem_raw + Y.over), *s_lend = (const i64 *)(smem_raw + Y.lend);
+    const i64 *s_lend = (const i64 *)(smem_raw + Y.lend);
     for (int r = glane; r < R; r += NG) {
-      i64 bo = s_over[hq * R + r];
+      i64 bo = 0;  // over-usage of the row in resource r, summed over the flavors
+      for (int c = hq * FR + r; c < (hq + 1) * FR; c += R) bo += imax(0, s_u[c] - s_sub[c]);
       const int f = o_fl[(size_t)l * R + r];
       if (f >= 0) {
         const int c = hq * FR + f * R + r;
@@ -341,6 +376,13 @@ __device__ __forceinline__ void flat_nominate_group(const FlatLay &Y, int i, int
                    fair ? (unsigned)((const int32_t *)(s_blob + BH->gid))[hq] : (unsigned)((const int *)(smem_raw + Y.e_gid))[i],
                    (u64 *)(smem_raw + Y.key) + (size_t)i * 4);
   }
+  if (qrow) {  // one podset: the row is its request on the assigned flavors
+    __syncwarp(gmask);  // the assignment row was written by all lanes of the group
+    for (int fr = glane; fr < FR; fr += NG) {
+      const int f = fr / R, r = fr - f * R;
+      qrow[fr] = o_fl[(size_t)l * R + r] == f ? request(r) : -1;
+    }
+  }
 }
 
 __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_constant__ DevSnap D, const __grid_constant__ FlatLay Y) {
@@ -352,12 +394,8 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
   auto row_of = [&](int i) { return fr_p2 ? i >> fr_sh : i / FR; };
   auto col_of = [&](int i) { return fr_p2 ? i & (FR - 1) : i % FR; };
   long long tk0 = clock64();
-#ifndef KB_FLAT_PROBE
-#define KB_FLAT_PROBE 0
-#endif
-  // fine-grained probe points of thread 0 (instrumented builds only: -DKB_FLAT_PROBE=<set>): cycles since the previous point
-#define KB_PP(set, k) do { if (KB_FLAT_PROBE == (set) && blockIdx.x == 0 && threadIdx.x == 0) { long long now_ = clock64(); D.sstat[k] = (u64)(now_ - tk0); tk0 = now_; } } while (0)
-#define KB_FPHASE(k) do { if (KB_FLAT_PROBE) break; if (blockIdx.x == 0 && threadIdx.x == 0) { long long now_ = clock64(); D.sstat[k] = (u64)(now_ - tk0); tk0 = now_; } } while (0)
+  // phase probe (tools/phase_probe.py): SM cycles of thread 0 of CTA 0 since the previous point
+#define KB_FPHASE(k) do { if (blockIdx.x == 0 && threadIdx.x == 0) { long long now_ = clock64(); D.sstat[k] = (u64)(now_ - tk0); tk0 = now_; } } while (0)
   i64 *s_u = (i64 *)(smem_raw + Y.u), *s_sub = (i64 *)(smem_raw + Y.sub), *s_lq = (i64 *)(smem_raw + Y.lq), *s_bl = (i64 *)(smem_raw + Y.bl);
   i64 *s_av = (i64 *)(smem_raw + Y.av), *s_pot = (i64 *)(smem_raw + Y.pot), *s_over = (i64 *)(smem_raw + Y.over), *s_lend = (i64 *)(smem_raw + Y.lend);
   unsigned char *s_blob = smem_raw + Y.blob;
@@ -365,9 +403,9 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
   int *e_gid = (int *)(smem_raw + Y.e_gid), *e_cq = (int *)(smem_raw + Y.e_cq), *e_prio = (int *)(smem_raw + Y.e_prio), *e_ident = (int *)(smem_raw + Y.e_ident);
   int *e_psn = (int *)(smem_raw + Y.e_psn), *e_wl = (int *)(smem_raw + Y.e_wl), *e_ps0 = (int *)(smem_raw + Y.e_ps0);
   i64 *e_ts = (i64 *)(smem_raw + Y.e_ts), *e_lg = (i64 *)(smem_raw + Y.e_lg); uint8_t *e_qr = smem_raw + Y.e_qr;
-  uint8_t *e_fast = smem_raw + Y.e_fast;  // bit 0: nominated by the group walk of phase 5, bit 1: its ClusterQueue covers the pods resource
+  uint8_t *e_fast = smem_raw + Y.e_fast;  // bit 0: nominated by the group walk, bit 1: its ClusterQueue covers the pods resource
   int *e_mode = (int *)(smem_raw + Y.e_mode), *e_borrow = (int *)(smem_raw + Y.e_borrow), *e_rank = (int *)(smem_raw + Y.e_rank);
-  int *s_sorted = (int *)(smem_raw + Y.sorted), *m_sorted = (int *)(smem_raw + Y.m_sorted); uint32_t *ok_bits = (uint32_t *)(smem_raw + Y.d_sorted);
+  int *m_sorted = (int *)(smem_raw + Y.m_sorted); uint32_t *ok_bits = (uint32_t *)(smem_raw + Y.d_sorted);
   int *r_gid = (int *)(smem_raw + Y.r_gid), *r_count = (int *)(smem_raw + Y.r_count), *r_min = (int *)(smem_raw + Y.r_min);
   uint32_t *r_mask = (uint32_t *)(smem_raw + Y.r_mask); int *r_group = (int *)(smem_raw + Y.r_group); u64 *r_ok = (u64 *)(smem_raw + Y.r_ok);
   i64 *r_req = (i64 *)(smem_raw + Y.r_req); int8_t *r_last = (int8_t *)(smem_raw + Y.r_last);
@@ -378,24 +416,23 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
   // ---- 0. staging.  Everything this CTA will read from global memory is requested here, all loads independent.
   const int ts0 = D.tree_start[t];
   const int nn = D.tree_start[t + 1] - ts0;
-  const int32_t *nodes = D.tree_nodes + ts0;
   const int tb = nn * FR;
+  const size_t r0 = (size_t)ts0 * FR;  // first cell of the tree in the tree-local tables (DevSnap::tl_*)
   int4 *s_rec = (int4 *)(smem_raw + Y.rec);
   __shared__ __align__(8) unsigned long long s_mbar;
-  // Tree-local tables (DevSnap::tl_*): a root's rows are contiguous -> one bulk copy per table, issued by one thread,
-  // completion counted in bytes on an mbarrier.  Otherwise (odd rows: 16 B alignment) per-thread cp.async gathers.
-  const bool bulk = D.tl_nominal != nullptr && (FR & 1) == 0;
-  if (bulk) {
+  // A root's rows are contiguous in the tree-local tables -> one bulk copy per table, issued by one thread, completion
+  // counted in bytes on an mbarrier.  Rows of odd width are not 16 B aligned: per-thread loads.
+  // SubtreeQuota and localQuota arrive final (k_tl_static / k_tl_root): the tree pass below only sums usage.
+  if ((FR & 1) == 0) {
     if (tid == 0) mbar_init(&s_mbar, 1);
     __syncthreads();
     if (tid == 0) {
       const int b0 = D.tree_blob_off[t], bn = D.tree_blob_off[t + 1] - b0;  // static block of the tree (multiple of 16 B)
       const unsigned tbytes = (unsigned)tb * 8u;
       mbar_expect_tx(&s_mbar, 4u * tbytes + (unsigned)bn + (unsigned)nn * 16u);
-      const size_t r0 = (size_t)ts0 * FR;
-      bulk_g2s(s_sub, D.tl_nominal + r0, tbytes, &s_mbar);  // SubtreeQuota = Nominal (updateCohortResourceNode resource_node.go:184-190)
+      bulk_g2s(s_sub, D.tl_subtree + r0, tbytes, &s_mbar);
       bulk_g2s(s_bl, D.tl_blimit + r0, tbytes, &s_mbar);
-      bulk_g2s(s_lq, D.tl_llimit + r0, tbytes, &s_mbar);    // lending limit for now; localQuota once SubtreeQuota is final
+      bulk_g2s(s_lq, D.tl_lquota + r0, tbytes, &s_mbar);
       bulk_g2s(s_u, D.tl_usage + r0, tbytes, &s_mbar);      // ClusterQueue usage, zero rows for cohorts
       bulk_g2s(s_blob, D.tree_blob + b0, (unsigned)bn, &s_mbar);
       bulk_g2s(s_rec, D.cq_rec + ts0, (unsigned)nn * 16u, &s_mbar);
@@ -406,59 +443,46 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
       while (!mbar_try_wait(&s_mbar, 0)) if (++spins > (1u << 24)) __trap();  // a lost copy must not hang the device
     }
   } else {
-  {
-    const int b0 = D.tree_blob_off[t], bn = D.tree_blob_off[t + 1] - b0;  // static block of the tree (multiple of 16 B)
-    for (int c = tid * 16; c < bn; c += nthreads * 16) cp_async16(s_blob + c, D.tree_blob + b0 + c);
-  }
-  if ((FR & 1) == 0) {  // rows are 16 B aligned: two cells per request, straight into shared memory
-    const int half = tb >> 1;
-    for (int c = tid; c < half; c += nthreads) {
-      const int i = c << 1;
-      const int nd = nodes[row_of(i)];
-      const size_t g = (size_t)nd * FR + col_of(i);
-      cp_async16(s_sub + i, D.nominal + g);
-      cp_async16(s_bl + i, D.blimit + g);
-      cp_async16(s_lq + i, D.llimit + g);
-      if (nd < D.Q) cp_async16(s_u + i, D.cq_usage + g);
-      else { s_u[i] = 0; s_u[i + 1] = 0; }
+    {
+      const int b0 = D.tree_blob_off[t], bn = D.tree_blob_off[t + 1] - b0;  // static block of the tree (multiple of 16 B)
+      for (int c = tid * 16; c < bn; c += nthreads * 16) cp_async16(s_blob + c, D.tree_blob + b0 + c);
     }
-  } else {
     for (int i = tid; i < tb; i += nthreads) {
-      const int nd = nodes[row_of(i)];
-      const size_t g = (size_t)nd * FR + col_of(i);
-      s_sub[i] = D.nominal[g]; s_bl[i] = D.blimit[g]; s_lq[i] = D.llimit[g];
-      s_u[i] = nd < D.Q ? D.cq_usage[g] : 0;
+      s_sub[i] = D.tl_subtree[r0 + i]; s_bl[i] = D.tl_blimit[r0 + i]; s_lq[i] = D.tl_lquota[r0 + i]; s_u[i] = D.tl_usage[r0 + i];
     }
+    for (int h = tid; h < nn; h += nthreads) s_rec[h] = D.cq_rec[ts0 + h];
+    if (tid == nthreads - 1) *(DevSnap *)(smem_raw + Y.snap) = D;
+    cp_async_wait_all();
+    __syncthreads();
   }
-  for (int h = tid; h < nn; h += nthreads) s_rec[h] = D.cq_rec[ts0 + h];
-  if (tid == nthreads - 1) *(DevSnap *)(smem_raw + Y.snap) = D;
-  cp_async_wait_all();
-  __syncthreads();
-  }
+  bool general_mine = false;  // a head of the general walk (see phase 2)
   for (int h = tid; h < nn; h += nthreads) {  // the head of every ClusterQueue of the tree (record written by k_flat_prep / k_cq_rec)
     const int4 rc = s_rec[h];
     const bool live = ((unsigned)rc.w >> 16) == D.rec_stamp;  // written for this cycle
-    n_e[h] = live ? rc.x : -1; n_wl[h] = rc.y; n_ps0[h] = rc.z; n_psn[h] = live ? (rc.w & 0xffff) : 0;
+    n_e[h] = live ? rc.x : -1; n_wl[h] = rc.y; n_ps0[h] = rc.z; n_psn[h] = live ? (rc.w & (KB_REC_GENERAL - 1)) : 0;
     if (live) {  // the entry's per-cycle records are gathered in phase 2: request their lines now
       auto touch = [](const void *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); };
       const int wl = rc.y, row = rc.z;
       touch(D.wl_priority + wl); touch(D.wl_ts + wl); touch(D.wl_last_gen + wl);
       if (D.wl_has_qr) touch(D.wl_has_qr + wl);
-      if ((rc.w & 0xffff) > 0) {
+      if ((rc.w & (KB_REC_GENERAL - 1)) > 0) {
         touch(D.ps_count + row); touch(D.ps_min_count + row); touch(D.ps_req_mask + row); touch(D.ps_flavor_ok + row);
         touch(D.ps_req + (size_t)row * R); touch(D.ps_last_tried + (size_t)row * R);
         if (D.ps_group) touch(D.ps_group + row);
       }
+      if (rc.w & KB_REC_GENERAL) general_mine = true;
     }
   }
-  __syncthreads();
+  // The general walk reads available / potentialAvailable and the fair-sharing sums of every cell: the sweep of
+  // phase 2 runs only for a root with a head of the general walk.
+  const bool sweep = __syncthreads_or(general_mine);
   KB_FPHASE(0);
-  KB_PP(1, 0);
   const TreeBlobHdr *BH = (const TreeBlobHdr *)s_blob;
   const int32_t *b_gid = (const int32_t *)(s_blob + BH->gid), *b_par = (const int32_t *)(s_blob + BH->par), *b_hgt = (const int32_t *)(s_blob + BH->hgt);
   const uint8_t *b_reclaim = s_blob + BH->reclaim;
+  const bool fair = (D.flags & KB_F_FAIR_SHARING) != 0;  // every tree is flat here: all entries take the fair flat key
 
-  // ---- 1. entries of the root in ClusterQueue (= local handle) order + local podset-row numbering (warp 0), and the
+  // ---- 1. entries of the root in ClusterQueue (= local handle) order + local podset-row numbering, and the
   // bottom-up pass of the flat tree for everyone: accumulateFromChild resource_node.go:210-217, children -> root
   // one warp per 32 nodes: ballot + warp scan, then the warps' totals are scanned (chunks of 32 warps, carried)
   {
@@ -485,13 +509,14 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
       if (e >= 0) {
         const int i = cnt_base + pc + __popc(m & ((1u << lane) - 1));
         e_gid[i] = e; e_cq[i] = h; e_ident[i] = i; e_wl[i] = n_wl[h]; e_ps0[i] = n_ps0[h]; e_psn[i] = rows_base + pr + incl - pn;
+        e_fast[i] = (s_rec[h].w & KB_REC_GENERAL) ? 0 : 1;
+        n_e[h] = i;  // from here on: the local entry of the ClusterQueue (publish)
       }
       cnt_base += tc; rows_base += tr;
       if (c0 + nthreads < nn) __syncthreads();  // w_cnt / w_rows are rewritten by the next chunk
     }
     if (tid == 0) { e_psn[cnt_base] = rows_base; s_misc[0] = cnt_base; s_misc[1] = rows_base; }
   }
-  KB_PP(1, 1);
   // the relocated snapshot: every table the shared device functions read, in local numbering.  It lives in shared
   // memory itself (one thread fills it in): ~50 patched pointers would otherwise sit in every thread's stack.
   if (tid == nthreads - 1) {
@@ -514,161 +539,139 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
   }
   if (nthreads % FR == 0) {  // a thread stays in one column: private partial sums over its rows
     const int fr = tid % FR, g = tid / FR, G = nthreads / FR;
-    i64 dsub = 0, dus = 0;
-    for (int h = 1 + g; h < nn; h += G) {
-      const int c = h * FR + fr;
-      const i64 sub = s_sub[c];
-      const i64 lq = local_quota(sub, s_lq[c]);
-      dsub += sub - lq;
-      dus += imax(0, s_u[c] - lq);
-    }
+    i64 dus = 0;
+    for (int h = 1 + g; h < nn; h += G) { const int c = h * FR + fr; dus += imax(0, s_u[c] - s_lq[c]); }
     const int pitch = FR + 1;  // padded: the column-wise read below is conflict free
-    if ((size_t)2 * tb >= (size_t)2 * G * pitch) {
-      // partials -> scratch (avail / potential are not written yet), one warp per column sums them by shuffles
-      i64 *p_sub = s_av, *p_u = s_av + (size_t)G * pitch;
-      p_sub[g * pitch + fr] = dsub; p_u[g * pitch + fr] = dus;
-      KB_PP(1, 2);
+    if ((size_t)tb >= (size_t)G * pitch) {
+      // partials -> scratch (avail is not written yet), one warp per column sums them by shuffles
+      i64 *p_u = s_av;
+      p_u[g * pitch + fr] = dus;
       __syncthreads();
-      KB_PP(1, 3);
       for (int c = warp; c < FR; c += nthreads >> 5) {
-        i64 a = 0, b = 0;
-        for (int k = lane; k < G; k += 32) { a += p_sub[k * pitch + c]; b += p_u[k * pitch + c]; }
-        for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); b += __shfl_xor_sync(0xffffffffu, b, o); }
-        if (lane == 0) { s_sub[c] += a; s_u[c] += b; }
+        i64 b = 0;
+        for (int k = lane; k < G; k += 32) b += p_u[k * pitch + c];
+        for (int o = 16; o > 0; o >>= 1) b += __shfl_xor_sync(0xffffffffu, b, o);
+        if (lane == 0) s_u[c] += b;
       }
-    } else {  // small tree: few rows per column, little contention
-      if (dsub) atomicAdd((u64 *)&s_sub[fr], (u64)dsub);
-      if (dus) atomicAdd((u64 *)&s_u[fr], (u64)dus);
+    } else if (dus) {  // small tree: few rows per column, little contention
+      atomicAdd((u64 *)&s_u[fr], (u64)dus);
     }
   } else {
     for (int c = FR + tid; c < tb; c += nthreads) {
-      const int fr = col_of(c);
-      const i64 sub = s_sub[c];
-      const i64 lq = local_quota(sub, s_lq[c]);
-      if (sub - lq) atomicAdd((u64 *)&s_sub[fr], (u64)(sub - lq));
-      const i64 spill = imax(0, s_u[c] - lq);
-      if (spill) atomicAdd((u64 *)&s_u[fr], (u64)spill);
+      const i64 spill = imax(0, s_u[c] - s_lq[c]);
+      if (spill) atomicAdd((u64 *)&s_u[col_of(c)], (u64)spill);
     }
   }
-  KB_PP(1, 4);
+  // the root's lendable per resource (k_fair_prep): potentialAvailable of the root == its SubtreeQuota, static
+  if (fair)
+    for (int r = tid; r < R; r += nthreads) {
+      i64 lend = 0;
+      for (int c = r; c < FR; c += R) lend += s_sub[c];
+      s_lend[r] = lend;
+    }
   __syncthreads();
   KB_FPHASE(1);
-  KB_PP(1, 5);
   const int n = s_misc[0], nrows = s_misc[1];
   if (n == 0) {
     for (int i = tid; i < tb; i += nthreads) D.usage[(size_t)b_gid[row_of(i)] * FR + col_of(i)] = s_u[i];
     return;
   }
-  // ---- 2. per-cycle records of the entries (one hop: the workload / row ids are known), then localQuota and
-  // available / potentialAvailable (resource_node.go:104-133) for every cell in one sweep: the root's cells are final
-  for (int i = tid; i < n; i += nthreads) {
-    // all loads of a record are issued before its first store (read-only path: the compiler may hoist them freely)
-    const int wl = e_wl[i];
-    const int ps0 = e_ps0[i], l0 = e_psn[i], np = e_psn[i + 1] - l0;
-    const int pr = __ldg(D.wl_priority + wl); const i64 ts = __ldg(D.wl_ts + wl), lg = __ldg(D.wl_last_gen + wl);
-    const uint8_t qr = D.wl_has_qr ? __ldg(D.wl_has_qr + wl) : 0;
-    bool fast = np == 1;  // see phase 5
-    for (int k = 0; k < np; k++) {
-      const int row = ps0 + k, l = l0 + k;
-      const int cnt = __ldg(D.ps_count + row), mn = __ldg(D.ps_min_count + row); const uint32_t msk = __ldg(D.ps_req_mask + row);
-      const int grp = D.ps_group ? __ldg(D.ps_group + row) : -1; const u64 ok = __ldg(D.ps_flavor_ok + row);
-      for (int r0 = 0; r0 < R; r0 += 4) {
-        i64 q[4]; int8_t lt[4];
-#pragma unroll
-        for (int j = 0; j < 4; j++) if (r0 + j < R) { q[j] = __ldg(D.ps_req + (size_t)row * R + r0 + j); lt[j] = __ldg(D.ps_last_tried + (size_t)row * R + r0 + j); }
-#pragma unroll
-        for (int j = 0; j < 4; j++) if (r0 + j < R) { r_req[(size_t)l * R + r0 + j] = q[j]; r_last[(size_t)l * R + r0 + j] = lt[j]; }
-      }
-      r_gid[l] = row; r_count[l] = cnt; r_min[l] = mn; r_mask[l] = msk; r_group[l] = grp; r_ok[l] = ok;
-      if ((D.flags & KB_F_PARTIAL_ADMISSION) && mn >= 0 && cnt > mn) fast = false;
-    }
-    e_prio[i] = pr; e_ts[i] = ts; e_lg[i] = lg; e_qr[i] = qr; e_fast[i] = fast;
-  }
-  KB_PP(1, 6);
-  // fair sharing inputs (k_fair_prep): over-usage per (ClusterQueue, resource), lendable per (node, resource).  When a
-  // row is one aligned segment of a warp they are summed over the flavors by shuffles in this sweep (phase 4 otherwise)
-  const bool fair = (D.flags & KB_F_FAIR_SHARING) != 0;  // every tree is flat here: all entries take the fair flat key
-  const bool fair_rows = fair && FR <= 32 && fr_p2 && (R & (R - 1)) == 0;
-  const int tb_sweep = fair_rows ? (tb + 31) & ~31 : tb;
-  for (int i = tid; i < tb_sweep; i += nthreads) {
-    i64 pot = 0, over = 0;
-    if (i < tb) {
-      const int fr = col_of(i);
-      const i64 sub = s_sub[i], u = s_u[i];
-      const i64 lq = local_quota(sub, s_lq[i]);
-      s_lq[i] = lq;
-      if (i < FR) { s_av[i] = sub - u; pot = sub; }
-      else {
-        const i64 bl = s_bl[i];
-        i64 pa = s_sub[fr] - s_u[fr];
-        pot = lq + s_sub[fr];
-        if (bl != KB_NO_LIMIT) { pa = imin((sub - lq) - imax(0, u - lq) + bl, pa); pot = imin(sub + bl, pot); }
-        s_av[i] = imax(0, lq - u) + pa;
-      }
-      s_pot[i] = pot;
-      over = imax(0, u - sub);
-    }
-    if (fair_rows) {
-      i64 lend = pot;
-      for (int o = R; o < FR; o <<= 1) { lend += __shfl_xor_sync(0xffffffffu, lend, o); over += __shfl_xor_sync(0xffffffffu, over, o); }
-      if (i < tb && col_of(i) < R) { const int h = row_of(i); s_lend[h * R + col_of(i)] = lend; s_over[h * R + col_of(i)] = over; }
-    }
-  }
-  KB_PP(1, 7);
-  {
-    const int walked = __syncthreads_count(tid < n && e_fast[tid]);  // e_fast of entry tid was written by this thread
-    if (blockIdx.x == 0 && tid == 0) { D.sstat[8] = (u64)walked; D.sstat[9] = (u64)min(n, nthreads); }  // CTA 0: group walk / entries, of the first nthreads
-  }
-  KB_FPHASE(2);
-  KB_PP(2, 0);
   const DevSnap &L = *(const DevSnap *)(smem_raw + Y.snap);
-  // ---- 4. fair sharing inputs of rows that do not fit a warp segment
-  if (fair && !fair_rows) {
-    const int Fn = D.F;
-    for (int i = tid; i < nn * R; i += nthreads) {
-      const int h = i / R, r = i % R;
-      i64 over = 0, lend = 0;
-      for (int f = 0; f < Fn; f++) {
-        const int c = h * FR + f * R + r;
-        lend += s_pot[c];
-        const i64 o = s_u[c] - s_sub[c];
-        if (o > 0) over += o;
+  // ---- 2. for the general walk only: available / potentialAvailable (resource_node.go:104-133) of every cell in one
+  // sweep, with the fair-sharing inputs (k_fair_prep: over-usage per (ClusterQueue, resource), lendable per (node,
+  // resource)) summed by shuffles when a row is one aligned segment of a warp, in a pass of their own otherwise
+  if (sweep) {
+    const bool fair_rows = fair && FR <= 32 && fr_p2 && (R & (R - 1)) == 0;
+    const int tb_sweep = fair_rows ? (tb + 31) & ~31 : tb;
+    for (int i = tid; i < tb_sweep; i += nthreads) {
+      i64 pot = 0, over = 0;
+      if (i < tb) {
+        const int fr = col_of(i);
+        const i64 sub = s_sub[i], u = s_u[i];
+        if (i < FR) { s_av[i] = sub - u; pot = sub; }
+        else { i64 av; flat_cell_available(sub, u, s_lq[i], s_bl[i], s_sub[fr], s_u[fr], av, pot); s_av[i] = av; }
+        s_pot[i] = pot;
+        over = imax(0, u - sub);
       }
-      s_lend[i] = lend; s_over[i] = over;
+      if (fair_rows) {
+        i64 lend = pot;
+        for (int o = R; o < FR; o <<= 1) { lend += __shfl_xor_sync(0xffffffffu, lend, o); over += __shfl_xor_sync(0xffffffffu, over, o); }
+        if (i < tb && col_of(i) < R) { const int h = row_of(i); s_lend[h * R + col_of(i)] = lend; s_over[h * R + col_of(i)] = over; }
+      }
     }
-    __syncthreads();  // the group walk below reads s_over / s_lend for the iterator key
+    __syncthreads();
+    if (fair && !fair_rows) {
+      const int Fn = D.F;
+      for (int i = tid; i < nn * R; i += nthreads) {
+        const int h = i / R, r = i % R;
+        i64 over = 0, lend = 0;
+        for (int f = 0; f < Fn; f++) {
+          const int c = h * FR + f * R + r;
+          lend += s_pot[c];
+          const i64 o = s_u[c] - s_sub[c];
+          if (o > 0) over += o;
+        }
+        s_lend[i] = lend; s_over[i] = over;
+      }
+      __syncthreads();
+    }
   }
-  KB_PP(2, 1);
-  // ---- 5. nominate (getInitialAssignments, scheduler.go:584-625): KB_FLAT_NG lanes per entry.  Entries with one
-  // podset that cannot be reduced take the group walk on the shared tables (flat_nominate_group); every other entry
-  // (several podsets, or partial admission with a reducible podset) takes get_assignments_coop on the relocated
-  // snapshot L.  A round evaluates KB_FLAT_NG flavors of a resource group at once; the walk usually stops in its first
-  // round, so fewer lanes per entry mean fewer warps competing for the SM's issue slots at the same chain length.
+  // ---- 3. one pass per entry, KB_FLAT_NG lanes each: per-cycle records (one hop: the workload / row ids are known),
+  // nominate (getInitialAssignments, scheduler.go:584-625), iterator key and dense request row (Assignment.Usage.Quota,
+  // absent = -1), with no barrier in between.  Entries with one podset that cannot be reduced take the group walk on
+  // the shared tables (flat_nominate_group); every other entry (several podsets, or partial admission with a reducible
+  // podset) takes get_assignments_coop on the relocated snapshot L.  A round evaluates KB_FLAT_NG flavors of a resource
+  // group at once; the walk usually stops in its first round, so fewer lanes per entry mean fewer warps competing for
+  // the SM's issue slots at the same chain length.
+  i64 *s_q = s_av;    // [n][FR]: written here when there is no sweep, after this pass otherwise (avail is live until then)
+  i64 *s_lim = s_pot; // [n][FR] thresholds in iterator order
+  int walked = 0;
   {
     const int glane = lane % KB_FLAT_NG, gbase = lane - glane;
     const unsigned gmask = (KB_FLAT_NG == 32 ? 0xffffffffu : ((1u << KB_FLAT_NG) - 1u)) << gbase;
     const int groups = nthreads / KB_FLAT_NG;
-    for (int i0 = 0; i0 < n; i0 += groups) {
+    bool fast_mine = false;  // lane k of a group reports the entry of its round k: every entry < nthreads once
+    for (int i0 = 0, k = 0; i0 < n; i0 += groups, k++) {
       const int i = i0 + tid / KB_FLAT_NG;
       if (i >= n) continue;  // whole lane groups take the branches together
-      if (e_fast[i] & 1) {
-        flat_nominate_group<KB_FLAT_NG>(Y, i, R, FR, D.flags, D.pods_res, D.wl_has_qr != nullptr, gmask, gbase, glane);
+      const int wl = e_wl[i];
+      const int ps0 = e_ps0[i], l0 = e_psn[i], np = e_psn[i + 1] - l0;
+      for (int kk = glane; kk < np; kk += KB_FLAT_NG) {  // podset rows over the lanes; all loads of a row before its stores
+        const int row = ps0 + kk, l = l0 + kk;
+        const int cnt = __ldg(D.ps_count + row), mn = __ldg(D.ps_min_count + row); const uint32_t msk = __ldg(D.ps_req_mask + row);
+        const int grp = D.ps_group ? __ldg(D.ps_group + row) : -1; const u64 ok = __ldg(D.ps_flavor_ok + row);
+        for (int rr = 0; rr < R; rr += 4) {
+          i64 q[4]; int8_t lt[4];
+#pragma unroll
+          for (int j = 0; j < 4; j++) if (rr + j < R) { q[j] = __ldg(D.ps_req + (size_t)row * R + rr + j); lt[j] = __ldg(D.ps_last_tried + (size_t)row * R + rr + j); }
+#pragma unroll
+          for (int j = 0; j < 4; j++) if (rr + j < R) { r_req[(size_t)l * R + rr + j] = q[j]; r_last[(size_t)l * R + rr + j] = lt[j]; }
+        }
+        r_gid[l] = row; r_count[l] = cnt; r_min[l] = mn; r_mask[l] = msk; r_group[l] = grp; r_ok[l] = ok;
+      }
+      if (glane == 0) {
+        const int pr = __ldg(D.wl_priority + wl); const i64 ts = __ldg(D.wl_ts + wl), lg = __ldg(D.wl_last_gen + wl);
+        const uint8_t qr = D.wl_has_qr ? __ldg(D.wl_has_qr + wl) : 0;
+        e_prio[i] = pr; e_ts[i] = ts; e_lg[i] = lg; e_qr[i] = qr;
+      }
+      const bool fast = e_fast[i] & 1;
+      __syncwarp(gmask);  // the records are read by every lane of the group
+      if (fast) {
+        flat_nominate_group<KB_FLAT_NG>(Y, i, R, FR, D.flags, D.pods_res, D.wl_has_qr != nullptr, gmask, gbase, glane,
+                                        sweep ? nullptr : s_q + (size_t)i * FR);
       } else {
         int borrowing;
         const int mode = flat_nominate_general(L, i, &borrowing, gmask, gbase, glane);
         if (glane == 0) { e_mode[i] = mode; e_borrow[i] = borrowing; }
+        __syncwarp(gmask);  // the assignment rows were written by all lanes of the group
+        if (glane == 0) flat_key_general(L, i, s_key + (size_t)i * 4);
       }
+      if (glane == k) fast_mine = fast;
     }
+    walked = __syncthreads_count(fast_mine);
   }
-  KB_PP(2, 2);
-  __syncthreads();
-  KB_FPHASE(3);
-  KB_PP(2, 3);
-  // ---- 6. dense request rows (Assignment.Usage.Quota per entry, absent = -1) and, for the entries of the general
-  // walk, iterator keys; avail / potential are dead from here on
-  i64 *s_q = s_av;    // [n][FR]
-  i64 *s_lim = s_pot; // [n][FR] thresholds in iterator order
-  {
+  if (blockIdx.x == 0 && tid == 0) { D.sstat[8] = (u64)walked; D.sstat[9] = (u64)min(n, nthreads); }  // CTA 0: group walk / entries, of the first nthreads
+  if (sweep) {  // request rows, now that avail is dead
     const bool r_p2 = (R & (R - 1)) == 0;
     const int r_sh = 31 - __clz(R);
     for (int c = tid; c < n * FR; c += nthreads) {  // the group walk's entries, cell-parallel (one podset: the row is its request)
@@ -681,22 +684,13 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
       if (o_fl[(size_t)l * R + r] == f) q = (fb & 2) && r == D.pods_res ? (i64)o_cnt[l] : r_req[(size_t)l * R + r];
       s_q[c] = q;
     }
+    for (int i = tid; i < n; i += nthreads)
+      if (!(e_fast[i] & 1)) flat_expand_general(L, i, s_q + (size_t)i * FR, FR);
+    __syncthreads();
   }
-  KB_PP(2, 4);
-  {
-    const int half = nthreads / 2;
-    for (int i = tid < half ? tid : tid - half; i < n; i += half) {
-      if (e_fast[i] & 1) continue;
-      if (tid < half) flat_key_general(L, i, s_key + (size_t)i * 4);
-      else flat_expand_general(L, i, s_q + (size_t)i * FR, FR);
-    }
-  }
-  KB_PP(2, 5);
-  KB_PP(2, 6);
-  __syncthreads();
-  KB_FPHASE(4);
-  KB_PP(2, 7); KB_PP(3, 0);
-  // ---- 7. position in the iterator order: S lanes share the comparisons of one entry
+  KB_FPHASE(2);
+  // ---- 4. position in the iterator order: S lanes share the comparisons of one entry, then write its thresholds
+  // (see flat_ordered_loop) at that position
   {
     int S = 32;
     while (S > 1 && n * S > nthreads) S >>= 1;
@@ -710,77 +704,67 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
         for (int j = sub; j < n; j += S) cnt += key4_less(s_key + (size_t)j * 4, mine) ? 1 : 0;
       }
       for (int o = S >> 1; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-      if (act && sub == 0) { s_sorted[cnt] = i; e_rank[i] = cnt; }
+      if (!act) continue;
+      const int mode = e_mode[i], hq = e_cq[i];
+      if (sub == 0) { e_rank[i] = cnt; m_sorted[cnt] = mode; }
+      for (int fr = sub; fr < FR; fr += S) {
+        const i64 q = s_q[(size_t)i * FR + fr];
+        const int r = hq * FR + fr;
+        const i64 u = s_u[r], l = s_lq[r], bl = s_bl[r], sb = s_sub[r];
+        const i64 A = imax(0, l - u);
+        i64 v = INT64_MAX;  // Fit: threshold on the root usage; Preempt: SubtreeQuota_root - amount added to the root
+        if (mode == KB_MODE_FIT) {
+          if (q > 0) {
+            const i64 x = q - A;
+            const bool cap_ok = bl == KB_NO_LIMIT || (sb - l) - imax(0, u - l) + bl >= x;
+            v = cap_ok ? s_sub[fr] - x : INT64_MIN;
+          }
+        } else if (mode == KB_MODE_PREEMPT) {
+          i64 amt = 0;
+          if (q >= 0 && b_reclaim[hq] != KB_POLICY_ANY) {  // quotaResourcesToReserve scheduler.go:530-548
+            const i64 rsv = e_borrow[i] > 0 ? (bl == KB_NO_LIMIT ? q : imin(q, sb + bl - u)) : imax(0, imin(q, sb - u));
+            amt = rsv > A ? rsv - A : 0;
+          }
+          v = s_sub[fr] - amt;
+        }
+        s_lim[(size_t)cnt * FR + fr] = v;
+      }
     }
   }
-  KB_PP(3, 1);
   __syncthreads();
-  // ---- 8. thresholds, stored in iterator order (see flat_ordered_loop)
-  for (int c = tid; c < n * FR; c += nthreads) {
-    const int pos = row_of(c), fr = col_of(c);
-    const int i = s_sorted[pos];
-    const i64 q = s_q[(size_t)i * FR + fr];
-    const int hq = e_cq[i];
-    const int r = hq * FR + fr;
-    const i64 u = s_u[r], l = s_lq[r], bl = s_bl[r], sub = s_sub[r];
-    const i64 A = imax(0, l - u);
-    i64 v = INT64_MAX;  // Fit: threshold on the root usage; Preempt: SubtreeQuota_root - amount added to the root
-    const int mode = e_mode[i];
-    if (mode == KB_MODE_FIT) {
-      if (q > 0) {
-        const i64 x = q - A;
-        const bool cap_ok = bl == KB_NO_LIMIT || (sub - l) - imax(0, u - l) + bl >= x;
-        v = cap_ok ? s_sub[fr] - x : INT64_MIN;
-      }
-    } else if (mode == KB_MODE_PREEMPT) {
-      i64 amt = 0;
-      if (q >= 0 && b_reclaim[hq] != KB_POLICY_ANY) {  // quotaResourcesToReserve scheduler.go:530-548
-        const i64 rsv = e_borrow[i] > 0 ? (bl == KB_NO_LIMIT ? q : imin(q, sub + bl - u)) : imax(0, imin(q, sub - u));
-        amt = rsv > A ? rsv - A : 0;
-      }
-      v = s_sub[fr] - amt;
-    }
-    s_lim[c] = v;
-    if (fr == 0) m_sorted[pos] = mode;
-  }
-  KB_PP(3, 2);
-  __syncthreads();
-  KB_FPHASE(5);
-  // ---- 9. the ordered loop
+  KB_FPHASE(3);
+  // ---- 5. the ordered loop
   if (warp == 0) {
     if (FR > 32) flat_ordered_loop<true>(n, FR, lane, s_lim, m_sorted, ok_bits, s_u, s_sub);
     else flat_ordered_loop<false>(n, FR, lane, s_lim, m_sorted, ok_bits, s_u, s_sub);
   }
   __syncthreads();
-  KB_FPHASE(6);
-  KB_PP(3, 3);
-  // ---- 10. ClusterQueue rows of the admitted / reserving entries (cq.AddUsage)
-  for (int c = tid; c < n * FR; c += nthreads) {
-    const int i = row_of(c), fr = col_of(c);
-    const int dec = flat_decision(e_mode[i], ok_bits, e_rank[i]);
-    const i64 q = s_q[c];
-    const int hq = e_cq[i];
-    const int r = hq * FR + fr;
-    if (dec == KB_DEC_ASSUMED) { if (q > 0) s_u[r] += q; }
-    else if (dec == KB_DEC_PREEMPT_NO_TARGETS && q >= 0 && b_reclaim[hq] != KB_POLICY_ANY) {
-      const i64 u = s_u[r], bl = s_bl[r], sub = s_sub[r];
-      s_u[r] = u + (e_borrow[i] > 0 ? (bl == KB_NO_LIMIT ? q : imin(q, sub + bl - u)) : imax(0, imin(q, sub - u)));
+  KB_FPHASE(4);
+  // ---- 6. publish: usage table with the ClusterQueue rows of the admitted / reserving entries (cq.AddUsage) applied
+  // on the way out, decisions, flavor assignment rows
+  auto final_usage = [&](int c) {
+    const int h = row_of(c), i = n_e[h];
+    i64 u = s_u[c];
+    if (i >= 0) {
+      const int dec = flat_decision(e_mode[i], ok_bits, e_rank[i]);
+      const i64 q = s_q[(size_t)i * FR + col_of(c)];
+      if (dec == KB_DEC_ASSUMED) { if (q > 0) u += q; }
+      else if (dec == KB_DEC_PREEMPT_NO_TARGETS && q >= 0 && b_reclaim[h] != KB_POLICY_ANY) {
+        const i64 bl = s_bl[c], sb = s_sub[c];
+        u = u + (e_borrow[i] > 0 ? (bl == KB_NO_LIMIT ? q : imin(q, sb + bl - u)) : imax(0, imin(q, sb - u)));
+      }
     }
-  }
-  KB_PP(3, 4);
-  __syncthreads();
-  // ---- 11. publish: usage table, decisions, flavor assignment rows
-  KB_PP(3, 5);
+    return u;
+  };
   if ((FR & 1) == 0) {
     const int half = tb >> 1;
     for (int c = tid; c < half; c += nthreads) {
       const int i = c << 1;
-      *(longlong2 *)(D.usage + (size_t)b_gid[row_of(i)] * FR + col_of(i)) = *(const longlong2 *)(s_u + i);
+      *(longlong2 *)(D.usage + (size_t)b_gid[row_of(i)] * FR + col_of(i)) = make_longlong2(final_usage(i), final_usage(i + 1));
     }
   } else {
-    for (int i = tid; i < tb; i += nthreads) D.usage[(size_t)b_gid[row_of(i)] * FR + col_of(i)] = s_u[i];
+    for (int i = tid; i < tb; i += nthreads) D.usage[(size_t)b_gid[row_of(i)] * FR + col_of(i)] = final_usage(i);
   }
-  KB_PP(3, 6);
   for (int i = tid; i < n; i += nthreads) {
     const int e = e_gid[i];
     D.mode[e] = (uint8_t)e_mode[i]; D.borrow[e] = e_borrow[i]; D.decision[e] = (uint8_t)flat_decision(e_mode[i], ok_bits, e_rank[i]); D.rank[e] = e_rank[i];
@@ -807,7 +791,6 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
       }
     }
   }
-  KB_PP(3, 7);
-  KB_FPHASE(7);
+  KB_FPHASE(5);
 #undef KB_FPHASE
 }
