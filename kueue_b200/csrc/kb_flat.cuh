@@ -9,16 +9,17 @@
 // expansion are the SAME device functions every other kernel uses (assign_workload_coop, compute_entry_key,
 // expand_entry): they run on a DevSnap whose table pointers all point into that relocated copy (tab_local == 2), so
 // their chains of dependent loads (head -> workload -> podset rows -> resource group -> flavors -> quota cells) cost
-// shared-memory latency instead of an L2 / HBM round trip per hop.  Global memory is touched in two bursts: the
-// staging at the start (every load independent, at most three dependent hops: tree_start -> node / head record ->
-// rows) and the publication of usage + decisions at the end.
+// shared-memory latency instead of an L2 / HBM round trip per hop.  Global memory is touched in two bursts, each
+// overlapped with compute: the staging at the start (every load independent, at most three dependent hops:
+// tree_start -> node / head record -> rows; the tables read late land while phase 1 runs, the entries' records while
+// the tree pass runs) and the publication of usage + decisions, which runs on the other warps behind the ordered loop.
 //
 // Used when k_cycle_root's conditions hold and, in addition, every tree is flat, FR <= 64 and the relocated copy fits
 // shared memory (host: flat_layout).  Reference semantics are cited at the shared device functions.
 #pragma once
 
 struct FlatLay {  // byte offsets into the dynamic shared memory of k_cycle_flat (computed on the host, passed by value)
-  uint32_t u, sub, lq, bl, av, pot, over, lend, blob, n_e, n_wl, n_ps0, n_psn, e_gid, e_cq, e_prio, e_ident, e_psn, e_wl, e_ps0, e_ts, e_lg, e_qr,
+  uint32_t u, sub, lq, bl, av, pot, over, lend, blob, n_e, n_wl, n_ps0, n_psn, e_gid, e_cq, e_prio, e_ident, e_psn, e_at, blk_bar, e_ts, e_lg, e_qr,
       e_fast, e_mode, e_borrow, e_rank, m_sorted, d_sorted, r_gid, r_count, r_min, r_mask, r_group, r_ok, r_req, r_last, o_fl, o_md, o_tr, o_cnt, key, misc, snap, rec, total;
 };
 __host__ __device__ inline FlatLay flat_layout(int ncap, int FR, int R, int rcap, int bcap) {
@@ -31,7 +32,7 @@ __host__ __device__ inline FlatLay flat_layout(int ncap, int FR, int R, int rcap
   L.blob = take((size_t)bcap);
   L.n_e = take((size_t)ncap * 4); L.n_wl = take((size_t)ncap * 4); L.n_ps0 = take((size_t)ncap * 4); L.n_psn = take((size_t)ncap * 4);
   L.e_gid = take((size_t)ncap * 4); L.e_cq = take((size_t)ncap * 4); L.e_prio = take((size_t)ncap * 4); L.e_ident = take((size_t)ncap * 4);
-  L.e_psn = take((size_t)(ncap + 1) * 4); L.e_wl = take((size_t)ncap * 4); L.e_ps0 = take((size_t)ncap * 4);
+  L.e_psn = take((size_t)(ncap + 1) * 4); L.e_at = take((size_t)ncap * 4); L.blk_bar = take(((size_t)ncap / 32 + 2) * 8);
   L.e_ts = take((size_t)ncap * 8); L.e_lg = take((size_t)ncap * 8); L.e_qr = take((size_t)ncap);
   L.e_fast = take((size_t)ncap);
   L.e_mode = take((size_t)ncap * 4); L.e_borrow = take((size_t)ncap * 4); L.e_rank = take((size_t)ncap * 4);
@@ -124,6 +125,15 @@ __device__ __forceinline__ void cp_async16(void *smem_dst, const void *gsrc) {
   unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gsrc) : "memory");
 }
+// 4- and 8-byte copies (naturally aligned on both sides)
+template <int B>
+__device__ __forceinline__ void cp_async_small(void *smem_dst, const void *gsrc) {
+  static_assert(B == 4 || B == 8, "cp.async.ca copies 4, 8 or 16 bytes");
+  unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
+  asm volatile("cp.async.ca.shared.global [%0], [%1], %2;" ::"r"(d), "l"(gsrc), "n"(B) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_prior1() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
 // 1-D bulk copies (the TMA engine, no tensor map) completing on an mbarrier
 __device__ __forceinline__ void mbar_init(unsigned long long *bar, unsigned count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n\tfence.mbarrier_init.release.cluster;" ::"r"((unsigned)__cvta_generic_to_shared(bar)), "r"(count) : "memory");
@@ -141,6 +151,14 @@ __device__ __forceinline__ bool mbar_try_wait(unsigned long long *bar, unsigned 
                : "=r"(ok) : "r"((unsigned)__cvta_generic_to_shared(bar)), "r"(parity) : "memory");
   return ok != 0;
 }
+// waits (suspended in try_wait, acquire at CTA scope) until the barrier's phase of the given parity has completed
+__device__ __forceinline__ void mbar_wait(unsigned long long *bar, unsigned parity) {
+  unsigned spins = 0;
+  while (!mbar_try_wait(bar, parity)) if (++spins > (1u << 24)) __trap();  // a lost copy or signal must not hang the device
+}
+__device__ __forceinline__ void mbar_arrive(unsigned long long *bar) {  // release at CTA scope
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"((unsigned)__cvta_generic_to_shared(bar)) : "memory");
+}
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory"); }
 
 // ordered admit loop over the entries in iterator order (scheduler.go:269-401) on one threshold per (position, column):
@@ -150,9 +168,11 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.com
 //              so the amount added has the same form as for Fit
 // One warp; lane = column (and column + 32 when kTwo).  Per entry the dependent chain is compare -> vote -> add; the
 // thresholds of the next four positions are in flight while the current four are decided.  Results: one bit per
-// position (the vote) in ok_bits; the decision follows from the bit and the entry's mode.
+// position (the vote) in ok_bits; the decision follows from the bit and the entry's mode.  Block b of 32 positions is
+// signalled on blk_bar[b] as soon as its word is written, so the decisions can be published behind the loop.
 template <bool kTwo>
-__device__ inline void flat_ordered_loop(int n, int FR, int lane, const i64 *s_lim, const int *m_sorted, uint32_t *ok_bits, i64 *s_u, const i64 *s_sub) {
+__device__ inline void flat_ordered_loop(int n, int FR, int lane, const i64 *s_lim, const int *m_sorted, uint32_t *ok_bits,
+                                         unsigned long long *blk_bar, i64 *s_u, const i64 *s_sub) {
   const int fr0 = lane, fr1 = lane + 32;
   const bool c0 = fr0 < FR, c1 = kTwo && fr1 < FR;
   i64 urt0 = c0 ? s_u[fr0] : 0, urt1 = c1 ? s_u[fr1] : 0;
@@ -193,7 +213,7 @@ __device__ inline void flat_ordered_loop(int n, int FR, int lane, const i64 *s_l
       fetch(a0, a1, blk + p + 8);
       decide(b0, b1, p + 4);
     }
-    if (lane == 0) ok_bits[blk >> 5] = okb;
+    if (lane == 0) { ok_bits[blk >> 5] = okb; mbar_arrive(blk_bar + (blk >> 5)); }
   }
   if (c0) s_u[fr0] = urt0;
   if (c1) s_u[fr1] = urt1;
@@ -401,7 +421,8 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
   unsigned char *s_blob = smem_raw + Y.blob;
   int *n_e = (int *)(smem_raw + Y.n_e), *n_wl = (int *)(smem_raw + Y.n_wl), *n_ps0 = (int *)(smem_raw + Y.n_ps0), *n_psn = (int *)(smem_raw + Y.n_psn);
   int *e_gid = (int *)(smem_raw + Y.e_gid), *e_cq = (int *)(smem_raw + Y.e_cq), *e_prio = (int *)(smem_raw + Y.e_prio), *e_ident = (int *)(smem_raw + Y.e_ident);
-  int *e_psn = (int *)(smem_raw + Y.e_psn), *e_wl = (int *)(smem_raw + Y.e_wl), *e_ps0 = (int *)(smem_raw + Y.e_ps0);
+  int *e_psn = (int *)(smem_raw + Y.e_psn), *e_at = (int *)(smem_raw + Y.e_at);  // e_at: the entry at each iterator position
+  unsigned long long *blk_bar = (unsigned long long *)(smem_raw + Y.blk_bar);    // one per 32 positions (flat_ordered_loop)
   i64 *e_ts = (i64 *)(smem_raw + Y.e_ts), *e_lg = (i64 *)(smem_raw + Y.e_lg); uint8_t *e_qr = smem_raw + Y.e_qr;
   uint8_t *e_fast = smem_raw + Y.e_fast;  // bit 0: nominated by the group walk, bit 1: its ClusterQueue covers the pods resource
   int *e_mode = (int *)(smem_raw + Y.e_mode), *e_borrow = (int *)(smem_raw + Y.e_borrow), *e_rank = (int *)(smem_raw + Y.e_rank);
@@ -419,40 +440,42 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
   const int tb = nn * FR;
   const size_t r0 = (size_t)ts0 * FR;  // first cell of the tree in the tree-local tables (DevSnap::tl_*)
   int4 *s_rec = (int4 *)(smem_raw + Y.rec);
-  __shared__ __align__(8) unsigned long long s_mbar;
-  // A root's rows are contiguous in the tree-local tables -> one bulk copy per table, issued by one thread, completion
-  // counted in bytes on an mbarrier.  Rows of odd width are not 16 B aligned: per-thread loads.
+  __shared__ __align__(8) unsigned long long s_mbar[2];
+  // Two stages, both requested here.  Stage A is what the entry compaction and the tree pass of phase 1 read: head
+  // records, usage, localQuota.  Stage B is read from the end of phase 1 on: SubtreeQuota, borrowing limits and the
+  // static tree block; it lands while phase 1 runs.  A root's rows are contiguous in the tree-local tables -> one bulk
+  // copy per table, issued by one thread, completion counted in bytes on the stage's mbarrier.  Rows of odd width are
+  // not 16 B aligned: per-thread cp.async, one commit group per stage.
   // SubtreeQuota and localQuota arrive final (k_tl_static / k_tl_root): the tree pass below only sums usage.
   if ((FR & 1) == 0) {
-    if (tid == 0) mbar_init(&s_mbar, 1);
+    if (tid == 0) { mbar_init(&s_mbar[0], 1); mbar_init(&s_mbar[1], 1); }
     __syncthreads();
     if (tid == 0) {
       const int b0 = D.tree_blob_off[t], bn = D.tree_blob_off[t + 1] - b0;  // static block of the tree (multiple of 16 B)
       const unsigned tbytes = (unsigned)tb * 8u;
-      mbar_expect_tx(&s_mbar, 4u * tbytes + (unsigned)bn + (unsigned)nn * 16u);
-      bulk_g2s(s_sub, D.tl_subtree + r0, tbytes, &s_mbar);
-      bulk_g2s(s_bl, D.tl_blimit + r0, tbytes, &s_mbar);
-      bulk_g2s(s_lq, D.tl_lquota + r0, tbytes, &s_mbar);
-      bulk_g2s(s_u, D.tl_usage + r0, tbytes, &s_mbar);      // ClusterQueue usage, zero rows for cohorts
-      bulk_g2s(s_blob, D.tree_blob + b0, (unsigned)bn, &s_mbar);
-      bulk_g2s(s_rec, D.cq_rec + ts0, (unsigned)nn * 16u, &s_mbar);
+      mbar_expect_tx(&s_mbar[0], 2u * tbytes + (unsigned)nn * 16u);
+      bulk_g2s(s_rec, D.cq_rec + ts0, (unsigned)nn * 16u, &s_mbar[0]);
+      bulk_g2s(s_u, D.tl_usage + r0, tbytes, &s_mbar[0]);      // ClusterQueue usage, zero rows for cohorts
+      bulk_g2s(s_lq, D.tl_lquota + r0, tbytes, &s_mbar[0]);
+      mbar_expect_tx(&s_mbar[1], 2u * tbytes + (unsigned)bn);
+      bulk_g2s(s_sub, D.tl_subtree + r0, tbytes, &s_mbar[1]);
+      bulk_g2s(s_bl, D.tl_blimit + r0, tbytes, &s_mbar[1]);
+      bulk_g2s(s_blob, D.tree_blob + b0, (unsigned)bn, &s_mbar[1]);
     }
     if (tid == nthreads - 1) *(DevSnap *)(smem_raw + Y.snap) = D;  // bulk of the relocated view (patched below), under the load latency
-    {
-      unsigned spins = 0;
-      while (!mbar_try_wait(&s_mbar, 0)) if (++spins > (1u << 24)) __trap();  // a lost copy must not hang the device
-    }
+    mbar_wait(&s_mbar[0], 0);
   } else {
+    for (int h = tid; h < nn; h += nthreads) cp_async16(s_rec + h, D.cq_rec + ts0 + h);
+    for (int i = tid; i < tb; i += nthreads) { cp_async_small<8>(s_u + i, D.tl_usage + r0 + i); cp_async_small<8>(s_lq + i, D.tl_lquota + r0 + i); }
+    cp_async_commit();
     {
       const int b0 = D.tree_blob_off[t], bn = D.tree_blob_off[t + 1] - b0;  // static block of the tree (multiple of 16 B)
       for (int c = tid * 16; c < bn; c += nthreads * 16) cp_async16(s_blob + c, D.tree_blob + b0 + c);
     }
-    for (int i = tid; i < tb; i += nthreads) {
-      s_sub[i] = D.tl_subtree[r0 + i]; s_bl[i] = D.tl_blimit[r0 + i]; s_lq[i] = D.tl_lquota[r0 + i]; s_u[i] = D.tl_usage[r0 + i];
-    }
-    for (int h = tid; h < nn; h += nthreads) s_rec[h] = D.cq_rec[ts0 + h];
+    for (int i = tid; i < tb; i += nthreads) { cp_async_small<8>(s_sub + i, D.tl_subtree + r0 + i); cp_async_small<8>(s_bl + i, D.tl_blimit + r0 + i); }
+    cp_async_commit();
     if (tid == nthreads - 1) *(DevSnap *)(smem_raw + Y.snap) = D;
-    cp_async_wait_all();
+    cp_async_wait_prior1();  // stage A
     __syncthreads();
   }
   bool general_mine = false;  // a head of the general walk (see phase 2)
@@ -460,7 +483,7 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
     const int4 rc = s_rec[h];
     const bool live = ((unsigned)rc.w >> 16) == D.rec_stamp;  // written for this cycle
     n_e[h] = live ? rc.x : -1; n_wl[h] = rc.y; n_ps0[h] = rc.z; n_psn[h] = live ? (rc.w & (KB_REC_GENERAL - 1)) : 0;
-    if (live) {  // the entry's per-cycle records are gathered in phase 2: request their lines now
+    if (live) {  // the entry's per-cycle records are copied in phase 1: request their lines now
       auto touch = [](const void *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); };
       const int wl = rc.y, row = rc.z;
       touch(D.wl_priority + wl); touch(D.wl_ts + wl); touch(D.wl_last_gen + wl);
@@ -477,15 +500,16 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
   // phase 2 runs only for a root with a head of the general walk.
   const bool sweep = __syncthreads_or(general_mine);
   KB_FPHASE(0);
-  const TreeBlobHdr *BH = (const TreeBlobHdr *)s_blob;
-  const int32_t *b_gid = (const int32_t *)(s_blob + BH->gid), *b_par = (const int32_t *)(s_blob + BH->par), *b_hgt = (const int32_t *)(s_blob + BH->hgt);
-  const uint8_t *b_reclaim = s_blob + BH->reclaim;
   const bool fair = (D.flags & KB_F_FAIR_SHARING) != 0;  // every tree is flat here: all entries take the fair flat key
 
   // ---- 1. entries of the root in ClusterQueue (= local handle) order + local podset-row numbering, and the
   // bottom-up pass of the flat tree for everyone: accumulateFromChild resource_node.go:210-217, children -> root
-  // one warp per 32 nodes: ballot + warp scan, then the warps' totals are scanned (chunks of 32 warps, carried)
+  // one warp per 32 nodes: ballot + warp scan, then the warps' totals are scanned (chunks of 32 warps, carried).
+  // The thread that places an entry copies its per-cycle records (one hop: the workload / row ids are in the head
+  // record) with cp.async; they land while the tree pass runs and are waited for at the end of the phase.
   {
+    // ps_last_tried rows by words when they are word aligned on both sides, byte by byte otherwise
+    const bool lt_words = (R & 3) == 0 && ((uintptr_t)D.ps_last_tried & 3) == 0;
     const int nw = nthreads >> 5;
     int *w_cnt = s_misc + 4, *w_rows = s_misc + 4 + 32;  // [32] each (misc is 64 + 256 B)
     int cnt_base = 0, rows_base = 0;
@@ -507,35 +531,28 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
         tc = __shfl_sync(0xffffffffu, ic, 31); tr = __shfl_sync(0xffffffffu, ir, 31);
       }
       if (e >= 0) {
-        const int i = cnt_base + pc + __popc(m & ((1u << lane) - 1));
-        e_gid[i] = e; e_cq[i] = h; e_ident[i] = i; e_wl[i] = n_wl[h]; e_ps0[i] = n_ps0[h]; e_psn[i] = rows_base + pr + incl - pn;
+        const int i = cnt_base + pc + __popc(m & ((1u << lane) - 1)), l0 = rows_base + pr + incl - pn;
+        const int wl = n_wl[h], ps0 = n_ps0[h];
+        e_gid[i] = e; e_cq[i] = h; e_ident[i] = i; e_psn[i] = l0;
         e_fast[i] = (s_rec[h].w & KB_REC_GENERAL) ? 0 : 1;
         n_e[h] = i;  // from here on: the local entry of the ClusterQueue (publish)
+        cp_async_small<4>(e_prio + i, D.wl_priority + wl); cp_async_small<8>(e_ts + i, D.wl_ts + wl); cp_async_small<8>(e_lg + i, D.wl_last_gen + wl);
+        if (D.wl_has_qr) e_qr[i] = D.wl_has_qr[wl];
+        for (int k = 0; k < pn; k++) {  // every podset row of the entry, for either walk
+          const int row = ps0 + k, l = l0 + k;
+          r_gid[l] = row;
+          cp_async_small<4>(r_count + l, D.ps_count + row); cp_async_small<4>(r_min + l, D.ps_min_count + row);
+          cp_async_small<4>(r_mask + l, D.ps_req_mask + row); cp_async_small<8>(r_ok + l, D.ps_flavor_ok + row);
+          if (D.ps_group) cp_async_small<4>(r_group + l, D.ps_group + row); else r_group[l] = -1;
+          for (int r = 0; r < R; r++) cp_async_small<8>(r_req + (size_t)l * R + r, D.ps_req + (size_t)row * R + r);
+          if (lt_words) for (int r = 0; r < R; r += 4) cp_async_small<4>(r_last + (size_t)l * R + r, D.ps_last_tried + (size_t)row * R + r);
+          else for (int r = 0; r < R; r++) r_last[(size_t)l * R + r] = D.ps_last_tried[(size_t)row * R + r];
+        }
       }
       cnt_base += tc; rows_base += tr;
       if (c0 + nthreads < nn) __syncthreads();  // w_cnt / w_rows are rewritten by the next chunk
     }
     if (tid == 0) { e_psn[cnt_base] = rows_base; s_misc[0] = cnt_base; s_misc[1] = rows_base; }
-  }
-  // the relocated snapshot: every table the shared device functions read, in local numbering.  It lives in shared
-  // memory itself (one thread fills it in): ~50 patched pointers would otherwise sit in every thread's stack.
-  if (tid == nthreads - 1) {
-  DevSnap &L = *(DevSnap *)(smem_raw + Y.snap);
-  L.tab_local = 2; L.local_flat = 1; L.ent_gid = e_gid; L.node_gid = b_gid;
-  L.parent = b_par; L.height = b_hgt; L.lq = s_lq;
-  L.nominal = s_sub;  // only ever read for ClusterQueues: SubtreeQuota == Nominal there (resource_node.go:160-166)
-  L.subtree = s_sub; L.usage = s_u; L.avail = s_av; L.potential = s_pot; L.blimit = s_bl; L.fs_over = s_over; L.fs_lend = s_lend;
-  L.fair_weight = (const double *)(s_blob + BH->wgt); L.cq_generation = (const i64 *)(s_blob + BH->gen);
-  L.cq_within_cq = s_blob + BH->within; L.cq_reclaim_within = b_reclaim; L.cq_borrow_within = s_blob + BH->borrow_w;
-  L.cq_when_can_borrow = s_blob + BH->wcb; L.cq_when_can_preempt = s_blob + BH->wcp; L.cq_preference = s_blob + BH->pref;
-  L.cq_rg_start = (const int32_t *)(s_blob + BH->rgs); L.rg_res_mask = (const uint32_t *)(s_blob + BH->rgmask);
-  L.rg_flavor_start = (const int32_t *)(s_blob + BH->rgfl); L.rg_flavors = (const int32_t *)(s_blob + BH->fl);
-  L.heads = e_ident; L.wl_cq = e_cq; L.wl_priority = e_prio; L.wl_ts = e_ts; L.wl_last_gen = e_lg; L.wl_ps_start = e_psn;
-  L.wl_has_qr = D.wl_has_qr ? e_qr : nullptr;
-  L.ps_req = r_req; L.ps_req_mask = r_mask; L.ps_count = r_count; L.ps_min_count = r_min; L.ps_flavor_ok = r_ok; L.ps_last_tried = r_last;
-  L.ps_group = D.ps_group ? r_group : nullptr;
-  L.ps_flavor = o_fl; L.ps_res_mode = o_md; L.ps_tried = o_tr; L.ps_count_out = o_cnt;
-  L.borrow = e_borrow;
   }
   if (nthreads % FR == 0) {  // a thread stays in one column: private partial sums over its rows
     const int fr = tid % FR, g = tid / FR, G = nthreads / FR;
@@ -561,6 +578,37 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
       const i64 spill = imax(0, s_u[c] - s_lq[c]);
       if (spill) atomicAdd((u64 *)&s_u[col_of(c)], (u64)spill);
     }
+  }
+  // stage B and this thread's record copies have landed (a CTA never exits with a copy in flight into its shared memory)
+  if ((FR & 1) == 0) {
+    mbar_wait(&s_mbar[1], 0);
+    cp_async_wait_all();
+  } else {
+    cp_async_wait_all();
+    __syncthreads();  // stage B was copied by every thread
+  }
+  const TreeBlobHdr *BH = (const TreeBlobHdr *)s_blob;
+  const int32_t *b_gid = (const int32_t *)(s_blob + BH->gid), *b_par = (const int32_t *)(s_blob + BH->par), *b_hgt = (const int32_t *)(s_blob + BH->hgt);
+  const uint8_t *b_reclaim = s_blob + BH->reclaim;
+  // the relocated snapshot: every table the shared device functions read, in local numbering.  It lives in shared
+  // memory itself (one thread fills it in): ~50 patched pointers would otherwise sit in every thread's stack.
+  if (tid == nthreads - 1) {
+  DevSnap &L = *(DevSnap *)(smem_raw + Y.snap);
+  L.tab_local = 2; L.local_flat = 1; L.ent_gid = e_gid; L.node_gid = b_gid;
+  L.parent = b_par; L.height = b_hgt; L.lq = s_lq;
+  L.nominal = s_sub;  // only ever read for ClusterQueues: SubtreeQuota == Nominal there (resource_node.go:160-166)
+  L.subtree = s_sub; L.usage = s_u; L.avail = s_av; L.potential = s_pot; L.blimit = s_bl; L.fs_over = s_over; L.fs_lend = s_lend;
+  L.fair_weight = (const double *)(s_blob + BH->wgt); L.cq_generation = (const i64 *)(s_blob + BH->gen);
+  L.cq_within_cq = s_blob + BH->within; L.cq_reclaim_within = b_reclaim; L.cq_borrow_within = s_blob + BH->borrow_w;
+  L.cq_when_can_borrow = s_blob + BH->wcb; L.cq_when_can_preempt = s_blob + BH->wcp; L.cq_preference = s_blob + BH->pref;
+  L.cq_rg_start = (const int32_t *)(s_blob + BH->rgs); L.rg_res_mask = (const uint32_t *)(s_blob + BH->rgmask);
+  L.rg_flavor_start = (const int32_t *)(s_blob + BH->rgfl); L.rg_flavors = (const int32_t *)(s_blob + BH->fl);
+  L.heads = e_ident; L.wl_cq = e_cq; L.wl_priority = e_prio; L.wl_ts = e_ts; L.wl_last_gen = e_lg; L.wl_ps_start = e_psn;
+  L.wl_has_qr = D.wl_has_qr ? e_qr : nullptr;
+  L.ps_req = r_req; L.ps_req_mask = r_mask; L.ps_count = r_count; L.ps_min_count = r_min; L.ps_flavor_ok = r_ok; L.ps_last_tried = r_last;
+  L.ps_group = D.ps_group ? r_group : nullptr;
+  L.ps_flavor = o_fl; L.ps_res_mode = o_md; L.ps_tried = o_tr; L.ps_count_out = o_cnt;
+  L.borrow = e_borrow;
   }
   // the root's lendable per resource (k_fair_prep): potentialAvailable of the root == its SubtreeQuota, static
   if (fair)
@@ -616,9 +664,9 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
       __syncthreads();
     }
   }
-  // ---- 3. one pass per entry, KB_FLAT_NG lanes each: per-cycle records (one hop: the workload / row ids are known),
-  // nominate (getInitialAssignments, scheduler.go:584-625), iterator key and dense request row (Assignment.Usage.Quota,
-  // absent = -1), with no barrier in between.  Entries with one podset that cannot be reduced take the group walk on
+  // ---- 3. one pass per entry, KB_FLAT_NG lanes each, on the records staged in phase 1: nominate (getInitialAssignments,
+  // scheduler.go:584-625), iterator key and dense request row (Assignment.Usage.Quota, absent = -1), with no barrier in
+  // between.  Entries with one podset that cannot be reduced take the group walk on
   // the shared tables (flat_nominate_group); every other entry (several podsets, or partial admission with a reducible
   // podset) takes get_assignments_coop on the relocated snapshot L.  A round evaluates KB_FLAT_NG flavors of a resource
   // group at once; the walk usually stops in its first round, so fewer lanes per entry mean fewer warps competing for
@@ -634,28 +682,7 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
     for (int i0 = 0, k = 0; i0 < n; i0 += groups, k++) {
       const int i = i0 + tid / KB_FLAT_NG;
       if (i >= n) continue;  // whole lane groups take the branches together
-      const int wl = e_wl[i];
-      const int ps0 = e_ps0[i], l0 = e_psn[i], np = e_psn[i + 1] - l0;
-      for (int kk = glane; kk < np; kk += KB_FLAT_NG) {  // podset rows over the lanes; all loads of a row before its stores
-        const int row = ps0 + kk, l = l0 + kk;
-        const int cnt = __ldg(D.ps_count + row), mn = __ldg(D.ps_min_count + row); const uint32_t msk = __ldg(D.ps_req_mask + row);
-        const int grp = D.ps_group ? __ldg(D.ps_group + row) : -1; const u64 ok = __ldg(D.ps_flavor_ok + row);
-        for (int rr = 0; rr < R; rr += 4) {
-          i64 q[4]; int8_t lt[4];
-#pragma unroll
-          for (int j = 0; j < 4; j++) if (rr + j < R) { q[j] = __ldg(D.ps_req + (size_t)row * R + rr + j); lt[j] = __ldg(D.ps_last_tried + (size_t)row * R + rr + j); }
-#pragma unroll
-          for (int j = 0; j < 4; j++) if (rr + j < R) { r_req[(size_t)l * R + rr + j] = q[j]; r_last[(size_t)l * R + rr + j] = lt[j]; }
-        }
-        r_gid[l] = row; r_count[l] = cnt; r_min[l] = mn; r_mask[l] = msk; r_group[l] = grp; r_ok[l] = ok;
-      }
-      if (glane == 0) {
-        const int pr = __ldg(D.wl_priority + wl); const i64 ts = __ldg(D.wl_ts + wl), lg = __ldg(D.wl_last_gen + wl);
-        const uint8_t qr = D.wl_has_qr ? __ldg(D.wl_has_qr + wl) : 0;
-        e_prio[i] = pr; e_ts[i] = ts; e_lg[i] = lg; e_qr[i] = qr;
-      }
       const bool fast = e_fast[i] & 1;
-      __syncwarp(gmask);  // the records are read by every lane of the group
       if (fast) {
         flat_nominate_group<KB_FLAT_NG>(Y, i, R, FR, D.flags, D.pods_res, D.wl_has_qr != nullptr, gmask, gbase, glane,
                                         sweep ? nullptr : s_q + (size_t)i * FR);
@@ -706,7 +733,7 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
       for (int o = S >> 1; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
       if (!act) continue;
       const int mode = e_mode[i], hq = e_cq[i];
-      if (sub == 0) { e_rank[i] = cnt; m_sorted[cnt] = mode; }
+      if (sub == 0) { e_rank[i] = cnt; m_sorted[cnt] = mode; e_at[cnt] = i; }
       for (int fr = sub; fr < FR; fr += S) {
         const i64 q = s_q[(size_t)i * FR + fr];
         const int r = hq * FR + fr;
@@ -731,23 +758,19 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
       }
     }
   }
+  for (int b = tid; b < (n + 31) >> 5; b += nthreads) mbar_init(blk_bar + b, 1);  // arrived on by warp 0 (flat_ordered_loop)
   __syncthreads();
   KB_FPHASE(3);
-  // ---- 5. the ordered loop
-  if (warp == 0) {
-    if (FR > 32) flat_ordered_loop<true>(n, FR, lane, s_lim, m_sorted, ok_bits, s_u, s_sub);
-    else flat_ordered_loop<false>(n, FR, lane, s_lim, m_sorted, ok_bits, s_u, s_sub);
-  }
-  __syncthreads();
-  KB_FPHASE(4);
-  // ---- 6. publish: usage table with the ClusterQueue rows of the admitted / reserving entries (cq.AddUsage) applied
-  // on the way out, decisions, flavor assignment rows
-  auto final_usage = [&](int c) {
-    const int h = row_of(c), i = n_e[h];
+  // ---- 5. the ordered loop on warp 0, and 6. publication behind it on the other warps: usage table with the
+  // ClusterQueue rows of the admitted / reserving entries (cq.AddUsage) applied on the way out, decisions, flavor
+  // assignment rows.  Only a ClusterQueue row of an entry and its decision wait for the loop, each for the block of 32
+  // positions that holds the entry; the root row is the loop's own result.
+  auto final_usage = [&](int h, int c) {  // cell c of row h
+    const int i = n_e[h];
     i64 u = s_u[c];
     if (i >= 0) {
       const int dec = flat_decision(e_mode[i], ok_bits, e_rank[i]);
-      const i64 q = s_q[(size_t)i * FR + col_of(c)];
+      const i64 q = s_q[(size_t)i * FR + (c - h * FR)];
       if (dec == KB_DEC_ASSUMED) { if (q > 0) u += q; }
       else if (dec == KB_DEC_PREEMPT_NO_TARGETS && q >= 0 && b_reclaim[h] != KB_POLICY_ANY) {
         const i64 bl = s_bl[c], sb = s_sub[c];
@@ -756,41 +779,65 @@ __global__ void __launch_bounds__(KB_FLAT_THREADS) k_cycle_flat(const __grid_con
     }
     return u;
   };
-  if ((FR & 1) == 0) {
-    const int half = tb >> 1;
-    for (int c = tid; c < half; c += nthreads) {
-      const int i = c << 1;
-      *(longlong2 *)(D.usage + (size_t)b_gid[row_of(i)] * FR + col_of(i)) = make_longlong2(final_usage(i), final_usage(i + 1));
+  const int upr = (FR & 1) == 0 ? FR >> 1 : FR;  // stores per usage row: pairs of cells (16 B), single cells for odd FR
+  auto publish_usage = [&](int h, int k) {       // store k of row h
+    const int fr = (FR & 1) == 0 ? k << 1 : k, c = h * FR + fr;
+    i64 *dst = D.usage + (size_t)b_gid[h] * FR + fr;
+    if ((FR & 1) == 0) *(longlong2 *)dst = make_longlong2(final_usage(h, c), final_usage(h, c + 1));
+    else *dst = final_usage(h, c);
+  };
+  const int nw = nthreads >> 5;
+  if (warp == 0) {
+    if (FR > 32) flat_ordered_loop<true>(n, FR, lane, s_lim, m_sorted, ok_bits, blk_bar, s_u, s_sub);
+    else flat_ordered_loop<false>(n, FR, lane, s_lim, m_sorted, ok_bits, blk_bar, s_u, s_sub);
+    KB_FPHASE(4);
+    for (int c = lane; c < FR; c += 32) D.usage[(size_t)b_gid[0] * FR + c] = s_u[c];  // the root row (h = 0, no entry)
+  } else if ((warp & 3) != 0) {  // off warp 0's scheduler (warp % 4): its compare -> vote -> add chain keeps the issue slots
+    const int pw = warp - 1 - (warp >> 2), npw = nw - 1 - ((nw - 1) >> 2);  // publisher warp index / count
+    const int pt = pw * 32 + lane, NP = npw * 32;
+    // ---- 6a. what no decision changes
+    for (int i = pt; i < n; i += NP) {
+      const int e = e_gid[i];
+      D.mode[e] = (uint8_t)e_mode[i]; D.borrow[e] = e_borrow[i]; D.rank[e] = e_rank[i];
+      D.tgt_cnt[e] = 0; D.tgt_off[e] = 0;
     }
-  } else {
-    for (int i = tid; i < tb; i += nthreads) D.usage[(size_t)b_gid[row_of(i)] * FR + col_of(i)] = final_usage(i);
-  }
-  for (int i = tid; i < n; i += nthreads) {
-    const int e = e_gid[i];
-    D.mode[e] = (uint8_t)e_mode[i]; D.borrow[e] = e_borrow[i]; D.decision[e] = (uint8_t)flat_decision(e_mode[i], ok_bits, e_rank[i]); D.rank[e] = e_rank[i];
-    D.tgt_cnt[e] = 0; D.tgt_off[e] = 0;
-  }
-  if ((R & 3) == 0) {  // rows of R bytes are word aligned in both copies
-    const int wpr = R >> 2;
-    for (int c = tid; c < nrows * wpr; c += nthreads) {
-      const int l = c / wpr, w = c % wpr;
-      const size_t dst = (size_t)r_gid[l] * wpr + w, src = (size_t)l * wpr + w;
-      ((uint32_t *)D.ps_flavor)[dst] = ((const uint32_t *)o_fl)[src];
-      ((uint32_t *)D.ps_res_mode)[dst] = ((const uint32_t *)o_md)[src];
-      ((uint32_t *)D.ps_tried)[dst] = ((const uint32_t *)o_tr)[src];
-      if (w == 0) D.ps_count_out[r_gid[l]] = o_cnt[l];
-    }
-  } else {
-    for (int l = tid; l < nrows; l += nthreads) {
-      const int row = r_gid[l];
-      D.ps_count_out[row] = o_cnt[l];
-      for (int r = 0; r < R; r++) {
-        D.ps_flavor[(size_t)row * R + r] = o_fl[(size_t)l * R + r];
-        D.ps_res_mode[(size_t)row * R + r] = o_md[(size_t)l * R + r];
-        D.ps_tried[(size_t)row * R + r] = o_tr[(size_t)l * R + r];
+    if ((R & 3) == 0) {  // rows of R bytes are word aligned in both copies
+      const int wpr = R >> 2;
+      for (int c = pt; c < nrows * wpr; c += NP) {
+        const int l = c / wpr, w = c % wpr;
+        const size_t dst = (size_t)r_gid[l] * wpr + w, src = (size_t)l * wpr + w;
+        ((uint32_t *)D.ps_flavor)[dst] = ((const uint32_t *)o_fl)[src];
+        ((uint32_t *)D.ps_res_mode)[dst] = ((const uint32_t *)o_md)[src];
+        ((uint32_t *)D.ps_tried)[dst] = ((const uint32_t *)o_tr)[src];
+        if (w == 0) D.ps_count_out[r_gid[l]] = o_cnt[l];
+      }
+    } else {
+      for (int l = pt; l < nrows; l += NP) {
+        const int row = r_gid[l];
+        D.ps_count_out[row] = o_cnt[l];
+        for (int r = 0; r < R; r++) {
+          D.ps_flavor[(size_t)row * R + r] = o_fl[(size_t)l * R + r];
+          D.ps_res_mode[(size_t)row * R + r] = o_md[(size_t)l * R + r];
+          D.ps_tried[(size_t)row * R + r] = o_tr[(size_t)l * R + r];
+        }
       }
     }
+    for (int k = upr + pt; k < nn * upr; k += NP) {  // ClusterQueue rows without an entry
+      const int h = k / upr;
+      if (n_e[h] < 0) publish_usage(h, k - h * upr);
+    }
+    // ---- 6b. per block of 32 positions, once the loop has passed it: decisions and ClusterQueue rows of its entries.
+    // The publisher warps form min(warps, blocks) groups; group g takes blocks g, g + groups, ...
+    const int nblk = (n + 31) >> 5, ng = min(npw, nblk), g = pw % ng;
+    const int gi = (pw / ng) * 32 + lane, GT = ((npw - 1 - g) / ng + 1) * 32;
+    for (int b = g; b < nblk; b += ng) {
+      mbar_wait(blk_bar + b, 0);
+      const int p0 = b << 5, np = min(32, n - p0);
+      for (int k = gi; k < np; k += GT) { const int i = e_at[p0 + k]; D.decision[e_gid[i]] = (uint8_t)flat_decision(e_mode[i], ok_bits, p0 + k); }
+      for (int k = gi; k < np * upr; k += GT) { const int p = k / upr, i = e_at[p0 + p]; publish_usage(e_cq[i], k - p * upr); }
+    }
   }
+  __syncthreads();
   KB_FPHASE(5);
 #undef KB_FPHASE
 }

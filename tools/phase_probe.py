@@ -13,4 +13,4 @@ for _ in range(4):
         flush.zero_(); torch.cuda.synchronize()
     ev.cycle_resident()
 st = ev.stats(); print("cold" if cold else "warm", "cycle ms", st.last_cycle_gpu_ms, [ (abi.KERNEL_NAMES[i], round(st.kernel_ms[i],4)) for i in range(16) if st.kernel_ms[i]>0])
-print("phase cycles (k_cycle_flat: stage, entries+tree, records+nominate+keys+requests, rank+thresholds, ordered loop, commit+publish):", list(st.search_stat)[:6])
+print("phase cycles (k_cycle_flat: stage A, entries+records+tree+stage B, nominate+keys+requests, rank+thresholds, ordered loop+publish, publish tail):", list(st.search_stat)[:6])
