@@ -33,6 +33,12 @@ struct TasDev {
   int32_t *status, *n_out, *tmp_start, *tmp_leaf, *tmp_count;
   // per-CTA lists of k_tas_select
   int32_t *lists; int list_cap;
+  // CountIn can be negative (a leaf with less free capacity than usage, or a chain that mixes simulate-empty): walks
+  // keep zero-count domains (see TasSel::next), and lists / output regions may need more than `count` entries
+  int keep_zero;
+  // [0] = 1 when a list or an output region was too small (nothing is written past either), [1] = longest list needed;
+  // the host grows what was short and runs the batch again
+  int32_t *overflow;
 };
 
 // slot descriptors: which request defines the shape of slot s (its request row / mask / flags / eligibility / chain)
@@ -135,8 +141,11 @@ struct TasSel {
   }
   // next domain of S in sorted order strictly after `after` (after.d < 0: the first).  filter 1: only domains whose
   // sliceState >= arg; filter 2 / 3: skip domains whose sliceState / state is 0 — the reference appends them with zero
-  // pods (they sort first under LeastFreeCapacity), which changes nothing downstream: their descendants get zero
-  // pods and buildTopologyAssignmentForLevels drops zero counts (:1443-1446)
+  // pods (they sort first under LeastFreeCapacity), which changes nothing downstream as long as no count is negative:
+  // their descendants get zero pods and buildTopologyAssignmentForLevels drops zero counts (:1443-1446).  When a leaf
+  // is over-used (T.keep_zero) a zero domain can hold a negative child and a positive one, and the reference hands the
+  // positive one pods while distributing the zero domain's 0, so the walks use filter 0 instead (skip_zero()).
+  __device__ __forceinline__ int skip_zero(int filter) const { return T.keep_zero ? 0 : filter; }
   // Large level sets (tens of thousands of hosts) are walked through a sorted CACHE of their smallest keys: one pass
   // keeps every thread's KB_TAS_LOCAL best candidates, the block sorts their union in shared memory, and all keys up
   // to T = the smallest "worst kept key" among the threads that had to drop something are provably complete (every
@@ -254,6 +263,7 @@ __device__ inline void tas_select_one(const TasDev &T, const int q, TasKey *s_re
   const int levelIdx = T.level[q], sliceLevel = T.slice_level[q], L = T.L;
   const bool required = flags & KB_TAS_REQUIRED, unconstrained = flags & KB_TAS_UNCONSTRAINED;
   auto finish = [&](int status, int n) { if (threadIdx.x == 0) { T.status[q] = status; T.n_out[q] = n; } };
+  auto list_short = [&](int need) { if (threadIdx.x == 0) { T.overflow[0] = 1; atomicMax(&T.overflow[1], need); } finish(KB_TAS_NO_FIT, 0); };
   if (T.pred[q] >= 0 && T.status[T.pred[q]] != KB_TAS_OK) { finish(-1, 0); return; }  // the chain stopped at an earlier podset (:551-553)
   if (levelIdx < 0 || levelIdx >= L || sliceLevel < 0 || sliceLevel >= L || levelIdx > sliceLevel || sliceSize < 1) { finish(KB_TAS_BAD_REQUEST, 0); return; }
   const int slot = T.slot[q];
@@ -282,7 +292,7 @@ __device__ inline void tas_select_one(const TasDev &T, const int q, TasKey *s_re
       TasKey cur = none;
       ncur = 0;
       while (remaining > 0) {
-        TasKey d = X.next(S, cur, 2, 0);
+        TasKey d = X.next(S, cur, X.skip_zero(2), 0);
         if (d.d < 0) break;
         cur = d;
         if (!lfc && X.sl[d.d] >= remaining) d = X.best_fit(S, d, remaining, true);
@@ -290,7 +300,8 @@ __device__ inline void tas_select_one(const TasDev &T, const int q, TasKey *s_re
         ncur++;
         remaining -= X.sl[d.d];
       }
-      if (remaining > 0 || ncur > cap) { finish(KB_TAS_NO_FIT, 0); return; }
+      if (remaining > 0) { finish(KB_TAS_NO_FIT, 0); return; }  // the walk counted every domain, listed or not
+      if (ncur > cap) { list_short(ncur); return; }
       fitLevel = lv;
       break;
     }
@@ -322,23 +333,23 @@ __device__ inline void tas_select_one(const TasDev &T, const int q, TasKey *s_re
     ncur = s_n;
     int32_t *t; t = c_d; c_d = n_d; n_d = t; t = c_st; c_st = n_st; n_st = t; t = c_sl; c_sl = n_sl; n_sl = t;
   }
-  // ordered greedy over a SET (children of parents) walked in sorted order; appends to the next-level list
+  // ordered greedy over a SET (children of parents) walked in sorted order; appends to the next-level list (entries past
+  // `cap` are counted, not written: the caller reports the length it needed)
   auto update_set = [&](const TasSet &S, int32_t cnt, int32_t ss, bool slices, int *nn) -> bool {
     int32_t remaining = slices ? cnt / ss : cnt;
     TasKey cur = none;
     while (true) {
-      TasKey d = X.next(S, cur, remaining > 0 ? (slices ? 2 : 3) : 0, 0);
+      TasKey d = X.next(S, cur, remaining > 0 ? X.skip_zero(slices ? 2 : 3) : 0, 0);
       if (d.d < 0) return false;
       cur = d;
       int32_t v = slices ? X.sl[d.d] : X.st[d.d];
       if (!lfc && v >= remaining) { d = X.best_fit(S, d, remaining, slices); v = slices ? X.sl[d.d] : X.st[d.d]; }
-      if (*nn >= cap) return false;
       if (v >= remaining) {
-        if (threadIdx.x == 0) { n_d[*nn] = d.d; n_st[*nn] = slices ? remaining * ss : remaining; n_sl[*nn] = slices ? remaining : X.sl[d.d]; }
+        if (threadIdx.x == 0 && *nn < cap) { n_d[*nn] = d.d; n_st[*nn] = slices ? remaining * ss : remaining; n_sl[*nn] = slices ? remaining : X.sl[d.d]; }
         (*nn)++;
         return true;
       }
-      if (threadIdx.x == 0) { n_d[*nn] = d.d; n_st[*nn] = slices ? v * ss : v; n_sl[*nn] = X.sl[d.d]; }
+      if (threadIdx.x == 0 && *nn < cap) { n_d[*nn] = d.d; n_st[*nn] = slices ? v * ss : v; n_sl[*nn] = X.sl[d.d]; }
       (*nn)++;
       remaining -= v;
     }
@@ -349,6 +360,7 @@ __device__ inline void tas_select_one(const TasDev &T, const int q, TasKey *s_re
     TasSet S{0, 0, c_d, ncur};
     int nn = 0;
     if (!update_set(S, count, sliceSize, true, &nn)) { finish(KB_TAS_NO_FIT, 0); return; }
+    if (nn > cap) { list_short(nn); return; }
     __syncthreads();
     ncur = nn;
     int32_t *t; t = c_d; c_d = n_d; n_d = t; t = c_st; c_st = n_st; n_st = t; t = c_sl; c_sl = n_sl; n_sl = t;
@@ -360,21 +372,25 @@ __device__ inline void tas_select_one(const TasDev &T, const int q, TasKey *s_re
       TasSet S{0, 0, c_d + i, 1};
       if (!update_set(S, c_st[i], 1, false, &nn)) { finish(KB_TAS_NO_FIT, 0); return; }
     }
+    if (nn > cap) { list_short(nn); return; }
     __syncthreads();
     ncur = nn;
     int32_t *t; t = c_d; c_d = n_d; n_d = t; t = c_st; c_st = n_st; n_st = t; t = c_sl; c_sl = n_sl; n_sl = t;
   }
   __syncthreads();
   // ---- buildAssignment :1455-1466: leaves in lexicographic (= index) order, zero counts dropped
-  const int out0 = T.tmp_start[q];
+  const int out0 = T.tmp_start[q], region = T.tmp_start[q + 1] - out0;
   int nout = 0;
   for (int i = threadIdx.x; i < ncur; i += blockDim.x) {
     if (c_st[i] == 0) continue;
     int rank = 0;
     for (int j = 0; j < ncur; j++) if (c_st[j] != 0 && c_d[j] < c_d[i]) rank++;
-    T.tmp_leaf[out0 + rank] = c_d[i] - T.leaf0; T.tmp_count[out0 + rank] = c_st[i];
+    if (rank < region) { T.tmp_leaf[out0 + rank] = c_d[i] - T.leaf0; T.tmp_count[out0 + rank] = c_st[i]; }
   }
-  if (threadIdx.x == 0) { for (int j = 0; j < ncur; j++) if (c_st[j] != 0) nout++; }
+  if (threadIdx.x == 0) {
+    for (int j = 0; j < ncur; j++) if (c_st[j] != 0) nout++;
+    if (nout > region) T.overflow[0] = 1;  // n_out[q] = nout tells the host how large the region must be
+  }
   // ---- addAssumedUsage :619-627 for the next podset of the chain
   const int cs = T.chain_slot[q];
   if (cs >= 0) {
@@ -404,7 +420,8 @@ __global__ void __launch_bounds__(KB_TAS_THREADS) k_tas_select(TasDev T, const i
 // temporary per-request regions -> CSR
 __global__ void k_tas_compact(TasDev T, const int32_t *asg_start, int32_t *asg_leaf, int32_t *asg_count, int capacity) {
   int q = blockIdx.x;
-  int n = T.n_out[q], src = T.tmp_start[q], dst = asg_start[q];
+  // n_out can exceed the region (or its prefix sum wrap) only in a run the host discards: read and write in bounds anyway
+  int src = T.tmp_start[q], n = min(T.n_out[q], T.tmp_start[q + 1] - src), dst = asg_start[q];
   for (int i = threadIdx.x; i < n; i += blockDim.x)
-    if (dst + i < capacity) { asg_leaf[dst + i] = T.tmp_leaf[src + i]; asg_count[dst + i] = T.tmp_count[src + i]; }
+    if (dst >= 0 && dst + i < capacity) { asg_leaf[dst + i] = T.tmp_leaf[src + i]; asg_count[dst + i] = T.tmp_count[src + i]; }
 }

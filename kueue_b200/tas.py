@@ -237,9 +237,11 @@ def synth_topology(blocks: int = 10, racks: int = 100, hosts: int = 100, seed: i
     return t
 
 
-def synth_requests(topo: TasTopology, n: int, seed: int = 7, shapes: int = 16, chains: bool = False, max_pods: int = 64) -> TasRequests:
+def synth_requests(topo: TasTopology, n: int, seed: int = 7, shapes: int = 16, chains: bool = False, max_pods: int = 64,
+                   profile_mixed: Optional[bool] = True) -> TasRequests:
     """n podset requests: `shapes` distinct pod templates, 1..max_pods pods, required / preferred at rack or block level or
-    unconstrained; with chains=True some workloads carry two or three podsets."""
+    unconstrained; with chains=True some workloads carry two or three podsets.  profile_mixed=None draws the TASProfileMixed
+    flag per request, so unconstrained requests run in both LeastFreeCapacity and BestFit order."""
     rng = np.random.Generator(np.random.PCG64(seed))
     tmpl = [{"cpu": int(rng.integers(1, 33)) * 1000, "memory": int(rng.integers(1, 65)) << 30, **({"gpu": int(rng.integers(1, 5))} if rng.random() < 0.5 else {})}
             for _ in range(shapes)]
@@ -256,5 +258,7 @@ def synth_requests(topo: TasTopology, n: int, seed: int = 7, shapes: int = 16, c
         count = int(rng.integers(1, max_pods + 1))
         if mode == 4:
             count += count % 2
-        reqs.add(chain, tmpl[int(rng.integers(0, shapes))], count, None if tr is None else {"required": None, "preferred": None, "unconstrained": False, "sliceRequiredTopology": None, "sliceSize": None, **tr})
+        mixed = bool(rng.integers(0, 2)) if profile_mixed is None else profile_mixed
+        reqs.add(chain, tmpl[int(rng.integers(0, shapes))], count, None if tr is None else {"required": None, "preferred": None, "unconstrained": False, "sliceRequiredTopology": None, "sliceSize": None, **tr},
+                 profile_mixed=mixed)
     return reqs.finalize()
