@@ -253,6 +253,19 @@ typedef struct kb_snapshot {
   const int64_t *afs_milli_mul;     /* [R] MilliValue factor of the library's unit: 1 for cpu (milli), else 1000   */
   double afs_alpha;                 /* 1 - 0.5^(UsageSamplingInterval / UsageHalfLifeTime), 0 when the half-life is 0
                                        (calculateAlphaRate); computed by the caller so the Go shim passes math.Pow's bits */
+
+  /* ---- eviction replay (optional; read by kb_run_drain only, kb_run_cycle ignores it) ----
+     adm_wl[a] = index into the pending tables of admitted workload a's own record: its spec as it would be requeued
+     (full counts and per-podset requests; its adm_use_* cells may reflect a partial admission).  Those records hold
+     quota, so they start out of every queue.  NULL = evictions are not replayed and the drain is unchanged.
+     With adm_wl, every target of a Preempting entry of cycle c leaves the admitted tables before cycle c+1 (its cells
+     leave its ClusterQueue's usage, its row is removed) and its record returns to its queue with LastAssignment nil;
+     then every workload set aside by the ClusterQueues of the victims' root cohort trees returns to its queue
+     (QueueAssociatedInadmissibleWorkloadsAfter, manager.go:670-697; inadmissible_workloads.go:128-223).  See
+     kb_run_drain.  Errors: KB_ERR_INVALID for an index out of range, an index named twice or
+     wl_cq[adm_wl[a]] != adm_cq[a]; KB_ERR_UNSUPPORTED without KB_F_PRIORITY_SORTING_WITHIN_COHORT (a preempted
+     workload's queue-order timestamp would become its eviction time, workload.go:1174-1193). */
+  const int32_t *adm_wl;            /* [n_adm] */
 } kb_snapshot;
 
 /* ------------------------------------------------------------------------
@@ -373,7 +386,21 @@ int32_t kb_download(kb_handle *h, kb_cycle_out *out);
  *                              while LastAssignment.PendingFlavors() (workload.go:163-176), else the next workload
  *                              becomes the head; a NoFit head with a known wl_sched_hash also sets aside every queued
  *                              workload of its class (handleInadmissibleHash, cluster_queue.go:408-425).
- * Evictions are asynchronous in the reference and are not replayed: the targets of a Preempting entry stay admitted.
+ * Without kb_snapshot.adm_wl evictions are not replayed: the targets of a Preempting entry stay admitted, and the drain
+ * ends with the first cycle that admits nothing.  With adm_wl the drain takes the limit in which every eviction issued
+ * in cycle c completes before cycle c+1 (in the reference it completes asynchronously), in this order:
+ *   1. the decisions are applied as above;
+ *   2. every target of every Preempting entry (adm_evicted or not) leaves the admitted tables: its cells leave its own
+ *      ClusterQueue's usage (cache.DeleteWorkload), its row is removed (the other rows keep their order), and its
+ *      record adm_wl[row] returns to its queue at once (preemption sets no RequeueState, workload_controller.go:827-832)
+ *      with LastAssignment nil (wl_last_gen = -1, ps_last_tried = -1, HasQuotaReservation false);
+ *   3. for every root cohort with a victim in its tree (the ClusterQueue itself when it has no cohort) every workload
+ *      its ClusterQueues set aside returns to its queue and keeps its LastAssignment (requeueWorkloadsCohort /
+ *      queueInadmissibleWorkloads, inadmissible_workloads.go:128-223; the scheduling-hash sets are cleared);
+ *   4. the head of every queue in cycle c+1 is its first queued workload in queueOrderingFunc order; a requeued victim
+ *      takes the place its priority, creation timestamp and UID give it (workload.go:1174-1193).
+ * The drain then ends after the first cycle that neither admits nor evicts.  Evictions under way before the drain
+ * (adm_evicted rows that are never targeted) are not completed.
  * Cycle c runs with now_ns + c.  Bit-exact with iterating kb_run_cycle under the same rules (kueue_b200/drain.py).
  * With the AdmissionFairSharing tables (kb_snapshot.wl_lq != NULL), the queue of a ClusterQueue with cq_afs set is one
  * segment per LocalQueue, each in the order above; its head is the workload with the smallest (LocalQueue usage by
@@ -389,7 +416,7 @@ typedef struct kb_drain_out {
   int32_t *cycle_heads;      /* [max_cycles] entries per cycle (may be NULL) */
   int32_t *cycle_admitted;   /* [max_cycles] admissions per cycle (may be NULL) */
   /* per pending workload [n_wl] (each may be NULL) */
-  int32_t *wl_admit_cycle;   /* cycle that admitted it, -1 = still pending */
+  int32_t *wl_admit_cycle;   /* cycle of its last admission if it holds quota at the end, else -1 */
   uint8_t *wl_last_decision; /* KB_DEC_* of its last evaluation, 0xff = never a head */
   int32_t *wl_evals;         /* cycles that evaluated it */
   /* assignment of the last evaluation, indexed like the input podset tables (may be NULL) */
@@ -401,6 +428,10 @@ typedef struct kb_drain_out {
   uint8_t *trace_decision;   /* [trace_capacity] KB_DEC_* */
   int64_t trace_capacity;
   double gpu_ms;             /* out: device time of all cycles (kernels of the cycles + queue layer) */
+  /* eviction replay (kb_snapshot.adm_wl != NULL; zero otherwise) */
+  int64_t n_evicted;         /* out: evictions over all cycles */
+  int32_t *cycle_evicted;    /* [max_cycles] evictions per cycle (may be NULL) */
+  int32_t *wl_evictions;     /* [n_wl] times each pending record was evicted (may be NULL) */
 } kb_drain_out;
 int32_t kb_run_drain(kb_handle *h, const kb_snapshot *s, kb_drain_out *out);
 

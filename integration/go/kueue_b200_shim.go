@@ -353,6 +353,11 @@ func (s *Scheduler) flatten(snap *schdcache.Snapshot, heads []workload.Info, gen
 	c.adm_cq, c.adm_priority, c.adm_ts, c.adm_qr_ts, c.adm_uid = cp32(admCq), cp32(admPrio), cp64(admTs), cp64(admQr), cp64(admUID)
 	c.adm_evicted, c.adm_use_start, c.adm_use_fr, c.adm_use_qty = cpU8(admEv), cp32(admUseStart), cp32(admFr), cp64(admQty)
 	c.heads = cp32(headsIdx)
+	// Eviction replay in kb_run_drain (kb_snapshot.adm_wl, INTEGRATION.md): before the copies above, append one pending
+	// record per admitted workload (its ClusterQueue, priority, queue-order timestamp, UID and podsets with full counts, as
+	// it would be requeued) and keep its index:
+	//   admWl[a] = int32(len(wlCq)); wlCq = append(wlCq, admCq[a]); ...   then c.adm_wl = cp32(admWl)
+	// This shim runs single cycles and leaves c.adm_wl nil.
 	if anyGroup { // optional table: NULL when no podset is grouped
 		c.ps_group = cp32(psGroup)
 	}

@@ -77,6 +77,7 @@ class kb_snapshot(C.Structure):
         ("lq_weight", _P(C.c_double)), ("lq_consumed", _P(C.c_int64)), ("lq_consumed_scale", _P(C.c_int32)),
         ("lq_penalty", _P(C.c_int64)), ("afs_res_weight", _P(C.c_double)), ("afs_milli_mul", _P(C.c_int64)),
         ("afs_alpha", C.c_double),
+        ("adm_wl", _P(C.c_int32)),
     ]
 
 
@@ -120,6 +121,7 @@ class kb_drain_out(C.Structure):
         ("ps_flavor", _P(C.c_int8)), ("ps_count", _P(C.c_int32)), ("cq_usage", _P(C.c_int64)),
         ("trace_wl", _P(C.c_int32)), ("trace_decision", _P(C.c_uint8)), ("trace_capacity", C.c_int64),
         ("gpu_ms", C.c_double),
+        ("n_evicted", C.c_int64), ("cycle_evicted", _P(C.c_int32)), ("wl_evictions", _P(C.c_int32)),
     ]
 
 
@@ -171,11 +173,12 @@ _DT = {
     "usage_delta_cq": np.int32, "usage_delta_rows": np.int64,
     "wl_lq": np.int32, "lq_cq": np.int32, "cq_afs": np.uint8, "lq_weight": np.float64, "lq_consumed": np.int64,
     "lq_consumed_scale": np.int32, "lq_penalty": np.int64, "afs_res_weight": np.float64, "afs_milli_mul": np.int64,
+    "adm_wl": np.int32,
 }
 # AdmissionFairSharing tables (include/kueue_b200.h): wl_lq absent = AFS off
 AFS_FIELDS = ("wl_lq", "lq_cq", "cq_afs", "lq_weight", "lq_consumed", "lq_consumed_scale", "lq_penalty", "afs_res_weight",
               "afs_milli_mul")
-OPTIONAL_FIELDS = ("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows") + AFS_FIELDS  # NULL in kb_snapshot when absent
+OPTIONAL_FIELDS = ("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows", "adm_wl") + AFS_FIELDS  # NULL in kb_snapshot when absent
 ARRAY_FIELDS = list(_DT.keys())
 # tables the library keeps resident while kb_snapshot.static_generation is unchanged (include/kueue_b200.h)
 STATIC_FIELDS = ("parent", "fair_weight", "nominal", "borrow_limit", "lend_limit", "cq_within_cq", "cq_reclaim_within",
@@ -385,6 +388,8 @@ class DrainOut:
         self.ps_flavor = np.full((snap.n_podset, R), -1, np.int8)
         self.ps_count = np.zeros(snap.n_podset, np.int32)
         self.cq_usage = np.zeros((Q, snap.n_fr), np.int64)
+        self.cycle_evicted = np.zeros(max_cycles, np.int32)
+        self.wl_evictions = np.zeros(W, np.int32)
         cap = min(W * 4 + Q, min(Q, W) * max_cycles) if trace else 0
         self.trace_wl = np.zeros(max(1, cap), np.int32)
         self.trace_decision = np.zeros(max(1, cap), np.uint8)
@@ -395,6 +400,7 @@ class DrainOut:
         s.wl_evals = _ptr(self.wl_evals, C.c_int32)
         s.ps_flavor = _ptr(self.ps_flavor, C.c_int8); s.ps_count = _ptr(self.ps_count, C.c_int32)
         s.cq_usage = _ptr(self.cq_usage, C.c_int64)
+        s.cycle_evicted = _ptr(self.cycle_evicted, C.c_int32); s.wl_evictions = _ptr(self.wl_evictions, C.c_int32)
         if trace:
             s.trace_wl = _ptr(self.trace_wl, C.c_int32); s.trace_decision = _ptr(self.trace_decision, C.c_uint8)
         s.trace_capacity = cap
@@ -408,6 +414,8 @@ class DrainOut:
     def n_admitted(self): return int(self.struct.n_admitted)
     @property
     def gpu_ms(self): return float(self.struct.gpu_ms)
+    @property
+    def n_evicted(self): return int(self.struct.n_evicted)
 
     def cycles(self):
         """[(heads, decisions)] per cycle from the trace."""

@@ -1351,7 +1351,21 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   const int Q = s->n_cq, W = s->n_wl, R = s->n_resource, FR = s->n_flavor * s->n_resource;
   const int Hcap = std::min(Q, W);
   const int max_cycles = std::max(0, out->max_cycles);
-  out->n_cycles = 0; out->n_decisions = 0; out->n_admitted = 0; out->gpu_ms = 0;
+  out->n_cycles = 0; out->n_decisions = 0; out->n_admitted = 0; out->gpu_ms = 0; out->n_evicted = 0;
+  // ---- eviction replay: host-side checks of adm_wl (include/kueue_b200.h)
+  const bool replay = s->adm_wl != nullptr;
+  if (replay) {
+    if (!(s->flags & KB_F_PRIORITY_SORTING_WITHIN_COHORT))
+      return fail(h, KB_ERR_UNSUPPORTED, "adm_wl: eviction replay needs KB_F_PRIORITY_SORTING_WITHIN_COHORT (a preempted workload's queue-order timestamp would be its eviction time)");
+    std::vector<uint8_t> named((size_t)std::max(1, W), 0);
+    for (int a = 0; a < s->n_adm; a++) {
+      const int w = s->adm_wl[a];
+      if (w < 0 || w >= W) return fail(h, KB_ERR_INVALID, "adm_wl out of range");
+      if (named[w]) return fail(h, KB_ERR_INVALID, "adm_wl names a pending record twice");
+      named[w] = 1;
+      if (s->adm_cq[a] < 0 || s->adm_cq[a] >= Q || s->wl_cq[w] != s->adm_cq[a]) return fail(h, KB_ERR_INVALID, "adm_wl: the record's ClusterQueue is not the admitted workload's");
+    }
+  }
   if (Hcap == 0 || max_cycles == 0) return KB_OK;
   size_t extra = (size_t)std::min<long long>((long long)W, (long long)Hcap * max_cycles);
   h->drain_extra_adm = extra;
@@ -1367,6 +1381,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   // ClusterQueue, numbered ClusterQueue-major; the initial LocalQueue usage (kb_drain.cuh afs_lq_usage)
   const bool afs = s->wl_lq != nullptr;
   const int L = afs ? s->n_lq : 0;
+  // evictions happen only where a target search can: without a preemption policy adm_wl only keeps its records queued-out
+  const bool evict = replay && h->preempt_possible;
   std::vector<int32_t> seg_start, lq_seg, seg_lq, afs_cqs;
   std::vector<double> lq_usage;
   int S = Q;
@@ -1406,6 +1422,19 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   need(Sz + 2, 4); need(Sz + 2, 4); need(Sz, 4); need(Wz, 1); need((size_t)Q + 2, 4); need((size_t)Q + 2, 4);
   for (int k = 0; k < 4; k++) need(Hz + 2, 4);
   need(16, 4); need(Wz, 4); need(Wz, 4); need(Wz, 1); need(trace_cap, 4); need(trace_cap, 1);
+  // replay: a workload holds at most one live row, so the live rows after a compaction plus the cycle's admissions stay
+  // within the capacity upload_impl reserved: rows <= min(W, A_in + admissions) <= A_in + min(W, Hcap * max_cycles),
+  // cells <= AU_in + min(P * R, that bound * FR) (a readmitted victim's old cells left with its old row)
+  const size_t Acap = (size_t)s->n_adm + h->drain_extra_adm, AUcap = (size_t)s->n_adm_use + h->drain_extra_au;
+  size_t scan_bytes = 0;
+  if (evict) cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (int32_t *)nullptr, (int32_t *)nullptr, (int)Acap + 1, h->stream);
+  const size_t nR = (size_t)std::max(1, D.nRoots);
+  if (replay) { need(Acap, 4); need(Wz, 4); need(Wz, 4); need(Wz, 4); need(Sz, 4); }
+  if (evict) {
+    need(Acap, 4); need(Acap, 4); need(nR, 4); for (int k = 0; k < 4; k++) need(Acap + 1, 4); need(scan_bytes + 256, 1);
+    need(Acap, 4); need(Acap, 4); need(Acap, 8); need(Acap, 8); need(Acap, 8); need(Acap, 1); need(Acap + 1, 4); need(AUcap, 4); need(AUcap, 8);
+  }
+  if (!replay) need(Sz, 4);
   if (afs) {
     need((size_t)Q + 1, 4); need(Lz, 4); need(seg_lq.size(), 4); need(afs_cqs.size() + 1, 4); need(Q, 4); need(Wz, 4); need(Q, 1);
     need(Lz, 8); need(LR, 8); need(LR, 4); need(LR, 8); need(Lz, 8); need(R, 8); need(R, 8);
@@ -1424,7 +1453,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   void *sort_tmp = take(sort_bytes, 1);
   DrainDev X{};
   int32_t *q_count = (int32_t *)take(Sz + 2, 4);
-  X.q_start = (int32_t *)take(Sz + 2, 4); X.cursor = (int32_t *)take(Sz, 4); X.gone = (uint8_t *)take(Wz, 1);
+  X.q_start = (int32_t *)take(Sz + 2, 4); X.cursor = (int32_t *)take(Sz, 4); X.wl_state = (uint8_t *)take(Wz, 1);
+  X.first_aside = (int32_t *)take(Sz, 4);
   X.flag = (int32_t *)take((size_t)Q + 2, 4); X.pos = (int32_t *)take((size_t)Q + 2, 4);
   X.e_assumed = (int32_t *)take(Hz + 2, 4); X.e_ncells = (int32_t *)take(Hz + 2, 4);
   X.e_adm_off = (int32_t *)take(Hz + 2, 4); X.e_cell_off = (int32_t *)take(Hz + 2, 4);
@@ -1437,7 +1467,28 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   X.adm_ts = const_cast<i64 *>(D.adm_ts); X.adm_qr_ts = const_cast<i64 *>(D.adm_qr_ts); X.adm_uid = const_cast<i64 *>(D.adm_uid);
   X.adm_evicted = const_cast<uint8_t *>(D.adm_evicted); X.adm_use_start = const_cast<int32_t *>(D.adm_use_start);
   X.adm_use_fr = const_cast<int32_t *>(D.adm_use_fr); X.adm_use_qty = const_cast<i64 *>(D.adm_use_qty);
-  if (afs) {
+  X.A_cap = (int)Acap; X.AU_cap = (int)AUcap;
+  AdmTabs other{};  // replay: the other half of the admitted tables' double buffer
+  void *scan_tmp = nullptr;
+  if (replay) {
+    X.adm_wl = (int32_t *)take(Acap, 4);
+    CUDA_TRY(h, cudaMemcpyAsync(X.adm_wl, s->adm_wl, (size_t)s->n_adm * 4, cudaMemcpyHostToDevice, h->stream));
+    X.wl_seg = (int32_t *)take(Wz, 4); X.wl_pos = (int32_t *)take(Wz, 4); X.wl_evictions = (int32_t *)take(Wz, 4);
+    X.wl_has_qr = const_cast<uint8_t *>(D.wl_has_qr);
+  }
+  if (evict) {
+    X.adm_dead = (int32_t *)take(Acap, 4);
+    CUDA_TRY(h, cudaMemsetAsync(X.adm_dead, 0, Acap * 4, h->stream));
+    other.wl = (int32_t *)take(Acap, 4);
+    X.root_mark = (int32_t *)take(nR, 4);
+    CUDA_TRY(h, cudaMemsetAsync(X.root_mark, 0, nR * 4, h->stream));
+    X.row_live = (int32_t *)take(Acap + 1, 4); X.row_cells = (int32_t *)take(Acap + 1, 4);
+    X.row_new = (int32_t *)take(Acap + 1, 4); X.cell_new = (int32_t *)take(Acap + 1, 4);
+    scan_tmp = take(scan_bytes + 256, 1);
+    other.cq = (int32_t *)take(Acap, 4); other.priority = (int32_t *)take(Acap, 4); other.ts = (i64 *)take(Acap, 8);
+    other.qr_ts = (i64 *)take(Acap, 8); other.uid = (i64 *)take(Acap, 8); other.evicted = (uint8_t *)take(Acap, 1);
+    other.use_start = (int32_t *)take(Acap + 1, 4); other.use_fr = (int32_t *)take(AUcap, 4); other.use_qty = (i64 *)take(AUcap, 8);
+  }  if (afs) {
     auto h2d = [&](const void *src, size_t n, size_t sz) {
       char *p = take(n, sz);
       if (n) { cudaError_t e = cudaMemcpyAsync(p, src, n * sz, cudaMemcpyHostToDevice, h->stream); if (e != cudaSuccess) return (char *)nullptr; }
@@ -1482,6 +1533,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   }
   k_scan_i32<<<1, 1024, 0, h->stream>>>(q_count, X.q_start, S);
   k_drain_init<<<std::max(nbW, (S + tb - 1) / tb), tb, 0, h->stream>>>(D, X, S);
+  if (replay) k_drain_init_replay<<<std::max(nbW, (s->n_adm + tb - 1) / tb), tb, 0, h->stream>>>(D, X, s->n_adm);
+  k_drain_advance<<<(S + tb - 1) / tb, tb, 0, h->stream>>>(X, S);
   int32_t *d_heads = const_cast<int32_t *>(D.heads);
   auto enqueue_heads = [&]() {
     k_drain_flag<<<nbQ, tb, 0, h->stream>>>(D, X);
@@ -1489,6 +1542,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     k_scan_i32<<<1, 1024, 0, h->stream>>>(X.flag, X.pos, Q);
     k_drain_heads<<<nbQ, tb, 0, h->stream>>>(D, X, d_heads);
   };
+  CUDA_TRY(h, cudaMemsetAsync(X.counters + 1, 0, 5 * 4, h->stream));
   enqueue_heads();
   CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[8], X.counters, 4, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
@@ -1508,7 +1562,23 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     k_drain_apply<<<nbH, tb, 0, h->stream>>>(D, X);
     k_scan_i32<<<1, 1024, 0, h->stream>>>(X.e_assumed, X.e_adm_off, n_live);
     k_scan_i32<<<1, 1024, 0, h->stream>>>(X.e_ncells, X.e_cell_off, n_live);
-    k_drain_admit<<<nbH, tb, 0, h->stream>>>(D, X, s->now_ns + cyc);
+    DrainDev Xa = X;  // the tables k_drain_admit appends to
+    if (evict) {
+      CUDA_TRY(h, cudaMemsetAsync(X.counters + 1, 0, 4 * 4, h->stream));
+      k_drain_evict<<<nbH, tb, 0, h->stream>>>(D, X);
+      k_drain_requeue<<<nbQ, tb, 0, h->stream>>>(D, X);
+      const int nbA = (A_cur + 1 + tb - 1) / tb;
+      k_drain_live<<<nbA, tb, 0, h->stream>>>(X);
+      size_t sb = scan_bytes;
+      CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(scan_tmp, sb, X.row_live, X.row_new, A_cur + 1, h->stream));
+      sb = scan_bytes;
+      CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(scan_tmp, sb, X.row_cells, X.cell_new, A_cur + 1, h->stream));
+      k_drain_compact<<<nbA, tb, 0, h->stream>>>(X, other);
+      Xa.adm_cq = other.cq; Xa.adm_priority = other.priority; Xa.adm_ts = other.ts; Xa.adm_qr_ts = other.qr_ts; Xa.adm_uid = other.uid;
+      Xa.adm_evicted = other.evicted; Xa.adm_use_start = other.use_start; Xa.adm_use_fr = other.use_fr; Xa.adm_use_qty = other.use_qty;
+      Xa.adm_wl = other.wl;
+    }
+    k_drain_admit<<<nbH, tb, 0, h->stream>>>(D, Xa, s->now_ns + cyc, evict ? X.counters + 2 : nullptr);
     enqueue_heads();
     kmark(h, -1);
     CUDA_TRY(h, cudaEventRecord(h->ev_d, h->stream));
@@ -1516,19 +1586,33 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[9], X.e_adm_off + n_live, 4, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[10], X.e_cell_off + n_live, 4, cudaMemcpyDeviceToHost, h->stream));
     if (afs) CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[11], D.status, 4, cudaMemcpyDeviceToHost, h->stream));  // after k_drain_admit
+    if (evict) CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[12], X.counters + 1, 5 * 4, cudaMemcpyDeviceToHost, h->stream));  // evictions, live rows / cells, capacity
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     rc = cycle_finish(h);
     if (rc != KB_OK) return rc;
     if (afs && (h->host_words[11] & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: an entry penalty overflows int64");
     for (int i = 0; i < KB_N_KERNELS; i++) kms[i] += h->stats.kernel_ms[i];
     { float ms = 0; cudaEventElapsedTime(&ms, h->ev2, h->ev_d); gpu_ms += ms; }
+    if (evict && h->host_words[16]) return fail(h, KB_ERR_CAPACITY, "kb_run_drain: the admitted tables are full");
     int n_new = (int)h->host_words[9], n_cells = (int)h->host_words[10];
+    const int n_ev = evict ? (int)h->host_words[12] : 0;
     if (out->cycle_heads) out->cycle_heads[cyc] = n_live;
     if (out->cycle_admitted) out->cycle_admitted[cyc] = n_new;
-    out->n_cycles = cyc + 1; out->n_decisions += n_live; out->n_admitted += n_new;
-    A_cur += n_new; AU_cur += n_cells;
+    if (out->cycle_evicted) out->cycle_evicted[cyc] = n_ev;
+    out->n_cycles = cyc + 1; out->n_decisions += n_live; out->n_admitted += n_new; out->n_evicted += n_ev;
+    if (evict) {  // the compacted half becomes the admitted tables of the next cycle
+      A_cur = (int)h->host_words[13] + n_new; AU_cur = (int)h->host_words[14] + n_cells;
+      AdmTabs cur{X.adm_cq, X.adm_priority, X.adm_ts, X.adm_qr_ts, X.adm_uid, X.adm_evicted, X.adm_use_start, X.adm_use_fr, X.adm_use_qty, X.adm_wl};
+      X.adm_cq = other.cq; X.adm_priority = other.priority; X.adm_ts = other.ts; X.adm_qr_ts = other.qr_ts; X.adm_uid = other.uid;
+      X.adm_evicted = other.evicted; X.adm_use_start = other.use_start; X.adm_use_fr = other.use_fr; X.adm_use_qty = other.use_qty; X.adm_wl = other.wl;
+      D.adm_cq = X.adm_cq; D.adm_priority = X.adm_priority; D.adm_ts = X.adm_ts; D.adm_qr_ts = X.adm_qr_ts; D.adm_uid = X.adm_uid;
+      D.adm_evicted = X.adm_evicted; D.adm_use_start = X.adm_use_start; D.adm_use_fr = X.adm_use_fr; D.adm_use_qty = X.adm_use_qty;
+      other = cur;
+    } else {
+      A_cur += n_new; AU_cur += n_cells;
+    }
     n_live = (int)h->host_words[8];
-    if (n_new == 0) break;  // nothing admitted: the next cycle would see the same snapshot
+    if (n_new == 0 && n_ev == 0) break;  // nothing admitted or evicted: the next cycle would see the same snapshot
   }
   out->gpu_ms = gpu_ms;
   h->stats.last_cycle_gpu_ms = gpu_ms;
@@ -1538,6 +1622,10 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   if (out->wl_admit_cycle) CUDA_TRY(h, cudaMemcpyAsync(out->wl_admit_cycle, X.wl_admit_cycle, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
   if (out->wl_last_decision) CUDA_TRY(h, cudaMemcpyAsync(out->wl_last_decision, X.wl_last_decision, Wz, cudaMemcpyDeviceToHost, h->stream));
   if (out->wl_evals) CUDA_TRY(h, cudaMemcpyAsync(out->wl_evals, X.wl_evals, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (out->wl_evictions) {
+    if (replay) CUDA_TRY(h, cudaMemcpyAsync(out->wl_evictions, X.wl_evictions, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
+    else memset(out->wl_evictions, 0, Wz * 4);
+  }
   if (out->ps_flavor && PR) CUDA_TRY(h, cudaMemcpyAsync(out->ps_flavor, D.ps_flavor, PR, cudaMemcpyDeviceToHost, h->stream));
   if (out->ps_count && D.P) CUDA_TRY(h, cudaMemcpyAsync(out->ps_count, D.ps_count_out, (size_t)D.P * 4, cudaMemcpyDeviceToHost, h->stream));
   if (out->cq_usage) CUDA_TRY(h, cudaMemcpyAsync(out->cq_usage, D.cq_usage, (size_t)Q * FR * 8, cudaMemcpyDeviceToHost, h->stream));

@@ -5,11 +5,21 @@
 // 823-850 (requeueAndUpdate); pkg/workload/workload.go:161-191 (PendingFlavors, NextFlavorToTryForPodSetResource).
 //
 // The heaps of the reference become, per ClusterQueue, one segment of the pending workloads sorted once by
-// queueOrderingFunc (priority desc, queue-order timestamp, UID) plus a cursor: inside a drain nothing re-enters a
-// queue (no cluster events), so "pop the heap" is "first queued workload at or after the cursor that was not moved
-// to the inadmissible set".  Every cycle: pick the heads (ordered compaction over ClusterQueues), run the unchanged
-// cycle kernels on them, then apply the decisions — admissions extend the admitted tables and the ClusterQueue
-// usage on the device, the others keep their LastAssignment and move per the Strict / BestEffort FIFO rules.
+// queueOrderingFunc (priority desc, queue-order timestamp, UID) plus a cursor, and one state byte per workload
+// (KB_WS_QUEUED / KB_WS_SET_ASIDE: the inadmissible set / KB_WS_HELD: holds quota).  "Pop the heap" is "first QUEUED
+// workload in the static order": the cursor of a segment always points at it (no QUEUED workload lies before it).
+// Every cycle: pick the heads (ordered compaction over ClusterQueues), run the unchanged cycle kernels on them, then
+// apply the decisions — admissions extend the admitted tables and the ClusterQueue usage on the device, the others
+// keep their LastAssignment and move per the Strict / BestEffort FIFO rules.
+//
+// Eviction replay (kb_snapshot.adm_wl != NULL, a preemption policy somewhere): after the decisions, k_drain_evict
+// takes every target of every Preempting entry out of the ClusterQueue usage, flags its row dead and requeues its
+// pending record (LastAssignment nil; the cursor moves back to it if it lies before).  k_drain_requeue then returns
+// every set-aside workload of the ClusterQueues of the victims' root cohort trees to its queue, moving the cursor back
+// to the first of them (first_aside tracks that position per segment).  k_drain_live + two exclusive scans +
+// k_drain_compact copy the live rows, in order, into the other half of a double buffer, and k_drain_admit appends
+// the cycle's admissions after them.  A workload holds at most one live row, so the live rows never exceed the
+// capacity drain_impl reserves (kb_api.cu).
 //
 // AdmissionFairSharing (kb_snapshot.wl_lq != NULL): the queue of a ClusterQueue with cq_afs set is one SEGMENT per
 // LocalQueue (each sorted as above, each with its own cursor); every other ClusterQueue is one segment.  Segments are
@@ -17,6 +27,8 @@
 // cmp.Compare, -priority, timestamp, UID) over the heads of its segments (one warp per ClusterQueue, k_drain_afs_heads);
 // an admission adds its entry penalty to its LocalQueue and recomputes that LocalQueue's usage (k_drain_admit).
 #pragma once
+
+#include <cub/device/device_scan.cuh>
 
 #include "kb_device.cuh"
 
@@ -75,7 +87,8 @@ __host__ __device__ inline bool afs_lq_usage(const i64 *consumed, const int32_t 
 
 struct DrainDev {
   // queues
-  int32_t *q_order, *q_start, *cursor; uint8_t *gone;
+  int32_t *q_order, *q_start, *cursor; uint8_t *wl_state;  // wl_state: KB_WS_* per pending workload
+  int32_t *first_aside;                      // [S] smallest KB_WS_SET_ASIDE position of a segment (its length = none)
   int32_t *flag, *pos;                       // [Q+1] ClusterQueues with work left / their entry position
   int32_t *e_assumed, *e_ncells, *e_adm_off, *e_cell_off;  // [Hcap+1]
   int32_t *counters;                          // [0] entries of the next cycle
@@ -86,6 +99,15 @@ struct DrainDev {
   i64 *cq_usage, *wl_last_gen; int8_t *ps_last_tried;
   int32_t *adm_cq, *adm_priority; i64 *adm_ts, *adm_qr_ts, *adm_uid; uint8_t *adm_evicted; int32_t *adm_use_start, *adm_use_fr; i64 *adm_use_qty;
   int A, AU, cycle;  // admitted workloads / usage cells before this cycle's admissions
+  int A_cap, AU_cap; // capacity of the admitted tables (rows / usage cells)
+  // eviction replay; adm_wl == nullptr: off
+  int32_t *adm_wl;                 // [A_cap] pending record of each admitted row (current half)
+  int32_t *wl_seg, *wl_pos;        // [W] segment of a pending workload / its position in the segment
+  int32_t *adm_dead;               // [A_cap] cycle + 1 when the row was evicted in that cycle
+  int32_t *root_mark;              // [nRoots] cycle + 1 when the root cohort tree had a victim in that cycle
+  int32_t *wl_evictions;           // [W]
+  int32_t *row_live, *row_cells, *row_new, *cell_new;  // [A_cap + 1] compaction: flags / cells of live rows / their scans
+  uint8_t *wl_has_qr;              // mutable view of wl_has_quota_reservation (may be null)
   // AdmissionFairSharing; seg_start == nullptr: no AFS tables, segment = ClusterQueue
   const int32_t *seg_start;   // [Q+1] first segment of every ClusterQueue
   const int32_t *lq_seg;      // [n_lq] segment of a LocalQueue of an AFS ClusterQueue
@@ -124,10 +146,32 @@ __global__ void k_drain_keys_cq(DevSnap D, DrainDev X, const int32_t *vals, u64 
   keys[i] = ((u64)seg << 32) | (u64)(~((unsigned)D.wl_priority[w] ^ 0x80000000u));  // higher priority first
   atomicAdd(&q_count[seg], 1);
 }
+enum { KB_WS_QUEUED = 0, KB_WS_SET_ASIDE = 1, KB_WS_HELD = 2 };
 __global__ void k_drain_init(DevSnap D, DrainDev X, int S) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < D.W) { X.gone[i] = 0; X.wl_admit_cycle[i] = -1; X.wl_evals[i] = 0; X.wl_last_decision[i] = 0xff; }
-  if (i < S) X.cursor[i] = 0;
+  if (i < D.W) { X.wl_state[i] = KB_WS_QUEUED; X.wl_admit_cycle[i] = -1; X.wl_evals[i] = 0; X.wl_last_decision[i] = 0xff; }
+  if (i < D.W && X.wl_evictions) X.wl_evictions[i] = 0;
+  if (i < S) { X.cursor[i] = 0; X.first_aside[i] = X.q_start[i + 1] - X.q_start[i]; }
+}
+// replay: the records named by adm_wl hold quota (out of every queue); segment and position of every workload
+__global__ void k_drain_init_replay(DevSnap D, DrainDev X, int n_adm) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_adm) X.wl_state[X.adm_wl[i]] = KB_WS_HELD;
+  if (i < D.W) {
+    const int w = X.q_order[i];
+    const int cq = D.wl_cq[w];
+    const int seg = (X.seg_start && X.cq_afs[cq]) ? X.lq_seg[X.wl_lq[w]] : drain_seg0(X, cq);
+    X.wl_seg[w] = seg; X.wl_pos[w] = i - X.q_start[seg];
+  }
+}
+// the cursor of every segment at its first QUEUED workload (the start of a drain)
+__global__ void k_drain_advance(DrainDev X, int S) {
+  int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= S) return;
+  const int qs = X.q_start[s], qn = X.q_start[s + 1] - qs;
+  int cur = X.cursor[s];
+  while (cur < qn && X.wl_state[X.q_order[qs + cur]] != KB_WS_QUEUED) cur++;
+  X.cursor[s] = cur;
 }
 
 // heads of the next cycle (queues.Heads manager.go:770-794): one per ClusterQueue with work left, in ClusterQueue order.
@@ -215,6 +259,7 @@ __global__ void k_drain_apply(DevSnap D, DrainDev X) {
   bool pending_flavors = false;
   if (ok) {
     X.wl_admit_cycle[wl] = X.cycle;
+    X.wl_state[wl] = KB_WS_HELD;
     for (int row = ps0; row < ps1; row++)  // distinct flavor-resource cells of Assignment.Usage
       for (int r = 0; r < R; r++) {
         int f = D.ps_flavor[(size_t)row * R + r];
@@ -239,27 +284,34 @@ __global__ void k_drain_apply(DevSnap D, DrainDev X) {
     const i64 hsh = D.wl_sched_hash[wl];
     for (int s = s0; s < s1; s++) {
       const int qs = X.q_start[s], qn = X.q_start[s + 1] - qs;
-      for (int p = X.cursor[s] + (s == hs); p < qn; p++) { int w2 = X.q_order[qs + p]; if (D.wl_sched_hash[w2] == hsh) X.gone[w2] = 1; }
+      for (int p = X.cursor[s] + (s == hs); p < qn; p++) {
+        const int w2 = X.q_order[qs + p];
+        if (D.wl_sched_hash[w2] == hsh && X.wl_state[w2] == KB_WS_QUEUED) { X.wl_state[w2] = KB_WS_SET_ASIDE; X.first_aside[s] = min(X.first_aside[s], p); }
+      }
     }
   }
+  if (inadmissible && !strict) { X.wl_state[wl] = KB_WS_SET_ASIDE; X.first_aside[hs] = min(X.first_aside[hs], X.cursor[hs]); }
   if (ok || (inadmissible && !strict)) X.cursor[hs]++;
   for (int s = s0; s < s1; s++) {
     if (s != hs && !bulk) continue;
     const int qs = X.q_start[s], qn = X.q_start[s + 1] - qs;
     int cur = X.cursor[s];
-    while (cur < qn && X.gone[X.q_order[qs + cur]]) cur++;
+    while (cur < qn && X.wl_state[X.q_order[qs + cur]] != KB_WS_QUEUED) cur++;
     X.cursor[s] = cur;
   }
 }
 
 // admitted entries join the admitted tables (cache.AssumeWorkload) and the ClusterQueue usage
-__global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
+// (replay: after the compaction, base = {live rows, their cells} on the device; otherwise X.A / X.AU)
+__global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts, const int32_t *base) {
   int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= D.H || !X.e_assumed[e]) return;
   const int R = D.R;
   int wl = D.heads[e], cq = D.wl_cq[wl];
-  int a = X.A + X.e_adm_off[e];
-  int c0 = X.AU + X.e_cell_off[e];
+  int a = (base ? base[0] : X.A) + X.e_adm_off[e];
+  int c0 = (base ? base[1] : X.AU) + X.e_cell_off[e];
+  if (a >= X.A_cap || c0 + X.e_ncells[e] > X.AU_cap) { atomicOr(&X.counters[5], 1); return; }  // nothing past the end
+  if (X.adm_wl) X.adm_wl[a] = wl;
   X.adm_cq[a] = cq; X.adm_priority[a] = D.wl_priority[wl]; X.adm_ts[a] = D.wl_ts[wl]; X.adm_qr_ts[a] = qr_ts;
   X.adm_uid[a] = D.wl_uid[wl]; X.adm_evicted[a] = 0;
   X.adm_use_start[a] = c0;
@@ -302,4 +354,62 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
     X.lq_usage[lq] = u;
     if (bad) atomicOr(D.status, KBS_AFS_OVERFLOW);
   }
+}
+
+// ---- eviction replay ---------------------------------------------------------------------------------------------
+// every target of every Preempting entry (thread per entry): cells out of its ClusterQueue's usage (integer atomics:
+// the order does not matter), row dead, pending record QUEUED with LastAssignment nil, its root tree marked
+__global__ void k_drain_evict(DevSnap D, DrainDev X) {
+  int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= D.H || D.decision[e] != KB_DEC_PREEMPTING) return;
+  const int R = D.R, stamp = X.cycle + 1;
+  const int off = D.tgt_off[e], n = D.tgt_cnt[e];
+  for (int k = 0; k < n; k++) {
+    const int a = D.tgt_pool_adm[off + k];
+    if (atomicExch(&X.adm_dead[a], stamp) == stamp) continue;  // one eviction per row
+    const int cq = X.adm_cq[a];
+    for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)  // cache.DeleteWorkload
+      atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
+    const int w = X.adm_wl[a];
+    X.wl_state[w] = KB_WS_QUEUED;
+    X.wl_last_gen[w] = -1;
+    for (int i = D.wl_ps_start[w] * R; i < D.wl_ps_start[w + 1] * R; i++) X.ps_last_tried[i] = -1;
+    if (X.wl_has_qr) X.wl_has_qr[w] = 0;
+    X.wl_admit_cycle[w] = -1;
+    X.wl_evictions[w]++;  // a workload holds at most one row: one writer
+    atomicMin(&X.cursor[X.wl_seg[w]], X.wl_pos[w]);
+    X.root_mark[D.root_slot[cq]] = stamp;
+    atomicAdd(&X.counters[1], 1);
+  }
+}
+// inadmissible requeue (thread per ClusterQueue of a marked root): set aside -> queued, cursor back to the first of them
+__global__ void k_drain_requeue(DevSnap D, DrainDev X) {
+  int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= D.Q || X.root_mark[D.root_slot[q]] != X.cycle + 1) return;
+  for (int s = drain_seg0(X, q); s < drain_seg1(X, q); s++) {
+    const int qs = X.q_start[s], qn = X.q_start[s + 1] - qs, fa = X.first_aside[s];
+    for (int p = fa; p < qn; p++) { const int w = X.q_order[qs + p]; if (X.wl_state[w] == KB_WS_SET_ASIDE) X.wl_state[w] = KB_WS_QUEUED; }
+    X.cursor[s] = min(X.cursor[s], fa);
+    X.first_aside[s] = qn;
+  }
+}
+// compaction: live flags and cell counts of the rows before this cycle's admissions ([A] = 0 closes the scans)
+__global__ void k_drain_live(DrainDev X) {
+  int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a > X.A) return;
+  const bool live = a < X.A && X.adm_dead[a] != X.cycle + 1;
+  X.row_live[a] = live;
+  X.row_cells[a] = live ? X.adm_use_start[a + 1] - X.adm_use_start[a] : 0;
+}
+struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; };
+// live rows, in order, into the other half of the double buffer; thread A writes the totals (counters[2..3])
+__global__ void k_drain_compact(DrainDev X, AdmTabs O) {
+  int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a > X.A) return;
+  if (a == X.A) { O.use_start[X.row_new[a]] = X.cell_new[a]; X.counters[2] = X.row_new[a]; X.counters[3] = X.cell_new[a]; return; }
+  if (!X.row_live[a]) return;
+  const int n = X.row_new[a], c0 = X.cell_new[a], u0 = X.adm_use_start[a], nc = X.adm_use_start[a + 1] - u0;
+  O.cq[n] = X.adm_cq[a]; O.priority[n] = X.adm_priority[a]; O.ts[n] = X.adm_ts[a]; O.qr_ts[n] = X.adm_qr_ts[a];
+  O.uid[n] = X.adm_uid[a]; O.evicted[n] = X.adm_evicted[a]; O.wl[n] = X.adm_wl[a]; O.use_start[n] = c0;
+  for (int c = 0; c < nc; c++) { O.use_fr[c0 + c] = X.adm_use_fr[u0 + c]; O.use_qty[c0 + c] = X.adm_use_qty[u0 + c]; }
 }

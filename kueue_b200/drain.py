@@ -19,9 +19,32 @@ loop on the oracle and compares kb_run_drain with it cycle by cycle.
         workload.go:163-176) and otherwise go to the inadmissible set: the next workload becomes the head;
       - BestEffortFIFO, mode NoFit, known SchedulingHash: every queued workload of the same equivalence class moves to
         the inadmissible set as well (handleInadmissibleHash, cluster_queue.go:408-425; scheduler.go:292-300);
-  * the drain ends with the first cycle that admits nothing (no cluster event can change the outcome after that;
-    evictions are asynchronous in the reference and are not replayed: a Preempting entry keeps its place and its
-    targets stay admitted).
+  * the drain ends with the first cycle that admits nothing and evicts nothing (no cluster event can change the outcome
+    after that).  Without `adm_wl` evictions are not replayed: a Preempting entry keeps its place and its targets stay
+    admitted.
+
+Queue state: every pending workload is QUEUED, SET_ASIDE (the inadmissible set: BestEffortFIFO requeue or the hash
+bulk move) or HELD (holds quota: admitted in the drain, or named by `adm_wl`).  The head of a queue is its first QUEUED
+workload in the static order; the cursor of a segment is the position of that workload (no QUEUED workload before it).
+
+Eviction replay (the snapshot carries `adm_wl`, include/kueue_b200.h).  In the reference an eviction completes
+asynchronously (the job is suspended, the pods terminate); the drain takes the limit in which every eviction issued in
+cycle c completes before cycle c+1.  After cycle c, in this order:
+  1. the decisions are applied as above;
+  2. every target of every Preempting entry leaves the admitted tables (the QuotaReserved -> Pending transition of
+     workload_controller.go:973-1004): its cells leave its ClusterQueue's usage (cache.DeleteWorkload), its row is
+     removed (the other rows keep their order) and its pending record `adm_wl[row]` is QUEUED again with
+     LastAssignment nil (wl_last_gen = -1, ps_last_tried = -1, HasQuotaReservation false).  Preemption evictions set
+     no RequeueState (only PodsReady timeouts do, workload_controller.go:827-832), so the requeue is immediate.
+     Targets that already carried adm_evicted count too (IssuePreemptions, preemption.go:183-186); evictions under way
+     before the drain are not completed;
+  3. QueueAssociatedInadmissibleWorkloadsAfter (manager.go:670-697 -> notifyRetryInadmissibleWithoutLock,
+     inadmissible_workloads.go:128-223): for every root cohort with an evicted workload in its tree (the ClusterQueue
+     itself when it has no cohort) every SET_ASIDE workload of its ClusterQueues is QUEUED again, keeping its
+     LastAssignment; noFitSchedulingHashes is cleared with them (`requeue_inadmissible`);
+  4. the head of every queue in cycle c+1 is its first QUEUED workload: a requeued victim takes the place its
+     priority, timestamp and UID give it (with PrioritySortingWithinCohort the queue-order timestamp of a preempted
+     workload is its creation timestamp, workload.go:1174-1193, so the static order holds).
 
 AdmissionFairSharing (the snapshot carries `wl_lq` and the LocalQueue tables, include/kueue_b200.h): the queue of a
 ClusterQueue with `cq_afs` set is one segment per LocalQueue, each in the static order above with its own cursor.
@@ -54,6 +77,15 @@ class DrainResult:
     heads: List[np.ndarray] = field(default_factory=list)      # per cycle: global pending indices evaluated
     decisions: List[np.ndarray] = field(default_factory=list)  # per cycle: KB_DEC_* per entry
     cq_usage: np.ndarray | None = None                         # final ClusterQueue usage [Q][FR]
+    evicted: List[np.ndarray] = field(default_factory=list)    # per cycle: pending indices evicted (replay only)
+    wl_evictions: np.ndarray | None = None                     # [n_wl] times each pending record was evicted
+    wl_admit_cycle: np.ndarray | None = None                   # [n_wl] cycle of its last admission if it holds quota, else -1
+    state: np.ndarray | None = None                            # [n_wl] final QUEUED / SET_ASIDE / HELD
+    adm: dict | None = None                                    # final admitted tables (adm_* plus adm_wl when replaying)
+
+    @property
+    def n_evicted(self) -> int:
+        return int(sum(len(e) for e in self.evicted))
 
     @property
     def n_admitted(self) -> int:
@@ -97,6 +129,37 @@ def requeue_goes_inadmissible(strict_fifo: bool, reason: str, last_tried) -> boo
     else:
         immediate = reason in (REASON_FAILED_AFTER_NOMINATION, REASON_PENDING_PREEMPTION, "PreemptionFailed")
     return not (immediate or pending_flavors(last_tried))
+
+
+QUEUED, SET_ASIDE, HELD = 0, 1, 2  # per-workload queue state (kb_drain.cuh KB_WS_*)
+
+
+def root_of(parent) -> np.ndarray:
+    """Root node of every node of the cohort forest (a ClusterQueue without a cohort is its own root)."""
+    parent = np.asarray(parent, np.int64)
+    root = np.arange(len(parent))
+    for _ in range(len(parent)):
+        up = parent[root]
+        nxt = np.where(up >= 0, up, root)
+        if np.array_equal(nxt, root):
+            break
+        root = nxt
+    return root
+
+
+def requeue_inadmissible(parent, n_cq: int, notified, aside):
+    """QueueAssociatedInadmissibleWorkloads for the ClusterQueues `notified` (notifyRetryInadmissibleWithoutLock +
+    requeueWorkloadsCohort + queueInadmissibleWorkloads, inadmissible_workloads.go:128-223): every root of their cohort
+    trees is visited once, and every set-aside workload of every ClusterQueue of a visited tree returns to its queue
+    (the ClusterQueue's noFitSchedulingHashes are cleared with them).  `aside`: {cq: [workloads]}.
+    Returns ({cq: [workloads moved]}, visited roots in ascending order)."""
+    root = root_of(parent)
+    roots = sorted({int(root[int(q)]) for q in notified})
+    moved = {}
+    for q in range(n_cq):
+        if int(root[q]) in roots and aside.get(q):
+            moved[q] = list(aside[q])
+    return moved, roots
 
 
 class AfsOverflow(ValueError):
@@ -202,8 +265,29 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     Q, R, FR = snap.n_cq, snap.n_resource, snap.n_fr
     order, qstart, seg_start, seg_lq = _queue_order(a, Q)
     qlen = np.diff(qstart)
-    cursor = np.zeros(len(qlen), np.int64)
     afs_cq = a["cq_afs"].astype(bool) if "wl_lq" in a else np.zeros(Q, bool)
+    replay = "adm_wl" in a
+    state = np.full(snap.n_wl, QUEUED, np.uint8)
+    seg_of = np.zeros(snap.n_wl, np.int64)                        # segment of every pending workload
+    pos_of = np.zeros(snap.n_wl, np.int64)                        # its position in the segment's static order
+    for s in range(len(qlen)):
+        seg_of[order[qstart[s]:qstart[s + 1]]] = s
+        pos_of[order[qstart[s]:qstart[s + 1]]] = np.arange(qlen[s])
+    adm_wl = a["adm_wl"].astype(np.int64).copy() if replay else None
+    if replay:
+        state[adm_wl] = HELD  # holds quota: out of every queue
+    cursor = np.zeros(len(qlen), np.int64)
+    first_aside = qlen.copy()                                     # smallest SET_ASIDE position per segment (qlen = none)
+
+    def advance(s):
+        while cursor[s] < qlen[s] and state[order[qstart[s] + cursor[s]]] != QUEUED:
+            cursor[s] += 1
+
+    def set_aside(w):
+        state[w] = SET_ASIDE
+        first_aside[seg_of[w]] = min(first_aside[seg_of[w]], pos_of[w])
+    for s in range(len(qlen)):
+        advance(s)
     if afs_cq.any():
         L = len(a["lq_cq"])
         penalty = (a["lq_penalty"].reshape(L, R).astype(object) if "lq_penalty" in a else np.zeros((L, R), object))
@@ -238,8 +322,10 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     last_gen = a["wl_last_gen"].astype(np.int64).copy()          # LastAssignment.ClusterQueueGeneration, -1 = nil
     last_tried = a["ps_last_tried"].reshape(-1, R).copy()         # LastAssignment.LastTriedFlavorIdx
     shash = a.get("wl_sched_hash")
-    has_qr = a.get("wl_has_quota_reservation")
-    gone = np.zeros(snap.n_wl, bool)                              # moved to the inadmissible set by its scheduling hash
+    has_qr = a["wl_has_quota_reservation"].copy() if "wl_has_quota_reservation" in a else None
+    admit_cycle = np.full(snap.n_wl, -1, np.int64)
+    evictions = np.zeros(snap.n_wl, np.int64)
+    root = root_of(a["parent"])
     static = {k: v for k, v in a.items() if not (k.startswith(("wl_", "ps_", "adm_")) or k in ("heads", "cq_usage") + abi.AFS_FIELDS)}
     covers_pods = np.zeros(Q, bool)
     if snap.pods_resource >= 0:
@@ -312,6 +398,10 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         n_new = int(ok.sum())
         if n_new:
             g = heads[ok]
+            admit_cycle[g] = cyc
+            state[g] = HELD
+        if n_new:
+            g = heads[ok]
             adm["adm_cq"] = np.concatenate([adm["adm_cq"], a["wl_cq"][g]])
             adm["adm_priority"] = np.concatenate([adm["adm_priority"], a["wl_priority"][g]])
             adm["adm_ts"] = np.concatenate([adm["adm_ts"], a["wl_ts"][g]])
@@ -321,6 +411,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             adm["adm_use_start"] = np.concatenate([adm["adm_use_start"], np.asarray(new_start[1:], np.int32)])
             adm["adm_use_fr"] = np.concatenate([adm["adm_use_fr"], np.asarray(new_fr, np.int32)])
             adm["adm_use_qty"] = np.concatenate([adm["adm_use_qty"], np.asarray(new_qty, np.int64)])
+            if replay:
+                adm_wl = np.concatenate([adm_wl, g])
         # ---- LastAssignment of the entries that stay pending (scheduler.go:345,494)
         tried = np.asarray(out.ps_tried_idx).reshape(-1, R)
         cqs = live
@@ -339,22 +431,71 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 last = tried[r0:r1]
             # ---- queue movement (cluster_queue.go:362-425,609-633); a StrictFIFO queue keeps its head either way
             inadmissible[e] = requeue_goes_inadmissible(False, requeue_reason(int(dec[e])), last)
-        advance = ok | (inadmissible & ~strict[cqs])
+            if inadmissible[e] and not strict[cqs[e]]:
+                set_aside(w)
         if shash is not None:
             for e in np.flatnonzero((dec == abi.DEC_NOFIT) & ~strict[cqs]):
                 hsh = int(shash[heads[e]])
                 if hsh == 0:
                     continue
                 q = int(cqs[e])
-                for s in range(int(seg_start[q]), int(seg_start[q + 1])):  # every segment of the ClusterQueue's queue
+                for s in range(int(seg_start[q]), int(seg_start[q + 1])):  # every queued workload of the class, every segment
                     rest = order[qstart[s] + cursor[s] + (s == segs[e]):qstart[s + 1]]
-                    gone[rest[shash[rest] == hsh]] = True
-        cursor[segs[advance]] += 1
-        for q in cqs:  # the next head is the first queued workload that was not set aside
+                    for w in rest[(shash[rest] == hsh) & (state[rest] == QUEUED)]:
+                        set_aside(int(w))
+        for q in cqs:  # the next head is the first queued workload
             for s in range(int(seg_start[q]), int(seg_start[q + 1])):
-                while cursor[s] < qlen[s] and gone[order[qstart[s] + cursor[s]]]:
-                    cursor[s] += 1
-        if n_new == 0:
+                advance(s)
+        # ---- evictions (replay): every target of every Preempting entry, as rows of the tables the cycle saw
+        victims = []
+        if replay:
+            for e in np.flatnonzero(dec == abi.DEC_PREEMPTING):
+                victims.extend(int(out.tgt_adm[k]) for k in range(int(out.tgt_start[e]), int(out.tgt_start[e + 1])))
+            victims = sorted(set(victims))
+        res.evicted.append(np.sort(adm_wl[victims]) if victims else np.zeros(0, np.int64))
+        if victims:
+            us, uf, uq = adm["adm_use_start"], adm["adm_use_fr"], adm["adm_use_qty"]
+            notified = set()
+            for row in victims:
+                cqi, w = int(adm["adm_cq"][row]), int(adm_wl[row])
+                for k in range(int(us[row]), int(us[row + 1])):
+                    usage[cqi, int(uf[k])] -= int(uq[k])  # cache.DeleteWorkload
+                state[w] = QUEUED
+                last_gen[w] = -1
+                last_tried[int(ps_start[w]):int(ps_start[w + 1])] = -1
+                if has_qr is not None:
+                    has_qr[w] = 0
+                admit_cycle[w] = -1
+                evictions[w] += 1
+                cursor[seg_of[w]] = min(cursor[seg_of[w]], pos_of[w])
+                notified.add(cqi)
+            keep = np.ones(len(adm["adm_cq"]), bool)  # stable removal of the victims' rows
+            keep[victims] = False
+            cnt = np.diff(us.astype(np.int64))
+            cell_keep = np.repeat(keep, cnt)
+            for k in ("adm_cq", "adm_priority", "adm_ts", "adm_qr_ts", "adm_uid", "adm_evicted"):
+                adm[k] = adm[k][keep]
+            adm["adm_use_fr"], adm["adm_use_qty"] = uf[cell_keep], uq[cell_keep]
+            adm["adm_use_start"] = np.concatenate([[0], np.cumsum(cnt[keep])]).astype(np.int32)
+            adm_wl = adm_wl[keep]
+            # ---- inadmissible requeue in the root cohort trees of the victims
+            aside = {}
+            for q in range(Q):
+                for s in range(int(seg_start[q]), int(seg_start[q + 1])):
+                    seg = order[qstart[s] + first_aside[s]:qstart[s + 1]]
+                    aside.setdefault(q, []).extend(int(w) for w in seg[state[seg] == SET_ASIDE])
+            moved, roots = requeue_inadmissible(a["parent"], Q, sorted(notified), aside)
+            for ws in moved.values():
+                state[np.asarray(ws, np.int64)] = QUEUED
+            for q in np.flatnonzero(np.isin(root[:Q], roots)):
+                for s in range(int(seg_start[q]), int(seg_start[q + 1])):
+                    cursor[s] = min(cursor[s], first_aside[s])
+                    first_aside[s] = qlen[s]
+        if n_new == 0 and not victims:
             break
     res.cq_usage = usage
+    res.wl_evictions = evictions
+    res.wl_admit_cycle = admit_cycle
+    res.state = state
+    res.adm = dict(adm, **({"adm_wl": adm_wl} if replay else {}))
     return res

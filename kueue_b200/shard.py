@@ -125,6 +125,8 @@ def shard(snap: abi.FlatSnapshot, rank: int, world: int, node_rank: np.ndarray |
     us, ui = _csr_take(a["adm_use_start"].astype(np.int64), adms)
     out.set("adm_use_start", us)
     out.set("adm_use_fr", a["adm_use_fr"][ui]); out.set("adm_use_qty", a["adm_use_qty"][ui])
+    if "adm_wl" in a:  # eviction replay: a record lives with its ClusterQueue, as does its admitted row
+        out.set("adm_wl", wl_remap[a["adm_wl"][adms]])
     if "wl_lq" in a:  # AdmissionFairSharing: the LocalQueues travel with their ClusterQueues (still ClusterQueue-major)
         L = len(a["lq_cq"])
         lqs = np.flatnonzero(node_rank[a["lq_cq"]] == rank) if L else np.zeros(0, np.int64)

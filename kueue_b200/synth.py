@@ -29,14 +29,16 @@ def _cohort_forest(n_root: int, fanouts, cqs_per_leaf: int):
 def make_snapshot(config: int = 2, W: int | None = None, Q: int | None = None, F: int | None = None,
                   R: int | None = None, seed: int | None = None, heads: str = "all",
                   podsets_max: int = 1, admitted: int | None = None, preemption: bool | None = None,
-                  partial: bool = False, tight: float = 1.0, afs: int = 0) -> abi.FlatSnapshot:
+                  partial: bool = False, tight: float = 1.0, afs: int = 0, evictable: bool = False) -> abi.FlatSnapshot:
     """config 1: 100 wl x 10 CQ x 2 flavors x 3 resources, no cohort
        config 2: 100k x 1k x 8 x 4, StrictFIFO, no cohort, usage 60-90% of nominal
        config 3: 1M x 10k, 100 flat cohorts x 100 CQ, BestEffortFIFO, fair sharing
        config 4: 1M x 10k, depth-4 cohort forest (10 -> 5 -> 5 -> 4), classical
     heads: "all" (batched evaluator over every pending workload) | "one_per_cq"
     (reference cycle: the best-ordered workload of each CQ).
-    afs: k > 0 gives every ClusterQueue k LocalQueues with UsageBasedAdmissionFairSharing (see `add_afs`)."""
+    afs: k > 0 gives every ClusterQueue k LocalQueues with UsageBasedAdmissionFairSharing (see `add_afs`).
+    evictable: every admitted workload also gets a pending record and `adm_wl` names it (see `add_evictable`): a drain
+    replays the evictions of its preemptions."""
     dflt = {1: (100, 10, 2, 3), 2: (100_000, 1_000, 8, 4), 3: (1_000_000, 10_000, 8, 4), 4: (1_000_000, 10_000, 8, 4)}[config]
     W = W or dflt[0]; Q = Q or dflt[1]; F = F or dflt[2]; R = R or dflt[3]
     rng = np.random.Generator(np.random.PCG64(config if seed is None else seed))
@@ -150,10 +152,12 @@ def make_snapshot(config: int = 2, W: int | None = None, Q: int | None = None, F
         snap.set("ps_min_count", mc)
     ok = rng.integers(0, 2**63, P, dtype=np.uint64) | rng.integers(0, 2**63, P, dtype=np.uint64) | np.uint64(1 << (F - 1))
     snap.set("ps_flavor_ok", ok)  # ~75% of flavors eligible, last flavor always
+    if evictable:
+        add_evictable(snap)
     if afs:
         add_afs(snap, afs, seed=(config if seed is None else seed) + 1000)
     if heads == "all":
-        snap.set("heads", np.arange(W))
+        snap.set("heads", np.arange(snap.n_wl))
     else:
         # reference Heads(): per CQ the first in (priority desc, ts asc, uid) order (cluster_queue.go:636-685)
         order = np.lexsort((snap.wl_uid, snap.wl_ts, -snap.wl_priority, snap.wl_cq))
@@ -214,4 +218,35 @@ def add_afs(snap: abi.FlatSnapshot, k: int, seed: int = 0, half_life_s: float = 
     snap.set("afs_res_weight", rng.choice([0.5, 1.0, 2.0], R))
     snap.set("afs_milli_mul", np.where(np.arange(R) == 0, 1, 1000))
     snap.afs_alpha = 1.0 - 0.5 ** (sampling_s / half_life_s) if half_life_s else 0.0
+    return snap
+
+
+def add_evictable(snap: abi.FlatSnapshot) -> abi.FlatSnapshot:
+    """Give every admitted workload a pending record consistent with its usage and name it in `adm_wl`
+    (include/kueue_b200.h): same ClusterQueue, priority, queue-order timestamp and UID, one podset of count 1 whose
+    requests are the workload's usage cells (every flavor eligible).  The records are appended after the existing
+    pending workloads; admitted UIDs and pending UIDs stay distinct."""
+    a = snap.arrays
+    R, A, W = snap.n_resource, snap.n_adm, snap.n_wl
+    use_start = a["adm_use_start"].astype(np.int64)
+    req = np.zeros((A, R), np.int64)
+    rows = np.repeat(np.arange(A), np.diff(use_start))
+    np.add.at(req, (rows, a["adm_use_fr"].astype(np.int64) % R), a["adm_use_qty"])
+    mask = np.zeros(A, np.int64)
+    np.bitwise_or.at(mask, rows, 1 << (a["adm_use_fr"].astype(np.int64) % R))
+    P = int(a["wl_ps_start"][-1]) if W else 0
+    cat = lambda name, extra: snap.set(name, np.concatenate([a[name], np.asarray(extra).astype(a[name].dtype)]))  # noqa: E731
+    cat("wl_cq", a["adm_cq"]); cat("wl_priority", a["adm_priority"]); cat("wl_ts", a["adm_ts"]); cat("wl_uid", a["adm_uid"])
+    cat("wl_ps_start", P + 1 + np.arange(A))
+    snap.set("ps_req", np.concatenate([a["ps_req"].reshape(-1, R), req]))
+    cat("ps_req_mask", mask); cat("ps_count", np.ones(A))
+    cat("ps_flavor_ok", np.full(A, np.iinfo(np.uint64).max, np.uint64))
+    if "ps_last_tried" in a:
+        snap.set("ps_last_tried", np.concatenate([a["ps_last_tried"].reshape(-1, R), np.full((A, R), -1)]))
+    for name, fill in (("wl_last_gen", -1), ("ps_min_count", -1), ("wl_sched_hash", 0), ("wl_has_quota_reservation", 0)):
+        if name in a:
+            cat(name, np.full(A, fill))
+    if "ps_group" in a:
+        cat("ps_group", np.full(A, -1))
+    snap.set("adm_wl", W + np.arange(A))
     return snap
