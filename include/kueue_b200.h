@@ -266,6 +266,20 @@ typedef struct kb_snapshot {
      wl_cq[adm_wl[a]] != adm_cq[a]; KB_ERR_UNSUPPORTED without KB_F_PRIORITY_SORTING_WITHIN_COHORT (a preempted
      workload's queue-order timestamp would become its eviction time, workload.go:1174-1193). */
   const int32_t *adm_wl;            /* [n_adm] */
+
+  /* ---- arrivals and completions: event mode (optional; read by kb_run_drain only, kb_run_cycle ignores them) ----
+     The reference's scheduler performance runner (test/performance/scheduler) creates workloads at fixed intervals
+     (runner/generator/generator.go) and finishes each one runtimeMs after its admission (runner/controller/
+     controller.go:100-160; an eviction restarts that clock, setAdmittedTime :62-72).  A finish is
+     workload_controller.go:936-952: the workload leaves the cache and QueueAssociatedInadmissibleWorkloadsAfter
+     requeues its root cohort tree (the same step as an eviction).  A creation is AddOrUpdateWorkload -> PushOrUpdate
+     (manager.go:524-560), which requeues nothing else.  "Event mode" = at least one of the three tables is non-NULL;
+     without them kb_run_drain is unchanged.  INT64_MAX as a time means never.  Errors (KB_ERR_INVALID):
+     adm_finish_ns[a] <= now_ns, adm_wl naming a record with wl_create_ns > now_ns. */
+  int64_t drain_cycle_ns;           /* simulated time one cycle takes; <= 0 means 1 (cycle c at now_ns + c)         */
+  const int64_t *wl_create_ns;      /* [n_wl] creation time; <= now_ns: present at the start; NULL = all present    */
+  const int64_t *wl_run_ns;         /* [n_wl] run time once admitted; < 0: never finishes; NULL = none finishes     */
+  const int64_t *adm_finish_ns;     /* [n_adm] finish time of each row admitted before the drain; NULL = never      */
 } kb_snapshot;
 
 /* ------------------------------------------------------------------------
@@ -407,7 +421,32 @@ int32_t kb_download(kb_handle *h, kb_cycle_out *out);
  * cmp.Compare — NaN first —, -priority, timestamp, UID) among the segments' heads, and every admission adds its entry
  * penalty to its LocalQueue before the next cycle.  StrictFIFO keeps the head (the next cycle picks the minimum again),
  * BestEffortFIFO advances the head's own segment, the scheduling-hash move covers every segment of the ClusterQueue.
- * Consumed usage does not decay inside a drain (CalculateDecayedConsumed is the LocalQueue reconciler's). */
+ * Consumed usage does not decay inside a drain (CalculateDecayedConsumed is the LocalQueue reconciler's).
+ *
+ * Event mode (kb_snapshot.wl_create_ns / wl_run_ns / adm_finish_ns, any non-NULL): a simulated clock t starts at
+ * now_ns; cycle c runs at t_c (its now_ns and the QuotaReserved time of its admissions).  Two more queue states:
+ * ABSENT (created after t, in no queue) and FINISHED (never requeued).  A pending event is the finish time of a live
+ * admitted row or the creation time of an ABSENT workload.  The loop:
+ *   1. no queue has a head: t jumps to E, the earliest pending event, and steps 5-7 apply the events at E (no cycle is
+ *      counted); without E the drain ends;
+ *   2. cycle c runs at t_c and its decisions are applied as above; 3. evictions are replayed as above (adm_wl);
+ *   4. a cycle that admitted or evicted: t_{c+1} = t_c + drain_cycle_ns; a quiet cycle (the stop rule of the plain
+ *      drain) waits instead: t_{c+1} = max(t_c + drain_cycle_ns, E), and without E the drain ends;
+ *   5. every live row with finish <= t_{c+1} finishes (a row admitted at t finishes at t + wl_run_ns, saturating; one
+ *      admitted in cycle c that finishes by t_{c+1} never enters the tables): its cells leave its ClusterQueue's usage,
+ *      its row is removed, its record (adm_wl for the rows of the snapshot) becomes FINISHED, its root tree is marked;
+ *   6. every ABSENT workload with create <= t_{c+1} joins its queue, except that in a BestEffortFIFO ClusterQueue a
+ *      workload whose known wl_sched_hash is in the ClusterQueue's NoFit set goes straight to the inadmissible set
+ *      (PushOrUpdate, cluster_queue.go:288-293).  The NoFit set holds the hashes of the NoFit heads since the
+ *      ClusterQueue's last inadmissible requeue (handleInadmissibleHash :414; cleared by queueInadmissibleWorkloads,
+ *      inadmissible_workloads.go:174);
+ *   7. the inadmissible requeue of step 3 runs over every root tree marked in steps 3 or 5;  8. heads of cycle c+1.
+ * Steps 5-7 only set state bytes and lower cursors: their order does not change the result.  A quiet cycle waiting for
+ * the next event is the canonical choice; with every run time < 0 and every creation <= now_ns the drain equals the
+ * plain drain.  An evicted workload loses its finish time; a readmission restarts the full run time.  The clock is
+ * global (a quiet cycle depends on every root), so event drains are not sharded.  max_cycles counts cycles; the drain
+ * stops before running cycle max_cycles.  Events applied before cycle 0 count in n_finished / n_arrived only; the
+ * events applied between the start of cycle c and the start of cycle c+1 count in cycle_finished / cycle_arrived[c]. */
 typedef struct kb_drain_out {
   int32_t max_cycles;        /* in */
   int32_t n_cycles;          /* out: cycles run */
@@ -432,6 +471,15 @@ typedef struct kb_drain_out {
   int64_t n_evicted;         /* out: evictions over all cycles */
   int32_t *cycle_evicted;    /* [max_cycles] evictions per cycle (may be NULL) */
   int32_t *wl_evictions;     /* [n_wl] times each pending record was evicted (may be NULL) */
+  /* event mode (zero / unset otherwise; every pointer may be NULL) */
+  int64_t n_finished;        /* out: completions applied */
+  int64_t n_arrived;         /* out: arrivals applied */
+  int64_t end_ns;            /* out: the clock when the drain stopped (last cycle start or last event applied) */
+  int64_t *cycle_start_ns;   /* [max_cycles] t_c */
+  int32_t *cycle_finished;   /* [max_cycles] completions applied from the start of cycle c to the start of c+1 */
+  int32_t *cycle_arrived;    /* [max_cycles] arrivals, likewise */
+  int64_t *wl_admit_ns;      /* [n_wl] time of the workload's last admission, INT64_MIN if never admitted */
+  int64_t *wl_finish_ns;     /* [n_wl] finish time, INT64_MAX if it has not finished */
 } kb_drain_out;
 int32_t kb_run_drain(kb_handle *h, const kb_snapshot *s, kb_drain_out *out);
 

@@ -358,6 +358,10 @@ func (s *Scheduler) flatten(snap *schdcache.Snapshot, heads []workload.Info, gen
 	// it would be requeued) and keep its index:
 	//   admWl[a] = int32(len(wlCq)); wlCq = append(wlCq, admCq[a]); ...   then c.adm_wl = cp32(admWl)
 	// This shim runs single cycles and leaves c.adm_wl nil.
+	// Arrivals and completions in kb_run_drain (INTEGRATION.md): a queue simulation fills one creation time per pending
+	// workload and one run time, plus one finish time per admitted workload, and the length of one cycle:
+	//   c.wl_create_ns, c.wl_run_ns, c.adm_finish_ns = cp64(wlCreate), cp64(wlRun), cp64(admFinish); c.drain_cycle_ns = C.int64_t(cycleNs)
+	// They stay nil here: a single cycle ignores them.
 	if anyGroup { // optional table: NULL when no podset is grouped
 		c.ps_group = cp32(psGroup)
 	}

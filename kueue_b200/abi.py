@@ -78,6 +78,8 @@ class kb_snapshot(C.Structure):
         ("lq_penalty", _P(C.c_int64)), ("afs_res_weight", _P(C.c_double)), ("afs_milli_mul", _P(C.c_int64)),
         ("afs_alpha", C.c_double),
         ("adm_wl", _P(C.c_int32)),
+        ("drain_cycle_ns", C.c_int64), ("wl_create_ns", _P(C.c_int64)), ("wl_run_ns", _P(C.c_int64)),
+        ("adm_finish_ns", _P(C.c_int64)),
     ]
 
 
@@ -122,6 +124,9 @@ class kb_drain_out(C.Structure):
         ("trace_wl", _P(C.c_int32)), ("trace_decision", _P(C.c_uint8)), ("trace_capacity", C.c_int64),
         ("gpu_ms", C.c_double),
         ("n_evicted", C.c_int64), ("cycle_evicted", _P(C.c_int32)), ("wl_evictions", _P(C.c_int32)),
+        ("n_finished", C.c_int64), ("n_arrived", C.c_int64), ("end_ns", C.c_int64),
+        ("cycle_start_ns", _P(C.c_int64)), ("cycle_finished", _P(C.c_int32)), ("cycle_arrived", _P(C.c_int32)),
+        ("wl_admit_ns", _P(C.c_int64)), ("wl_finish_ns", _P(C.c_int64)),
     ]
 
 
@@ -174,11 +179,14 @@ _DT = {
     "wl_lq": np.int32, "lq_cq": np.int32, "cq_afs": np.uint8, "lq_weight": np.float64, "lq_consumed": np.int64,
     "lq_consumed_scale": np.int32, "lq_penalty": np.int64, "afs_res_weight": np.float64, "afs_milli_mul": np.int64,
     "adm_wl": np.int32,
+    "wl_create_ns": np.int64, "wl_run_ns": np.int64, "adm_finish_ns": np.int64,
 }
 # AdmissionFairSharing tables (include/kueue_b200.h): wl_lq absent = AFS off
 AFS_FIELDS = ("wl_lq", "lq_cq", "cq_afs", "lq_weight", "lq_consumed", "lq_consumed_scale", "lq_penalty", "afs_res_weight",
               "afs_milli_mul")
-OPTIONAL_FIELDS = ("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows", "adm_wl") + AFS_FIELDS  # NULL in kb_snapshot when absent
+# arrivals and completions of kb_run_drain's event mode (include/kueue_b200.h): all absent = event mode off
+EVENT_FIELDS = ("wl_create_ns", "wl_run_ns", "adm_finish_ns")
+OPTIONAL_FIELDS = ("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows", "adm_wl") + AFS_FIELDS + EVENT_FIELDS  # NULL in kb_snapshot when absent
 ARRAY_FIELDS = list(_DT.keys())
 # tables the library keeps resident while kb_snapshot.static_generation is unchanged (include/kueue_b200.h)
 STATIC_FIELDS = ("parent", "fair_weight", "nominal", "borrow_limit", "lend_limit", "cq_within_cq", "cq_reclaim_within",
@@ -190,6 +198,7 @@ def _ptr(arr: np.ndarray, ctype):
     return arr.ctypes.data_as(_P(ctype))
 
 
+_EMPTY = {dt: np.zeros(1, dt) for dt in set(_DT.values())}  # one-element buffers behind empty optional tables
 _CT = {np.int32: C.c_int32, np.int64: C.c_int64, np.uint8: C.c_uint8, np.uint32: C.c_uint32,
        np.uint64: C.c_uint64, np.int8: C.c_int8, np.float64: C.c_double}
 
@@ -206,6 +215,7 @@ class FlatSnapshot:
     now_ns: int = 0
     static_generation: int = 0
     afs_alpha: float = 0.0  # kb_snapshot.afs_alpha: entry-penalty rate of AdmissionFairSharing
+    drain_cycle_ns: int = 0  # kb_snapshot.drain_cycle_ns: simulated time of one drain cycle (<= 0 means 1)
     arrays: dict = field(default_factory=dict)
 
     def __getattr__(self, name):
@@ -300,6 +310,7 @@ class FlatSnapshot:
             s = self._struct
             s.flags, s.now_ns, s.static_generation = self.flags, self.now_ns, self.static_generation
             s.afs_alpha = self.afs_alpha
+            s.drain_cycle_ns = self.drain_cycle_ns
             return s
         s = kb_snapshot()
         s.n_cq, s.n_cohort, s.n_flavor, s.n_resource = self.n_cq, self.n_cohort, self.n_flavor, self.n_resource
@@ -311,10 +322,13 @@ class FlatSnapshot:
         s.static_generation = self.static_generation
         s.n_lq = len(self.arrays["lq_cq"]) if "lq_cq" in self.arrays else 0
         s.afs_alpha = self.afs_alpha
+        s.drain_cycle_ns = self.drain_cycle_ns
         for name in ARRAY_FIELDS:
             if name in OPTIONAL_FIELDS and name not in self.arrays:
                 continue  # stays NULL
             arr = self.arrays[name]
+            if arr.size == 0 and name in OPTIONAL_FIELDS:
+                arr = _EMPTY[_DT[name]]  # a present empty table (adm_wl with n_adm = 0) must not read as NULL
             setattr(s, name, _ptr(arr, _CT[_DT[name]]))
         s._keepalive = self  # noqa: keep numpy buffers alive with the struct
         self._struct = s
@@ -377,7 +391,7 @@ class TreeOut:
 class DrainOut:
     """Caller-allocated output buffers of kb_run_drain."""
 
-    def __init__(self, snap: FlatSnapshot, max_cycles: int = 10_000, trace: bool = True):
+    def __init__(self, snap: FlatSnapshot, max_cycles: int = 10_000, trace: bool = True, trace_capacity: int | None = None):
         W, Q, R = snap.n_wl, snap.n_cq, snap.n_resource
         self.max_cycles = max_cycles
         self.cycle_heads = np.zeros(max_cycles, np.int32)
@@ -390,7 +404,12 @@ class DrainOut:
         self.cq_usage = np.zeros((Q, snap.n_fr), np.int64)
         self.cycle_evicted = np.zeros(max_cycles, np.int32)
         self.wl_evictions = np.zeros(W, np.int32)
-        cap = min(W * 4 + Q, min(Q, W) * max_cycles) if trace else 0
+        self.cycle_start_ns = np.zeros(max_cycles, np.int64)
+        self.cycle_finished = np.zeros(max_cycles, np.int32)
+        self.cycle_arrived = np.zeros(max_cycles, np.int32)
+        self.wl_admit_ns = np.full(W, KB_TS_UNSET, np.int64)
+        self.wl_finish_ns = np.full(W, KB_NO_LIMIT, np.int64)
+        cap = (min(W * 4 + Q, min(Q, W) * max_cycles) if trace_capacity is None else trace_capacity) if trace else 0
         self.trace_wl = np.zeros(max(1, cap), np.int32)
         self.trace_decision = np.zeros(max(1, cap), np.uint8)
         s = kb_drain_out()
@@ -401,6 +420,9 @@ class DrainOut:
         s.ps_flavor = _ptr(self.ps_flavor, C.c_int8); s.ps_count = _ptr(self.ps_count, C.c_int32)
         s.cq_usage = _ptr(self.cq_usage, C.c_int64)
         s.cycle_evicted = _ptr(self.cycle_evicted, C.c_int32); s.wl_evictions = _ptr(self.wl_evictions, C.c_int32)
+        s.cycle_start_ns = _ptr(self.cycle_start_ns, C.c_int64)
+        s.cycle_finished = _ptr(self.cycle_finished, C.c_int32); s.cycle_arrived = _ptr(self.cycle_arrived, C.c_int32)
+        s.wl_admit_ns = _ptr(self.wl_admit_ns, C.c_int64); s.wl_finish_ns = _ptr(self.wl_finish_ns, C.c_int64)
         if trace:
             s.trace_wl = _ptr(self.trace_wl, C.c_int32); s.trace_decision = _ptr(self.trace_decision, C.c_uint8)
         s.trace_capacity = cap
@@ -416,6 +438,12 @@ class DrainOut:
     def gpu_ms(self): return float(self.struct.gpu_ms)
     @property
     def n_evicted(self): return int(self.struct.n_evicted)
+    @property
+    def n_finished(self): return int(self.struct.n_finished)
+    @property
+    def n_arrived(self): return int(self.struct.n_arrived)
+    @property
+    def end_ns(self): return int(self.struct.end_ns)
 
     def cycles(self):
         """[(heads, decisions)] per cycle from the trace."""

@@ -87,6 +87,7 @@ struct kb_handle {
   int sa_list_cap = 32, sb_list_cap = 32;
   // kb_run_drain: capacity reserved beyond the snapshot's admitted tables, heads chosen on the device
   size_t drain_extra_adm = 0, drain_extra_au = 0; bool drain_mode = false; bool preempt_possible = true;
+  bool drain_events = false;  // kb_run_drain in event mode: rows admitted during the drain are preemption candidates
   char *drain_buf = nullptr; size_t drain_buf_cap = 0; cudaEvent_t ev_d = nullptr;
   char *tas_buf = nullptr; size_t tas_buf_cap = 0;
   bool fused_on = false; size_t fused_smem = 0; bool one_head_per_cq = false; int32_t *d_cq_entry = nullptr;
@@ -881,7 +882,7 @@ static int32_t upload_impl(kb_handle *h, const kb_snapshot *s, bool sync) {
     size_t nnm = (size_t)h->max_tree_nodes, tbm = nnm * FR;
     size_t sm = 6 * tbm * 8 + 2 * nnm * R * 8 + 4 * nnm * 4 + 7 * KB_TILE * 4 + (KB_MAX_DEPTH + 2 + 4) * 4 + 32 + nnm * 32;
     h->fused_smem = sm;
-    h->fused_on = D.nLone == 0 && D.nTrees > 0 && h->one_head_per_cq && sm <= 220 * 1024 && (A_in == 0 || !h->preempt_possible) &&
+    h->fused_on = D.nLone == 0 && D.nTrees > 0 && h->one_head_per_cq && sm <= 220 * 1024 && ((A_in == 0 && !h->drain_events) || !h->preempt_possible) &&
                   (!(s->flags & KB_F_FAIR_SHARING) || all_flat) && getenv("KB_NO_FUSED") == nullptr;
     // k_cycle_flat: every tree flat, FR <= 64, the relocated copy of the largest root fits shared memory
     h->d_cq_rec = h->arena.take<int4>(h->tree_nodes.size() + 1); D.cq_rec = h->d_cq_rec;
@@ -1352,6 +1353,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   const int Hcap = std::min(Q, W);
   const int max_cycles = std::max(0, out->max_cycles);
   out->n_cycles = 0; out->n_decisions = 0; out->n_admitted = 0; out->gpu_ms = 0; out->n_evicted = 0;
+  out->n_finished = 0; out->n_arrived = 0; out->end_ns = s->now_ns;
   // ---- eviction replay: host-side checks of adm_wl (include/kueue_b200.h)
   const bool replay = s->adm_wl != nullptr;
   if (replay) {
@@ -1366,11 +1368,22 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       if (s->adm_cq[a] < 0 || s->adm_cq[a] >= Q || s->wl_cq[w] != s->adm_cq[a]) return fail(h, KB_ERR_INVALID, "adm_wl: the record's ClusterQueue is not the admitted workload's");
     }
   }
+  // ---- event mode: host-side checks of the arrival and completion tables (include/kueue_b200.h)
+  const bool events = s->wl_create_ns || s->wl_run_ns || s->adm_finish_ns;
+  if (events) {
+    if (s->adm_finish_ns)
+      for (int a = 0; a < s->n_adm; a++)
+        if (s->adm_finish_ns[a] <= s->now_ns) return fail(h, KB_ERR_INVALID, "adm_finish_ns: a row admitted before the drain finishes at or before now_ns");
+    if (replay && s->wl_create_ns)
+      for (int a = 0; a < s->n_adm; a++)
+        if (s->wl_create_ns[s->adm_wl[a]] > s->now_ns) return fail(h, KB_ERR_INVALID, "adm_wl names a record created after now_ns");
+  }
   if (Hcap == 0 || max_cycles == 0) return KB_OK;
   size_t extra = (size_t)std::min<long long>((long long)W, (long long)Hcap * max_cycles);
   h->drain_extra_adm = extra;
   h->drain_extra_au = std::min<size_t>((size_t)s->n_podset * R, extra * (size_t)FR);
   h->drain_mode = true;
+  h->drain_events = events;
   kb_snapshot s2 = *s;
   s2.n_heads = Hcap; s2.heads = nullptr;
   int32_t rc = upload_impl(h, &s2, false);
@@ -1383,6 +1396,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   const int L = afs ? s->n_lq : 0;
   // evictions happen only where a target search can: without a preemption policy adm_wl only keeps its records queued-out
   const bool evict = replay && h->preempt_possible;
+  const bool compact = evict || events;  // rows can die: the admitted tables are compacted after every boundary
   std::vector<int32_t> seg_start, lq_seg, seg_lq, afs_cqs;
   std::vector<double> lq_usage;
   int S = Q;
@@ -1427,12 +1441,35 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   // cells <= AU_in + min(P * R, that bound * FR) (a readmitted victim's old cells left with its old row)
   const size_t Acap = (size_t)s->n_adm + h->drain_extra_adm, AUcap = (size_t)s->n_adm_use + h->drain_extra_au;
   size_t scan_bytes = 0;
-  if (evict) cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (int32_t *)nullptr, (int32_t *)nullptr, (int)Acap + 1, h->stream);
+  if (compact) cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (int32_t *)nullptr, (int32_t *)nullptr, (int)Acap + 1, h->stream);
   const size_t nR = (size_t)std::max(1, D.nRoots);
-  if (replay) { need(Acap, 4); need(Wz, 4); need(Wz, 4); need(Wz, 4); need(Sz, 4); }
-  if (evict) {
+  if (replay || events) { need(Acap, 4); need(Wz, 4); need(Wz, 4); need(Wz, 4); need(Sz, 4); }
+  if (compact) {
     need(Acap, 4); need(Acap, 4); need(nR, 4); for (int k = 0; k < 4; k++) need(Acap + 1, 4); need(scan_bytes + 256, 1);
     need(Acap, 4); need(Acap, 4); need(Acap, 8); need(Acap, 8); need(Acap, 8); need(Acap, 1); need(Acap + 1, 4); need(AUcap, 4); need(AUcap, 8);
+  }
+  // event mode: finish columns of both halves, run times, admit / finish times, the clock, the arrival order (sorted
+  // pairs and their double buffers) and the NoFit classes
+  std::vector<int32_t> wl_class, cq_class_start;
+  int n_class = 0;
+  if (events && s->wl_create_ns && s->wl_sched_hash) {  // dense class id per (BestEffortFIFO ClusterQueue, known hash)
+    std::vector<std::pair<std::pair<int32_t, int64_t>, int32_t>> cls;
+    for (int w = 0; w < W; w++)
+      if (s->wl_sched_hash[w] != 0 && s->cq_strategy[s->wl_cq[w]] != KB_QUEUE_STRICT_FIFO) cls.push_back({{s->wl_cq[w], s->wl_sched_hash[w]}, w});
+    std::sort(cls.begin(), cls.end());
+    wl_class.assign(Wz, -1); cq_class_start.assign((size_t)Q + 1, 0);
+    for (size_t i = 0; i < cls.size(); i++) {
+      if (i > 0 && cls[i].first != cls[i - 1].first) n_class++;
+      wl_class[cls[i].second] = n_class;
+      cq_class_start[cls[i].first.first + 1] = n_class + 1;
+    }
+    if (!cls.empty()) n_class++;
+    for (int q = 0; q < Q; q++) cq_class_start[q + 1] = std::max(cq_class_start[q + 1], cq_class_start[q]);
+  }
+  if (events) {
+    need(Acap, 8); need(Acap, 8); need(Wz, 8); need(Wz, 8); need(Wz, 8); need(4, 8);
+    if (s->wl_create_ns) { need(Wz, 8); need(Wz, 8); need(Wz, 4); need(Wz, 4); need(Wz, 8); }
+    if (n_class) { need(Wz, 4); need((size_t)Q + 1, 4); need((size_t)n_class, 1); }
   }
   if (!replay) need(Sz, 4);
   if (afs) {
@@ -1470,13 +1507,14 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   X.A_cap = (int)Acap; X.AU_cap = (int)AUcap;
   AdmTabs other{};  // replay: the other half of the admitted tables' double buffer
   void *scan_tmp = nullptr;
-  if (replay) {
+  if (replay || events) {  // event mode without adm_wl: the rows of the snapshot have no record (-1)
     X.adm_wl = (int32_t *)take(Acap, 4);
-    CUDA_TRY(h, cudaMemcpyAsync(X.adm_wl, s->adm_wl, (size_t)s->n_adm * 4, cudaMemcpyHostToDevice, h->stream));
+    if (replay) CUDA_TRY(h, cudaMemcpyAsync(X.adm_wl, s->adm_wl, (size_t)s->n_adm * 4, cudaMemcpyHostToDevice, h->stream));
+    else CUDA_TRY(h, cudaMemsetAsync(X.adm_wl, 0xff, (size_t)s->n_adm * 4, h->stream));
     X.wl_seg = (int32_t *)take(Wz, 4); X.wl_pos = (int32_t *)take(Wz, 4); X.wl_evictions = (int32_t *)take(Wz, 4);
     X.wl_has_qr = const_cast<uint8_t *>(D.wl_has_qr);
   }
-  if (evict) {
+  if (compact) {
     X.adm_dead = (int32_t *)take(Acap, 4);
     CUDA_TRY(h, cudaMemsetAsync(X.adm_dead, 0, Acap * 4, h->stream));
     other.wl = (int32_t *)take(Acap, 4);
@@ -1488,7 +1526,38 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     other.cq = (int32_t *)take(Acap, 4); other.priority = (int32_t *)take(Acap, 4); other.ts = (i64 *)take(Acap, 8);
     other.qr_ts = (i64 *)take(Acap, 8); other.uid = (i64 *)take(Acap, 8); other.evicted = (uint8_t *)take(Acap, 1);
     other.use_start = (int32_t *)take(Acap + 1, 4); other.use_fr = (int32_t *)take(AUcap, 4); other.use_qty = (i64 *)take(AUcap, 8);
-  }  if (afs) {
+  }
+  u64 *arr_keys[2] = {nullptr, nullptr}; int32_t *arr_vals[2] = {nullptr, nullptr};
+  const i64 *d_create = nullptr;
+  if (events) {
+    X.adm_finish = (i64 *)take(Acap, 8); other.finish = (i64 *)take(Acap, 8);
+    if (s->adm_finish_ns) CUDA_TRY(h, cudaMemcpyAsync(X.adm_finish, s->adm_finish_ns, (size_t)s->n_adm * 8, cudaMemcpyHostToDevice, h->stream));
+    else {
+      std::vector<i64> never((size_t)s->n_adm, INT64_MAX);
+      CUDA_TRY(h, cudaMemcpyAsync(X.adm_finish, never.data(), (size_t)s->n_adm * 8, cudaMemcpyHostToDevice, h->stream));
+      CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // `never` leaves scope
+    }
+    i64 *run = (i64 *)take(Wz, 8);
+    if (s->wl_run_ns) { CUDA_TRY(h, cudaMemcpyAsync(run, s->wl_run_ns, Wz * 8, cudaMemcpyHostToDevice, h->stream)); X.wl_run = run; }
+    X.wl_admit_ns = (i64 *)take(Wz, 8); X.wl_finish_ns = (i64 *)take(Wz, 8); X.clock = (i64 *)take(4, 8);
+    if (s->wl_create_ns) {
+      arr_keys[0] = (u64 *)take(Wz, 8); arr_keys[1] = (u64 *)take(Wz, 8);
+      arr_vals[0] = (int32_t *)take(Wz, 4); arr_vals[1] = (int32_t *)take(Wz, 4);
+      i64 *create = (i64 *)take(Wz, 8);
+      CUDA_TRY(h, cudaMemcpyAsync(create, s->wl_create_ns, Wz * 8, cudaMemcpyHostToDevice, h->stream));
+      d_create = create;
+      X.n_arr = W;
+    }
+    if (n_class) {
+      int32_t *wc = (int32_t *)take(Wz, 4), *cs = (int32_t *)take((size_t)Q + 1, 4);
+      X.class_nofit = (uint8_t *)take((size_t)n_class, 1);
+      CUDA_TRY(h, cudaMemcpyAsync(wc, wl_class.data(), Wz * 4, cudaMemcpyHostToDevice, h->stream));
+      CUDA_TRY(h, cudaMemcpyAsync(cs, cq_class_start.data(), ((size_t)Q + 1) * 4, cudaMemcpyHostToDevice, h->stream));
+      CUDA_TRY(h, cudaMemsetAsync(X.class_nofit, 0, (size_t)n_class, h->stream));
+      X.wl_class = wc; X.cq_class_start = cs;
+    }
+  }
+  if (afs) {
     auto h2d = [&](const void *src, size_t n, size_t sz) {
       char *p = take(n, sz);
       if (n) { cudaError_t e = cudaMemcpyAsync(p, src, n * sz, cudaMemcpyHostToDevice, h->stream); if (e != cudaSuccess) return (char *)nullptr; }
@@ -1531,9 +1600,17 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 32 + cq_bits, h->stream));
     X.q_order = dv.Current();
   }
+  if (d_create) {  // arrival order: (creation time, index); the workloads present at the start are its first k_drain_init_events prefix
+    cub::DoubleBuffer<u64> dk(arr_keys[0], arr_keys[1]); cub::DoubleBuffer<int32_t> dv(arr_vals[0], arr_vals[1]);
+    size_t bytes = sort_bytes;
+    k_drain_keys_create<<<nbW, tb, 0, h->stream>>>(W, d_create, dk.Current(), dv.Current());
+    CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 64, h->stream));
+    X.arr_key = dk.Current(); X.arr_order = dv.Current();
+  }
   k_scan_i32<<<1, 1024, 0, h->stream>>>(q_count, X.q_start, S);
   k_drain_init<<<std::max(nbW, (S + tb - 1) / tb), tb, 0, h->stream>>>(D, X, S);
-  if (replay) k_drain_init_replay<<<std::max(nbW, (s->n_adm + tb - 1) / tb), tb, 0, h->stream>>>(D, X, s->n_adm);
+  if (events) k_drain_init_events<<<std::max(1, nbW), tb, 0, h->stream>>>(D, X, d_create, s->now_ns);
+  if (replay || events) k_drain_init_replay<<<std::max(nbW, (s->n_adm + tb - 1) / tb), tb, 0, h->stream>>>(D, X, replay ? s->n_adm : 0);
   k_drain_advance<<<(S + tb - 1) / tb, tb, 0, h->stream>>>(X, S);
   int32_t *d_heads = const_cast<int32_t *>(D.heads);
   auto enqueue_heads = [&]() {
@@ -1551,7 +1628,109 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   const bool pre = h->preempt_possible;
   double gpu_ms = 0;
   float kms[KB_N_KERNELS] = {};  // per-kernel times summed over the cycles (kb_set_profile)
-  for (int cyc = 0; cyc < max_cycles && n_live > 0; cyc++) {
+  i64 t = s->now_ns;  // event mode: the simulated clock
+  const i64 step = s->drain_cycle_ns > 0 ? s->drain_cycle_ns : 1;
+  const int nbArr = std::max(1, std::min(nbW, 8 * std::max(1, h->sm_count)));
+  for (int cyc = 0, jumps = 0; events && cyc < max_cycles;) {
+    // one boundary: cycle c at t (or, without heads, a jump to the next event), then E, t_{c+1}, completions,
+    // arrivals, inadmissible requeue, compaction and the next heads; one synchronisation
+    const bool jump = n_live == 0;
+    const int32_t *n_new_d = jump ? nullptr : X.e_adm_off + n_live;
+    if (!jump) {
+      D.H = n_live; D.now_ns = t;
+      D.A = pre ? A_cur : 0; D.AU = pre ? AU_cur : 0;
+      rc = cycle_enqueue(h);
+      if (rc != KB_OK) return rc;
+      X.cycle = cyc;
+    } else {
+      CUDA_TRY(h, cudaEventRecord(h->ev2, h->stream));
+      X.cycle = -2 - jumps;  // stamps of a jump (cycle + 1 < 0) never meet those of a cycle
+    }
+    X.A = A_cur; X.AU = AU_cur; X.trace_off = (long long)out->n_decisions;
+    kmark(h, KB_K_DRAIN);
+    CUDA_TRY(h, cudaMemsetAsync(X.counters + 1, 0, 4 * 4, h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_FINISHED, 0, 3 * 4, h->stream));
+    int bound = A_cur;  // rows the boundary looks at: the tables plus room for this cycle's admissions
+    if (!jump) {
+      const int nbH = (n_live + tb - 1) / tb;
+      k_drain_apply<<<nbH, tb, 0, h->stream>>>(D, X);
+      k_scan_i32<<<1, 1024, 0, h->stream>>>(X.e_assumed, X.e_adm_off, n_live);
+      k_scan_i32<<<1, 1024, 0, h->stream>>>(X.e_ncells, X.e_cell_off, n_live);
+      k_drain_admit<<<nbH, tb, 0, h->stream>>>(D, X, t, nullptr);
+      if (evict) k_drain_evict<<<nbH, tb, 0, h->stream>>>(D, X);
+      bound = (int)std::min<size_t>((size_t)A_cur + n_live, Acap);
+    }
+    const int nbB = std::max(1, (bound + tb - 1) / tb);
+    k_drain_ev_min<<<nbB, tb, 0, h->stream>>>(X, bound, n_new_d);
+    k_drain_ev_next<<<1, 1, 0, h->stream>>>(X, t, step, jump, n_new_d);
+    k_drain_finish<<<nbB, tb, 0, h->stream>>>(D, X, bound, n_new_d);
+    if (X.arr_key) k_drain_arrive<<<nbArr, tb, 0, h->stream>>>(X);
+    k_drain_requeue<<<nbQ, tb, 0, h->stream>>>(D, X);
+    {
+      DrainDev Xc = X;  // compaction over [0, bound]: the padding rows are stamped dead
+      Xc.A = bound;
+      const int nbA = (bound + 1 + tb - 1) / tb;
+      k_drain_live<<<nbA, tb, 0, h->stream>>>(Xc);
+      size_t sb = scan_bytes;
+      CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(scan_tmp, sb, X.row_live, X.row_new, bound + 1, h->stream));
+      sb = scan_bytes;
+      CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(scan_tmp, sb, X.row_cells, X.cell_new, bound + 1, h->stream));
+      k_drain_compact<<<nbA, tb, 0, h->stream>>>(Xc, other);
+    }
+    enqueue_heads();
+    kmark(h, -1);
+    CUDA_TRY(h, cudaEventRecord(h->ev_d, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[8], X.counters, 4, cudaMemcpyDeviceToHost, h->stream));
+    if (!jump) CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[9], n_new_d, 4, cudaMemcpyDeviceToHost, h->stream));
+    if (afs && !jump) CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[11], D.status, 4, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[12], X.counters + 1, 10 * 4, cudaMemcpyDeviceToHost, h->stream));  // .. [KB_DC_ARR_HI]
+    CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[22], X.clock, 8, cudaMemcpyDeviceToHost, h->stream));             // t_{c+1}
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    if (!jump) {
+      rc = cycle_finish(h);
+      if (rc != KB_OK) return rc;
+      if (afs && (h->host_words[11] & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: an entry penalty overflows int64");
+      for (int i = 0; i < KB_N_KERNELS; i++) kms[i] += h->stats.kernel_ms[i];
+    }
+    { float ms = 0; cudaEventElapsedTime(&ms, h->ev2, h->ev_d); gpu_ms += ms; }
+    if (h->host_words[16]) return fail(h, KB_ERR_CAPACITY, "kb_run_drain: the admitted tables are full");
+    const int fin = (int)h->host_words[12 + KB_DC_FINISHED - 1], arr = (int)h->host_words[12 + KB_DC_ARRIVED - 1];
+    const bool end = h->host_words[12 + KB_DC_END - 1] != 0;
+    i64 t_next;
+    memcpy(&t_next, &h->host_words[22], 8);
+    if (!jump) {
+      const int n_new = (int)h->host_words[9], n_ev = (int)h->host_words[12];
+      if (out->cycle_heads) out->cycle_heads[cyc] = n_live;
+      if (out->cycle_admitted) out->cycle_admitted[cyc] = n_new;
+      if (out->cycle_evicted) out->cycle_evicted[cyc] = n_ev;
+      if (out->cycle_start_ns) out->cycle_start_ns[cyc] = t;
+      if (out->cycle_finished) out->cycle_finished[cyc] = 0;
+      if (out->cycle_arrived) out->cycle_arrived[cyc] = 0;
+      out->n_decisions += n_live; out->n_admitted += n_new; out->n_evicted += n_ev;
+      out->n_cycles = ++cyc;
+    } else {
+      jumps++;
+    }
+    out->n_finished += fin; out->n_arrived += arr;
+    if (cyc > 0) {  // events between the start of the last cycle and the next one are that cycle's
+      if (out->cycle_finished) out->cycle_finished[cyc - 1] += fin;
+      if (out->cycle_arrived) out->cycle_arrived[cyc - 1] += arr;
+    }
+    // the compacted half becomes the admitted tables of the next boundary
+    A_cur = (int)h->host_words[13]; AU_cur = (int)h->host_words[14];
+    AdmTabs cur{X.adm_cq, X.adm_priority, X.adm_ts, X.adm_qr_ts, X.adm_uid, X.adm_evicted, X.adm_use_start, X.adm_use_fr, X.adm_use_qty, X.adm_wl, X.adm_finish};
+    X.adm_cq = other.cq; X.adm_priority = other.priority; X.adm_ts = other.ts; X.adm_qr_ts = other.qr_ts; X.adm_uid = other.uid;
+    X.adm_evicted = other.evicted; X.adm_use_start = other.use_start; X.adm_use_fr = other.use_fr; X.adm_use_qty = other.use_qty; X.adm_wl = other.wl;
+    X.adm_finish = other.finish;
+    D.adm_cq = X.adm_cq; D.adm_priority = X.adm_priority; D.adm_ts = X.adm_ts; D.adm_qr_ts = X.adm_qr_ts; D.adm_uid = X.adm_uid;
+    D.adm_evicted = X.adm_evicted; D.adm_use_start = X.adm_use_start; D.adm_use_fr = X.adm_use_fr; D.adm_use_qty = X.adm_use_qty;
+    other = cur;
+    n_live = (int)h->host_words[8];
+    if (end) break;
+    t = t_next;
+  }
+  if (events) out->end_ns = t;
+  for (int cyc = 0; !events && cyc < max_cycles && n_live > 0; cyc++) {
     D.H = n_live; D.now_ns = s->now_ns + cyc;
     D.A = pre ? A_cur : 0; D.AU = pre ? AU_cur : 0;  // without preemption policies the cycle never looks at the admitted tables
     rc = cycle_enqueue(h);
@@ -1622,6 +1801,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   if (out->wl_admit_cycle) CUDA_TRY(h, cudaMemcpyAsync(out->wl_admit_cycle, X.wl_admit_cycle, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
   if (out->wl_last_decision) CUDA_TRY(h, cudaMemcpyAsync(out->wl_last_decision, X.wl_last_decision, Wz, cudaMemcpyDeviceToHost, h->stream));
   if (out->wl_evals) CUDA_TRY(h, cudaMemcpyAsync(out->wl_evals, X.wl_evals, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (events && out->wl_admit_ns) CUDA_TRY(h, cudaMemcpyAsync(out->wl_admit_ns, X.wl_admit_ns, Wz * 8, cudaMemcpyDeviceToHost, h->stream));
+  if (events && out->wl_finish_ns) CUDA_TRY(h, cudaMemcpyAsync(out->wl_finish_ns, X.wl_finish_ns, Wz * 8, cudaMemcpyDeviceToHost, h->stream));
   if (out->wl_evictions) {
     if (replay) CUDA_TRY(h, cudaMemcpyAsync(out->wl_evictions, X.wl_evictions, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
     else memset(out->wl_evictions, 0, Wz * 4);
@@ -1641,7 +1822,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
 extern "C" int32_t kb_run_drain(kb_handle *h, const kb_snapshot *s, kb_drain_out *out) {
   if (!h || !s || !out) return KB_ERR_INVALID;
   int32_t rc = drain_impl(h, s, out);
-  h->drain_mode = false; h->drain_extra_adm = 0; h->drain_extra_au = 0;
+  h->drain_mode = false; h->drain_events = false; h->drain_extra_adm = 0; h->drain_extra_au = 0;
   h->uploaded = false;  // the resident snapshot was consumed (queues advanced, admitted tables grown)
   return rc;
 }

@@ -26,6 +26,18 @@
 // numbered ClusterQueue-major (seg_start[Q+1]).  The head of an AFS ClusterQueue is the minimum of (LocalQueue usage by
 // cmp.Compare, -priority, timestamp, UID) over the heads of its segments (one warp per ClusterQueue, k_drain_afs_heads);
 // an admission adds its entry penalty to its LocalQueue and recomputes that LocalQueue's usage (k_drain_admit).
+//
+// Event mode (kb_snapshot.wl_create_ns / wl_run_ns / adm_finish_ns; include/kueue_b200.h): two more states,
+// KB_WS_ABSENT (not created yet) and KB_WS_FINISHED.  Every admitted row carries its finish time (adm_finish, written by
+// k_drain_admit, carried by the compaction) and its record (adm_wl, -1 for a row of the snapshot without one).  After
+// the decisions of a cycle: k_drain_admit appends the admissions to the current half, k_drain_evict replays the
+// evictions, k_drain_ev_min reduces E (the earliest finish of a live row and the next creation), k_drain_ev_next (one
+// thread) computes t_{c+1} and the end flag, k_drain_finish stamps the finished rows dead with the eviction stamp and
+// takes their cells out (a row admitted in this cycle that finishes by t_{c+1} dies before any cycle sees it),
+// k_drain_arrive walks the arrived prefix of the (create, index) order, k_drain_requeue visits the marked roots, and
+// the compaction copies the live rows into the other half.  A cycle without heads is replaced by the same boundary
+// with t_{c+1} = E and a negative stamp (no cycle is counted).  The NoFit set of a ClusterQueue is one byte per
+// (ClusterQueue, scheduling hash) class: k_drain_apply sets it, k_drain_requeue clears the bytes of the queues it visits.
 #pragma once
 
 #include <cub/device/device_scan.cuh>
@@ -119,7 +131,20 @@ struct DrainDev {
   i64 *lq_penalty; double *lq_usage;
   double alpha;
   int n_afs_cq;
+  // event mode; adm_finish == nullptr: off
+  i64 *adm_finish;                 // [A_cap] finish time of each admitted row (current half), INT64_MAX = never
+  const i64 *wl_run;               // [W] run time once admitted (< 0 never finishes); null = none finishes
+  i64 *wl_admit_ns, *wl_finish_ns; // [W]
+  i64 *clock;                      // [0] t_{c+1} of the boundary, [1] E (INT64_MAX = none; reset by k_drain_ev_next)
+  const u64 *arr_key;              // [n_arr] creation times (sign flipped) of the ABSENT workloads, ascending
+  const int32_t *arr_order;        // [n_arr] their indices, ties by index
+  int n_arr;
+  const int32_t *wl_class;         // [W] (ClusterQueue, hash) class of a BestEffortFIFO workload with a known hash, -1
+  const int32_t *cq_class_start;   // [Q+1] classes of a ClusterQueue
+  uint8_t *class_nofit;            // [classes] in the ClusterQueue's NoFit set; null = no arrivals or no hashes
 };
+// counters of event mode: [6] completions, [7] arrivals, [8] end flag, [9] / [10] arrived prefix of arr_order [lo, hi)
+enum { KB_DC_FINISHED = 6, KB_DC_ARRIVED = 7, KB_DC_END = 8, KB_DC_ARR_LO = 9, KB_DC_ARR_HI = 10 };
 
 __device__ __forceinline__ int drain_seg0(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq] : cq; }
 __device__ __forceinline__ int drain_seg1(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq + 1] : cq + 1; }
@@ -146,7 +171,7 @@ __global__ void k_drain_keys_cq(DevSnap D, DrainDev X, const int32_t *vals, u64 
   keys[i] = ((u64)seg << 32) | (u64)(~((unsigned)D.wl_priority[w] ^ 0x80000000u));  // higher priority first
   atomicAdd(&q_count[seg], 1);
 }
-enum { KB_WS_QUEUED = 0, KB_WS_SET_ASIDE = 1, KB_WS_HELD = 2 };
+enum { KB_WS_QUEUED = 0, KB_WS_SET_ASIDE = 1, KB_WS_HELD = 2, KB_WS_ABSENT = 3, KB_WS_FINISHED = 4 };
 __global__ void k_drain_init(DevSnap D, DrainDev X, int S) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < D.W) { X.wl_state[i] = KB_WS_QUEUED; X.wl_admit_cycle[i] = -1; X.wl_evals[i] = 0; X.wl_last_decision[i] = 0xff; }
@@ -282,6 +307,7 @@ __global__ void k_drain_apply(DevSnap D, DrainDev X) {
   const bool bulk = dec == KB_DEC_NOFIT && !strict && D.wl_sched_hash && D.wl_sched_hash[wl] != 0;
   if (bulk) {  // handleInadmissibleHash :408-425: every queued workload of the class, in every segment of the queue
     const i64 hsh = D.wl_sched_hash[wl];
+    if (X.class_nofit) X.class_nofit[X.wl_class[wl]] = 1;  // noFitSchedulingHashes.Insert (:414)
     for (int s = s0; s < s1; s++) {
       const int qs = X.q_start[s], qn = X.q_start[s + 1] - qs;
       for (int p = X.cursor[s] + (s == hs); p < qn; p++) {
@@ -315,6 +341,11 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts, const int32_t *b
   X.adm_cq[a] = cq; X.adm_priority[a] = D.wl_priority[wl]; X.adm_ts[a] = D.wl_ts[wl]; X.adm_qr_ts[a] = qr_ts;
   X.adm_uid[a] = D.wl_uid[wl]; X.adm_evicted[a] = 0;
   X.adm_use_start[a] = c0;
+  if (X.adm_finish) {  // finish = QuotaReserved time + run time, saturating; run < 0 never finishes
+    const i64 run = X.wl_run ? X.wl_run[wl] : -1;
+    X.adm_finish[a] = run < 0 ? INT64_MAX : (qr_ts > INT64_MAX - run ? INT64_MAX : qr_ts + run);
+    X.wl_admit_ns[wl] = qr_ts;
+  }
   const bool covers_pods = drain_covers_pods(D, cq);
   const int ps0 = D.wl_ps_start[wl], ps1 = D.wl_ps_start[wl + 1];
   int n = 0;
@@ -386,6 +417,7 @@ __global__ void k_drain_evict(DevSnap D, DrainDev X) {
 __global__ void k_drain_requeue(DevSnap D, DrainDev X) {
   int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= D.Q || X.root_mark[D.root_slot[q]] != X.cycle + 1) return;
+  if (X.class_nofit) for (int k = X.cq_class_start[q]; k < X.cq_class_start[q + 1]; k++) X.class_nofit[k] = 0;  // inadmissible_workloads.go:174
   for (int s = drain_seg0(X, q); s < drain_seg1(X, q); s++) {
     const int qs = X.q_start[s], qn = X.q_start[s + 1] - qs, fa = X.first_aside[s];
     for (int p = fa; p < qn; p++) { const int w = X.q_order[qs + p]; if (X.wl_state[w] == KB_WS_SET_ASIDE) X.wl_state[w] = KB_WS_QUEUED; }
@@ -401,7 +433,7 @@ __global__ void k_drain_live(DrainDev X) {
   X.row_live[a] = live;
   X.row_cells[a] = live ? X.adm_use_start[a + 1] - X.adm_use_start[a] : 0;
 }
-struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; };
+struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; i64 *finish; };
 // live rows, in order, into the other half of the double buffer; thread A writes the totals (counters[2..3])
 __global__ void k_drain_compact(DrainDev X, AdmTabs O) {
   int a = blockIdx.x * blockDim.x + threadIdx.x;
@@ -411,5 +443,99 @@ __global__ void k_drain_compact(DrainDev X, AdmTabs O) {
   const int n = X.row_new[a], c0 = X.cell_new[a], u0 = X.adm_use_start[a], nc = X.adm_use_start[a + 1] - u0;
   O.cq[n] = X.adm_cq[a]; O.priority[n] = X.adm_priority[a]; O.ts[n] = X.adm_ts[a]; O.qr_ts[n] = X.adm_qr_ts[a];
   O.uid[n] = X.adm_uid[a]; O.evicted[n] = X.adm_evicted[a]; O.wl[n] = X.adm_wl[a]; O.use_start[n] = c0;
+  if (X.adm_finish) O.finish[n] = X.adm_finish[a];
   for (int c = 0; c < nc; c++) { O.use_fr[c0 + c] = X.adm_use_fr[u0 + c]; O.use_qty[c0 + c] = X.adm_use_qty[u0 + c]; }
+}
+
+// ---- event mode ---------------------------------------------------------------------------------------------------
+__device__ __forceinline__ i64 ev_time(u64 key) { return (i64)(key ^ 0x8000000000000000ull); }
+// first i in [lo, n) with arr_key[i] > t (the creations up to t are [.., i))
+__device__ __forceinline__ int ev_upper_bound(const u64 *key, int lo, int n, i64 t) {
+  const u64 k = (u64)t ^ 0x8000000000000000ull;
+  int hi = n;
+  while (lo < hi) { const int m = lo + (hi - lo) / 2; if (key[m] <= k) lo = m + 1; else hi = m; }
+  return lo;
+}
+// sort keys of the arrival order: creation time, then index (the radix sort is stable)
+__global__ void k_drain_keys_create(int W, const i64 *create, u64 *keys, int32_t *vals) {
+  int w = blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= W) return;
+  keys[w] = (u64)create[w] ^ 0x8000000000000000ull;
+  vals[w] = w;
+}
+// start of an event drain: workloads created after now_ns are ABSENT, no admission or finish yet, E = none, and the
+// arrived prefix of the arrival order holds the workloads present at the start
+__global__ void k_drain_init_events(DevSnap D, DrainDev X, const i64 *create, i64 now_ns) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) {
+    X.clock[1] = INT64_MAX;
+    const int lo = X.arr_key ? ev_upper_bound(X.arr_key, 0, X.n_arr, now_ns) : 0;
+    X.counters[KB_DC_ARR_LO] = lo; X.counters[KB_DC_ARR_HI] = lo;
+  }
+  if (i >= D.W) return;
+  if (create && create[i] > now_ns) X.wl_state[i] = KB_WS_ABSENT;
+  X.wl_admit_ns[i] = INT64_MIN; X.wl_finish_ns[i] = INT64_MAX;
+}
+// E: the earliest finish of a live row (rows [0, A + *n_new), the ones stamped this boundary excluded) and the next
+// creation; warp minimum, one atomic per warp
+__global__ void k_drain_ev_min(DrainDev X, int bound, const int32_t *n_new) {
+  const int a = blockIdx.x * blockDim.x + threadIdx.x;
+  const int n_rows = X.A + (n_new ? *n_new : 0);
+  i64 v = INT64_MAX;
+  if (a < bound && a < n_rows && X.adm_dead[a] != X.cycle + 1) v = X.adm_finish[a];
+  if (a == 0 && X.counters[KB_DC_ARR_HI] < X.n_arr) v = min(v, ev_time(X.arr_key[X.counters[KB_DC_ARR_HI]]));
+  for (int o = 16; o > 0; o >>= 1) v = min(v, (i64)__shfl_xor_sync(0xffffffffu, (long long)v, o));
+  if ((threadIdx.x & 31) == 0 && v < INT64_MAX) atomicMin((long long *)&X.clock[1], (long long)v);
+}
+// t_{c+1} and the end flag (one thread).  jump: no heads, the clock goes to E.  Otherwise a cycle that admitted or
+// evicted steps, a quiet one waits for E; no E ends the drain.  Then the arrived prefix up to t_{c+1}.
+__global__ void k_drain_ev_next(DrainDev X, i64 t_c, i64 step, int jump, const int32_t *n_new) {
+  const i64 E = X.clock[1];
+  const i64 stepped = t_c > INT64_MAX - step ? INT64_MAX : t_c + step;
+  const bool active = !jump && ((n_new && *n_new > 0) || X.counters[1] > 0);
+  i64 tn;
+  bool end = false;
+  if (jump) { end = E == INT64_MAX; tn = E; }
+  else if (active) tn = stepped;
+  else { end = E == INT64_MAX; tn = max(stepped, E); }
+  X.clock[0] = end ? t_c : tn;
+  X.clock[1] = INT64_MAX;
+  X.counters[KB_DC_END] = end;
+  const int lo = X.counters[KB_DC_ARR_HI];
+  X.counters[KB_DC_ARR_LO] = lo;
+  X.counters[KB_DC_ARR_HI] = (end || !X.arr_key) ? lo : ev_upper_bound(X.arr_key, lo, X.n_arr, tn);
+}
+// completions (thread per row): a live row with finish <= t_{c+1} gets the dead stamp, its cells leave its ClusterQueue's
+// usage (cache.DeleteWorkload, integer atomics), its record becomes FINISHED and its root tree is marked.  Rows in
+// [A + *n_new, bound) only pad the compaction's range: they are stamped dead.
+__global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *n_new) {
+  const int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a >= bound || X.counters[5]) return;
+  const int stamp = X.cycle + 1;
+  if (a >= X.A + (n_new ? *n_new : 0)) { X.adm_dead[a] = stamp; return; }
+  if (X.counters[KB_DC_END] || X.adm_dead[a] == stamp || X.adm_finish[a] > X.clock[0]) return;
+  X.adm_dead[a] = stamp;
+  const int cq = X.adm_cq[a];
+  for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)
+    atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
+  const int w = X.adm_wl[a];
+  if (w >= 0) { X.wl_state[w] = KB_WS_FINISHED; X.wl_admit_cycle[w] = -1; X.wl_finish_ns[w] = X.adm_finish[a]; }
+  X.root_mark[D.root_slot[cq]] = stamp;
+  atomicAdd(&X.counters[KB_DC_FINISHED], 1);
+}
+// arrivals (grid-stride over the arrived prefix [lo, hi)): the workload joins its queue and the cursor moves back to it;
+// in a BestEffortFIFO ClusterQueue a known hash in the NoFit set sets it aside (PushOrUpdate, cluster_queue.go:288-293)
+__global__ void k_drain_arrive(DrainDev X) {
+  const int lo = X.counters[KB_DC_ARR_LO], hi = X.counters[KB_DC_ARR_HI];
+  if (blockIdx.x == 0 && threadIdx.x == 0) X.counters[KB_DC_ARRIVED] = hi - lo;
+  for (int i = lo + blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += gridDim.x * blockDim.x) {
+    const int w = X.arr_order[i], s = X.wl_seg[w], p = X.wl_pos[w];
+    if (X.class_nofit && X.wl_class[w] >= 0 && X.class_nofit[X.wl_class[w]]) {
+      X.wl_state[w] = KB_WS_SET_ASIDE;
+      atomicMin(&X.first_aside[s], p);
+    } else {
+      X.wl_state[w] = KB_WS_QUEUED;
+      atomicMin(&X.cursor[s], p);
+    }
+  }
 }

@@ -58,6 +58,34 @@ ClusterQueue with `cq_afs` set is one segment per LocalQueue, each in the static
     the next cycle; consumed usage does not decay inside a drain;
   * StrictFIFO keeps its head (the next cycle picks the minimum again), BestEffortFIFO advances the head's own segment,
     handleInadmissibleHash sets aside the workloads of the class in every segment of the ClusterQueue.
+
+Event mode (the snapshot carries `wl_create_ns`, `wl_run_ns` or `adm_finish_ns`, include/kueue_b200.h): arrivals and
+completions on a simulated clock, as the reference's scheduler performance runner drives them (generator.go creates
+workloads at fixed intervals; controller.go:100-160 finishes each one runtimeMs after its admission, an eviction
+restarting that clock).  The clock t starts at now_ns; cycle c runs at t_c (its now_ns and the QuotaReserved time of
+its admissions).  Two more states: ABSENT (not created yet, in no queue) and FINISHED (never requeued).  A pending event
+is the finish time of a live admitted row or the creation time of an ABSENT workload; INT64_MAX means never.
+  1. no queue has a head: t jumps to E, the earliest pending event, and steps 5-7 apply the events at E without
+     counting a cycle; without E the drain ends;
+  2. cycle c runs at t_c, its decisions are applied as above;  3. evictions are replayed as above (with `adm_wl`);
+  4. a cycle that admitted or evicted: t_{c+1} = t_c + step (drain_cycle_ns, <= 0 means 1).  A quiet cycle, the stop
+     rule of the plain drain, waits instead: t_{c+1} = max(t_c + step, E); without E the drain ends;
+  5. completions (workload_controller.go:936-952): every live row with finish <= t_{c+1} finishes, a row admitted in
+     cycle c included (it never enters the tables).  Its cells leave its ClusterQueue's usage (cache.DeleteWorkload),
+     its row is removed, its record becomes FINISHED and its root cohort tree is marked.  A row admitted at t finishes
+     at t + wl_run_ns[w] (saturating at INT64_MAX); an evicted workload loses its finish time and a readmission restarts
+     the full run time;
+  6. arrivals (AddOrUpdateWorkload -> PushOrUpdate, manager.go:524-560): every ABSENT workload with create <= t_{c+1}
+     joins its queue; the cursor moves back to it if it comes earlier.  In a BestEffortFIFO ClusterQueue a workload
+     whose known scheduling hash is in the ClusterQueue's NoFit set goes straight to SET_ASIDE (cluster_queue.go:288-293;
+     `NoFitSets`);
+  7. the inadmissible requeue (`requeue_inadmissible`) over every root tree marked in step 3 or 5; it clears the NoFit
+     sets of the ClusterQueues it visits;
+  8. the heads of cycle c+1.
+Steps 5-7 only set state bytes and lower cursors: their order does not change the result.  Waiting in a quiet cycle is
+the canonical choice; with every run time < 0 and every creation <= now_ns the drain is the plain drain.  The drain
+stops before cycle max_cycles.  Events applied before cycle 0 count only in the totals; the events applied between the
+start of cycle c and the start of cycle c+1 are cycle c's (`finished`, `arrived`).
 """
 from __future__ import annotations
 
@@ -82,6 +110,15 @@ class DrainResult:
     wl_admit_cycle: np.ndarray | None = None                   # [n_wl] cycle of its last admission if it holds quota, else -1
     state: np.ndarray | None = None                            # [n_wl] final QUEUED / SET_ASIDE / HELD
     adm: dict | None = None                                    # final admitted tables (adm_* plus adm_wl when replaying)
+    # event mode
+    cycle_start_ns: List[int] = field(default_factory=list)    # per cycle: t_c
+    finished: List[np.ndarray] = field(default_factory=list)   # per cycle: pending indices finished (-1: a row without one)
+    arrived: List[np.ndarray] = field(default_factory=list)    # per cycle: pending indices arrived
+    n_finished: int = 0                                        # including the events applied before cycle 0
+    n_arrived: int = 0
+    wl_admit_ns: np.ndarray | None = None                      # [n_wl] time of its last admission, INT64_MIN = never
+    wl_finish_ns: np.ndarray | None = None                     # [n_wl] finish time, INT64_MAX = not finished
+    end_ns: int = 0                                            # the clock when the drain stopped
 
     @property
     def n_evicted(self) -> int:
@@ -131,7 +168,32 @@ def requeue_goes_inadmissible(strict_fifo: bool, reason: str, last_tried) -> boo
     return not (immediate or pending_flavors(last_tried))
 
 
-QUEUED, SET_ASIDE, HELD = 0, 1, 2  # per-workload queue state (kb_drain.cuh KB_WS_*)
+QUEUED, SET_ASIDE, HELD, ABSENT, FINISHED = 0, 1, 2, 3, 4  # per-workload queue state (kb_drain.cuh KB_WS_*)
+NEVER = np.iinfo(np.int64).max  # an event time that never comes
+
+
+class NoFitSets:
+    """noFitSchedulingHashes of every ClusterQueue: handleInadmissibleHash inserts the hash of a NoFit head
+    (cluster_queue.go:408-425, :414), queueInadmissibleWorkloads clears the set (inadmissible_workloads.go:174), and
+    PushOrUpdate sets a new workload aside when its known hash is in the set of a BestEffortFIFO ClusterQueue
+    (cluster_queue.go:288-293)."""
+
+    def __init__(self):
+        self.sets = {}
+
+    def insert(self, cq: int, hsh: int) -> None:
+        self.sets.setdefault(int(cq), set()).add(int(hsh))
+
+    def clear(self, cq: int) -> None:
+        self.sets.pop(int(cq), None)
+
+    def arrival_goes_aside(self, cq: int, strict_fifo: bool, hsh: int) -> bool:
+        return not strict_fifo and hsh != 0 and int(hsh) in self.sets.get(int(cq), ())
+
+
+def finish_time(admit_ns: int, run_ns: int) -> int:
+    """Finish time of a row admitted at admit_ns: admit + run saturating at INT64_MAX; run < 0 never finishes."""
+    return NEVER if run_ns < 0 else min(int(admit_ns) + int(run_ns), NEVER)
 
 
 def root_of(parent) -> np.ndarray:
@@ -267,6 +329,10 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     qlen = np.diff(qstart)
     afs_cq = a["cq_afs"].astype(bool) if "wl_lq" in a else np.zeros(Q, bool)
     replay = "adm_wl" in a
+    events = any(k in a for k in abi.EVENT_FIELDS)
+    step = max(1, int(snap.drain_cycle_ns)) if events else 1
+    create = a.get("wl_create_ns")
+    run_ns = a.get("wl_run_ns")
     state = np.full(snap.n_wl, QUEUED, np.uint8)
     seg_of = np.zeros(snap.n_wl, np.int64)                        # segment of every pending workload
     pos_of = np.zeros(snap.n_wl, np.int64)                        # its position in the segment's static order
@@ -274,10 +340,16 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         seg_of[order[qstart[s]:qstart[s + 1]]] = s
         pos_of[order[qstart[s]:qstart[s + 1]]] = np.arange(qlen[s])
     adm_wl = a["adm_wl"].astype(np.int64).copy() if replay else None
+    if events:  # the record of every row (-1: a row of the snapshot without adm_wl) and its finish time
+        adm_wl = adm_wl if replay else np.full(snap.n_adm, -1, np.int64)
+        adm_finish = a["adm_finish_ns"].astype(np.int64).copy() if "adm_finish_ns" in a else np.full(snap.n_adm, NEVER, np.int64)
+        if create is not None:
+            state[create > snap.now_ns] = ABSENT
     if replay:
-        state[adm_wl] = HELD  # holds quota: out of every queue
+        state[a["adm_wl"].astype(np.int64)] = HELD  # holds quota: out of every queue
     cursor = np.zeros(len(qlen), np.int64)
     first_aside = qlen.copy()                                     # smallest SET_ASIDE position per segment (qlen = none)
+    nofit = NoFitSets()
 
     def advance(s):
         while cursor[s] < qlen[s] and state[order[qstart[s] + cursor[s]]] != QUEUED:
@@ -325,6 +397,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     has_qr = a["wl_has_quota_reservation"].copy() if "wl_has_quota_reservation" in a else None
     admit_cycle = np.full(snap.n_wl, -1, np.int64)
     evictions = np.zeros(snap.n_wl, np.int64)
+    admit_ns = np.full(snap.n_wl, np.iinfo(np.int64).min, np.int64)
+    finish_ns = np.full(snap.n_wl, NEVER, np.int64)
     root = root_of(a["parent"])
     static = {k: v for k, v in a.items() if not (k.startswith(("wl_", "ps_", "adm_")) or k in ("heads", "cq_usage") + abi.AFS_FIELDS)}
     covers_pods = np.zeros(Q, bool)
@@ -332,17 +406,111 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         for q in range(Q):
             masks = a["rg_res_mask"][a["cq_rg_start"][q]:a["cq_rg_start"][q + 1]]
             covers_pods[q] = bool(np.any(masks & (1 << snap.pods_resource)))
-    for cyc in range(max_cycles if len(qlen) else 0):
+    if events and create is not None:  # ABSENT workloads in (create, index) order; `arr_next` is the first not arrived
+        arr_order = np.lexsort((np.arange(snap.n_wl), create))
+        arr_order = arr_order[create[arr_order] > snap.now_ns]
+    else:
+        arr_order = np.zeros(0, np.int64)
+    arr_next = 0
+
+    def remove_rows(rows):
+        """rows leave the admitted tables (cache.DeleteWorkload: cells out of the usage; the other rows keep their order)"""
+        nonlocal adm_wl, adm_finish
+        us, uf, uq = adm["adm_use_start"], adm["adm_use_fr"], adm["adm_use_qty"]
+        for row in rows:
+            cqi = int(adm["adm_cq"][row])
+            for k in range(int(us[row]), int(us[row + 1])):
+                usage[cqi, int(uf[k])] -= int(uq[k])
+        keep = np.ones(len(adm["adm_cq"]), bool)
+        keep[rows] = False
+        cnt = np.diff(us.astype(np.int64))
+        cell_keep = np.repeat(keep, cnt)
+        for k in ("adm_cq", "adm_priority", "adm_ts", "adm_qr_ts", "adm_uid", "adm_evicted"):
+            adm[k] = adm[k][keep]
+        adm["adm_use_fr"], adm["adm_use_qty"] = uf[cell_keep], uq[cell_keep]
+        adm["adm_use_start"] = np.concatenate([[0], np.cumsum(cnt[keep])]).astype(np.int32)
+        if adm_wl is not None:
+            adm_wl = adm_wl[keep]
+        if events:
+            adm_finish = adm_finish[keep]
+
+    def next_event():
+        """earliest pending event after the evictions: a live row's finish or an ABSENT workload's creation (None = none)"""
+        e = int(adm_finish.min()) if len(adm_finish) else NEVER
+        if arr_next < len(arr_order):
+            e = min(e, int(create[arr_order[arr_next]]))
+        return None if e >= NEVER else e
+
+    def apply_events(t_next, notified):
+        """steps 5 and 6 at t_next; returns (finished records, arrived records)"""
+        nonlocal arr_next
+        done = np.flatnonzero(adm_finish <= t_next)
+        fin = adm_wl[done].copy()
+        for row in done:
+            notified.add(int(adm["adm_cq"][row]))
+            w = int(adm_wl[row])
+            if w >= 0:
+                state[w] = FINISHED
+                admit_cycle[w] = -1
+                finish_ns[w] = int(adm_finish[row])
+        if len(done):
+            remove_rows(done)
+        arr = []
+        while arr_next < len(arr_order) and int(create[arr_order[arr_next]]) <= t_next:
+            w = int(arr_order[arr_next]); arr_next += 1
+            q = int(a["wl_cq"][w])
+            if shash is not None and nofit.arrival_goes_aside(q, bool(strict[q]), int(shash[w])):
+                set_aside(w)
+            else:
+                state[w] = QUEUED
+                cursor[seg_of[w]] = min(cursor[seg_of[w]], pos_of[w])
+            arr.append(w)
+        return fin, np.asarray(arr, np.int64)
+
+    def requeue(notified):
+        """step 7: the inadmissible requeue in the root cohort trees of `notified`"""
+        aside = {}
+        for q in range(Q):
+            for s in range(int(seg_start[q]), int(seg_start[q + 1])):
+                seg = order[qstart[s] + first_aside[s]:qstart[s + 1]]
+                aside.setdefault(q, []).extend(int(w) for w in seg[state[seg] == SET_ASIDE])
+        moved, roots = requeue_inadmissible(a["parent"], Q, sorted(notified), aside)
+        for ws in moved.values():
+            state[np.asarray(ws, np.int64)] = QUEUED
+        for q in np.flatnonzero(np.isin(root[:Q], roots)):
+            nofit.clear(q)
+            for s in range(int(seg_start[q]), int(seg_start[q + 1])):
+                cursor[s] = min(cursor[s], first_aside[s])
+                first_aside[s] = qlen[s]
+
+    def after(fin, arr):  # events applied between the start of the last cycle and the next one
+        res.n_finished += len(fin); res.n_arrived += len(arr)
+        if res.cycles:
+            res.finished[-1] = np.concatenate([res.finished[-1], fin]); res.arrived[-1] = np.concatenate([res.arrived[-1], arr])
+
+    t = int(snap.now_ns)
+    cyc = 0
+    while len(qlen) and cyc < max_cycles:
         hseg = np.where(cursor[np.minimum(first_seg, len(qlen) - 1)] < qlen[np.minimum(first_seg, len(qlen) - 1)], first_seg, -1)
         for q in np.flatnonzero(afs_cq):
             hseg[q] = afs_head_seg(q)
         live = np.flatnonzero(hseg >= 0)
         if len(live) == 0:
-            break
+            if not events:
+                break
+            e = next_event()  # step 1: the clock jumps to the next event
+            if e is None:
+                break
+            t = e
+            notified = set()
+            after(*apply_events(t, notified))
+            if notified:
+                requeue(notified)
+            continue
         segs = hseg[live]
         heads = order[qstart[segs] + cursor[segs]]  # global pending indices, one per ClusterQueue with work left
         cs = abi.FlatSnapshot(n_cq=Q, n_cohort=snap.n_cohort, n_flavor=snap.n_flavor, n_resource=R, pods_resource=snap.pods_resource,
-                              flags=snap.flags, now_ns=snap.now_ns + cyc, static_generation=snap.static_generation)
+                              flags=snap.flags, now_ns=t, static_generation=snap.static_generation)
         cs.arrays.update(static)
         cs.set("cq_usage", usage)
         for k, v in adm.items():
@@ -365,6 +533,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         dec = np.asarray(out.decision).copy()
         res.cycles += 1
         res.heads.append(heads); res.decisions.append(dec)
+        res.cycle_start_ns.append(t)
+        res.finished.append(np.zeros(0, np.int64)); res.arrived.append(np.zeros(0, np.int64))
         ok = dec == abi.DEC_ASSUMED
         res.admitted.append(heads[ok])
         # ---- apply the admissions: Assignment.Usage (flavorassigner.go:198-218) with the admitted counts
@@ -399,20 +569,24 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         if n_new:
             g = heads[ok]
             admit_cycle[g] = cyc
+            admit_ns[g] = t
             state[g] = HELD
         if n_new:
             g = heads[ok]
             adm["adm_cq"] = np.concatenate([adm["adm_cq"], a["wl_cq"][g]])
             adm["adm_priority"] = np.concatenate([adm["adm_priority"], a["wl_priority"][g]])
             adm["adm_ts"] = np.concatenate([adm["adm_ts"], a["wl_ts"][g]])
-            adm["adm_qr_ts"] = np.concatenate([adm["adm_qr_ts"], np.full(n_new, snap.now_ns + cyc, np.int64)])
+            adm["adm_qr_ts"] = np.concatenate([adm["adm_qr_ts"], np.full(n_new, t, np.int64)])
             adm["adm_uid"] = np.concatenate([adm["adm_uid"], a["wl_uid"][g]])
             adm["adm_evicted"] = np.concatenate([adm["adm_evicted"], np.zeros(n_new, np.uint8)])
             adm["adm_use_start"] = np.concatenate([adm["adm_use_start"], np.asarray(new_start[1:], np.int32)])
             adm["adm_use_fr"] = np.concatenate([adm["adm_use_fr"], np.asarray(new_fr, np.int32)])
             adm["adm_use_qty"] = np.concatenate([adm["adm_use_qty"], np.asarray(new_qty, np.int64)])
-            if replay:
+            if adm_wl is not None:
                 adm_wl = np.concatenate([adm_wl, g])
+            if events:
+                fin_new = [finish_time(t, int(run_ns[w])) if run_ns is not None else NEVER for w in g]
+                adm_finish = np.concatenate([adm_finish, np.asarray(fin_new, np.int64)])
         # ---- LastAssignment of the entries that stay pending (scheduler.go:345,494)
         tried = np.asarray(out.ps_tried_idx).reshape(-1, R)
         cqs = live
@@ -439,6 +613,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 if hsh == 0:
                     continue
                 q = int(cqs[e])
+                nofit.insert(q, hsh)
                 for s in range(int(seg_start[q]), int(seg_start[q + 1])):  # every queued workload of the class, every segment
                     rest = order[qstart[s] + cursor[s] + (s == segs[e]):qstart[s + 1]]
                     for w in rest[(shash[rest] == hsh) & (state[rest] == QUEUED)]:
@@ -453,13 +628,10 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 victims.extend(int(out.tgt_adm[k]) for k in range(int(out.tgt_start[e]), int(out.tgt_start[e + 1])))
             victims = sorted(set(victims))
         res.evicted.append(np.sort(adm_wl[victims]) if victims else np.zeros(0, np.int64))
+        notified = set()
         if victims:
-            us, uf, uq = adm["adm_use_start"], adm["adm_use_fr"], adm["adm_use_qty"]
-            notified = set()
             for row in victims:
                 cqi, w = int(adm["adm_cq"][row]), int(adm_wl[row])
-                for k in range(int(us[row]), int(us[row + 1])):
-                    usage[cqi, int(uf[k])] -= int(uq[k])  # cache.DeleteWorkload
                 state[w] = QUEUED
                 last_gen[w] = -1
                 last_tried[int(ps_start[w]):int(ps_start[w + 1])] = -1
@@ -469,33 +641,35 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 evictions[w] += 1
                 cursor[seg_of[w]] = min(cursor[seg_of[w]], pos_of[w])
                 notified.add(cqi)
-            keep = np.ones(len(adm["adm_cq"]), bool)  # stable removal of the victims' rows
-            keep[victims] = False
-            cnt = np.diff(us.astype(np.int64))
-            cell_keep = np.repeat(keep, cnt)
-            for k in ("adm_cq", "adm_priority", "adm_ts", "adm_qr_ts", "adm_uid", "adm_evicted"):
-                adm[k] = adm[k][keep]
-            adm["adm_use_fr"], adm["adm_use_qty"] = uf[cell_keep], uq[cell_keep]
-            adm["adm_use_start"] = np.concatenate([[0], np.cumsum(cnt[keep])]).astype(np.int32)
-            adm_wl = adm_wl[keep]
-            # ---- inadmissible requeue in the root cohort trees of the victims
-            aside = {}
-            for q in range(Q):
-                for s in range(int(seg_start[q]), int(seg_start[q + 1])):
-                    seg = order[qstart[s] + first_aside[s]:qstart[s + 1]]
-                    aside.setdefault(q, []).extend(int(w) for w in seg[state[seg] == SET_ASIDE])
-            moved, roots = requeue_inadmissible(a["parent"], Q, sorted(notified), aside)
-            for ws in moved.values():
-                state[np.asarray(ws, np.int64)] = QUEUED
-            for q in np.flatnonzero(np.isin(root[:Q], roots)):
-                for s in range(int(seg_start[q]), int(seg_start[q + 1])):
-                    cursor[s] = min(cursor[s], first_aside[s])
-                    first_aside[s] = qlen[s]
-        if n_new == 0 and not victims:
-            break
+            remove_rows(victims)
+        cyc += 1
+        if not events:
+            if notified:  # ---- inadmissible requeue in the root cohort trees of the victims
+                requeue(notified)
+            if n_new == 0 and not victims:
+                break
+            t += 1
+            continue
+        # ---- the next time, then the completions and arrivals up to it
+        if n_new or victims:
+            t_next = min(t + step, NEVER)
+        else:
+            e = next_event()
+            if e is None:
+                break  # quiet, and nothing will ever happen again
+            t_next = max(min(t + step, NEVER), e)
+        t = t_next
+        after(*apply_events(t, notified))
+        if notified:
+            requeue(notified)
     res.cq_usage = usage
     res.wl_evictions = evictions
     res.wl_admit_cycle = admit_cycle
     res.state = state
     res.adm = dict(adm, **({"adm_wl": adm_wl} if replay else {}))
+    if events:
+        res.adm["adm_finish_ns"] = adm_finish
+    res.wl_admit_ns = admit_ns
+    res.wl_finish_ns = finish_ns
+    res.end_ns = t
     return res

@@ -250,3 +250,72 @@ def add_evictable(snap: abi.FlatSnapshot) -> abi.FlatSnapshot:
         cat("ps_group", np.full(A, -1))
     snap.set("adm_wl", W + np.arange(A))
     return snap
+
+
+def add_events(snap: abi.FlatSnapshot, seed: int = 0, present: float = 0.5, span_ns: int = 50_000, run_ns=(1_000, 20_000),
+               never: float = 0.05, step_ns: int = 1_000) -> abi.FlatSnapshot:
+    """Arrival and completion tables of kb_run_drain's event mode (include/kueue_b200.h), seeded, for any config: a
+    share `present` of the workloads exists at now_ns, the others are created uniformly in (now_ns, now_ns + span_ns];
+    run times are uniform in `run_ns`, a share `never` never finishes; every row admitted before the drain finishes in
+    (now_ns, now_ns + span_ns].  Records named by adm_wl exist at now_ns.  One cycle takes step_ns."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    W, A, now = snap.n_wl, snap.n_adm, int(snap.now_ns)
+    create = np.where(rng.random(W) < present, now - rng.integers(0, 1000, W), now + rng.integers(1, span_ns + 1, W))
+    if "adm_wl" in snap.arrays:
+        create[snap.arrays["adm_wl"]] = now
+    run = np.where(rng.random(W) < never, -1, rng.integers(run_ns[0], run_ns[1] + 1, W))
+    snap.set("wl_create_ns", create)
+    snap.set("wl_run_ns", run)
+    snap.set("adm_finish_ns", now + rng.integers(1, span_ns + 1, A))
+    snap.drain_cycle_ns = step_ns
+    return snap
+
+
+# The reference's scheduler performance scenario (test/performance/scheduler/configs/baseline/generator.yaml, generated
+# by runner/generator/generator.go): 5 cohorts of 6 ClusterQueues, one flavor, cpu only; per ClusterQueue, workload k of
+# a class is created at (k + 1) * interval and runs `run` once admitted (runner/controller/controller.go).
+PERF_CLASSES = (  # (name, count per ClusterQueue, interval ms, run time ms, priority, cpu)
+    ("small", 350, 100, 200, 50, 1),
+    ("medium", 100, 500, 500, 100, 5),
+    ("large", 50, 1200, 1000, 200, 20),
+)
+PERF_COHORTS, PERF_CQS_PER_COHORT = 5, 6
+PERF_NOMINAL_CPU, PERF_BORROW_CPU = 20, 100
+_MS = 1_000_000
+
+
+def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS) -> abi.FlatSnapshot:
+    """The baseline scenario as numbers (15,000 workloads at scale 1; `scale` multiplies the count of every class):
+    nominal 20 cpu and borrowingLimit 100 cpu per ClusterQueue, preemption reclaimWithinCohort Any and
+    withinClusterQueue LowerPriority, BestEffortFIFO.  cpu is in milli-units.  wl_ts is the creation time, an empty
+    adm_wl turns eviction replay on, and `snap.perf_class` holds each workload's index into PERF_CLASSES.  One drain cycle takes cycle_ns of simulated time."""
+    Q = PERF_COHORTS * PERF_CQS_PER_COHORT
+    snap = abi.FlatSnapshot(n_cq=Q, n_cohort=PERF_COHORTS, n_flavor=1, n_resource=1)
+    snap.set("parent", np.concatenate([Q + np.arange(Q) // PERF_CQS_PER_COHORT, np.full(PERF_COHORTS, -1)]))
+    nominal = np.zeros((Q + PERF_COHORTS, 1), np.int64)
+    nominal[:Q] = PERF_NOMINAL_CPU * 1000
+    bl = np.full((Q + PERF_COHORTS, 1), abi.KB_NO_LIMIT, np.int64)
+    bl[:Q] = PERF_BORROW_CPU * 1000
+    snap.set("nominal", nominal); snap.set("borrow_limit", bl)
+    snap.set("cq_within_cq", np.full(Q, abi.POLICY_LOWER_PRIORITY)); snap.set("cq_reclaim_within", np.full(Q, abi.POLICY_ANY))
+    snap.set("cq_strategy", np.full(Q, abi.QUEUE_BEST_EFFORT_FIFO))
+    snap.set("cq_rg_start", np.arange(Q + 1)); snap.set("rg_res_mask", np.ones(Q)); snap.set("rg_flavor_start", np.arange(Q + 1))
+    snap.set("rg_flavors", np.zeros(Q))
+    cq, cls, create, run, prio, cpu = [], [], [], [], [], []
+    for q in range(Q):
+        for c, (_, count, interval, run_ms, p, req) in enumerate(PERF_CLASSES):
+            n = max(1, int(round(count * scale)))
+            cq += [q] * n; cls += [c] * n
+            create += list((np.arange(n) + 1) * interval * _MS)
+            run += [run_ms * _MS] * n; prio += [p] * n; cpu += [req * 1000] * n
+    W = len(cq)
+    snap.set("wl_cq", cq); snap.set("wl_priority", prio)
+    snap.set("wl_ts", create); snap.set("wl_uid", np.arange(W))
+    snap.set("ps_req", np.asarray(cpu, np.int64)[:, None]); snap.set("ps_req_mask", np.ones(W)); snap.set("ps_count", np.ones(W))
+    snap.set("wl_create_ns", create); snap.set("wl_run_ns", run)
+    snap.set("adm_wl", np.zeros(0))
+    snap.now_ns = 0
+    snap.drain_cycle_ns = cycle_ns
+    snap.finalize()
+    snap.__dict__["perf_class"] = np.asarray(cls, np.int64)
+    return snap
