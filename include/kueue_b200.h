@@ -280,6 +280,40 @@ typedef struct kb_snapshot {
   const int64_t *wl_create_ns;      /* [n_wl] creation time; <= now_ns: present at the start; NULL = all present    */
   const int64_t *wl_run_ns;         /* [n_wl] run time once admitted; < 0: never finishes; NULL = none finishes     */
   const int64_t *adm_finish_ns;     /* [n_adm] finish time of each row admitted before the drain; NULL = never      */
+
+  /* ---- decay of AdmissionFairSharing consumed usage (optional; event mode of kb_run_drain with wl_lq only) ----
+     lq_last_update_ns == NULL: off, and every launch, index and result of the drain stays as without this block.  With
+     it, the consumed usage of every LocalQueue of an AFS ClusterQueue decays over simulated time as the LocalQueue
+     reconciler decays it (localqueue_controller.go:210-229,363-398; CalculateDecayedConsumed,
+     admission_fair_sharing.go:39-66):
+       Decay(consumed, adm, elapsed) = MulByFloat(consumed, 1 - a) (+) MulByFloat(adm, a),  a = 1 - 0.5^(elapsed / half-life)
+     where MulByFloat(q, f) = int64(float64(MilliValue(q)) * f) milli-units (resource.go:72-99), every resource is
+     written back as (milli, -3), MilliValue rounds a finer scale away from zero (negativeScaleInt64) and fails with
+     KB_ERR_UNSUPPORTED when a coarser one overflows, and adm[r] is the LocalQueue's admitted usage: the cells with
+     fr % R == r of its live admitted rows (library units; its MilliValue is adm[r] * afs_milli_mul[r]).  Durations
+     go through Duration.Seconds() before the division.
+       1. samples: the next one of a LocalQueue is due at LastUpdate + afs_sampling_ns.  At the start every sample due
+          at or before now_ns is taken; at every boundary t -> t' (cycle or jump) every sample due in (t, t'], in time
+          order, before the boundary's completions, with a = afs_alpha (one interval elapsed).  With afs_half_life_ns = 0
+          a sample resets consumed to empty.  A sample sets LastUpdate to its due time;
+       2. an admission at t_c of a workload of LocalQueue l (workload_controller.go:965-971,1030-1056): its cells join
+          adm[l], consumed = Decay(consumed, adm, t_c - LastUpdate) (+) entry penalty, LastUpdate = t_c.  The penalty
+          goes into consumed, not into the pending penalties (lq_penalty stays as the snapshot gave it);
+       3. a completion takes its row's cells out of adm[adm_lq[row]]; consumed changes at the next sample;
+       4. the LocalQueue usage of the queue order is recomputed whenever consumed changes.
+     Canonical choices: samples do not wake the clock (a quiet cycle still waits for the next arrival or completion,
+     and the drain still ends without one); the early resample while penalties are pending (HasPendingFor,
+     localqueue_controller.go:219) is not modelled; 0.5^x is the library's afs_half_pow (kb_drain.cuh; Go's math.Pow
+     bits depend on the platform), restated in kueue_b200/drain.py.  A LocalQueue without a cache entry is initialised
+     by the caller as initializeAfsIfNeeded does (localqueue_controller.go:327-353): consumed = its admitted usage,
+     LastUpdate = now_ns.  A drain that runs no cycle (max_cycles = 0, no pending workload) takes no sample.
+     Errors (KB_ERR_INVALID): the tables without wl_lq or outside event mode, afs_half_life_ns < 0,
+     afs_sampling_ns <= 0, afs_alpha outside [0, 1) or non-zero with half-life 0, lq_last_update_ns[l] > now_ns,
+     adm_lq NULL while n_adm > 0, adm_lq[a] outside [-1, n_lq) or lq_cq[adm_lq[a]] != adm_cq[a]. */
+  int64_t afs_half_life_ns;         /* UsageHalfLifeTime (>= 0, pkg/config/validation.go:360-366)                   */
+  int64_t afs_sampling_ns;          /* UsageSamplingInterval (> 0)                                                 */
+  const int64_t *lq_last_update_ns; /* [n_lq] AfsConsumedResources LastUpdate, each <= now_ns; NULL = no decay      */
+  const int32_t *adm_lq;            /* [n_adm] LocalQueue of each admitted row, -1 for none                         */
 } kb_snapshot;
 
 /* ------------------------------------------------------------------------
@@ -421,7 +455,7 @@ int32_t kb_download(kb_handle *h, kb_cycle_out *out);
  * cmp.Compare — NaN first —, -priority, timestamp, UID) among the segments' heads, and every admission adds its entry
  * penalty to its LocalQueue before the next cycle.  StrictFIFO keeps the head (the next cycle picks the minimum again),
  * BestEffortFIFO advances the head's own segment, the scheduling-hash move covers every segment of the ClusterQueue.
- * Consumed usage does not decay inside a drain (CalculateDecayedConsumed is the LocalQueue reconciler's).
+ * Consumed usage does not decay inside a drain, except in event mode with kb_snapshot.lq_last_update_ns (see there).
  *
  * Event mode (kb_snapshot.wl_create_ns / wl_run_ns / adm_finish_ns, any non-NULL): a simulated clock t starts at
  * now_ns; cycle c runs at t_c (its now_ns and the QuotaReserved time of its admissions).  Two more queue states:
@@ -480,6 +514,12 @@ typedef struct kb_drain_out {
   int32_t *cycle_arrived;    /* [max_cycles] arrivals, likewise */
   int64_t *wl_admit_ns;      /* [n_wl] time of the workload's last admission, INT64_MIN if never admitted */
   int64_t *wl_finish_ns;     /* [n_wl] finish time, INT64_MAX if it has not finished */
+  /* decay of consumed usage (kb_snapshot.lq_last_update_ns != NULL; untouched otherwise; each pointer may be NULL):
+     the AfsConsumedResources entries after the drain, for AfsConsumedResources.Set */
+  int64_t *lq_consumed;       /* [n_lq][R] int64Amount values (0 = absent) */
+  int32_t *lq_consumed_scale; /* [n_lq][R] their scales */
+  int64_t *lq_last_update_ns; /* [n_lq] LastUpdate */
+  int64_t n_afs_samples;      /* out: decay samples due over the drain (those a fixed point skips included); 0 without decay */
 } kb_drain_out;
 int32_t kb_run_drain(kb_handle *h, const kb_snapshot *s, kb_drain_out *out);
 

@@ -429,6 +429,12 @@ func (s *Scheduler) flattenAFS(f *flat, wlQueue []utilqueue.LocalQueueReference)
 	c.n_lq, c.wl_lq, c.lq_cq, c.cq_afs = C.int32_t(len(lqKeys)), cp32(wlLq), cp32(lqCq), cpU8(cqAfs)
 	c.lq_weight, c.lq_consumed, c.lq_consumed_scale = cpF64(lqWeight), cp64(consumed), cp32(scale)
 	c.lq_penalty, c.afs_res_weight, c.afs_milli_mul, c.afs_alpha = cp64(penalty), cpF64(resWeight), cp64(milliMul), C.double(alpha)
+	// Decay of consumed usage in an event drain (INTEGRATION.md): a LocalQueue without a cache entry is initialised as
+	// initializeAfsIfNeeded does (consumed = its admitted usage, LastUpdate = now), then
+	//   c.afs_half_life_ns, c.afs_sampling_ns = C.int64_t(cfg.UsageHalfLifeTime.Nanoseconds()), C.int64_t(cfg.UsageSamplingInterval.Nanoseconds())
+	//   c.lq_last_update_ns, c.adm_lq = cp64(lastUpdate), cp32(admLq)   // entry.LastUpdate.UnixNano(); LocalQueue per admitted row, -1 for none
+	// and after kb_run_drain: s.queues.AfsConsumedResources.Set(key, consumed from out.lq_consumed / lq_consumed_scale,
+	// time.Unix(0, out.lq_last_update_ns[l])).  A single cycle leaves them nil.
 	return nil
 }
 

@@ -80,6 +80,8 @@ class kb_snapshot(C.Structure):
         ("adm_wl", _P(C.c_int32)),
         ("drain_cycle_ns", C.c_int64), ("wl_create_ns", _P(C.c_int64)), ("wl_run_ns", _P(C.c_int64)),
         ("adm_finish_ns", _P(C.c_int64)),
+        ("afs_half_life_ns", C.c_int64), ("afs_sampling_ns", C.c_int64), ("lq_last_update_ns", _P(C.c_int64)),
+        ("adm_lq", _P(C.c_int32)),
     ]
 
 
@@ -127,6 +129,8 @@ class kb_drain_out(C.Structure):
         ("n_finished", C.c_int64), ("n_arrived", C.c_int64), ("end_ns", C.c_int64),
         ("cycle_start_ns", _P(C.c_int64)), ("cycle_finished", _P(C.c_int32)), ("cycle_arrived", _P(C.c_int32)),
         ("wl_admit_ns", _P(C.c_int64)), ("wl_finish_ns", _P(C.c_int64)),
+        ("lq_consumed", _P(C.c_int64)), ("lq_consumed_scale", _P(C.c_int32)), ("lq_last_update_ns", _P(C.c_int64)),
+        ("n_afs_samples", C.c_int64),
     ]
 
 
@@ -180,13 +184,17 @@ _DT = {
     "lq_consumed_scale": np.int32, "lq_penalty": np.int64, "afs_res_weight": np.float64, "afs_milli_mul": np.int64,
     "adm_wl": np.int32,
     "wl_create_ns": np.int64, "wl_run_ns": np.int64, "adm_finish_ns": np.int64,
+    "lq_last_update_ns": np.int64, "adm_lq": np.int32,
 }
 # AdmissionFairSharing tables (include/kueue_b200.h): wl_lq absent = AFS off
 AFS_FIELDS = ("wl_lq", "lq_cq", "cq_afs", "lq_weight", "lq_consumed", "lq_consumed_scale", "lq_penalty", "afs_res_weight",
               "afs_milli_mul")
 # arrivals and completions of kb_run_drain's event mode (include/kueue_b200.h): all absent = event mode off
 EVENT_FIELDS = ("wl_create_ns", "wl_run_ns", "adm_finish_ns")
-OPTIONAL_FIELDS = ("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows", "adm_wl") + AFS_FIELDS + EVENT_FIELDS  # NULL in kb_snapshot when absent
+# decay of the AdmissionFairSharing consumed usage in event mode (include/kueue_b200.h): lq_last_update_ns absent = off
+AFS_DECAY_FIELDS = ("lq_last_update_ns", "adm_lq")
+OPTIONAL_FIELDS = (("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows", "adm_wl") + AFS_FIELDS +
+                   EVENT_FIELDS + AFS_DECAY_FIELDS)  # NULL in kb_snapshot when absent
 ARRAY_FIELDS = list(_DT.keys())
 # tables the library keeps resident while kb_snapshot.static_generation is unchanged (include/kueue_b200.h)
 STATIC_FIELDS = ("parent", "fair_weight", "nominal", "borrow_limit", "lend_limit", "cq_within_cq", "cq_reclaim_within",
@@ -216,6 +224,8 @@ class FlatSnapshot:
     static_generation: int = 0
     afs_alpha: float = 0.0  # kb_snapshot.afs_alpha: entry-penalty rate of AdmissionFairSharing
     drain_cycle_ns: int = 0  # kb_snapshot.drain_cycle_ns: simulated time of one drain cycle (<= 0 means 1)
+    afs_half_life_ns: int = 0  # kb_snapshot.afs_half_life_ns: UsageHalfLifeTime (decay of consumed usage)
+    afs_sampling_ns: int = 0   # kb_snapshot.afs_sampling_ns: UsageSamplingInterval
     arrays: dict = field(default_factory=dict)
 
     def __getattr__(self, name):
@@ -311,6 +321,7 @@ class FlatSnapshot:
             s.flags, s.now_ns, s.static_generation = self.flags, self.now_ns, self.static_generation
             s.afs_alpha = self.afs_alpha
             s.drain_cycle_ns = self.drain_cycle_ns
+            s.afs_half_life_ns, s.afs_sampling_ns = self.afs_half_life_ns, self.afs_sampling_ns
             return s
         s = kb_snapshot()
         s.n_cq, s.n_cohort, s.n_flavor, s.n_resource = self.n_cq, self.n_cohort, self.n_flavor, self.n_resource
@@ -323,6 +334,7 @@ class FlatSnapshot:
         s.n_lq = len(self.arrays["lq_cq"]) if "lq_cq" in self.arrays else 0
         s.afs_alpha = self.afs_alpha
         s.drain_cycle_ns = self.drain_cycle_ns
+        s.afs_half_life_ns, s.afs_sampling_ns = self.afs_half_life_ns, self.afs_sampling_ns
         for name in ARRAY_FIELDS:
             if name in OPTIONAL_FIELDS and name not in self.arrays:
                 continue  # stays NULL
@@ -409,6 +421,10 @@ class DrainOut:
         self.cycle_arrived = np.zeros(max_cycles, np.int32)
         self.wl_admit_ns = np.full(W, KB_TS_UNSET, np.int64)
         self.wl_finish_ns = np.full(W, KB_NO_LIMIT, np.int64)
+        L = len(snap.arrays["lq_cq"]) if "lq_cq" in snap.arrays else 0
+        self.lq_consumed = np.zeros((max(1, L), R), np.int64)[:L]  # decay of consumed usage: the entries after the drain
+        self.lq_consumed_scale = np.zeros((max(1, L), R), np.int32)[:L]
+        self.lq_last_update_ns = np.zeros(max(1, L), np.int64)[:L]
         cap = (min(W * 4 + Q, min(Q, W) * max_cycles) if trace_capacity is None else trace_capacity) if trace else 0
         self.trace_wl = np.zeros(max(1, cap), np.int32)
         self.trace_decision = np.zeros(max(1, cap), np.uint8)
@@ -423,6 +439,8 @@ class DrainOut:
         s.cycle_start_ns = _ptr(self.cycle_start_ns, C.c_int64)
         s.cycle_finished = _ptr(self.cycle_finished, C.c_int32); s.cycle_arrived = _ptr(self.cycle_arrived, C.c_int32)
         s.wl_admit_ns = _ptr(self.wl_admit_ns, C.c_int64); s.wl_finish_ns = _ptr(self.wl_finish_ns, C.c_int64)
+        s.lq_consumed = _ptr(self.lq_consumed, C.c_int64); s.lq_consumed_scale = _ptr(self.lq_consumed_scale, C.c_int32)
+        s.lq_last_update_ns = _ptr(self.lq_last_update_ns, C.c_int64)
         if trace:
             s.trace_wl = _ptr(self.trace_wl, C.c_int32); s.trace_decision = _ptr(self.trace_decision, C.c_uint8)
         s.trace_capacity = cap
@@ -444,6 +462,8 @@ class DrainOut:
     def n_arrived(self): return int(self.struct.n_arrived)
     @property
     def end_ns(self): return int(self.struct.end_ns)
+    @property
+    def n_afs_samples(self): return int(self.struct.n_afs_samples)
 
     def cycles(self):
         """[(heads, decisions)] per cycle from the trace."""

@@ -212,6 +212,39 @@ def _flatten_afs(snap, idx, cqs, pending, local_queues, afs_config, consumed, pe
     snap.afs_alpha = afs_config.alpha if on else 0.0
 
 
+def add_afs_decay(snap, afs_config: AdmissionFairSharing, last_update_ns, adm_lq):
+    """Decay tables of an event drain (kb_snapshot.afs_half_life_ns, afs_sampling_ns, lq_last_update_ns, adm_lq;
+    include/kueue_b200.h) on a snapshot that carries the AdmissionFairSharing tables.  `last_update_ns[l]`: LastUpdate of
+    LocalQueue l's AfsConsumedResources entry, None where the cache has no entry yet: such a LocalQueue is initialised
+    as initializeAfsIfNeeded does (localqueue_controller.go:327-353), consumed = its admitted usage (GetAdmittedUsage,
+    flattened over flavors, as milli-units) and LastUpdate = now_ns.  `adm_lq[a]`: LocalQueue of admitted row a, -1
+    for none.  Durations in seconds as in the Configuration."""
+    a, R = snap.arrays, snap.n_resource
+    L = len(a["lq_cq"])
+    adm_lq = np.asarray(adm_lq, np.int64)
+    assert len(last_update_ns) == L and len(adm_lq) == snap.n_adm
+    adm = np.zeros((L, R), np.int64)  # admitted usage per LocalQueue in library units
+    us = a["adm_use_start"]
+    for row in np.flatnonzero(adm_lq >= 0):
+        for k in range(int(us[row]), int(us[row + 1])):
+            adm[adm_lq[row], int(a["adm_use_fr"][k]) % R] += int(a["adm_use_qty"][k])
+    cons = a["lq_consumed"].reshape(L, R).copy()
+    sc = a["lq_consumed_scale"].reshape(L, R).copy()
+    last = np.zeros(L, np.int64)
+    for l, t in enumerate(last_update_ns):
+        if t is None:
+            cons[l], sc[l] = adm[l] * a["afs_milli_mul"], -3
+            last[l] = snap.now_ns
+        else:
+            last[l] = int(t)
+    snap.set("lq_consumed", cons); snap.set("lq_consumed_scale", sc)
+    snap.set("lq_last_update_ns", last); snap.set("adm_lq", adm_lq)
+    snap.afs_half_life_ns = int(round(afs_config.usage_half_life_s * 1e9))
+    snap.afs_sampling_ns = int(round(afs_config.usage_sampling_s * 1e9))
+    snap.afs_alpha = afs_config.alpha
+    return snap
+
+
 class MakeCohort(_QuotaHolder):
     def __init__(self, name: str):
         super().__init__()

@@ -1378,6 +1378,23 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       for (int a = 0; a < s->n_adm; a++)
         if (s->wl_create_ns[s->adm_wl[a]] > s->now_ns) return fail(h, KB_ERR_INVALID, "adm_wl names a record created after now_ns");
   }
+  // ---- decay of AdmissionFairSharing consumed usage: host-side checks (include/kueue_b200.h)
+  const bool decay = s->lq_last_update_ns != nullptr;
+  if (decay) {
+    if (!s->wl_lq || !s->lq_cq || !events) return fail(h, KB_ERR_INVALID, "afs decay: lq_last_update_ns needs wl_lq and event mode");
+    if (s->afs_half_life_ns < 0 || s->afs_sampling_ns <= 0) return fail(h, KB_ERR_INVALID, "afs decay: half-life < 0 or sampling interval <= 0");
+    if (!(s->afs_alpha >= 0.0 && s->afs_alpha < 1.0) || (s->afs_half_life_ns == 0 && s->afs_alpha != 0.0))
+      return fail(h, KB_ERR_INVALID, "afs decay: afs_alpha outside [0, 1), or non-zero with half-life 0");
+    for (int l = 0; l < s->n_lq; l++)
+      if (s->lq_last_update_ns[l] > s->now_ns) return fail(h, KB_ERR_INVALID, "afs decay: lq_last_update_ns after now_ns");
+    if (s->n_adm > 0 && !s->adm_lq) return fail(h, KB_ERR_INVALID, "afs decay: adm_lq is NULL while n_adm > 0");
+    for (int a = 0; a < s->n_adm; a++) {
+      const int l = s->adm_lq[a];
+      if (l < -1 || l >= s->n_lq) return fail(h, KB_ERR_INVALID, "afs decay: adm_lq out of range");
+      if (l >= 0 && s->lq_cq[l] != s->adm_cq[a]) return fail(h, KB_ERR_INVALID, "afs decay: the LocalQueue of an admitted row feeds another ClusterQueue");
+    }
+  }
+  out->n_afs_samples = 0;
   if (Hcap == 0 || max_cycles == 0) return KB_OK;
   size_t extra = (size_t)std::min<long long>((long long)W, (long long)Hcap * max_cycles);
   h->drain_extra_adm = extra;
@@ -1476,6 +1493,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     need((size_t)Q + 1, 4); need(Lz, 4); need(seg_lq.size(), 4); need(afs_cqs.size() + 1, 4); need(Q, 4); need(Wz, 4); need(Q, 1);
     need(Lz, 8); need(LR, 8); need(LR, 4); need(LR, 8); need(Lz, 8); need(R, 8); need(R, 8);
   }
+  if (decay) { need(Lz, 8); need(LR, 8); need(Acap, 4); need(Acap, 4); need(1, 8); }
   if (tot > h->drain_buf_cap) {
     if (h->drain_buf) cudaFree(h->drain_buf);
   if (h->tas_buf) cudaFree(h->tas_buf);
@@ -1571,8 +1589,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     X.wl_lq = (const int32_t *)h2d(s->wl_lq, Wz, 4);
     X.cq_afs = (const uint8_t *)h2d(s->cq_afs, Q, 1);
     X.lq_weight = (const double *)h2d(s->lq_weight, L, 8);
-    X.lq_consumed = (const i64 *)h2d(s->lq_consumed, (size_t)L * R, 8);
-    X.lq_consumed_scale = (const int32_t *)h2d(s->lq_consumed_scale, (size_t)L * R, 4);
+    X.lq_consumed = (i64 *)h2d(s->lq_consumed, (size_t)L * R, 8);
+    X.lq_consumed_scale = (int32_t *)h2d(s->lq_consumed_scale, (size_t)L * R, 4);
     X.lq_penalty = (i64 *)take(LR, 8);
     if (s->lq_penalty) CUDA_TRY(h, cudaMemcpyAsync(X.lq_penalty, s->lq_penalty, (size_t)L * R * 8, cudaMemcpyHostToDevice, h->stream));
     else CUDA_TRY(h, cudaMemsetAsync(X.lq_penalty, 0, LR * 8, h->stream));
@@ -1584,6 +1602,21 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (!X.seg_start || !X.lq_seg || !X.seg_lq || !X.afs_cqs || !X.wl_lq || !X.cq_afs || !X.lq_weight || !X.lq_consumed ||
         !X.lq_consumed_scale || !X.lq_usage || !X.res_weight || !X.milli_mul)
       return fail(h, KB_ERR_CUDA, "afs: upload of the LocalQueue tables failed");
+  }
+  std::vector<i64> lq_adm;  // decay: the initial admitted usage of every LocalQueue (live rows of the snapshot)
+  if (decay) {
+    lq_adm.assign(LR, 0);
+    for (int a = 0; a < s->n_adm; a++)
+      if (s->adm_lq[a] >= 0)
+        for (int c = s->adm_use_start[a]; c < s->adm_use_start[a + 1]; c++) lq_adm[(size_t)s->adm_lq[a] * R + s->adm_use_fr[c] % R] += s->adm_use_qty[c];
+    X.lq_last = (i64 *)take(Lz, 8); X.lq_adm = (i64 *)take(LR, 8);
+    X.adm_lq = (int32_t *)take(Acap, 4); other.lq = (int32_t *)take(Acap, 4);
+    X.afs_samples = (unsigned long long *)take(1, 8);
+    if (L) CUDA_TRY(h, cudaMemcpyAsync(X.lq_last, s->lq_last_update_ns, (size_t)L * 8, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(X.lq_adm, lq_adm.data(), LR * 8, cudaMemcpyHostToDevice, h->stream));
+    if (s->n_adm) CUDA_TRY(h, cudaMemcpyAsync(X.adm_lq, s->adm_lq, (size_t)s->n_adm * 4, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(X.afs_samples, 0, 8, h->stream));
+    X.half_life_ns = s->afs_half_life_ns; X.sampling_ns = s->afs_sampling_ns;
   }
   // ---- per-ClusterQueue order (queueOrderingFunc): stable LSD passes uid -> timestamp -> (ClusterQueue | priority desc)
   const int tb = 256, nbW = (W + tb - 1) / tb, nbQ = (Q + tb - 1) / tb;
@@ -1612,6 +1645,11 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   if (events) k_drain_init_events<<<std::max(1, nbW), tb, 0, h->stream>>>(D, X, d_create, s->now_ns);
   if (replay || events) k_drain_init_replay<<<std::max(nbW, (s->n_adm + tb - 1) / tb), tb, 0, h->stream>>>(D, X, replay ? s->n_adm : 0);
   k_drain_advance<<<(S + tb - 1) / tb, tb, 0, h->stream>>>(X, S);
+  const int nbL = std::max(1, (L + tb - 1) / tb);
+  if (decay) {  // the samples due at or before now_ns (k_drain_init_events set clock[0] = now_ns), before the first heads
+    CUDA_TRY(h, cudaMemsetAsync(D.status, 0, 4, h->stream));
+    k_drain_afs_decay<<<nbL, tb, 0, h->stream>>>(D, X, L);
+  }
   int32_t *d_heads = const_cast<int32_t *>(D.heads);
   auto enqueue_heads = [&]() {
     k_drain_flag<<<nbQ, tb, 0, h->stream>>>(D, X);
@@ -1622,7 +1660,9 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   CUDA_TRY(h, cudaMemsetAsync(X.counters + 1, 0, 5 * 4, h->stream));
   enqueue_heads();
   CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[8], X.counters, 4, cudaMemcpyDeviceToHost, h->stream));
+  if (decay) CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[11], D.status, 4, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  if (decay && (h->host_words[11] & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: a decayed consumed quantity overflows int64");
   int n_live = (int)h->host_words[8];
   int A_cur = s->n_adm, AU_cur = s->n_adm_use;
   const bool pre = h->preempt_possible;
@@ -1663,6 +1703,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     const int nbB = std::max(1, (bound + tb - 1) / tb);
     k_drain_ev_min<<<nbB, tb, 0, h->stream>>>(X, bound, n_new_d);
     k_drain_ev_next<<<1, 1, 0, h->stream>>>(X, t, step, jump, n_new_d);
+    if (decay) k_drain_afs_decay<<<nbL, tb, 0, h->stream>>>(D, X, L);  // samples due in (t, t_{c+1}], before the completions
     k_drain_finish<<<nbB, tb, 0, h->stream>>>(D, X, bound, n_new_d);
     if (X.arr_key) k_drain_arrive<<<nbArr, tb, 0, h->stream>>>(X);
     k_drain_requeue<<<nbQ, tb, 0, h->stream>>>(D, X);
@@ -1682,7 +1723,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     CUDA_TRY(h, cudaEventRecord(h->ev_d, h->stream));
     CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[8], X.counters, 4, cudaMemcpyDeviceToHost, h->stream));
     if (!jump) CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[9], n_new_d, 4, cudaMemcpyDeviceToHost, h->stream));
-    if (afs && !jump) CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[11], D.status, 4, cudaMemcpyDeviceToHost, h->stream));
+    if (afs && (!jump || decay)) CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[11], D.status, 4, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[12], X.counters + 1, 10 * 4, cudaMemcpyDeviceToHost, h->stream));  // .. [KB_DC_ARR_HI]
     CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[22], X.clock, 8, cudaMemcpyDeviceToHost, h->stream));             // t_{c+1}
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
@@ -1692,6 +1733,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       if (afs && (h->host_words[11] & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: an entry penalty overflows int64");
       for (int i = 0; i < KB_N_KERNELS; i++) kms[i] += h->stats.kernel_ms[i];
     }
+    if (decay && (h->host_words[11] & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: a decayed consumed quantity overflows int64");
     { float ms = 0; cudaEventElapsedTime(&ms, h->ev2, h->ev_d); gpu_ms += ms; }
     if (h->host_words[16]) return fail(h, KB_ERR_CAPACITY, "kb_run_drain: the admitted tables are full");
     const int fin = (int)h->host_words[12 + KB_DC_FINISHED - 1], arr = (int)h->host_words[12 + KB_DC_ARRIVED - 1];
@@ -1718,10 +1760,10 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     }
     // the compacted half becomes the admitted tables of the next boundary
     A_cur = (int)h->host_words[13]; AU_cur = (int)h->host_words[14];
-    AdmTabs cur{X.adm_cq, X.adm_priority, X.adm_ts, X.adm_qr_ts, X.adm_uid, X.adm_evicted, X.adm_use_start, X.adm_use_fr, X.adm_use_qty, X.adm_wl, X.adm_finish};
+    AdmTabs cur{X.adm_cq, X.adm_priority, X.adm_ts, X.adm_qr_ts, X.adm_uid, X.adm_evicted, X.adm_use_start, X.adm_use_fr, X.adm_use_qty, X.adm_wl, X.adm_finish, X.adm_lq};
     X.adm_cq = other.cq; X.adm_priority = other.priority; X.adm_ts = other.ts; X.adm_qr_ts = other.qr_ts; X.adm_uid = other.uid;
     X.adm_evicted = other.evicted; X.adm_use_start = other.use_start; X.adm_use_fr = other.use_fr; X.adm_use_qty = other.use_qty; X.adm_wl = other.wl;
-    X.adm_finish = other.finish;
+    X.adm_finish = other.finish; X.adm_lq = other.lq;
     D.adm_cq = X.adm_cq; D.adm_priority = X.adm_priority; D.adm_ts = X.adm_ts; D.adm_qr_ts = X.adm_qr_ts; D.adm_uid = X.adm_uid;
     D.adm_evicted = X.adm_evicted; D.adm_use_start = X.adm_use_start; D.adm_use_fr = X.adm_use_fr; D.adm_use_qty = X.adm_use_qty;
     other = cur;
@@ -1803,6 +1845,12 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   if (out->wl_evals) CUDA_TRY(h, cudaMemcpyAsync(out->wl_evals, X.wl_evals, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
   if (events && out->wl_admit_ns) CUDA_TRY(h, cudaMemcpyAsync(out->wl_admit_ns, X.wl_admit_ns, Wz * 8, cudaMemcpyDeviceToHost, h->stream));
   if (events && out->wl_finish_ns) CUDA_TRY(h, cudaMemcpyAsync(out->wl_finish_ns, X.wl_finish_ns, Wz * 8, cudaMemcpyDeviceToHost, h->stream));
+  if (decay) {
+    if (out->lq_consumed && L) CUDA_TRY(h, cudaMemcpyAsync(out->lq_consumed, X.lq_consumed, (size_t)L * R * 8, cudaMemcpyDeviceToHost, h->stream));
+    if (out->lq_consumed_scale && L) CUDA_TRY(h, cudaMemcpyAsync(out->lq_consumed_scale, X.lq_consumed_scale, (size_t)L * R * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (out->lq_last_update_ns && L) CUDA_TRY(h, cudaMemcpyAsync(out->lq_last_update_ns, X.lq_last, (size_t)L * 8, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(&out->n_afs_samples, X.afs_samples, 8, cudaMemcpyDeviceToHost, h->stream));
+  }
   if (out->wl_evictions) {
     if (replay) CUDA_TRY(h, cudaMemcpyAsync(out->wl_evictions, X.wl_evictions, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
     else memset(out->wl_evictions, 0, Wz * 4);

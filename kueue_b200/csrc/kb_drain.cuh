@@ -25,7 +25,10 @@
 // LocalQueue (each sorted as above, each with its own cursor); every other ClusterQueue is one segment.  Segments are
 // numbered ClusterQueue-major (seg_start[Q+1]).  The head of an AFS ClusterQueue is the minimum of (LocalQueue usage by
 // cmp.Compare, -priority, timestamp, UID) over the heads of its segments (one warp per ClusterQueue, k_drain_afs_heads);
-// an admission adds its entry penalty to its LocalQueue and recomputes that LocalQueue's usage (k_drain_admit).
+// an admission adds its entry penalty to its LocalQueue and recomputes that LocalQueue's usage (k_drain_admit).  In event
+// mode with lq_last_update_ns the consumed usage decays (include/kueue_b200.h): k_drain_afs_decay takes the samples due
+// at the start and at every boundary, k_drain_admit decays to t_c and puts the penalty into consumed, k_drain_finish
+// takes finished rows out of the LocalQueue's admitted usage (adm_lq, carried by the compaction).
 //
 // Event mode (kb_snapshot.wl_create_ns / wl_run_ns / adm_finish_ns; include/kueue_b200.h): two more states,
 // KB_WS_ABSENT (not created yet) and KB_WS_FINISHED.  Every admitted row carries its finish time (adm_finish, written by
@@ -97,6 +100,67 @@ __host__ __device__ inline bool afs_lq_usage(const i64 *consumed, const int32_t 
   return true;
 }
 
+// ---- decay of consumed usage (CalculateDecayedConsumed, admission_fair_sharing.go:39-66) ---------------------------
+// 0.5^x for x >= 0 in plain fp64 operations, restated operation for operation by kueue_b200/drain.py half_pow, so the
+// device and the host definition agree bit for bit (Go's math.Pow bits depend on the platform).  Go's Pow for base 0.5:
+// x = yi + yf with |yf| <= 0.5, 0.5^yf = exp(yf * Log(0.5)) by the fdlibm reduction and polynomial of Go's exp, then
+// ldexp by -yi.  Exactly 1 at 0 and 2^-n at an integer n.  Built with -fmad=false (host: -ffp-contract=off).
+__host__ __device__ inline double afs_half_pow(double x) {
+  double yi = trunc(x), yf = x - yi;
+  if (yf > 0.5) { yf -= 1.0; yi += 1.0; }
+  if (yi >= 2048.0) return 0.0;
+  const double v = yf * -0.6931471805599453;
+  double a;
+  if (-3.725290298461914e-09 < v && v < 3.725290298461914e-09) {
+    a = 1.0 + v;  // |v| < 2^-28
+  } else {
+    const double Ln2Hi = 6.93147180369123816490e-01, Ln2Lo = 1.90821492927058770002e-10, Log2e = 1.44269504088896338700e+00;
+    const double P1 = 1.66666666666666657415e-01, P2 = -2.77777777770155933842e-03, P3 = 6.61375632143793436117e-05,
+                 P4 = -1.65339022054652515390e-06, P5 = 4.13813679705723846039e-08;
+    const int k = v < 0 ? (int)(Log2e * v - 0.5) : (int)(Log2e * v + 0.5);
+    const double hi = v - (double)k * Ln2Hi, lo = (double)k * Ln2Lo;
+    const double r = hi - lo, t = r * r;
+    const double c = r - t * (P1 + t * (P2 + t * (P3 + t * (P4 + t * P5))));
+    a = ldexp(1.0 - ((lo - (r * c) / (2.0 - c)) - hi), k);
+  }
+  return ldexp(a, -(int)yi);
+}
+// Duration.Seconds(): whole seconds and the remainder converted separately
+__host__ __device__ inline double afs_seconds(i64 d) { return (double)(d / 1000000000ll) + (double)(d % 1000000000ll) / 1e9; }
+// calculateAlphaRate(elapsed, halfLife) on durations in ns: 1 - 0.5^(elapsed / halfLife), 0 when halfLife is 0
+__host__ __device__ inline double afs_alpha_of(i64 elapsed_ns, i64 half_life_ns) {
+  return half_life_ns == 0 ? 0.0 : 1.0 - afs_half_pow(afs_seconds(elapsed_ns) / afs_seconds(half_life_ns));
+}
+// Quantity.MilliValue of (v, s) (int64Amount.AsScaledInt64(-3)): a coarser scale multiplies (false on overflow), a finer
+// one divides and rounds away from zero (negativeScaleInt64, apimachinery math.go:166-198)
+__host__ __device__ inline bool afs_milli(i64 v, int s, i64 *out) {
+  if (s >= -3) return afs_scale_up(v, s + 3, out);
+  i64 q = v;
+  bool frac = false;
+  for (int i = 0; i < -3 - s; i++) { frac |= q % 10 != 0; q /= 10; }
+  *out = frac ? (v > 0 ? q + 1 : q - 1) : q;
+  return true;
+}
+// consumed = MulByFloat(consumed, 1 - alpha) (+) MulByFloat(admitted, alpha) for one LocalQueue, every resource written
+// back as (milli, -3); admitted usage in library units, MilliValue = adm * milli_mul.  *changed: some pair differs.
+// false = int64 overflow.
+__host__ __device__ inline bool afs_decay(i64 *cons, int32_t *scale, const i64 *adm, const i64 *milli_mul, double alpha, int R,
+                                          bool *changed) {
+  const double keep = 1.0 - alpha;
+  bool ok = true;
+  for (int r = 0; r < R; r++) {
+    i64 old_m = 0, new_m = 0, sum = 0;
+    if (!afs_milli(cons[r], scale[r], &old_m)) { ok = false; continue; }
+    const i64 mul = milli_mul[r];
+    if (adm[r] > INT64_MAX / mul || adm[r] < -INT64_MAX / mul) { ok = false; continue; }
+    new_m = adm[r] * mul;
+    if (!afs_add64((i64)((double)old_m * keep), (i64)((double)new_m * alpha), &sum)) { ok = false; continue; }
+    if (sum != cons[r] || scale[r] != -3) *changed = true;
+    cons[r] = sum; scale[r] = -3;
+  }
+  return ok;
+}
+
 struct DrainDev {
   // queues
   int32_t *q_order, *q_start, *cursor; uint8_t *wl_state;  // wl_state: KB_WS_* per pending workload
@@ -126,11 +190,18 @@ struct DrainDev {
   const int32_t *seg_lq;      // [S] LocalQueue of a segment of an AFS ClusterQueue
   const int32_t *afs_cqs;     // [n_afs_cq] ClusterQueues with cq_afs set
   int32_t *head_seg;          // [Q] segment of this cycle's head
-  const int32_t *wl_lq, *lq_consumed_scale; const uint8_t *cq_afs; const double *lq_weight, *res_weight;
-  const i64 *lq_consumed, *milli_mul;
+  const int32_t *wl_lq; const uint8_t *cq_afs; const double *lq_weight, *res_weight;
+  const i64 *milli_mul;
+  i64 *lq_consumed; int32_t *lq_consumed_scale;  // device copies: decay rewrites them
   i64 *lq_penalty; double *lq_usage;
   double alpha;
   int n_afs_cq;
+  // decay of consumed usage (event mode); lq_last == nullptr: off
+  i64 *lq_last;               // [n_lq] LastUpdate of the consumed usage
+  i64 *lq_adm;                // [n_lq][R] admitted usage in library units: cells of the LocalQueue's live rows
+  int32_t *adm_lq;            // [A_cap] LocalQueue of each admitted row (current half), -1 = none
+  unsigned long long *afs_samples;  // [1] samples taken
+  i64 half_life_ns, sampling_ns;
   // event mode; adm_finish == nullptr: off
   i64 *adm_finish;                 // [A_cap] finish time of each admitted row (current half), INT64_MAX = never
   const i64 *wl_run;               // [W] run time once admitted (< 0 never finishes); null = none finishes
@@ -338,6 +409,7 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts, const int32_t *b
   int c0 = (base ? base[1] : X.AU) + X.e_cell_off[e];
   if (a >= X.A_cap || c0 + X.e_ncells[e] > X.AU_cap) { atomicOr(&X.counters[5], 1); return; }  // nothing past the end
   if (X.adm_wl) X.adm_wl[a] = wl;
+  if (X.adm_lq) X.adm_lq[a] = X.wl_lq[wl];
   X.adm_cq[a] = cq; X.adm_priority[a] = D.wl_priority[wl]; X.adm_ts[a] = D.wl_ts[wl]; X.adm_qr_ts[a] = qr_ts;
   X.adm_uid[a] = D.wl_uid[wl]; X.adm_evicted[a] = 0;
   X.adm_use_start[a] = c0;
@@ -367,9 +439,20 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts, const int32_t *b
     // (the full TotalRequests, partial admission does not reduce it), int64(float64(MilliValue) * alpha) milli-units,
     // pushed into the LocalQueue's penalties (AfsEntryPenalties.Push: Quantity.Add at scale -3).  A ClusterQueue admits
     // one entry per cycle and a LocalQueue belongs to one ClusterQueue: one writer per LocalQueue, no atomics.
+    // With decay (workload_controller.go:965-971,1030-1056): the cells join the LocalQueue's admitted usage, consumed
+    // decays over t_c - LastUpdate, LastUpdate = t_c, and the penalty goes into consumed instead of the pending ones.
     const int lq = X.wl_lq[wl];
     i64 *pen = X.lq_penalty + (size_t)lq * R;
+    i64 *cons = X.lq_consumed + (size_t)lq * R;
+    int32_t *csc = X.lq_consumed_scale + (size_t)lq * R;
     bool bad = false;
+    if (X.lq_last) {
+      i64 *adm = X.lq_adm + (size_t)lq * R;
+      for (int j = 0; j < n; j++) adm[X.adm_use_fr[c0 + j] % R] += X.adm_use_qty[c0 + j];
+      bool changed = false;
+      bad |= !afs_decay(cons, csc, adm, X.milli_mul, afs_alpha_of(qr_ts - X.lq_last[lq], X.half_life_ns), R, &changed);
+      X.lq_last[lq] = qr_ts;
+    }
     for (int r = 0; r < R; r++) {
       i64 total = 0;
       for (int row = ps0; row < ps1; row++)
@@ -378,10 +461,11 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts, const int32_t *b
       const i64 mul = X.milli_mul[r];
       if (total > INT64_MAX / mul || total < -INT64_MAX / mul) { bad = true; continue; }
       const i64 delta = (i64)((double)(total * mul) * X.alpha);
-      bad |= !afs_add64(pen[r], delta, &pen[r]);
+      if (X.lq_last) { int s; bad |= !afs_qty_add(cons[r], csc[r], delta, -3, &cons[r], &s); csc[r] = s; }
+      else bad |= !afs_add64(pen[r], delta, &pen[r]);
     }
     double u = 0.0;
-    bad |= !afs_lq_usage(X.lq_consumed + (size_t)lq * R, X.lq_consumed_scale + (size_t)lq * R, pen, X.res_weight, X.lq_weight[lq], R, &u);
+    bad |= !afs_lq_usage(cons, csc, pen, X.res_weight, X.lq_weight[lq], R, &u);
     X.lq_usage[lq] = u;
     if (bad) atomicOr(D.status, KBS_AFS_OVERFLOW);
   }
@@ -433,7 +517,7 @@ __global__ void k_drain_live(DrainDev X) {
   X.row_live[a] = live;
   X.row_cells[a] = live ? X.adm_use_start[a + 1] - X.adm_use_start[a] : 0;
 }
-struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; i64 *finish; };
+struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; i64 *finish; int32_t *lq; };
 // live rows, in order, into the other half of the double buffer; thread A writes the totals (counters[2..3])
 __global__ void k_drain_compact(DrainDev X, AdmTabs O) {
   int a = blockIdx.x * blockDim.x + threadIdx.x;
@@ -444,6 +528,7 @@ __global__ void k_drain_compact(DrainDev X, AdmTabs O) {
   O.cq[n] = X.adm_cq[a]; O.priority[n] = X.adm_priority[a]; O.ts[n] = X.adm_ts[a]; O.qr_ts[n] = X.adm_qr_ts[a];
   O.uid[n] = X.adm_uid[a]; O.evicted[n] = X.adm_evicted[a]; O.wl[n] = X.adm_wl[a]; O.use_start[n] = c0;
   if (X.adm_finish) O.finish[n] = X.adm_finish[a];
+  if (X.adm_lq) O.lq[n] = X.adm_lq[a];
   for (int c = 0; c < nc; c++) { O.use_fr[c0 + c] = X.adm_use_fr[u0 + c]; O.use_qty[c0 + c] = X.adm_use_qty[u0 + c]; }
 }
 
@@ -468,7 +553,7 @@ __global__ void k_drain_keys_create(int W, const i64 *create, u64 *keys, int32_t
 __global__ void k_drain_init_events(DevSnap D, DrainDev X, const i64 *create, i64 now_ns) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i == 0) {
-    X.clock[1] = INT64_MAX;
+    X.clock[0] = now_ns; X.clock[1] = INT64_MAX;
     const int lo = X.arr_key ? ev_upper_bound(X.arr_key, 0, X.n_arr, now_ns) : 0;
     X.counters[KB_DC_ARR_LO] = lo; X.counters[KB_DC_ARR_HI] = lo;
   }
@@ -520,8 +605,50 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
     atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
   const int w = X.adm_wl[a];
   if (w >= 0) { X.wl_state[w] = KB_WS_FINISHED; X.wl_admit_cycle[w] = -1; X.wl_finish_ns[w] = X.adm_finish[a]; }
+  if (X.lq_last && X.adm_lq[a] >= 0 && X.cq_afs[cq]) {  // several rows of one LocalQueue can finish together
+    i64 *adm = X.lq_adm + (size_t)X.adm_lq[a] * D.R;
+    for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)
+      atomicAdd((unsigned long long *)&adm[X.adm_use_fr[c] % D.R], (unsigned long long)(-X.adm_use_qty[c]));
+  }
   X.root_mark[D.root_slot[cq]] = stamp;
   atomicAdd(&X.counters[KB_DC_FINISHED], 1);
+}
+// decay samples (thread per LocalQueue of an AFS ClusterQueue): every sample due in (t, t'] with t' = clock[0], in time
+// order, each with alpha = afs_alpha (one interval elapsed), or a reset to empty with half-life 0; LastUpdate moves to
+// each due time.  Launched after k_drain_ev_next and before k_drain_finish, so the samples see the admitted usage the
+// cycle left.  Nothing is due at or before t (the previous boundary took those samples, an admission at t sets
+// LastUpdate = t), so a drain that ends (clock[0] = t) takes none.  The admitted usage is constant here: once a sample
+// leaves consumed unchanged so do the later ones, and LastUpdate jumps to the last due time.  AFS drains cannot evict
+// (the preemption guard), so k_drain_evict never changes the admitted usage.
+__global__ void k_drain_afs_decay(DevSnap D, DrainDev X, int L) {
+  const int l = blockIdx.x * blockDim.x + threadIdx.x;
+  if (l >= L || X.lq_seg[l] < 0) return;
+  const int R = D.R;
+  const i64 last = X.lq_last[l];
+  const u64 gap = (u64)X.clock[0] - (u64)last, samp = (u64)X.sampling_ns;  // t' >= LastUpdate
+  if (gap < samp) return;
+  const u64 due = gap / samp;
+  i64 *cons = X.lq_consumed + (size_t)l * R;
+  int32_t *csc = X.lq_consumed_scale + (size_t)l * R;
+  bool bad = false, any = false;
+  for (u64 k = 0; k < due; k++) {
+    bool changed = false;
+    if (X.half_life_ns == 0) {
+      for (int r = 0; r < R; r++) { changed |= cons[r] != 0 || csc[r] != 0; cons[r] = 0; csc[r] = 0; }
+    } else {
+      bad |= !afs_decay(cons, csc, X.lq_adm + (size_t)l * R, X.milli_mul, X.alpha, R, &changed);
+    }
+    if (!changed || bad) break;
+    any = true;
+  }
+  X.lq_last[l] = last + (i64)(due * samp);
+  atomicAdd(X.afs_samples, (unsigned long long)due);
+  if (any) {
+    double u = 0.0;
+    bad |= !afs_lq_usage(cons, csc, X.lq_penalty + (size_t)l * R, X.res_weight, X.lq_weight[l], R, &u);
+    X.lq_usage[l] = u;
+  }
+  if (bad) atomicOr(D.status, KBS_AFS_OVERFLOW);
 }
 // arrivals (grid-stride over the arrived prefix [lo, hi)): the workload joins its queue and the cursor moves back to it;
 // in a BestEffortFIFO ClusterQueue a known hash in the NoFit set sets it aside (PushOrUpdate, cluster_queue.go:288-293)

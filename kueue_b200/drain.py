@@ -55,7 +55,7 @@ ClusterQueue with `cq_afs` set is one segment per LocalQueue, each in the static
   * LocalQueue usage is `lq_usage` (Info.CalcLocalQueueFSUsage, workload.go:391-427), summed in resource-index order
     (the reference sums over a map, in random order: resource-index order is the canonical choice);
   * every admission adds its entry penalty to its LocalQueue (`entry_penalty`; scheduler.go:727-742,946-960) before
-    the next cycle; consumed usage does not decay inside a drain;
+    the next cycle; consumed usage does not decay inside a drain, except in event mode with `lq_last_update_ns` (below);
   * StrictFIFO keeps its head (the next cycle picks the minimum again), BestEffortFIFO advances the head's own segment,
     handleInadmissibleHash sets aside the workloads of the class in every segment of the ClusterQueue.
 
@@ -86,9 +86,37 @@ Steps 5-7 only set state bytes and lower cursors: their order does not change th
 the canonical choice; with every run time < 0 and every creation <= now_ns the drain is the plain drain.  The drain
 stops before cycle max_cycles.  Events applied before cycle 0 count only in the totals; the events applied between the
 start of cycle c and the start of cycle c+1 are cycle c's (`finished`, `arrived`).
+
+Decay of the AdmissionFairSharing consumed usage (event mode, the snapshot carries `lq_last_update_ns` and `adm_lq`,
+include/kueue_b200.h), as the LocalQueue reconciler decays it (localqueue_controller.go:210-229,363-398):
+  1. state per LocalQueue of an AFS ClusterQueue: `consumed[r]` as int64Amount (value, scale), 0 = an absent key; `last`,
+     the entry's LastUpdate; `adm[r]`, the admitted usage in library units (the cells with fr % R == r of the
+     LocalQueue's live rows);
+  2. Decay(consumed, adm, elapsed) = MulByFloat(consumed, 1 - a) (+) MulByFloat(adm, a) with a = 1 - 0.5^(elapsed /
+     half-life) (CalculateDecayedConsumed, admission_fair_sharing.go:39-66): MulByFloat(q, f) = int64(float64(
+     MilliValue(q)) * f) milli-units (resource.go:72-99), `milli_value` rounds a finer scale away from zero
+     (negativeScaleInt64), the MilliValue of adm[r] is adm[r] * afs_milli_mul[r], and every resource is written back as
+     (milli, -3).  Durations go through Duration.Seconds() (`seconds`) before the division; 0.5^x is `half_pow`;
+  3. samples: the next one is due at last + sampling.  At the start every sample due at or before now_ns is taken; at
+     every boundary t -> t' (a cycle boundary or a jump) every sample due in (t, t'], in time order, with a =
+     afs_alpha (one interval elapsed: the caller's calculateAlphaRate(sampling, half-life)); with half-life 0 a sample
+     resets consumed to empty.  Each sample sets last to its due time.  A boundary's samples run before its
+     completions.  Once a sample leaves consumed unchanged, so would every later one of the boundary (adm is constant
+     there): last goes to the last due time;
+  4. an admission at t_c of a workload of LocalQueue l (workload_controller.go:965-971,1030-1056): its cells join
+     adm[l], consumed = Decay(consumed, adm, t_c - last) (+) entry penalty, last = t_c.  The pending penalties
+     (`lq_penalty`) are not touched: the ones of the snapshot stay pending for the whole drain;
+  5. a completion takes its row's cells out of adm[adm_lq[row]] at the boundary, after the samples; consumed changes at
+     the next sample;
+  6. the LocalQueue usage of the queue order is recomputed whenever consumed changes.
+Canonical choices: samples do not wake the clock (a quiet cycle still waits for the next arrival or completion); the
+early resample while penalties are pending (HasPendingFor, localqueue_controller.go:219) is not modelled; 0.5^x is
+`half_pow`, the library's afs_half_pow (kb_drain.cuh) restated operation for operation, not Go's platform-dependent
+math.Pow.  A drain that runs no cycle takes no sample.
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass, field
 from typing import Callable, List
 
@@ -119,6 +147,11 @@ class DrainResult:
     wl_admit_ns: np.ndarray | None = None                      # [n_wl] time of its last admission, INT64_MIN = never
     wl_finish_ns: np.ndarray | None = None                     # [n_wl] finish time, INT64_MAX = not finished
     end_ns: int = 0                                            # the clock when the drain stopped
+    # decay of consumed usage (lq_last_update_ns in the snapshot; None / 0 otherwise)
+    lq_consumed: np.ndarray | None = None                      # [n_lq][R] int64Amount values after the drain
+    lq_consumed_scale: np.ndarray | None = None                # [n_lq][R] their scales
+    lq_last_update_ns: np.ndarray | None = None                # [n_lq] LastUpdate
+    n_afs_samples: int = 0                                     # samples due over the drain (fixed-point skips included)
 
     @property
     def n_evicted(self) -> int:
@@ -285,6 +318,79 @@ def lq_usage(consumed, scale, penalty_milli, res_weight, lq_weight) -> float:
         return float(np.float64(usage) / np.float64(lq_weight))
 
 
+# ---- decay of consumed usage: restatements of kb_drain.cuh afs_half_pow / afs_seconds / afs_alpha_of / afs_milli / afs_decay
+_LN2HI, _LN2LO, _LOG2E = 6.93147180369123816490e-01, 1.90821492927058770002e-10, 1.44269504088896338700e+00
+_EXP_P = (1.66666666666666657415e-01, -2.77777777770155933842e-03, 6.61375632143793436117e-05, -1.65339022054652515390e-06,
+          4.13813679705723846039e-08)
+
+
+def half_pow(x: float) -> float:
+    """0.5^x for x >= 0, operation for operation as kb_drain.cuh afs_half_pow: Go's Pow for base 0.5 (x = yi + yf with
+    |yf| <= 0.5, exp(yf * Log(0.5)) by the fdlibm reduction and polynomial of Go's exp, then ldexp by -yi)."""
+    yi = float(math.trunc(x))
+    yf = x - yi
+    if yf > 0.5:
+        yf -= 1.0
+        yi += 1.0
+    if yi >= 2048.0:
+        return 0.0
+    v = yf * -0.6931471805599453
+    if -3.725290298461914e-09 < v < 3.725290298461914e-09:
+        a = 1.0 + v
+    else:
+        p1, p2, p3, p4, p5 = _EXP_P
+        k = int(_LOG2E * v - 0.5) if v < 0 else int(_LOG2E * v + 0.5)
+        hi = v - float(k) * _LN2HI
+        lo = float(k) * _LN2LO
+        r = hi - lo
+        t = r * r
+        c = r - t * (p1 + t * (p2 + t * (p3 + t * (p4 + t * p5))))
+        a = math.ldexp(1.0 - ((lo - (r * c) / (2.0 - c)) - hi), k)
+    return math.ldexp(a, -int(yi))
+
+
+def _cdiv(a: int, b: int):
+    """C's truncating a / b and a % b"""
+    q, r = divmod(abs(a), b)
+    return (q, r) if a >= 0 else (-q, -r)
+
+
+def seconds(d_ns: int) -> float:
+    """time.Duration.Seconds(): float64(d / 1e9) + float64(d % 1e9) / 1e9"""
+    q, r = _cdiv(int(d_ns), 1_000_000_000)
+    return float(q) + float(r) / 1e9
+
+
+def alpha_of(elapsed_ns: int, half_life_ns: int) -> float:
+    """calculateAlphaRate(elapsed.Seconds(), halfLife.Seconds()) with half_pow: 0 when the half-life is 0"""
+    return 0.0 if half_life_ns == 0 else 1.0 - half_pow(seconds(elapsed_ns) / seconds(half_life_ns))
+
+
+def milli_value(v: int, s: int) -> int:
+    """Quantity.MilliValue of the int64Amount (v, s): a coarser scale multiplies (AfsOverflow when it leaves int64), a
+    finer one divides and rounds away from zero (negativeScaleInt64, apimachinery math.go:166-198)."""
+    if s >= -3:
+        return _int64(v * 10**(s + 3))
+    q, rem = _cdiv(v, 10**(-3 - s))
+    return q + (1 if v > 0 else -1) if rem else q
+
+
+def decay_quantities(cons, scale, adm, milli_mul, alpha: float):
+    """CalculateDecayedConsumed of one LocalQueue: MulByFloat(consumed, 1 - alpha) (+) MulByFloat(admitted, alpha), every
+    resource as (milli, -3).  Returns (values, changed)."""
+    keep = 1.0 - alpha
+    out, changed = [], False
+    for r in range(len(cons)):
+        old = milli_value(int(cons[r]), int(scale[r]))
+        mul, q = int(milli_mul[r]), int(adm[r])
+        if q > (2**63 - 1) // mul or q < -((2**63 - 1) // mul):
+            raise AfsOverflow(q)
+        v = _int64(int(float(old) * keep) + int(float(q * mul) * alpha))
+        changed |= v != int(cons[r]) or int(scale[r]) != -3
+        out.append(v)
+    return out, changed
+
+
 def entry_penalty(req_rows, mask_rows, milli_mul, alpha: float):
     """CalculateEntryPenalty (admission_fair_sharing.go) of one workload in milli-units per resource:
     int64(float64(MilliValue(SumTotalRequests_r)) * alpha), over the full TotalRequests (the keys of Requests only)."""
@@ -360,14 +466,49 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         first_aside[seg_of[w]] = min(first_aside[seg_of[w]], pos_of[w])
     for s in range(len(qlen)):
         advance(s)
-    if afs_cq.any():
+    decay = events and "wl_lq" in a and "lq_last_update_ns" in a
+    if afs_cq.any() or decay:
         L = len(a["lq_cq"])
         penalty = (a["lq_penalty"].reshape(L, R).astype(object) if "lq_penalty" in a else np.zeros((L, R), object))
         consumed, cscale = a["lq_consumed"].reshape(L, R), a["lq_consumed_scale"].reshape(L, R)
+        if decay:  # rule 1: mutable consumed usage, LastUpdate and the admitted usage of the snapshot's rows
+            consumed, cscale = consumed.astype(object), cscale.astype(np.int64)
+            lq_last = a["lq_last_update_ns"].astype(np.int64).copy()
+            lq_afs = afs_cq[a["lq_cq"].astype(np.int64)]
+            adm_lq = a["adm_lq"].astype(np.int64).copy() if "adm_lq" in a else np.zeros(0, np.int64)
+            ladm = np.zeros((L, R), object)
+            us = a["adm_use_start"]
+            for row in np.flatnonzero(adm_lq >= 0):
+                for k in range(int(us[row]), int(us[row + 1])):
+                    ladm[adm_lq[row], int(a["adm_use_fr"][k]) % R] += int(a["adm_use_qty"][k])
+            hl, samp = int(snap.afs_half_life_ns), int(snap.afs_sampling_ns)
+            n_samples = 0
         usage_of = lambda l: lq_usage(consumed[l], cscale[l], penalty[l], a["afs_res_weight"], a["lq_weight"][l])  # noqa: E731
         lqu = {int(l): usage_of(l) for l in seg_lq if l >= 0}
 
     first_seg = seg_start[:-1]
+
+    def sample(t_to):
+        """rule 3: every sample due at or before t_to (nothing is due at or before the previous boundary)"""
+        nonlocal n_samples
+        for l in np.flatnonzero(lq_afs & (lq_last <= t_to - samp)):
+            k = (int(t_to) - int(lq_last[l])) // samp
+            n_samples += k
+            moved = False
+            for _ in range(k):
+                if hl == 0:
+                    vals, sc = [0] * R, 0
+                    changed = any(int(v) != 0 for v in consumed[l]) or bool((cscale[l] != 0).any())
+                else:
+                    (vals, changed), sc = decay_quantities(consumed[l], cscale[l], ladm[l], a["afs_milli_mul"], snap.afs_alpha), -3
+                consumed[l, :] = vals
+                cscale[l, :] = sc
+                if not changed:
+                    break
+                moved = True
+            lq_last[l] += k * samp
+            if moved:
+                lqu[int(l)] = usage_of(l)
 
     def afs_head_seg(q):
         """segment of the head of AFS ClusterQueue q, -1 = nothing queued"""
@@ -400,7 +541,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     admit_ns = np.full(snap.n_wl, np.iinfo(np.int64).min, np.int64)
     finish_ns = np.full(snap.n_wl, NEVER, np.int64)
     root = root_of(a["parent"])
-    static = {k: v for k, v in a.items() if not (k.startswith(("wl_", "ps_", "adm_")) or k in ("heads", "cq_usage") + abi.AFS_FIELDS)}
+    static = {k: v for k, v in a.items() if not (k.startswith(("wl_", "ps_", "adm_")) or k in ("heads", "cq_usage") + abi.AFS_FIELDS +
+                                                                                               abi.AFS_DECAY_FIELDS)}
     covers_pods = np.zeros(Q, bool)
     if snap.pods_resource >= 0:
         for q in range(Q):
@@ -415,7 +557,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
 
     def remove_rows(rows):
         """rows leave the admitted tables (cache.DeleteWorkload: cells out of the usage; the other rows keep their order)"""
-        nonlocal adm_wl, adm_finish
+        nonlocal adm_wl, adm_finish, adm_lq
         us, uf, uq = adm["adm_use_start"], adm["adm_use_fr"], adm["adm_use_qty"]
         for row in rows:
             cqi = int(adm["adm_cq"][row])
@@ -433,6 +575,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             adm_wl = adm_wl[keep]
         if events:
             adm_finish = adm_finish[keep]
+        if decay:
+            adm_lq = adm_lq[keep]
 
     def next_event():
         """earliest pending event after the evictions: a live row's finish or an ABSENT workload's creation (None = none)"""
@@ -448,6 +592,9 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         fin = adm_wl[done].copy()
         for row in done:
             notified.add(int(adm["adm_cq"][row]))
+            if decay and adm_lq[row] >= 0 and afs_cq[int(adm["adm_cq"][row])]:  # rule 5
+                for k in range(int(adm["adm_use_start"][row]), int(adm["adm_use_start"][row + 1])):
+                    ladm[adm_lq[row], int(adm["adm_use_fr"][k]) % R] -= int(adm["adm_use_qty"][k])
             w = int(adm_wl[row])
             if w >= 0:
                 state[w] = FINISHED
@@ -490,6 +637,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
 
     t = int(snap.now_ns)
     cyc = 0
+    if decay and len(qlen) and snap.n_wl and max_cycles > 0:
+        sample(t)
     while len(qlen) and cyc < max_cycles:
         hseg = np.where(cursor[np.minimum(first_seg, len(qlen) - 1)] < qlen[np.minimum(first_seg, len(qlen) - 1)], first_seg, -1)
         for q in np.flatnonzero(afs_cq):
@@ -501,6 +650,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             e = next_event()  # step 1: the clock jumps to the next event
             if e is None:
                 break
+            if decay:
+                sample(e)
             t = e
             notified = set()
             after(*apply_events(t, notified))
@@ -562,8 +713,19 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             if afs_cq[cqi]:  # AfsEntryPenalties.Push of the entry penalty, then the LocalQueue's usage again
                 w, lq = int(heads[e]), int(a["wl_lq"][heads[e]])
                 rows = slice(int(ps_start[w]), int(ps_start[w + 1]))
-                for r, d in enumerate(entry_penalty(ps_req[rows], a["ps_req_mask"][rows], a["afs_milli_mul"], snap.afs_alpha)):
-                    penalty[lq, r] = _int64(int(penalty[lq, r]) + d)
+                pen = entry_penalty(ps_req[rows], a["ps_req_mask"][rows], a["afs_milli_mul"], snap.afs_alpha)
+                if decay:  # rule 4: admitted usage, decay to t, LastUpdate = t, the penalty into consumed
+                    for fr, q in cells.items():
+                        ladm[lq, fr % R] += q
+                    vals, _ = decay_quantities(consumed[lq], cscale[lq], ladm[lq], a["afs_milli_mul"], alpha_of(t - int(lq_last[lq]), hl))
+                    consumed[lq, :] = vals
+                    cscale[lq, :] = -3
+                    lq_last[lq] = t
+                    for r, d in enumerate(pen):
+                        consumed[lq, r], cscale[lq, r] = quantity_add((int(consumed[lq, r]), int(cscale[lq, r])), (d, -3))
+                else:
+                    for r, d in enumerate(pen):
+                        penalty[lq, r] = _int64(int(penalty[lq, r]) + d)
                 lqu[lq] = usage_of(lq)
         n_new = int(ok.sum())
         if n_new:
@@ -584,6 +746,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             adm["adm_use_qty"] = np.concatenate([adm["adm_use_qty"], np.asarray(new_qty, np.int64)])
             if adm_wl is not None:
                 adm_wl = np.concatenate([adm_wl, g])
+            if decay:
+                adm_lq = np.concatenate([adm_lq, a["wl_lq"][g].astype(np.int64)])
             if events:
                 fin_new = [finish_time(t, int(run_ns[w])) if run_ns is not None else NEVER for w in g]
                 adm_finish = np.concatenate([adm_finish, np.asarray(fin_new, np.int64)])
@@ -658,6 +822,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             if e is None:
                 break  # quiet, and nothing will ever happen again
             t_next = max(min(t + step, NEVER), e)
+        if decay:
+            sample(t_next)
         t = t_next
         after(*apply_events(t, notified))
         if notified:
@@ -672,4 +838,9 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     res.wl_admit_ns = admit_ns
     res.wl_finish_ns = finish_ns
     res.end_ns = t
+    if decay:
+        res.lq_consumed = consumed.astype(np.int64)
+        res.lq_consumed_scale = cscale.astype(np.int32)
+        res.lq_last_update_ns = lq_last
+        res.n_afs_samples = n_samples
     return res

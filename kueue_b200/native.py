@@ -87,6 +87,7 @@ def pin_snapshot(snap: abi.FlatSnapshot) -> abi.FlatSnapshot:
     out._pinned_block = block
     out.static_generation = snap.static_generation
     out.afs_alpha = snap.afs_alpha
+    out.afs_half_life_ns, out.afs_sampling_ns = snap.afs_half_life_ns, snap.afs_sampling_ns
     return out
 
 

@@ -221,6 +221,25 @@ def add_afs(snap: abi.FlatSnapshot, k: int, seed: int = 0, half_life_s: float = 
     return snap
 
 
+def add_afs_decay(snap: abi.FlatSnapshot, seed: int = 0, half_life_ns: int = 100_000, sampling_ns: int = 20_000) -> abi.FlatSnapshot:
+    """Decay tables of an event drain (include/kueue_b200.h) on a snapshot with `add_afs` tables: every LocalQueue's
+    LastUpdate spread over the last sampling interval, every admitted row in a random LocalQueue of its ClusterQueue
+    (-1 where it has none), the two durations, and afs_alpha = calculateAlphaRate(sampling, half-life)."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    a = snap.arrays
+    L = len(a["lq_cq"])
+    now = int(snap.now_ns)
+    snap.set("lq_last_update_ns", now - rng.integers(0, sampling_ns, L))
+    n_of = np.bincount(a["lq_cq"].astype(np.int64), minlength=snap.n_cq)
+    first = np.concatenate([[0], np.cumsum(n_of)])
+    cq = a["adm_cq"].astype(np.int64)
+    pick = first[cq] + (rng.random(len(cq)) * np.maximum(n_of[cq], 1)).astype(np.int64)
+    snap.set("adm_lq", np.where(n_of[cq] > 0, pick, -1))
+    snap.afs_half_life_ns, snap.afs_sampling_ns = int(half_life_ns), int(sampling_ns)
+    snap.afs_alpha = 1.0 - 0.5 ** (sampling_ns / half_life_ns) if half_life_ns else 0.0
+    return snap
+
+
 def add_evictable(snap: abi.FlatSnapshot) -> abi.FlatSnapshot:
     """Give every admitted workload a pending record consistent with its usage and name it in `adm_wl`
     (include/kueue_b200.h): same ClusterQueue, priority, queue-order timestamp and UID, one podset of count 1 whose
