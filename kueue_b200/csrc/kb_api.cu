@@ -17,7 +17,11 @@
 
 namespace {
 
-struct Arena {  // grow-only device arena, 256 B aligned sub-allocations
+inline size_t pad256(size_t b) { b = (b + 255) & ~(size_t)255; return b ? b : 256; }
+
+// Grow-only device arena, 256 B aligned sub-allocations.  An arena without a base is a sizing pass: take() only
+// counts bytes (returns nullptr), so one layout function run on it and then on the real arena describes a buffer once.
+struct Arena {
   char *base = nullptr;
   size_t cap = 0, used = 0;
   void reset() { used = 0; }
@@ -31,14 +35,20 @@ struct Arena {  // grow-only device arena, 256 B aligned sub-allocations
     return true;
   }
   template <typename T> T *take(size_t n) {
-    size_t b = (n * sizeof(T) + 255) & ~(size_t)255;
-    if (b == 0) b = 256;
-    T *p = (T *)(base + used);
-    used += b;
+    T *p = base ? (T *)(base + used) : nullptr;
+    used += pad256(n * sizeof(T));
     return p;
   }
+  // layout(Arena &) takes every sub-allocation of a buffer: run once to size, once to carve this arena from the start
+  template <typename F> bool carve(F &&layout) {
+    Arena sizing;
+    layout(sizing);
+    if (!reserve(sizing.used)) return false;
+    reset();
+    layout(*this);
+    return true;
+  }
 };
-inline size_t pad256(size_t b) { b = (b + 255) & ~(size_t)255; return b ? b : 256; }
 
 }  // namespace
 
@@ -88,8 +98,8 @@ struct kb_handle {
   // kb_run_drain: capacity reserved beyond the snapshot's admitted tables, heads chosen on the device
   size_t drain_extra_adm = 0, drain_extra_au = 0; bool drain_mode = false; bool preempt_possible = true;
   bool drain_events = false;  // kb_run_drain in event mode: rows admitted during the drain are preemption candidates
-  char *drain_buf = nullptr; size_t drain_buf_cap = 0; cudaEvent_t ev_d = nullptr;
-  char *tas_buf = nullptr; size_t tas_buf_cap = 0;
+  Arena drain_arena; cudaEvent_t ev_d = nullptr;  // kb_run_drain's queue tables, double buffer and scratch
+  Arena tas_arena;  // kb_tas_find's inputs, lists and outputs
   bool fused_on = false; size_t fused_smem = 0; bool one_head_per_cq = false; int32_t *d_cq_entry = nullptr;
   // k_cycle_flat (kb_flat.cuh): static per-tree blocks in local numbering, head records per tree node
   std::vector<unsigned char> tree_blob; std::vector<int32_t> tree_blob_off; int max_blob_bytes = 16;
@@ -214,9 +224,9 @@ void kb_destroy(kb_handle *h) {
   if (h->arena.base) cudaFree(h->arena.base);
   if (h->sarena.base) cudaFree(h->sarena.base);
   if (h->iarena.base) cudaFree(h->iarena.base);
-  if (h->drain_buf) cudaFree(h->drain_buf);
+  if (h->drain_arena.base) cudaFree(h->drain_arena.base);
+  if (h->tas_arena.base) cudaFree(h->tas_arena.base);
   if (h->d_usage_res) cudaFree(h->d_usage_res);
-  if (h->tas_buf) cudaFree(h->tas_buf);
   if (h->ev_d) cudaEventDestroy(h->ev_d);
   if (h->host_words) cudaFreeHost(h->host_words);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -591,6 +601,10 @@ static cudaError_t up(kb_handle *h, Arena &arena, const T *&dst, const T *src, s
   if (n == 0) return cudaSuccess;
   *bytes += (int64_t)(n * sizeof(T));
   return cudaMemcpyAsync(d, src, n * sizeof(T), cudaMemcpyHostToDevice, h->stream);
+}
+// host -> device on the handle's stream; an empty table copies nothing
+static cudaError_t h2d(kb_handle *h, const void *dst, const void *src, size_t bytes) {
+  return bytes ? cudaMemcpyAsync(const_cast<void *>(dst), src, bytes, cudaMemcpyHostToDevice, h->stream) : cudaSuccess;
 }
 
 static int32_t upload_impl(kb_handle *h, const kb_snapshot *s, bool sync) {
@@ -1348,6 +1362,15 @@ extern "C" int32_t kb_run_cycle(kb_handle *h, const kb_snapshot *s, kb_cycle_out
 // ---------------------------------------------------------------------------
 // kb_run_drain: iterated cycles with the queue layer on the device (kb_drain.cuh)
 // ---------------------------------------------------------------------------
+// what a boundary of kb_run_drain reads back, in the pinned host words [8, 24)
+struct DrainWords {
+  uint32_t counters[KB_DC_ARR_HI + 1];  // DrainDev::counters; [0] = heads of the next cycle
+  uint32_t n_new, n_cells;              // this cycle's admissions and their usage cells (the admit scans' totals)
+  uint32_t status;                      // the cycle's status word (KBS_AFS_OVERFLOW)
+  i64 t_next;                           // event mode: t_{c+1}
+};
+static_assert(8 * 4 + sizeof(DrainWords) <= 32 * 4, "host_words[32..63] hold the cycle header");
+
 static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out) {
   const int Q = s->n_cq, W = s->n_wl, R = s->n_resource, FR = s->n_flavor * s->n_resource;
   const int Hcap = std::min(Q, W);
@@ -1447,26 +1470,10 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     sort_bytes += 256;
   }
   const size_t trace_cap = out->trace_wl && out->trace_decision ? (size_t)std::max<int64_t>(0, out->trace_capacity) : 0;
-  size_t tot = 0;
-  auto need = [&](size_t n, size_t sz) { tot += pad256(n * sz); };
-  need(Wz, 8); need(Wz, 8); need(Wz, 4); need(Wz, 4); need(sort_bytes, 1);
-  need(Sz + 2, 4); need(Sz + 2, 4); need(Sz, 4); need(Wz, 1); need((size_t)Q + 2, 4); need((size_t)Q + 2, 4);
-  for (int k = 0; k < 4; k++) need(Hz + 2, 4);
-  need(16, 4); need(Wz, 4); need(Wz, 4); need(Wz, 1); need(trace_cap, 4); need(trace_cap, 1);
-  // replay: a workload holds at most one live row, so the live rows after a compaction plus the cycle's admissions stay
-  // within the capacity upload_impl reserved: rows <= min(W, A_in + admissions) <= A_in + min(W, Hcap * max_cycles),
-  // cells <= AU_in + min(P * R, that bound * FR) (a readmitted victim's old cells left with its old row)
-  const size_t Acap = (size_t)s->n_adm + h->drain_extra_adm, AUcap = (size_t)s->n_adm_use + h->drain_extra_au;
+  const size_t Acap = (size_t)s->n_adm + h->drain_extra_adm, AUcap = (size_t)s->n_adm_use + h->drain_extra_au;  // see the boundary loop
   size_t scan_bytes = 0;
   if (compact) cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (int32_t *)nullptr, (int32_t *)nullptr, (int)Acap + 1, h->stream);
   const size_t nR = (size_t)std::max(1, D.nRoots);
-  if (replay || events) { need(Acap, 4); need(Wz, 4); need(Wz, 4); need(Wz, 4); need(Sz, 4); }
-  if (compact) {
-    need(Acap, 4); need(Acap, 4); need(nR, 4); for (int k = 0; k < 4; k++) need(Acap + 1, 4); need(scan_bytes + 256, 1);
-    need(Acap, 4); need(Acap, 4); need(Acap, 8); need(Acap, 8); need(Acap, 8); need(Acap, 1); need(Acap + 1, 4); need(AUcap, 4); need(AUcap, 8);
-  }
-  // event mode: finish columns of both halves, run times, admit / finish times, the clock, the arrival order (sorted
-  // pairs and their double buffers) and the NoFit classes
   std::vector<int32_t> wl_class, cq_class_start;
   int n_class = 0;
   if (events && s->wl_create_ns && s->wl_sched_hash) {  // dense class id per (BestEffortFIFO ClusterQueue, known hash)
@@ -1483,39 +1490,66 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (!cls.empty()) n_class++;
     for (int q = 0; q < Q; q++) cq_class_start[q + 1] = std::max(cq_class_start[q + 1], cq_class_start[q]);
   }
-  if (events) {
-    need(Acap, 8); need(Acap, 8); need(Wz, 8); need(Wz, 8); need(Wz, 8); need(4, 8);
-    if (s->wl_create_ns) { need(Wz, 8); need(Wz, 8); need(Wz, 4); need(Wz, 4); need(Wz, 8); }
-    if (n_class) { need(Wz, 4); need((size_t)Q + 1, 4); need((size_t)n_class, 1); }
-  }
-  if (!replay) need(Sz, 4);
-  if (afs) {
-    need((size_t)Q + 1, 4); need(Lz, 4); need(seg_lq.size(), 4); need(afs_cqs.size() + 1, 4); need(Q, 4); need(Wz, 4); need(Q, 1);
-    need(Lz, 8); need(LR, 8); need(LR, 4); need(LR, 8); need(Lz, 8); need(R, 8); need(R, 8);
-  }
-  if (decay) { need(Lz, 8); need(LR, 8); need(Acap, 4); need(Acap, 4); need(1, 8); }
-  if (tot > h->drain_buf_cap) {
-    if (h->drain_buf) cudaFree(h->drain_buf);
-  if (h->tas_buf) cudaFree(h->tas_buf);
-    h->drain_buf = nullptr; h->drain_buf_cap = 0;
-    CUDA_TRY(h, cudaMalloc(&h->drain_buf, tot + (1 << 20)));
-    h->drain_buf_cap = tot + (1 << 20);
-  }
-  size_t used = 0;
-  auto take = [&](size_t n, size_t sz) { char *p = h->drain_buf + used; used += pad256(n * sz); return p; };
-  u64 *keys[2] = {(u64 *)take(Wz, 8), (u64 *)take(Wz, 8)};
-  int32_t *vals[2] = {(int32_t *)take(Wz, 4), (int32_t *)take(Wz, 4)};
-  void *sort_tmp = take(sort_bytes, 1);
+  // every buffer of the drain, described once (Arena::carve)
+  u64 *keys[2], *arr_keys[2] = {nullptr, nullptr};
+  int32_t *vals[2], *arr_vals[2] = {nullptr, nullptr}, *q_count, *d_wl_class = nullptr, *d_cq_class_start = nullptr;
+  char *sort_tmp, *scan_tmp = nullptr;
+  i64 *run = nullptr, *create = nullptr;
   DrainDev X{};
-  int32_t *q_count = (int32_t *)take(Sz + 2, 4);
-  X.q_start = (int32_t *)take(Sz + 2, 4); X.cursor = (int32_t *)take(Sz, 4); X.wl_state = (uint8_t *)take(Wz, 1);
-  X.first_aside = (int32_t *)take(Sz, 4);
-  X.flag = (int32_t *)take((size_t)Q + 2, 4); X.pos = (int32_t *)take((size_t)Q + 2, 4);
-  X.e_assumed = (int32_t *)take(Hz + 2, 4); X.e_ncells = (int32_t *)take(Hz + 2, 4);
-  X.e_adm_off = (int32_t *)take(Hz + 2, 4); X.e_cell_off = (int32_t *)take(Hz + 2, 4);
-  X.counters = (int32_t *)take(16, 4);
-  X.wl_admit_cycle = (int32_t *)take(Wz, 4); X.wl_evals = (int32_t *)take(Wz, 4); X.wl_last_decision = (uint8_t *)take(Wz, 1);
-  X.trace_wl = trace_cap ? (int32_t *)take(trace_cap, 4) : nullptr; X.trace_dec = trace_cap ? (uint8_t *)take(trace_cap, 1) : nullptr;
+  AdmTabs other{};  // compaction: the other half of the admitted tables' double buffer
+  auto layout = [&](Arena &a) {
+    keys[0] = a.take<u64>(Wz); keys[1] = a.take<u64>(Wz);
+    vals[0] = a.take<int32_t>(Wz); vals[1] = a.take<int32_t>(Wz);
+    sort_tmp = a.take<char>(sort_bytes);
+    q_count = a.take<int32_t>(Sz + 2);
+    X.q_start = a.take<int32_t>(Sz + 2); X.cursor = a.take<int32_t>(Sz); X.wl_state = a.take<uint8_t>(Wz);
+    X.first_aside = a.take<int32_t>(Sz);
+    X.flag = a.take<int32_t>((size_t)Q + 2); X.pos = a.take<int32_t>((size_t)Q + 2);
+    X.e_assumed = a.take<int32_t>(Hz + 2); X.e_ncells = a.take<int32_t>(Hz + 2);
+    X.e_adm_off = a.take<int32_t>(Hz + 2); X.e_cell_off = a.take<int32_t>(Hz + 2);
+    X.counters = a.take<int32_t>(16);
+    X.wl_admit_cycle = a.take<int32_t>(Wz); X.wl_evals = a.take<int32_t>(Wz); X.wl_last_decision = a.take<uint8_t>(Wz);
+    if (trace_cap) { X.trace_wl = a.take<int32_t>(trace_cap); X.trace_dec = a.take<uint8_t>(trace_cap); }
+    if (replay || events) {
+      X.adm_wl = a.take<int32_t>(Acap);
+      X.wl_seg = a.take<int32_t>(Wz); X.wl_pos = a.take<int32_t>(Wz); X.wl_evictions = a.take<int32_t>(Wz);
+    }
+    if (compact) {
+      X.adm_dead = a.take<int32_t>(Acap); other.wl = a.take<int32_t>(Acap); X.root_mark = a.take<int32_t>(nR);
+      X.row_live = a.take<int32_t>(Acap + 1); X.row_cells = a.take<int32_t>(Acap + 1);
+      X.row_new = a.take<int32_t>(Acap + 1); X.cell_new = a.take<int32_t>(Acap + 1);
+      scan_tmp = a.take<char>(scan_bytes + 256);
+      other.cq = a.take<int32_t>(Acap); other.priority = a.take<int32_t>(Acap); other.ts = a.take<i64>(Acap);
+      other.qr_ts = a.take<i64>(Acap); other.uid = a.take<i64>(Acap); other.evicted = a.take<uint8_t>(Acap);
+      other.use_start = a.take<int32_t>(Acap + 1); other.use_fr = a.take<int32_t>(AUcap); other.use_qty = a.take<i64>(AUcap);
+    }
+    if (events) {  // finish columns of both halves, run times, admit / finish times, the clock, the arrival order (sorted
+                   // pairs and their double buffers) and the NoFit classes
+      X.adm_finish = a.take<i64>(Acap); other.finish = a.take<i64>(Acap);
+      run = a.take<i64>(Wz);
+      X.wl_admit_ns = a.take<i64>(Wz); X.wl_finish_ns = a.take<i64>(Wz); X.clock = a.take<i64>(4);
+      if (s->wl_create_ns) {
+        arr_keys[0] = a.take<u64>(Wz); arr_keys[1] = a.take<u64>(Wz);
+        arr_vals[0] = a.take<int32_t>(Wz); arr_vals[1] = a.take<int32_t>(Wz);
+        create = a.take<i64>(Wz);
+      }
+      if (n_class) { d_wl_class = a.take<int32_t>(Wz); d_cq_class_start = a.take<int32_t>((size_t)Q + 1); X.class_nofit = a.take<uint8_t>(n_class); }
+    }
+    if (afs) {
+      X.seg_start = a.take<int32_t>(seg_start.size()); X.lq_seg = a.take<int32_t>(lq_seg.size());
+      X.seg_lq = a.take<int32_t>(seg_lq.size()); X.afs_cqs = a.take<int32_t>(afs_cqs.size());
+      X.head_seg = a.take<int32_t>(Q); X.wl_lq = a.take<int32_t>(Wz); X.cq_afs = a.take<uint8_t>(Q);
+      X.lq_weight = a.take<double>(L); X.lq_consumed = a.take<i64>((size_t)L * R); X.lq_consumed_scale = a.take<int32_t>((size_t)L * R);
+      X.lq_penalty = a.take<i64>(LR); X.lq_usage = a.take<double>(Lz);
+      X.res_weight = a.take<double>(R); X.milli_mul = a.take<i64>(R);
+    }
+    if (decay) {
+      X.lq_last = a.take<i64>(Lz); X.lq_adm = a.take<i64>(LR);
+      X.adm_lq = a.take<int32_t>(Acap); other.lq = a.take<int32_t>(Acap);
+      X.afs_samples = a.take<unsigned long long>(1);
+    }
+  };
+  if (!h->drain_arena.carve(layout)) return fail(h, KB_ERR_CUDA, "kb_run_drain: cudaMalloc of the drain buffer failed");
   X.trace_cap = (long long)trace_cap;
   X.cq_usage = const_cast<i64 *>(D.cq_usage); X.wl_last_gen = const_cast<i64 *>(D.wl_last_gen); X.ps_last_tried = const_cast<int8_t *>(D.ps_last_tried);
   X.adm_cq = const_cast<int32_t *>(D.adm_cq); X.adm_priority = const_cast<int32_t *>(D.adm_priority);
@@ -1523,85 +1557,47 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   X.adm_evicted = const_cast<uint8_t *>(D.adm_evicted); X.adm_use_start = const_cast<int32_t *>(D.adm_use_start);
   X.adm_use_fr = const_cast<int32_t *>(D.adm_use_fr); X.adm_use_qty = const_cast<i64 *>(D.adm_use_qty);
   X.A_cap = (int)Acap; X.AU_cap = (int)AUcap;
-  AdmTabs other{};  // replay: the other half of the admitted tables' double buffer
-  void *scan_tmp = nullptr;
+  // ---- uploads and initial values
   if (replay || events) {  // event mode without adm_wl: the rows of the snapshot have no record (-1)
-    X.adm_wl = (int32_t *)take(Acap, 4);
-    if (replay) CUDA_TRY(h, cudaMemcpyAsync(X.adm_wl, s->adm_wl, (size_t)s->n_adm * 4, cudaMemcpyHostToDevice, h->stream));
+    if (replay) CUDA_TRY(h, h2d(h, X.adm_wl, s->adm_wl, (size_t)s->n_adm * 4));
     else CUDA_TRY(h, cudaMemsetAsync(X.adm_wl, 0xff, (size_t)s->n_adm * 4, h->stream));
-    X.wl_seg = (int32_t *)take(Wz, 4); X.wl_pos = (int32_t *)take(Wz, 4); X.wl_evictions = (int32_t *)take(Wz, 4);
     X.wl_has_qr = const_cast<uint8_t *>(D.wl_has_qr);
   }
   if (compact) {
-    X.adm_dead = (int32_t *)take(Acap, 4);
     CUDA_TRY(h, cudaMemsetAsync(X.adm_dead, 0, Acap * 4, h->stream));
-    other.wl = (int32_t *)take(Acap, 4);
-    X.root_mark = (int32_t *)take(nR, 4);
     CUDA_TRY(h, cudaMemsetAsync(X.root_mark, 0, nR * 4, h->stream));
-    X.row_live = (int32_t *)take(Acap + 1, 4); X.row_cells = (int32_t *)take(Acap + 1, 4);
-    X.row_new = (int32_t *)take(Acap + 1, 4); X.cell_new = (int32_t *)take(Acap + 1, 4);
-    scan_tmp = take(scan_bytes + 256, 1);
-    other.cq = (int32_t *)take(Acap, 4); other.priority = (int32_t *)take(Acap, 4); other.ts = (i64 *)take(Acap, 8);
-    other.qr_ts = (i64 *)take(Acap, 8); other.uid = (i64 *)take(Acap, 8); other.evicted = (uint8_t *)take(Acap, 1);
-    other.use_start = (int32_t *)take(Acap + 1, 4); other.use_fr = (int32_t *)take(AUcap, 4); other.use_qty = (i64 *)take(AUcap, 8);
   }
-  u64 *arr_keys[2] = {nullptr, nullptr}; int32_t *arr_vals[2] = {nullptr, nullptr};
-  const i64 *d_create = nullptr;
+  std::vector<i64> never;  // event mode without adm_finish_ns: the rows of the snapshot never finish
   if (events) {
-    X.adm_finish = (i64 *)take(Acap, 8); other.finish = (i64 *)take(Acap, 8);
-    if (s->adm_finish_ns) CUDA_TRY(h, cudaMemcpyAsync(X.adm_finish, s->adm_finish_ns, (size_t)s->n_adm * 8, cudaMemcpyHostToDevice, h->stream));
-    else {
-      std::vector<i64> never((size_t)s->n_adm, INT64_MAX);
-      CUDA_TRY(h, cudaMemcpyAsync(X.adm_finish, never.data(), (size_t)s->n_adm * 8, cudaMemcpyHostToDevice, h->stream));
-      CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // `never` leaves scope
-    }
-    i64 *run = (i64 *)take(Wz, 8);
-    if (s->wl_run_ns) { CUDA_TRY(h, cudaMemcpyAsync(run, s->wl_run_ns, Wz * 8, cudaMemcpyHostToDevice, h->stream)); X.wl_run = run; }
-    X.wl_admit_ns = (i64 *)take(Wz, 8); X.wl_finish_ns = (i64 *)take(Wz, 8); X.clock = (i64 *)take(4, 8);
-    if (s->wl_create_ns) {
-      arr_keys[0] = (u64 *)take(Wz, 8); arr_keys[1] = (u64 *)take(Wz, 8);
-      arr_vals[0] = (int32_t *)take(Wz, 4); arr_vals[1] = (int32_t *)take(Wz, 4);
-      i64 *create = (i64 *)take(Wz, 8);
-      CUDA_TRY(h, cudaMemcpyAsync(create, s->wl_create_ns, Wz * 8, cudaMemcpyHostToDevice, h->stream));
-      d_create = create;
-      X.n_arr = W;
-    }
+    const void *finish = s->adm_finish_ns;
+    if (!finish) { never.assign((size_t)s->n_adm, INT64_MAX); finish = never.data(); }
+    CUDA_TRY(h, h2d(h, X.adm_finish, finish, (size_t)s->n_adm * 8));
+    if (s->wl_run_ns) { CUDA_TRY(h, h2d(h, run, s->wl_run_ns, Wz * 8)); X.wl_run = run; }
+    if (create) { CUDA_TRY(h, h2d(h, create, s->wl_create_ns, Wz * 8)); X.n_arr = W; }
     if (n_class) {
-      int32_t *wc = (int32_t *)take(Wz, 4), *cs = (int32_t *)take((size_t)Q + 1, 4);
-      X.class_nofit = (uint8_t *)take((size_t)n_class, 1);
-      CUDA_TRY(h, cudaMemcpyAsync(wc, wl_class.data(), Wz * 4, cudaMemcpyHostToDevice, h->stream));
-      CUDA_TRY(h, cudaMemcpyAsync(cs, cq_class_start.data(), ((size_t)Q + 1) * 4, cudaMemcpyHostToDevice, h->stream));
+      CUDA_TRY(h, h2d(h, d_wl_class, wl_class.data(), Wz * 4));
+      CUDA_TRY(h, h2d(h, d_cq_class_start, cq_class_start.data(), ((size_t)Q + 1) * 4));
       CUDA_TRY(h, cudaMemsetAsync(X.class_nofit, 0, (size_t)n_class, h->stream));
-      X.wl_class = wc; X.cq_class_start = cs;
+      X.wl_class = d_wl_class; X.cq_class_start = d_cq_class_start;
     }
   }
   if (afs) {
-    auto h2d = [&](const void *src, size_t n, size_t sz) {
-      char *p = take(n, sz);
-      if (n) { cudaError_t e = cudaMemcpyAsync(p, src, n * sz, cudaMemcpyHostToDevice, h->stream); if (e != cudaSuccess) return (char *)nullptr; }
-      return p;
-    };
-    X.seg_start = (const int32_t *)h2d(seg_start.data(), seg_start.size(), 4);
-    X.lq_seg = (const int32_t *)h2d(lq_seg.data(), lq_seg.size(), 4);
-    X.seg_lq = (const int32_t *)h2d(seg_lq.data(), seg_lq.size(), 4);
-    X.afs_cqs = (const int32_t *)h2d(afs_cqs.data(), afs_cqs.size(), 4);
-    X.head_seg = (int32_t *)take(Q, 4);
-    X.wl_lq = (const int32_t *)h2d(s->wl_lq, Wz, 4);
-    X.cq_afs = (const uint8_t *)h2d(s->cq_afs, Q, 1);
-    X.lq_weight = (const double *)h2d(s->lq_weight, L, 8);
-    X.lq_consumed = (i64 *)h2d(s->lq_consumed, (size_t)L * R, 8);
-    X.lq_consumed_scale = (int32_t *)h2d(s->lq_consumed_scale, (size_t)L * R, 4);
-    X.lq_penalty = (i64 *)take(LR, 8);
-    if (s->lq_penalty) CUDA_TRY(h, cudaMemcpyAsync(X.lq_penalty, s->lq_penalty, (size_t)L * R * 8, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, h2d(h, X.seg_start, seg_start.data(), seg_start.size() * 4));
+    CUDA_TRY(h, h2d(h, X.lq_seg, lq_seg.data(), lq_seg.size() * 4));
+    CUDA_TRY(h, h2d(h, X.seg_lq, seg_lq.data(), seg_lq.size() * 4));
+    CUDA_TRY(h, h2d(h, X.afs_cqs, afs_cqs.data(), afs_cqs.size() * 4));
+    CUDA_TRY(h, h2d(h, X.wl_lq, s->wl_lq, Wz * 4));
+    CUDA_TRY(h, h2d(h, X.cq_afs, s->cq_afs, (size_t)Q));
+    CUDA_TRY(h, h2d(h, X.lq_weight, s->lq_weight, (size_t)L * 8));
+    CUDA_TRY(h, h2d(h, X.lq_consumed, s->lq_consumed, (size_t)L * R * 8));
+    CUDA_TRY(h, h2d(h, X.lq_consumed_scale, s->lq_consumed_scale, (size_t)L * R * 4));
+    if (s->lq_penalty) CUDA_TRY(h, h2d(h, X.lq_penalty, s->lq_penalty, (size_t)L * R * 8));
     else CUDA_TRY(h, cudaMemsetAsync(X.lq_penalty, 0, LR * 8, h->stream));
-    X.lq_usage = (double *)h2d(lq_usage.data(), Lz, 8);
-    X.res_weight = (const double *)h2d(s->afs_res_weight, R, 8);
-    X.milli_mul = (const i64 *)h2d(s->afs_milli_mul, R, 8);
+    CUDA_TRY(h, h2d(h, X.lq_usage, lq_usage.data(), Lz * 8));
+    CUDA_TRY(h, h2d(h, X.res_weight, s->afs_res_weight, (size_t)R * 8));
+    CUDA_TRY(h, h2d(h, X.milli_mul, s->afs_milli_mul, (size_t)R * 8));
     X.alpha = s->afs_alpha;
     X.n_afs_cq = (int)afs_cqs.size();
-    if (!X.seg_start || !X.lq_seg || !X.seg_lq || !X.afs_cqs || !X.wl_lq || !X.cq_afs || !X.lq_weight || !X.lq_consumed ||
-        !X.lq_consumed_scale || !X.lq_usage || !X.res_weight || !X.milli_mul)
-      return fail(h, KB_ERR_CUDA, "afs: upload of the LocalQueue tables failed");
   }
   std::vector<i64> lq_adm;  // decay: the initial admitted usage of every LocalQueue (live rows of the snapshot)
   if (decay) {
@@ -1609,12 +1605,9 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     for (int a = 0; a < s->n_adm; a++)
       if (s->adm_lq[a] >= 0)
         for (int c = s->adm_use_start[a]; c < s->adm_use_start[a + 1]; c++) lq_adm[(size_t)s->adm_lq[a] * R + s->adm_use_fr[c] % R] += s->adm_use_qty[c];
-    X.lq_last = (i64 *)take(Lz, 8); X.lq_adm = (i64 *)take(LR, 8);
-    X.adm_lq = (int32_t *)take(Acap, 4); other.lq = (int32_t *)take(Acap, 4);
-    X.afs_samples = (unsigned long long *)take(1, 8);
-    if (L) CUDA_TRY(h, cudaMemcpyAsync(X.lq_last, s->lq_last_update_ns, (size_t)L * 8, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(X.lq_adm, lq_adm.data(), LR * 8, cudaMemcpyHostToDevice, h->stream));
-    if (s->n_adm) CUDA_TRY(h, cudaMemcpyAsync(X.adm_lq, s->adm_lq, (size_t)s->n_adm * 4, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, h2d(h, X.lq_last, s->lq_last_update_ns, (size_t)L * 8));
+    CUDA_TRY(h, h2d(h, X.lq_adm, lq_adm.data(), LR * 8));
+    CUDA_TRY(h, h2d(h, X.adm_lq, s->adm_lq, (size_t)s->n_adm * 4));
     CUDA_TRY(h, cudaMemsetAsync(X.afs_samples, 0, 8, h->stream));
     X.half_life_ns = s->afs_half_life_ns; X.sampling_ns = s->afs_sampling_ns;
   }
@@ -1633,16 +1626,16 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 32 + cq_bits, h->stream));
     X.q_order = dv.Current();
   }
-  if (d_create) {  // arrival order: (creation time, index); the workloads present at the start are its first k_drain_init_events prefix
+  if (create) {  // arrival order: (creation time, index); the workloads present at the start are its first k_drain_init_events prefix
     cub::DoubleBuffer<u64> dk(arr_keys[0], arr_keys[1]); cub::DoubleBuffer<int32_t> dv(arr_vals[0], arr_vals[1]);
     size_t bytes = sort_bytes;
-    k_drain_keys_create<<<nbW, tb, 0, h->stream>>>(W, d_create, dk.Current(), dv.Current());
+    k_drain_keys_create<<<nbW, tb, 0, h->stream>>>(W, create, dk.Current(), dv.Current());
     CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 64, h->stream));
     X.arr_key = dk.Current(); X.arr_order = dv.Current();
   }
   k_scan_i32<<<1, 1024, 0, h->stream>>>(q_count, X.q_start, S);
   k_drain_init<<<std::max(nbW, (S + tb - 1) / tb), tb, 0, h->stream>>>(D, X, S);
-  if (events) k_drain_init_events<<<std::max(1, nbW), tb, 0, h->stream>>>(D, X, d_create, s->now_ns);
+  if (events) k_drain_init_events<<<std::max(1, nbW), tb, 0, h->stream>>>(D, X, create, s->now_ns);
   if (replay || events) k_drain_init_replay<<<std::max(nbW, (s->n_adm + tb - 1) / tb), tb, 0, h->stream>>>(D, X, replay ? s->n_adm : 0);
   k_drain_advance<<<(S + tb - 1) / tb, tb, 0, h->stream>>>(X, S);
   const int nbL = std::max(1, (L + tb - 1) / tb);
@@ -1657,28 +1650,37 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     k_scan_i32<<<1, 1024, 0, h->stream>>>(X.flag, X.pos, Q);
     k_drain_heads<<<nbQ, tb, 0, h->stream>>>(D, X, d_heads);
   };
+  DrainWords &hw = *reinterpret_cast<DrainWords *>(&h->host_words[8]);
   CUDA_TRY(h, cudaMemsetAsync(X.counters + 1, 0, 5 * 4, h->stream));
   enqueue_heads();
-  CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[8], X.counters, 4, cudaMemcpyDeviceToHost, h->stream));
-  if (decay) CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[11], D.status, 4, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[0], X.counters, 4, cudaMemcpyDeviceToHost, h->stream));
+  if (decay) CUDA_TRY(h, cudaMemcpyAsync(&hw.status, D.status, 4, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  if (decay && (h->host_words[11] & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: a decayed consumed quantity overflows int64");
-  int n_live = (int)h->host_words[8];
+  if (decay && (hw.status & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: a decayed consumed quantity overflows int64");
+  int n_live = (int)hw.counters[0];
   int A_cur = s->n_adm, AU_cur = s->n_adm_use;
   const bool pre = h->preempt_possible;
   double gpu_ms = 0;
   float kms[KB_N_KERNELS] = {};  // per-kernel times summed over the cycles (kb_set_profile)
-  i64 t = s->now_ns;  // event mode: the simulated clock
+  i64 t = s->now_ns;  // the clock: the plain drain steps it by one per cycle
   const i64 step = s->drain_cycle_ns > 0 ? s->drain_cycle_ns : 1;
   const int nbArr = std::max(1, std::min(nbW, 8 * std::max(1, h->sm_count)));
-  for (int cyc = 0, jumps = 0; events && cyc < max_cycles;) {
-    // one boundary: cycle c at t (or, without heads, a jump to the next event), then E, t_{c+1}, completions,
-    // arrivals, inadmissible requeue, compaction and the next heads; one synchronisation
+  // ---- one boundary per iteration, one synchronisation each (kueue_b200/drain.py): cycle c at t (in event mode, a
+  // jump to the next event when there are no heads), its decisions and admissions, the evictions; in event mode E,
+  // t_{c+1}, the decay samples, completions and arrivals; where rows can die (compact) the inadmissible requeue and the
+  // compaction over [0, bound); then the heads of the next cycle.  A plain drain ends at a cycle without heads or one
+  // that neither admits nor evicts (the next cycle would see the same snapshot); an event drain when no event is left.
+  // Capacity: before the compaction the tables hold the live rows plus this cycle's admissions, and every admitted head
+  // is a workload that holds no row, so the rows stay within A_in + min(W, Hcap * max_cycles) and the cells within
+  // AU_in + min(P * R, that bound * FR) (a readmitted victim's old cells left with its old row): what upload_impl
+  // reserved.  An admission past the end is not written and the call fails.
+  for (int cyc = 0, jumps = 0; cyc < max_cycles;) {
     const bool jump = n_live == 0;
+    if (jump && !events) break;
     const int32_t *n_new_d = jump ? nullptr : X.e_adm_off + n_live;
     if (!jump) {
       D.H = n_live; D.now_ns = t;
-      D.A = pre ? A_cur : 0; D.AU = pre ? AU_cur : 0;
+      D.A = pre ? A_cur : 0; D.AU = pre ? AU_cur : 0;  // without preemption policies the cycle never looks at the admitted tables
       rc = cycle_enqueue(h);
       if (rc != KB_OK) return rc;
       X.cycle = cyc;
@@ -1688,153 +1690,93 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     }
     X.A = A_cur; X.AU = AU_cur; X.trace_off = (long long)out->n_decisions;
     kmark(h, KB_K_DRAIN);
-    CUDA_TRY(h, cudaMemsetAsync(X.counters + 1, 0, 4 * 4, h->stream));
-    CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_FINISHED, 0, 3 * 4, h->stream));
+    if (compact) CUDA_TRY(h, cudaMemsetAsync(X.counters + 1, 0, 4 * 4, h->stream));
+    if (events) CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_FINISHED, 0, 3 * 4, h->stream));
     int bound = A_cur;  // rows the boundary looks at: the tables plus room for this cycle's admissions
     if (!jump) {
       const int nbH = (n_live + tb - 1) / tb;
       k_drain_apply<<<nbH, tb, 0, h->stream>>>(D, X);
       k_scan_i32<<<1, 1024, 0, h->stream>>>(X.e_assumed, X.e_adm_off, n_live);
       k_scan_i32<<<1, 1024, 0, h->stream>>>(X.e_ncells, X.e_cell_off, n_live);
-      k_drain_admit<<<nbH, tb, 0, h->stream>>>(D, X, t, nullptr);
+      k_drain_admit<<<nbH, tb, 0, h->stream>>>(D, X, t);
       if (evict) k_drain_evict<<<nbH, tb, 0, h->stream>>>(D, X);
       bound = (int)std::min<size_t>((size_t)A_cur + n_live, Acap);
     }
-    const int nbB = std::max(1, (bound + tb - 1) / tb);
-    k_drain_ev_min<<<nbB, tb, 0, h->stream>>>(X, bound, n_new_d);
-    k_drain_ev_next<<<1, 1, 0, h->stream>>>(X, t, step, jump, n_new_d);
-    if (decay) k_drain_afs_decay<<<nbL, tb, 0, h->stream>>>(D, X, L);  // samples due in (t, t_{c+1}], before the completions
-    k_drain_finish<<<nbB, tb, 0, h->stream>>>(D, X, bound, n_new_d);
-    if (X.arr_key) k_drain_arrive<<<nbArr, tb, 0, h->stream>>>(X);
-    k_drain_requeue<<<nbQ, tb, 0, h->stream>>>(D, X);
-    {
-      DrainDev Xc = X;  // compaction over [0, bound]: the padding rows are stamped dead
-      Xc.A = bound;
+    if (events) {
+      const int nbB = std::max(1, (bound + tb - 1) / tb);
+      k_drain_ev_min<<<nbB, tb, 0, h->stream>>>(X, bound, n_new_d);
+      k_drain_ev_next<<<1, 1, 0, h->stream>>>(X, t, step, jump, n_new_d);
+      if (decay) k_drain_afs_decay<<<nbL, tb, 0, h->stream>>>(D, X, L);  // samples due in (t, t_{c+1}], before the completions
+      k_drain_finish<<<nbB, tb, 0, h->stream>>>(D, X, bound, n_new_d);
+      if (X.arr_key) k_drain_arrive<<<nbArr, tb, 0, h->stream>>>(X);
+    }
+    if (compact) {
+      k_drain_requeue<<<nbQ, tb, 0, h->stream>>>(D, X);
       const int nbA = (bound + 1 + tb - 1) / tb;
-      k_drain_live<<<nbA, tb, 0, h->stream>>>(Xc);
+      k_drain_live<<<nbA, tb, 0, h->stream>>>(X, bound, n_new_d);
       size_t sb = scan_bytes;
       CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(scan_tmp, sb, X.row_live, X.row_new, bound + 1, h->stream));
       sb = scan_bytes;
       CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(scan_tmp, sb, X.row_cells, X.cell_new, bound + 1, h->stream));
-      k_drain_compact<<<nbA, tb, 0, h->stream>>>(Xc, other);
+      k_drain_compact<<<nbA, tb, 0, h->stream>>>(X, other, bound);
     }
     enqueue_heads();
     kmark(h, -1);
     CUDA_TRY(h, cudaEventRecord(h->ev_d, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[8], X.counters, 4, cudaMemcpyDeviceToHost, h->stream));
-    if (!jump) CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[9], n_new_d, 4, cudaMemcpyDeviceToHost, h->stream));
-    if (afs && (!jump || decay)) CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[11], D.status, 4, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[12], X.counters + 1, 10 * 4, cudaMemcpyDeviceToHost, h->stream));  // .. [KB_DC_ARR_HI]
-    CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[22], X.clock, 8, cudaMemcpyDeviceToHost, h->stream));             // t_{c+1}
+    CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[0], X.counters, 4, cudaMemcpyDeviceToHost, h->stream));
+    if (!jump) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_new, n_new_d, 4, cudaMemcpyDeviceToHost, h->stream));
+    if (!compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_cells, X.e_cell_off + n_live, 4, cudaMemcpyDeviceToHost, h->stream));
+    if (afs && (!jump || decay)) CUDA_TRY(h, cudaMemcpyAsync(&hw.status, D.status, 4, cudaMemcpyDeviceToHost, h->stream));
+    if (compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[1], X.counters + 1, (events ? KB_DC_ARR_HI : KB_DC_FULL) * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (events) CUDA_TRY(h, cudaMemcpyAsync(&hw.t_next, X.clock, 8, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     if (!jump) {
       rc = cycle_finish(h);
       if (rc != KB_OK) return rc;
-      if (afs && (h->host_words[11] & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: an entry penalty overflows int64");
+      if (afs && (hw.status & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: an entry penalty overflows int64");
       for (int i = 0; i < KB_N_KERNELS; i++) kms[i] += h->stats.kernel_ms[i];
     }
-    if (decay && (h->host_words[11] & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: a decayed consumed quantity overflows int64");
+    if (decay && (hw.status & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: a decayed consumed quantity overflows int64");
     { float ms = 0; cudaEventElapsedTime(&ms, h->ev2, h->ev_d); gpu_ms += ms; }
-    if (h->host_words[16]) return fail(h, KB_ERR_CAPACITY, "kb_run_drain: the admitted tables are full");
-    const int fin = (int)h->host_words[12 + KB_DC_FINISHED - 1], arr = (int)h->host_words[12 + KB_DC_ARRIVED - 1];
-    const bool end = h->host_words[12 + KB_DC_END - 1] != 0;
-    i64 t_next;
-    memcpy(&t_next, &h->host_words[22], 8);
+    if (compact && hw.counters[KB_DC_FULL]) return fail(h, KB_ERR_CAPACITY, "kb_run_drain: the admitted tables are full");
+    const int n_new = jump ? 0 : (int)hw.n_new, n_ev = evict ? (int)hw.counters[KB_DC_EVICTED] : 0;
     if (!jump) {
-      const int n_new = (int)h->host_words[9], n_ev = (int)h->host_words[12];
       if (out->cycle_heads) out->cycle_heads[cyc] = n_live;
       if (out->cycle_admitted) out->cycle_admitted[cyc] = n_new;
       if (out->cycle_evicted) out->cycle_evicted[cyc] = n_ev;
-      if (out->cycle_start_ns) out->cycle_start_ns[cyc] = t;
-      if (out->cycle_finished) out->cycle_finished[cyc] = 0;
-      if (out->cycle_arrived) out->cycle_arrived[cyc] = 0;
+      if (events && out->cycle_start_ns) out->cycle_start_ns[cyc] = t;
+      if (events && out->cycle_finished) out->cycle_finished[cyc] = 0;
+      if (events && out->cycle_arrived) out->cycle_arrived[cyc] = 0;
       out->n_decisions += n_live; out->n_admitted += n_new; out->n_evicted += n_ev;
       out->n_cycles = ++cyc;
     } else {
       jumps++;
     }
-    out->n_finished += fin; out->n_arrived += arr;
-    if (cyc > 0) {  // events between the start of the last cycle and the next one are that cycle's
-      if (out->cycle_finished) out->cycle_finished[cyc - 1] += fin;
-      if (out->cycle_arrived) out->cycle_arrived[cyc - 1] += arr;
+    if (events) {
+      const int fin = (int)hw.counters[KB_DC_FINISHED], arr = (int)hw.counters[KB_DC_ARRIVED];
+      out->n_finished += fin; out->n_arrived += arr;
+      if (cyc > 0) {  // events between the start of the last cycle and the next one are that cycle's
+        if (out->cycle_finished) out->cycle_finished[cyc - 1] += fin;
+        if (out->cycle_arrived) out->cycle_arrived[cyc - 1] += arr;
+      }
     }
-    // the compacted half becomes the admitted tables of the next boundary
-    A_cur = (int)h->host_words[13]; AU_cur = (int)h->host_words[14];
-    AdmTabs cur{X.adm_cq, X.adm_priority, X.adm_ts, X.adm_qr_ts, X.adm_uid, X.adm_evicted, X.adm_use_start, X.adm_use_fr, X.adm_use_qty, X.adm_wl, X.adm_finish, X.adm_lq};
-    X.adm_cq = other.cq; X.adm_priority = other.priority; X.adm_ts = other.ts; X.adm_qr_ts = other.qr_ts; X.adm_uid = other.uid;
-    X.adm_evicted = other.evicted; X.adm_use_start = other.use_start; X.adm_use_fr = other.use_fr; X.adm_use_qty = other.use_qty; X.adm_wl = other.wl;
-    X.adm_finish = other.finish; X.adm_lq = other.lq;
-    D.adm_cq = X.adm_cq; D.adm_priority = X.adm_priority; D.adm_ts = X.adm_ts; D.adm_qr_ts = X.adm_qr_ts; D.adm_uid = X.adm_uid;
-    D.adm_evicted = X.adm_evicted; D.adm_use_start = X.adm_use_start; D.adm_use_fr = X.adm_use_fr; D.adm_use_qty = X.adm_use_qty;
-    other = cur;
-    n_live = (int)h->host_words[8];
-    if (end) break;
-    t = t_next;
-  }
-  if (events) out->end_ns = t;
-  for (int cyc = 0; !events && cyc < max_cycles && n_live > 0; cyc++) {
-    D.H = n_live; D.now_ns = s->now_ns + cyc;
-    D.A = pre ? A_cur : 0; D.AU = pre ? AU_cur : 0;  // without preemption policies the cycle never looks at the admitted tables
-    rc = cycle_enqueue(h);
-    if (rc != KB_OK) return rc;
-    X.A = A_cur; X.AU = AU_cur; X.cycle = cyc; X.trace_off = (long long)out->n_decisions;
-    const int nbH = (n_live + tb - 1) / tb;
-    kmark(h, KB_K_DRAIN);
-    k_drain_apply<<<nbH, tb, 0, h->stream>>>(D, X);
-    k_scan_i32<<<1, 1024, 0, h->stream>>>(X.e_assumed, X.e_adm_off, n_live);
-    k_scan_i32<<<1, 1024, 0, h->stream>>>(X.e_ncells, X.e_cell_off, n_live);
-    DrainDev Xa = X;  // the tables k_drain_admit appends to
-    if (evict) {
-      CUDA_TRY(h, cudaMemsetAsync(X.counters + 1, 0, 4 * 4, h->stream));
-      k_drain_evict<<<nbH, tb, 0, h->stream>>>(D, X);
-      k_drain_requeue<<<nbQ, tb, 0, h->stream>>>(D, X);
-      const int nbA = (A_cur + 1 + tb - 1) / tb;
-      k_drain_live<<<nbA, tb, 0, h->stream>>>(X);
-      size_t sb = scan_bytes;
-      CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(scan_tmp, sb, X.row_live, X.row_new, A_cur + 1, h->stream));
-      sb = scan_bytes;
-      CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(scan_tmp, sb, X.row_cells, X.cell_new, A_cur + 1, h->stream));
-      k_drain_compact<<<nbA, tb, 0, h->stream>>>(X, other);
-      Xa.adm_cq = other.cq; Xa.adm_priority = other.priority; Xa.adm_ts = other.ts; Xa.adm_qr_ts = other.qr_ts; Xa.adm_uid = other.uid;
-      Xa.adm_evicted = other.evicted; Xa.adm_use_start = other.use_start; Xa.adm_use_fr = other.use_fr; Xa.adm_use_qty = other.use_qty;
-      Xa.adm_wl = other.wl;
-    }
-    k_drain_admit<<<nbH, tb, 0, h->stream>>>(D, Xa, s->now_ns + cyc, evict ? X.counters + 2 : nullptr);
-    enqueue_heads();
-    kmark(h, -1);
-    CUDA_TRY(h, cudaEventRecord(h->ev_d, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[8], X.counters, 4, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[9], X.e_adm_off + n_live, 4, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[10], X.e_cell_off + n_live, 4, cudaMemcpyDeviceToHost, h->stream));
-    if (afs) CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[11], D.status, 4, cudaMemcpyDeviceToHost, h->stream));  // after k_drain_admit
-    if (evict) CUDA_TRY(h, cudaMemcpyAsync(&h->host_words[12], X.counters + 1, 5 * 4, cudaMemcpyDeviceToHost, h->stream));  // evictions, live rows / cells, capacity
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    rc = cycle_finish(h);
-    if (rc != KB_OK) return rc;
-    if (afs && (h->host_words[11] & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: an entry penalty overflows int64");
-    for (int i = 0; i < KB_N_KERNELS; i++) kms[i] += h->stats.kernel_ms[i];
-    { float ms = 0; cudaEventElapsedTime(&ms, h->ev2, h->ev_d); gpu_ms += ms; }
-    if (evict && h->host_words[16]) return fail(h, KB_ERR_CAPACITY, "kb_run_drain: the admitted tables are full");
-    int n_new = (int)h->host_words[9], n_cells = (int)h->host_words[10];
-    const int n_ev = evict ? (int)h->host_words[12] : 0;
-    if (out->cycle_heads) out->cycle_heads[cyc] = n_live;
-    if (out->cycle_admitted) out->cycle_admitted[cyc] = n_new;
-    if (out->cycle_evicted) out->cycle_evicted[cyc] = n_ev;
-    out->n_cycles = cyc + 1; out->n_decisions += n_live; out->n_admitted += n_new; out->n_evicted += n_ev;
-    if (evict) {  // the compacted half becomes the admitted tables of the next cycle
-      A_cur = (int)h->host_words[13] + n_new; AU_cur = (int)h->host_words[14] + n_cells;
-      AdmTabs cur{X.adm_cq, X.adm_priority, X.adm_ts, X.adm_qr_ts, X.adm_uid, X.adm_evicted, X.adm_use_start, X.adm_use_fr, X.adm_use_qty, X.adm_wl};
+    if (compact) {  // the compacted half becomes the admitted tables of the next boundary
+      A_cur = (int)hw.counters[KB_DC_ROWS]; AU_cur = (int)hw.counters[KB_DC_CELLS];
+      AdmTabs cur{X.adm_cq, X.adm_priority, X.adm_ts, X.adm_qr_ts, X.adm_uid, X.adm_evicted, X.adm_use_start, X.adm_use_fr, X.adm_use_qty, X.adm_wl, X.adm_finish, X.adm_lq};
       X.adm_cq = other.cq; X.adm_priority = other.priority; X.adm_ts = other.ts; X.adm_qr_ts = other.qr_ts; X.adm_uid = other.uid;
       X.adm_evicted = other.evicted; X.adm_use_start = other.use_start; X.adm_use_fr = other.use_fr; X.adm_use_qty = other.use_qty; X.adm_wl = other.wl;
+      X.adm_finish = other.finish; X.adm_lq = other.lq;
       D.adm_cq = X.adm_cq; D.adm_priority = X.adm_priority; D.adm_ts = X.adm_ts; D.adm_qr_ts = X.adm_qr_ts; D.adm_uid = X.adm_uid;
       D.adm_evicted = X.adm_evicted; D.adm_use_start = X.adm_use_start; D.adm_use_fr = X.adm_use_fr; D.adm_use_qty = X.adm_use_qty;
       other = cur;
     } else {
-      A_cur += n_new; AU_cur += n_cells;
+      A_cur += n_new; AU_cur += (int)hw.n_cells;
     }
-    n_live = (int)h->host_words[8];
-    if (n_new == 0 && n_ev == 0) break;  // nothing admitted or evicted: the next cycle would see the same snapshot
+    n_live = (int)hw.counters[0];
+    if (events ? hw.counters[KB_DC_END] != 0 : n_new == 0 && n_ev == 0) break;
+    t = events ? hw.t_next : t + 1;
   }
+  if (events) out->end_ns = t;
   out->gpu_ms = gpu_ms;
   h->stats.last_cycle_gpu_ms = gpu_ms;
   memcpy(h->stats.kernel_ms, kms, sizeof(kms));
@@ -1970,48 +1912,47 @@ extern "C" int32_t kb_tas_find(kb_handle *h, const kb_tas_topology *t, const kb_
     }
     // the per-CTA lists stay under 256 MiB: a long list_cap (over-used leaves) runs fewer CTAs, each walking more requests
     const int sel_grid = (int)std::max<size_t>(1, std::min<size_t>({max_round, (size_t)h->sm_count * 8, ((size_t)256 << 20) / ((size_t)24 * list_cap)}));
-    // ---- device buffer (grow-only)
-    size_t tot = 0;
-    auto need = [&](size_t n, size_t sz) { tot += pad256(n * sz); };
-    need(L + 1, 4); need(ND, 4); need(ND + 1, 4); need((size_t)NL * R, 8); need(NL, 4); need((size_t)NL * R, 8); need(NL, 4);
-    need((size_t)NQ * R, 8); for (int k = 0; k < 10; k++) need(NQ, 4); need(r->leaf_ok ? (size_t)NQ * ok_words : 1, 4);
-    need(max_slots * ND, 4); need(max_slots * ND, 4); need((size_t)n_chain_slots * NL * R, 8); need((size_t)n_chain_slots * NL, 4);
-    need(NQ + 1, 4); need(NQ + 1, 4); need(NQ + 2, 4); need(tmp_start[NQ] + 1, 4); need(tmp_start[NQ] + 1, 4);
-    need((size_t)sel_grid * 6 * list_cap, 4); need(2, 4); need(max_round, 4); need(max_slots, 4); need(std::max(1, out->capacity), 4); need(std::max(1, out->capacity), 4);
-    if (tot > h->tas_buf_cap) {
-      if (h->tas_buf) cudaFree(h->tas_buf);
-      h->tas_buf = nullptr; h->tas_buf_cap = 0;
-      CUDA_TRY(h, cudaMalloc(&h->tas_buf, tot + (1 << 20)));
-      h->tas_buf_cap = tot + (1 << 20);
-    }
-    size_t used = 0;
-    auto take = [&](size_t n, size_t sz) { char *p = h->tas_buf + used; used += pad256(n * sz); return p; };
-    auto upl = [&](const void *src, size_t n, size_t sz) -> char * { char *d = take(n, sz); if (n) cudaMemcpyAsync(d, src, n * sz, cudaMemcpyHostToDevice, h->stream); return d; };
+    // ---- device buffer (grow-only), described once (Arena::carve)
     TasDev T{};
+    int32_t *d_asg_start, *d_round, *d_slotreq, *d_leaf, *d_cnt;
+    const size_t n_tmp = (size_t)tmp_start[NQ] + 1, n_asg = (size_t)std::max(1, out->capacity);
+    auto layout = [&](Arena &a) {
+      T.level_start = a.take<int32_t>(L + 1); T.parent = a.take<int32_t>(ND); T.child_start = a.take<int32_t>(ND + 1);
+      T.free_cap = a.take<i64>((size_t)NL * R); T.cap_mask = a.take<uint32_t>(NL);
+      T.tas_usage = a.take<i64>((size_t)NL * R); T.usage_mask = a.take<uint32_t>(NL);
+      T.pod_request = a.take<i64>((size_t)NQ * R); T.request_mask = a.take<uint32_t>(NQ);
+      T.flags = a.take<uint32_t>(NQ); T.count = a.take<int32_t>(NQ);
+      T.slice_size = a.take<int32_t>(NQ); T.level = a.take<int32_t>(NQ); T.slice_level = a.take<int32_t>(NQ);
+      T.slot = a.take<int32_t>(NQ); T.chain_slot = a.take<int32_t>(NQ); T.pred = a.take<int32_t>(NQ);
+      if (r->leaf_ok) T.leaf_ok = a.take<uint32_t>((size_t)NQ * ok_words);
+      T.state = a.take<int32_t>(max_slots * ND); T.slice = a.take<int32_t>(max_slots * ND);
+      T.assumed = a.take<i64>((size_t)n_chain_slots * NL * R); T.assumed_mask = a.take<uint32_t>((size_t)n_chain_slots * NL);
+      T.status = a.take<int32_t>(NQ + 1); T.n_out = a.take<int32_t>(NQ + 1);
+      d_asg_start = a.take<int32_t>(NQ + 2);
+      T.tmp_start = a.take<int32_t>(NQ + 1); T.tmp_leaf = a.take<int32_t>(n_tmp); T.tmp_count = a.take<int32_t>(n_tmp);
+      T.lists = a.take<int32_t>((size_t)sel_grid * 6 * list_cap);
+      T.overflow = a.take<int32_t>(2);
+      d_round = a.take<int32_t>(max_round); d_slotreq = a.take<int32_t>(max_slots);
+      d_leaf = a.take<int32_t>(n_asg); d_cnt = a.take<int32_t>(n_asg);
+    };
+    if (!h->tas_arena.carve(layout)) return fail(h, KB_ERR_CUDA, "tas: cudaMalloc of the device buffer failed");
     T.L = L; T.n_domains = ND; T.n_leaves = NL; T.leaf0 = leaf0; T.R = R; T.pods_res = t->pods_resource; T.n_req = NQ;
-    T.level_start = (const int32_t *)upl(t->level_start, L + 1, 4); T.parent = (const int32_t *)upl(t->parent, ND, 4);
-    T.child_start = (const int32_t *)upl(cstart.data(), ND + 1, 4);
-    T.free_cap = (const i64 *)upl(t->free_capacity, (size_t)NL * R, 8); T.cap_mask = (const uint32_t *)upl(t->cap_mask, NL, 4);
-    T.tas_usage = (const i64 *)upl(t->tas_usage, (size_t)NL * R, 8); T.usage_mask = (const uint32_t *)upl(t->usage_mask, NL, 4);
-    T.pod_request = (const i64 *)upl(r->pod_request, (size_t)NQ * R, 8); T.request_mask = (const uint32_t *)upl(r->request_mask, NQ, 4);
-    T.flags = (const uint32_t *)upl(r->flags, NQ, 4); T.count = (const int32_t *)upl(r->count, NQ, 4);
-    T.slice_size = (const int32_t *)upl(r->slice_size, NQ, 4); T.level = (const int32_t *)upl(r->level, NQ, 4);
-    T.slice_level = (const int32_t *)upl(r->slice_level, NQ, 4);
-    T.slot = (const int32_t *)upl(slot.data(), NQ, 4); T.chain_slot = (const int32_t *)upl(chain_slot.data(), NQ, 4); T.pred = (const int32_t *)upl(pred.data(), NQ, 4);
-    T.leaf_ok = r->leaf_ok ? (const uint32_t *)upl(r->leaf_ok, (size_t)NQ * ok_words, 4) : nullptr; T.ok_words = ok_words;
-    T.state = (int32_t *)take(max_slots * ND, 4); T.slice = (int32_t *)take(max_slots * ND, 4);
-    T.assumed = (i64 *)take((size_t)n_chain_slots * NL * R, 8); T.assumed_mask = (uint32_t *)take((size_t)n_chain_slots * NL, 4);
-    if (n_chain_slots) { cudaMemsetAsync(T.assumed, 0, (size_t)n_chain_slots * NL * R * 8, h->stream); cudaMemsetAsync(T.assumed_mask, 0, (size_t)n_chain_slots * NL * 4, h->stream); }
-    T.status = (int32_t *)take(NQ + 1, 4); T.n_out = (int32_t *)take(NQ + 1, 4);
-    int32_t *d_asg_start = (int32_t *)take(NQ + 2, 4);
-    T.tmp_start = (int32_t *)upl(tmp_start.data(), NQ + 1, 4);
-    T.tmp_leaf = (int32_t *)take(tmp_start[NQ] + 1, 4); T.tmp_count = (int32_t *)take(tmp_start[NQ] + 1, 4);
-    T.lists = (int32_t *)take((size_t)sel_grid * 6 * list_cap, 4); T.list_cap = list_cap; T.keep_zero = keep_zero;
-    T.overflow = (int32_t *)take(2, 4);
-    cudaMemsetAsync(T.overflow, 0, 8, h->stream);
-    int32_t *d_round = (int32_t *)take(max_round, 4), *d_slotreq = (int32_t *)take(max_slots, 4);
-    int32_t *d_leaf = (int32_t *)take(std::max(1, out->capacity), 4), *d_cnt = (int32_t *)take(std::max(1, out->capacity), 4);
-    if (NQ) cudaMemsetAsync(T.n_out, 0, (size_t)(NQ + 1) * 4, h->stream);
+    T.ok_words = ok_words; T.list_cap = list_cap; T.keep_zero = keep_zero;
+    const size_t nq = (size_t)NQ, nl = (size_t)NL;
+    const struct { const void *dst, *src; size_t bytes; } uploads[] = {
+        {T.level_start, t->level_start, (size_t)(L + 1) * 4}, {T.parent, t->parent, (size_t)ND * 4}, {T.child_start, cstart.data(), (size_t)(ND + 1) * 4},
+        {T.free_cap, t->free_capacity, nl * R * 8}, {T.cap_mask, t->cap_mask, nl * 4}, {T.tas_usage, t->tas_usage, nl * R * 8}, {T.usage_mask, t->usage_mask, nl * 4},
+        {T.pod_request, r->pod_request, nq * R * 8}, {T.request_mask, r->request_mask, nq * 4}, {T.flags, r->flags, nq * 4}, {T.count, r->count, nq * 4},
+        {T.slice_size, r->slice_size, nq * 4}, {T.level, r->level, nq * 4}, {T.slice_level, r->slice_level, nq * 4},
+        {T.slot, slot.data(), nq * 4}, {T.chain_slot, chain_slot.data(), nq * 4}, {T.pred, pred.data(), nq * 4},
+        {T.leaf_ok, r->leaf_ok, r->leaf_ok ? nq * ok_words * 4 : 0}, {T.tmp_start, tmp_start.data(), (nq + 1) * 4}};
+    for (const auto &u : uploads) CUDA_TRY(h, h2d(h, u.dst, u.src, u.bytes));
+    if (n_chain_slots) {
+      CUDA_TRY(h, cudaMemsetAsync(T.assumed, 0, (size_t)n_chain_slots * nl * R * 8, h->stream));
+      CUDA_TRY(h, cudaMemsetAsync(T.assumed_mask, 0, (size_t)n_chain_slots * nl * 4, h->stream));
+    }
+    CUDA_TRY(h, cudaMemsetAsync(T.overflow, 0, 8, h->stream));
+    if (NQ) CUDA_TRY(h, cudaMemsetAsync(T.n_out, 0, (nq + 1) * 4, h->stream));
     CUDA_TRY(h, cudaEventRecord(h->ev2, h->stream));
     h->kev_n = 0;
     int launches = 0;

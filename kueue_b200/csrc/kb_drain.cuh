@@ -12,14 +12,14 @@
 // apply the decisions — admissions extend the admitted tables and the ClusterQueue usage on the device, the others
 // keep their LastAssignment and move per the Strict / BestEffort FIFO rules.
 //
-// Eviction replay (kb_snapshot.adm_wl != NULL, a preemption policy somewhere): after the decisions, k_drain_evict
-// takes every target of every Preempting entry out of the ClusterQueue usage, flags its row dead and requeues its
-// pending record (LastAssignment nil; the cursor moves back to it if it lies before).  k_drain_requeue then returns
-// every set-aside workload of the ClusterQueues of the victims' root cohort trees to its queue, moving the cursor back
-// to the first of them (first_aside tracks that position per segment).  k_drain_live + two exclusive scans +
-// k_drain_compact copy the live rows, in order, into the other half of a double buffer, and k_drain_admit appends
-// the cycle's admissions after them.  A workload holds at most one live row, so the live rows never exceed the
-// capacity drain_impl reserves (kb_api.cu).
+// Eviction replay (kb_snapshot.adm_wl != NULL, a preemption policy somewhere): after the decisions and k_drain_admit,
+// k_drain_evict takes every target of every Preempting entry out of the ClusterQueue usage, flags its row dead and
+// requeues its pending record (LastAssignment nil; the cursor moves back to it if it lies before).  k_drain_requeue
+// then returns every set-aside workload of the ClusterQueues of the victims' root cohort trees to its queue, moving the
+// cursor back to the first of them (first_aside tracks that position per segment).  k_drain_live + two exclusive scans
+// + k_drain_compact copy the live rows, in order, into the other half of a double buffer: the rows the cycle started
+// with, then the admissions k_drain_admit appended after them.  A workload holds at most one live row, so the rows
+// never exceed the capacity drain_impl reserves (kb_api.cu).
 //
 // AdmissionFairSharing (kb_snapshot.wl_lq != NULL): the queue of a ClusterQueue with cq_afs set is one SEGMENT per
 // LocalQueue (each sorted as above, each with its own cursor); every other ClusterQueue is one segment.  Segments are
@@ -32,15 +32,15 @@
 //
 // Event mode (kb_snapshot.wl_create_ns / wl_run_ns / adm_finish_ns; include/kueue_b200.h): two more states,
 // KB_WS_ABSENT (not created yet) and KB_WS_FINISHED.  Every admitted row carries its finish time (adm_finish, written by
-// k_drain_admit, carried by the compaction) and its record (adm_wl, -1 for a row of the snapshot without one).  After
-// the decisions of a cycle: k_drain_admit appends the admissions to the current half, k_drain_evict replays the
-// evictions, k_drain_ev_min reduces E (the earliest finish of a live row and the next creation), k_drain_ev_next (one
-// thread) computes t_{c+1} and the end flag, k_drain_finish stamps the finished rows dead with the eviction stamp and
-// takes their cells out (a row admitted in this cycle that finishes by t_{c+1} dies before any cycle sees it),
-// k_drain_arrive walks the arrived prefix of the (create, index) order, k_drain_requeue visits the marked roots, and
-// the compaction copies the live rows into the other half.  A cycle without heads is replaced by the same boundary
-// with t_{c+1} = E and a negative stamp (no cycle is counted).  The NoFit set of a ClusterQueue is one byte per
-// (ClusterQueue, scheduling hash) class: k_drain_apply sets it, k_drain_requeue clears the bytes of the queues it visits.
+// k_drain_admit, carried by the compaction) and its record (adm_wl, -1 for a row of the snapshot without one).  The
+// boundary is the replay's, with the clock between the evictions and the requeue: k_drain_ev_min reduces E (the
+// earliest finish of a live row and the next creation), k_drain_ev_next (one thread) computes t_{c+1} and the end
+// flag, k_drain_finish stamps the finished rows dead with the eviction stamp and takes their cells out (a row admitted
+// in this cycle that finishes by t_{c+1} dies before any cycle sees it), k_drain_arrive walks the arrived prefix of the
+// (create, index) order; then k_drain_requeue visits the marked roots and the compaction follows.  A cycle without heads
+// is replaced by the same boundary with t_{c+1} = E and a negative stamp (no cycle is counted).  The NoFit set of a
+// ClusterQueue is one byte per (ClusterQueue, scheduling hash) class: k_drain_apply sets it, k_drain_requeue clears the
+// bytes of the queues it visits.
 #pragma once
 
 #include <cub/device/device_scan.cuh>
@@ -214,8 +214,10 @@ struct DrainDev {
   const int32_t *cq_class_start;   // [Q+1] classes of a ClusterQueue
   uint8_t *class_nofit;            // [classes] in the ClusterQueue's NoFit set; null = no arrivals or no hashes
 };
-// counters of event mode: [6] completions, [7] arrivals, [8] end flag, [9] / [10] arrived prefix of arr_order [lo, hi)
-enum { KB_DC_FINISHED = 6, KB_DC_ARRIVED = 7, KB_DC_END = 8, KB_DC_ARR_LO = 9, KB_DC_ARR_HI = 10 };
+// counters of a boundary: [1] evictions, [2] / [3] rows / cells after the compaction, [5] capacity flag; event mode:
+// [6] completions, [7] arrivals, [8] end flag, [9] / [10] arrived prefix of arr_order [lo, hi)
+enum { KB_DC_EVICTED = 1, KB_DC_ROWS = 2, KB_DC_CELLS = 3, KB_DC_FULL = 5,
+       KB_DC_FINISHED = 6, KB_DC_ARRIVED = 7, KB_DC_END = 8, KB_DC_ARR_LO = 9, KB_DC_ARR_HI = 10 };
 
 __device__ __forceinline__ int drain_seg0(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq] : cq; }
 __device__ __forceinline__ int drain_seg1(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq + 1] : cq + 1; }
@@ -398,16 +400,15 @@ __global__ void k_drain_apply(DevSnap D, DrainDev X) {
   }
 }
 
-// admitted entries join the admitted tables (cache.AssumeWorkload) and the ClusterQueue usage
-// (replay: after the compaction, base = {live rows, their cells} on the device; otherwise X.A / X.AU)
-__global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts, const int32_t *base) {
+// admitted entries join the admitted tables (cache.AssumeWorkload), appended at X.A / X.AU, and the ClusterQueue usage
+__global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
   int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= D.H || !X.e_assumed[e]) return;
   const int R = D.R;
   int wl = D.heads[e], cq = D.wl_cq[wl];
-  int a = (base ? base[0] : X.A) + X.e_adm_off[e];
-  int c0 = (base ? base[1] : X.AU) + X.e_cell_off[e];
-  if (a >= X.A_cap || c0 + X.e_ncells[e] > X.AU_cap) { atomicOr(&X.counters[5], 1); return; }  // nothing past the end
+  int a = X.A + X.e_adm_off[e];
+  int c0 = X.AU + X.e_cell_off[e];
+  if (a >= X.A_cap || c0 + X.e_ncells[e] > X.AU_cap) { atomicOr(&X.counters[KB_DC_FULL], 1); return; }  // nothing past the end
   if (X.adm_wl) X.adm_wl[a] = wl;
   if (X.adm_lq) X.adm_lq[a] = X.wl_lq[wl];
   X.adm_cq[a] = cq; X.adm_priority[a] = D.wl_priority[wl]; X.adm_ts[a] = D.wl_ts[wl]; X.adm_qr_ts[a] = qr_ts;
@@ -494,7 +495,7 @@ __global__ void k_drain_evict(DevSnap D, DrainDev X) {
     X.wl_evictions[w]++;  // a workload holds at most one row: one writer
     atomicMin(&X.cursor[X.wl_seg[w]], X.wl_pos[w]);
     X.root_mark[D.root_slot[cq]] = stamp;
-    atomicAdd(&X.counters[1], 1);
+    atomicAdd(&X.counters[KB_DC_EVICTED], 1);
   }
 }
 // inadmissible requeue (thread per ClusterQueue of a marked root): set aside -> queued, cursor back to the first of them
@@ -509,20 +510,22 @@ __global__ void k_drain_requeue(DevSnap D, DrainDev X) {
     X.first_aside[s] = qn;
   }
 }
-// compaction: live flags and cell counts of the rows before this cycle's admissions ([A] = 0 closes the scans)
-__global__ void k_drain_live(DrainDev X) {
+// compaction: live flags and cell counts of the rows [0, bound) ([bound] = 0 closes the scans).  The rows are the
+// tables the cycle started with, less those stamped dead at this boundary, and the *n_new admissions appended after
+// them; rows past those only pad the range.  After a capacity overflow no row is live: not every admission was written.
+__global__ void k_drain_live(DrainDev X, int bound, const int32_t *n_new) {
   int a = blockIdx.x * blockDim.x + threadIdx.x;
-  if (a > X.A) return;
-  const bool live = a < X.A && X.adm_dead[a] != X.cycle + 1;
+  if (a > bound) return;
+  const bool live = a < bound && a < X.A + (n_new ? *n_new : 0) && !X.counters[KB_DC_FULL] && X.adm_dead[a] != X.cycle + 1;
   X.row_live[a] = live;
   X.row_cells[a] = live ? X.adm_use_start[a + 1] - X.adm_use_start[a] : 0;
 }
 struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; i64 *finish; int32_t *lq; };
-// live rows, in order, into the other half of the double buffer; thread A writes the totals (counters[2..3])
-__global__ void k_drain_compact(DrainDev X, AdmTabs O) {
+// live rows of [0, bound), in order, into the other half of the double buffer; thread bound writes the totals
+__global__ void k_drain_compact(DrainDev X, AdmTabs O, int bound) {
   int a = blockIdx.x * blockDim.x + threadIdx.x;
-  if (a > X.A) return;
-  if (a == X.A) { O.use_start[X.row_new[a]] = X.cell_new[a]; X.counters[2] = X.row_new[a]; X.counters[3] = X.cell_new[a]; return; }
+  if (a > bound) return;
+  if (a == bound) { O.use_start[X.row_new[a]] = X.cell_new[a]; X.counters[KB_DC_ROWS] = X.row_new[a]; X.counters[KB_DC_CELLS] = X.cell_new[a]; return; }
   if (!X.row_live[a]) return;
   const int n = X.row_new[a], c0 = X.cell_new[a], u0 = X.adm_use_start[a], nc = X.adm_use_start[a + 1] - u0;
   O.cq[n] = X.adm_cq[a]; O.priority[n] = X.adm_priority[a]; O.ts[n] = X.adm_ts[a]; O.qr_ts[n] = X.adm_qr_ts[a];
@@ -577,7 +580,7 @@ __global__ void k_drain_ev_min(DrainDev X, int bound, const int32_t *n_new) {
 __global__ void k_drain_ev_next(DrainDev X, i64 t_c, i64 step, int jump, const int32_t *n_new) {
   const i64 E = X.clock[1];
   const i64 stepped = t_c > INT64_MAX - step ? INT64_MAX : t_c + step;
-  const bool active = !jump && ((n_new && *n_new > 0) || X.counters[1] > 0);
+  const bool active = !jump && ((n_new && *n_new > 0) || X.counters[KB_DC_EVICTED] > 0);
   i64 tn;
   bool end = false;
   if (jump) { end = E == INT64_MAX; tn = E; }
@@ -592,12 +595,11 @@ __global__ void k_drain_ev_next(DrainDev X, i64 t_c, i64 step, int jump, const i
 }
 // completions (thread per row): a live row with finish <= t_{c+1} gets the dead stamp, its cells leave its ClusterQueue's
 // usage (cache.DeleteWorkload, integer atomics), its record becomes FINISHED and its root tree is marked.  Rows in
-// [A + *n_new, bound) only pad the compaction's range: they are stamped dead.
+// [A + *n_new, bound) only pad the compaction's range.
 __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *n_new) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x;
-  if (a >= bound || X.counters[5]) return;
+  if (a >= bound || a >= X.A + (n_new ? *n_new : 0) || X.counters[KB_DC_FULL]) return;
   const int stamp = X.cycle + 1;
-  if (a >= X.A + (n_new ? *n_new : 0)) { X.adm_dead[a] = stamp; return; }
   if (X.counters[KB_DC_END] || X.adm_dead[a] == stamp || X.adm_finish[a] > X.clock[0]) return;
   X.adm_dead[a] = stamp;
   const int cq = X.adm_cq[a];
