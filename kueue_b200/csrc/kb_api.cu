@@ -25,10 +25,13 @@ struct Arena {
   char *base = nullptr;
   size_t cap = 0, used = 0;
   void reset() { used = 0; }
+  void release() {
+    if (base) cudaFree(base);
+    base = nullptr; cap = used = 0;
+  }
   bool reserve(size_t bytes) {
     if (bytes <= cap) return true;
-    if (base) cudaFree(base);
-    base = nullptr; cap = 0;
+    release();
     size_t want = bytes + bytes / 4 + (1 << 20);
     if (cudaMalloc(&base, want) != cudaSuccess) return false;
     cap = want;
@@ -48,6 +51,20 @@ struct Arena {
     layout(*this);
     return true;
   }
+};
+
+// Launch configuration of the preemption-target searches, and the scratch sizes the per-cycle arena takes for them
+// (plan_search).  The classical-search fields keep their values through uploads that have no classical search.
+struct SearchPlan {
+  // fair-sharing search: single-warp CTAs on a private copy of the whole tree
+  int search_grid = 1; bool search_smem = true; size_t search_smem_bytes = 0;
+  // warp-cooperative classical search (k_search_cells / k_nominate_walk)
+  int sa_wpb = 1, sa_grid = 1, sa_col_elems = 0, sa_codes = 0; size_t sa_smem = 0;
+  int sb_wpb = 1, sb_grid = 1, sb_col_elems = 0; size_t sb_smem = 0;
+  int sa_list_cap = 32, sb_list_cap = 32;
+  bool sg_on = false; int sg_wpb = 1, sg_grid = 1, sg_ncap = 1; size_t sg_smem = 0;  // grouped form of k_search_cells
+  // scratch: memo rows, per-warp columns and lists, fair-search state for G CTAs of acap admitted rows and ncap nodes
+  size_t memo_items = 0, ws_warps = 1, ws_col_stride = 0, ws_list_total = 32, G = 1, acap = 1, ncap = 1;
 };
 
 }  // namespace
@@ -91,10 +108,7 @@ struct kb_handle {
   int max_root_adm = 1;
   int max_frl_len = 1;      // longest (root, flavor-resource) candidate bucket of this cycle
   int max_head_podsets = 1; // most podsets of one entry (bounds the columns a GetTargets search tracks)
-  // launch configuration of the warp-cooperative classical search (k_search_cells / k_nominate_walk)
-  int sa_wpb = 1, sa_grid = 1, sa_col_elems = 0, sa_codes = 0; size_t sa_smem = 0;
-  int sb_wpb = 1, sb_grid = 1, sb_col_elems = 0; size_t sb_smem = 0;
-  int sa_list_cap = 32, sb_list_cap = 32;
+  SearchPlan plan;
   // kb_run_drain: capacity reserved beyond the snapshot's admitted tables, heads chosen on the device
   size_t drain_extra_adm = 0, drain_extra_au = 0; bool drain_mode = false; bool preempt_possible = true;
   bool drain_events = false;  // kb_run_drain in event mode: rows admitted during the drain are preemption candidates
@@ -107,12 +121,8 @@ struct kb_handle {
   i64 *d_usage_res = nullptr; size_t usage_res_cells = 0; bool usage_res_valid = false; int64_t usage_res_gen = 0;
   std::vector<uint32_t> delta_seen; uint32_t delta_stamp = 0;
   bool flat_on = false, flat_attr_set = false, hdr_clean = false; size_t flat_static_smem = 0; unsigned rec_stamp = 0; const void *rec_seen = nullptr; size_t rec_seen_n = 0; size_t flat_smem = 0; int flat_rcap = 1; int4 *d_cq_rec = nullptr;
-  bool sg_on = false; int sg_wpb = 1, sg_grid = 1, sg_ncap = 1; size_t sg_smem = 0;  // grouped form of k_search_cells
   // device ranking of the admitted workloads (kb_rank.cuh)
   u64 *rk_keys[2] = {nullptr, nullptr}; int32_t *rk_vals[2] = {nullptr, nullptr}; void *rk_temp = nullptr; size_t rk_temp_bytes = 0;
-  int search_grid = 1;
-  bool search_smem = true;
-  size_t search_smem_bytes = 0;
   int max_tree_nodes = 1;
   int max_root_entries_hint = 0;
 };
@@ -221,11 +231,7 @@ int32_t kb_create(const kb_config *cfg, kb_handle **out) {
 void kb_destroy(kb_handle *h) {
   if (!h) return;
   cudaSetDevice(h->device);
-  if (h->arena.base) cudaFree(h->arena.base);
-  if (h->sarena.base) cudaFree(h->sarena.base);
-  if (h->iarena.base) cudaFree(h->iarena.base);
-  if (h->drain_arena.base) cudaFree(h->drain_arena.base);
-  if (h->tas_arena.base) cudaFree(h->tas_arena.base);
+  for (Arena *a : {&h->arena, &h->sarena, &h->iarena, &h->drain_arena, &h->tas_arena}) a->release();
   if (h->d_usage_res) cudaFree(h->d_usage_res);
   if (h->ev_d) cudaEventDestroy(h->ev_d);
   if (h->host_words) cudaFreeHost(h->host_words);
@@ -594,95 +600,76 @@ __global__ void k_usage_patch(i64 *usage, const int32_t *cq, const i64 *rows, in
   usage[(size_t)cq[i / FR] * FR + i % FR] = rows[i];
 }
 
-template <typename T>
-static cudaError_t up(kb_handle *h, Arena &arena, const T *&dst, const T *src, size_t n, int64_t *bytes) {
-  T *d = arena.take<T>(n);
-  dst = d;
-  if (n == 0) return cudaSuccess;
-  *bytes += (int64_t)(n * sizeof(T));
-  return cudaMemcpyAsync(d, src, n * sizeof(T), cudaMemcpyHostToDevice, h->stream);
-}
 // host -> device on the handle's stream; an empty table copies nothing
 static cudaError_t h2d(kb_handle *h, const void *dst, const void *src, size_t bytes) {
   return bytes ? cudaMemcpyAsync(const_cast<void *>(dst), src, bytes, cudaMemcpyHostToDevice, h->stream) : cudaSuccess;
 }
 
-static int32_t upload_impl(kb_handle *h, const kb_snapshot *s, bool sync) {
-  if (!h || !s) return KB_ERR_INVALID;
-  cudaSetDevice(h->device);
-  h->uploaded = false;
-  DevSnap &D = h->D;
-  int Q = s->n_cq, C = s->n_cohort, N = Q + C, F = s->n_flavor, R = s->n_resource, FR = F * R;
-  // A / AU are CAPACITIES (kb_run_drain grows the admitted tables on the device); A_in / AU_in what the caller passed
-  const size_t A_in = (size_t)s->n_adm, AU_in = (size_t)s->n_adm_use;
-  size_t NF = (size_t)N * FR, P = (size_t)s->n_podset, W = (size_t)s->n_wl, A = A_in + h->drain_extra_adm, H = (size_t)s->n_heads;
-  const size_t AUc = AU_in + h->drain_extra_au;
-  int n_rg_fl = (s->n_rg > 0 && s->rg_flavor_start) ? s->rg_flavor_start[s->n_rg] : 0;
-  int dims[6] = {Q, C, F, R, s->n_rg, n_rg_fl};
-  bool reuse = s->static_generation != 0 && s->static_generation == h->static_gen && memcmp(dims, h->s_dims, sizeof(dims)) == 0;
-  int64_t bytes = 0;
-  int32_t rc;
-  if (!reuse) {
-    h->static_gen = 0;
-    rc = build_static(h, s);
-    if (rc != KB_OK) return rc;
-    size_t stot = 0;
-    auto sneed = [&](size_t n, size_t sz) { stot += pad256(n * sz); };
-    sneed(N, 4); sneed(N, 8); sneed(NF, 8); sneed(NF, 8); sneed(NF, 8);
-    for (int k = 0; k < 4; k++) sneed(Q, 1);
-    sneed(Q, 4); for (int k = 0; k < 4; k++) sneed(Q, 1); sneed(Q, 8);
-    sneed(Q + 1, 4); sneed(s->n_rg, 4); sneed(s->n_rg + 1, 4); sneed(n_rg_fl, 4);
-    sneed(N, 4); sneed(N, 4); sneed(N, 4); sneed(D.nTrees + 1, 4); sneed(h->tree_nodes.size(), 4); sneed(h->tree_level.size(), 4);
-    sneed(h->lone.size(), 4); sneed(N, 4); sneed(h->tree_flat.size(), 1); sneed(N + 1, 4); sneed(h->child_list.size(), 4); sneed(h->root_cq_start.size(), 4);
-    sneed(h->sn_node.size(), 4); sneed(h->slot_base.size(), 4); sneed(h->nd_tin.size(), 4); sneed(h->nd_tout.size(), 4);
-    sneed(h->cq_path.size(), 4); sneed(h->cq_plen.size(), 4);
-    sneed(h->tree_blob.size(), 1); sneed(h->tree_blob_off.size(), 4);
-    const size_t tl_cells = h->tree_nodes.size() * (size_t)FR;
-    sneed(tl_cells, 8); sneed(tl_cells, 8); sneed(tl_cells, 8);
-    if (!h->sarena.reserve(stot + 4096)) return fail(h, KB_ERR_CUDA, "cudaMalloc failed");
-    h->sarena.reset();
-#define SUP(field, src, n) CUDA_TRY(h, up(h, h->sarena, D.field, src, (size_t)(n), &bytes))
-    SUP(parent, s->parent, N); SUP(fair_weight, s->fair_weight, N);
-    SUP(nominal, (const i64 *)s->nominal, NF); SUP(blimit, (const i64 *)s->borrow_limit, NF); SUP(llimit, (const i64 *)s->lend_limit, NF);
-    SUP(cq_within_cq, s->cq_within_cq, Q); SUP(cq_reclaim_within, s->cq_reclaim_within, Q); SUP(cq_borrow_within, s->cq_borrow_within, Q);
-    SUP(cq_has_bwc_threshold, s->cq_has_bwc_threshold, Q); SUP(cq_bwc_threshold, s->cq_bwc_threshold, Q);
-    SUP(cq_when_can_borrow, s->cq_when_can_borrow, Q); SUP(cq_when_can_preempt, s->cq_when_can_preempt, Q);
-    SUP(cq_preference, s->cq_preference, Q); SUP(cq_strategy, s->cq_strategy, Q); SUP(cq_generation, (const i64 *)s->cq_generation, Q);
-    SUP(cq_rg_start, s->cq_rg_start, Q + 1); SUP(rg_res_mask, s->rg_res_mask, s->n_rg); SUP(rg_flavor_start, s->rg_flavor_start, s->n_rg + 1);
-    SUP(rg_flavors, s->rg_flavors, n_rg_fl);
-    SUP(root_slot, h->root_slot.data(), N); SUP(depth, h->depth.data(), N); SUP(height, h->height.data(), N);
-    SUP(tree_start, h->tree_start.data(), D.nTrees + 1); SUP(tree_nodes, h->tree_nodes.data(), h->tree_nodes.size());
-    SUP(tree_level, h->tree_level.data(), h->tree_level.size()); SUP(lone_cqs, h->lone.data(), h->lone.size());
-    SUP(local_idx, h->local_idx.data(), N);
-    SUP(tree_flat, h->tree_flat.data(), h->tree_flat.size());
-    SUP(child_start, h->child_start.data(), N + 1); SUP(child_list, h->child_list.data(), h->child_list.size());
-    SUP(root_cq_start, h->root_cq_start.data(), h->root_cq_start.size());
-    SUP(sn_node, h->sn_node.data(), h->sn_node.size()); SUP(slot_base, h->slot_base.data(), h->slot_base.size());
-    SUP(nd_tin, h->nd_tin.data(), h->nd_tin.size()); SUP(nd_tout, h->nd_tout.data(), h->nd_tout.size());
-    SUP(cq_path, h->cq_path.data(), h->cq_path.size()); SUP(cq_plen, h->cq_plen.data(), h->cq_plen.size());
-    SUP(tree_blob, h->tree_blob.data(), h->tree_blob.size()); SUP(tree_blob_off, h->tree_blob_off.data(), h->tree_blob_off.size());
-    D.tl_subtree = D.tl_blimit = D.tl_lquota = nullptr; D.tl_usage = nullptr;
-    if (tl_cells && tl_cells < (size_t)INT32_MAX) {  // quota tables in tree-local row order (k_cycle_flat's bulk staging)
-      i64 *tn = h->sarena.take<i64>(tl_cells), *tb_ = h->sarena.take<i64>(tl_cells), *tl_ = h->sarena.take<i64>(tl_cells);
-      D.FR = FR; D.Q = Q;
-      k_tl_static<<<(unsigned)((tl_cells + 255) / 256), 256, 0, h->stream>>>(D, tn, tb_, tl_, (int)tl_cells);
-      k_tl_root<<<(unsigned)(((size_t)D.nTrees * FR + 255) / 256), 256, 0, h->stream>>>(D, tn, tl_);
-      D.tl_subtree = tn; D.tl_blimit = tb_; D.tl_lquota = tl_;
-    }
-    D.path_stride = h->path_stride;
-#undef SUP
-    memcpy(h->s_dims, dims, sizeof(dims));
-    h->static_gen = s->static_generation;
-  }
-  // Per-cycle input tables, enqueued FIRST: the DMA runs while the host validates the tables and sizes the scratch
-  // arena below (build_dynamic).  The caller's tables (dynamic part of kb_snapshot) usually sit close together in
-  // one pinned block (kb_alloc_pinned carved by the shim): when their host span is not much larger than their
-  // total size the whole span goes to the device with ONE DMA and the device tables alias into it at the same
-  // offsets; otherwise every table is copied on its own.
-  struct Tab { const void *src; size_t bytes; const void **dst; size_t cap; };
-  std::vector<Tab> tabs;
-#define UPC(field, src, n, capn) tabs.push_back(Tab{(const void *)(src), (size_t)(n) * sizeof(*D.field), (const void **)&D.field, (size_t)(capn) * sizeof(*D.field)})
+// One table of an upload: host source, bytes to copy, the DevSnap pointer that receives its device address, and the
+// device bytes it needs (more than it copies for the admitted tables kb_run_drain grows on the device).
+struct HostTab { const void *src; size_t bytes; const void **dst; size_t cap; };
+#define UPC(field, src, n, capn) tabs.push_back(HostTab{(const void *)(src), (size_t)(n) * sizeof(*D.field), (const void **)&D.field, (size_t)(capn) * sizeof(*D.field)})
 #define UP(field, src, n) UPC(field, src, n, n)
+
+// Static tables (quotas, policies, topology), and the tree-local quota tables k_tl_static / k_tl_root derive from them
+static int32_t upload_static(kb_handle *h, const kb_snapshot *s, int n_rg_fl, int64_t *bytes) {
+  int32_t rc = build_static(h, s);
+  if (rc != KB_OK) return rc;
+  DevSnap &D = h->D;
+  const int Q = s->n_cq, N = Q + s->n_cohort, FR = s->n_flavor * s->n_resource;
+  const size_t NF = (size_t)N * FR;
+  std::vector<HostTab> tabs;
+  UP(parent, s->parent, N); UP(fair_weight, s->fair_weight, N);
+  UP(nominal, (const i64 *)s->nominal, NF); UP(blimit, (const i64 *)s->borrow_limit, NF); UP(llimit, (const i64 *)s->lend_limit, NF);
+  UP(cq_within_cq, s->cq_within_cq, Q); UP(cq_reclaim_within, s->cq_reclaim_within, Q); UP(cq_borrow_within, s->cq_borrow_within, Q);
+  UP(cq_has_bwc_threshold, s->cq_has_bwc_threshold, Q); UP(cq_bwc_threshold, s->cq_bwc_threshold, Q);
+  UP(cq_when_can_borrow, s->cq_when_can_borrow, Q); UP(cq_when_can_preempt, s->cq_when_can_preempt, Q);
+  UP(cq_preference, s->cq_preference, Q); UP(cq_strategy, s->cq_strategy, Q); UP(cq_generation, (const i64 *)s->cq_generation, Q);
+  UP(cq_rg_start, s->cq_rg_start, Q + 1); UP(rg_res_mask, s->rg_res_mask, s->n_rg); UP(rg_flavor_start, s->rg_flavor_start, s->n_rg + 1);
+  UP(rg_flavors, s->rg_flavors, n_rg_fl);
+  UP(root_slot, h->root_slot.data(), N); UP(depth, h->depth.data(), N); UP(height, h->height.data(), N);
+  UP(tree_start, h->tree_start.data(), D.nTrees + 1); UP(tree_nodes, h->tree_nodes.data(), h->tree_nodes.size());
+  UP(tree_level, h->tree_level.data(), h->tree_level.size()); UP(lone_cqs, h->lone.data(), h->lone.size());
+  UP(local_idx, h->local_idx.data(), N);
+  UP(tree_flat, h->tree_flat.data(), h->tree_flat.size());
+  UP(child_start, h->child_start.data(), N + 1); UP(child_list, h->child_list.data(), h->child_list.size());
+  UP(root_cq_start, h->root_cq_start.data(), h->root_cq_start.size());
+  UP(sn_node, h->sn_node.data(), h->sn_node.size()); UP(slot_base, h->slot_base.data(), h->slot_base.size());
+  UP(nd_tin, h->nd_tin.data(), h->nd_tin.size()); UP(nd_tout, h->nd_tout.data(), h->nd_tout.size());
+  UP(cq_path, h->cq_path.data(), h->cq_path.size()); UP(cq_plen, h->cq_plen.data(), h->cq_plen.size());
+  UP(tree_blob, h->tree_blob.data(), h->tree_blob.size()); UP(tree_blob_off, h->tree_blob_off.data(), h->tree_blob_off.size());
+  const size_t tl_cells = h->tree_nodes.size() * (size_t)FR;
+  const bool tree_local = tl_cells && tl_cells < (size_t)INT32_MAX;
+  i64 *tl[3] = {nullptr, nullptr, nullptr};  // subtree quota, borrowing limit, local quota
+  auto layout = [&](Arena &a) {
+    for (const HostTab &t : tabs) *t.dst = a.take<char>(t.bytes);
+    if (tree_local) for (i64 *&t : tl) t = a.take<i64>(tl_cells);
+  };
+  if (!h->sarena.carve(layout)) return fail(h, KB_ERR_CUDA, "cudaMalloc failed");
+  for (const HostTab &t : tabs) { CUDA_TRY(h, h2d(h, *t.dst, t.src, t.bytes)); *bytes += (int64_t)t.bytes; }
+  D.tl_subtree = D.tl_blimit = D.tl_lquota = nullptr; D.tl_usage = nullptr;
+  if (tree_local) {
+    D.FR = FR; D.Q = Q;
+    k_tl_static<<<(unsigned)((tl_cells + 255) / 256), 256, 0, h->stream>>>(D, tl[0], tl[1], tl[2], (int)tl_cells);
+    k_tl_root<<<(unsigned)(((size_t)D.nTrees * FR + 255) / 256), 256, 0, h->stream>>>(D, tl[0], tl[2]);
+    D.tl_subtree = tl[0]; D.tl_blimit = tl[1]; D.tl_lquota = tl[2];
+  }
+  D.path_stride = h->path_stride;
+  return KB_OK;
+}
+
+// Per-cycle input tables, enqueued before build_dynamic: the DMA runs while the host validates the tables and sizes
+// the scratch arena.  The caller's tables (dynamic part of kb_snapshot) usually sit close together in one pinned
+// block (kb_alloc_pinned carved by the shim): when their host span is not much larger than their total size the
+// whole span goes to the device with ONE DMA and the device tables alias into it at the same offsets; otherwise every
+// table is copied on its own.
+static int32_t upload_inputs(kb_handle *h, const kb_snapshot *s, bool reuse, int64_t *bytes) {
+  DevSnap &D = h->D;
+  const int Q = s->n_cq, R = s->n_resource, FR = s->n_flavor * R;
+  // A / AU are CAPACITIES (kb_run_drain grows the admitted tables on the device); A_in / AU_in what the caller passed
+  const size_t A_in = (size_t)s->n_adm, AU_in = (size_t)s->n_adm_use, A = A_in + h->drain_extra_adm, AUc = AU_in + h->drain_extra_au;
+  const size_t P = (size_t)s->n_podset, W = (size_t)s->n_wl, H = (size_t)s->n_heads;
+  std::vector<HostTab> tabs;
   // ClusterQueue usage: the full table with the other per-cycle tables | into the resident buffer (KB_F_USAGE_RESIDENT)
   // | the resident buffer patched with the caller's rows (usage_delta_*)
   const bool delta = s->usage_delta_cq != nullptr;
@@ -701,13 +688,13 @@ static int32_t upload_impl(kb_handle *h, const kb_snapshot *s, bool sync) {
       if (h->delta_seen[c] == h->delta_stamp) return fail(h, KB_ERR_INVALID, "usage_delta_cq lists a ClusterQueue twice");
       h->delta_seen[c] = h->delta_stamp;
     }
-    tabs.push_back(Tab{(const void *)s->usage_delta_cq, (size_t)s->n_usage_delta * 4, (const void **)&d_delta_cq, (size_t)s->n_usage_delta * 4});
-    tabs.push_back(Tab{(const void *)s->usage_delta_rows, (size_t)s->n_usage_delta * FR * 8, (const void **)&d_delta_rows, (size_t)s->n_usage_delta * FR * 8});
+    tabs.push_back(HostTab{(const void *)s->usage_delta_cq, (size_t)s->n_usage_delta * 4, (const void **)&d_delta_cq, (size_t)s->n_usage_delta * 4});
+    tabs.push_back(HostTab{(const void *)s->usage_delta_rows, (size_t)s->n_usage_delta * FR * 8, (const void **)&d_delta_rows, (size_t)s->n_usage_delta * FR * 8});
   } else if (keep_usage) {
     if (h->usage_res_cells != (size_t)Q * FR || !h->d_usage_res) {
       if (h->d_usage_res) cudaFree(h->d_usage_res);
       h->d_usage_res = nullptr; h->usage_res_cells = 0;
-      if (cudaMalloc((void **)&h->d_usage_res, std::max<size_t>(8, (size_t)Q * FR * 8)) != cudaSuccess) { cudaStreamSynchronize(h->stream); return fail(h, KB_ERR_CUDA, "cudaMalloc failed"); }
+      if (cudaMalloc((void **)&h->d_usage_res, std::max<size_t>(8, (size_t)Q * FR * 8)) != cudaSuccess) return fail(h, KB_ERR_CUDA, "cudaMalloc failed");
       h->usage_res_cells = (size_t)Q * FR;
     }
   } else {
@@ -726,39 +713,30 @@ static int32_t upload_impl(kb_handle *h, const kb_snapshot *s, bool sync) {
   if (s->ps_group) UP(ps_group, s->ps_group, P);
   if (s->wl_has_quota_reservation) UP(wl_has_qr, s->wl_has_quota_reservation, W);
   if (s->wl_sched_hash) UP(wl_sched_hash, (const i64 *)s->wl_sched_hash, W);
-  size_t caller_tabs = tabs.size();
-#undef UP
-#undef UPC
-  {
-    uintptr_t lo = UINTPTR_MAX, hi = 0; size_t sum = 0;
-    for (size_t i = 0; i < caller_tabs; i++) {
-      if (!tabs[i].bytes) continue;
-      if (!tabs[i].src) return fail(h, KB_ERR_INVALID, "null table with non-zero length");
-      if (tabs[i].cap != tabs[i].bytes) continue;  // growable table: its own allocation
-      lo = std::min(lo, (uintptr_t)tabs[i].src); hi = std::max(hi, (uintptr_t)tabs[i].src + tabs[i].bytes); sum += tabs[i].bytes;
-    }
-    uintptr_t lo_al = lo & ~(uintptr_t)255;
-    bool span = sum > 0 && (hi - lo) <= sum + sum / 4 + (64u << 10) && inside_one_pinned_block(lo_al, hi);
-    size_t itot = span ? pad256(hi - lo_al) : 0;
-    for (size_t i = 0; i < tabs.size(); i++) {
-      const Tab &t = tabs[i];
-      if (!(span && i < caller_tabs && t.bytes && t.cap == t.bytes)) itot += pad256(std::max(t.bytes, t.cap));
-    }
-    if (!h->iarena.reserve(itot + 4096)) return fail(h, KB_ERR_CUDA, "cudaMalloc failed");
-    h->iarena.reset();
-    CUDA_TRY(h, cudaEventRecord(h->ev0, h->stream));
-    char *dspan = span ? h->iarena.take<char>(hi - lo_al) : nullptr;
-    if (span) {
-      CUDA_TRY(h, cudaMemcpyAsync(dspan, (const void *)lo_al, hi - lo_al, cudaMemcpyHostToDevice, h->stream));
-      bytes += (int64_t)(hi - lo_al);
-    }
-    for (size_t i = 0; i < tabs.size(); i++) {
-      const Tab &t = tabs[i];
-      if (span && i < caller_tabs && t.bytes && t.cap == t.bytes) { *t.dst = dspan + ((uintptr_t)t.src - lo_al); continue; }
-      char *d = h->iarena.take<char>(std::max(t.bytes, t.cap));
-      *t.dst = d;
-      if (t.bytes) { CUDA_TRY(h, cudaMemcpyAsync(d, t.src, t.bytes, cudaMemcpyHostToDevice, h->stream)); bytes += (int64_t)t.bytes; }
-    }
+  uintptr_t lo = UINTPTR_MAX, hi = 0; size_t sum = 0;
+  for (const HostTab &t : tabs) {
+    if (!t.bytes) continue;
+    if (!t.src) return fail(h, KB_ERR_INVALID, "null table with non-zero length");
+    if (t.cap != t.bytes) continue;  // growable table: its own allocation
+    lo = std::min(lo, (uintptr_t)t.src); hi = std::max(hi, (uintptr_t)t.src + t.bytes); sum += t.bytes;
+  }
+  const uintptr_t lo_al = lo & ~(uintptr_t)255;
+  const bool span = sum > 0 && (hi - lo) <= sum + sum / 4 + (64u << 10) && inside_one_pinned_block(lo_al, hi);
+  auto in_span = [&](const HostTab &t) { return span && t.bytes && t.cap == t.bytes; };
+  char *dspan = nullptr;
+  auto layout = [&](Arena &a) {
+    if (span) dspan = a.take<char>(hi - lo_al);
+    for (const HostTab &t : tabs) if (!in_span(t)) *t.dst = a.take<char>(std::max(t.bytes, t.cap));
+  };
+  if (!h->iarena.carve(layout)) return fail(h, KB_ERR_CUDA, "cudaMalloc failed");
+  CUDA_TRY(h, cudaEventRecord(h->ev0, h->stream));
+  if (span) {
+    CUDA_TRY(h, cudaMemcpyAsync(dspan, (const void *)lo_al, hi - lo_al, cudaMemcpyHostToDevice, h->stream));
+    *bytes += (int64_t)(hi - lo_al);
+  }
+  for (const HostTab &t : tabs) {
+    if (in_span(t)) *t.dst = dspan + ((uintptr_t)t.src - lo_al);
+    else { CUDA_TRY(h, h2d(h, *t.dst, t.src, t.bytes)); *bytes += (int64_t)t.bytes; }
   }
   if (delta) {
     D.cq_usage = h->d_usage_res;
@@ -766,68 +744,46 @@ static int32_t upload_impl(kb_handle *h, const kb_snapshot *s, bool sync) {
     if (nd > 0) k_usage_patch<<<(unsigned)(((size_t)nd * FR + 255) / 256), 256, 0, h->stream>>>(h->d_usage_res, d_delta_cq, d_delta_rows, nd, FR);
   } else if (keep_usage) {
     if ((size_t)Q * FR) {
-      if (!s->cq_usage) { cudaStreamSynchronize(h->stream); return fail(h, KB_ERR_INVALID, "null table with non-zero length"); }
+      if (!s->cq_usage) return fail(h, KB_ERR_INVALID, "null table with non-zero length");
       CUDA_TRY(h, cudaMemcpyAsync(h->d_usage_res, s->cq_usage, (size_t)Q * FR * 8, cudaMemcpyHostToDevice, h->stream));
-      bytes += (int64_t)Q * FR * 8;
+      *bytes += (int64_t)Q * FR * 8;
     }
     D.cq_usage = h->d_usage_res;
     h->usage_res_valid = s->static_generation != 0; h->usage_res_gen = s->static_generation;
   }
   CUDA_TRY(h, cudaEventRecord(h->ev1, h->stream));
-  rc = build_dynamic(h, s);
-  if (rc != KB_OK) { cudaStreamSynchronize(h->stream); return rc; }  // the copies read the caller's buffers
-  D.tab_local = 0; D.gparent = D.parent; D.lq = nullptr; D.cq_entry = nullptr; D.ent_gid = nullptr; D.node_gid = nullptr; D.local_flat = 0; D.cq_rec = nullptr;
-  D.Q = Q; D.C = C; D.N = N; D.F = F; D.R = R; D.FR = FR; D.W = s->n_wl; D.P = s->n_podset; D.A = s->n_adm;
-  D.AU = s->n_adm_use; D.H = s->n_heads; D.NRG = s->n_rg; D.pods_res = s->pods_resource; D.flags = s->flags; D.now_ns = s->now_ns;
-  int nroots = D.nRoots;
-  // exact size of the per-cycle arena
-  size_t tot = 0;
-  auto need = [&](size_t n, size_t sz) { tot += pad256(n * sz); };
-  need((size_t)Q * FR, 8);
-  need(W, 4); need(W, 4); need(W, 8); need(W, 8); need(W, 8); need(W + 1, 4);
-  need(P * R, 8); need(P, 4); need(P, 4); need(P, 4); need(P, 8); need(P * R, 1);
-  need(A, 4); need(A, 4); need(A, 8); need(A, 8); need(A, 8); need(A, 1); need(A + 1, 4); need(AUc, 4); need(AUc, 8);
-  need(H, 4); need(W, 1); need(W, 8); need(P, 4); need(Q, 4); need(h->tree_nodes.size() + 1, 16); need(256, 1); need(h->tree_nodes.size() * (size_t)FR, 8);
-  need(Q + 1, 4); need(A, 4); need(A, 4); need(Q, 4); need(nroots, 4);
-  need(nroots + 2, 4); need(Q + 2, 4); need(A, 8); need(A, 8); need(A, 4); need(A, 4);
-  size_t rk_temp_bytes = 0;
-  if (A) {
-    size_t b1 = 0, b2 = 0;
-    cub::DoubleBuffer<u64> dk(nullptr, nullptr); cub::DoubleBuffer<int32_t> dv(nullptr, nullptr);
-    cub::DeviceRadixSort::SortPairs(nullptr, b1, dk, dv, (int)A, 0, 64, h->stream);
-    cub::DeviceRadixSort::SortPairs(nullptr, b2, (const u64 *)nullptr, (u64 *)nullptr, (const int32_t *)nullptr, (int32_t *)nullptr, (int)A, 0, 32, h->stream);
-    rk_temp_bytes = std::max(b1, b2) + 256;
-  }
-  need(rk_temp_bytes, 1);
-  need(NF, 8); need(NF, 8); need(NF, 8); need(NF, 8);
-  need(nroots, 4); need(nroots + 1, 4); need(nroots, 4); need(H, 4); need(H, 4); need(H, 4); need(H * 4, 8); need(H * 4, 8); need((size_t)Q * R, 8); need((size_t)N * R, 8);
-  need(H, 1); need(H, 1); need(H, 4); need(H, 4); need(P * R, 1); need(P * R, 1); need(P * R, 1); need(P, 4);
-  need(1, 4); need(N, 8); need(N, 4); need(N, 1);
-  // fair-sharing preemption: search kernel configuration (single-warp CTAs on a private copy of the whole tree)
-  bool fair = (s->flags & KB_F_FAIR_SHARING) != 0;
-  h->search_grid = 1; h->search_smem = true; h->search_smem_bytes = 0;
-  size_t fair_memo_items = 0;
-  if (fair && A) {
+  return KB_OK;
+}
+#undef UP
+#undef UPC
+
+// Launch configuration of the preemption-target searches of this upload (h->plan), and the scratch sizes they need.
+static void plan_search(kb_handle *h, const kb_snapshot *s) {
+  SearchPlan &p = h->plan;
+  const int R = s->n_resource, FR = s->n_flavor * R;
+  const size_t H = (size_t)s->n_heads, A = (size_t)s->n_adm + h->drain_extra_adm;
+  const bool fair = (s->flags & KB_F_FAIR_SHARING) != 0;
+  p.search_grid = 1; p.search_smem = true; p.search_smem_bytes = 0;
+  p.ws_warps = 1; p.ws_col_stride = 0; p.ws_list_total = 32;
+  p.memo_items = A ? std::min<size_t>(H, (64u << 20) / ((size_t)FR * sizeof(SimMemo))) : 0;
+  if (fair && A) {  // fair-sharing preemption: single-warp CTAs on a private copy of the whole tree
     // private tree tables [nodes][FR] x 4, parent links, per-node search state (16 B: queue head, cached share, flags)
     size_t tb = (size_t)h->max_tree_nodes * FR * 32 + (size_t)h->max_tree_nodes * 4 + (size_t)h->max_tree_nodes * 16 + 128;
-    h->search_smem = tb <= 190 * 1024;
-    h->search_smem_bytes = h->search_smem ? tb : 0;
+    p.search_smem = tb <= 190 * 1024;
+    p.search_smem_bytes = p.search_smem ? tb : 0;
     // resident single-warp CTAs per SM as the occupancy calculator sees them (registers / shared memory)
     int per_sm = 1;
-    if (h->search_smem) {
+    if (p.search_smem) {
       cudaFuncSetAttribute(k_nominate_search_fair<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_nominate_search_fair<true, true>, 32, h->search_smem_bytes);
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_nominate_search_fair<true, true>, 32, p.search_smem_bytes);
     } else {
       cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_nominate_search_fair<false, true>, 32, 0);
     }
     per_sm = std::max(1, std::min(per_sm, 16));
     // the oracle-cell pass has up to FR tasks per entry
-    h->search_grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)h->sm_count * per_sm, std::max<size_t>(1, H * (size_t)FR)));
-    fair_memo_items = std::min<size_t>(H, (64u << 20) / ((size_t)FR * sizeof(SimMemo)));
-  }
-  // warp-cooperative classical search: shared memory per warp = context + private column(s) + candidate codes
-  size_t ws_warps = 1, ws_col_stride = 0, memo_items = 0, ws_list_total = 32;
-  if (A && !fair) {
+    p.search_grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)h->sm_count * per_sm, std::max<size_t>(1, H * (size_t)FR)));
+  } else if (A) {
+    // warp-cooperative classical search: shared memory per warp = context + private column(s) + candidate codes
     const size_t kSmemBudget = 200 * 1024;
     size_t ncap_s = (size_t)h->max_tree_nodes;
     // k_search_cells: one column, codes of the longest bucket
@@ -837,19 +793,17 @@ static int32_t upload_impl(kb_handle *h, const kb_snapshot *s, bool sync) {
     size_t perA = ctxA + ((colA * 8 + 15) & ~(size_t)15) + ((codesA + 15) & ~(size_t)15);
     int wpbA = (int)std::max<size_t>(1, std::min<size_t>(16, kSmemBudget / perA));
     int bpsA = (int)std::max<size_t>(1, std::min<size_t>(32 / wpbA, (220 * 1024) / (perA * wpbA + 1024)));
-    h->sa_wpb = wpbA; h->sa_col_elems = (int)colA; h->sa_codes = (int)codesA; h->sa_smem = perA * wpbA;
-    h->sa_grid = std::max(1, std::min(h->sm_count * bpsA, (int)((H * (size_t)FR + 31) / 32)));
+    p.sa_wpb = wpbA; p.sa_col_elems = (int)colA; p.sa_codes = (int)codesA; p.sa_smem = perA * wpbA;
+    p.sa_grid = std::max(1, std::min(h->sm_count * bpsA, (int)((H * (size_t)FR + 31) / 32)));
     // grouped form: one column's statics + base usage shared by the CTA, private column + codes per warp
-    {
-      size_t shared_b = ((ncap_s * (sizeof(ColStat) + 8)) + 15) & ~(size_t)15;
-      size_t perG = ctxA + ((ncap_s * 8 + 15) & ~(size_t)15) + ((codesA + 15) & ~(size_t)15);
-      size_t budget = 220 * 1024;
-      int wpbG = shared_b + perG <= budget ? (int)std::min<size_t>(16, (budget - shared_b) / perG) : 0;
-      h->sg_on = wpbG >= 4;
-      h->sg_wpb = std::max(1, wpbG); h->sg_ncap = (int)ncap_s; h->sg_smem = shared_b + perG * h->sg_wpb;
-      h->sg_grid = h->sm_count;
-      if (h->sg_on) { wpbA = std::max(wpbA, wpbG); h->sa_grid = std::max(h->sa_grid, h->sg_grid); }
-    }
+    size_t shared_b = ((ncap_s * (sizeof(ColStat) + 8)) + 15) & ~(size_t)15;
+    size_t perG = ctxA + ((ncap_s * 8 + 15) & ~(size_t)15) + ((codesA + 15) & ~(size_t)15);
+    size_t budget = 220 * 1024;
+    int wpbG = shared_b + perG <= budget ? (int)std::min<size_t>(16, (budget - shared_b) / perG) : 0;
+    p.sg_on = wpbG >= 4;
+    p.sg_wpb = std::max(1, wpbG); p.sg_ncap = (int)ncap_s; p.sg_smem = shared_b + perG * p.sg_wpb;
+    p.sg_grid = h->sm_count;
+    if (p.sg_on) { wpbA = std::max(wpbA, wpbG); p.sa_grid = std::max(p.sa_grid, p.sg_grid); }
     // k_nominate_walk: up to Kcap columns (cells of one workload's assignment)
     size_t kcap = std::min<size_t>(std::min<size_t>((size_t)FR, KB_MAX_CELLS), (size_t)h->max_head_podsets * R);
     size_t ctxB = (sizeof(WCtx<KB_MAX_CELLS>) + 15) & ~(size_t)15;
@@ -859,127 +813,131 @@ static int32_t upload_impl(kb_handle *h, const kb_snapshot *s, bool sync) {
     size_t perB = ctxB;
     int wpbB = 8;
     int bpsB = 2;
-    h->sb_wpb = wpbB; h->sb_col_elems = (int)colB; h->sb_smem = perB * wpbB;
-    h->sb_grid = std::max(1, std::min(h->sm_count * bpsB, (int)((H + wpbB - 1) / wpbB)));
-    ws_warps = std::max((size_t)h->sa_grid * wpbA, (size_t)h->sb_grid * wpbB);
+    p.sb_wpb = wpbB; p.sb_col_elems = (int)colB; p.sb_smem = perB * wpbB;
+    p.sb_grid = std::max(1, std::min(h->sm_count * bpsB, (int)((H + wpbB - 1) / wpbB)));
+    p.ws_warps = std::max((size_t)p.sa_grid * wpbA, (size_t)p.sb_grid * wpbB);
     // per-warp candidate-code / target scratch: a single-cell search sees one bucket, GetTargets at most the root's list
-    h->sa_list_cap = (int)(((size_t)h->max_frl_len + 31) & ~(size_t)31);
-    h->sb_list_cap = (int)(((size_t)h->max_root_adm + 31) & ~(size_t)31);
-    ws_list_total = std::max((size_t)h->sa_grid * wpbA * h->sa_list_cap, (size_t)h->sb_grid * wpbB * h->sb_list_cap);
-    if (colA == 0) ws_col_stride = ncap_s;
-    if (kcap * ncap_s > colB) ws_col_stride = std::max(ws_col_stride, std::min<size_t>((size_t)FR, KB_MAX_CELLS) * ncap_s);
-    memo_items = std::min<size_t>(H, (64u << 20) / ((size_t)FR * sizeof(SimMemo)));
+    p.sa_list_cap = (int)(((size_t)h->max_frl_len + 31) & ~(size_t)31);
+    p.sb_list_cap = (int)(((size_t)h->max_root_adm + 31) & ~(size_t)31);
+    p.ws_list_total = std::max((size_t)p.sa_grid * wpbA * p.sa_list_cap, (size_t)p.sb_grid * wpbB * p.sb_list_cap);
+    if (colA == 0) p.ws_col_stride = ncap_s;
+    if (kcap * ncap_s > colB) p.ws_col_stride = std::max(p.ws_col_stride, std::min<size_t>((size_t)FR, KB_MAX_CELLS) * ncap_s);
   }
-  if (fair && A) memo_items = fair_memo_items;
-  size_t G = (fair && A) ? (size_t)h->search_grid : 1, acap = (fair && A) ? (size_t)h->max_root_adm : 1, ncap = (size_t)h->max_tree_nodes;
-  size_t pool_cap = A * 4 + 1024;
-  need(A, 4); need(nroots + 1, 4); need(H, 4); need(2, 4); need(H, 4); need(H, 4); need(pool_cap, 4); need(pool_cap, 1); need(1, 4);
-  need(H + 1, 4); need(pool_cap, 4); need(pool_cap, 1);  // preemption targets in CSR order (download)
-  need(A, 1); need(A, 4); need(nroots, 4); need(A ? NF : 1, 8);
-  need(G * acap, 4); need(G * acap, 4); need(G * acap, 4); need(G * acap, 4); need(G * ncap, 4); need(G * acap, 1); need(G * acap, 1); need(G * ncap, 1); need(G * ncap, 1); need(G * ncap, 1); need(G * ncap, 8); need(G * ncap, 1);
-  if (fair && A && !h->search_smem) need(G * ncap * FR, 8);
-  // classical search tables + per-warp scratch
-  const size_t nbuckets = (size_t)nroots * FR;
-  const size_t sNF = A ? NF : 1, sAU = A ? AUc : 1;
-  need(A, 4); need(sNF, 8); need(sNF, sizeof(ColStat)); need(sNF, 4); need(A ? nbuckets + 1 : 1, 4); need(A ? nbuckets + 2 : 1, 4); need(sAU, sizeof(FrRec)); need(A, sizeof(FrRec));
-  need(memo_items * FR, sizeof(SimMemo)); need(1, 4); need(8, 8);
-  need(A ? nbuckets + 2 : 1, 4); need(A ? nbuckets + 2 : 1, 4); need(A ? nbuckets + 2 : 1, 4); need(memo_items * FR, 4); need(memo_items * FR, 4);
-  need(ws_warps * ws_col_stride, 8); need(ws_list_total, 1); need(ws_list_total, 4); need(ws_list_total, 1); need(ws_warps * (size_t)h->sa_list_cap, 8);
-  if (fair) { need(H * FR, 8); need(H * (48 + 16 * KB_MAX_DEPTH), 1); need(N, 4); need(N, 4); }
-  if (!h->arena.reserve(tot + (1u << 20))) { cudaStreamSynchronize(h->stream); return fail(h, KB_ERR_CUDA, "cudaMalloc failed"); }
-  h->arena.reset();
-  if (h->drain_mode) D.heads = h->arena.take<int32_t>(H);
-  h->d_cq_entry = h->arena.take<int32_t>(Q); D.cq_entry = h->d_cq_entry;
-  {  // fused per-root cycle (k_cycle_root): see the kernel's header for the conditions
-    bool all_flat = true;
-    for (uint8_t f : h->tree_flat) if (!f) all_flat = false;
-    size_t nnm = (size_t)h->max_tree_nodes, tbm = nnm * FR;
-    size_t sm = 6 * tbm * 8 + 2 * nnm * R * 8 + 4 * nnm * 4 + 7 * KB_TILE * 4 + (KB_MAX_DEPTH + 2 + 4) * 4 + 32 + nnm * 32;
-    h->fused_smem = sm;
-    h->fused_on = D.nLone == 0 && D.nTrees > 0 && h->one_head_per_cq && sm <= 220 * 1024 && ((A_in == 0 && !h->drain_events) || !h->preempt_possible) &&
-                  (!(s->flags & KB_F_FAIR_SHARING) || all_flat) && getenv("KB_NO_FUSED") == nullptr;
-    // k_cycle_flat: every tree flat, FR <= 64, the relocated copy of the largest root fits shared memory
-    h->d_cq_rec = h->arena.take<int4>(h->tree_nodes.size() + 1); D.cq_rec = h->d_cq_rec;
-    D.tl_usage = D.tl_subtree ? h->arena.take<i64>(h->tree_nodes.size() * (size_t)FR) : nullptr;
-    h->flat_rcap = (int)std::min<size_t>((size_t)1 << 20, nnm * (size_t)std::max(1, h->max_head_podsets));
-    h->flat_smem = flat_layout((int)nnm, FR, R, h->flat_rcap, h->max_blob_bytes).total;
-    if (h->flat_static_smem == 0) { cudaFuncAttributes fa{}; cudaFuncGetAttributes(&fa, k_cycle_flat); h->flat_static_smem = std::max<size_t>(16, fa.sharedSizeBytes); }
-    h->flat_on = h->fused_on && all_flat && FR <= 64 && h->flat_smem + h->flat_static_smem <= 227 * 1024 && getenv("KB_FUSED_V1") == nullptr;
-    h->flat_on = h->flat_on && h->max_head_podsets < KB_REC_GENERAL && D.tl_subtree != nullptr;  // head record; staged from the tree-local tables only
-    if (h->fused_on && !h->flat_on && !h->drain_mode) {
-      CUDA_TRY(h, cudaMemsetAsync(h->d_cq_entry, 0xff, sizeof(int32_t) * (size_t)Q, h->stream));
-      if (H) k_cq_entry<<<(unsigned)((H + 255) / 256), 256, 0, h->stream>>>(D, h->d_cq_entry);
+  p.G = (fair && A) ? (size_t)p.search_grid : 1, p.acap = (fair && A) ? (size_t)h->max_root_adm : 1, p.ncap = (size_t)h->max_tree_nodes;
+}
+
+// Fused per-root cycle (k_cycle_root), and its k_cycle_flat form: see the kernels' headers for the conditions
+static void choose_route(kb_handle *h, const kb_snapshot *s) {
+  const DevSnap &D = h->D;
+  const int R = s->n_resource, FR = s->n_flavor * R;
+  bool all_flat = true;
+  for (uint8_t f : h->tree_flat) if (!f) all_flat = false;
+  size_t nnm = (size_t)h->max_tree_nodes, tbm = nnm * FR;
+  h->fused_smem = 6 * tbm * 8 + 2 * nnm * R * 8 + 4 * nnm * 4 + 7 * KB_TILE * 4 + (KB_MAX_DEPTH + 2 + 4) * 4 + 32 + nnm * 32;
+  h->fused_on = D.nLone == 0 && D.nTrees > 0 && h->one_head_per_cq && h->fused_smem <= 220 * 1024 &&
+                ((s->n_adm == 0 && !h->drain_events) || !h->preempt_possible) && (!(s->flags & KB_F_FAIR_SHARING) || all_flat) &&
+                getenv("KB_NO_FUSED") == nullptr;
+  // k_cycle_flat: every tree flat, FR <= 64, the relocated copy of the largest root fits shared memory
+  h->flat_rcap = (int)std::min<size_t>((size_t)1 << 20, nnm * (size_t)std::max(1, h->max_head_podsets));
+  h->flat_smem = flat_layout((int)nnm, FR, R, h->flat_rcap, h->max_blob_bytes).total;
+  if (h->flat_static_smem == 0) { cudaFuncAttributes fa{}; cudaFuncGetAttributes(&fa, k_cycle_flat); h->flat_static_smem = std::max<size_t>(16, fa.sharedSizeBytes); }
+  h->flat_on = h->fused_on && all_flat && FR <= 64 && h->flat_smem + h->flat_static_smem <= 227 * 1024 && getenv("KB_FUSED_V1") == nullptr;
+  h->flat_on = h->flat_on && h->max_head_podsets < KB_REC_GENERAL && D.tl_subtree != nullptr;  // head record; staged from the tree-local tables only
+}
+
+// Per-cycle scratch and result block, described once (Arena::carve), and the clears and launches that prepare them
+static int32_t carve_scratch(kb_handle *h, const kb_snapshot *s) {
+  DevSnap &D = h->D;
+  const SearchPlan &p = h->plan;
+  const int Q = s->n_cq, N = Q + s->n_cohort, R = s->n_resource, FR = s->n_flavor * R, nroots = D.nRoots;
+  const size_t NF = (size_t)N * FR, P = (size_t)s->n_podset, H = (size_t)s->n_heads;
+  const size_t A = (size_t)s->n_adm + h->drain_extra_adm, AUc = (size_t)s->n_adm_use + h->drain_extra_au;
+  const bool fair = (s->flags & KB_F_FAIR_SHARING) != 0;
+  h->rk_temp_bytes = 0;
+  if (A) {
+    size_t b1 = 0, b2 = 0;
+    cub::DoubleBuffer<u64> dk(nullptr, nullptr); cub::DoubleBuffer<int32_t> dv(nullptr, nullptr);
+    cub::DeviceRadixSort::SortPairs(nullptr, b1, dk, dv, (int)A, 0, 64, h->stream);
+    cub::DeviceRadixSort::SortPairs(nullptr, b2, (const u64 *)nullptr, (u64 *)nullptr, (const int32_t *)nullptr, (int32_t *)nullptr, (int)A, 0, 32, h->stream);
+    h->rk_temp_bytes = std::max(b1, b2) + 256;
+  }
+  const size_t G = p.G, acap = p.acap, ncap = p.ncap, pool_cap = A * 4 + 1024;
+  const size_t nbuckets = (size_t)nroots * FR, sNF = A ? NF : 1, sAU = A ? AUc : 1, tl_cells = h->tree_nodes.size() * (size_t)FR;
+  const OutLayout L = out_layout(H, P, (size_t)R);
+  auto layout = [&](Arena &a) {
+    if (h->drain_mode) D.heads = a.take<int32_t>(H);
+    D.cq_entry = h->d_cq_entry = a.take<int32_t>(Q);
+    D.cq_rec = h->d_cq_rec = a.take<int4>(h->tree_nodes.size() + 1);
+    D.tl_usage = D.tl_subtree ? a.take<i64>(tl_cells) : nullptr;
+    D.over_list = a.take<int32_t>(Q); D.over_count = a.take<int32_t>(nroots);
+    D.root_adm_start = a.take<int32_t>(nroots + 1); D.cq_adm_start = a.take<int32_t>(Q + 1);
+    D.cq_adm = a.take<int32_t>(A); D.adm_rank = a.take<int32_t>(A);
+    D.root_adm_count = a.take<int32_t>(nroots + 2); D.cq_adm_count = a.take<int32_t>(Q + 2);
+    h->rk_keys[0] = a.take<u64>(A); h->rk_keys[1] = a.take<u64>(A);
+    D.adm_sorted = h->rk_vals[0] = a.take<int32_t>(A); h->rk_vals[1] = a.take<int32_t>(A);
+    h->rk_temp = a.take<char>(h->rk_temp_bytes);
+    D.subtree = a.take<i64>(NF); D.usage = a.take<i64>(NF);
+    D.avail = a.take<i64>(NF); D.potential = a.take<i64>(NF);
+    D.root_count = a.take<int32_t>(nroots); D.root_offset = a.take<int32_t>(nroots + 1);
+    D.root_cursor = a.take<int32_t>(nroots); D.root_entries = a.take<int32_t>(H);
+    D.sorted = a.take<int32_t>(H); D.pos_slot = a.take<int32_t>(H); D.ekey = a.take<u64>(H * 4); D.skey = a.take<u64>(H * 4);
+    D.fs_over = a.take<i64>((size_t)Q * R); D.fs_lend = a.take<i64>((size_t)N * R);
+    h->d_out_block = a.take<char>(L.prefix);  // the result tables and the cycle header in the canonical layout (out_layout)
+    D.ps_list = a.take<int32_t>(H);
+    D.tgt_off = a.take<int32_t>(H); D.tgt_cnt = a.take<int32_t>(H);
+    D.tgt_pool_adm = a.take<int32_t>(pool_cap); D.tgt_pool_reason = a.take<uint8_t>(pool_cap);
+    h->d_tgt_start = a.take<int32_t>(H + 1); h->d_tgt_adm = a.take<int32_t>(pool_cap); h->d_tgt_reason = a.take<uint8_t>(pool_cap);
+    D.preempted = a.take<uint8_t>(A);
+    D.usage_shadow = a.take<i64>(A ? NF : 1);
+    D.sc_cand = a.take<int32_t>(G * acap); D.sc_tgt = a.take<int32_t>(G * acap); D.sc_cq_lca = a.take<int32_t>(G * ncap);
+    D.sc_aux1 = a.take<int32_t>(G * acap); D.sc_aux2 = a.take<int32_t>(G * acap);
+    D.sc_variant = a.take<uint8_t>(G * acap); D.sc_tgt_reason = a.take<uint8_t>(G * acap);
+    D.sc_cq_class = a.take<int8_t>(G * ncap); D.sc_on_path = a.take<int8_t>(G * ncap);
+    D.sc_dirty = a.take<uint8_t>(G * ncap); D.sc_drs_ratio = a.take<double>(G * ncap); D.sc_drs_meta = a.take<int8_t>(G * ncap);
+    D.sc_usage = (fair && A && !p.search_smem) ? a.take<i64>(G * ncap * FR) : nullptr;
+    D.colU = a.take<i64>(sNF); D.colS = a.take<ColStat>(sNF); D.ovm = a.take<uint32_t>(sNF);
+    D.frl_count = a.take<int32_t>(A ? nbuckets + 1 : 1); D.frl_start = a.take<int32_t>(A ? nbuckets + 2 : 1);
+    D.frl = a.take<FrRec>(sAU); D.rrec = a.take<FrRec>(A);
+    D.memo = a.take<SimMemo>(p.memo_items * FR);
+    D.cell_cursor = a.take<int32_t>(1);
+    D.cell_count = a.take<int32_t>(A ? nbuckets + 2 : 1); D.cell_start = a.take<int32_t>(A ? nbuckets + 2 : 1);
+    D.cell_fill = a.take<int32_t>(A ? nbuckets + 2 : 1);
+    D.cell_list = a.take<int32_t>(p.memo_items * FR); D.cell_bucket = a.take<int32_t>(p.memo_items * FR);
+    D.ws_col = a.take<i64>(p.ws_warps * p.ws_col_stride);
+    D.ws_codes = a.take<uint8_t>(p.ws_list_total); D.ws_tgt = a.take<int32_t>(p.ws_list_total);
+    D.ws_tgt_reason = a.take<uint8_t>(p.ws_list_total);
+    D.ws_tgtq = a.take<i64>(p.ws_warps * (size_t)p.sa_list_cap);
+    if (fair) {
+      D.q_scratch = a.take<i64>(H * FR); D.fs_state = a.take<unsigned char>(H * (48 + 16 * KB_MAX_DEPTH));
+      D.fs_cq_entry = a.take<int32_t>(N); D.fs_winner = a.take<int32_t>(N);
     }
+    h->d_drs_rounded = a.take<i64>(N); h->d_drs_res = a.take<int32_t>(N); h->d_drs_borrowing = a.take<uint8_t>(N);
+  };
+  if (!h->arena.carve(layout)) return fail(h, KB_ERR_CUDA, "cudaMalloc failed");
+  char *ob = h->d_out_block;
+  D.decision = (uint8_t *)(ob + L.off[0]); D.mode = (uint8_t *)(ob + L.off[1]);
+  D.borrow = (int32_t *)(ob + L.off[2]); D.rank = (int32_t *)(ob + L.off[3]);
+  D.ps_flavor = (int8_t *)(ob + L.off[4]); D.ps_res_mode = (int8_t *)(ob + L.off[5]); D.ps_tried = (int8_t *)(ob + L.off[6]);
+  D.ps_count_out = (int32_t *)(ob + L.off[7]);
+  // cycle header, cleared once per cycle: [0] status, [2..3] ps_n / ps_cursor, [4] target pool cursor, [8..23] search counters
+  uint32_t *hdr = (uint32_t *)(ob + L.hdr);
+  D.status = hdr; D.ps_n = (int32_t *)(hdr + 2); D.ps_cursor = D.ps_n + 1; D.tgt_pool_used = (int32_t *)(hdr + 4); D.sstat = (u64 *)(hdr + 8);
+  D.tgt_pool_cap = (int)pool_cap; D.sc_adm_cap = (int)acap; D.sc_node_cap = (int)ncap;
+  D.memo_items = (int)p.memo_items; D.ws_col_stride = p.ws_col_stride; D.ws_tgtq_cap = p.sa_list_cap;
+  if (h->fused_on && !h->flat_on && !h->drain_mode) {
+    CUDA_TRY(h, cudaMemsetAsync(h->d_cq_entry, 0xff, sizeof(int32_t) * (size_t)Q, h->stream));
+    if (H) k_cq_entry<<<(unsigned)((H + 255) / 256), 256, 0, h->stream>>>(D, h->d_cq_entry);
   }
-  D.over_list = h->arena.take<int32_t>(Q); D.over_count = h->arena.take<int32_t>(nroots);
-  D.root_adm_start = h->arena.take<int32_t>(nroots + 1); D.cq_adm_start = h->arena.take<int32_t>(Q + 1);
-  D.cq_adm = h->arena.take<int32_t>(A); D.adm_rank = h->arena.take<int32_t>(A);
-  D.root_adm_count = h->arena.take<int32_t>(nroots + 2); D.cq_adm_count = h->arena.take<int32_t>(Q + 2);
-  h->rk_keys[0] = h->arena.take<u64>(A); h->rk_keys[1] = h->arena.take<u64>(A);
-  h->rk_vals[0] = h->arena.take<int32_t>(A); h->rk_vals[1] = h->arena.take<int32_t>(A);
-  h->rk_temp = h->arena.take<char>(rk_temp_bytes); h->rk_temp_bytes = rk_temp_bytes;
-  D.adm_sorted = h->rk_vals[0];
   if (!A) {  // candidates_possible() reads the (empty) group tables
     CUDA_TRY(h, cudaMemsetAsync(D.root_adm_start, 0, sizeof(int32_t) * (size_t)(nroots + 1), h->stream));
     CUDA_TRY(h, cudaMemsetAsync(D.cq_adm_start, 0, sizeof(int32_t) * (size_t)(Q + 1), h->stream));
   }
-  D.subtree = h->arena.take<i64>(NF); D.usage = h->arena.take<i64>(NF);
-  D.avail = h->arena.take<i64>(NF); D.potential = h->arena.take<i64>(NF);
-  D.root_count = h->arena.take<int32_t>(nroots); D.root_offset = h->arena.take<int32_t>(nroots + 1);
-  D.root_cursor = h->arena.take<int32_t>(nroots); D.root_entries = h->arena.take<int32_t>(H);
-  D.sorted = h->arena.take<int32_t>(H); D.pos_slot = h->arena.take<int32_t>(H); D.ekey = h->arena.take<u64>(H * 4); D.skey = h->arena.take<u64>(H * 4);
-  D.fs_over = h->arena.take<i64>((size_t)Q * R); D.fs_lend = h->arena.take<i64>((size_t)N * R);
-  {  // the result tables in the canonical layout (out_layout)
-    OutLayout L = out_layout(H, P, (size_t)R);
-    char *ob = h->arena.take<char>(L.prefix);
-    h->d_out_block = ob;
-    D.decision = (uint8_t *)(ob + L.off[0]); D.mode = (uint8_t *)(ob + L.off[1]);
-    D.borrow = (int32_t *)(ob + L.off[2]); D.rank = (int32_t *)(ob + L.off[3]);
-    D.ps_flavor = (int8_t *)(ob + L.off[4]); D.ps_res_mode = (int8_t *)(ob + L.off[5]); D.ps_tried = (int8_t *)(ob + L.off[6]);
-    D.ps_count_out = (int32_t *)(ob + L.off[7]);
-  }
-  {  // cycle header block, cleared once per cycle: [0] status, [2..3] ps_n / ps_cursor, [4] target pool cursor, [8..23] search counters
-    uint32_t *hdr = (uint32_t *)(h->d_out_block + out_layout(H, P, (size_t)R).hdr);
-    D.status = hdr; D.ps_n = (int32_t *)(hdr + 2); D.ps_cursor = D.ps_n + 1; D.tgt_pool_used = (int32_t *)(hdr + 4); D.sstat = (u64 *)(hdr + 8);
-  }
-  D.ps_list = h->arena.take<int32_t>(H);
-  D.tgt_off = h->arena.take<int32_t>(H); D.tgt_cnt = h->arena.take<int32_t>(H);
-  D.tgt_pool_adm = h->arena.take<int32_t>(pool_cap); D.tgt_pool_reason = h->arena.take<uint8_t>(pool_cap);
-  D.tgt_pool_cap = (int)pool_cap;
-  h->d_tgt_start = h->arena.take<int32_t>(H + 1); h->d_tgt_adm = h->arena.take<int32_t>(pool_cap); h->d_tgt_reason = h->arena.take<uint8_t>(pool_cap);
-  D.preempted = h->arena.take<uint8_t>(A);
-  D.usage_shadow = h->arena.take<i64>(A ? NF : 1);
-  D.sc_cand = h->arena.take<int32_t>(G * acap); D.sc_tgt = h->arena.take<int32_t>(G * acap); D.sc_cq_lca = h->arena.take<int32_t>(G * ncap);
-  D.sc_aux1 = h->arena.take<int32_t>(G * acap); D.sc_aux2 = h->arena.take<int32_t>(G * acap);
-  D.sc_variant = h->arena.take<uint8_t>(G * acap); D.sc_tgt_reason = h->arena.take<uint8_t>(G * acap);
-  D.sc_cq_class = h->arena.take<int8_t>(G * ncap); D.sc_on_path = h->arena.take<int8_t>(G * ncap);
-  D.sc_dirty = h->arena.take<uint8_t>(G * ncap); D.sc_drs_ratio = h->arena.take<double>(G * ncap); D.sc_drs_meta = h->arena.take<int8_t>(G * ncap);
-  D.sc_usage = (fair && A && !h->search_smem) ? h->arena.take<i64>(G * ncap * FR) : nullptr;
-  D.sc_adm_cap = (int)acap; D.sc_node_cap = (int)ncap;
-  D.colU = h->arena.take<i64>(sNF); D.colS = h->arena.take<ColStat>(sNF); D.ovm = h->arena.take<uint32_t>(sNF);
-  D.frl_count = h->arena.take<int32_t>(A ? nbuckets + 1 : 1); D.frl_start = h->arena.take<int32_t>(A ? nbuckets + 2 : 1);
-  D.frl = h->arena.take<FrRec>(sAU); D.rrec = h->arena.take<FrRec>(A);
-  D.memo = h->arena.take<SimMemo>(memo_items * FR); D.memo_items = (int)memo_items;
-  D.cell_cursor = h->arena.take<int32_t>(1);
-  D.cell_count = h->arena.take<int32_t>(A ? nbuckets + 2 : 1); D.cell_start = h->arena.take<int32_t>(A ? nbuckets + 2 : 1);
-  D.cell_fill = h->arena.take<int32_t>(A ? nbuckets + 2 : 1);
-  D.cell_list = h->arena.take<int32_t>(memo_items * FR); D.cell_bucket = h->arena.take<int32_t>(memo_items * FR);
-  D.ws_col = h->arena.take<i64>(ws_warps * ws_col_stride); D.ws_col_stride = ws_col_stride;
-  D.ws_codes = h->arena.take<uint8_t>(ws_list_total); D.ws_tgt = h->arena.take<int32_t>(ws_list_total);
-  D.ws_tgt_reason = h->arena.take<uint8_t>(ws_list_total);
-  D.ws_tgtq = h->arena.take<i64>(ws_warps * (size_t)h->sa_list_cap); D.ws_tgtq_cap = h->sa_list_cap;
-  if (fair) {
-    D.q_scratch = h->arena.take<i64>(H * FR); D.fs_state = h->arena.take<unsigned char>(H * (48 + 16 * KB_MAX_DEPTH));
-    D.fs_cq_entry = h->arena.take<int32_t>(N); D.fs_winner = h->arena.take<int32_t>(N);
-  }
-  h->d_drs_rounded = h->arena.take<i64>(N); h->d_drs_res = h->arena.take<int32_t>(N); h->d_drs_borrowing = h->arena.take<uint8_t>(N);
-  if (h->arena.used > h->arena.cap) { cudaStreamSynchronize(h->stream); return fail(h, KB_ERR_CUDA, "device arena accounting"); }
   h->hdr_clean = false;
   if (h->flat_on && !h->drain_mode) {  // head records + result-row fills + cleared header: one launch (k_flat_prep)
-    int32_t rc2 = flat_rec_stamp(h);
-    if (rc2 != KB_OK) return rc2;
+    int32_t rc = flat_rec_stamp(h);
+    if (rc != KB_OK) return rc;
     const size_t fill_words = 3 * pad256(P * R) / 4;
-    const size_t tlc = D.tl_usage ? h->tree_nodes.size() * (size_t)FR : 0;
+    const size_t tlc = D.tl_usage ? tl_cells : 0;
     const size_t nthr = std::max(std::max(std::max(H, fill_words), std::max(P, (size_t)32)), tlc);
     k_flat_prep<<<(unsigned)((nthr + 255) / 256), 256, 0, h->stream>>>(D, h->d_cq_rec, (int)fill_words, (int)P, (int)tlc);
     h->hdr_clean = true;
@@ -988,6 +946,39 @@ static int32_t upload_impl(kb_handle *h, const kb_snapshot *s, bool sync) {
     CUDA_TRY(h, cudaMemsetAsync(D.ps_flavor, 0xff, 3 * pad256(P * R), h->stream));  // flavor, res_mode, tried are adjacent (out_layout)
     CUDA_TRY(h, cudaMemsetAsync(D.ps_count_out, 0, P * 4, h->stream));
   }
+  return KB_OK;
+}
+
+// The failure paths past the first copy synchronise the stream before they return: the copies read the caller's
+// buffers, which the caller may release once the call returns.
+static int32_t upload_impl(kb_handle *h, const kb_snapshot *s, bool sync) {
+  if (!h || !s) return KB_ERR_INVALID;
+  cudaSetDevice(h->device);
+  h->uploaded = false;
+  DevSnap &D = h->D;
+  const int Q = s->n_cq, C = s->n_cohort, F = s->n_flavor, R = s->n_resource;
+  const int n_rg_fl = (s->n_rg > 0 && s->rg_flavor_start) ? s->rg_flavor_start[s->n_rg] : 0;
+  const int dims[6] = {Q, C, F, R, s->n_rg, n_rg_fl};
+  const bool reuse = s->static_generation != 0 && s->static_generation == h->static_gen && memcmp(dims, h->s_dims, sizeof(dims)) == 0;
+  auto refuse = [h](int32_t rc) { cudaStreamSynchronize(h->stream); return rc; };
+  int64_t bytes = 0;
+  if (!reuse) {
+    h->static_gen = 0;
+    const int32_t rc = upload_static(h, s, n_rg_fl, &bytes);
+    if (rc != KB_OK) return refuse(rc);
+    memcpy(h->s_dims, dims, sizeof(dims));
+    h->static_gen = s->static_generation;
+  }
+  int32_t rc = upload_inputs(h, s, reuse, &bytes);
+  if (rc == KB_OK) rc = build_dynamic(h, s);
+  if (rc != KB_OK) return refuse(rc);
+  D.tab_local = 0; D.gparent = D.parent; D.lq = nullptr; D.cq_entry = nullptr; D.ent_gid = nullptr; D.node_gid = nullptr; D.local_flat = 0; D.cq_rec = nullptr;
+  D.Q = Q; D.C = C; D.N = Q + C; D.F = F; D.R = R; D.FR = F * R; D.W = s->n_wl; D.P = s->n_podset; D.A = s->n_adm;
+  D.AU = s->n_adm_use; D.H = s->n_heads; D.NRG = s->n_rg; D.pods_res = s->pods_resource; D.flags = s->flags; D.now_ns = s->now_ns;
+  plan_search(h, s);
+  choose_route(h, s);
+  rc = carve_scratch(h, s);
+  if (rc != KB_OK) return refuse(rc);
   h->stats.h2d_bytes = bytes;
   h->uploaded = true;
   if (sync) {  // caller buffers may be released after return
@@ -1153,19 +1144,20 @@ static int32_t cycle_enqueue(kb_handle *h, bool hdr_copy = true) {
     else k_nominate<<<(D.H + 127) / 128, 128, 0, h->stream>>>(D);
     launches++;
     if (D.A) {  // target search for the entries k_nominate deferred
+      const SearchPlan &p = h->plan;
       if (D.flags & KB_F_FAIR_SHARING) {
         kmark(h, KB_K_PREEMPT);
         CUDA_TRY(h, cudaMemsetAsync(D.over_count, 0, sizeof(int32_t) * (size_t)std::max(1, D.nRoots), h->stream));
         k_over<<<(D.Q + 255) / 256, 256, 0, h->stream>>>(D); launches++;
         CUDA_TRY(h, cudaMemsetAsync(D.cell_cursor, 0, 4, h->stream));
-        if (h->search_smem) {
+        if (p.search_smem) {
           CUDA_TRY(h, cudaFuncSetAttribute(k_nominate_search_fair<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
           CUDA_TRY(h, cudaFuncSetAttribute(k_nominate_search_fair<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-          if (D.memo_items) { k_nominate_search_fair<true, true><<<h->search_grid, 32, h->search_smem_bytes, h->stream>>>(D); launches++; }
-          k_nominate_search_fair<true, false><<<h->search_grid, 32, h->search_smem_bytes, h->stream>>>(D);
+          if (D.memo_items) { k_nominate_search_fair<true, true><<<p.search_grid, 32, p.search_smem_bytes, h->stream>>>(D); launches++; }
+          k_nominate_search_fair<true, false><<<p.search_grid, 32, p.search_smem_bytes, h->stream>>>(D);
         } else {
-          if (D.memo_items) { k_nominate_search_fair<false, true><<<h->search_grid, 32, 0, h->stream>>>(D); launches++; }
-          k_nominate_search_fair<false, false><<<h->search_grid, 32, 0, h->stream>>>(D);
+          if (D.memo_items) { k_nominate_search_fair<false, true><<<p.search_grid, 32, 0, h->stream>>>(D); launches++; }
+          k_nominate_search_fair<false, false><<<p.search_grid, 32, 0, h->stream>>>(D);
         }
         launches++;
       } else {
@@ -1183,7 +1175,7 @@ static int32_t cycle_enqueue(kb_handle *h, bool hdr_copy = true) {
         CUDA_TRY(h, cudaFuncSetAttribute(k_search_cells, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
         CUDA_TRY(h, cudaFuncSetAttribute(k_nominate_walk, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
         kmark(h, KB_K_SEARCH_CELLS);
-        if (h->sg_on && D.memo_items) {
+        if (p.sg_on && D.memo_items) {
           long long ncell = (long long)D.memo_items * D.FR;
           CUDA_TRY(h, cudaMemsetAsync(D.cell_count, 0, sizeof(int32_t) * (size_t)(nb + 1), h->stream));
           CUDA_TRY(h, cudaMemsetAsync(D.cell_fill, 0, sizeof(int32_t) * (size_t)(nb + 1), h->stream));
@@ -1191,12 +1183,12 @@ static int32_t cycle_enqueue(kb_handle *h, bool hdr_copy = true) {
           k_scan_i32<<<1, 1024, 0, h->stream>>>(D.cell_count, D.cell_start, nb); launches++;
           k_cells_scatter<<<(unsigned)((ncell + 255) / 256), 256, 0, h->stream>>>(D); launches++;
           CUDA_TRY(h, cudaFuncSetAttribute(k_search_cells_grouped, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-          k_search_cells_grouped<<<h->sg_grid, h->sg_wpb * 32, h->sg_smem, h->stream>>>(D, h->sg_ncap, h->sa_codes, h->sa_list_cap); launches++;
+          k_search_cells_grouped<<<p.sg_grid, p.sg_wpb * 32, p.sg_smem, h->stream>>>(D, p.sg_ncap, p.sa_codes, p.sa_list_cap); launches++;
         } else {
-          k_search_cells<<<h->sa_grid, h->sa_wpb * 32, h->sa_smem, h->stream>>>(D, h->sa_col_elems, h->sa_codes, h->sa_list_cap); launches++;
+          k_search_cells<<<p.sa_grid, p.sa_wpb * 32, p.sa_smem, h->stream>>>(D, p.sa_col_elems, p.sa_codes, p.sa_list_cap); launches++;
         }
         kmark(h, KB_K_WALK);
-        k_nominate_walk<<<h->sb_grid, h->sb_wpb * 32, h->sb_smem, h->stream>>>(D, h->sb_col_elems, h->sb_list_cap); launches++;
+        k_nominate_walk<<<p.sb_grid, p.sb_wpb * 32, p.sb_smem, h->stream>>>(D, p.sb_col_elems, p.sb_list_cap); launches++;
       }
     }
     kmark(h, KB_K_SCAN); k_scan_roots<<<1, 1024, 0, h->stream>>>(D); launches++;
