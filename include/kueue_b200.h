@@ -273,7 +273,7 @@ typedef struct kb_snapshot {
      controller.go:100-160; an eviction restarts that clock, setAdmittedTime :62-72).  A finish is
      workload_controller.go:936-952: the workload leaves the cache and QueueAssociatedInadmissibleWorkloadsAfter
      requeues its root cohort tree (the same step as an eviction).  A creation is AddOrUpdateWorkload -> PushOrUpdate
-     (manager.go:524-560), which requeues nothing else.  "Event mode" = at least one of the three tables is non-NULL;
+     (manager.go:524-560), which requeues nothing else.  "Event mode" = at least one of the three tables, or wl_evict_ns, is non-NULL;
      without them kb_run_drain is unchanged.  INT64_MAX as a time means never.  Errors (KB_ERR_INVALID):
      adm_finish_ns[a] <= now_ns, adm_wl naming a record with wl_create_ns > now_ns. */
   int64_t drain_cycle_ns;           /* simulated time one cycle takes; <= 0 means 1 (cycle c at now_ns + c)         */
@@ -314,6 +314,20 @@ typedef struct kb_snapshot {
   int64_t afs_sampling_ns;          /* UsageSamplingInterval (> 0)                                                 */
   const int64_t *lq_last_update_ns; /* [n_lq] AfsConsumedResources LastUpdate, each <= now_ns; NULL = no decay      */
   const int32_t *adm_lq;            /* [n_adm] LocalQueue of each admitted row, -1 for none                         */
+
+  /* ---- eviction latency (optional; read by kb_run_drain only, kb_run_cycle ignores them) ----
+     In the reference an eviction releases nothing at once: IssuePreemptions only sets the Evicted condition
+     (pkg/scheduler/preemption/preemption.go:175-215); the quota is released when the job is stopped and its pods are
+     gone (pkg/controller/jobframework/reconciler.go:576-590, UnsetQuotaReservationWithCondition), then the cache drops
+     the workload and its root cohort tree is requeued (workload_controller.go:973-1004).  wl_evict_ns == NULL: every
+     eviction completes before the next cycle, as without this block.  A non-NULL wl_evict_ns turns on event mode and
+     delays every release by the evicted workload's latency (see kb_run_drain).  adm_evict_end_ns gives the end time of
+     the evictions under way before the drain (rows with adm_evicted set; read only there, INT64_MAX = never); NULL =
+     such rows are issued like any other row when a preemptor targets them.  Errors (KB_ERR_INVALID): either table
+     without adm_wl, adm_evict_end_ns without wl_evict_ns, wl_evict_ns[w] < 0, adm_evict_end_ns[a] <= now_ns on a row
+     with adm_evicted set. */
+  const int64_t *wl_evict_ns;       /* [n_wl] time from the workload's eviction until its quota is released (>= 0)  */
+  const int64_t *adm_evict_end_ns;  /* [n_adm] end of the eviction under way of a row with adm_evicted; NULL = none */
 } kb_snapshot;
 
 /* ------------------------------------------------------------------------
@@ -448,7 +462,8 @@ int32_t kb_download(kb_handle *h, kb_cycle_out *out);
  *   4. the head of every queue in cycle c+1 is its first queued workload in queueOrderingFunc order; a requeued victim
  *      takes the place its priority, creation timestamp and UID give it (workload.go:1174-1193).
  * The drain then ends after the first cycle that neither admits nor evicts.  Evictions under way before the drain
- * (adm_evicted rows that are never targeted) are not completed.
+ * (adm_evicted rows that are never targeted) are not completed, except with kb_snapshot.adm_evict_end_ns (eviction
+ * latency, below).
  * Cycle c runs with now_ns + c.  Bit-exact with iterating kb_run_cycle under the same rules (kueue_b200/drain.py).
  * With the AdmissionFairSharing tables (kb_snapshot.wl_lq != NULL), the queue of a ClusterQueue with cq_afs set is one
  * segment per LocalQueue, each in the order above; its head is the workload with the smallest (LocalQueue usage by
@@ -457,7 +472,7 @@ int32_t kb_download(kb_handle *h, kb_cycle_out *out);
  * BestEffortFIFO advances the head's own segment, the scheduling-hash move covers every segment of the ClusterQueue.
  * Consumed usage does not decay inside a drain, except in event mode with kb_snapshot.lq_last_update_ns (see there).
  *
- * Event mode (kb_snapshot.wl_create_ns / wl_run_ns / adm_finish_ns, any non-NULL): a simulated clock t starts at
+ * Event mode (kb_snapshot.wl_create_ns / wl_run_ns / adm_finish_ns / wl_evict_ns, any non-NULL): a simulated clock t starts at
  * now_ns; cycle c runs at t_c (its now_ns and the QuotaReserved time of its admissions).  Two more queue states:
  * ABSENT (created after t, in no queue) and FINISHED (never requeued).  A pending event is the finish time of a live
  * admitted row or the creation time of an ABSENT workload.  The loop:
@@ -480,7 +495,31 @@ int32_t kb_download(kb_handle *h, kb_cycle_out *out);
  * plain drain.  An evicted workload loses its finish time; a readmission restarts the full run time.  The clock is
  * global (a quiet cycle depends on every root), so event drains are not sharded.  max_cycles counts cycles; the drain
  * stops before running cycle max_cycles.  Events applied before cycle 0 count in n_finished / n_arrived only; the
- * events applied between the start of cycle c and the start of cycle c+1 count in cycle_finished / cycle_arrived[c]. */
+ * events applied between the start of cycle c and the start of cycle c+1 count in cycle_finished / cycle_arrived[c].
+ *
+ * Eviction latency (kb_snapshot.wl_evict_ns != NULL, with adm_wl; event mode): an eviction is issued at once and
+ * completes later, on the clock, as in the reference (preemption.go:175-215 issues, reconciler.go:576-590 releases the
+ * quota once the pods are gone, workload_controller.go:973-1004 requeues).  Step 3 becomes the issue and the release
+ * joins step 5:
+ *   3. issue at t_c: every target row of every Preempting entry that is not already evicting gets adm_evicted = 1 and
+ *      the end time t_c + wl_evict_ns[adm_wl[row]] (saturating at INT64_MAX), which replaces its finish time (an
+ *      evicted workload never finishes; the runner's controller.go:119-127).  It counts in cycle_evicted, n_evicted,
+ *      wl_evictions and the active-cycle rule of step 4.  The row keeps its cells in the usage and stays in the
+ *      admitted tables, a preemption candidate ordered first because it is evicted (preemption/common/ordering.go:
+ *      41-47); its record still holds quota.  A target already evicting gets nothing ("Preemption ongoing",
+ *      preemption.go:183-186): its preemptor stays PendingPreemption (scheduler.go:345-358), and a cycle whose
+ *      Preempting entries only re-target evicting rows is quiet and waits for E;
+ *   5. every evicting row with end <= t_{c+1} completes: its cells leave the usage, its row is removed, its record
+ *      returns to its queue with LastAssignment nil and HasQuotaReservation false, and its root tree is marked for the
+ *      requeue of step 7.  It counts in n_evict_done / cycle_evict_done.  E includes these end times.
+ * Rows with adm_evicted set before the drain complete at adm_evict_end_ns and count as ongoing when targeted; without
+ * that table they are issued at t_c like any other row.  With every wl_evict_ns <= max(drain_cycle_ns, 1) and no
+ * adm_evict_end_ns the drain equals the drain without latency (heads, decisions, evictions, usage, per-workload
+ * results): every issued eviction completes at the next boundary, and steps 5-7 do not depend on their order.
+ * Not modelled: the sticky workload (cluster_queue.go:64-93,609-624,656-665), which in the reference keeps a preemptor
+ * that waits for its evictions at the head of its queue; here every waiting preemptor is ordered again each cycle and
+ * re-runs its target search.  Nor are preemption expectations between issue and observation (the drain observes an
+ * eviction at once). */
 typedef struct kb_drain_out {
   int32_t max_cycles;        /* in */
   int32_t n_cycles;          /* out: cycles run */
@@ -520,6 +559,9 @@ typedef struct kb_drain_out {
   int32_t *lq_consumed_scale; /* [n_lq][R] their scales */
   int64_t *lq_last_update_ns; /* [n_lq] LastUpdate */
   int64_t n_afs_samples;      /* out: decay samples due over the drain (those a fixed point skips included); 0 without decay */
+  /* eviction latency (kb_snapshot.wl_evict_ns != NULL; zero / untouched otherwise; the pointer may be NULL) */
+  int64_t n_evict_done;       /* out: evictions completed (quota released), those before cycle 0 included */
+  int32_t *cycle_evict_done;  /* [max_cycles] evictions completed from the start of cycle c to the start of c+1 */
 } kb_drain_out;
 int32_t kb_run_drain(kb_handle *h, const kb_snapshot *s, kb_drain_out *out);
 

@@ -361,6 +361,9 @@ func (s *Scheduler) flatten(snap *schdcache.Snapshot, heads []workload.Info, gen
 	// Arrivals and completions in kb_run_drain (INTEGRATION.md): a queue simulation fills one creation time per pending
 	// workload and one run time, plus one finish time per admitted workload, and the length of one cycle:
 	//   c.wl_create_ns, c.wl_run_ns, c.adm_finish_ns = cp64(wlCreate), cp64(wlRun), cp64(admFinish); c.drain_cycle_ns = C.int64_t(cycleNs)
+	// With eviction replay it may also fill each workload's eviction latency (until its pods are gone) and, for the
+	// admitted workloads already evicted, the time their quota is released (read where adm_evicted is set):
+	//   c.wl_evict_ns, c.adm_evict_end_ns = cp64(wlEvict), cp64(admEvictEnd)
 	// They stay nil here: a single cycle ignores them.
 	if anyGroup { // optional table: NULL when no podset is grouped
 		c.ps_group = cp32(psGroup)

@@ -82,6 +82,7 @@ class kb_snapshot(C.Structure):
         ("adm_finish_ns", _P(C.c_int64)),
         ("afs_half_life_ns", C.c_int64), ("afs_sampling_ns", C.c_int64), ("lq_last_update_ns", _P(C.c_int64)),
         ("adm_lq", _P(C.c_int32)),
+        ("wl_evict_ns", _P(C.c_int64)), ("adm_evict_end_ns", _P(C.c_int64)),
     ]
 
 
@@ -131,6 +132,7 @@ class kb_drain_out(C.Structure):
         ("wl_admit_ns", _P(C.c_int64)), ("wl_finish_ns", _P(C.c_int64)),
         ("lq_consumed", _P(C.c_int64)), ("lq_consumed_scale", _P(C.c_int32)), ("lq_last_update_ns", _P(C.c_int64)),
         ("n_afs_samples", C.c_int64),
+        ("n_evict_done", C.c_int64), ("cycle_evict_done", _P(C.c_int32)),
     ]
 
 
@@ -185,16 +187,19 @@ _DT = {
     "adm_wl": np.int32,
     "wl_create_ns": np.int64, "wl_run_ns": np.int64, "adm_finish_ns": np.int64,
     "lq_last_update_ns": np.int64, "adm_lq": np.int32,
+    "wl_evict_ns": np.int64, "adm_evict_end_ns": np.int64,
 }
 # AdmissionFairSharing tables (include/kueue_b200.h): wl_lq absent = AFS off
 AFS_FIELDS = ("wl_lq", "lq_cq", "cq_afs", "lq_weight", "lq_consumed", "lq_consumed_scale", "lq_penalty", "afs_res_weight",
               "afs_milli_mul")
 # arrivals and completions of kb_run_drain's event mode (include/kueue_b200.h): all absent = event mode off
-EVENT_FIELDS = ("wl_create_ns", "wl_run_ns", "adm_finish_ns")
+EVENT_FIELDS = ("wl_create_ns", "wl_run_ns", "adm_finish_ns", "wl_evict_ns")
 # decay of the AdmissionFairSharing consumed usage in event mode (include/kueue_b200.h): lq_last_update_ns absent = off
 AFS_DECAY_FIELDS = ("lq_last_update_ns", "adm_lq")
+# end times of the evictions under way before an event drain with wl_evict_ns (include/kueue_b200.h): absent = none known
+EVICT_END_FIELDS = ("adm_evict_end_ns",)
 OPTIONAL_FIELDS = (("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows", "adm_wl") + AFS_FIELDS +
-                   EVENT_FIELDS + AFS_DECAY_FIELDS)  # NULL in kb_snapshot when absent
+                   EVENT_FIELDS + AFS_DECAY_FIELDS + EVICT_END_FIELDS)  # NULL in kb_snapshot when absent
 ARRAY_FIELDS = list(_DT.keys())
 # tables the library keeps resident while kb_snapshot.static_generation is unchanged (include/kueue_b200.h)
 STATIC_FIELDS = ("parent", "fair_weight", "nominal", "borrow_limit", "lend_limit", "cq_within_cq", "cq_reclaim_within",
@@ -419,6 +424,7 @@ class DrainOut:
         self.cycle_start_ns = np.zeros(max_cycles, np.int64)
         self.cycle_finished = np.zeros(max_cycles, np.int32)
         self.cycle_arrived = np.zeros(max_cycles, np.int32)
+        self.cycle_evict_done = np.zeros(max_cycles, np.int32)
         self.wl_admit_ns = np.full(W, KB_TS_UNSET, np.int64)
         self.wl_finish_ns = np.full(W, KB_NO_LIMIT, np.int64)
         L = len(snap.arrays["lq_cq"]) if "lq_cq" in snap.arrays else 0
@@ -438,6 +444,7 @@ class DrainOut:
         s.cycle_evicted = _ptr(self.cycle_evicted, C.c_int32); s.wl_evictions = _ptr(self.wl_evictions, C.c_int32)
         s.cycle_start_ns = _ptr(self.cycle_start_ns, C.c_int64)
         s.cycle_finished = _ptr(self.cycle_finished, C.c_int32); s.cycle_arrived = _ptr(self.cycle_arrived, C.c_int32)
+        s.cycle_evict_done = _ptr(self.cycle_evict_done, C.c_int32)
         s.wl_admit_ns = _ptr(self.wl_admit_ns, C.c_int64); s.wl_finish_ns = _ptr(self.wl_finish_ns, C.c_int64)
         s.lq_consumed = _ptr(self.lq_consumed, C.c_int64); s.lq_consumed_scale = _ptr(self.lq_consumed_scale, C.c_int32)
         s.lq_last_update_ns = _ptr(self.lq_last_update_ns, C.c_int64)
@@ -464,6 +471,8 @@ class DrainOut:
     def end_ns(self): return int(self.struct.end_ns)
     @property
     def n_afs_samples(self): return int(self.struct.n_afs_samples)
+    @property
+    def n_evict_done(self): return int(self.struct.n_evict_done)
 
     def cycles(self):
         """[(heads, decisions)] per cycle from the trace."""

@@ -1368,7 +1368,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   const int Hcap = std::min(Q, W);
   const int max_cycles = std::max(0, out->max_cycles);
   out->n_cycles = 0; out->n_decisions = 0; out->n_admitted = 0; out->gpu_ms = 0; out->n_evicted = 0;
-  out->n_finished = 0; out->n_arrived = 0; out->end_ns = s->now_ns;
+  out->n_finished = 0; out->n_arrived = 0; out->end_ns = s->now_ns; out->n_evict_done = 0;
   // ---- eviction replay: host-side checks of adm_wl (include/kueue_b200.h)
   const bool replay = s->adm_wl != nullptr;
   if (replay) {
@@ -1384,7 +1384,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     }
   }
   // ---- event mode: host-side checks of the arrival and completion tables (include/kueue_b200.h)
-  const bool events = s->wl_create_ns || s->wl_run_ns || s->adm_finish_ns;
+  const bool events = s->wl_create_ns || s->wl_run_ns || s->adm_finish_ns || s->wl_evict_ns;
   if (events) {
     if (s->adm_finish_ns)
       for (int a = 0; a < s->n_adm; a++)
@@ -1392,6 +1392,18 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (replay && s->wl_create_ns)
       for (int a = 0; a < s->n_adm; a++)
         if (s->wl_create_ns[s->adm_wl[a]] > s->now_ns) return fail(h, KB_ERR_INVALID, "adm_wl names a record created after now_ns");
+  }
+  // ---- eviction latency: host-side checks (include/kueue_b200.h)
+  const bool lat = s->wl_evict_ns != nullptr;
+  if (lat || s->adm_evict_end_ns) {
+    if (!replay) return fail(h, KB_ERR_INVALID, "eviction latency: wl_evict_ns / adm_evict_end_ns need adm_wl");
+    if (!lat) return fail(h, KB_ERR_INVALID, "eviction latency: adm_evict_end_ns needs wl_evict_ns");
+    for (int w = 0; w < W; w++)
+      if (s->wl_evict_ns[w] < 0) return fail(h, KB_ERR_INVALID, "eviction latency: wl_evict_ns < 0");
+    if (s->adm_evict_end_ns && s->adm_evicted)
+      for (int a = 0; a < s->n_adm; a++)
+        if (s->adm_evicted[a] && s->adm_evict_end_ns[a] <= s->now_ns)
+          return fail(h, KB_ERR_INVALID, "eviction latency: an eviction under way before the drain ends at or before now_ns");
   }
   // ---- decay of AdmissionFairSharing consumed usage: host-side checks (include/kueue_b200.h)
   const bool decay = s->lq_last_update_ns != nullptr;
@@ -1486,7 +1498,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   u64 *keys[2], *arr_keys[2] = {nullptr, nullptr};
   int32_t *vals[2], *arr_vals[2] = {nullptr, nullptr}, *q_count, *d_wl_class = nullptr, *d_cq_class_start = nullptr;
   char *sort_tmp, *scan_tmp = nullptr;
-  i64 *run = nullptr, *create = nullptr;
+  i64 *run = nullptr, *create = nullptr, *evict_ns = nullptr;
   DrainDev X{};
   AdmTabs other{};  // compaction: the other half of the admitted tables' double buffer
   auto layout = [&](Arena &a) {
@@ -1527,6 +1539,10 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       }
       if (n_class) { d_wl_class = a.take<int32_t>(Wz); d_cq_class_start = a.take<int32_t>((size_t)Q + 1); X.class_nofit = a.take<uint8_t>(n_class); }
     }
+    if (lat) {  // latencies and the evicting byte of both halves
+      evict_ns = a.take<i64>(Wz);
+      X.adm_evicting = a.take<uint8_t>(Acap); other.evicting = a.take<uint8_t>(Acap);
+    }
     if (afs) {
       X.seg_start = a.take<int32_t>(seg_start.size()); X.lq_seg = a.take<int32_t>(lq_seg.size());
       X.seg_lq = a.take<int32_t>(seg_lq.size()); X.afs_cqs = a.take<int32_t>(afs_cqs.size());
@@ -1560,9 +1576,19 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     CUDA_TRY(h, cudaMemsetAsync(X.root_mark, 0, nR * 4, h->stream));
   }
   std::vector<i64> never;  // event mode without adm_finish_ns: the rows of the snapshot never finish
+  std::vector<uint8_t> evicting;  // latency with adm_evict_end_ns: the rows whose eviction is under way
   if (events) {
     const void *finish = s->adm_finish_ns;
     if (!finish) { never.assign((size_t)s->n_adm, INT64_MAX); finish = never.data(); }
+    if (lat && s->adm_evict_end_ns) {  // their end time replaces their finish time (an evicted workload never finishes)
+      std::vector<i64> fin((size_t)s->n_adm);
+      memcpy(fin.data(), finish, (size_t)s->n_adm * 8);
+      evicting.assign((size_t)s->n_adm, 0);
+      for (int a = 0; a < s->n_adm; a++)
+        if (s->adm_evicted[a]) { fin[a] = s->adm_evict_end_ns[a]; evicting[a] = 1; }
+      never.swap(fin);
+      finish = never.data();
+    }
     CUDA_TRY(h, h2d(h, X.adm_finish, finish, (size_t)s->n_adm * 8));
     if (s->wl_run_ns) { CUDA_TRY(h, h2d(h, run, s->wl_run_ns, Wz * 8)); X.wl_run = run; }
     if (create) { CUDA_TRY(h, h2d(h, create, s->wl_create_ns, Wz * 8)); X.n_arr = W; }
@@ -1571,6 +1597,12 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       CUDA_TRY(h, h2d(h, d_cq_class_start, cq_class_start.data(), ((size_t)Q + 1) * 4));
       CUDA_TRY(h, cudaMemsetAsync(X.class_nofit, 0, (size_t)n_class, h->stream));
       X.wl_class = d_wl_class; X.cq_class_start = d_cq_class_start;
+    }
+    if (lat) {
+      CUDA_TRY(h, h2d(h, evict_ns, s->wl_evict_ns, Wz * 8));
+      X.wl_evict = evict_ns;
+      if (!evicting.empty()) CUDA_TRY(h, h2d(h, X.adm_evicting, evicting.data(), evicting.size()));
+      else CUDA_TRY(h, cudaMemsetAsync(X.adm_evicting, 0, (size_t)s->n_adm, h->stream));
     }
   }
   if (afs) {
@@ -1739,6 +1771,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       if (events && out->cycle_start_ns) out->cycle_start_ns[cyc] = t;
       if (events && out->cycle_finished) out->cycle_finished[cyc] = 0;
       if (events && out->cycle_arrived) out->cycle_arrived[cyc] = 0;
+      if (lat && out->cycle_evict_done) out->cycle_evict_done[cyc] = 0;
       out->n_decisions += n_live; out->n_admitted += n_new; out->n_evicted += n_ev;
       out->n_cycles = ++cyc;
     } else {
@@ -1752,12 +1785,18 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
         if (out->cycle_arrived) out->cycle_arrived[cyc - 1] += arr;
       }
     }
+    if (lat) {  // evictions completed at this boundary (counter slot 4, inside the events copy)
+      const int done = (int)hw.counters[KB_DC_EVICT_DONE];
+      out->n_evict_done += done;
+      if (cyc > 0 && out->cycle_evict_done) out->cycle_evict_done[cyc - 1] += done;
+    }
     if (compact) {  // the compacted half becomes the admitted tables of the next boundary
       A_cur = (int)hw.counters[KB_DC_ROWS]; AU_cur = (int)hw.counters[KB_DC_CELLS];
-      AdmTabs cur{X.adm_cq, X.adm_priority, X.adm_ts, X.adm_qr_ts, X.adm_uid, X.adm_evicted, X.adm_use_start, X.adm_use_fr, X.adm_use_qty, X.adm_wl, X.adm_finish, X.adm_lq};
+      AdmTabs cur{X.adm_cq, X.adm_priority, X.adm_ts, X.adm_qr_ts, X.adm_uid, X.adm_evicted, X.adm_use_start, X.adm_use_fr, X.adm_use_qty, X.adm_wl, X.adm_finish, X.adm_lq,
+                  X.adm_evicting};
       X.adm_cq = other.cq; X.adm_priority = other.priority; X.adm_ts = other.ts; X.adm_qr_ts = other.qr_ts; X.adm_uid = other.uid;
       X.adm_evicted = other.evicted; X.adm_use_start = other.use_start; X.adm_use_fr = other.use_fr; X.adm_use_qty = other.use_qty; X.adm_wl = other.wl;
-      X.adm_finish = other.finish; X.adm_lq = other.lq;
+      X.adm_finish = other.finish; X.adm_lq = other.lq; X.adm_evicting = other.evicting;
       D.adm_cq = X.adm_cq; D.adm_priority = X.adm_priority; D.adm_ts = X.adm_ts; D.adm_qr_ts = X.adm_qr_ts; D.adm_uid = X.adm_uid;
       D.adm_evicted = X.adm_evicted; D.adm_use_start = X.adm_use_start; D.adm_use_fr = X.adm_use_fr; D.adm_use_qty = X.adm_use_qty;
       other = cur;

@@ -30,7 +30,7 @@
 // at the start and at every boundary, k_drain_admit decays to t_c and puts the penalty into consumed, k_drain_finish
 // takes finished rows out of the LocalQueue's admitted usage (adm_lq, carried by the compaction).
 //
-// Event mode (kb_snapshot.wl_create_ns / wl_run_ns / adm_finish_ns; include/kueue_b200.h): two more states,
+// Event mode (kb_snapshot.wl_create_ns / wl_run_ns / adm_finish_ns / wl_evict_ns; include/kueue_b200.h): two more states,
 // KB_WS_ABSENT (not created yet) and KB_WS_FINISHED.  Every admitted row carries its finish time (adm_finish, written by
 // k_drain_admit, carried by the compaction) and its record (adm_wl, -1 for a row of the snapshot without one).  The
 // boundary is the replay's, with the clock between the evictions and the requeue: k_drain_ev_min reduces E (the
@@ -40,7 +40,9 @@
 // (create, index) order; then k_drain_requeue visits the marked roots and the compaction follows.  A cycle without heads
 // is replaced by the same boundary with t_{c+1} = E and a negative stamp (no cycle is counted).  The NoFit set of a
 // ClusterQueue is one byte per (ClusterQueue, scheduling hash) class: k_drain_apply sets it, k_drain_requeue clears the
-// bytes of the queues it visits.
+// bytes of the queues it visits.  With eviction latency (wl_evict_ns) k_drain_evict only issues: it sets adm_evicted and
+// the byte column adm_evicting (carried by the compaction) and writes the end time into the finish column, so E and the
+// compaction see it unchanged; k_drain_finish releases the row at its end time through the replay's requeue path.
 #pragma once
 
 #include <cub/device/device_scan.cuh>
@@ -213,10 +215,14 @@ struct DrainDev {
   const int32_t *wl_class;         // [W] (ClusterQueue, hash) class of a BestEffortFIFO workload with a known hash, -1
   const int32_t *cq_class_start;   // [Q+1] classes of a ClusterQueue
   uint8_t *class_nofit;            // [classes] in the ClusterQueue's NoFit set; null = no arrivals or no hashes
+  // eviction latency (event mode); wl_evict == nullptr: off
+  const i64 *wl_evict;             // [W] time from a workload's eviction until its quota is released
+  uint8_t *adm_evicting;           // [A_cap] 1 while the row's eviction is under way (current half); its end is adm_finish
 };
-// counters of a boundary: [1] evictions, [2] / [3] rows / cells after the compaction, [5] capacity flag; event mode:
-// [6] completions, [7] arrivals, [8] end flag, [9] / [10] arrived prefix of arr_order [lo, hi)
-enum { KB_DC_EVICTED = 1, KB_DC_ROWS = 2, KB_DC_CELLS = 3, KB_DC_FULL = 5,
+// counters of a boundary: [1] evictions (issued, with latency), [2] / [3] rows / cells after the compaction, [4]
+// evictions completed (latency), [5] capacity flag; event mode: [6] completions, [7] arrivals, [8] end flag, [9] / [10]
+// arrived prefix of arr_order [lo, hi)
+enum { KB_DC_EVICTED = 1, KB_DC_ROWS = 2, KB_DC_CELLS = 3, KB_DC_EVICT_DONE = 4, KB_DC_FULL = 5,
        KB_DC_FINISHED = 6, KB_DC_ARRIVED = 7, KB_DC_END = 8, KB_DC_ARR_LO = 9, KB_DC_ARR_HI = 10 };
 
 __device__ __forceinline__ int drain_seg0(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq] : cq; }
@@ -413,6 +419,7 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
   if (X.adm_lq) X.adm_lq[a] = X.wl_lq[wl];
   X.adm_cq[a] = cq; X.adm_priority[a] = D.wl_priority[wl]; X.adm_ts[a] = D.wl_ts[wl]; X.adm_qr_ts[a] = qr_ts;
   X.adm_uid[a] = D.wl_uid[wl]; X.adm_evicted[a] = 0;
+  if (X.adm_evicting) X.adm_evicting[a] = 0;
   X.adm_use_start[a] = c0;
   if (X.adm_finish) {  // finish = QuotaReserved time + run time, saturating; run < 0 never finishes
     const i64 run = X.wl_run ? X.wl_run[wl] : -1;
@@ -473,27 +480,49 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
 }
 
 // ---- eviction replay ---------------------------------------------------------------------------------------------
+// the record of an evicted row returns to its queue with LastAssignment nil (the eviction completed)
+__device__ __forceinline__ void drain_release(const DevSnap &D, const DrainDev &X, int w) {
+  X.wl_state[w] = KB_WS_QUEUED;
+  X.wl_last_gen[w] = -1;
+  for (int i = D.wl_ps_start[w] * D.R; i < D.wl_ps_start[w + 1] * D.R; i++) X.ps_last_tried[i] = -1;
+  if (X.wl_has_qr) X.wl_has_qr[w] = 0;
+  X.wl_admit_cycle[w] = -1;
+  atomicMin(&X.cursor[X.wl_seg[w]], X.wl_pos[w]);
+}
+// sets byte i of a byte column (256-byte aligned, padded) and returns whether it was set: atomicOr on its aligned word
+__device__ __forceinline__ bool drain_claim_byte(uint8_t *col, int i) {
+  const uintptr_t p = (uintptr_t)(col + i);
+  const unsigned bit = 1u << (8 * (unsigned)(p & 3));
+  return (atomicOr((unsigned *)(p & ~(uintptr_t)3), bit) & bit) != 0;
+}
 // every target of every Preempting entry (thread per entry): cells out of its ClusterQueue's usage (integer atomics:
-// the order does not matter), row dead, pending record QUEUED with LastAssignment nil, its root tree marked
+// the order does not matter), row dead, pending record QUEUED with LastAssignment nil, its root tree marked.  With
+// latency (wl_evict) the eviction is only issued: a row not evicting yet is claimed once, gets adm_evicted and its end
+// time t_c + latency (saturating) in its finish column, and keeps its cells and its record; k_drain_finish releases it.
 __global__ void k_drain_evict(DevSnap D, DrainDev X) {
   int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= D.H || D.decision[e] != KB_DEC_PREEMPTING) return;
-  const int R = D.R, stamp = X.cycle + 1;
+  const int stamp = X.cycle + 1;
   const int off = D.tgt_off[e], n = D.tgt_cnt[e];
   for (int k = 0; k < n; k++) {
     const int a = D.tgt_pool_adm[off + k];
+    if (X.wl_evict) {
+      if (drain_claim_byte(X.adm_evicting, a)) continue;  // under way: "Preemption ongoing" (preemption.go:183-186)
+      const int w = X.adm_wl[a];
+      const i64 lat = X.wl_evict[w];
+      X.adm_evicted[a] = 1;
+      X.adm_finish[a] = D.now_ns > INT64_MAX - lat ? INT64_MAX : D.now_ns + lat;
+      X.wl_evictions[w]++;
+      atomicAdd(&X.counters[KB_DC_EVICTED], 1);
+      continue;
+    }
     if (atomicExch(&X.adm_dead[a], stamp) == stamp) continue;  // one eviction per row
     const int cq = X.adm_cq[a];
     for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)  // cache.DeleteWorkload
       atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
     const int w = X.adm_wl[a];
-    X.wl_state[w] = KB_WS_QUEUED;
-    X.wl_last_gen[w] = -1;
-    for (int i = D.wl_ps_start[w] * R; i < D.wl_ps_start[w + 1] * R; i++) X.ps_last_tried[i] = -1;
-    if (X.wl_has_qr) X.wl_has_qr[w] = 0;
-    X.wl_admit_cycle[w] = -1;
+    drain_release(D, X, w);
     X.wl_evictions[w]++;  // a workload holds at most one row: one writer
-    atomicMin(&X.cursor[X.wl_seg[w]], X.wl_pos[w]);
     X.root_mark[D.root_slot[cq]] = stamp;
     atomicAdd(&X.counters[KB_DC_EVICTED], 1);
   }
@@ -520,7 +549,7 @@ __global__ void k_drain_live(DrainDev X, int bound, const int32_t *n_new) {
   X.row_live[a] = live;
   X.row_cells[a] = live ? X.adm_use_start[a + 1] - X.adm_use_start[a] : 0;
 }
-struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; i64 *finish; int32_t *lq; };
+struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; i64 *finish; int32_t *lq; uint8_t *evicting; };
 // live rows of [0, bound), in order, into the other half of the double buffer; thread bound writes the totals
 __global__ void k_drain_compact(DrainDev X, AdmTabs O, int bound) {
   int a = blockIdx.x * blockDim.x + threadIdx.x;
@@ -532,6 +561,7 @@ __global__ void k_drain_compact(DrainDev X, AdmTabs O, int bound) {
   O.uid[n] = X.adm_uid[a]; O.evicted[n] = X.adm_evicted[a]; O.wl[n] = X.adm_wl[a]; O.use_start[n] = c0;
   if (X.adm_finish) O.finish[n] = X.adm_finish[a];
   if (X.adm_lq) O.lq[n] = X.adm_lq[a];
+  if (X.adm_evicting) O.evicting[n] = X.adm_evicting[a];
   for (int c = 0; c < nc; c++) { O.use_fr[c0 + c] = X.adm_use_fr[u0 + c]; O.use_qty[c0 + c] = X.adm_use_qty[u0 + c]; }
 }
 
@@ -594,7 +624,8 @@ __global__ void k_drain_ev_next(DrainDev X, i64 t_c, i64 step, int jump, const i
   X.counters[KB_DC_ARR_HI] = (end || !X.arr_key) ? lo : ev_upper_bound(X.arr_key, lo, X.n_arr, tn);
 }
 // completions (thread per row): a live row with finish <= t_{c+1} gets the dead stamp, its cells leave its ClusterQueue's
-// usage (cache.DeleteWorkload, integer atomics), its record becomes FINISHED and its root tree is marked.  Rows in
+// usage (cache.DeleteWorkload, integer atomics), its record becomes FINISHED and its root tree is marked.  An evicting
+// row's finish column holds its end time: it completes the eviction instead, its record returns to its queue.  Rows in
 // [A + *n_new, bound) only pad the compaction's range.
 __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *n_new) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x;
@@ -606,14 +637,16 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
   for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)
     atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
   const int w = X.adm_wl[a];
-  if (w >= 0) { X.wl_state[w] = KB_WS_FINISHED; X.wl_admit_cycle[w] = -1; X.wl_finish_ns[w] = X.adm_finish[a]; }
+  const bool released = X.adm_evicting && X.adm_evicting[a];
+  if (released) drain_release(D, X, w);
+  else if (w >= 0) { X.wl_state[w] = KB_WS_FINISHED; X.wl_admit_cycle[w] = -1; X.wl_finish_ns[w] = X.adm_finish[a]; }
   if (X.lq_last && X.adm_lq[a] >= 0 && X.cq_afs[cq]) {  // several rows of one LocalQueue can finish together
     i64 *adm = X.lq_adm + (size_t)X.adm_lq[a] * D.R;
     for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)
       atomicAdd((unsigned long long *)&adm[X.adm_use_fr[c] % D.R], (unsigned long long)(-X.adm_use_qty[c]));
   }
   X.root_mark[D.root_slot[cq]] = stamp;
-  atomicAdd(&X.counters[KB_DC_FINISHED], 1);
+  atomicAdd(&X.counters[released ? KB_DC_EVICT_DONE : KB_DC_FINISHED], 1);
 }
 // decay samples (thread per LocalQueue of an AFS ClusterQueue): every sample due in (t, t'] with t' = clock[0], in time
 // order, each with alpha = afs_alpha (one interval elapsed), or a reset to empty with half-life 0; LastUpdate moves to

@@ -85,7 +85,26 @@ is the finish time of a live admitted row or the creation time of an ABSENT work
 Steps 5-7 only set state bytes and lower cursors: their order does not change the result.  Waiting in a quiet cycle is
 the canonical choice; with every run time < 0 and every creation <= now_ns the drain is the plain drain.  The drain
 stops before cycle max_cycles.  Events applied before cycle 0 count only in the totals; the events applied between the
-start of cycle c and the start of cycle c+1 are cycle c's (`finished`, `arrived`).
+start of cycle c and the start of cycle c+1 are cycle c's (`finished`, `arrived`, `evict_done`).
+
+Eviction latency (event mode, the snapshot carries `wl_evict_ns` and `adm_wl`, include/kueue_b200.h).  In the
+reference IssuePreemptions only sets the Evicted condition (preemption.go:175-215); the quota is released once the job
+is stopped and its pods are gone (reconciler.go:576-590, UnsetQuotaReservationWithCondition), then the workload leaves
+the cache and its root tree is requeued (workload_controller.go:973-1004).  `wl_evict_ns[w]` is that time.  Step 3
+becomes the issue, the release moves to step 5:
+  3. issue at t_c: every target row of every Preempting entry that is not already evicting gets adm_evicted = 1 and the
+     end time t_c + wl_evict_ns[adm_wl[row]] (saturating), which replaces its finish time (an evicted workload never
+     finishes, the runner's controller.go:119-127).  It counts in `evicted`, `wl_evictions` and the active-cycle rule;
+     the row keeps its cells in the usage and stays in the tables (a candidate ordered first, ordering.go:41-47), its
+     record stays HELD.  A target that is already evicting gets nothing ("Preemption ongoing", preemption.go:183-186):
+     a cycle whose Preempting entries only re-target evicting rows is quiet and waits for E;
+  5. complete: every evicting row with end <= t_{c+1} leaves the tables (its cells leave the usage), its record is
+     QUEUED with LastAssignment nil and HasQuotaReservation false, the cursor moves back, its root tree is marked, and
+     it counts in `evict_done`.  E includes these end times.
+Rows with adm_evicted set before the drain complete at `adm_evict_end_ns` (never targeted as new evictions) when the
+snapshot carries it; without it they are issued like any other row when targeted.  With every wl_evict_ns <=
+max(drain_cycle_ns, 1) and no `adm_evict_end_ns` the drain equals the drain without latency: every issued eviction
+completes at the next boundary, and steps 5-7 do not depend on their order.
 
 Decay of the AdmissionFairSharing consumed usage (event mode, the snapshot carries `lq_last_update_ns` and `adm_lq`,
 include/kueue_b200.h), as the LocalQueue reconciler decays it (localqueue_controller.go:210-229,363-398):
@@ -147,6 +166,9 @@ class DrainResult:
     wl_admit_ns: np.ndarray | None = None                      # [n_wl] time of its last admission, INT64_MIN = never
     wl_finish_ns: np.ndarray | None = None                     # [n_wl] finish time, INT64_MAX = not finished
     end_ns: int = 0                                            # the clock when the drain stopped
+    # eviction latency (wl_evict_ns in the snapshot; empty / 0 otherwise)
+    evict_done: List[np.ndarray] = field(default_factory=list) # per cycle: pending indices whose eviction completed
+    n_evict_done: int = 0                                      # including the completions applied before cycle 0
     # decay of consumed usage (lq_last_update_ns in the snapshot; None / 0 otherwise)
     lq_consumed: np.ndarray | None = None                      # [n_lq][R] int64Amount values after the drain
     lq_consumed_scale: np.ndarray | None = None                # [n_lq][R] their scales
@@ -439,6 +461,10 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     step = max(1, int(snap.drain_cycle_ns)) if events else 1
     create = a.get("wl_create_ns")
     run_ns = a.get("wl_run_ns")
+    lat = a.get("wl_evict_ns")  # eviction latency: issue at t_c, release at the end time
+    if lat is not None and not replay:
+        raise ValueError("wl_evict_ns needs adm_wl")
+    evicting = None                                               # [rows] the row's eviction is under way (latency)
     state = np.full(snap.n_wl, QUEUED, np.uint8)
     seg_of = np.zeros(snap.n_wl, np.int64)                        # segment of every pending workload
     pos_of = np.zeros(snap.n_wl, np.int64)                        # its position in the segment's static order
@@ -451,6 +477,11 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         adm_finish = a["adm_finish_ns"].astype(np.int64).copy() if "adm_finish_ns" in a else np.full(snap.n_adm, NEVER, np.int64)
         if create is not None:
             state[create > snap.now_ns] = ABSENT
+        if lat is not None:
+            evicting = np.zeros(snap.n_adm, bool)
+            if "adm_evict_end_ns" in a:  # evictions under way before the drain complete at their end time
+                evicting = a["adm_evicted"].astype(bool).copy()
+                adm_finish[evicting] = a["adm_evict_end_ns"][evicting]
     if replay:
         state[a["adm_wl"].astype(np.int64)] = HELD  # holds quota: out of every queue
     cursor = np.zeros(len(qlen), np.int64)
@@ -557,7 +588,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
 
     def remove_rows(rows):
         """rows leave the admitted tables (cache.DeleteWorkload: cells out of the usage; the other rows keep their order)"""
-        nonlocal adm_wl, adm_finish, adm_lq
+        nonlocal adm_wl, adm_finish, adm_lq, evicting
         us, uf, uq = adm["adm_use_start"], adm["adm_use_fr"], adm["adm_use_qty"]
         for row in rows:
             cqi = int(adm["adm_cq"][row])
@@ -577,6 +608,19 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             adm_finish = adm_finish[keep]
         if decay:
             adm_lq = adm_lq[keep]
+        if evicting is not None:
+            evicting = evicting[keep]
+
+    def release(w):
+        """the record of an evicted row returns to its queue with LastAssignment nil (workload_controller.go:973-1004);
+        preemption sets no RequeueState, so the requeue is immediate"""
+        state[w] = QUEUED
+        last_gen[w] = -1
+        last_tried[int(ps_start[w]):int(ps_start[w + 1])] = -1
+        if has_qr is not None:
+            has_qr[w] = 0
+        admit_cycle[w] = -1
+        cursor[seg_of[w]] = min(cursor[seg_of[w]], pos_of[w])
 
     def next_event():
         """earliest pending event after the evictions: a live row's finish or an ABSENT workload's creation (None = none)"""
@@ -586,17 +630,20 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         return None if e >= NEVER else e
 
     def apply_events(t_next, notified):
-        """steps 5 and 6 at t_next; returns (finished records, arrived records)"""
+        """steps 5 and 6 at t_next; returns (finished records, arrived records, records whose eviction completed)"""
         nonlocal arr_next
         done = np.flatnonzero(adm_finish <= t_next)
-        fin = adm_wl[done].copy()
+        gone = evicting[done] if evicting is not None else np.zeros(len(done), bool)
+        fin, released = adm_wl[done[~gone]].copy(), adm_wl[done[gone]].copy()
         for row in done:
             notified.add(int(adm["adm_cq"][row]))
             if decay and adm_lq[row] >= 0 and afs_cq[int(adm["adm_cq"][row])]:  # rule 5
                 for k in range(int(adm["adm_use_start"][row]), int(adm["adm_use_start"][row + 1])):
                     ladm[adm_lq[row], int(adm["adm_use_fr"][k]) % R] -= int(adm["adm_use_qty"][k])
             w = int(adm_wl[row])
-            if w >= 0:
+            if evicting is not None and evicting[row]:
+                release(w)
+            elif w >= 0:
                 state[w] = FINISHED
                 admit_cycle[w] = -1
                 finish_ns[w] = int(adm_finish[row])
@@ -612,7 +659,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 state[w] = QUEUED
                 cursor[seg_of[w]] = min(cursor[seg_of[w]], pos_of[w])
             arr.append(w)
-        return fin, np.asarray(arr, np.int64)
+        return fin, np.asarray(arr, np.int64), released
 
     def requeue(notified):
         """step 7: the inadmissible requeue in the root cohort trees of `notified`"""
@@ -630,10 +677,11 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 cursor[s] = min(cursor[s], first_aside[s])
                 first_aside[s] = qlen[s]
 
-    def after(fin, arr):  # events applied between the start of the last cycle and the next one
-        res.n_finished += len(fin); res.n_arrived += len(arr)
+    def after(fin, arr, released):  # events applied between the start of the last cycle and the next one
+        res.n_finished += len(fin); res.n_arrived += len(arr); res.n_evict_done += len(released)
         if res.cycles:
             res.finished[-1] = np.concatenate([res.finished[-1], fin]); res.arrived[-1] = np.concatenate([res.arrived[-1], arr])
+            res.evict_done[-1] = np.concatenate([res.evict_done[-1], released])
 
     t = int(snap.now_ns)
     cyc = 0
@@ -685,7 +733,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         res.cycles += 1
         res.heads.append(heads); res.decisions.append(dec)
         res.cycle_start_ns.append(t)
-        res.finished.append(np.zeros(0, np.int64)); res.arrived.append(np.zeros(0, np.int64))
+        res.finished.append(np.zeros(0, np.int64)); res.arrived.append(np.zeros(0, np.int64)); res.evict_done.append(np.zeros(0, np.int64))
         ok = dec == abi.DEC_ASSUMED
         res.admitted.append(heads[ok])
         # ---- apply the admissions: Assignment.Usage (flavorassigner.go:198-218) with the admitted counts
@@ -751,6 +799,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             if events:
                 fin_new = [finish_time(t, int(run_ns[w])) if run_ns is not None else NEVER for w in g]
                 adm_finish = np.concatenate([adm_finish, np.asarray(fin_new, np.int64)])
+            if evicting is not None:
+                evicting = np.concatenate([evicting, np.zeros(n_new, bool)])
         # ---- LastAssignment of the entries that stay pending (scheduler.go:345,494)
         tried = np.asarray(out.ps_tried_idx).reshape(-1, R)
         cqs = live
@@ -791,20 +841,23 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             for e in np.flatnonzero(dec == abi.DEC_PREEMPTING):
                 victims.extend(int(out.tgt_adm[k]) for k in range(int(out.tgt_start[e]), int(out.tgt_start[e + 1])))
             victims = sorted(set(victims))
+        if evicting is not None:  # latency: issue the evictions not under way yet; the rows stay until their end time
+            victims = [row for row in victims if not evicting[row]]
         res.evicted.append(np.sort(adm_wl[victims]) if victims else np.zeros(0, np.int64))
         notified = set()
-        if victims:
+        if victims and evicting is not None:
             for row in victims:
-                cqi, w = int(adm["adm_cq"][row]), int(adm_wl[row])
-                state[w] = QUEUED
-                last_gen[w] = -1
-                last_tried[int(ps_start[w]):int(ps_start[w + 1])] = -1
-                if has_qr is not None:
-                    has_qr[w] = 0
-                admit_cycle[w] = -1
+                w = int(adm_wl[row])
+                evicting[row] = True
+                adm["adm_evicted"][row] = 1
+                adm_finish[row] = min(t + int(lat[w]), NEVER)
                 evictions[w] += 1
-                cursor[seg_of[w]] = min(cursor[seg_of[w]], pos_of[w])
-                notified.add(cqi)
+        elif victims:
+            for row in victims:
+                w = int(adm_wl[row])
+                release(w)
+                evictions[w] += 1
+                notified.add(int(adm["adm_cq"][row]))
             remove_rows(victims)
         cyc += 1
         if not events:
@@ -835,6 +888,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     res.adm = dict(adm, **({"adm_wl": adm_wl} if replay else {}))
     if events:
         res.adm["adm_finish_ns"] = adm_finish
+    if evicting is not None:
+        res.adm["adm_evicting"] = evicting
     res.wl_admit_ns = admit_ns
     res.wl_finish_ns = finish_ns
     res.end_ns = t

@@ -290,6 +290,16 @@ def add_events(snap: abi.FlatSnapshot, seed: int = 0, present: float = 0.5, span
     return snap
 
 
+def add_evict_latency(snap: abi.FlatSnapshot, ns_range=(0, 0), seed: int = 0) -> abi.FlatSnapshot:
+    """Eviction latency of an event drain (include/kueue_b200.h) on a snapshot with `adm_wl`: every workload's time from
+    its eviction until its quota is released, seeded uniform in `ns_range` (inclusive; the pods' termination grace period
+    defaults to 30 s).  Adds no `adm_evict_end_ns`: rows evicted before the drain are issued when targeted."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    lo, hi = int(ns_range[0]), int(ns_range[1])
+    snap.set("wl_evict_ns", rng.integers(lo, hi + 1, snap.n_wl))
+    return snap
+
+
 # The reference's scheduler performance scenario (test/performance/scheduler/configs/baseline/generator.yaml, generated
 # by runner/generator/generator.go): 5 cohorts of 6 ClusterQueues, one flavor, cpu only; per ClusterQueue, workload k of
 # a class is created at (k + 1) * interval and runs `run` once admitted (runner/controller/controller.go).
@@ -303,11 +313,13 @@ PERF_NOMINAL_CPU, PERF_BORROW_CPU = 20, 100
 _MS = 1_000_000
 
 
-def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS) -> abi.FlatSnapshot:
+def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None = None) -> abi.FlatSnapshot:
     """The baseline scenario as numbers (15,000 workloads at scale 1; `scale` multiplies the count of every class):
     nominal 20 cpu and borrowingLimit 100 cpu per ClusterQueue, preemption reclaimWithinCohort Any and
     withinClusterQueue LowerPriority, BestEffortFIFO.  cpu is in milli-units.  wl_ts is the creation time, an empty
-    adm_wl turns eviction replay on, and `snap.perf_class` holds each workload's index into PERF_CLASSES.  One drain cycle takes cycle_ns of simulated time."""
+    adm_wl turns eviction replay on, and `snap.perf_class` holds each workload's index into PERF_CLASSES.  One drain cycle takes cycle_ns of simulated time.
+    evict_ns: the termination latency of every workload (wl_evict_ns: an eviction releases its quota that long after it
+    is issued); None = every eviction completes before the next cycle."""
     Q = PERF_COHORTS * PERF_CQS_PER_COHORT
     snap = abi.FlatSnapshot(n_cq=Q, n_cohort=PERF_COHORTS, n_flavor=1, n_resource=1)
     snap.set("parent", np.concatenate([Q + np.arange(Q) // PERF_CQS_PER_COHORT, np.full(PERF_COHORTS, -1)]))
@@ -333,6 +345,8 @@ def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS) -> abi.FlatSnapshot:
     snap.set("ps_req", np.asarray(cpu, np.int64)[:, None]); snap.set("ps_req_mask", np.ones(W)); snap.set("ps_count", np.ones(W))
     snap.set("wl_create_ns", create); snap.set("wl_run_ns", run)
     snap.set("adm_wl", np.zeros(0))
+    if evict_ns is not None:
+        snap.set("wl_evict_ns", np.full(W, evict_ns))
     snap.now_ns = 0
     snap.drain_cycle_ns = cycle_ns
     snap.finalize()

@@ -1,0 +1,78 @@
+"""kb_run_drain in event mode with eviction latency (kb_snapshot.wl_evict_ns), latency 0 against a latency longer than a
+cycle, on the reference's baseline scenario and on cfg4 with evictable admitted workloads, in one process.
+
+Four legs, alternated after a warm-up: the baseline scenario (synth.perf_scenario, 15,000 workloads, 1 ms cycles, run to
+the end) with every latency 0 and with a termination latency of --baseline-ms; cfg4 at full size with events
+(synth.add_events) with every latency 0 and with latencies drawn in [--cfg4-lo, --cfg4-hi] cycles (synth.
+add_evict_latency), over --max-cycles cycles.  Latency 0 gives the results of the drain without the table.  Per leg: device
+ms per cycle, cycles, evictions issued and completed, and the queue layer's share of the device time (KB_K_DRAIN, from one
+more run of each with per-kernel events).  Prints one JSON line with the card name and power limit read in the same call.
+
+    python tools/evict_latency_drain_bench.py [--reps 5] [--warmup 2] [--max-cycles 300]
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import statistics
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--max-cycles", type=int, default=300, help="cycles of the cfg4 legs (the baseline runs to the end)")
+    ap.add_argument("--baseline-ms", type=int, default=30, help="termination latency of the baseline scenario, ms")
+    ap.add_argument("--cfg4-lo", type=int, default=5, help="smallest cfg4 latency, in cycles")
+    ap.add_argument("--cfg4-hi", type=int, default=40, help="largest cfg4 latency, in cycles")
+    args = ap.parse_args()
+    from afs_drain_bench import card
+    from kueue_b200 import abi, native, synth
+    ms = 1_000_000
+
+    def cfg4(lo, hi):
+        snap = synth.add_events(synth.make_snapshot(4, evictable=True), seed=3)
+        step = snap.drain_cycle_ns
+        return synth.add_evict_latency(snap, (lo * step, hi * step), seed=4)
+    legs = {
+        "baseline_latency_0": (synth.perf_scenario(1.0, evict_ns=0), 1_000_000),
+        f"baseline_latency_{args.baseline_ms}ms": (synth.perf_scenario(1.0, evict_ns=args.baseline_ms * ms), 1_000_000),
+        "cfg4_latency_0": (cfg4(0, 0), args.max_cycles),
+        f"cfg4_latency_{args.cfg4_lo}_{args.cfg4_hi}_cycles": (cfg4(args.cfg4_lo, args.cfg4_hi), args.max_cycles),
+    }
+    ev = native.Evaluator(0)
+    outs = {k: abi.DrainOut(s, max_cycles=mc, trace=False) for k, (s, mc) in legs.items()}
+    for _ in range(args.warmup):
+        for k, (s, _) in legs.items():
+            ev.run_drain(s, outs[k])
+    per_cycle = {k: [] for k in legs}
+    for _ in range(args.reps):
+        for k, (s, _) in legs.items():
+            o = ev.run_drain(s, outs[k])
+            per_cycle[k].append(o.gpu_ms / max(1, o.n_cycles))
+    res = {"what": "kb_run_drain event mode, eviction latency 0 vs longer than a cycle", "card": card(), "reps": args.reps,
+           "warmup": args.warmup, "max_cycles_cfg4": args.max_cycles, "baseline_cycle_ms": 1,
+           "cfg4_cycle_ns": legs["cfg4_latency_0"][0].drain_cycle_ns}
+    ev.set_profile(True)
+    slot = abi.KERNEL_NAMES.index("k_drain")
+    for k, (s, _) in legs.items():
+        o = ev.run_drain(s, outs[k])
+        st = ev.stats()
+        res[k] = {"cycles": o.n_cycles, "admitted": o.n_admitted, "finished": o.n_finished, "evictions_issued": o.n_evicted,
+                  "evictions_completed": o.n_evict_done, "end_s": o.end_ns / 1e9,
+                  "ms_per_cycle_median": statistics.median(per_cycle[k]), "ms_per_cycle_min": min(per_cycle[k]),
+                  "ms_per_cycle_max": max(per_cycle[k]),
+                  "k_drain_share_profiled": st.kernel_ms[slot] / max(1e-9, o.gpu_ms)}
+    ev.set_profile(False)
+    ev.close()
+    print(json.dumps(res))
+
+
+if __name__ == "__main__":
+    main()
