@@ -227,8 +227,8 @@ typedef struct kb_snapshot {
      and AsApproximateFloat64 is value * Pow10(scale) (quantity.go:468-483; Pow10(-k) = 1 / 10^k).  Canonical choices:
      Go sums over a map in random order, the library sums in resource-index order; after penalties the reference's Pop
      (rebuildAll + heap.Fix per item in map order, cluster_queue.go:494-531) may return a workload that is not the
-     minimum, the library takes the true minimum of (usage, -priority, timestamp, UID) over the LocalQueue heads.  The
-     sticky workload is not modelled.  Every admitted workload of such a ClusterQueue adds its entry penalty to its
+     minimum, the library takes the true minimum of (usage, -priority, timestamp, UID) over the LocalQueue heads.  A
+     sticky workload is refused here (kb_snapshot.cq_sticky).  Every admitted workload of such a ClusterQueue adds its entry penalty to its
      LocalQueue (scheduler.go:727-742,946-960; pkg/util/admissionfairsharing/admission_fair_sharing.go):
        penalty_r += int64(float64(MilliValue(SumTotalRequests_r)) * afs_alpha)   (milli-units, truncated toward zero)
      over the workload's full TotalRequests (ps_req where ps_req_mask has bit r, before partial admission).
@@ -328,6 +328,21 @@ typedef struct kb_snapshot {
      with adm_evicted set. */
   const int64_t *wl_evict_ns;       /* [n_wl] time from the workload's eviction until its quota is released (>= 0)  */
   const int64_t *adm_evict_end_ns;  /* [n_adm] end of the eviction under way of a row with adm_evicted; NULL = none */
+
+  /* ---- sticky workload (optional; read by kb_run_drain only, kb_run_cycle ignores it: the caller picks the heads of a
+     single cycle) ----
+     In the reference a BestEffortFIFO ClusterQueue keeps a preemptor that waits for its evictions at its head
+     (stickyWorkload, pkg/cache/queue/cluster_queue.go:64-93; kueue#6929, kueue#7101): RequeueIfNotPresent (:609-619)
+     sets it to a workload requeued with RequeueReasonPendingPreemption, queueOrderingFunc (:656-665) orders it before
+     every other workload (after the AFS LocalQueue usage, before priority), and only delete (:330-340) clears it.
+     cq_sticky[q] is the pending index of ClusterQueue q's sticky workload at the start, -1 = none (the shim reads it
+     from the queue manager, INTEGRATION.md).  NULL = the rule is off and the drain is as without this block; non-NULL
+     turns it on in plain and event drains, and kb_drain_out.cq_sticky receives the slots after the drain.  See
+     kb_run_drain.  Errors: KB_ERR_INVALID for an index outside [-1, n_wl), wl_cq[cq_sticky[q]] != q, an index named by
+     adm_wl (a record that holds quota was deleted from its queue) or a record with wl_create_ns > now_ns;
+     KB_ERR_UNSUPPORTED for a sticky workload on a ClusterQueue with cq_afs set (in the reference that state needs a
+     preemption policy, which the AFS preemption guard refuses). */
+  const int32_t *cq_sticky;         /* [n_cq] */
 } kb_snapshot;
 
 /* ------------------------------------------------------------------------
@@ -516,10 +531,23 @@ int32_t kb_download(kb_handle *h, kb_cycle_out *out);
  * that table they are issued at t_c like any other row.  With every wl_evict_ns <= max(drain_cycle_ns, 1) and no
  * adm_evict_end_ns the drain equals the drain without latency (heads, decisions, evictions, usage, per-workload
  * results): every issued eviction completes at the next boundary, and steps 5-7 do not depend on their order.
- * Not modelled: the sticky workload (cluster_queue.go:64-93,609-624,656-665), which in the reference keeps a preemptor
- * that waits for its evictions at the head of its queue; here every waiting preemptor is ordered again each cycle and
- * re-runs its target search.  Nor are preemption expectations between issue and observation (the drain observes an
- * eviction at once). */
+ *
+ * Sticky workload (kb_snapshot.cq_sticky != NULL; plain and event drains): one slot per ClusterQueue, seeded from the
+ * table, as the reference keeps a preemptor that waits for its evictions at the head of its queue
+ * (cluster_queue.go:64-93,330-340,609-624,656-665):
+ *   - heads (step 4 / 8): a ClusterQueue whose sticky workload is queued takes it as its head; otherwise the head is its
+ *     first queued workload.  A set-aside sticky workload has no effect and is first again once requeued;
+ *   - after the decisions (step 1): an assumed head that is its ClusterQueue's sticky workload clears the slot (admission
+ *     deletes the workload from its queue, workload_controller.go:965-966); a Preempting head of a BestEffortFIFO
+ *     ClusterQueue becomes the sticky workload (scheduler.go:344-358: targets already evicting count,
+ *     preemption.go:183-194), replacing the previous one; every other decision leaves the slot alone, a sticky head
+ *     that goes NoFit and is set aside included;
+ *   - arrivals, completions, releases and the inadmissible requeue only change state bytes.  The head may lie past the
+ *     first queued workload: it is set aside from its own position, and the scheduling-hash move excludes it by identity.
+ * With every slot -1 at the start the drain equals the drain without the table when (a) there is no adm_wl and no event
+ * table (nothing ahead of a Preempting head ever becomes queued again), (b) every ClusterQueue is StrictFIFO, or (c) no
+ * ClusterQueue has a preemption policy.
+ * Not modelled: preemption expectations between issue and observation (the drain observes an eviction at once). */
 typedef struct kb_drain_out {
   int32_t max_cycles;        /* in */
   int32_t n_cycles;          /* out: cycles run */
@@ -562,6 +590,9 @@ typedef struct kb_drain_out {
   /* eviction latency (kb_snapshot.wl_evict_ns != NULL; zero / untouched otherwise; the pointer may be NULL) */
   int64_t n_evict_done;       /* out: evictions completed (quota released), those before cycle 0 included */
   int32_t *cycle_evict_done;  /* [max_cycles] evictions completed from the start of cycle c to the start of c+1 */
+  /* sticky workload (kb_snapshot.cq_sticky != NULL; untouched otherwise; the pointer may be NULL): the slots after the
+     drain, for the caller to write back */
+  int32_t *cq_sticky;         /* [n_cq] pending index of each ClusterQueue's sticky workload, -1 = none */
 } kb_drain_out;
 int32_t kb_run_drain(kb_handle *h, const kb_snapshot *s, kb_drain_out *out);
 

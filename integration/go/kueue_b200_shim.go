@@ -364,6 +364,9 @@ func (s *Scheduler) flatten(snap *schdcache.Snapshot, heads []workload.Info, gen
 	// With eviction replay it may also fill each workload's eviction latency (until its pods are gone) and, for the
 	// admitted workloads already evicted, the time their quota is released (read where adm_evicted is set):
 	//   c.wl_evict_ns, c.adm_evict_end_ns = cp64(wlEvict), cp64(admEvictEnd)
+	// The sticky workload of every ClusterQueue (INTEGRATION.md) comes from an accessor in pkg/cache/queue, since the
+	// field sw is unexported, mapped to its pending index (-1 = none):
+	//   c.cq_sticky = cp32(cqSticky)   // after kb_run_drain, kb_drain_out.cq_sticky is written back through a setter
 	// They stay nil here: a single cycle ignores them.
 	if anyGroup { // optional table: NULL when no podset is grouped
 		c.ps_group = cp32(psGroup)

@@ -83,6 +83,7 @@ class kb_snapshot(C.Structure):
         ("afs_half_life_ns", C.c_int64), ("afs_sampling_ns", C.c_int64), ("lq_last_update_ns", _P(C.c_int64)),
         ("adm_lq", _P(C.c_int32)),
         ("wl_evict_ns", _P(C.c_int64)), ("adm_evict_end_ns", _P(C.c_int64)),
+        ("cq_sticky", _P(C.c_int32)),
     ]
 
 
@@ -133,6 +134,7 @@ class kb_drain_out(C.Structure):
         ("lq_consumed", _P(C.c_int64)), ("lq_consumed_scale", _P(C.c_int32)), ("lq_last_update_ns", _P(C.c_int64)),
         ("n_afs_samples", C.c_int64),
         ("n_evict_done", C.c_int64), ("cycle_evict_done", _P(C.c_int32)),
+        ("cq_sticky", _P(C.c_int32)),
     ]
 
 
@@ -188,6 +190,7 @@ _DT = {
     "wl_create_ns": np.int64, "wl_run_ns": np.int64, "adm_finish_ns": np.int64,
     "lq_last_update_ns": np.int64, "adm_lq": np.int32,
     "wl_evict_ns": np.int64, "adm_evict_end_ns": np.int64,
+    "cq_sticky": np.int32,
 }
 # AdmissionFairSharing tables (include/kueue_b200.h): wl_lq absent = AFS off
 AFS_FIELDS = ("wl_lq", "lq_cq", "cq_afs", "lq_weight", "lq_consumed", "lq_consumed_scale", "lq_penalty", "afs_res_weight",
@@ -198,8 +201,10 @@ EVENT_FIELDS = ("wl_create_ns", "wl_run_ns", "adm_finish_ns", "wl_evict_ns")
 AFS_DECAY_FIELDS = ("lq_last_update_ns", "adm_lq")
 # end times of the evictions under way before an event drain with wl_evict_ns (include/kueue_b200.h): absent = none known
 EVICT_END_FIELDS = ("adm_evict_end_ns",)
+# the sticky workload of every ClusterQueue at the start of a drain (include/kueue_b200.h): absent = the rule is off
+STICKY_FIELDS = ("cq_sticky",)
 OPTIONAL_FIELDS = (("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows", "adm_wl") + AFS_FIELDS +
-                   EVENT_FIELDS + AFS_DECAY_FIELDS + EVICT_END_FIELDS)  # NULL in kb_snapshot when absent
+                   EVENT_FIELDS + AFS_DECAY_FIELDS + EVICT_END_FIELDS + STICKY_FIELDS)  # NULL in kb_snapshot when absent
 ARRAY_FIELDS = list(_DT.keys())
 # tables the library keeps resident while kb_snapshot.static_generation is unchanged (include/kueue_b200.h)
 STATIC_FIELDS = ("parent", "fair_weight", "nominal", "borrow_limit", "lend_limit", "cq_within_cq", "cq_reclaim_within",
@@ -431,6 +436,7 @@ class DrainOut:
         self.lq_consumed = np.zeros((max(1, L), R), np.int64)[:L]  # decay of consumed usage: the entries after the drain
         self.lq_consumed_scale = np.zeros((max(1, L), R), np.int32)[:L]
         self.lq_last_update_ns = np.zeros(max(1, L), np.int64)[:L]
+        self.cq_sticky = np.full(max(1, Q), -1, np.int32)[:Q]  # the sticky slots after the drain (with kb_snapshot.cq_sticky)
         cap = (min(W * 4 + Q, min(Q, W) * max_cycles) if trace_capacity is None else trace_capacity) if trace else 0
         self.trace_wl = np.zeros(max(1, cap), np.int32)
         self.trace_decision = np.zeros(max(1, cap), np.uint8)
@@ -448,6 +454,7 @@ class DrainOut:
         s.wl_admit_ns = _ptr(self.wl_admit_ns, C.c_int64); s.wl_finish_ns = _ptr(self.wl_finish_ns, C.c_int64)
         s.lq_consumed = _ptr(self.lq_consumed, C.c_int64); s.lq_consumed_scale = _ptr(self.lq_consumed_scale, C.c_int32)
         s.lq_last_update_ns = _ptr(self.lq_last_update_ns, C.c_int64)
+        s.cq_sticky = _ptr(self.cq_sticky, C.c_int32)
         if trace:
             s.trace_wl = _ptr(self.trace_wl, C.c_int32); s.trace_decision = _ptr(self.trace_decision, C.c_uint8)
         s.trace_capacity = cap

@@ -1421,6 +1421,23 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       if (l >= 0 && s->lq_cq[l] != s->adm_cq[a]) return fail(h, KB_ERR_INVALID, "afs decay: the LocalQueue of an admitted row feeds another ClusterQueue");
     }
   }
+  // ---- sticky workload: host-side checks of cq_sticky (include/kueue_b200.h)
+  const bool sticky = s->cq_sticky != nullptr;
+  if (sticky) {
+    std::vector<uint8_t> held((size_t)std::max(1, W), 0);
+    if (replay) for (int a = 0; a < s->n_adm; a++) held[s->adm_wl[a]] = 1;
+    for (int q = 0; q < Q; q++) {
+      const int w = s->cq_sticky[q];
+      if (w < -1 || w >= W) return fail(h, KB_ERR_INVALID, "cq_sticky out of range");
+      if (w < 0) continue;
+      if (s->wl_cq[w] != q) return fail(h, KB_ERR_INVALID, "cq_sticky: the workload is not in the ClusterQueue's queue");
+      if (held[w]) return fail(h, KB_ERR_INVALID, "cq_sticky names a record that holds quota (adm_wl): admission deleted it from its queue");
+      if (s->wl_create_ns && s->wl_create_ns[w] > s->now_ns) return fail(h, KB_ERR_INVALID, "cq_sticky names a record created after now_ns");
+      if (s->wl_lq && s->cq_afs && s->cq_afs[q])
+        return fail(h, KB_ERR_UNSUPPORTED, "cq_sticky: a sticky workload on a ClusterQueue with AdmissionFairSharing");
+    }
+    if (out->cq_sticky) memcpy(out->cq_sticky, s->cq_sticky, (size_t)Q * 4);  // the slots of a drain that runs no cycle
+  }
   out->n_afs_samples = 0;
   if (Hcap == 0 || max_cycles == 0) return KB_OK;
   size_t extra = (size_t)std::min<long long>((long long)W, (long long)Hcap * max_cycles);
@@ -1517,7 +1534,10 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (replay || events) {
       X.adm_wl = a.take<int32_t>(Acap);
       X.wl_seg = a.take<int32_t>(Wz); X.wl_pos = a.take<int32_t>(Wz); X.wl_evictions = a.take<int32_t>(Wz);
+    } else if (sticky) {  // the sticky head's position
+      X.wl_seg = a.take<int32_t>(Wz); X.wl_pos = a.take<int32_t>(Wz);
     }
+    if (sticky) X.cq_sticky = a.take<int32_t>((size_t)Q);
     if (compact) {
       X.adm_dead = a.take<int32_t>(Acap); other.wl = a.take<int32_t>(Acap); X.root_mark = a.take<int32_t>(nR);
       X.row_live = a.take<int32_t>(Acap + 1); X.row_cells = a.take<int32_t>(Acap + 1);
@@ -1623,6 +1643,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     X.alpha = s->afs_alpha;
     X.n_afs_cq = (int)afs_cqs.size();
   }
+  if (sticky) CUDA_TRY(h, h2d(h, X.cq_sticky, s->cq_sticky, (size_t)Q * 4));
   std::vector<i64> lq_adm;  // decay: the initial admitted usage of every LocalQueue (live rows of the snapshot)
   if (decay) {
     lq_adm.assign(LR, 0);
@@ -1660,7 +1681,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   k_scan_i32<<<1, 1024, 0, h->stream>>>(q_count, X.q_start, S);
   k_drain_init<<<std::max(nbW, (S + tb - 1) / tb), tb, 0, h->stream>>>(D, X, S);
   if (events) k_drain_init_events<<<std::max(1, nbW), tb, 0, h->stream>>>(D, X, create, s->now_ns);
-  if (replay || events) k_drain_init_replay<<<std::max(nbW, (s->n_adm + tb - 1) / tb), tb, 0, h->stream>>>(D, X, replay ? s->n_adm : 0);
+  if (replay || events || sticky) k_drain_init_replay<<<std::max(nbW, (s->n_adm + tb - 1) / tb), tb, 0, h->stream>>>(D, X, replay ? s->n_adm : 0);
   k_drain_advance<<<(S + tb - 1) / tb, tb, 0, h->stream>>>(X, S);
   const int nbL = std::max(1, (L + tb - 1) / tb);
   if (decay) {  // the samples due at or before now_ns (k_drain_init_events set clock[0] = now_ns), before the first heads
@@ -1828,6 +1849,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (replay) CUDA_TRY(h, cudaMemcpyAsync(out->wl_evictions, X.wl_evictions, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
     else memset(out->wl_evictions, 0, Wz * 4);
   }
+  if (sticky && out->cq_sticky) CUDA_TRY(h, cudaMemcpyAsync(out->cq_sticky, X.cq_sticky, (size_t)Q * 4, cudaMemcpyDeviceToHost, h->stream));
   if (out->ps_flavor && PR) CUDA_TRY(h, cudaMemcpyAsync(out->ps_flavor, D.ps_flavor, PR, cudaMemcpyDeviceToHost, h->stream));
   if (out->ps_count && D.P) CUDA_TRY(h, cudaMemcpyAsync(out->ps_count, D.ps_count_out, (size_t)D.P * 4, cudaMemcpyDeviceToHost, h->stream));
   if (out->cq_usage) CUDA_TRY(h, cudaMemcpyAsync(out->cq_usage, D.cq_usage, (size_t)Q * FR * 8, cudaMemcpyDeviceToHost, h->stream));

@@ -43,6 +43,13 @@
 // bytes of the queues it visits.  With eviction latency (wl_evict_ns) k_drain_evict only issues: it sets adm_evicted and
 // the byte column adm_evicting (carried by the compaction) and writes the end time into the finish column, so E and the
 // compaction see it unchanged; k_drain_finish releases the row at its end time through the replay's requeue path.
+//
+// Sticky workload (kb_snapshot.cq_sticky; include/kueue_b200.h): one slot per ClusterQueue.  k_drain_heads takes a QUEUED
+// sticky workload as the head instead of the one at the cursor, so the head may lie past the cursor: k_drain_apply moves
+// the queue from the head's own position (wl_pos), excludes the head from the scheduling-hash move by identity, and sets
+// (a Preempting head of a BestEffortFIFO ClusterQueue) or clears (its admission) the slot.  One head per ClusterQueue per
+// cycle: one writer per slot.  Never set on an AFS ClusterQueue (refused, and no preemption there), so k_drain_afs_heads
+// does not read it.
 #pragma once
 
 #include <cub/device/device_scan.cuh>
@@ -218,6 +225,8 @@ struct DrainDev {
   // eviction latency (event mode); wl_evict == nullptr: off
   const i64 *wl_evict;             // [W] time from a workload's eviction until its quota is released
   uint8_t *adm_evicting;           // [A_cap] 1 while the row's eviction is under way (current half); its end is adm_finish
+  // sticky workload; cq_sticky == nullptr: off
+  int32_t *cq_sticky;              // [Q] pending index of each ClusterQueue's sticky workload, -1 = none
 };
 // counters of a boundary: [1] evictions (issued, with latency), [2] / [3] rows / cells after the compaction, [4]
 // evictions completed (latency), [5] capacity flag; event mode: [6] completions, [7] arrivals, [8] end flag, [9] / [10]
@@ -330,7 +339,12 @@ __global__ void k_drain_afs_heads(DevSnap D, DrainDev X) {
 __global__ void k_drain_heads(DevSnap D, DrainDev X, int32_t *heads) {
   int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= D.Q) return;
-  if (X.flag[q]) { int s = X.head_seg ? X.head_seg[q] : q; heads[X.pos[q]] = X.q_order[X.q_start[s] + X.cursor[s]]; }
+  if (X.flag[q]) {  // a queued sticky workload implies cursor < length: the flag is set
+    int s = X.head_seg ? X.head_seg[q] : q;
+    int w = X.q_order[X.q_start[s] + X.cursor[s]];
+    if (X.cq_sticky) { const int sw = X.cq_sticky[q]; if (sw >= 0 && X.wl_state[sw] == KB_WS_QUEUED) w = sw; }
+    heads[X.pos[q]] = w;
+  }
   if (q == 0) X.counters[0] = X.pos[D.Q];
 }
 
@@ -381,23 +395,27 @@ __global__ void k_drain_apply(DevSnap D, DrainDev X) {
   X.e_assumed[e] = ok; X.e_ncells[e] = ncell;
   // ---- queue movement (cluster_queue.go:362-425,609-633)
   const bool strict = D.cq_strategy[cq] == KB_QUEUE_STRICT_FIFO;
+  if (X.cq_sticky) {  // delete (cluster_queue.go:330-340) on admission; RequeueIfNotPresent with PendingPreemption (:609-619)
+    if (ok) { if (X.cq_sticky[cq] == wl) X.cq_sticky[cq] = -1; }
+    else if (dec == KB_DEC_PREEMPTING && !strict) X.cq_sticky[cq] = wl;
+  }
   const bool inadmissible = (dec == KB_DEC_NOFIT || dec == KB_DEC_PREEMPT_NO_TARGETS) && !pending_flavors;
   const int hs = X.head_seg ? X.head_seg[cq] : cq, s0 = drain_seg0(X, cq), s1 = drain_seg1(X, cq);
+  const int hp = X.cq_sticky ? X.wl_pos[wl] : X.cursor[hs];  // the head's position: a sticky head may lie past the cursor
   const bool bulk = dec == KB_DEC_NOFIT && !strict && D.wl_sched_hash && D.wl_sched_hash[wl] != 0;
-  if (bulk) {  // handleInadmissibleHash :408-425: every queued workload of the class, in every segment of the queue
+  if (bulk) {  // handleInadmissibleHash :408-425: every queued workload of the class but the head, in every segment
     const i64 hsh = D.wl_sched_hash[wl];
     if (X.class_nofit) X.class_nofit[X.wl_class[wl]] = 1;  // noFitSchedulingHashes.Insert (:414)
     for (int s = s0; s < s1; s++) {
       const int qs = X.q_start[s], qn = X.q_start[s + 1] - qs;
-      for (int p = X.cursor[s] + (s == hs); p < qn; p++) {
+      for (int p = X.cursor[s]; p < qn; p++) {
         const int w2 = X.q_order[qs + p];
-        if (D.wl_sched_hash[w2] == hsh && X.wl_state[w2] == KB_WS_QUEUED) { X.wl_state[w2] = KB_WS_SET_ASIDE; X.first_aside[s] = min(X.first_aside[s], p); }
+        if (w2 != wl && D.wl_sched_hash[w2] == hsh && X.wl_state[w2] == KB_WS_QUEUED) { X.wl_state[w2] = KB_WS_SET_ASIDE; X.first_aside[s] = min(X.first_aside[s], p); }
       }
     }
   }
-  if (inadmissible && !strict) { X.wl_state[wl] = KB_WS_SET_ASIDE; X.first_aside[hs] = min(X.first_aside[hs], X.cursor[hs]); }
-  if (ok || (inadmissible && !strict)) X.cursor[hs]++;
-  for (int s = s0; s < s1; s++) {
+  if (inadmissible && !strict) { X.wl_state[wl] = KB_WS_SET_ASIDE; X.first_aside[hs] = min(X.first_aside[hs], hp); }
+  for (int s = s0; s < s1; s++) {  // the cursor past the workloads that left the queue, the head among them
     if (s != hs && !bulk) continue;
     const int qs = X.q_start[s], qn = X.q_start[s + 1] - qs;
     int cur = X.cursor[s];

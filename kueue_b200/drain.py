@@ -49,9 +49,10 @@ cycle c completes before cycle c+1.  After cycle c, in this order:
 AdmissionFairSharing (the snapshot carries `wl_lq` and the LocalQueue tables, include/kueue_b200.h): the queue of a
 ClusterQueue with `cq_afs` set is one segment per LocalQueue, each in the static order above with its own cursor.
   * the head is the minimum of (LocalQueue usage by cmp.Compare, -priority, timestamp, UID) over the segment heads
-    (queueOrderingFunc with enableAdmissionFs, cluster_queue.go:636-685; the sticky workload is not modelled).  After
-    penalties the reference's Pop re-heapifies in map order (rebuildAll, cluster_queue.go:494-531; heap.go:115-123,
-    166-172) and may return a workload that is not the minimum: the true minimum is this definition's canonical rule;
+    (queueOrderingFunc with enableAdmissionFs, cluster_queue.go:636-685; kb_run_drain refuses a sticky workload here,
+    and without preemption none arises).  After penalties the reference's Pop re-heapifies in map order (rebuildAll,
+    cluster_queue.go:494-531; heap.go:115-123, 166-172) and may return a workload that is not the minimum: the true
+    minimum is this definition's canonical rule;
   * LocalQueue usage is `lq_usage` (Info.CalcLocalQueueFSUsage, workload.go:391-427), summed in resource-index order
     (the reference sums over a map, in random order: resource-index order is the canonical choice);
   * every admission adds its entry penalty to its LocalQueue (`entry_penalty`; scheduler.go:727-742,946-960) before
@@ -132,6 +133,28 @@ Canonical choices: samples do not wake the clock (a quiet cycle still waits for 
 early resample while penalties are pending (HasPendingFor, localqueue_controller.go:219) is not modelled; 0.5^x is
 `half_pow`, the library's afs_half_pow (kb_drain.cuh) restated operation for operation, not Go's platform-dependent
 math.Pow.  A drain that runs no cycle takes no sample.
+
+The sticky workload (the snapshot carries `cq_sticky`, include/kueue_b200.h).  In the reference a BestEffortFIFO
+ClusterQueue keeps a preemptor that waits for its evictions at its head (stickyWorkload, cluster_queue.go:64-93; kueue#6929,
+kueue#7101): RequeueIfNotPresent (:609-619) sets `sw` to a workload requeued with RequeueReasonPendingPreemption (the
+entry issued preemptions, scheduler.go:344-358; targets already evicting count, preemption.go:183-194), queueOrderingFunc
+(:656-665) orders it first after the AFS LocalQueue usage and before priority, and only `delete` (:330-340) clears it,
+which for a drain is the admission (Pending -> QuotaReserved calls queues.DeleteWorkload, workload_controller.go:965-966).
+One slot per ClusterQueue, -1 = none, seeded from the table:
+  1. heads (step 8): a ClusterQueue whose sticky workload is QUEUED takes it as its head; otherwise the head is the first
+     QUEUED workload as above.  A SET_ASIDE sticky workload has no effect and is first again once it is requeued (`sw`
+     survives the inadmissible set: fair_sharing_test.go:866);
+  2. after the decisions (step 1): an ASSUMED head that is its ClusterQueue's sticky workload clears the slot; a
+     Preempting head of a BestEffortFIFO ClusterQueue becomes the sticky workload (one value per ClusterQueue: a new one
+     replaces the old); every other decision leaves the slot alone, a sticky head that goes NoFit and is set aside too;
+  3. arrivals, completions, releases and the inadmissible requeue only change state bytes: steps 5-7 stay
+     order-independent.
+The head may lie past the cursor, so queue movement uses the head's own position: set-aside and first_aside use it, the
+cursor moves only by the advance loop, and the scheduling-hash bulk move excludes the head by identity (the popped head
+is not in the heap; the workload at the cursor is an ordinary queued one).  With every slot -1 at the start the drain
+equals the drain without the table when (a) there is no `adm_wl` and no event table (nothing before a Preempting head
+ever becomes queued again), (b) every ClusterQueue is StrictFIFO, or (c) no ClusterQueue has a preemption policy.
+Preemption expectations are not modelled: the drain observes an eviction at once.
 """
 from __future__ import annotations
 
@@ -174,6 +197,9 @@ class DrainResult:
     lq_consumed_scale: np.ndarray | None = None                # [n_lq][R] their scales
     lq_last_update_ns: np.ndarray | None = None                # [n_lq] LastUpdate
     n_afs_samples: int = 0                                     # samples due over the drain (fixed-point skips included)
+    # sticky workload (cq_sticky in the snapshot; None / empty otherwise)
+    cq_sticky: np.ndarray | None = None                        # [n_cq] the slots after the drain, -1 = none
+    sticky_heads: List[np.ndarray] = field(default_factory=list)  # per cycle: heads the rule chose over the first queued
 
     @property
     def n_evicted(self) -> int:
@@ -484,6 +510,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 adm_finish[evicting] = a["adm_evict_end_ns"][evicting]
     if replay:
         state[a["adm_wl"].astype(np.int64)] = HELD  # holds quota: out of every queue
+    sticky = a["cq_sticky"].astype(np.int64).copy() if "cq_sticky" in a else None  # sticky workload per ClusterQueue
     cursor = np.zeros(len(qlen), np.int64)
     first_aside = qlen.copy()                                     # smallest SET_ASIDE position per segment (qlen = none)
     nofit = NoFitSets()
@@ -573,7 +600,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     finish_ns = np.full(snap.n_wl, NEVER, np.int64)
     root = root_of(a["parent"])
     static = {k: v for k, v in a.items() if not (k.startswith(("wl_", "ps_", "adm_")) or k in ("heads", "cq_usage") + abi.AFS_FIELDS +
-                                                                                               abi.AFS_DECAY_FIELDS)}
+                                                                                               abi.AFS_DECAY_FIELDS +
+                                                                                               abi.STICKY_FIELDS)}
     covers_pods = np.zeros(Q, bool)
     if snap.pods_resource >= 0:
         for q in range(Q):
@@ -708,6 +736,13 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             continue
         segs = hseg[live]
         heads = order[qstart[segs] + cursor[segs]]  # global pending indices, one per ClusterQueue with work left
+        chosen = []
+        if sticky is not None:  # a queued sticky workload is its ClusterQueue's head
+            for e, q in enumerate(live):
+                w = int(sticky[q])
+                if w >= 0 and state[w] == QUEUED and w != heads[e]:
+                    heads[e] = w
+                    chosen.append(w)
         cs = abi.FlatSnapshot(n_cq=Q, n_cohort=snap.n_cohort, n_flavor=snap.n_flavor, n_resource=R, pods_resource=snap.pods_resource,
                               flags=snap.flags, now_ns=t, static_generation=snap.static_generation)
         cs.arrays.update(static)
@@ -732,6 +767,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         dec = np.asarray(out.decision).copy()
         res.cycles += 1
         res.heads.append(heads); res.decisions.append(dec)
+        res.sticky_heads.append(np.asarray(chosen, np.int64))
         res.cycle_start_ns.append(t)
         res.finished.append(np.zeros(0, np.int64)); res.arrived.append(np.zeros(0, np.int64)); res.evict_done.append(np.zeros(0, np.int64))
         ok = dec == abi.DEC_ASSUMED
@@ -821,6 +857,13 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             inadmissible[e] = requeue_goes_inadmissible(False, requeue_reason(int(dec[e])), last)
             if inadmissible[e] and not strict[cqs[e]]:
                 set_aside(w)
+        if sticky is not None:  # admission deletes the sticky workload, a BestEffortFIFO preemptor becomes it
+            for e in range(len(heads)):
+                q, w = int(cqs[e]), int(heads[e])
+                if ok[e] and sticky[q] == w:
+                    sticky[q] = -1
+                elif dec[e] == abi.DEC_PREEMPTING and not strict[q]:
+                    sticky[q] = w
         if shash is not None:
             for e in np.flatnonzero((dec == abi.DEC_NOFIT) & ~strict[cqs]):
                 hsh = int(shash[heads[e]])
@@ -828,9 +871,9 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                     continue
                 q = int(cqs[e])
                 nofit.insert(q, hsh)
-                for s in range(int(seg_start[q]), int(seg_start[q + 1])):  # every queued workload of the class, every segment
-                    rest = order[qstart[s] + cursor[s] + (s == segs[e]):qstart[s + 1]]
-                    for w in rest[(shash[rest] == hsh) & (state[rest] == QUEUED)]:
+                for s in range(int(seg_start[q]), int(seg_start[q + 1])):  # every queued workload of the class but the head
+                    rest = order[qstart[s] + cursor[s]:qstart[s + 1]]
+                    for w in rest[(shash[rest] == hsh) & (state[rest] == QUEUED) & (rest != heads[e])]:
                         set_aside(int(w))
         for q in cqs:  # the next head is the first queued workload
             for s in range(int(seg_start[q]), int(seg_start[q + 1])):
@@ -893,6 +936,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     res.wl_admit_ns = admit_ns
     res.wl_finish_ns = finish_ns
     res.end_ns = t
+    res.cq_sticky = sticky
     if decay:
         res.lq_consumed = consumed.astype(np.int64)
         res.lq_consumed_scale = cscale.astype(np.int32)

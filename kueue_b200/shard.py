@@ -127,6 +127,9 @@ def shard(snap: abi.FlatSnapshot, rank: int, world: int, node_rank: np.ndarray |
     out.set("adm_use_fr", a["adm_use_fr"][ui]); out.set("adm_use_qty", a["adm_use_qty"][ui])
     if "adm_wl" in a:  # eviction replay: a record lives with its ClusterQueue, as does its admitted row
         out.set("adm_wl", wl_remap[a["adm_wl"][adms]])
+    if "cq_sticky" in a:  # the sticky workload of a ClusterQueue is one of its records
+        sw = a["cq_sticky"][cqs].astype(np.int64)
+        out.set("cq_sticky", np.where(sw >= 0, wl_remap[np.maximum(sw, 0)], -1))
     if "wl_lq" in a:  # AdmissionFairSharing: the LocalQueues travel with their ClusterQueues (still ClusterQueue-major)
         L = len(a["lq_cq"])
         lqs = np.flatnonzero(node_rank[a["lq_cq"]] == rank) if L else np.zeros(0, np.int64)
