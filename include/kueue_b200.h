@@ -343,6 +343,34 @@ typedef struct kb_snapshot {
      KB_ERR_UNSUPPORTED for a sticky workload on a ClusterQueue with cq_afs set (in the reference that state needs a
      preemption policy, which the AFS preemption guard refuses). */
   const int32_t *cq_sticky;         /* [n_cq] */
+
+  /* ---- admission checks (optional; read by kb_run_drain only, kb_run_cycle ignores them) ----
+     In the reference a workload whose ClusterQueue has admission checks (ProvisioningRequest: the autoscaler has to
+     find nodes) reserves quota first and becomes Admitted once every check is Ready (SyncAdmittedCondition,
+     admissionchecks.go:36-70); the run clock starts at Admitted (the performance runner, controller.go:62-72,131).  A
+     failing attempt n goes to Retry while n <= BackoffLimitCount and to Rejected otherwise (provisioning controller.go:
+     536-580).  Retry evicts (reason AdmissionCheck), releases the quota and requeues the workload once RequeueAt = verdict
+     + WaitTime(n) has passed (workload_controller.go:330-375,650-678); while it waits its queue-order timestamp is the
+     eviction time (GetQueueOrderTimestamp, workload.go:1180-1182).  Rejected deactivates the workload.  wl_check_ns ==
+     NULL: off, and every launch, copy and result of the drain stays as without this block.  A non-NULL wl_check_ns turns
+     on event mode.  With the tables wl_ts is the creation timestamp.  See kb_run_drain.  Errors: KB_ERR_INVALID for any
+     table of this block without adm_wl or without wl_check_ns, wl_check_ns[w] < 0, wl_check_fail[w] < 0,
+     wl_check_retries[w] < 0, adm_check_end_ns[a] <= now_ns on a row (INT64_MIN excepted), wl_requeue_at_ns on a record
+     named by adm_wl or created after now_ns, a row with a check under way that also has an eviction under way (adm_evicted
+     with adm_evict_end_ns), check_backoff_base_s <= 0, check_backoff_max_s < 0, check_backoff_limit < 0;
+     KB_ERR_UNSUPPORTED when the longest WaitTime of attempts 1..limit (see kb_run_drain) is 10,000 s or more (the
+     reference's jitter makes it random there) and for the tables together with lq_last_update_ns (a workload with
+     checks never makes the Pending -> Admitted transition that updates consumed usage, workload_controller.go:965-972). */
+  const int64_t *wl_check_ns;       /* [n_wl] time from a quota reservation to that attempt's verdict; 0 = Ready at once */
+  const int32_t *wl_check_fail;     /* [n_wl] how many next attempts fail before one is Ready; INT32_MAX = all; NULL = 0  */
+  const int32_t *wl_check_retries;  /* [n_wl] Status.AdmissionChecks[*].RetryCount at the start; NULL = 0              */
+  const int64_t *wl_check_evict_ns; /* [n_wl] Evicted LastTransitionTime of a record last evicted by an admission check;
+                                       INT64_MIN = not; read for records adm_wl does not name; NULL = none             */
+  const int64_t *wl_requeue_at_ns;  /* [n_wl] Status.RequeueState.RequeueAt of a record in check backoff; INT64_MIN = none */
+  const int64_t *adm_check_end_ns;  /* [n_adm] verdict time of the attempt under way; INT64_MIN = the row is Admitted   */
+  int32_t check_backoff_base_s;     /* RetryStrategy.BackoffBaseSeconds (> 0)                                            */
+  int32_t check_backoff_max_s;      /* RetryStrategy.BackoffMaxSeconds (0 = no cap)                                      */
+  int32_t check_backoff_limit;      /* RetryStrategy.BackoffLimitCount (>= 0)                                            */
 } kb_snapshot;
 
 /* ------------------------------------------------------------------------
@@ -547,7 +575,31 @@ int32_t kb_download(kb_handle *h, kb_cycle_out *out);
  * With every slot -1 at the start the drain equals the drain without the table when (a) there is no adm_wl and no event
  * table (nothing ahead of a Preempting head ever becomes queued again), (b) every ClusterQueue is StrictFIFO, or (c) no
  * ClusterQueue has a preemption policy.
- * Not modelled: preemption expectations between issue and observation (the drain observes an eviction at once). */
+ * Not modelled: preemption expectations between issue and observation (the drain observes an eviction at once).
+ *
+ * Admission checks (kb_snapshot.wl_check_ns != NULL, with adm_wl; event mode).  Two more queue states: BACKOFF and
+ * DEACTIVATED.  Each record has a queue-order timestamp: wl_check_evict_ns when set (records adm_wl does not name),
+ * else wl_ts.  Additions to the loop above:
+ *   1. an admission at t_c of a workload with wl_check_ns > 0 reserves quota and starts attempt k = RetryCount + 1; its
+ *      verdict comes at t_c + wl_check_ns (saturating).  With 0 the row is Ready at t_c, as without the tables;
+ *   2. verdicts are events (E includes them), applied in step 5 before the completions.  Ready (no failure left):
+ *      wl_ready_ns = verdict, finish = verdict + wl_run_ns (saturating), the row may finish in the same boundary.
+ *      Retry (a failing attempt, k <= check_backoff_limit): the row's cells leave the usage, the row is removed, its
+ *      root tree is marked; the record goes to BACKOFF with RequeueAt = verdict + WaitTime(k), RetryCount = k, queue
+ *      timestamp = verdict and LastAssignment nil.  Rejected (k > limit): released the same way, the record is
+ *      DEACTIVATED and never queued again.  A failing attempt uses up one unit of wl_check_fail;
+ *   3. a BACKOFF record whose RequeueAt <= t_{c+1} arrives through step 6 (NoFit rule included); E includes RequeueAt;
+ *   4. an admission resets the queue timestamp to wl_ts; the new row's adm_ts is wl_ts;
+ *   5. a preempted row whose checks run holds no pods: with wl_evict_ns it is released at the next boundary; the
+ *      attempt under way is dropped, not counted and uses up no failure (a canonical choice);
+ *   6. the cycle sees the queue timestamp (entry order, preemption policy), and the queues are re-sorted by it whenever a
+ *      record enters its queue with a timestamp other than the key of its position (n_resorts);
+ *   7. with every wl_check_ns = 0, every wl_check_fail = 0 and no start-state tables the drain equals the drain without
+ *      the tables.
+ * WaitTime(k) is wait.NewBackoff(base, max, 2, 0.0001).WaitTime(k) truncated to whole seconds (kb_drain.cuh
+ * kb_check_wait_ns; exact below 10,000 s): min(check_backoff_base_s * 2^(k-1), check_backoff_max_s or infinity), except
+ * that with base > max > 0 the first Step returns the base uncapped (attempt 1 waits base, later ones max).  Verdicts
+ * applied between the start of cycle c and of c+1 count in cycle_check_retry / cycle_check_rejected[c]. */
 typedef struct kb_drain_out {
   int32_t max_cycles;        /* in */
   int32_t n_cycles;          /* out: cycles run */
@@ -593,6 +645,15 @@ typedef struct kb_drain_out {
   /* sticky workload (kb_snapshot.cq_sticky != NULL; untouched otherwise; the pointer may be NULL): the slots after the
      drain, for the caller to write back */
   int32_t *cq_sticky;         /* [n_cq] pending index of each ClusterQueue's sticky workload, -1 = none */
+  /* admission checks (kb_snapshot.wl_check_ns != NULL; zero / untouched otherwise; each pointer may be NULL) */
+  int64_t n_check_ready, n_check_retry, n_check_rejected;  /* out: verdicts over the drain, those before cycle 0 included */
+  int32_t *cycle_check_retry;    /* [max_cycles] Retry verdicts applied from the start of cycle c to the start of c+1 */
+  int32_t *cycle_check_rejected; /* [max_cycles] Rejected verdicts, likewise */
+  int64_t *wl_ready_ns;          /* [n_wl] time of the last Admitted in the drain, INT64_MIN if none */
+  int32_t *wl_check_retries_out; /* [n_wl] final RetryCount */
+  uint8_t *wl_deactivated;       /* [n_wl] 1 if the workload was deactivated (Rejected) */
+  int64_t n_resorts;             /* out: queue re-sorts (a record entered its queue with a new queue-order timestamp) */
+  double resort_ms;              /* out: device time of those re-sorts (part of gpu_ms) */
 } kb_drain_out;
 int32_t kb_run_drain(kb_handle *h, const kb_snapshot *s, kb_drain_out *out);
 

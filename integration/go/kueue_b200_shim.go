@@ -367,6 +367,12 @@ func (s *Scheduler) flatten(snap *schdcache.Snapshot, heads []workload.Info, gen
 	// The sticky workload of every ClusterQueue (INTEGRATION.md) comes from an accessor in pkg/cache/queue, since the
 	// field sw is unexported, mapped to its pending index (-1 = none):
 	//   c.cq_sticky = cp32(cqSticky)   // after kb_run_drain, kb_drain_out.cq_sticky is written back through a setter
+	// Admission checks (INTEGRATION.md): a modelled check delay and fail count per workload, and the start state read from
+	// Status.AdmissionChecks[*].RetryCount, Status.RequeueState.RequeueAt, the Evicted condition (reason AdmissionCheck)
+	// and ProvisioningRequestConfig.Spec.RetryStrategy:
+	//   c.wl_check_ns, c.wl_check_fail, c.wl_check_retries = cp64(chkNs), cp32(chkFail), cp32(retryCount)
+	//   c.wl_check_evict_ns, c.wl_requeue_at_ns, c.adm_check_end_ns = cp64(evictedAt), cp64(requeueAt), cp64(checkEnd)
+	//   c.check_backoff_base_s, c.check_backoff_max_s, c.check_backoff_limit = base, max, limit
 	// They stay nil here: a single cycle ignores them.
 	if anyGroup { // optional table: NULL when no podset is grouped
 		c.ps_group = cp32(psGroup)

@@ -84,6 +84,9 @@ class kb_snapshot(C.Structure):
         ("adm_lq", _P(C.c_int32)),
         ("wl_evict_ns", _P(C.c_int64)), ("adm_evict_end_ns", _P(C.c_int64)),
         ("cq_sticky", _P(C.c_int32)),
+        ("wl_check_ns", _P(C.c_int64)), ("wl_check_fail", _P(C.c_int32)), ("wl_check_retries", _P(C.c_int32)),
+        ("wl_check_evict_ns", _P(C.c_int64)), ("wl_requeue_at_ns", _P(C.c_int64)), ("adm_check_end_ns", _P(C.c_int64)),
+        ("check_backoff_base_s", C.c_int32), ("check_backoff_max_s", C.c_int32), ("check_backoff_limit", C.c_int32),
     ]
 
 
@@ -135,6 +138,10 @@ class kb_drain_out(C.Structure):
         ("n_afs_samples", C.c_int64),
         ("n_evict_done", C.c_int64), ("cycle_evict_done", _P(C.c_int32)),
         ("cq_sticky", _P(C.c_int32)),
+        ("n_check_ready", C.c_int64), ("n_check_retry", C.c_int64), ("n_check_rejected", C.c_int64),
+        ("cycle_check_retry", _P(C.c_int32)), ("cycle_check_rejected", _P(C.c_int32)),
+        ("wl_ready_ns", _P(C.c_int64)), ("wl_check_retries_out", _P(C.c_int32)), ("wl_deactivated", _P(C.c_uint8)),
+        ("n_resorts", C.c_int64), ("resort_ms", C.c_double),
     ]
 
 
@@ -191,20 +198,24 @@ _DT = {
     "lq_last_update_ns": np.int64, "adm_lq": np.int32,
     "wl_evict_ns": np.int64, "adm_evict_end_ns": np.int64,
     "cq_sticky": np.int32,
+    "wl_check_ns": np.int64, "wl_check_fail": np.int32, "wl_check_retries": np.int32, "wl_check_evict_ns": np.int64,
+    "wl_requeue_at_ns": np.int64, "adm_check_end_ns": np.int64,
 }
 # AdmissionFairSharing tables (include/kueue_b200.h): wl_lq absent = AFS off
 AFS_FIELDS = ("wl_lq", "lq_cq", "cq_afs", "lq_weight", "lq_consumed", "lq_consumed_scale", "lq_penalty", "afs_res_weight",
               "afs_milli_mul")
 # arrivals and completions of kb_run_drain's event mode (include/kueue_b200.h): all absent = event mode off
-EVENT_FIELDS = ("wl_create_ns", "wl_run_ns", "adm_finish_ns", "wl_evict_ns")
+EVENT_FIELDS = ("wl_create_ns", "wl_run_ns", "adm_finish_ns", "wl_evict_ns", "wl_check_ns")
 # decay of the AdmissionFairSharing consumed usage in event mode (include/kueue_b200.h): lq_last_update_ns absent = off
 AFS_DECAY_FIELDS = ("lq_last_update_ns", "adm_lq")
 # end times of the evictions under way before an event drain with wl_evict_ns (include/kueue_b200.h): absent = none known
 EVICT_END_FIELDS = ("adm_evict_end_ns",)
 # the sticky workload of every ClusterQueue at the start of a drain (include/kueue_b200.h): absent = the rule is off
 STICKY_FIELDS = ("cq_sticky",)
+# admission checks in event mode (include/kueue_b200.h): wl_check_ns absent = off; the others need it
+CHECK_FIELDS = ("wl_check_ns", "wl_check_fail", "wl_check_retries", "wl_check_evict_ns", "wl_requeue_at_ns", "adm_check_end_ns")
 OPTIONAL_FIELDS = (("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows", "adm_wl") + AFS_FIELDS +
-                   EVENT_FIELDS + AFS_DECAY_FIELDS + EVICT_END_FIELDS + STICKY_FIELDS)  # NULL in kb_snapshot when absent
+                   EVENT_FIELDS + AFS_DECAY_FIELDS + EVICT_END_FIELDS + STICKY_FIELDS + CHECK_FIELDS)  # NULL in kb_snapshot when absent
 ARRAY_FIELDS = list(_DT.keys())
 # tables the library keeps resident while kb_snapshot.static_generation is unchanged (include/kueue_b200.h)
 STATIC_FIELDS = ("parent", "fair_weight", "nominal", "borrow_limit", "lend_limit", "cq_within_cq", "cq_reclaim_within",
@@ -236,6 +247,9 @@ class FlatSnapshot:
     drain_cycle_ns: int = 0  # kb_snapshot.drain_cycle_ns: simulated time of one drain cycle (<= 0 means 1)
     afs_half_life_ns: int = 0  # kb_snapshot.afs_half_life_ns: UsageHalfLifeTime (decay of consumed usage)
     afs_sampling_ns: int = 0   # kb_snapshot.afs_sampling_ns: UsageSamplingInterval
+    check_backoff_base_s: int = 60    # kb_snapshot.check_backoff_*: the admission checks' RetryStrategy (defaults of
+    check_backoff_max_s: int = 1800   # ProvisioningRequestConfig, provisioningrequestconfig_types.go:123-154)
+    check_backoff_limit: int = 3
     arrays: dict = field(default_factory=dict)
 
     def __getattr__(self, name):
@@ -332,6 +346,8 @@ class FlatSnapshot:
             s.afs_alpha = self.afs_alpha
             s.drain_cycle_ns = self.drain_cycle_ns
             s.afs_half_life_ns, s.afs_sampling_ns = self.afs_half_life_ns, self.afs_sampling_ns
+            s.check_backoff_base_s, s.check_backoff_max_s = self.check_backoff_base_s, self.check_backoff_max_s
+            s.check_backoff_limit = self.check_backoff_limit
             return s
         s = kb_snapshot()
         s.n_cq, s.n_cohort, s.n_flavor, s.n_resource = self.n_cq, self.n_cohort, self.n_flavor, self.n_resource
@@ -345,6 +361,8 @@ class FlatSnapshot:
         s.afs_alpha = self.afs_alpha
         s.drain_cycle_ns = self.drain_cycle_ns
         s.afs_half_life_ns, s.afs_sampling_ns = self.afs_half_life_ns, self.afs_sampling_ns
+        s.check_backoff_base_s, s.check_backoff_max_s = self.check_backoff_base_s, self.check_backoff_max_s
+        s.check_backoff_limit = self.check_backoff_limit
         for name in ARRAY_FIELDS:
             if name in OPTIONAL_FIELDS and name not in self.arrays:
                 continue  # stays NULL
@@ -437,6 +455,11 @@ class DrainOut:
         self.lq_consumed_scale = np.zeros((max(1, L), R), np.int32)[:L]
         self.lq_last_update_ns = np.zeros(max(1, L), np.int64)[:L]
         self.cq_sticky = np.full(max(1, Q), -1, np.int32)[:Q]  # the sticky slots after the drain (with kb_snapshot.cq_sticky)
+        self.cycle_check_retry = np.zeros(max_cycles, np.int32)  # admission checks (kb_snapshot.wl_check_ns)
+        self.cycle_check_rejected = np.zeros(max_cycles, np.int32)
+        self.wl_ready_ns = np.full(W, KB_TS_UNSET, np.int64)
+        self.wl_check_retries_out = np.zeros(W, np.int32)
+        self.wl_deactivated = np.zeros(W, np.uint8)
         cap = (min(W * 4 + Q, min(Q, W) * max_cycles) if trace_capacity is None else trace_capacity) if trace else 0
         self.trace_wl = np.zeros(max(1, cap), np.int32)
         self.trace_decision = np.zeros(max(1, cap), np.uint8)
@@ -455,6 +478,11 @@ class DrainOut:
         s.lq_consumed = _ptr(self.lq_consumed, C.c_int64); s.lq_consumed_scale = _ptr(self.lq_consumed_scale, C.c_int32)
         s.lq_last_update_ns = _ptr(self.lq_last_update_ns, C.c_int64)
         s.cq_sticky = _ptr(self.cq_sticky, C.c_int32)
+        s.cycle_check_retry = _ptr(self.cycle_check_retry, C.c_int32)
+        s.cycle_check_rejected = _ptr(self.cycle_check_rejected, C.c_int32)
+        s.wl_ready_ns = _ptr(self.wl_ready_ns, C.c_int64)
+        s.wl_check_retries_out = _ptr(self.wl_check_retries_out, C.c_int32)
+        s.wl_deactivated = _ptr(self.wl_deactivated, C.c_uint8)
         if trace:
             s.trace_wl = _ptr(self.trace_wl, C.c_int32); s.trace_decision = _ptr(self.trace_decision, C.c_uint8)
         s.trace_capacity = cap
@@ -480,6 +508,16 @@ class DrainOut:
     def n_afs_samples(self): return int(self.struct.n_afs_samples)
     @property
     def n_evict_done(self): return int(self.struct.n_evict_done)
+    @property
+    def n_check_ready(self): return int(self.struct.n_check_ready)
+    @property
+    def n_check_retry(self): return int(self.struct.n_check_retry)
+    @property
+    def n_check_rejected(self): return int(self.struct.n_check_rejected)
+    @property
+    def n_resorts(self): return int(self.struct.n_resorts)
+    @property
+    def resort_ms(self): return float(self.struct.resort_ms)
 
     def cycles(self):
         """[(heads, decisions)] per cycle from the trace."""

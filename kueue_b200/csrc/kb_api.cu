@@ -1356,7 +1356,7 @@ extern "C" int32_t kb_run_cycle(kb_handle *h, const kb_snapshot *s, kb_cycle_out
 // ---------------------------------------------------------------------------
 // what a boundary of kb_run_drain reads back, in the pinned host words [8, 24)
 struct DrainWords {
-  uint32_t counters[KB_DC_ARR_HI + 1];  // DrainDev::counters; [0] = heads of the next cycle
+  uint32_t counters[KB_DC_CHECK_REJECTED + 1];  // DrainDev::counters; [0] = heads of the next cycle
   uint32_t n_new, n_cells;              // this cycle's admissions and their usage cells (the admit scans' totals)
   uint32_t status;                      // the cycle's status word (KBS_AFS_OVERFLOW)
   i64 t_next;                           // event mode: t_{c+1}
@@ -1369,6 +1369,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   const int max_cycles = std::max(0, out->max_cycles);
   out->n_cycles = 0; out->n_decisions = 0; out->n_admitted = 0; out->gpu_ms = 0; out->n_evicted = 0;
   out->n_finished = 0; out->n_arrived = 0; out->end_ns = s->now_ns; out->n_evict_done = 0;
+  out->n_check_ready = 0; out->n_check_retry = 0; out->n_check_rejected = 0; out->n_resorts = 0; out->resort_ms = 0;
   // ---- eviction replay: host-side checks of adm_wl (include/kueue_b200.h)
   const bool replay = s->adm_wl != nullptr;
   if (replay) {
@@ -1384,7 +1385,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     }
   }
   // ---- event mode: host-side checks of the arrival and completion tables (include/kueue_b200.h)
-  const bool events = s->wl_create_ns || s->wl_run_ns || s->adm_finish_ns || s->wl_evict_ns;
+  const bool events = s->wl_create_ns || s->wl_run_ns || s->adm_finish_ns || s->wl_evict_ns || s->wl_check_ns;
   if (events) {
     if (s->adm_finish_ns)
       for (int a = 0; a < s->n_adm; a++)
@@ -1437,6 +1438,39 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
         return fail(h, KB_ERR_UNSUPPORTED, "cq_sticky: a sticky workload on a ClusterQueue with AdmissionFairSharing");
     }
     if (out->cq_sticky) memcpy(out->cq_sticky, s->cq_sticky, (size_t)Q * 4);  // the slots of a drain that runs no cycle
+  }
+  // ---- admission checks: host-side checks (include/kueue_b200.h)
+  const bool checks = s->wl_check_ns != nullptr;
+  if (checks || s->wl_check_fail || s->wl_check_retries || s->wl_check_evict_ns || s->wl_requeue_at_ns || s->adm_check_end_ns) {
+    if (!checks) return fail(h, KB_ERR_INVALID, "admission checks: the tables need wl_check_ns");
+    if (!replay) return fail(h, KB_ERR_INVALID, "admission checks: the tables need adm_wl");
+    if (decay) return fail(h, KB_ERR_UNSUPPORTED, "admission checks with afs decay: a workload with checks never makes the Pending -> Admitted transition that updates consumed usage");
+    if (s->check_backoff_base_s <= 0 || s->check_backoff_max_s < 0 || s->check_backoff_limit < 0)
+      return fail(h, KB_ERR_INVALID, "admission checks: backoff base <= 0, max < 0 or limit < 0");
+    {  // the longest WaitTime of attempts 1..limit (constant once capped: a base of >= 1 s gets there in < 64 doublings)
+      i64 longest = 0;
+      for (int k = 1; k <= std::min(s->check_backoff_limit, 64); k++)
+        longest = std::max(longest, kb_check_wait_ns(k, s->check_backoff_base_s, s->check_backoff_max_s));
+      if (longest >= 10000ll * 1000000000ll)
+        return fail(h, KB_ERR_UNSUPPORTED, "admission checks: a reachable backoff of 10,000 s or more is random in the reference (jitter)");
+    }
+    std::vector<uint8_t> held((size_t)std::max(1, W), 0);
+    for (int a = 0; a < s->n_adm; a++) held[s->adm_wl[a]] = 1;
+    for (int w = 0; w < W; w++) {
+      if (s->wl_check_ns[w] < 0 || (s->wl_check_fail && s->wl_check_fail[w] < 0) || (s->wl_check_retries && s->wl_check_retries[w] < 0))
+        return fail(h, KB_ERR_INVALID, "admission checks: a negative delay, fail count or retry count");
+      if (s->wl_requeue_at_ns && s->wl_requeue_at_ns[w] != INT64_MIN) {
+        if (held[w]) return fail(h, KB_ERR_INVALID, "admission checks: wl_requeue_at_ns on a record that holds quota (adm_wl)");
+        if (s->wl_create_ns && s->wl_create_ns[w] > s->now_ns) return fail(h, KB_ERR_INVALID, "admission checks: wl_requeue_at_ns on a record created after now_ns");
+      }
+    }
+    if (s->adm_check_end_ns)
+      for (int a = 0; a < s->n_adm; a++) {
+        if (s->adm_check_end_ns[a] == INT64_MIN) continue;
+        if (s->adm_check_end_ns[a] <= s->now_ns) return fail(h, KB_ERR_INVALID, "admission checks: adm_check_end_ns at or before now_ns");
+        if (lat && s->adm_evict_end_ns && s->adm_evicted && s->adm_evicted[a])  // one end time per row
+          return fail(h, KB_ERR_INVALID, "admission checks: a row with both an eviction under way (adm_evict_end_ns) and a check under way");
+      }
   }
   out->n_afs_samples = 0;
   if (Hcap == 0 || max_cycles == 0) return KB_OK;
@@ -1515,7 +1549,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   u64 *keys[2], *arr_keys[2] = {nullptr, nullptr};
   int32_t *vals[2], *arr_vals[2] = {nullptr, nullptr}, *q_count, *d_wl_class = nullptr, *d_cq_class_start = nullptr;
   char *sort_tmp, *scan_tmp = nullptr;
-  i64 *run = nullptr, *create = nullptr, *evict_ns = nullptr;
+  i64 *run = nullptr, *create = nullptr, *evict_ns = nullptr, *check_ns = nullptr;
   DrainDev X{};
   AdmTabs other{};  // compaction: the other half of the admitted tables' double buffer
   auto layout = [&](Arena &a) {
@@ -1563,6 +1597,12 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       evict_ns = a.take<i64>(Wz);
       X.adm_evicting = a.take<uint8_t>(Acap); other.evicting = a.take<uint8_t>(Acap);
     }
+    if (checks) {  // delays, attempt state, timestamps and the checking byte of both halves
+      check_ns = a.take<i64>(Wz); X.wl_fail = a.take<int32_t>(Wz); X.wl_retries = a.take<int32_t>(Wz);
+      X.wl_ts0 = a.take<i64>(Wz); X.wl_sort_ts = a.take<i64>(Wz); X.wl_requeue_at = a.take<i64>(Wz);
+      X.wl_ready_ns = a.take<i64>(Wz); X.wl_deactivated = a.take<uint8_t>(Wz);
+      X.adm_checking = a.take<uint8_t>(Acap); other.checking = a.take<uint8_t>(Acap);
+    }
     if (afs) {
       X.seg_start = a.take<int32_t>(seg_start.size()); X.lq_seg = a.take<int32_t>(lq_seg.size());
       X.seg_lq = a.take<int32_t>(seg_lq.size()); X.afs_cqs = a.take<int32_t>(afs_cqs.size());
@@ -1609,6 +1649,19 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       never.swap(fin);
       finish = never.data();
     }
+    if (checks && s->adm_check_end_ns) {  // rows whose checks run: the verdict time in the finish column
+      std::vector<i64> fin((size_t)s->n_adm);
+      std::vector<uint8_t> chk((size_t)s->n_adm, 0);
+      memcpy(fin.data(), finish, (size_t)s->n_adm * 8);
+      for (int a = 0; a < s->n_adm; a++)
+        if (s->adm_check_end_ns[a] != INT64_MIN) { fin[a] = s->adm_check_end_ns[a]; chk[a] = 1; }
+      never.swap(fin);
+      finish = never.data();
+      CUDA_TRY(h, h2d(h, X.adm_checking, chk.data(), chk.size()));
+      CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // chk is a local
+    } else if (checks) {
+      CUDA_TRY(h, cudaMemsetAsync(X.adm_checking, 0, (size_t)s->n_adm, h->stream));
+    }
     CUDA_TRY(h, h2d(h, X.adm_finish, finish, (size_t)s->n_adm * 8));
     if (s->wl_run_ns) { CUDA_TRY(h, h2d(h, run, s->wl_run_ns, Wz * 8)); X.wl_run = run; }
     if (create) { CUDA_TRY(h, h2d(h, create, s->wl_create_ns, Wz * 8)); X.n_arr = W; }
@@ -1644,6 +1697,29 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     X.n_afs_cq = (int)afs_cqs.size();
   }
   if (sticky) CUDA_TRY(h, h2d(h, X.cq_sticky, s->cq_sticky, (size_t)Q * 4));
+  std::vector<i64> qts, requeue_at;  // admission checks: queue-order timestamps and RequeueAt at the start
+  std::vector<int32_t> fails, retries;
+  if (checks) {
+    std::vector<uint8_t> held(Wz, 0);
+    for (int a = 0; a < s->n_adm; a++) held[s->adm_wl[a]] = 1;
+    qts.assign(s->wl_ts, s->wl_ts + W);
+    if (s->wl_check_evict_ns)
+      for (int w = 0; w < W; w++) if (s->wl_check_evict_ns[w] != INT64_MIN && !held[w]) qts[w] = s->wl_check_evict_ns[w];
+    requeue_at.assign(Wz, INT64_MIN);
+    if (s->wl_requeue_at_ns) requeue_at.assign(s->wl_requeue_at_ns, s->wl_requeue_at_ns + W);
+    fails.assign(Wz, 0); retries.assign(Wz, 0);
+    if (s->wl_check_fail) fails.assign(s->wl_check_fail, s->wl_check_fail + W);
+    if (s->wl_check_retries) retries.assign(s->wl_check_retries, s->wl_check_retries + W);
+    X.wl_check = check_ns; X.wl_qts = const_cast<i64 *>(D.wl_ts);
+    CUDA_TRY(h, h2d(h, check_ns, s->wl_check_ns, Wz * 8));
+    CUDA_TRY(h, h2d(h, X.wl_ts0, s->wl_ts, Wz * 8));
+    CUDA_TRY(h, h2d(h, X.wl_qts, qts.data(), Wz * 8));       // the cycle kernels read the queue-order timestamp
+    CUDA_TRY(h, h2d(h, X.wl_sort_ts, qts.data(), Wz * 8));
+    CUDA_TRY(h, h2d(h, X.wl_requeue_at, requeue_at.data(), Wz * 8));
+    CUDA_TRY(h, h2d(h, X.wl_fail, fails.data(), Wz * 4));
+    CUDA_TRY(h, h2d(h, X.wl_retries, retries.data(), Wz * 4));
+    X.check_base_s = s->check_backoff_base_s; X.check_max_s = s->check_backoff_max_s; X.check_limit = s->check_backoff_limit;
+  }
   std::vector<i64> lq_adm;  // decay: the initial admitted usage of every LocalQueue (live rows of the snapshot)
   if (decay) {
     lq_adm.assign(LR, 0);
@@ -1658,19 +1734,22 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   }
   // ---- per-ClusterQueue order (queueOrderingFunc): stable LSD passes uid -> timestamp -> (ClusterQueue | priority desc)
   const int tb = 256, nbW = (W + tb - 1) / tb, nbQ = (Q + tb - 1) / tb;
-  CUDA_TRY(h, cudaMemsetAsync(q_count, 0, sizeof(int32_t) * (Sz + 2), h->stream));
-  {
+  auto sort_queues = [&]() -> cudaError_t {  // also the re-sort of admission checks (same segments, same q_start)
+    cudaError_t e = cudaMemsetAsync(q_count, 0, sizeof(int32_t) * (Sz + 2), h->stream);
+    if (e != cudaSuccess) return e;
     cub::DoubleBuffer<u64> dk(keys[0], keys[1]); cub::DoubleBuffer<int32_t> dv(vals[0], vals[1]);
     size_t bytes = sort_bytes;
     k_drain_keys_uid<<<nbW, tb, 0, h->stream>>>(D, dk.Current(), dv.Current());
-    CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 64, h->stream));
+    if ((e = cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 64, h->stream)) != cudaSuccess) return e;
     k_drain_keys_ts<<<nbW, tb, 0, h->stream>>>(D, dv.Current(), dk.Current());
-    CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 64, h->stream));
+    if ((e = cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 64, h->stream)) != cudaSuccess) return e;
     k_drain_keys_cq<<<nbW, tb, 0, h->stream>>>(D, X, dv.Current(), dk.Current(), q_count);
     int cq_bits = 1; while ((1ll << cq_bits) < (long long)S) cq_bits++;
-    CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 32 + cq_bits, h->stream));
+    if ((e = cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 32 + cq_bits, h->stream)) != cudaSuccess) return e;
     X.q_order = dv.Current();
-  }
+    return cudaSuccess;
+  };
+  CUDA_TRY(h, sort_queues());
   if (create) {  // arrival order: (creation time, index); the workloads present at the start are its first k_drain_init_events prefix
     cub::DoubleBuffer<u64> dk(arr_keys[0], arr_keys[1]); cub::DoubleBuffer<int32_t> dv(arr_vals[0], arr_vals[1]);
     size_t bytes = sort_bytes;
@@ -1682,6 +1761,10 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   k_drain_init<<<std::max(nbW, (S + tb - 1) / tb), tb, 0, h->stream>>>(D, X, S);
   if (events) k_drain_init_events<<<std::max(1, nbW), tb, 0, h->stream>>>(D, X, create, s->now_ns);
   if (replay || events || sticky) k_drain_init_replay<<<std::max(nbW, (s->n_adm + tb - 1) / tb), tb, 0, h->stream>>>(D, X, replay ? s->n_adm : 0);
+  if (checks) {  // records in backoff, and the first RequeueAt into clock[2] (k_drain_init_events set clock[0] = now_ns)
+    k_drain_init_checks<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W, s->now_ns);
+    k_drain_backoff<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W);
+  }
   k_drain_advance<<<(S + tb - 1) / tb, tb, 0, h->stream>>>(X, S);
   const int nbL = std::max(1, (L + tb - 1) / tb);
   if (decay) {  // the samples due at or before now_ns (k_drain_init_events set clock[0] = now_ns), before the first heads
@@ -1710,6 +1793,18 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   i64 t = s->now_ns;  // the clock: the plain drain steps it by one per cycle
   const i64 step = s->drain_cycle_ns > 0 ? s->drain_cycle_ns : 1;
   const int nbArr = std::max(1, std::min(nbW, 8 * std::max(1, h->sm_count)));
+  struct EventPair {  // around a re-sort (admission checks); destroyed on every return
+    cudaEvent_t e[2] = {nullptr, nullptr};
+    ~EventPair() { for (cudaEvent_t x : e) if (x) cudaEventDestroy(x); }
+  } resort_ev;
+  cudaEvent_t *ev_r = resort_ev.e;
+  bool resort_timed = false;
+  uint32_t verdicts_seen[3] = {0, 0, 0};  // cumulative Ready / Retry / Rejected counters at the previous boundary
+  if (checks) {
+    CUDA_TRY(h, cudaEventCreate(&ev_r[0]));
+    CUDA_TRY(h, cudaEventCreate(&ev_r[1]));
+    CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_RESORT, 0, 4 * 4, h->stream));  // once: the boundaries never clear them
+  }
   // ---- one boundary per iteration, one synchronisation each (kueue_b200/drain.py): cycle c at t (in event mode, a
   // jump to the next event when there are no heads), its decisions and admissions, the evictions; in event mode E,
   // t_{c+1}, the decay samples, completions and arrivals; where rows can die (compact) the inadmissible requeue and the
@@ -1754,6 +1849,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       if (decay) k_drain_afs_decay<<<nbL, tb, 0, h->stream>>>(D, X, L);  // samples due in (t, t_{c+1}], before the completions
       k_drain_finish<<<nbB, tb, 0, h->stream>>>(D, X, bound, n_new_d);
       if (X.arr_key) k_drain_arrive<<<nbArr, tb, 0, h->stream>>>(X);
+      if (checks) k_drain_backoff<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W);
     }
     if (compact) {
       k_drain_requeue<<<nbQ, tb, 0, h->stream>>>(D, X);
@@ -1772,7 +1868,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (!jump) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_new, n_new_d, 4, cudaMemcpyDeviceToHost, h->stream));
     if (!compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_cells, X.e_cell_off + n_live, 4, cudaMemcpyDeviceToHost, h->stream));
     if (afs && (!jump || decay)) CUDA_TRY(h, cudaMemcpyAsync(&hw.status, D.status, 4, cudaMemcpyDeviceToHost, h->stream));
-    if (compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[1], X.counters + 1, (events ? KB_DC_ARR_HI : KB_DC_FULL) * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[1], X.counters + 1, (checks ? KB_DC_CHECK_REJECTED : events ? KB_DC_ARR_HI : KB_DC_FULL) * 4, cudaMemcpyDeviceToHost, h->stream));
     if (events) CUDA_TRY(h, cudaMemcpyAsync(&hw.t_next, X.clock, 8, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     if (!jump) {
@@ -1793,6 +1889,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       if (events && out->cycle_finished) out->cycle_finished[cyc] = 0;
       if (events && out->cycle_arrived) out->cycle_arrived[cyc] = 0;
       if (lat && out->cycle_evict_done) out->cycle_evict_done[cyc] = 0;
+      if (checks && out->cycle_check_retry) out->cycle_check_retry[cyc] = 0;
+      if (checks && out->cycle_check_rejected) out->cycle_check_rejected[cyc] = 0;
       out->n_decisions += n_live; out->n_admitted += n_new; out->n_evicted += n_ev;
       out->n_cycles = ++cyc;
     } else {
@@ -1806,6 +1904,16 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
         if (out->cycle_arrived) out->cycle_arrived[cyc - 1] += arr;
       }
     }
+    if (checks) {  // verdicts of this boundary; a record that entered its queue with a new timestamp re-sorts the queues
+      const uint32_t *cum = &hw.counters[KB_DC_CHECK_READY];
+      const int ready = (int)(cum[0] - verdicts_seen[0]), ret = (int)(cum[1] - verdicts_seen[1]), rej = (int)(cum[2] - verdicts_seen[2]);
+      memcpy(verdicts_seen, cum, sizeof(verdicts_seen));
+      out->n_check_ready += ready; out->n_check_retry += ret; out->n_check_rejected += rej;
+      if (cyc > 0) {
+        if (out->cycle_check_retry) out->cycle_check_retry[cyc - 1] += ret;
+        if (out->cycle_check_rejected) out->cycle_check_rejected[cyc - 1] += rej;
+      }
+    }
     if (lat) {  // evictions completed at this boundary (counter slot 4, inside the events copy)
       const int done = (int)hw.counters[KB_DC_EVICT_DONE];
       out->n_evict_done += done;
@@ -1814,10 +1922,10 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (compact) {  // the compacted half becomes the admitted tables of the next boundary
       A_cur = (int)hw.counters[KB_DC_ROWS]; AU_cur = (int)hw.counters[KB_DC_CELLS];
       AdmTabs cur{X.adm_cq, X.adm_priority, X.adm_ts, X.adm_qr_ts, X.adm_uid, X.adm_evicted, X.adm_use_start, X.adm_use_fr, X.adm_use_qty, X.adm_wl, X.adm_finish, X.adm_lq,
-                  X.adm_evicting};
+                  X.adm_evicting, X.adm_checking};
       X.adm_cq = other.cq; X.adm_priority = other.priority; X.adm_ts = other.ts; X.adm_qr_ts = other.qr_ts; X.adm_uid = other.uid;
       X.adm_evicted = other.evicted; X.adm_use_start = other.use_start; X.adm_use_fr = other.use_fr; X.adm_use_qty = other.use_qty; X.adm_wl = other.wl;
-      X.adm_finish = other.finish; X.adm_lq = other.lq; X.adm_evicting = other.evicting;
+      X.adm_finish = other.finish; X.adm_lq = other.lq; X.adm_evicting = other.evicting; X.adm_checking = other.checking;
       D.adm_cq = X.adm_cq; D.adm_priority = X.adm_priority; D.adm_ts = X.adm_ts; D.adm_qr_ts = X.adm_qr_ts; D.adm_uid = X.adm_uid;
       D.adm_evicted = X.adm_evicted; D.adm_use_start = X.adm_use_start; D.adm_use_fr = X.adm_use_fr; D.adm_use_qty = X.adm_use_qty;
       other = cur;
@@ -1826,9 +1934,29 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     }
     n_live = (int)hw.counters[0];
     if (events ? hw.counters[KB_DC_END] != 0 : n_new == 0 && n_ev == 0) break;
+    if (checks && (int32_t)hw.counters[KB_DC_RESORT] == X.cycle + 1) {  // re-sort: the three passes over the queue-order timestamps, positions,
+      // cursors from 0, first_aside from the SET_ASIDE positions, then the heads again.  The segments and their
+      // lengths do not change, so n_live holds and no synchronisation is added; the events are read at the next one.
+      if (resort_timed) { float ms = 0; cudaEventElapsedTime(&ms, ev_r[0], ev_r[1]); out->resort_ms += ms; gpu_ms += ms; }
+      CUDA_TRY(h, cudaEventRecord(ev_r[0], h->stream));
+      CUDA_TRY(h, sort_queues());
+      k_drain_init_replay<<<std::max(1, nbW), tb, 0, h->stream>>>(D, X, 0);
+      k_drain_resort_reset<<<(S + tb - 1) / tb, tb, 0, h->stream>>>(X, S);
+      k_drain_resort_aside<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W);
+      k_drain_advance<<<(S + tb - 1) / tb, tb, 0, h->stream>>>(X, S);
+      CUDA_TRY(h, cudaMemcpyAsync(X.wl_sort_ts, X.wl_qts, Wz * 8, cudaMemcpyDeviceToDevice, h->stream));
+      enqueue_heads();
+      CUDA_TRY(h, cudaEventRecord(ev_r[1], h->stream));
+      resort_timed = true;
+      out->n_resorts++;
+    }
     t = events ? hw.t_next : t + 1;
   }
   if (events) out->end_ns = t;
+  if (resort_timed) {
+    CUDA_TRY(h, cudaEventSynchronize(ev_r[1]));
+    float ms = 0; cudaEventElapsedTime(&ms, ev_r[0], ev_r[1]); out->resort_ms += ms; gpu_ms += ms;
+  }
   out->gpu_ms = gpu_ms;
   h->stats.last_cycle_gpu_ms = gpu_ms;
   memcpy(h->stats.kernel_ms, kms, sizeof(kms));
@@ -1850,6 +1978,11 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     else memset(out->wl_evictions, 0, Wz * 4);
   }
   if (sticky && out->cq_sticky) CUDA_TRY(h, cudaMemcpyAsync(out->cq_sticky, X.cq_sticky, (size_t)Q * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (checks) {
+    if (out->wl_ready_ns) CUDA_TRY(h, cudaMemcpyAsync(out->wl_ready_ns, X.wl_ready_ns, Wz * 8, cudaMemcpyDeviceToHost, h->stream));
+    if (out->wl_check_retries_out) CUDA_TRY(h, cudaMemcpyAsync(out->wl_check_retries_out, X.wl_retries, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (out->wl_deactivated) CUDA_TRY(h, cudaMemcpyAsync(out->wl_deactivated, X.wl_deactivated, Wz, cudaMemcpyDeviceToHost, h->stream));
+  }
   if (out->ps_flavor && PR) CUDA_TRY(h, cudaMemcpyAsync(out->ps_flavor, D.ps_flavor, PR, cudaMemcpyDeviceToHost, h->stream));
   if (out->ps_count && D.P) CUDA_TRY(h, cudaMemcpyAsync(out->ps_count, D.ps_count_out, (size_t)D.P * 4, cudaMemcpyDeviceToHost, h->stream));
   if (out->cq_usage) CUDA_TRY(h, cudaMemcpyAsync(out->cq_usage, D.cq_usage, (size_t)Q * FR * 8, cudaMemcpyDeviceToHost, h->stream));

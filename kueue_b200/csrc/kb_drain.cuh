@@ -50,11 +50,45 @@
 // (a Preempting head of a BestEffortFIFO ClusterQueue) or clears (its admission) the slot.  One head per ClusterQueue per
 // cycle: one writer per slot.  Never set on an AFS ClusterQueue (refused, and no preemption there), so k_drain_afs_heads
 // does not read it.
+//
+// Admission checks (kb_snapshot.wl_check_ns; include/kueue_b200.h): the byte column adm_checking (both halves, carried by
+// the compaction) marks a row whose checks run; its verdict time lives in the finish column, so k_drain_ev_min sees it
+// unchanged.  k_drain_admit starts the attempt, k_drain_evict drops it (a preempted row without pods is released at the
+// next boundary), k_drain_finish applies the verdicts before the completions.  The DevSnap's wl_ts is the mutable
+// queue-order timestamp the cycle kernels read (wl_ts0 keeps the creation timestamps).  k_drain_backoff (one pass over
+// the records per boundary) requeues the BACKOFF records whose RequeueAt has come and reduces the next RequeueAt into
+// clock[2], which k_drain_ev_next folds into E.  A record that enters its queue with a timestamp other than the key the
+// order was built with (wl_sort_ts) stamps KB_DC_RESORT with the boundary; the host then rebuilds the order (kb_api.cu).
 #pragma once
 
 #include <cub/device/device_scan.cuh>
 
 #include "kb_device.cuh"
+
+// Backoff.WaitTime (pkg/util/wait/backoff.go:35-60) without jitter: wait.Backoff.Step `iteration` times (the duration
+// grows by `factor` in float64 and is capped at cap, after which Step returns cap), stopping at the cap.  cap 0 =
+// MaxInt64 / ceil(factor).  Restated by kueue_b200/drain.py wait_time.
+__host__ __device__ inline i64 kb_backoff_wait(i64 base, i64 cap, double factor, int iteration) {
+  if (cap == 0) cap = (i64)(9223372036854775807.0 / ceil(factor));
+  i64 dur = base, out = 0;
+  bool capped = false;
+  for (int i = 0; i < iteration; i++) {
+    out = dur;
+    if (!capped) {
+      const double x = (double)dur * factor;
+      if (x >= 9223372036854775808.0 || (i64)x > cap) { dur = cap; capped = true; }  // past int64 is past the cap too
+      else dur = (i64)x;
+    }
+    if (out == cap) break;
+  }
+  return out;
+}
+// RequeueAfterSeconds of admission-check attempt k: WaitTime(k) of wait.NewBackoff(base, max, 2, 0.0001) truncated to
+// whole seconds, exact below 10,000 s (kb_run_drain refuses a reachable backoff at or above it).  With base > max > 0 the
+// first Step returns the base uncapped.  Restated by kueue_b200/drain.py check_wait_s.
+__host__ __device__ inline i64 kb_check_wait_ns(int k, i64 base_s, i64 max_s) {
+  return kb_backoff_wait(base_s * 1000000000ll, max_s * 1000000000ll, 2.0, k) / 1000000000ll * 1000000000ll;
+}
 
 // ---- resource.Quantity in the int64Amount form (value * 10^scale), as AdmissionFairSharing sums it -----------------
 // Pow10 for |n| <= 22: 10^n is exact in a double, and Go's math.Pow10(-n) is 1 / 10^n (not a multiplication by 1e-n).
@@ -227,12 +261,24 @@ struct DrainDev {
   uint8_t *adm_evicting;           // [A_cap] 1 while the row's eviction is under way (current half); its end is adm_finish
   // sticky workload; cq_sticky == nullptr: off
   int32_t *cq_sticky;              // [Q] pending index of each ClusterQueue's sticky workload, -1 = none
+  // admission checks (event mode); wl_check == nullptr: off
+  const i64 *wl_check;             // [W] time from a reservation to the attempt's verdict
+  int32_t *wl_fail, *wl_retries;   // [W] failures left (INT32_MAX = all) / RetryCount
+  i64 *wl_qts;                     // [W] queue-order timestamps: the DevSnap's wl_ts
+  const i64 *wl_ts0;               // [W] creation timestamps
+  i64 *wl_sort_ts;                 // [W] the keys the current order was built with
+  i64 *wl_requeue_at;              // [W] RequeueAt of a BACKOFF record
+  i64 *wl_ready_ns; uint8_t *wl_deactivated;  // [W]
+  uint8_t *adm_checking;           // [A_cap] 1 while the row's checks run (current half); its verdict time is adm_finish
+  i64 check_base_s, check_max_s; int check_limit;
 };
 // counters of a boundary: [1] evictions (issued, with latency), [2] / [3] rows / cells after the compaction, [4]
 // evictions completed (latency), [5] capacity flag; event mode: [6] completions, [7] arrivals, [8] end flag, [9] / [10]
-// arrived prefix of arr_order [lo, hi)
+// arrived prefix of arr_order [lo, hi); admission checks: [11] the stamp (cycle + 1) of the last boundary that needs a
+// re-sort, [12] / [13] / [14] Ready / Retry / Rejected verdicts since the start (the host takes differences: no memset)
 enum { KB_DC_EVICTED = 1, KB_DC_ROWS = 2, KB_DC_CELLS = 3, KB_DC_EVICT_DONE = 4, KB_DC_FULL = 5,
-       KB_DC_FINISHED = 6, KB_DC_ARRIVED = 7, KB_DC_END = 8, KB_DC_ARR_LO = 9, KB_DC_ARR_HI = 10 };
+       KB_DC_FINISHED = 6, KB_DC_ARRIVED = 7, KB_DC_END = 8, KB_DC_ARR_LO = 9, KB_DC_ARR_HI = 10,
+       KB_DC_RESORT = 11, KB_DC_CHECK_READY = 12, KB_DC_CHECK_RETRY = 13, KB_DC_CHECK_REJECTED = 14 };
 
 __device__ __forceinline__ int drain_seg0(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq] : cq; }
 __device__ __forceinline__ int drain_seg1(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq + 1] : cq + 1; }
@@ -259,7 +305,8 @@ __global__ void k_drain_keys_cq(DevSnap D, DrainDev X, const int32_t *vals, u64 
   keys[i] = ((u64)seg << 32) | (u64)(~((unsigned)D.wl_priority[w] ^ 0x80000000u));  // higher priority first
   atomicAdd(&q_count[seg], 1);
 }
-enum { KB_WS_QUEUED = 0, KB_WS_SET_ASIDE = 1, KB_WS_HELD = 2, KB_WS_ABSENT = 3, KB_WS_FINISHED = 4 };
+enum { KB_WS_QUEUED = 0, KB_WS_SET_ASIDE = 1, KB_WS_HELD = 2, KB_WS_ABSENT = 3, KB_WS_FINISHED = 4, KB_WS_BACKOFF = 5,
+       KB_WS_DEACTIVATED = 6 };
 __global__ void k_drain_init(DevSnap D, DrainDev X, int S) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < D.W) { X.wl_state[i] = KB_WS_QUEUED; X.wl_admit_cycle[i] = -1; X.wl_evals[i] = 0; X.wl_last_decision[i] = 0xff; }
@@ -435,13 +482,21 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
   if (a >= X.A_cap || c0 + X.e_ncells[e] > X.AU_cap) { atomicOr(&X.counters[KB_DC_FULL], 1); return; }  // nothing past the end
   if (X.adm_wl) X.adm_wl[a] = wl;
   if (X.adm_lq) X.adm_lq[a] = X.wl_lq[wl];
-  X.adm_cq[a] = cq; X.adm_priority[a] = D.wl_priority[wl]; X.adm_ts[a] = D.wl_ts[wl]; X.adm_qr_ts[a] = qr_ts;
+  X.adm_cq[a] = cq; X.adm_priority[a] = D.wl_priority[wl]; X.adm_ts[a] = X.wl_ts0 ? X.wl_ts0[wl] : D.wl_ts[wl]; X.adm_qr_ts[a] = qr_ts;
   X.adm_uid[a] = D.wl_uid[wl]; X.adm_evicted[a] = 0;
   if (X.adm_evicting) X.adm_evicting[a] = 0;
   X.adm_use_start[a] = c0;
   if (X.adm_finish) {  // finish = QuotaReserved time + run time, saturating; run < 0 never finishes
     const i64 run = X.wl_run ? X.wl_run[wl] : -1;
-    X.adm_finish[a] = run < 0 ? INT64_MAX : (qr_ts > INT64_MAX - run ? INT64_MAX : qr_ts + run);
+    i64 fin = run < 0 ? INT64_MAX : (qr_ts > INT64_MAX - run ? INT64_MAX : qr_ts + run);
+    if (X.wl_check) {  // the reservation resets Evicted; a check delay starts an attempt, 0 is Ready at once
+      X.wl_qts[wl] = X.wl_ts0[wl];
+      const i64 chk = X.wl_check[wl];
+      X.adm_checking[a] = chk > 0;
+      if (chk > 0) fin = qr_ts > INT64_MAX - chk ? INT64_MAX : qr_ts + chk;
+      else X.wl_ready_ns[wl] = qr_ts;
+    }
+    X.adm_finish[a] = fin;
     X.wl_admit_ns[wl] = qr_ts;
   }
   const bool covers_pods = drain_covers_pods(D, cq);
@@ -506,6 +561,7 @@ __device__ __forceinline__ void drain_release(const DevSnap &D, const DrainDev &
   if (X.wl_has_qr) X.wl_has_qr[w] = 0;
   X.wl_admit_cycle[w] = -1;
   atomicMin(&X.cursor[X.wl_seg[w]], X.wl_pos[w]);
+  if (X.wl_sort_ts && X.wl_sort_ts[w] != X.wl_qts[w]) X.counters[KB_DC_RESORT] = X.cycle + 1;
 }
 // sets byte i of a byte column (256-byte aligned, padded) and returns whether it was set: atomicOr on its aligned word
 __device__ __forceinline__ bool drain_claim_byte(uint8_t *col, int i) {
@@ -530,6 +586,7 @@ __global__ void k_drain_evict(DevSnap D, DrainDev X) {
       const i64 lat = X.wl_evict[w];
       X.adm_evicted[a] = 1;
       X.adm_finish[a] = D.now_ns > INT64_MAX - lat ? INT64_MAX : D.now_ns + lat;
+      if (X.adm_checking && X.adm_checking[a]) { X.adm_checking[a] = 0; X.adm_finish[a] = D.now_ns; }  // no pods: the next boundary
       X.wl_evictions[w]++;
       atomicAdd(&X.counters[KB_DC_EVICTED], 1);
       continue;
@@ -567,7 +624,7 @@ __global__ void k_drain_live(DrainDev X, int bound, const int32_t *n_new) {
   X.row_live[a] = live;
   X.row_cells[a] = live ? X.adm_use_start[a + 1] - X.adm_use_start[a] : 0;
 }
-struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; i64 *finish; int32_t *lq; uint8_t *evicting; };
+struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; i64 *finish; int32_t *lq; uint8_t *evicting, *checking; };
 // live rows of [0, bound), in order, into the other half of the double buffer; thread bound writes the totals
 __global__ void k_drain_compact(DrainDev X, AdmTabs O, int bound) {
   int a = blockIdx.x * blockDim.x + threadIdx.x;
@@ -580,6 +637,7 @@ __global__ void k_drain_compact(DrainDev X, AdmTabs O, int bound) {
   if (X.adm_finish) O.finish[n] = X.adm_finish[a];
   if (X.adm_lq) O.lq[n] = X.adm_lq[a];
   if (X.adm_evicting) O.evicting[n] = X.adm_evicting[a];
+  if (X.adm_checking) O.checking[n] = X.adm_checking[a];
   for (int c = 0; c < nc; c++) { O.use_fr[c0 + c] = X.adm_use_fr[u0 + c]; O.use_qty[c0 + c] = X.adm_use_qty[u0 + c]; }
 }
 
@@ -604,7 +662,7 @@ __global__ void k_drain_keys_create(int W, const i64 *create, u64 *keys, int32_t
 __global__ void k_drain_init_events(DevSnap D, DrainDev X, const i64 *create, i64 now_ns) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i == 0) {
-    X.clock[0] = now_ns; X.clock[1] = INT64_MAX;
+    X.clock[0] = now_ns; X.clock[1] = INT64_MAX; X.clock[2] = INT64_MAX;
     const int lo = X.arr_key ? ev_upper_bound(X.arr_key, 0, X.n_arr, now_ns) : 0;
     X.counters[KB_DC_ARR_LO] = lo; X.counters[KB_DC_ARR_HI] = lo;
   }
@@ -626,7 +684,8 @@ __global__ void k_drain_ev_min(DrainDev X, int bound, const int32_t *n_new) {
 // t_{c+1} and the end flag (one thread).  jump: no heads, the clock goes to E.  Otherwise a cycle that admitted or
 // evicted steps, a quiet one waits for E; no E ends the drain.  Then the arrived prefix up to t_{c+1}.
 __global__ void k_drain_ev_next(DrainDev X, i64 t_c, i64 step, int jump, const int32_t *n_new) {
-  const i64 E = X.clock[1];
+  const i64 E = min(X.clock[1], X.clock[2]);  // [2]: the next RequeueAt (admission checks), INT64_MAX otherwise
+  X.clock[2] = INT64_MAX;
   const i64 stepped = t_c > INT64_MAX - step ? INT64_MAX : t_c + step;
   const bool active = !jump && ((n_new && *n_new > 0) || X.counters[KB_DC_EVICTED] > 0);
   i64 tn;
@@ -650,8 +709,45 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
   if (a >= bound || a >= X.A + (n_new ? *n_new : 0) || X.counters[KB_DC_FULL]) return;
   const int stamp = X.cycle + 1;
   if (X.counters[KB_DC_END] || X.adm_dead[a] == stamp || X.adm_finish[a] > X.clock[0]) return;
-  X.adm_dead[a] = stamp;
   const int cq = X.adm_cq[a];
+  if (X.adm_checking && X.adm_checking[a]) {  // a verdict (ProvisioningRequest controller.go:536-580)
+    const int w = X.adm_wl[a];
+    const i64 tv = X.adm_finish[a];
+    X.adm_checking[a] = 0;
+    if (X.wl_fail[w] == 0) {  // Ready: Admitted, the run clock starts; the row may finish in this boundary
+      const i64 run = X.wl_run ? X.wl_run[w] : -1;
+      const i64 fin = run < 0 ? INT64_MAX : (tv > INT64_MAX - run ? INT64_MAX : tv + run);
+      X.wl_ready_ns[w] = tv;
+      X.adm_finish[a] = fin;
+      atomicAdd(&X.counters[KB_DC_CHECK_READY], 1);
+      if (fin > X.clock[0]) return;
+    } else {  // Retry or Rejected: the workload holds no pods, its quota goes at once
+      if (X.wl_fail[w] != INT32_MAX) X.wl_fail[w]--;
+      const int k = X.wl_retries[w] + 1;
+      X.adm_dead[a] = stamp;
+      for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)
+        atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
+      X.wl_last_gen[w] = -1;
+      for (int i = D.wl_ps_start[w] * D.R; i < D.wl_ps_start[w + 1] * D.R; i++) X.ps_last_tried[i] = -1;
+      if (X.wl_has_qr) X.wl_has_qr[w] = 0;
+      X.wl_admit_cycle[w] = -1;
+      if (k <= X.check_limit) {  // Retry: RequeueAt = verdict + WaitTime(k), queue-order timestamp = the eviction time
+        const i64 wait = kb_check_wait_ns(k, X.check_base_s, X.check_max_s);
+        X.wl_retries[w] = k;
+        X.wl_requeue_at[w] = tv > INT64_MAX - wait ? INT64_MAX : tv + wait;
+        X.wl_qts[w] = tv;
+        X.wl_state[w] = KB_WS_BACKOFF;
+        atomicAdd(&X.counters[KB_DC_CHECK_RETRY], 1);
+      } else {  // Rejected: deactivated
+        X.wl_state[w] = KB_WS_DEACTIVATED;
+        X.wl_deactivated[w] = 1;
+        atomicAdd(&X.counters[KB_DC_CHECK_REJECTED], 1);
+      }
+      X.root_mark[D.root_slot[cq]] = stamp;
+      return;
+    }
+  }
+  X.adm_dead[a] = stamp;
   for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)
     atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
   const int w = X.adm_wl[a];
@@ -718,4 +814,41 @@ __global__ void k_drain_arrive(DrainDev X) {
       atomicMin(&X.cursor[s], p);
     }
   }
+}
+
+// ---- admission checks ------------------------------------------------------------------------------------------------
+// BACKOFF records (thread per record), after k_drain_finish and k_drain_ev_next: RequeueAt <= t_{c+1} joins its queue as
+// an arrival does (PushOrUpdate, NoFit rule included) and raises the re-sort flag when its queue-order timestamp is not
+// the key its position was sorted by; a later RequeueAt joins clock[2], the next boundary's E.  At the start (clock[0] =
+// now_ns) it only reduces clock[2].
+__global__ void k_drain_backoff(DrainDev X, int W) {
+  const int w = blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= W || X.wl_state[w] != KB_WS_BACKOFF) return;
+  const i64 at = X.wl_requeue_at[w];
+  if (at > X.clock[0]) { atomicMin((long long *)&X.clock[2], (long long)at); return; }
+  const int s = X.wl_seg[w], p = X.wl_pos[w];
+  if (X.class_nofit && X.wl_class[w] >= 0 && X.class_nofit[X.wl_class[w]]) {
+    X.wl_state[w] = KB_WS_SET_ASIDE;
+    atomicMin(&X.first_aside[s], p);
+  } else {
+    X.wl_state[w] = KB_WS_QUEUED;
+    atomicMin(&X.cursor[s], p);
+  }
+  if (X.wl_sort_ts[w] != X.wl_qts[w]) X.counters[KB_DC_RESORT] = X.cycle + 1;
+}
+// re-sort: every cursor back to 0 and no set-aside position, then the SET_ASIDE positions of the new order
+__global__ void k_drain_resort_reset(DrainDev X, int S) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s < S) { X.cursor[s] = 0; X.first_aside[s] = X.q_start[s + 1] - X.q_start[s]; }
+}
+__global__ void k_drain_resort_aside(DrainDev X, int W) {
+  const int w = blockIdx.x * blockDim.x + threadIdx.x;
+  if (w < W && X.wl_state[w] == KB_WS_SET_ASIDE) atomicMin(&X.first_aside[X.wl_seg[w]], X.wl_pos[w]);
+}
+// start of a drain with admission checks: records in check backoff (RequeueAt after now_ns) are BACKOFF; nothing is Admitted
+__global__ void k_drain_init_checks(DrainDev X, int W, i64 now_ns) {
+  const int w = blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= W) return;
+  if (X.wl_requeue_at[w] > now_ns) X.wl_state[w] = KB_WS_BACKOFF;
+  X.wl_ready_ns[w] = INT64_MIN; X.wl_deactivated[w] = 0;
 }

@@ -155,6 +155,46 @@ is not in the heap; the workload at the cursor is an ordinary queued one).  With
 equals the drain without the table when (a) there is no `adm_wl` and no event table (nothing before a Preempting head
 ever becomes queued again), (b) every ClusterQueue is StrictFIFO, or (c) no ClusterQueue has a preemption policy.
 Preemption expectations are not modelled: the drain observes an eviction at once.
+
+Admission checks (event mode, the snapshot carries `wl_check_ns` and `adm_wl`, include/kueue_b200.h).  In the reference
+a workload of a ClusterQueue with admission checks reserves quota and becomes Admitted once every check is Ready
+(SetQuotaReservation workload.go:830-853, SyncAdmittedCondition admissionchecks.go:36-70); the performance runner starts
+its run clock at Admitted (controller.go:62-72,131).  Two more states: BACKOFF (evicted by a check, waiting for RequeueAt)
+and DEACTIVATED (never queued again).  Every record has a mutable queue-order timestamp `qts`: `wl_check_evict_ns` when
+set (for a record adm_wl does not name), otherwise `wl_ts`, the creation timestamp.  Additions to the loop:
+  1. an admission at t_c of a workload with wl_check_ns > 0 reserves quota and starts attempt k = RetryCount + 1; its
+     row is checking and its verdict comes at t_c + wl_check_ns (saturating), kept in the finish column.  With 0 the
+     row is Ready at t_c, exactly as without the tables (wl_check_fail is then not read);
+  2. verdicts are events: E includes them, and in step 5 they are applied before the boundary's completions
+     (ProvisioningRequest controller.go:536-580, attempt numbering :249-263, provisioning.go:76-89):
+       - Ready (no failure left): wl_ready_ns = verdict, finish = verdict + wl_run_ns (saturating); the row may finish
+         in the same boundary;
+       - Retry (a failing attempt with k <= check_backoff_limit): the row's cells leave the usage, the row is removed,
+         its root tree is marked (reconcileCheckBasedEviction workload_controller.go:650-678: the workload holds no pods,
+         so the quota goes at once; :973-1004 requeues the tree).  The record goes to BACKOFF with RequeueAt = verdict +
+         WaitTime(k), RetryCount = k (resetChecksOnEviction admissionchecks.go:88-109, UpdateAdmissionCheckRequeueState
+         :250-262), qts = verdict (GetQueueOrderTimestamp workload.go:1180-1182) and LastAssignment nil;
+       - Rejected (k > limit): released the same way, the record is DEACTIVATED (SetDeactivationTarget,
+         workload_controller.go:386-433,656-671);
+       - a failing attempt uses up one unit of wl_check_fail (INT32_MAX: every attempt fails);
+  3. a BACKOFF record whose RequeueAt <= t_{c+1} arrives through step 6, NoFit rule included (workload_controller.go:
+     330-350,362-375 -> AddOrUpdateWorkload / PushOrUpdate); E includes the RequeueAt times;
+  4. an admission resets qts to wl_ts (SetQuotaReservation resets Evicted); the new row's adm_ts is wl_ts;
+  5. a preempted row whose checks are running holds no pods: with wl_evict_ns it is released at the next boundary
+     (its end time is t_c).  The attempt under way is dropped: it is not counted and uses up no failure (canonical);
+  6. the cycle sees qts as the heads' wl_ts (entry order scheduler.go:808, fair_sharing_iterator.go:196; preemption
+     policy preemption_policy.go:39-40), and each segment's order is by qts: when a record enters its queue with a qts
+     other than the key the order was built with, the order is rebuilt before the next heads (`n_resorts`): every
+     cursor at its first QUEUED workload, first_aside at the first SET_ASIDE one;
+  7. with every wl_check_ns = 0, every wl_check_fail = 0 and no start-state tables the drain equals the drain without
+     the tables.
+WaitTime(k) is `check_wait_s`: wait.NewBackoff(base, max, 2, 0.0001).WaitTime(k) (pkg/util/wait/backoff.go:35-60)
+truncated to whole seconds, exact below 10,000 s (kb_run_drain refuses a strategy whose longest reachable wait,
+`check_wait_bound_s`, is not below it).  It is min(base * 2^(k-1), max or infinity), except that with base > max > 0 the
+first Step returns the base uncapped (attempt 1 waits base, later ones max): the reference accepts such a strategy.  Start state:
+`adm_check_end_ns` (rows whose checks run, INT64_MIN = Admitted), `wl_requeue_at_ns` (records in backoff; one at or
+before now_ns is queued at the start), `wl_check_retries`.  Verdicts applied between the start of cycle c and of c+1
+are cycle c's (`check_retry`, `check_rejected`); those before cycle 0 count in the totals only.
 """
 from __future__ import annotations
 
@@ -200,6 +240,18 @@ class DrainResult:
     # sticky workload (cq_sticky in the snapshot; None / empty otherwise)
     cq_sticky: np.ndarray | None = None                        # [n_cq] the slots after the drain, -1 = none
     sticky_heads: List[np.ndarray] = field(default_factory=list)  # per cycle: heads the rule chose over the first queued
+    # admission checks (wl_check_ns in the snapshot; None / empty / 0 otherwise)
+    check_retry: List[np.ndarray] = field(default_factory=list)     # per cycle: pending indices that went to Retry
+    check_rejected: List[np.ndarray] = field(default_factory=list)  # per cycle: pending indices that were Rejected
+    n_check_ready: int = 0                                     # verdicts, those before cycle 0 included
+    n_check_retry: int = 0
+    n_check_rejected: int = 0
+    wl_ready_ns: np.ndarray | None = None                      # [n_wl] time of the last Admitted, INT64_MIN = none
+    wl_check_retries: np.ndarray | None = None                 # [n_wl] final RetryCount
+    wl_deactivated: np.ndarray | None = None                   # [n_wl] 1 = Rejected
+    wl_queue_ts: np.ndarray | None = None                      # [n_wl] final queue-order timestamps
+    n_resorts: int = 0
+    resort_orders: List[dict] = field(default_factory=list)    # the rebuilt queue state after every re-sort
 
     @property
     def n_evicted(self) -> int:
@@ -249,8 +301,43 @@ def requeue_goes_inadmissible(strict_fifo: bool, reason: str, last_tried) -> boo
     return not (immediate or pending_flavors(last_tried))
 
 
-QUEUED, SET_ASIDE, HELD, ABSENT, FINISHED = 0, 1, 2, 3, 4  # per-workload queue state (kb_drain.cuh KB_WS_*)
+QUEUED, SET_ASIDE, HELD, ABSENT, FINISHED, BACKOFF, DEACTIVATED = 0, 1, 2, 3, 4, 5, 6  # queue state (kb_drain.cuh KB_WS_*)
 NEVER = np.iinfo(np.int64).max  # an event time that never comes
+UNSET = np.iinfo(np.int64).min
+ALL_FAIL = np.iinfo(np.int32).max  # wl_check_fail: every attempt fails
+MAX_BACKOFF_S = 10_000  # below it the reference's jittered, truncated WaitTime is exact
+
+
+def wait_time(base_ns: int, cap_ns: int, factor: float, iteration: int) -> int:
+    """Backoff.WaitTime (pkg/util/wait/backoff.go:35-60) without jitter: wait.Backoff.Step `iteration` times (the
+    duration grows by `factor` in float64 and is capped at Cap, after which Steps is 0 and Step returns Cap), stopping
+    at the cap.  cap_ns 0 = MaxInt64 / ceil(factor)."""
+    cap = cap_ns if cap_ns else int(float(2**63 - 1) / math.ceil(factor))
+    dur, capped, out = int(base_ns), False, 0
+    for _ in range(iteration):
+        out = dur
+        if not capped:
+            x = float(dur) * factor
+            if x >= 2.0**63 or int(x) > cap:  # a product past int64 is past the cap too
+                dur, capped = cap, True
+            else:
+                dur = int(x)
+        if out == cap:
+            break
+    return out
+
+
+def check_wait_s(k: int, base_s: int, max_s: int) -> int:
+    """RequeueAfterSeconds of admission-check attempt k: WaitTime(k) of wait.NewBackoff(base, max, 2, 0.0001) without
+    jitter, in whole seconds (kb_drain.cuh kb_check_wait_ns).  The first Step returns the base uncapped, so with
+    base > max > 0 attempt 1 waits base and every later one max; otherwise it is min(base * 2^(k-1), max or infinity)."""
+    return wait_time(int(base_s) * 1_000_000_000, int(max_s) * 1_000_000_000, 2.0, int(k)) // 1_000_000_000
+
+
+def check_wait_bound_s(base_s: int, max_s: int, limit: int) -> int:
+    """the longest RequeueAfterSeconds a Retry can get (attempts 1..limit, 0 when limit is 0): WaitTime is constant once
+    capped, which takes fewer than 64 doublings of a base of at least 1 s"""
+    return max((check_wait_s(k, base_s, max_s) for k in range(1, min(int(limit), 64) + 1)), default=0)
 
 
 class NoFitSets:
@@ -451,7 +538,7 @@ def entry_penalty(req_rows, mask_rows, milli_mul, alpha: float):
     return out
 
 
-def _queue_order(a, Q):
+def _queue_order(a, Q, ts=None):
     """Pending workloads in queueOrderingFunc order per segment: (order, start[S+1], seg_start[Q+1], seg_lq[S]).  A
     segment is a ClusterQueue, or one LocalQueue of a ClusterQueue with AdmissionFairSharing (numbered
     ClusterQueue-major)."""
@@ -470,7 +557,7 @@ def _queue_order(a, Q):
     else:
         seg_start, seg_lq, seg = np.arange(Q + 1), np.full(Q, -1, np.int64), cq
     S = int(seg_start[-1])
-    order = np.lexsort((a["wl_uid"], a["wl_ts"], -a["wl_priority"].astype(np.int64), seg))
+    order = np.lexsort((a["wl_uid"], a["wl_ts"] if ts is None else ts, -a["wl_priority"].astype(np.int64), seg))
     start = np.zeros(S + 1, np.int64)
     np.add.at(start, seg + 1, 1)
     return order, np.cumsum(start), seg_start, seg_lq
@@ -479,7 +566,18 @@ def _queue_order(a, Q):
 def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.CycleOut], max_cycles: int = 10_000) -> DrainResult:
     a = snap.arrays
     Q, R, FR = snap.n_cq, snap.n_resource, snap.n_fr
-    order, qstart, seg_start, seg_lq = _queue_order(a, Q)
+    checks = "wl_check_ns" in a
+    qts = a["wl_ts"].astype(np.int64).copy()                      # queue-order timestamps (admission checks: mutable)
+    if checks:
+        if "adm_wl" not in a:
+            raise ValueError("wl_check_ns needs adm_wl")
+        held0 = np.zeros(snap.n_wl, bool)
+        held0[a["adm_wl"].astype(np.int64)] = True
+        if "wl_check_evict_ns" in a:
+            ce = a["wl_check_evict_ns"].astype(np.int64)
+            qts = np.where((ce != UNSET) & ~held0, ce, qts)
+    order, qstart, seg_start, seg_lq = _queue_order(a, Q, qts)
+    sort_ts = qts.copy()                                          # the keys the order was built with
     qlen = np.diff(qstart)
     afs_cq = a["cq_afs"].astype(bool) if "wl_lq" in a else np.zeros(Q, bool)
     replay = "adm_wl" in a
@@ -510,6 +608,26 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 adm_finish[evicting] = a["adm_evict_end_ns"][evicting]
     if replay:
         state[a["adm_wl"].astype(np.int64)] = HELD  # holds quota: out of every queue
+    if checks:  # rule 1: attempt state; start state of the rows whose checks run and of the records in backoff
+        chk_ns = a["wl_check_ns"].astype(np.int64)
+        chk_fail = a["wl_check_fail"].astype(np.int64).copy() if "wl_check_fail" in a else np.zeros(snap.n_wl, np.int64)
+        retries = a["wl_check_retries"].astype(np.int64).copy() if "wl_check_retries" in a else np.zeros(snap.n_wl, np.int64)
+        requeue_at = np.full(snap.n_wl, UNSET, np.int64)
+        if "wl_requeue_at_ns" in a:
+            ra = a["wl_requeue_at_ns"].astype(np.int64)
+            state[ra > snap.now_ns] = BACKOFF
+            requeue_at[ra > snap.now_ns] = ra[ra > snap.now_ns]
+        checking = np.zeros(snap.n_adm, bool)
+        if "adm_check_end_ns" in a:
+            ce = a["adm_check_end_ns"].astype(np.int64)
+            checking = ce != UNSET
+            adm_finish[checking] = ce[checking]
+        ready_ns = np.full(snap.n_wl, UNSET, np.int64)
+        deactivated = np.zeros(snap.n_wl, np.uint8)
+        base_s, max_s, limit = int(snap.check_backoff_base_s), int(snap.check_backoff_max_s), int(snap.check_backoff_limit)
+        verdicts = {"ready": 0, "retry": [], "rejected": []}
+    else:
+        checking = None
     sticky = a["cq_sticky"].astype(np.int64).copy() if "cq_sticky" in a else None  # sticky workload per ClusterQueue
     cursor = np.zeros(len(qlen), np.int64)
     first_aside = qlen.copy()                                     # smallest SET_ASIDE position per segment (qlen = none)
@@ -616,7 +734,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
 
     def remove_rows(rows):
         """rows leave the admitted tables (cache.DeleteWorkload: cells out of the usage; the other rows keep their order)"""
-        nonlocal adm_wl, adm_finish, adm_lq, evicting
+        nonlocal adm_wl, adm_finish, adm_lq, evicting, checking
         us, uf, uq = adm["adm_use_start"], adm["adm_use_fr"], adm["adm_use_qty"]
         for row in rows:
             cqi = int(adm["adm_cq"][row])
@@ -638,6 +756,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             adm_lq = adm_lq[keep]
         if evicting is not None:
             evicting = evicting[keep]
+        if checking is not None:
+            checking = checking[keep]
 
     def release(w):
         """the record of an evicted row returns to its queue with LastAssignment nil (workload_controller.go:973-1004);
@@ -655,11 +775,78 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         e = int(adm_finish.min()) if len(adm_finish) else NEVER
         if arr_next < len(arr_order):
             e = min(e, int(create[arr_order[arr_next]]))
+        if checks and (state == BACKOFF).any():
+            e = min(e, int(requeue_at[state == BACKOFF].min()))
         return None if e >= NEVER else e
+
+    def enqueue(w):
+        """step 6 for one record: PushOrUpdate, with the NoFit rule of a BestEffortFIFO ClusterQueue"""
+        q = int(a["wl_cq"][w])
+        if shash is not None and nofit.arrival_goes_aside(q, bool(strict[q]), int(shash[w])):
+            set_aside(w)
+        else:
+            state[w] = QUEUED
+            cursor[seg_of[w]] = min(cursor[seg_of[w]], pos_of[w])
+
+    def apply_verdicts(t_next, notified):
+        """rule 2: the verdicts due by t_next, before the completions"""
+        gone = []
+        for row in np.flatnonzero(checking & (adm_finish <= t_next)):
+            w, tv = int(adm_wl[row]), int(adm_finish[row])
+            checking[row] = False
+            if chk_fail[w] == 0:  # Ready: Admitted, the run clock starts
+                ready_ns[w] = tv
+                adm_finish[row] = finish_time(tv, int(run_ns[w])) if run_ns is not None else NEVER
+                verdicts["ready"] += 1
+                continue
+            if chk_fail[w] != ALL_FAIL:
+                chk_fail[w] -= 1
+            k = int(retries[w]) + 1
+            gone.append(row)
+            notified.add(int(adm["adm_cq"][row]))
+            last_gen[w] = -1
+            last_tried[int(ps_start[w]):int(ps_start[w + 1])] = -1
+            if has_qr is not None:
+                has_qr[w] = 0
+            admit_cycle[w] = -1
+            if k <= limit:  # Retry: backoff, then requeued with the eviction time as its queue-order timestamp
+                retries[w] = k
+                state[w] = BACKOFF
+                requeue_at[w] = min(tv + check_wait_s(k, base_s, max_s) * 1_000_000_000, NEVER)
+                qts[w] = tv
+                verdicts["retry"].append(w)
+            else:  # Rejected: deactivated
+                state[w] = DEACTIVATED
+                deactivated[w] = 1
+                verdicts["rejected"].append(w)
+        if gone:
+            remove_rows(gone)
+
+    def resort():
+        """rule 6: rebuild the order when a queued or set-aside record carries a key other than the one it was sorted by"""
+        nonlocal order, qstart, sort_ts
+        if not checks or not (((state == QUEUED) | (state == SET_ASIDE)) & (qts != sort_ts)).any():
+            return
+        order, qstart, _, _ = _queue_order(a, Q, qts)
+        sort_ts = qts.copy()
+        for s in range(len(qlen)):
+            seg_of[order[qstart[s]:qstart[s + 1]]] = s
+            pos_of[order[qstart[s]:qstart[s + 1]]] = np.arange(qlen[s])
+            cursor[s] = 0
+            advance(s)
+            seg = order[qstart[s]:qstart[s + 1]]
+            aside = np.flatnonzero(state[seg] == SET_ASIDE)
+            first_aside[s] = int(aside[0]) if len(aside) else qlen[s]
+        res.n_resorts += 1
+        res.resort_orders.append(dict(order=order.copy(), qstart=qstart.copy(), qts=qts.copy(), state=state.copy(),
+                                      cursor=cursor.copy(), first_aside=first_aside.copy(), seg_of=seg_of.copy(),
+                                      pos_of=pos_of.copy()))
 
     def apply_events(t_next, notified):
         """steps 5 and 6 at t_next; returns (finished records, arrived records, records whose eviction completed)"""
         nonlocal arr_next
+        if checks:
+            apply_verdicts(t_next, notified)
         done = np.flatnonzero(adm_finish <= t_next)
         gone = evicting[done] if evicting is not None else np.zeros(len(done), bool)
         fin, released = adm_wl[done[~gone]].copy(), adm_wl[done[gone]].copy()
@@ -680,13 +867,12 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         arr = []
         while arr_next < len(arr_order) and int(create[arr_order[arr_next]]) <= t_next:
             w = int(arr_order[arr_next]); arr_next += 1
-            q = int(a["wl_cq"][w])
-            if shash is not None and nofit.arrival_goes_aside(q, bool(strict[q]), int(shash[w])):
-                set_aside(w)
-            else:
-                state[w] = QUEUED
-                cursor[seg_of[w]] = min(cursor[seg_of[w]], pos_of[w])
+            enqueue(w)
             arr.append(w)
+        if checks:  # rule 3: the records whose RequeueAt has come
+            for w in np.flatnonzero((state == BACKOFF) & (requeue_at <= t_next)):
+                requeue_at[w] = UNSET
+                enqueue(int(w))
         return fin, np.asarray(arr, np.int64), released
 
     def requeue(notified):
@@ -710,6 +896,13 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         if res.cycles:
             res.finished[-1] = np.concatenate([res.finished[-1], fin]); res.arrived[-1] = np.concatenate([res.arrived[-1], arr])
             res.evict_done[-1] = np.concatenate([res.evict_done[-1], released])
+        if checks:
+            ret, rej = np.asarray(verdicts["retry"], np.int64), np.asarray(verdicts["rejected"], np.int64)
+            res.n_check_ready += verdicts["ready"]; res.n_check_retry += len(ret); res.n_check_rejected += len(rej)
+            if res.cycles:
+                res.check_retry[-1] = np.concatenate([res.check_retry[-1], ret])
+                res.check_rejected[-1] = np.concatenate([res.check_rejected[-1], rej])
+            verdicts.update(ready=0, retry=[], rejected=[])
 
     t = int(snap.now_ns)
     cyc = 0
@@ -733,6 +926,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             after(*apply_events(t, notified))
             if notified:
                 requeue(notified)
+            resort()
             continue
         segs = hseg[live]
         heads = order[qstart[segs] + cursor[segs]]  # global pending indices, one per ClusterQueue with work left
@@ -749,8 +943,9 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         cs.set("cq_usage", usage)
         for k, v in adm.items():
             cs.set(k, v)
-        for nm in ("wl_cq", "wl_priority", "wl_ts", "wl_uid"):
+        for nm in ("wl_cq", "wl_priority", "wl_uid"):
             cs.set(nm, a[nm][heads])
+        cs.set("wl_ts", qts[heads])  # the queue-order timestamp (rule 6)
         cs.set("wl_last_gen", last_gen[heads])
         if has_qr is not None:
             cs.set("wl_has_quota_reservation", has_qr[heads])
@@ -770,6 +965,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         res.sticky_heads.append(np.asarray(chosen, np.int64))
         res.cycle_start_ns.append(t)
         res.finished.append(np.zeros(0, np.int64)); res.arrived.append(np.zeros(0, np.int64)); res.evict_done.append(np.zeros(0, np.int64))
+        res.check_retry.append(np.zeros(0, np.int64)); res.check_rejected.append(np.zeros(0, np.int64))
         ok = dec == abi.DEC_ASSUMED
         res.admitted.append(heads[ok])
         # ---- apply the admissions: Assignment.Usage (flavorassigner.go:198-218) with the admitted counts
@@ -832,8 +1028,15 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 adm_wl = np.concatenate([adm_wl, g])
             if decay:
                 adm_lq = np.concatenate([adm_lq, a["wl_lq"][g].astype(np.int64)])
+            if checks:  # rules 1 and 4: a check delay starts an attempt, a delay of 0 is Ready at once
+                qts[g] = a["wl_ts"][g]
+                chk = chk_ns[g] > 0
+                checking = np.concatenate([checking, chk])
+                ready_ns[g[~chk]] = t
             if events:
                 fin_new = [finish_time(t, int(run_ns[w])) if run_ns is not None else NEVER for w in g]
+                if checks:
+                    fin_new = [min(t + int(chk_ns[w]), NEVER) if chk_ns[w] > 0 else f for w, f in zip(g, fin_new)]
                 adm_finish = np.concatenate([adm_finish, np.asarray(fin_new, np.int64)])
             if evicting is not None:
                 evicting = np.concatenate([evicting, np.zeros(n_new, bool)])
@@ -894,6 +1097,9 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 evicting[row] = True
                 adm["adm_evicted"][row] = 1
                 adm_finish[row] = min(t + int(lat[w]), NEVER)
+                if checking is not None and checking[row]:  # rule 5: no pods, released at the next boundary
+                    checking[row] = False
+                    adm_finish[row] = t
                 evictions[w] += 1
         elif victims:
             for row in victims:
@@ -924,6 +1130,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         after(*apply_events(t, notified))
         if notified:
             requeue(notified)
+        resort()
     res.cq_usage = usage
     res.wl_evictions = evictions
     res.wl_admit_cycle = admit_cycle
@@ -937,6 +1144,10 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     res.wl_finish_ns = finish_ns
     res.end_ns = t
     res.cq_sticky = sticky
+    if checks:
+        res.wl_ready_ns, res.wl_check_retries, res.wl_deactivated = ready_ns, retries, deactivated
+        res.wl_queue_ts = qts
+        res.adm["adm_checking"] = checking
     if decay:
         res.lq_consumed = consumed.astype(np.int64)
         res.lq_consumed_scale = cscale.astype(np.int32)

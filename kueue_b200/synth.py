@@ -300,6 +300,25 @@ def add_evict_latency(snap: abi.FlatSnapshot, ns_range=(0, 0), seed: int = 0) ->
     return snap
 
 
+def add_admission_checks(snap: abi.FlatSnapshot, seed: int = 0, delay_ns=(1_000, 5_000), fail_share: float = 0.3,
+                         max_fail: int = 2, all_fail_share: float = 0.05, cqs=None, backoff=(1, 8, 3)) -> abi.FlatSnapshot:
+    """Admission checks of an event drain (include/kueue_b200.h) on a snapshot with `adm_wl`, seeded: the workloads of
+    the ClusterQueues `cqs` (None = all) get a check delay uniform in `delay_ns` (inclusive; 0 elsewhere); a share
+    `fail_share` of them fails its next 1..max_fail attempts and a share `all_fail_share` every attempt.  `backoff` is
+    the RetryStrategy (base s, max s, limit)."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    W = snap.n_wl
+    on = np.ones(W, bool) if cqs is None else np.isin(snap.arrays["wl_cq"], np.asarray(cqs))
+    delay = np.where(on, rng.integers(int(delay_ns[0]), int(delay_ns[1]) + 1, W), 0)
+    u = rng.random(W)
+    fail = np.where(u < fail_share, rng.integers(1, max_fail + 1, W), 0)
+    fail = np.where(u > 1 - all_fail_share, np.iinfo(np.int32).max, fail)
+    snap.set("wl_check_ns", delay)
+    snap.set("wl_check_fail", np.where(on, fail, 0))
+    snap.check_backoff_base_s, snap.check_backoff_max_s, snap.check_backoff_limit = (int(v) for v in backoff)
+    return snap
+
+
 # The reference's scheduler performance scenario (test/performance/scheduler/configs/baseline/generator.yaml, generated
 # by runner/generator/generator.go): 5 cohorts of 6 ClusterQueues, one flavor, cpu only; per ClusterQueue, workload k of
 # a class is created at (k + 1) * interval and runs `run` once admitted (runner/controller/controller.go).
@@ -313,13 +332,15 @@ PERF_NOMINAL_CPU, PERF_BORROW_CPU = 20, 100
 _MS = 1_000_000
 
 
-def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None = None) -> abi.FlatSnapshot:
+def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None = None, checks: int | None = None) -> abi.FlatSnapshot:
     """The baseline scenario as numbers (15,000 workloads at scale 1; `scale` multiplies the count of every class):
     nominal 20 cpu and borrowingLimit 100 cpu per ClusterQueue, preemption reclaimWithinCohort Any and
     withinClusterQueue LowerPriority, BestEffortFIFO.  cpu is in milli-units.  wl_ts is the creation time, an empty
     adm_wl turns eviction replay on, and `snap.perf_class` holds each workload's index into PERF_CLASSES.  One drain cycle takes cycle_ns of simulated time.
     evict_ns: the termination latency of every workload (wl_evict_ns: an eviction releases its quota that long after it
-    is issued); None = every eviction completes before the next cycle."""
+    is issued); None = every eviction completes before the next cycle.
+    checks: a seed: every other ClusterQueue of each cohort gets an admission check (add_admission_checks: a
+    ProvisioningRequest-like delay of 20-200 ms, a share of failing attempts, backoff base 1 s, max 8 s, limit 3)."""
     Q = PERF_COHORTS * PERF_CQS_PER_COHORT
     snap = abi.FlatSnapshot(n_cq=Q, n_cohort=PERF_COHORTS, n_flavor=1, n_resource=1)
     snap.set("parent", np.concatenate([Q + np.arange(Q) // PERF_CQS_PER_COHORT, np.full(PERF_COHORTS, -1)]))
@@ -349,6 +370,8 @@ def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None 
         snap.set("wl_evict_ns", np.full(W, evict_ns))
     snap.now_ns = 0
     snap.drain_cycle_ns = cycle_ns
+    if checks is not None:
+        add_admission_checks(snap, checks, delay_ns=(20 * _MS, 200 * _MS), cqs=np.arange(0, Q, 2))
     snap.finalize()
     snap.__dict__["perf_class"] = np.asarray(cls, np.int64)
     return snap
