@@ -354,7 +354,8 @@ typedef struct kb_snapshot {
      eviction time (GetQueueOrderTimestamp, workload.go:1180-1182).  Rejected deactivates the workload.  wl_check_ns ==
      NULL: off, and every launch, copy and result of the drain stays as without this block.  A non-NULL wl_check_ns turns
      on event mode.  With the tables wl_ts is the creation timestamp.  See kb_run_drain.  Errors: KB_ERR_INVALID for any
-     table of this block without adm_wl or without wl_check_ns, wl_check_ns[w] < 0, wl_check_fail[w] < 0,
+     table of this block without adm_wl or without wl_check_ns (wl_requeue_at_ns is also accepted with
+     wl_pods_ready_ns), wl_check_ns[w] < 0, wl_check_fail[w] < 0,
      wl_check_retries[w] < 0, adm_check_end_ns[a] <= now_ns on a row (INT64_MIN excepted), wl_requeue_at_ns on a record
      named by adm_wl or created after now_ns, a row with a check under way that also has an eviction under way (adm_evicted
      with adm_evict_end_ns), check_backoff_base_s <= 0, check_backoff_max_s < 0, check_backoff_limit < 0;
@@ -371,6 +372,32 @@ typedef struct kb_snapshot {
   int32_t check_backoff_base_s;     /* RetryStrategy.BackoffBaseSeconds (> 0)                                            */
   int32_t check_backoff_max_s;      /* RetryStrategy.BackoffMaxSeconds (0 = no cap)                                      */
   int32_t check_backoff_limit;      /* RetryStrategy.BackoffLimitCount (>= 0)                                            */
+
+  /* ---- WaitForPodsReady (optional; read by kb_run_drain only, kb_run_cycle ignores them) ----
+     In the reference a workload whose pods are not all Ready within waitForPodsReady.timeout of its Admitted condition
+     is evicted (reason PodsReadyTimeout), so it stops holding quota it cannot use; it is requeued after an exponential
+     backoff (requeuingStrategy) and deactivated once backoffLimitCount is exceeded (workload_controller.go:805-855,
+     workload.go:707-722; defaults apis/config/v1beta2/defaults.go:95-100, validation pkg/config/validation.go:196-230).
+     wl_pods_ready_ns == NULL: off, and every launch, copy and result of the drain stays as without this block.  A
+     non-NULL wl_pods_ready_ns turns on event mode and needs adm_wl.  The block composes with admission checks (the
+     attempt starts at the Ready verdict), eviction latency, the sticky table and AFS with or without decay.  See
+     kb_run_drain.  blockAdmission: true is not modelled (a caller keeps its own path for it).  Errors: KB_ERR_INVALID
+     for any table of this block without adm_wl or without wl_pods_ready_ns, a negative delay, fail or count,
+     pods_ready_timeout_ns <= 0, a backoff base or max < 0, a limit < -1, pods_ready_requeue_creation outside {0, 1},
+     adm_admitted_ns[a] > now_ns (INT64_MIN excepted) or set on a row whose checks run (adm_check_end_ns) or whose
+     eviction is under way (adm_evicted with adm_evict_end_ns), wl_pods_ready_evict_ns on a record named by adm_wl or
+     on one that also has wl_check_evict_ns (a workload has one Evicted condition). */
+  const int64_t *wl_pods_ready_ns;       /* [n_wl] Admitted -> PodsReady delay of an attempt that becomes ready          */
+  const int32_t *wl_pods_ready_fail;     /* [n_wl] next attempts that never become ready; INT32_MAX = all; NULL = 0     */
+  const int32_t *wl_pods_ready_count;    /* [n_wl] Status.RequeueState.Count at the start; NULL = 0                      */
+  const int64_t *wl_pods_ready_evict_ns; /* [n_wl] Evicted LastTransitionTime of a record last evicted by a timeout, read
+                                            under the Eviction timestamp only; INT64_MIN = not; NULL = none              */
+  const int64_t *adm_admitted_ns;        /* [n_adm] Admitted time of a row whose pods are not ready yet; INT64_MIN = ready */
+  int64_t pods_ready_timeout_ns;         /* waitForPodsReady.timeout (> 0)                                                */
+  int32_t pods_ready_backoff_base_s;     /* requeuingStrategy.backoffBaseSeconds (>= 0)                                  */
+  int32_t pods_ready_backoff_max_s;      /* requeuingStrategy.backoffMaxSeconds (>= 0; 0 = no cap)                       */
+  int32_t pods_ready_backoff_limit;      /* requeuingStrategy.backoffLimitCount; -1 = nil (requeue forever)              */
+  int32_t pods_ready_requeue_creation;   /* requeuingStrategy.timestamp: 0 = Eviction (default), 1 = Creation            */
 } kb_snapshot;
 
 /* ------------------------------------------------------------------------
@@ -599,7 +626,48 @@ int32_t kb_download(kb_handle *h, kb_cycle_out *out);
  * WaitTime(k) is wait.NewBackoff(base, max, 2, 0.0001).WaitTime(k) truncated to whole seconds (kb_drain.cuh
  * kb_check_wait_ns; exact below 10,000 s): min(check_backoff_base_s * 2^(k-1), check_backoff_max_s or infinity), except
  * that with base > max > 0 the first Step returns the base uncapped (attempt 1 waits base, later ones max).  Verdicts
- * applied between the start of cycle c and of c+1 count in cycle_check_retry / cycle_check_rejected[c]. */
+ * applied between the start of cycle c and of c+1 count in cycle_check_retry / cycle_check_rejected[c].
+ *
+ * WaitForPodsReady (kb_snapshot.wl_pods_ready_ns != NULL, with adm_wl; event mode).  It uses the BACKOFF and
+ * DEACTIVATED states, RequeueAt, the queue-order timestamp and the re-sort of the admission checks above.  An attempt is
+ * one admission of a workload.  Additions to the loop:
+ *   1. the attempt starts at Admitted: the reservation at t_c when the workload has no check delay, else the Ready
+ *      verdict time;
+ *   2. it fails if the record has failures left in wl_pods_ready_fail (it uses up one; INT32_MAX = every attempt fails)
+ *      or wl_pods_ready_ns > pods_ready_timeout_ns; otherwise it is ready.  A delay equal to the timeout is ready (a
+ *      canonical tie-break).  A ready attempt reaches PodsReady at Admitted + wl_pods_ready_ns (wl_pods_ready_at_ns) and
+ *      finishes at PodsReady + wl_run_ns (saturating): no event is added.  With every delay 0 this is the finish without
+ *      the block;
+ *   3. a failing attempt has an event at T = Admitted + pods_ready_timeout_ns (saturating; E includes it), applied in
+ *      step 5 after that boundary's check verdicts (a Ready verdict and its timeout can fall in one boundary) and before
+ *      its completions (workload_controller.go:805-835,1106-1130).  With pods_ready_backoff_limit >= 0 and Count + 1 >
+ *      limit it is a deactivation (triggerDeactivation :840-855): Count = 0, the record will be DEACTIVATED and
+ *      wl_deactivated = 1.  Otherwise (UpdateRequeueState workload.go:707-722) Count += 1 (saturating at INT32_MAX),
+ *      RequeueAt = T + WaitTime(Count) (saturating), and under the Eviction timestamp the queue timestamp becomes T
+ *      (GetQueueOrderTimestamp workload.go:1174-1182; under Creation it is unchanged);
+ *   4. the timed-out row is evicted at T.  With wl_evict_ns it gets adm_evicted and the end time T + wl_evict_ns: it keeps
+ *      its cells, stays a preemption candidate, and a preemptor that targets it is ongoing (as for an evicting row).
+ *      Without, it is released at the boundary that applies T.  At release its cells leave the usage, the row is
+ *      removed, its root tree is marked, and the record goes to DEACTIVATED or to BACKOFF with LastAssignment nil; a
+ *      BACKOFF record is queued by rule 3 of the admission checks (at RequeueAt, in that same boundary when RequeueAt
+ *      <= t_{c+1}, NoFit rule included);
+ *   5. a row preempted while its attempt waits for PodsReady (before PodsReady, or before T) loses the attempt: it is not
+ *      counted, uses up no failure (workload_controller.go:808-811), and wl_pods_ready_at_ns keeps its previous value.
+ *      The row is released like any preempted row, with its pods' latency;
+ *   6. an admission resets the queue timestamp to wl_ts; Count survives a ready attempt;
+ *   7. start state: wl_pods_ready_count (Count), adm_admitted_ns (rows whose pods are not ready: their attempt runs from
+ *      there by rules 2-3, in place of adm_finish_ns), wl_requeue_at_ns (records in backoff) and wl_pods_ready_evict_ns
+ *      (the queue timestamp under Eviction of a record adm_wl does not name);
+ *   8. with every wl_pods_ready_ns = 0, every wl_pods_ready_fail = 0 and no start-state tables the drain equals the drain
+ *      without the block.
+ * WaitTime(k) is the jitter-free Backoff.WaitTime of wait.NewBackoff(base_s, max_s, 2, 0.0001) in nanoseconds (kb_drain.cuh
+ * kb_pods_ready_wait_ns):
+ * min(base * 2^(k-1), max, or MaxInt64 / 2 with max 0), the base uncapped for k = 1, and 0 with base 0.  The reference
+ * adds a random jitter below wait * 1e-4 and stores RequeueAt at second precision; the drain takes the jitter-free value.
+ * Timeouts applied between the start of cycle c and of c+1 count in cycle_pods_ready_timeout / _deactivated[c].
+ * Not modelled: waitForPodsReady.blockAdmission (the reference stops the admit loop mid-cycle until every admitted
+ * workload is ready, scheduler.go:361-373, which a cycle evaluated at one instant cannot express) and recoveryTimeout
+ * (the drain models no pod failure after PodsReady). */
 typedef struct kb_drain_out {
   int32_t max_cycles;        /* in */
   int32_t n_cycles;          /* out: cycles run */
@@ -651,9 +719,19 @@ typedef struct kb_drain_out {
   int32_t *cycle_check_rejected; /* [max_cycles] Rejected verdicts, likewise */
   int64_t *wl_ready_ns;          /* [n_wl] time of the last Admitted in the drain, INT64_MIN if none */
   int32_t *wl_check_retries_out; /* [n_wl] final RetryCount */
-  uint8_t *wl_deactivated;       /* [n_wl] 1 if the workload was deactivated (Rejected) */
+  uint8_t *wl_deactivated;       /* [n_wl] 1 if the workload was deactivated (Rejected, or RequeuingLimitExceeded with
+                                    kb_snapshot.wl_pods_ready_ns, which also writes it and the two fields below) */
   int64_t n_resorts;             /* out: queue re-sorts (a record entered its queue with a new queue-order timestamp) */
   double resort_ms;              /* out: device time of those re-sorts (part of gpu_ms) */
+  /* WaitForPodsReady (kb_snapshot.wl_pods_ready_ns != NULL; zero / untouched otherwise; each pointer may be NULL).
+     n_evicted, wl_evictions and n_evict_done keep counting preemptions only. */
+  int64_t n_pods_ready_timeout;          /* out: timeouts that requeue (deactivations excluded), those before cycle 0 included */
+  int64_t n_pods_ready_deactivated;      /* out: timeouts past the requeue limit */
+  int32_t *cycle_pods_ready_timeout;     /* [max_cycles] timeouts applied from the start of cycle c to the start of c+1 */
+  int32_t *cycle_pods_ready_deactivated; /* [max_cycles] deactivations, likewise */
+  int64_t *wl_pods_ready_at_ns;          /* [n_wl] PodsReady time of the last attempt that reached it, or will (a row still
+                                            waiting at the end of the drain); INT64_MIN if none */
+  int32_t *wl_pods_ready_count_out;      /* [n_wl] final RequeueState.Count */
 } kb_drain_out;
 int32_t kb_run_drain(kb_handle *h, const kb_snapshot *s, kb_drain_out *out);
 

@@ -373,6 +373,14 @@ func (s *Scheduler) flatten(snap *schdcache.Snapshot, heads []workload.Info, gen
 	//   c.wl_check_ns, c.wl_check_fail, c.wl_check_retries = cp64(chkNs), cp32(chkFail), cp32(retryCount)
 	//   c.wl_check_evict_ns, c.wl_requeue_at_ns, c.adm_check_end_ns = cp64(evictedAt), cp64(requeueAt), cp64(checkEnd)
 	//   c.check_backoff_base_s, c.check_backoff_max_s, c.check_backoff_limit = base, max, limit
+	// WaitForPodsReady (INTEGRATION.md): a modelled PodsReady delay and fail count per workload, the settings from
+	// Configuration.WaitForPodsReady (timeout, RequeuingStrategy; BlockAdmission true keeps the Go path), and the start
+	// state from Status.RequeueState.Count / RequeueAt and the Admitted, PodsReady and Evicted (reason PodsReadyTimeout)
+	// conditions:
+	//   c.wl_pods_ready_ns, c.wl_pods_ready_fail, c.wl_pods_ready_count = cp64(readyNs), cp32(readyFail), cp32(requeueCount)
+	//   c.wl_pods_ready_evict_ns, c.adm_admitted_ns = cp64(timeoutEvictedAt), cp64(admittedNotReadyAt)
+	//   c.pods_ready_timeout_ns, c.pods_ready_backoff_base_s, c.pods_ready_backoff_max_s = timeout, base, max
+	//   c.pods_ready_backoff_limit, c.pods_ready_requeue_creation = limitOrMinus1, creation
 	// They stay nil here: a single cycle ignores them.
 	if anyGroup { // optional table: NULL when no podset is grouped
 		c.ps_group = cp32(psGroup)

@@ -87,6 +87,10 @@ class kb_snapshot(C.Structure):
         ("wl_check_ns", _P(C.c_int64)), ("wl_check_fail", _P(C.c_int32)), ("wl_check_retries", _P(C.c_int32)),
         ("wl_check_evict_ns", _P(C.c_int64)), ("wl_requeue_at_ns", _P(C.c_int64)), ("adm_check_end_ns", _P(C.c_int64)),
         ("check_backoff_base_s", C.c_int32), ("check_backoff_max_s", C.c_int32), ("check_backoff_limit", C.c_int32),
+        ("wl_pods_ready_ns", _P(C.c_int64)), ("wl_pods_ready_fail", _P(C.c_int32)), ("wl_pods_ready_count", _P(C.c_int32)),
+        ("wl_pods_ready_evict_ns", _P(C.c_int64)), ("adm_admitted_ns", _P(C.c_int64)),
+        ("pods_ready_timeout_ns", C.c_int64), ("pods_ready_backoff_base_s", C.c_int32), ("pods_ready_backoff_max_s", C.c_int32),
+        ("pods_ready_backoff_limit", C.c_int32), ("pods_ready_requeue_creation", C.c_int32),
     ]
 
 
@@ -142,6 +146,9 @@ class kb_drain_out(C.Structure):
         ("cycle_check_retry", _P(C.c_int32)), ("cycle_check_rejected", _P(C.c_int32)),
         ("wl_ready_ns", _P(C.c_int64)), ("wl_check_retries_out", _P(C.c_int32)), ("wl_deactivated", _P(C.c_uint8)),
         ("n_resorts", C.c_int64), ("resort_ms", C.c_double),
+        ("n_pods_ready_timeout", C.c_int64), ("n_pods_ready_deactivated", C.c_int64),
+        ("cycle_pods_ready_timeout", _P(C.c_int32)), ("cycle_pods_ready_deactivated", _P(C.c_int32)),
+        ("wl_pods_ready_at_ns", _P(C.c_int64)), ("wl_pods_ready_count_out", _P(C.c_int32)),
     ]
 
 
@@ -200,12 +207,14 @@ _DT = {
     "cq_sticky": np.int32,
     "wl_check_ns": np.int64, "wl_check_fail": np.int32, "wl_check_retries": np.int32, "wl_check_evict_ns": np.int64,
     "wl_requeue_at_ns": np.int64, "adm_check_end_ns": np.int64,
+    "wl_pods_ready_ns": np.int64, "wl_pods_ready_fail": np.int32, "wl_pods_ready_count": np.int32,
+    "wl_pods_ready_evict_ns": np.int64, "adm_admitted_ns": np.int64,
 }
 # AdmissionFairSharing tables (include/kueue_b200.h): wl_lq absent = AFS off
 AFS_FIELDS = ("wl_lq", "lq_cq", "cq_afs", "lq_weight", "lq_consumed", "lq_consumed_scale", "lq_penalty", "afs_res_weight",
               "afs_milli_mul")
 # arrivals and completions of kb_run_drain's event mode (include/kueue_b200.h): all absent = event mode off
-EVENT_FIELDS = ("wl_create_ns", "wl_run_ns", "adm_finish_ns", "wl_evict_ns", "wl_check_ns")
+EVENT_FIELDS = ("wl_create_ns", "wl_run_ns", "adm_finish_ns", "wl_evict_ns", "wl_check_ns", "wl_pods_ready_ns")
 # decay of the AdmissionFairSharing consumed usage in event mode (include/kueue_b200.h): lq_last_update_ns absent = off
 AFS_DECAY_FIELDS = ("lq_last_update_ns", "adm_lq")
 # end times of the evictions under way before an event drain with wl_evict_ns (include/kueue_b200.h): absent = none known
@@ -214,8 +223,11 @@ EVICT_END_FIELDS = ("adm_evict_end_ns",)
 STICKY_FIELDS = ("cq_sticky",)
 # admission checks in event mode (include/kueue_b200.h): wl_check_ns absent = off; the others need it
 CHECK_FIELDS = ("wl_check_ns", "wl_check_fail", "wl_check_retries", "wl_check_evict_ns", "wl_requeue_at_ns", "adm_check_end_ns")
+# WaitForPodsReady in event mode (include/kueue_b200.h): wl_pods_ready_ns absent = off; the others need it
+PODS_READY_FIELDS = ("wl_pods_ready_ns", "wl_pods_ready_fail", "wl_pods_ready_count", "wl_pods_ready_evict_ns", "adm_admitted_ns")
 OPTIONAL_FIELDS = (("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows", "adm_wl") + AFS_FIELDS +
-                   EVENT_FIELDS + AFS_DECAY_FIELDS + EVICT_END_FIELDS + STICKY_FIELDS + CHECK_FIELDS)  # NULL in kb_snapshot when absent
+                   EVENT_FIELDS + AFS_DECAY_FIELDS + EVICT_END_FIELDS + STICKY_FIELDS + CHECK_FIELDS +
+                   PODS_READY_FIELDS)  # NULL in kb_snapshot when absent
 ARRAY_FIELDS = list(_DT.keys())
 # tables the library keeps resident while kb_snapshot.static_generation is unchanged (include/kueue_b200.h)
 STATIC_FIELDS = ("parent", "fair_weight", "nominal", "borrow_limit", "lend_limit", "cq_within_cq", "cq_reclaim_within",
@@ -250,6 +262,11 @@ class FlatSnapshot:
     check_backoff_base_s: int = 60    # kb_snapshot.check_backoff_*: the admission checks' RetryStrategy (defaults of
     check_backoff_max_s: int = 1800   # ProvisioningRequestConfig, provisioningrequestconfig_types.go:123-154)
     check_backoff_limit: int = 3
+    pods_ready_timeout_ns: int = 300_000_000_000  # kb_snapshot.pods_ready_*: waitForPodsReady (timeout 5 min and the
+    pods_ready_backoff_base_s: int = 60           # requeuingStrategy defaults, apis/config/v1beta2/defaults.go:95-100;
+    pods_ready_backoff_max_s: int = 3600          # limit -1 = nil, creation 0 = the Eviction timestamp)
+    pods_ready_backoff_limit: int = -1
+    pods_ready_requeue_creation: int = 0
     arrays: dict = field(default_factory=dict)
 
     def __getattr__(self, name):
@@ -333,6 +350,11 @@ class FlatSnapshot:
     @property
     def n_rg(self): return len(self.arrays["rg_res_mask"])
 
+    def _pods_ready_scalars(self, s: kb_snapshot) -> None:
+        s.pods_ready_timeout_ns = self.pods_ready_timeout_ns
+        s.pods_ready_backoff_base_s, s.pods_ready_backoff_max_s = self.pods_ready_backoff_base_s, self.pods_ready_backoff_max_s
+        s.pods_ready_backoff_limit, s.pods_ready_requeue_creation = self.pods_ready_backoff_limit, self.pods_ready_requeue_creation
+
     def head_podsets(self) -> int:
         st = self.arrays["wl_ps_start"]; h = self.arrays["heads"]
         return int((st[h + 1] - st[h]).sum()) if len(h) else 0
@@ -348,6 +370,7 @@ class FlatSnapshot:
             s.afs_half_life_ns, s.afs_sampling_ns = self.afs_half_life_ns, self.afs_sampling_ns
             s.check_backoff_base_s, s.check_backoff_max_s = self.check_backoff_base_s, self.check_backoff_max_s
             s.check_backoff_limit = self.check_backoff_limit
+            self._pods_ready_scalars(s)
             return s
         s = kb_snapshot()
         s.n_cq, s.n_cohort, s.n_flavor, s.n_resource = self.n_cq, self.n_cohort, self.n_flavor, self.n_resource
@@ -363,6 +386,7 @@ class FlatSnapshot:
         s.afs_half_life_ns, s.afs_sampling_ns = self.afs_half_life_ns, self.afs_sampling_ns
         s.check_backoff_base_s, s.check_backoff_max_s = self.check_backoff_base_s, self.check_backoff_max_s
         s.check_backoff_limit = self.check_backoff_limit
+        self._pods_ready_scalars(s)
         for name in ARRAY_FIELDS:
             if name in OPTIONAL_FIELDS and name not in self.arrays:
                 continue  # stays NULL
@@ -460,6 +484,10 @@ class DrainOut:
         self.wl_ready_ns = np.full(W, KB_TS_UNSET, np.int64)
         self.wl_check_retries_out = np.zeros(W, np.int32)
         self.wl_deactivated = np.zeros(W, np.uint8)
+        self.cycle_pods_ready_timeout = np.zeros(max_cycles, np.int32)  # WaitForPodsReady (kb_snapshot.wl_pods_ready_ns)
+        self.cycle_pods_ready_deactivated = np.zeros(max_cycles, np.int32)
+        self.wl_pods_ready_at_ns = np.full(W, KB_TS_UNSET, np.int64)
+        self.wl_pods_ready_count_out = np.zeros(W, np.int32)
         cap = (min(W * 4 + Q, min(Q, W) * max_cycles) if trace_capacity is None else trace_capacity) if trace else 0
         self.trace_wl = np.zeros(max(1, cap), np.int32)
         self.trace_decision = np.zeros(max(1, cap), np.uint8)
@@ -483,6 +511,10 @@ class DrainOut:
         s.wl_ready_ns = _ptr(self.wl_ready_ns, C.c_int64)
         s.wl_check_retries_out = _ptr(self.wl_check_retries_out, C.c_int32)
         s.wl_deactivated = _ptr(self.wl_deactivated, C.c_uint8)
+        s.cycle_pods_ready_timeout = _ptr(self.cycle_pods_ready_timeout, C.c_int32)
+        s.cycle_pods_ready_deactivated = _ptr(self.cycle_pods_ready_deactivated, C.c_int32)
+        s.wl_pods_ready_at_ns = _ptr(self.wl_pods_ready_at_ns, C.c_int64)
+        s.wl_pods_ready_count_out = _ptr(self.wl_pods_ready_count_out, C.c_int32)
         if trace:
             s.trace_wl = _ptr(self.trace_wl, C.c_int32); s.trace_decision = _ptr(self.trace_decision, C.c_uint8)
         s.trace_capacity = cap
@@ -518,6 +550,10 @@ class DrainOut:
     def n_resorts(self): return int(self.struct.n_resorts)
     @property
     def resort_ms(self): return float(self.struct.resort_ms)
+    @property
+    def n_pods_ready_timeout(self): return int(self.struct.n_pods_ready_timeout)
+    @property
+    def n_pods_ready_deactivated(self): return int(self.struct.n_pods_ready_deactivated)
 
     def cycles(self):
         """[(heads, decisions)] per cycle from the trace."""

@@ -1356,7 +1356,7 @@ extern "C" int32_t kb_run_cycle(kb_handle *h, const kb_snapshot *s, kb_cycle_out
 // ---------------------------------------------------------------------------
 // what a boundary of kb_run_drain reads back, in the pinned host words [8, 24)
 struct DrainWords {
-  uint32_t counters[KB_DC_CHECK_REJECTED + 1];  // DrainDev::counters; [0] = heads of the next cycle
+  uint32_t counters[KB_DC_PR_DEACTIVATED + 1];  // DrainDev::counters; [0] = heads of the next cycle
   uint32_t n_new, n_cells;              // this cycle's admissions and their usage cells (the admit scans' totals)
   uint32_t status;                      // the cycle's status word (KBS_AFS_OVERFLOW)
   i64 t_next;                           // event mode: t_{c+1}
@@ -1370,6 +1370,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   out->n_cycles = 0; out->n_decisions = 0; out->n_admitted = 0; out->gpu_ms = 0; out->n_evicted = 0;
   out->n_finished = 0; out->n_arrived = 0; out->end_ns = s->now_ns; out->n_evict_done = 0;
   out->n_check_ready = 0; out->n_check_retry = 0; out->n_check_rejected = 0; out->n_resorts = 0; out->resort_ms = 0;
+  out->n_pods_ready_timeout = 0; out->n_pods_ready_deactivated = 0;
   // ---- eviction replay: host-side checks of adm_wl (include/kueue_b200.h)
   const bool replay = s->adm_wl != nullptr;
   if (replay) {
@@ -1385,7 +1386,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     }
   }
   // ---- event mode: host-side checks of the arrival and completion tables (include/kueue_b200.h)
-  const bool events = s->wl_create_ns || s->wl_run_ns || s->adm_finish_ns || s->wl_evict_ns || s->wl_check_ns;
+  const bool events = s->wl_create_ns || s->wl_run_ns || s->adm_finish_ns || s->wl_evict_ns || s->wl_check_ns || s->wl_pods_ready_ns;
   if (events) {
     if (s->adm_finish_ns)
       for (int a = 0; a < s->n_adm; a++)
@@ -1441,7 +1442,9 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   }
   // ---- admission checks: host-side checks (include/kueue_b200.h)
   const bool checks = s->wl_check_ns != nullptr;
-  if (checks || s->wl_check_fail || s->wl_check_retries || s->wl_check_evict_ns || s->wl_requeue_at_ns || s->adm_check_end_ns) {
+  const bool pr = s->wl_pods_ready_ns != nullptr;  // WaitForPodsReady
+  const bool requeue = checks || pr;               // BACKOFF / DEACTIVATED, RequeueAt, queue-order timestamps, re-sorts
+  if (checks || s->wl_check_fail || s->wl_check_retries || s->wl_check_evict_ns || (s->wl_requeue_at_ns && !pr) || s->adm_check_end_ns) {
     if (!checks) return fail(h, KB_ERR_INVALID, "admission checks: the tables need wl_check_ns");
     if (!replay) return fail(h, KB_ERR_INVALID, "admission checks: the tables need adm_wl");
     if (decay) return fail(h, KB_ERR_UNSUPPORTED, "admission checks with afs decay: a workload with checks never makes the Pending -> Admitted transition that updates consumed usage");
@@ -1470,6 +1473,41 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
         if (s->adm_check_end_ns[a] <= s->now_ns) return fail(h, KB_ERR_INVALID, "admission checks: adm_check_end_ns at or before now_ns");
         if (lat && s->adm_evict_end_ns && s->adm_evicted && s->adm_evicted[a])  // one end time per row
           return fail(h, KB_ERR_INVALID, "admission checks: a row with both an eviction under way (adm_evict_end_ns) and a check under way");
+      }
+  }
+  // ---- WaitForPodsReady: host-side checks (include/kueue_b200.h)
+  if (pr || s->wl_pods_ready_fail || s->wl_pods_ready_count || s->wl_pods_ready_evict_ns || s->adm_admitted_ns) {
+    if (!pr) return fail(h, KB_ERR_INVALID, "pods ready: the tables need wl_pods_ready_ns");
+    if (!replay) return fail(h, KB_ERR_INVALID, "pods ready: the tables need adm_wl");
+    if (s->pods_ready_timeout_ns <= 0) return fail(h, KB_ERR_INVALID, "pods ready: timeout <= 0");
+    if (s->pods_ready_backoff_base_s < 0 || s->pods_ready_backoff_max_s < 0 || s->pods_ready_backoff_limit < -1)
+      return fail(h, KB_ERR_INVALID, "pods ready: backoff base < 0, max < 0 or limit < -1");
+    if (s->pods_ready_requeue_creation != 0 && s->pods_ready_requeue_creation != 1)
+      return fail(h, KB_ERR_INVALID, "pods ready: pods_ready_requeue_creation is neither 0 (Eviction) nor 1 (Creation)");
+    std::vector<uint8_t> held((size_t)std::max(1, W), 0);
+    for (int a = 0; a < s->n_adm; a++) held[s->adm_wl[a]] = 1;
+    for (int w = 0; w < W; w++) {
+      if (s->wl_pods_ready_ns[w] < 0 || (s->wl_pods_ready_fail && s->wl_pods_ready_fail[w] < 0) ||
+          (s->wl_pods_ready_count && s->wl_pods_ready_count[w] < 0))
+        return fail(h, KB_ERR_INVALID, "pods ready: a negative delay, fail count or requeue count");
+      if (s->wl_pods_ready_evict_ns && s->wl_pods_ready_evict_ns[w] != INT64_MIN) {
+        if (held[w]) return fail(h, KB_ERR_INVALID, "pods ready: wl_pods_ready_evict_ns on a record that holds quota (adm_wl)");
+        if (s->wl_check_evict_ns && s->wl_check_evict_ns[w] != INT64_MIN)
+          return fail(h, KB_ERR_INVALID, "pods ready: a record with both wl_pods_ready_evict_ns and wl_check_evict_ns (one Evicted condition)");
+      }
+      if (!checks && s->wl_requeue_at_ns && s->wl_requeue_at_ns[w] != INT64_MIN) {  // as the admission checks require
+        if (held[w]) return fail(h, KB_ERR_INVALID, "pods ready: wl_requeue_at_ns on a record that holds quota (adm_wl)");
+        if (s->wl_create_ns && s->wl_create_ns[w] > s->now_ns) return fail(h, KB_ERR_INVALID, "pods ready: wl_requeue_at_ns on a record created after now_ns");
+      }
+    }
+    if (s->adm_admitted_ns)
+      for (int a = 0; a < s->n_adm; a++) {
+        if (s->adm_admitted_ns[a] == INT64_MIN) continue;
+        if (s->adm_admitted_ns[a] > s->now_ns) return fail(h, KB_ERR_INVALID, "pods ready: adm_admitted_ns after now_ns");
+        if (s->adm_check_end_ns && s->adm_check_end_ns[a] != INT64_MIN)
+          return fail(h, KB_ERR_INVALID, "pods ready: adm_admitted_ns on a row whose checks run (adm_check_end_ns)");
+        if (lat && s->adm_evict_end_ns && s->adm_evicted && s->adm_evicted[a])
+          return fail(h, KB_ERR_INVALID, "pods ready: adm_admitted_ns on a row whose eviction is under way (adm_evict_end_ns)");
       }
   }
   out->n_afs_samples = 0;
@@ -1549,7 +1587,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   u64 *keys[2], *arr_keys[2] = {nullptr, nullptr};
   int32_t *vals[2], *arr_vals[2] = {nullptr, nullptr}, *q_count, *d_wl_class = nullptr, *d_cq_class_start = nullptr;
   char *sort_tmp, *scan_tmp = nullptr;
-  i64 *run = nullptr, *create = nullptr, *evict_ns = nullptr, *check_ns = nullptr;
+  i64 *run = nullptr, *create = nullptr, *evict_ns = nullptr, *check_ns = nullptr, *pr_ns = nullptr;
   DrainDev X{};
   AdmTabs other{};  // compaction: the other half of the admitted tables' double buffer
   auto layout = [&](Arena &a) {
@@ -1562,7 +1600,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     X.flag = a.take<int32_t>((size_t)Q + 2); X.pos = a.take<int32_t>((size_t)Q + 2);
     X.e_assumed = a.take<int32_t>(Hz + 2); X.e_ncells = a.take<int32_t>(Hz + 2);
     X.e_adm_off = a.take<int32_t>(Hz + 2); X.e_cell_off = a.take<int32_t>(Hz + 2);
-    X.counters = a.take<int32_t>(16);
+    X.counters = a.take<int32_t>(KB_DC_PR_DEACTIVATED + 1);
     X.wl_admit_cycle = a.take<int32_t>(Wz); X.wl_evals = a.take<int32_t>(Wz); X.wl_last_decision = a.take<uint8_t>(Wz);
     if (trace_cap) { X.trace_wl = a.take<int32_t>(trace_cap); X.trace_dec = a.take<uint8_t>(trace_cap); }
     if (replay || events) {
@@ -1597,11 +1635,17 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       evict_ns = a.take<i64>(Wz);
       X.adm_evicting = a.take<uint8_t>(Acap); other.evicting = a.take<uint8_t>(Acap);
     }
-    if (checks) {  // delays, attempt state, timestamps and the checking byte of both halves
+    if (checks) {  // check delays and attempt state
       check_ns = a.take<i64>(Wz); X.wl_fail = a.take<int32_t>(Wz); X.wl_retries = a.take<int32_t>(Wz);
+    }
+    if (pr) {  // PodsReady delays and attempt state
+      pr_ns = a.take<i64>(Wz); X.wl_pr_fail = a.take<int32_t>(Wz); X.wl_pr_count = a.take<int32_t>(Wz);
+      X.wl_pr_at = a.take<i64>(Wz); X.wl_pr_prev = a.take<i64>(Wz);
+    }
+    if (requeue) {  // timestamps, requeue state and the phase byte of both halves
       X.wl_ts0 = a.take<i64>(Wz); X.wl_sort_ts = a.take<i64>(Wz); X.wl_requeue_at = a.take<i64>(Wz);
       X.wl_ready_ns = a.take<i64>(Wz); X.wl_deactivated = a.take<uint8_t>(Wz);
-      X.adm_checking = a.take<uint8_t>(Acap); other.checking = a.take<uint8_t>(Acap);
+      X.adm_phase = a.take<uint8_t>(Acap); other.phase = a.take<uint8_t>(Acap);
     }
     if (afs) {
       X.seg_start = a.take<int32_t>(seg_start.size()); X.lq_seg = a.take<int32_t>(lq_seg.size());
@@ -1649,18 +1693,27 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       never.swap(fin);
       finish = never.data();
     }
-    if (checks && s->adm_check_end_ns) {  // rows whose checks run: the verdict time in the finish column
+    if ((checks && s->adm_check_end_ns) || (pr && s->adm_admitted_ns)) {  // rows whose checks run: the verdict time in the
+      // finish column; rows whose pods are not ready: their attempt from Admitted (drain_pr_attempt; no failure is used
+      // until a timeout is applied), T in the finish column of a failing one
       std::vector<i64> fin((size_t)s->n_adm);
-      std::vector<uint8_t> chk((size_t)s->n_adm, 0);
+      std::vector<uint8_t> ph((size_t)s->n_adm, KB_PH_RUN);
       memcpy(fin.data(), finish, (size_t)s->n_adm * 8);
-      for (int a = 0; a < s->n_adm; a++)
-        if (s->adm_check_end_ns[a] != INT64_MIN) { fin[a] = s->adm_check_end_ns[a]; chk[a] = 1; }
+      for (int a = 0; a < s->n_adm; a++) {
+        if (checks && s->adm_check_end_ns && s->adm_check_end_ns[a] != INT64_MIN) { fin[a] = s->adm_check_end_ns[a]; ph[a] = KB_PH_CHECK; }
+        if (!pr || !s->adm_admitted_ns || s->adm_admitted_ns[a] == INT64_MIN) continue;
+        const int w = s->adm_wl[a];
+        const i64 t0 = s->adm_admitted_ns[a], d = s->wl_pods_ready_ns[w], to = s->pods_ready_timeout_ns;
+        const i64 run = s->wl_run_ns ? s->wl_run_ns[w] : -1;
+        if ((s->wl_pods_ready_fail && s->wl_pods_ready_fail[w] > 0) || d > to) { fin[a] = t0 > INT64_MAX - to ? INT64_MAX : t0 + to; ph[a] = KB_PH_WAIT; }
+        else { const i64 at = t0 > INT64_MAX - d ? INT64_MAX : t0 + d; fin[a] = run < 0 ? INT64_MAX : (at > INT64_MAX - run ? INT64_MAX : at + run); }
+      }
       never.swap(fin);
       finish = never.data();
-      CUDA_TRY(h, h2d(h, X.adm_checking, chk.data(), chk.size()));
-      CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // chk is a local
-    } else if (checks) {
-      CUDA_TRY(h, cudaMemsetAsync(X.adm_checking, 0, (size_t)s->n_adm, h->stream));
+      CUDA_TRY(h, h2d(h, X.adm_phase, ph.data(), ph.size()));
+      CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // ph is a local
+    } else if (requeue) {
+      CUDA_TRY(h, cudaMemsetAsync(X.adm_phase, KB_PH_RUN, (size_t)s->n_adm, h->stream));
     }
     CUDA_TRY(h, h2d(h, X.adm_finish, finish, (size_t)s->n_adm * 8));
     if (s->wl_run_ns) { CUDA_TRY(h, h2d(h, run, s->wl_run_ns, Wz * 8)); X.wl_run = run; }
@@ -1697,28 +1750,52 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     X.n_afs_cq = (int)afs_cqs.size();
   }
   if (sticky) CUDA_TRY(h, h2d(h, X.cq_sticky, s->cq_sticky, (size_t)Q * 4));
-  std::vector<i64> qts, requeue_at;  // admission checks: queue-order timestamps and RequeueAt at the start
-  std::vector<int32_t> fails, retries;
-  if (checks) {
+  std::vector<i64> qts, requeue_at, pr_at, pr_none;  // checks / PodsReady: queue-order timestamps, RequeueAt, PodsReady at the start
+  std::vector<int32_t> fails, retries, pr_fails, pr_counts;
+  if (requeue) {
     std::vector<uint8_t> held(Wz, 0);
     for (int a = 0; a < s->n_adm; a++) held[s->adm_wl[a]] = 1;
     qts.assign(s->wl_ts, s->wl_ts + W);
     if (s->wl_check_evict_ns)
       for (int w = 0; w < W; w++) if (s->wl_check_evict_ns[w] != INT64_MIN && !held[w]) qts[w] = s->wl_check_evict_ns[w];
+    if (pr && s->wl_pods_ready_evict_ns && !s->pods_ready_requeue_creation)  // the Eviction timestamp of a timed-out record
+      for (int w = 0; w < W; w++) if (s->wl_pods_ready_evict_ns[w] != INT64_MIN) qts[w] = s->wl_pods_ready_evict_ns[w];
     requeue_at.assign(Wz, INT64_MIN);
     if (s->wl_requeue_at_ns) requeue_at.assign(s->wl_requeue_at_ns, s->wl_requeue_at_ns + W);
-    fails.assign(Wz, 0); retries.assign(Wz, 0);
-    if (s->wl_check_fail) fails.assign(s->wl_check_fail, s->wl_check_fail + W);
-    if (s->wl_check_retries) retries.assign(s->wl_check_retries, s->wl_check_retries + W);
-    X.wl_check = check_ns; X.wl_qts = const_cast<i64 *>(D.wl_ts);
-    CUDA_TRY(h, h2d(h, check_ns, s->wl_check_ns, Wz * 8));
+    X.wl_qts = const_cast<i64 *>(D.wl_ts);
     CUDA_TRY(h, h2d(h, X.wl_ts0, s->wl_ts, Wz * 8));
     CUDA_TRY(h, h2d(h, X.wl_qts, qts.data(), Wz * 8));       // the cycle kernels read the queue-order timestamp
     CUDA_TRY(h, h2d(h, X.wl_sort_ts, qts.data(), Wz * 8));
     CUDA_TRY(h, h2d(h, X.wl_requeue_at, requeue_at.data(), Wz * 8));
+  }
+  if (checks) {
+    fails.assign(Wz, 0); retries.assign(Wz, 0);
+    if (s->wl_check_fail) fails.assign(s->wl_check_fail, s->wl_check_fail + W);
+    if (s->wl_check_retries) retries.assign(s->wl_check_retries, s->wl_check_retries + W);
+    X.wl_check = check_ns;
+    CUDA_TRY(h, h2d(h, check_ns, s->wl_check_ns, Wz * 8));
     CUDA_TRY(h, h2d(h, X.wl_fail, fails.data(), Wz * 4));
     CUDA_TRY(h, h2d(h, X.wl_retries, retries.data(), Wz * 4));
     X.check_base_s = s->check_backoff_base_s; X.check_max_s = s->check_backoff_max_s; X.check_limit = s->check_backoff_limit;
+  }
+  if (pr) {
+    pr_fails.assign(Wz, 0); pr_counts.assign(Wz, 0); pr_at.assign(Wz, INT64_MIN); pr_none.assign(Wz, INT64_MIN);
+    if (s->wl_pods_ready_fail) pr_fails.assign(s->wl_pods_ready_fail, s->wl_pods_ready_fail + W);
+    if (s->wl_pods_ready_count) pr_counts.assign(s->wl_pods_ready_count, s->wl_pods_ready_count + W);
+    if (s->adm_admitted_ns)  // a ready attempt under way reaches PodsReady at Admitted + delay
+      for (int a = 0; a < s->n_adm; a++) {
+        const int w = s->adm_wl[a];
+        const i64 t0 = s->adm_admitted_ns[a], d = s->wl_pods_ready_ns[w];
+        if (t0 != INT64_MIN && pr_fails[w] == 0 && d <= s->pods_ready_timeout_ns) pr_at[w] = t0 > INT64_MAX - d ? INT64_MAX : t0 + d;
+      }
+    X.wl_pr = pr_ns;
+    CUDA_TRY(h, h2d(h, pr_ns, s->wl_pods_ready_ns, Wz * 8));
+    CUDA_TRY(h, h2d(h, X.wl_pr_fail, pr_fails.data(), Wz * 4));
+    CUDA_TRY(h, h2d(h, X.wl_pr_count, pr_counts.data(), Wz * 4));
+    CUDA_TRY(h, h2d(h, X.wl_pr_at, pr_at.data(), Wz * 8));
+    CUDA_TRY(h, h2d(h, X.wl_pr_prev, pr_none.data(), Wz * 8));  // no PodsReady before the attempts under way
+    X.pr_timeout = s->pods_ready_timeout_ns; X.pr_base_s = s->pods_ready_backoff_base_s; X.pr_max_s = s->pods_ready_backoff_max_s;
+    X.pr_limit = s->pods_ready_backoff_limit; X.pr_creation = s->pods_ready_requeue_creation;
   }
   std::vector<i64> lq_adm;  // decay: the initial admitted usage of every LocalQueue (live rows of the snapshot)
   if (decay) {
@@ -1761,7 +1838,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   k_drain_init<<<std::max(nbW, (S + tb - 1) / tb), tb, 0, h->stream>>>(D, X, S);
   if (events) k_drain_init_events<<<std::max(1, nbW), tb, 0, h->stream>>>(D, X, create, s->now_ns);
   if (replay || events || sticky) k_drain_init_replay<<<std::max(nbW, (s->n_adm + tb - 1) / tb), tb, 0, h->stream>>>(D, X, replay ? s->n_adm : 0);
-  if (checks) {  // records in backoff, and the first RequeueAt into clock[2] (k_drain_init_events set clock[0] = now_ns)
+  if (requeue) {  // records in backoff, and the first RequeueAt into clock[2] (k_drain_init_events set clock[0] = now_ns)
     k_drain_init_checks<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W, s->now_ns);
     k_drain_backoff<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W);
   }
@@ -1793,17 +1870,18 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   i64 t = s->now_ns;  // the clock: the plain drain steps it by one per cycle
   const i64 step = s->drain_cycle_ns > 0 ? s->drain_cycle_ns : 1;
   const int nbArr = std::max(1, std::min(nbW, 8 * std::max(1, h->sm_count)));
-  struct EventPair {  // around a re-sort (admission checks); destroyed on every return
+  struct EventPair {  // around a re-sort (admission checks, PodsReady); destroyed on every return
     cudaEvent_t e[2] = {nullptr, nullptr};
     ~EventPair() { for (cudaEvent_t x : e) if (x) cudaEventDestroy(x); }
   } resort_ev;
   cudaEvent_t *ev_r = resort_ev.e;
   bool resort_timed = false;
   uint32_t verdicts_seen[3] = {0, 0, 0};  // cumulative Ready / Retry / Rejected counters at the previous boundary
-  if (checks) {
+  uint32_t timeouts_seen[2] = {0, 0};     // cumulative PodsReady timeout / deactivation counters, likewise
+  if (requeue) {
     CUDA_TRY(h, cudaEventCreate(&ev_r[0]));
     CUDA_TRY(h, cudaEventCreate(&ev_r[1]));
-    CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_RESORT, 0, 4 * 4, h->stream));  // once: the boundaries never clear them
+    CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_RESORT, 0, (pr ? 6 : 4) * 4, h->stream));  // once: the boundaries never clear them
   }
   // ---- one boundary per iteration, one synchronisation each (kueue_b200/drain.py): cycle c at t (in event mode, a
   // jump to the next event when there are no heads), its decisions and admissions, the evictions; in event mode E,
@@ -1849,7 +1927,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       if (decay) k_drain_afs_decay<<<nbL, tb, 0, h->stream>>>(D, X, L);  // samples due in (t, t_{c+1}], before the completions
       k_drain_finish<<<nbB, tb, 0, h->stream>>>(D, X, bound, n_new_d);
       if (X.arr_key) k_drain_arrive<<<nbArr, tb, 0, h->stream>>>(X);
-      if (checks) k_drain_backoff<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W);
+      if (requeue) k_drain_backoff<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W);
     }
     if (compact) {
       k_drain_requeue<<<nbQ, tb, 0, h->stream>>>(D, X);
@@ -1868,7 +1946,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (!jump) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_new, n_new_d, 4, cudaMemcpyDeviceToHost, h->stream));
     if (!compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_cells, X.e_cell_off + n_live, 4, cudaMemcpyDeviceToHost, h->stream));
     if (afs && (!jump || decay)) CUDA_TRY(h, cudaMemcpyAsync(&hw.status, D.status, 4, cudaMemcpyDeviceToHost, h->stream));
-    if (compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[1], X.counters + 1, (checks ? KB_DC_CHECK_REJECTED : events ? KB_DC_ARR_HI : KB_DC_FULL) * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[1], X.counters + 1, (pr ? KB_DC_PR_DEACTIVATED : checks ? KB_DC_CHECK_REJECTED : events ? KB_DC_ARR_HI : KB_DC_FULL) * 4, cudaMemcpyDeviceToHost, h->stream));
     if (events) CUDA_TRY(h, cudaMemcpyAsync(&hw.t_next, X.clock, 8, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     if (!jump) {
@@ -1891,6 +1969,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       if (lat && out->cycle_evict_done) out->cycle_evict_done[cyc] = 0;
       if (checks && out->cycle_check_retry) out->cycle_check_retry[cyc] = 0;
       if (checks && out->cycle_check_rejected) out->cycle_check_rejected[cyc] = 0;
+      if (pr && out->cycle_pods_ready_timeout) out->cycle_pods_ready_timeout[cyc] = 0;
+      if (pr && out->cycle_pods_ready_deactivated) out->cycle_pods_ready_deactivated[cyc] = 0;
       out->n_decisions += n_live; out->n_admitted += n_new; out->n_evicted += n_ev;
       out->n_cycles = ++cyc;
     } else {
@@ -1914,6 +1994,16 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
         if (out->cycle_check_rejected) out->cycle_check_rejected[cyc - 1] += rej;
       }
     }
+    if (pr) {  // PodsReady timeouts of this boundary
+      const uint32_t *cum = &hw.counters[KB_DC_PR_TIMEOUT];
+      const int to = (int)(cum[0] - timeouts_seen[0]), de = (int)(cum[1] - timeouts_seen[1]);
+      memcpy(timeouts_seen, cum, sizeof(timeouts_seen));
+      out->n_pods_ready_timeout += to; out->n_pods_ready_deactivated += de;
+      if (cyc > 0) {
+        if (out->cycle_pods_ready_timeout) out->cycle_pods_ready_timeout[cyc - 1] += to;
+        if (out->cycle_pods_ready_deactivated) out->cycle_pods_ready_deactivated[cyc - 1] += de;
+      }
+    }
     if (lat) {  // evictions completed at this boundary (counter slot 4, inside the events copy)
       const int done = (int)hw.counters[KB_DC_EVICT_DONE];
       out->n_evict_done += done;
@@ -1922,10 +2012,10 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (compact) {  // the compacted half becomes the admitted tables of the next boundary
       A_cur = (int)hw.counters[KB_DC_ROWS]; AU_cur = (int)hw.counters[KB_DC_CELLS];
       AdmTabs cur{X.adm_cq, X.adm_priority, X.adm_ts, X.adm_qr_ts, X.adm_uid, X.adm_evicted, X.adm_use_start, X.adm_use_fr, X.adm_use_qty, X.adm_wl, X.adm_finish, X.adm_lq,
-                  X.adm_evicting, X.adm_checking};
+                  X.adm_evicting, X.adm_phase};
       X.adm_cq = other.cq; X.adm_priority = other.priority; X.adm_ts = other.ts; X.adm_qr_ts = other.qr_ts; X.adm_uid = other.uid;
       X.adm_evicted = other.evicted; X.adm_use_start = other.use_start; X.adm_use_fr = other.use_fr; X.adm_use_qty = other.use_qty; X.adm_wl = other.wl;
-      X.adm_finish = other.finish; X.adm_lq = other.lq; X.adm_evicting = other.evicting; X.adm_checking = other.checking;
+      X.adm_finish = other.finish; X.adm_lq = other.lq; X.adm_evicting = other.evicting; X.adm_phase = other.phase;
       D.adm_cq = X.adm_cq; D.adm_priority = X.adm_priority; D.adm_ts = X.adm_ts; D.adm_qr_ts = X.adm_qr_ts; D.adm_uid = X.adm_uid;
       D.adm_evicted = X.adm_evicted; D.adm_use_start = X.adm_use_start; D.adm_use_fr = X.adm_use_fr; D.adm_use_qty = X.adm_use_qty;
       other = cur;
@@ -1934,7 +2024,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     }
     n_live = (int)hw.counters[0];
     if (events ? hw.counters[KB_DC_END] != 0 : n_new == 0 && n_ev == 0) break;
-    if (checks && (int32_t)hw.counters[KB_DC_RESORT] == X.cycle + 1) {  // re-sort: the three passes over the queue-order timestamps, positions,
+    if (requeue && (int32_t)hw.counters[KB_DC_RESORT] == X.cycle + 1) {  // re-sort: the three passes over the queue-order timestamps, positions,
       // cursors from 0, first_aside from the SET_ASIDE positions, then the heads again.  The segments and their
       // lengths do not change, so n_live holds and no synchronisation is added; the events are read at the next one.
       if (resort_timed) { float ms = 0; cudaEventElapsedTime(&ms, ev_r[0], ev_r[1]); out->resort_ms += ms; gpu_ms += ms; }
@@ -1981,7 +2071,11 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   if (checks) {
     if (out->wl_ready_ns) CUDA_TRY(h, cudaMemcpyAsync(out->wl_ready_ns, X.wl_ready_ns, Wz * 8, cudaMemcpyDeviceToHost, h->stream));
     if (out->wl_check_retries_out) CUDA_TRY(h, cudaMemcpyAsync(out->wl_check_retries_out, X.wl_retries, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
-    if (out->wl_deactivated) CUDA_TRY(h, cudaMemcpyAsync(out->wl_deactivated, X.wl_deactivated, Wz, cudaMemcpyDeviceToHost, h->stream));
+  }
+  if (requeue && out->wl_deactivated) CUDA_TRY(h, cudaMemcpyAsync(out->wl_deactivated, X.wl_deactivated, Wz, cudaMemcpyDeviceToHost, h->stream));
+  if (pr) {
+    if (out->wl_pods_ready_at_ns) CUDA_TRY(h, cudaMemcpyAsync(out->wl_pods_ready_at_ns, X.wl_pr_at, Wz * 8, cudaMemcpyDeviceToHost, h->stream));
+    if (out->wl_pods_ready_count_out) CUDA_TRY(h, cudaMemcpyAsync(out->wl_pods_ready_count_out, X.wl_pr_count, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
   }
   if (out->ps_flavor && PR) CUDA_TRY(h, cudaMemcpyAsync(out->ps_flavor, D.ps_flavor, PR, cudaMemcpyDeviceToHost, h->stream));
   if (out->ps_count && D.P) CUDA_TRY(h, cudaMemcpyAsync(out->ps_count, D.ps_count_out, (size_t)D.P * 4, cudaMemcpyDeviceToHost, h->stream));

@@ -51,14 +51,21 @@
 // cycle: one writer per slot.  Never set on an AFS ClusterQueue (refused, and no preemption there), so k_drain_afs_heads
 // does not read it.
 //
-// Admission checks (kb_snapshot.wl_check_ns; include/kueue_b200.h): the byte column adm_checking (both halves, carried by
-// the compaction) marks a row whose checks run; its verdict time lives in the finish column, so k_drain_ev_min sees it
-// unchanged.  k_drain_admit starts the attempt, k_drain_evict drops it (a preempted row without pods is released at the
+// Admission checks (kb_snapshot.wl_check_ns; include/kueue_b200.h): the row-phase byte column adm_phase (both halves,
+// carried by the compaction) marks a row whose checks run (KB_PH_CHECK); its verdict time lives in the finish column, so
+// k_drain_ev_min sees it unchanged.  k_drain_admit starts the attempt, k_drain_evict drops it (a preempted row without pods is released at the
 // next boundary), k_drain_finish applies the verdicts before the completions.  The DevSnap's wl_ts is the mutable
 // queue-order timestamp the cycle kernels read (wl_ts0 keeps the creation timestamps).  k_drain_backoff (one pass over
 // the records per boundary) requeues the BACKOFF records whose RequeueAt has come and reduces the next RequeueAt into
 // clock[2], which k_drain_ev_next folds into E.  A record that enters its queue with a timestamp other than the key the
 // order was built with (wl_sort_ts) stamps KB_DC_RESORT with the boundary; the host then rebuilds the order (kb_api.cu).
+//
+// WaitForPodsReady (kb_snapshot.wl_pods_ready_ns) runs on the same machinery.  drain_pr_attempt starts an attempt at
+// Admitted (k_drain_admit, or a Ready verdict in k_drain_finish): a ready one only moves the finish column, a failing one
+// is KB_PH_WAIT with its timeout T in the finish column.  k_drain_finish applies the timeout after the verdicts: Count,
+// RequeueAt and the queue timestamp on the record, and the row is KB_PH_TIMED_OUT, released at once or, with latency, at
+// T + latency as an evicting row; its release sends the record to BACKOFF (k_drain_backoff queues it) or DEACTIVATED.
+// k_drain_evict drops a waiting attempt.
 #pragma once
 
 #include <cub/device/device_scan.cuh>
@@ -69,6 +76,7 @@
 // grows by `factor` in float64 and is capped at cap, after which Step returns cap), stopping at the cap.  cap 0 =
 // MaxInt64 / ceil(factor).  Restated by kueue_b200/drain.py wait_time.
 __host__ __device__ inline i64 kb_backoff_wait(i64 base, i64 cap, double factor, int iteration) {
+  if (base == 0) return 0;  // every Step returns 0: no loop over a large iteration count
   if (cap == 0) cap = (i64)(9223372036854775807.0 / ceil(factor));
   i64 dur = base, out = 0;
   bool capped = false;
@@ -88,6 +96,11 @@ __host__ __device__ inline i64 kb_backoff_wait(i64 base, i64 cap, double factor,
 // first Step returns the base uncapped.  Restated by kueue_b200/drain.py check_wait_s.
 __host__ __device__ inline i64 kb_check_wait_ns(int k, i64 base_s, i64 max_s) {
   return kb_backoff_wait(base_s * 1000000000ll, max_s * 1000000000ll, 2.0, k) / 1000000000ll * 1000000000ll;
+}
+// WaitTime of PodsReady requeue k (UpdateRequeueState workload.go:707-722): wait.NewBackoff(base, max, 2, 0.0001)
+// without jitter, in nanoseconds (RequeueAt = T + it).  Restated by kueue_b200/drain.py pods_ready_wait_ns.
+__host__ __device__ inline i64 kb_pods_ready_wait_ns(int k, i64 base_s, i64 max_s) {
+  return kb_backoff_wait(base_s * 1000000000ll, max_s * 1000000000ll, 2.0, k);
 }
 
 // ---- resource.Quantity in the int64Amount form (value * 10^scale), as AdmissionFairSharing sums it -----------------
@@ -269,16 +282,26 @@ struct DrainDev {
   i64 *wl_sort_ts;                 // [W] the keys the current order was built with
   i64 *wl_requeue_at;              // [W] RequeueAt of a BACKOFF record
   i64 *wl_ready_ns; uint8_t *wl_deactivated;  // [W]
-  uint8_t *adm_checking;           // [A_cap] 1 while the row's checks run (current half); its verdict time is adm_finish
+  uint8_t *adm_phase;              // [A_cap] KB_PH_* of each row (current half); also with WaitForPodsReady
   i64 check_base_s, check_max_s; int check_limit;
+  // WaitForPodsReady (event mode; the requeue state above is allocated with it); wl_pr == nullptr: off
+  const i64 *wl_pr;                // [W] Admitted -> PodsReady delay of a ready attempt
+  int32_t *wl_pr_fail, *wl_pr_count;  // [W] failures left (INT32_MAX = all) / RequeueState.Count
+  i64 *wl_pr_at, *wl_pr_prev;      // [W] PodsReady time of the last attempt that reaches it / the value before it
+  i64 pr_timeout, pr_base_s, pr_max_s; int pr_limit, pr_creation;
 };
+// adm_phase: what the finish column of a row holds.  RUN: its finish (or its eviction's end when adm_evicting); CHECK: its
+// checks' verdict; WAIT: the timeout T of a PodsReady attempt that fails; TIMED_OUT: the end of its eviction by that timeout
+enum { KB_PH_RUN = 0, KB_PH_CHECK = 1, KB_PH_WAIT = 2, KB_PH_TIMED_OUT = 3 };
 // counters of a boundary: [1] evictions (issued, with latency), [2] / [3] rows / cells after the compaction, [4]
 // evictions completed (latency), [5] capacity flag; event mode: [6] completions, [7] arrivals, [8] end flag, [9] / [10]
 // arrived prefix of arr_order [lo, hi); admission checks: [11] the stamp (cycle + 1) of the last boundary that needs a
-// re-sort, [12] / [13] / [14] Ready / Retry / Rejected verdicts since the start (the host takes differences: no memset)
+// re-sort, [12] / [13] / [14] Ready / Retry / Rejected verdicts since the start (the host takes differences: no memset);
+// WaitForPodsReady: [15] / [16] timeouts that requeue / deactivate since the start, likewise
 enum { KB_DC_EVICTED = 1, KB_DC_ROWS = 2, KB_DC_CELLS = 3, KB_DC_EVICT_DONE = 4, KB_DC_FULL = 5,
        KB_DC_FINISHED = 6, KB_DC_ARRIVED = 7, KB_DC_END = 8, KB_DC_ARR_LO = 9, KB_DC_ARR_HI = 10,
-       KB_DC_RESORT = 11, KB_DC_CHECK_READY = 12, KB_DC_CHECK_RETRY = 13, KB_DC_CHECK_REJECTED = 14 };
+       KB_DC_RESORT = 11, KB_DC_CHECK_READY = 12, KB_DC_CHECK_RETRY = 13, KB_DC_CHECK_REJECTED = 14,
+       KB_DC_PR_TIMEOUT = 15, KB_DC_PR_DEACTIVATED = 16 };
 
 __device__ __forceinline__ int drain_seg0(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq] : cq; }
 __device__ __forceinline__ int drain_seg1(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq + 1] : cq + 1; }
@@ -471,6 +494,19 @@ __global__ void k_drain_apply(DevSnap D, DrainDev X) {
   }
 }
 
+__device__ __forceinline__ i64 drain_sat_add(i64 t, i64 d) { return t > INT64_MAX - d ? INT64_MAX : t + d; }  // d >= 0
+// WaitForPodsReady: the attempt of row a (record w) Admitted at t.  A failing one (failures left, or a delay past the
+// timeout) waits for its timeout T = t + timeout in the finish column; a ready one reaches PodsReady at t + delay, and
+// its finish is PodsReady + run (run < 0 never finishes).  Returns the finish column's value.
+__device__ __forceinline__ i64 drain_pr_attempt(const DrainDev &X, int a, int w, i64 t) {
+  const i64 d = X.wl_pr[w];
+  if (X.wl_pr_fail[w] > 0 || d > X.pr_timeout) { X.adm_phase[a] = KB_PH_WAIT; return drain_sat_add(t, X.pr_timeout); }
+  const i64 at = drain_sat_add(t, d), run = X.wl_run ? X.wl_run[w] : -1;
+  X.adm_phase[a] = KB_PH_RUN;
+  X.wl_pr_prev[w] = X.wl_pr_at[w]; X.wl_pr_at[w] = at;
+  return run < 0 ? INT64_MAX : drain_sat_add(at, run);
+}
+
 // admitted entries join the admitted tables (cache.AssumeWorkload), appended at X.A / X.AU, and the ClusterQueue usage
 __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
   int e = blockIdx.x * blockDim.x + threadIdx.x;
@@ -489,12 +525,15 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
   if (X.adm_finish) {  // finish = QuotaReserved time + run time, saturating; run < 0 never finishes
     const i64 run = X.wl_run ? X.wl_run[wl] : -1;
     i64 fin = run < 0 ? INT64_MAX : (qr_ts > INT64_MAX - run ? INT64_MAX : qr_ts + run);
-    if (X.wl_check) {  // the reservation resets Evicted; a check delay starts an attempt, 0 is Ready at once
+    if (X.wl_qts) {  // checks or PodsReady: the reservation resets Evicted; a check delay starts an attempt, 0 is Ready at once
       X.wl_qts[wl] = X.wl_ts0[wl];
-      const i64 chk = X.wl_check[wl];
-      X.adm_checking[a] = chk > 0;
+      const i64 chk = X.wl_check ? X.wl_check[wl] : 0;
+      X.adm_phase[a] = chk > 0 ? KB_PH_CHECK : KB_PH_RUN;
       if (chk > 0) fin = qr_ts > INT64_MAX - chk ? INT64_MAX : qr_ts + chk;
-      else X.wl_ready_ns[wl] = qr_ts;
+      else {
+        X.wl_ready_ns[wl] = qr_ts;
+        if (X.wl_pr) fin = drain_pr_attempt(X, a, wl, qr_ts);  // Admitted now: the PodsReady attempt starts
+      }
     }
     X.adm_finish[a] = fin;
     X.wl_admit_ns[wl] = qr_ts;
@@ -554,12 +593,16 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
 
 // ---- eviction replay ---------------------------------------------------------------------------------------------
 // the record of an evicted row returns to its queue with LastAssignment nil (the eviction completed)
-__device__ __forceinline__ void drain_release(const DevSnap &D, const DrainDev &X, int w) {
-  X.wl_state[w] = KB_WS_QUEUED;
+// (a released record: LastAssignment nil, no reservation)
+__device__ __forceinline__ void drain_forget(const DevSnap &D, const DrainDev &X, int w) {
   X.wl_last_gen[w] = -1;
   for (int i = D.wl_ps_start[w] * D.R; i < D.wl_ps_start[w + 1] * D.R; i++) X.ps_last_tried[i] = -1;
   if (X.wl_has_qr) X.wl_has_qr[w] = 0;
   X.wl_admit_cycle[w] = -1;
+}
+__device__ __forceinline__ void drain_release(const DevSnap &D, const DrainDev &X, int w) {
+  X.wl_state[w] = KB_WS_QUEUED;
+  drain_forget(D, X, w);
   atomicMin(&X.cursor[X.wl_seg[w]], X.wl_pos[w]);
   if (X.wl_sort_ts && X.wl_sort_ts[w] != X.wl_qts[w]) X.counters[KB_DC_RESORT] = X.cycle + 1;
 }
@@ -586,7 +629,11 @@ __global__ void k_drain_evict(DevSnap D, DrainDev X) {
       const i64 lat = X.wl_evict[w];
       X.adm_evicted[a] = 1;
       X.adm_finish[a] = D.now_ns > INT64_MAX - lat ? INT64_MAX : D.now_ns + lat;
-      if (X.adm_checking && X.adm_checking[a]) { X.adm_checking[a] = 0; X.adm_finish[a] = D.now_ns; }  // no pods: the next boundary
+      if (X.adm_phase) {  // checks running: no pods, the next boundary; a PodsReady attempt waiting for T is dropped
+        if (X.adm_phase[a] == KB_PH_CHECK) X.adm_finish[a] = D.now_ns;
+        X.adm_phase[a] = KB_PH_RUN;
+      }
+      if (X.wl_pr && X.wl_pr_at[w] > D.now_ns) X.wl_pr_at[w] = X.wl_pr_prev[w];  // dropped before PodsReady
       X.wl_evictions[w]++;
       atomicAdd(&X.counters[KB_DC_EVICTED], 1);
       continue;
@@ -597,6 +644,7 @@ __global__ void k_drain_evict(DevSnap D, DrainDev X) {
       atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
     const int w = X.adm_wl[a];
     drain_release(D, X, w);
+    if (X.wl_pr && X.wl_pr_at[w] > D.now_ns) X.wl_pr_at[w] = X.wl_pr_prev[w];  // dropped before PodsReady
     X.wl_evictions[w]++;  // a workload holds at most one row: one writer
     X.root_mark[D.root_slot[cq]] = stamp;
     atomicAdd(&X.counters[KB_DC_EVICTED], 1);
@@ -624,7 +672,7 @@ __global__ void k_drain_live(DrainDev X, int bound, const int32_t *n_new) {
   X.row_live[a] = live;
   X.row_cells[a] = live ? X.adm_use_start[a + 1] - X.adm_use_start[a] : 0;
 }
-struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; i64 *finish; int32_t *lq; uint8_t *evicting, *checking; };
+struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; i64 *finish; int32_t *lq; uint8_t *evicting, *phase; };
 // live rows of [0, bound), in order, into the other half of the double buffer; thread bound writes the totals
 __global__ void k_drain_compact(DrainDev X, AdmTabs O, int bound) {
   int a = blockIdx.x * blockDim.x + threadIdx.x;
@@ -637,7 +685,7 @@ __global__ void k_drain_compact(DrainDev X, AdmTabs O, int bound) {
   if (X.adm_finish) O.finish[n] = X.adm_finish[a];
   if (X.adm_lq) O.lq[n] = X.adm_lq[a];
   if (X.adm_evicting) O.evicting[n] = X.adm_evicting[a];
-  if (X.adm_checking) O.checking[n] = X.adm_checking[a];
+  if (X.adm_phase) O.phase[n] = X.adm_phase[a];
   for (int c = 0; c < nc; c++) { O.use_fr[c0 + c] = X.adm_use_fr[u0 + c]; O.use_qty[c0 + c] = X.adm_use_qty[u0 + c]; }
 }
 
@@ -703,34 +751,34 @@ __global__ void k_drain_ev_next(DrainDev X, i64 t_c, i64 step, int jump, const i
 // completions (thread per row): a live row with finish <= t_{c+1} gets the dead stamp, its cells leave its ClusterQueue's
 // usage (cache.DeleteWorkload, integer atomics), its record becomes FINISHED and its root tree is marked.  An evicting
 // row's finish column holds its end time: it completes the eviction instead, its record returns to its queue.  Rows in
-// [A + *n_new, bound) only pad the compaction's range.
+// [A + *n_new, bound) only pad the compaction's range.  Verdicts (admission checks) and PodsReady timeouts come first; a
+// timed-out row releases its record to BACKOFF or DEACTIVATED, and counts as neither a completion nor an eviction.
 __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *n_new) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x;
   if (a >= bound || a >= X.A + (n_new ? *n_new : 0) || X.counters[KB_DC_FULL]) return;
   const int stamp = X.cycle + 1;
   if (X.counters[KB_DC_END] || X.adm_dead[a] == stamp || X.adm_finish[a] > X.clock[0]) return;
   const int cq = X.adm_cq[a];
-  if (X.adm_checking && X.adm_checking[a]) {  // a verdict (ProvisioningRequest controller.go:536-580)
+  int ph = X.adm_phase ? X.adm_phase[a] : KB_PH_RUN;
+  if (ph == KB_PH_CHECK) {  // a verdict (ProvisioningRequest controller.go:536-580)
     const int w = X.adm_wl[a];
     const i64 tv = X.adm_finish[a];
-    X.adm_checking[a] = 0;
-    if (X.wl_fail[w] == 0) {  // Ready: Admitted, the run clock starts; the row may finish in this boundary
+    X.adm_phase[a] = KB_PH_RUN;
+    if (X.wl_fail[w] == 0) {  // Ready: Admitted, the run clock (or the PodsReady attempt) starts; it may end in this boundary
       const i64 run = X.wl_run ? X.wl_run[w] : -1;
-      const i64 fin = run < 0 ? INT64_MAX : (tv > INT64_MAX - run ? INT64_MAX : tv + run);
+      const i64 fin = X.wl_pr ? drain_pr_attempt(X, a, w, tv) : run < 0 ? INT64_MAX : (tv > INT64_MAX - run ? INT64_MAX : tv + run);
       X.wl_ready_ns[w] = tv;
       X.adm_finish[a] = fin;
       atomicAdd(&X.counters[KB_DC_CHECK_READY], 1);
       if (fin > X.clock[0]) return;
+      ph = X.adm_phase[a];
     } else {  // Retry or Rejected: the workload holds no pods, its quota goes at once
       if (X.wl_fail[w] != INT32_MAX) X.wl_fail[w]--;
       const int k = X.wl_retries[w] + 1;
       X.adm_dead[a] = stamp;
       for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)
         atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
-      X.wl_last_gen[w] = -1;
-      for (int i = D.wl_ps_start[w] * D.R; i < D.wl_ps_start[w + 1] * D.R; i++) X.ps_last_tried[i] = -1;
-      if (X.wl_has_qr) X.wl_has_qr[w] = 0;
-      X.wl_admit_cycle[w] = -1;
+      drain_forget(D, X, w);
       if (k <= X.check_limit) {  // Retry: RequeueAt = verdict + WaitTime(k), queue-order timestamp = the eviction time
         const i64 wait = kb_check_wait_ns(k, X.check_base_s, X.check_max_s);
         X.wl_retries[w] = k;
@@ -747,12 +795,38 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
       return;
     }
   }
+  const int w = X.adm_wl[a];
+  if (ph == KB_PH_WAIT) {  // PodsReady timeout at T (workload_controller.go:805-855, UpdateRequeueState workload.go:707-722)
+    const i64 T = X.adm_finish[a];
+    if (X.wl_pr_fail[w] > 0 && X.wl_pr_fail[w] != INT32_MAX) X.wl_pr_fail[w]--;
+    const int n = X.wl_pr_count[w];
+    if (X.pr_limit >= 0 && n >= X.pr_limit) {  // Count + 1 > limit: deactivated, RequeueState cleared
+      X.wl_pr_count[w] = 0;
+      X.wl_deactivated[w] = 1;
+      atomicAdd(&X.counters[KB_DC_PR_DEACTIVATED], 1);
+    } else {  // BACKOFF at release: RequeueAt = T + WaitTime(Count); under Eviction the queue timestamp is T
+      const int k = n == INT32_MAX ? n : n + 1;
+      X.wl_pr_count[w] = k;
+      X.wl_requeue_at[w] = drain_sat_add(T, kb_pods_ready_wait_ns(k, X.pr_base_s, X.pr_max_s));
+      if (!X.pr_creation) X.wl_qts[w] = T;
+      atomicAdd(&X.counters[KB_DC_PR_TIMEOUT], 1);
+    }
+    ph = KB_PH_TIMED_OUT;
+    X.adm_phase[a] = ph;
+    if (X.wl_evict) {  // the pods terminate: the row holds its cells until T + latency, as an evicting row
+      X.adm_evicted[a] = 1;
+      X.adm_evicting[a] = 1;
+      X.adm_finish[a] = drain_sat_add(T, X.wl_evict[w]);
+      if (X.adm_finish[a] > X.clock[0]) return;
+    }
+  }
   X.adm_dead[a] = stamp;
   for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)
     atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
-  const int w = X.adm_wl[a];
+  const bool timed_out = ph == KB_PH_TIMED_OUT;
   const bool released = X.adm_evicting && X.adm_evicting[a];
-  if (released) drain_release(D, X, w);
+  if (timed_out) { drain_forget(D, X, w); X.wl_state[w] = X.wl_deactivated[w] ? KB_WS_DEACTIVATED : KB_WS_BACKOFF; }
+  else if (released) drain_release(D, X, w);
   else if (w >= 0) { X.wl_state[w] = KB_WS_FINISHED; X.wl_admit_cycle[w] = -1; X.wl_finish_ns[w] = X.adm_finish[a]; }
   if (X.lq_last && X.adm_lq[a] >= 0 && X.cq_afs[cq]) {  // several rows of one LocalQueue can finish together
     i64 *adm = X.lq_adm + (size_t)X.adm_lq[a] * D.R;
@@ -760,7 +834,7 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
       atomicAdd((unsigned long long *)&adm[X.adm_use_fr[c] % D.R], (unsigned long long)(-X.adm_use_qty[c]));
   }
   X.root_mark[D.root_slot[cq]] = stamp;
-  atomicAdd(&X.counters[released ? KB_DC_EVICT_DONE : KB_DC_FINISHED], 1);
+  if (!timed_out) atomicAdd(&X.counters[released ? KB_DC_EVICT_DONE : KB_DC_FINISHED], 1);
 }
 // decay samples (thread per LocalQueue of an AFS ClusterQueue): every sample due in (t, t'] with t' = clock[0], in time
 // order, each with alpha = afs_alpha (one interval elapsed), or a reset to empty with half-life 0; LastUpdate moves to

@@ -195,6 +195,36 @@ first Step returns the base uncapped (attempt 1 waits base, later ones max): the
 `adm_check_end_ns` (rows whose checks run, INT64_MIN = Admitted), `wl_requeue_at_ns` (records in backoff; one at or
 before now_ns is queued at the start), `wl_check_retries`.  Verdicts applied between the start of cycle c and of c+1
 are cycle c's (`check_retry`, `check_rejected`); those before cycle 0 count in the totals only.
+
+WaitForPodsReady (event mode, the snapshot carries `wl_pods_ready_ns` and `adm_wl`, include/kueue_b200.h).  A workload
+whose pods are not all Ready within `pods_ready_timeout_ns` of its Admitted condition is evicted (PodsReadyTimeout,
+reconcileNotReadyTimeout / admittedNotReadyWorkload workload_controller.go:805-835,1106-1130), requeued after a backoff
+(UpdateRequeueState workload.go:707-722) and deactivated past backoffLimitCount (triggerDeactivation :840-855).  It uses
+the BACKOFF / DEACTIVATED states, RequeueAt, `qts` and the re-sort of the admission checks.  An attempt is one admission:
+  1. it starts at Admitted: the reservation at t_c without a check delay, else the Ready verdict time;
+  2. it fails if the record has failures left in wl_pods_ready_fail (it uses one up; INT32_MAX = every attempt fails) or
+     wl_pods_ready_ns > pods_ready_timeout_ns; otherwise it is ready (a delay equal to the timeout is ready: a canonical
+     tie-break).  A ready attempt reaches PodsReady at Admitted + wl_pods_ready_ns and finishes at PodsReady + wl_run_ns
+     (saturating), with no event of its own;
+  3. a failing attempt has an event at T = Admitted + timeout (saturating; E includes it), applied after the boundary's
+     verdicts and before its completions.  With pods_ready_backoff_limit >= 0 and Count + 1 > limit: deactivation, Count
+     = 0.  Otherwise Count += 1 (saturating at INT32_MAX), RequeueAt = T + WaitTime(Count) (saturating), and under the
+     Eviction timestamp qts = T (GetQueueOrderTimestamp workload.go:1174-1182; Creation leaves it);
+  4. the timed-out row is evicted at T: with wl_evict_ns it is an evicting row until T + latency (it keeps its cells, a
+     preemptor that targets it is ongoing), without it is released by the boundary that applies T.  At release its cells
+     leave the usage, its root tree is requeued, and the record goes to DEACTIVATED or BACKOFF (rule 3 of the checks
+     queues it, in the same boundary when RequeueAt <= t_{c+1}) with LastAssignment nil (jobframework/reconciler.go:
+     576-590, workload_controller.go:323-375,973-1004).  Neither a completion nor a preemption eviction is counted;
+  5. a row preempted while its attempt waits (before PodsReady, or before T) loses it: not counted, no failure used
+     (workload_controller.go:808-811), wl_pods_ready_at keeps its previous value; the row goes as any preempted row;
+  6. an admission resets qts to wl_ts; Count survives a ready attempt;
+  7. start state: wl_pods_ready_count, adm_admitted_ns (a row whose pods are not ready: its attempt runs from that
+     Admitted time by rules 2-3 in place of adm_finish_ns), wl_requeue_at_ns, wl_pods_ready_evict_ns (qts under Eviction);
+  8. with every delay 0, every fail 0 and no start-state tables the drain equals the drain without the block.
+WaitTime(k) is `pods_ready_wait_ns`: wait.NewBackoff(base, max, 2, 0.0001).WaitTime(k) without jitter, in nanoseconds
+(the reference's RequeueAt carries a jitter below wait * 1e-4 at second precision).  Timeouts applied between the start of
+cycle c and of c+1 are cycle c's (`pods_ready_timeout`, `pods_ready_deactivated`).  blockAdmission and recoveryTimeout
+are not modelled.
 """
 from __future__ import annotations
 
@@ -252,6 +282,15 @@ class DrainResult:
     wl_queue_ts: np.ndarray | None = None                      # [n_wl] final queue-order timestamps
     n_resorts: int = 0
     resort_orders: List[dict] = field(default_factory=list)    # the rebuilt queue state after every re-sort
+    # WaitForPodsReady (wl_pods_ready_ns in the snapshot; None / empty / 0 otherwise); wl_deactivated also marks its
+    # deactivations
+    pods_ready_timeout: List[np.ndarray] = field(default_factory=list)      # per cycle: records timed out and requeued
+    pods_ready_timeout_at: List[np.ndarray] = field(default_factory=list)   # per cycle: [n, 2] their T and RequeueAt
+    pods_ready_deactivated: List[np.ndarray] = field(default_factory=list)  # per cycle: records deactivated by a timeout
+    n_pods_ready_timeout: int = 0                              # those before cycle 0 included
+    n_pods_ready_deactivated: int = 0
+    wl_pods_ready_at: np.ndarray | None = None                 # [n_wl] last PodsReady time, INT64_MIN = none
+    wl_pods_ready_count: np.ndarray | None = None              # [n_wl] final RequeueState.Count
 
     @property
     def n_evicted(self) -> int:
@@ -304,14 +343,17 @@ def requeue_goes_inadmissible(strict_fifo: bool, reason: str, last_tried) -> boo
 QUEUED, SET_ASIDE, HELD, ABSENT, FINISHED, BACKOFF, DEACTIVATED = 0, 1, 2, 3, 4, 5, 6  # queue state (kb_drain.cuh KB_WS_*)
 NEVER = np.iinfo(np.int64).max  # an event time that never comes
 UNSET = np.iinfo(np.int64).min
-ALL_FAIL = np.iinfo(np.int32).max  # wl_check_fail: every attempt fails
+ALL_FAIL = np.iinfo(np.int32).max  # wl_check_fail / wl_pods_ready_fail: every attempt fails
+RUN, WAIT, TIMED_OUT = 0, 2, 3  # PodsReady phase of a row (kb_drain.cuh KB_PH_*): its finish column holds the finish, T, the end
 MAX_BACKOFF_S = 10_000  # below it the reference's jittered, truncated WaitTime is exact
 
 
 def wait_time(base_ns: int, cap_ns: int, factor: float, iteration: int) -> int:
     """Backoff.WaitTime (pkg/util/wait/backoff.go:35-60) without jitter: wait.Backoff.Step `iteration` times (the
     duration grows by `factor` in float64 and is capped at Cap, after which Steps is 0 and Step returns Cap), stopping
-    at the cap.  cap_ns 0 = MaxInt64 / ceil(factor)."""
+    at the cap.  cap_ns 0 = MaxInt64 / ceil(factor).  A base of 0 stays 0 at every Step."""
+    if int(base_ns) == 0:
+        return 0
     cap = cap_ns if cap_ns else int(float(2**63 - 1) / math.ceil(factor))
     dur, capped, out = int(base_ns), False, 0
     for _ in range(iteration):
@@ -332,6 +374,12 @@ def check_wait_s(k: int, base_s: int, max_s: int) -> int:
     jitter, in whole seconds (kb_drain.cuh kb_check_wait_ns).  The first Step returns the base uncapped, so with
     base > max > 0 attempt 1 waits base and every later one max; otherwise it is min(base * 2^(k-1), max or infinity)."""
     return wait_time(int(base_s) * 1_000_000_000, int(max_s) * 1_000_000_000, 2.0, int(k)) // 1_000_000_000
+
+
+def pods_ready_wait_ns(k: int, base_s: int, max_s: int) -> int:
+    """WaitTime of PodsReady requeue k: wait.NewBackoff(base, max, 2, 0.0001).WaitTime(k) without jitter, in
+    nanoseconds (kb_drain.cuh kb_pods_ready_wait_ns)"""
+    return wait_time(int(base_s) * 1_000_000_000, int(max_s) * 1_000_000_000, 2.0, int(k))
 
 
 def check_wait_bound_s(base_s: int, max_s: int, limit: int) -> int:
@@ -567,15 +615,20 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     a = snap.arrays
     Q, R, FR = snap.n_cq, snap.n_resource, snap.n_fr
     checks = "wl_check_ns" in a
-    qts = a["wl_ts"].astype(np.int64).copy()                      # queue-order timestamps (admission checks: mutable)
-    if checks:
+    pr = "wl_pods_ready_ns" in a                                  # WaitForPodsReady
+    backoff = checks or pr                                        # BACKOFF / DEACTIVATED, RequeueAt, mutable qts
+    qts = a["wl_ts"].astype(np.int64).copy()                      # queue-order timestamps (checks, PodsReady: mutable)
+    if backoff:
         if "adm_wl" not in a:
-            raise ValueError("wl_check_ns needs adm_wl")
+            raise ValueError("wl_check_ns / wl_pods_ready_ns need adm_wl")
         held0 = np.zeros(snap.n_wl, bool)
         held0[a["adm_wl"].astype(np.int64)] = True
         if "wl_check_evict_ns" in a:
             ce = a["wl_check_evict_ns"].astype(np.int64)
             qts = np.where((ce != UNSET) & ~held0, ce, qts)
+        if pr and "wl_pods_ready_evict_ns" in a and not snap.pods_ready_requeue_creation:  # rule 7 (Eviction timestamp)
+            pe = a["wl_pods_ready_evict_ns"].astype(np.int64)
+            qts = np.where(pe != UNSET, pe, qts)
     order, qstart, seg_start, seg_lq = _queue_order(a, Q, qts)
     sort_ts = qts.copy()                                          # the keys the order was built with
     qlen = np.diff(qstart)
@@ -608,26 +661,51 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 adm_finish[evicting] = a["adm_evict_end_ns"][evicting]
     if replay:
         state[a["adm_wl"].astype(np.int64)] = HELD  # holds quota: out of every queue
-    if checks:  # rule 1: attempt state; start state of the rows whose checks run and of the records in backoff
-        chk_ns = a["wl_check_ns"].astype(np.int64)
-        chk_fail = a["wl_check_fail"].astype(np.int64).copy() if "wl_check_fail" in a else np.zeros(snap.n_wl, np.int64)
-        retries = a["wl_check_retries"].astype(np.int64).copy() if "wl_check_retries" in a else np.zeros(snap.n_wl, np.int64)
+    if backoff:  # records in backoff at the start
         requeue_at = np.full(snap.n_wl, UNSET, np.int64)
         if "wl_requeue_at_ns" in a:
             ra = a["wl_requeue_at_ns"].astype(np.int64)
             state[ra > snap.now_ns] = BACKOFF
             requeue_at[ra > snap.now_ns] = ra[ra > snap.now_ns]
+        deactivated = np.zeros(snap.n_wl, np.uint8)
+    if checks:  # rule 1: attempt state; start state of the rows whose checks run
+        chk_ns = a["wl_check_ns"].astype(np.int64)
+        chk_fail = a["wl_check_fail"].astype(np.int64).copy() if "wl_check_fail" in a else np.zeros(snap.n_wl, np.int64)
+        retries = a["wl_check_retries"].astype(np.int64).copy() if "wl_check_retries" in a else np.zeros(snap.n_wl, np.int64)
         checking = np.zeros(snap.n_adm, bool)
         if "adm_check_end_ns" in a:
             ce = a["adm_check_end_ns"].astype(np.int64)
             checking = ce != UNSET
             adm_finish[checking] = ce[checking]
         ready_ns = np.full(snap.n_wl, UNSET, np.int64)
-        deactivated = np.zeros(snap.n_wl, np.uint8)
         base_s, max_s, limit = int(snap.check_backoff_base_s), int(snap.check_backoff_max_s), int(snap.check_backoff_limit)
         verdicts = {"ready": 0, "retry": [], "rejected": []}
     else:
         checking = None
+    pr_phase = None                                               # [rows] PodsReady phase (RUN / WAIT / TIMED_OUT)
+    if pr:  # rules 2 and 7: attempt state, and the rows whose pods are not ready at the start
+        pr_ns = a["wl_pods_ready_ns"].astype(np.int64)
+        pr_fail = a["wl_pods_ready_fail"].astype(np.int64).copy() if "wl_pods_ready_fail" in a else np.zeros(snap.n_wl, np.int64)
+        pr_count = a["wl_pods_ready_count"].astype(np.int64).copy() if "wl_pods_ready_count" in a else np.zeros(snap.n_wl, np.int64)
+        pr_at = np.full(snap.n_wl, UNSET, np.int64)               # last PodsReady time
+        pr_prev = pr_at.copy()                                    # its value before the attempt under way
+        pr_timeout = int(snap.pods_ready_timeout_ns)
+        pr_base, pr_max, pr_limit = int(snap.pods_ready_backoff_base_s), int(snap.pods_ready_backoff_max_s), int(snap.pods_ready_backoff_limit)
+        pr_creation = bool(snap.pods_ready_requeue_creation)
+        timeouts = {"timeout": [], "at": [], "deactivated": []}
+
+        def pr_attempt(w, t0):
+            """rules 1-2: the attempt of record w Admitted at t0 -> (finish column, phase)"""
+            d = int(pr_ns[w])
+            if pr_fail[w] > 0 or d > pr_timeout:
+                return min(t0 + pr_timeout, NEVER), WAIT
+            pr_prev[w] = pr_at[w]
+            pr_at[w] = min(t0 + d, NEVER)
+            return (finish_time(int(pr_at[w]), int(run_ns[w])) if run_ns is not None else NEVER), RUN
+        pr_phase = np.full(snap.n_adm, RUN, np.int64)
+        if "adm_admitted_ns" in a:
+            for row in np.flatnonzero(a["adm_admitted_ns"] != UNSET):
+                adm_finish[row], pr_phase[row] = pr_attempt(int(adm_wl[row]), int(a["adm_admitted_ns"][row]))
     sticky = a["cq_sticky"].astype(np.int64).copy() if "cq_sticky" in a else None  # sticky workload per ClusterQueue
     cursor = np.zeros(len(qlen), np.int64)
     first_aside = qlen.copy()                                     # smallest SET_ASIDE position per segment (qlen = none)
@@ -734,7 +812,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
 
     def remove_rows(rows):
         """rows leave the admitted tables (cache.DeleteWorkload: cells out of the usage; the other rows keep their order)"""
-        nonlocal adm_wl, adm_finish, adm_lq, evicting, checking
+        nonlocal adm_wl, adm_finish, adm_lq, evicting, checking, pr_phase
         us, uf, uq = adm["adm_use_start"], adm["adm_use_fr"], adm["adm_use_qty"]
         for row in rows:
             cqi = int(adm["adm_cq"][row])
@@ -758,6 +836,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             evicting = evicting[keep]
         if checking is not None:
             checking = checking[keep]
+        if pr_phase is not None:
+            pr_phase = pr_phase[keep]
 
     def release(w):
         """the record of an evicted row returns to its queue with LastAssignment nil (workload_controller.go:973-1004);
@@ -775,7 +855,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         e = int(adm_finish.min()) if len(adm_finish) else NEVER
         if arr_next < len(arr_order):
             e = min(e, int(create[arr_order[arr_next]]))
-        if checks and (state == BACKOFF).any():
+        if backoff and (state == BACKOFF).any():
             e = min(e, int(requeue_at[state == BACKOFF].min()))
         return None if e >= NEVER else e
 
@@ -794,9 +874,12 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         for row in np.flatnonzero(checking & (adm_finish <= t_next)):
             w, tv = int(adm_wl[row]), int(adm_finish[row])
             checking[row] = False
-            if chk_fail[w] == 0:  # Ready: Admitted, the run clock starts
+            if chk_fail[w] == 0:  # Ready: Admitted, the run clock (or the PodsReady attempt) starts
                 ready_ns[w] = tv
-                adm_finish[row] = finish_time(tv, int(run_ns[w])) if run_ns is not None else NEVER
+                if pr:
+                    adm_finish[row], pr_phase[row] = pr_attempt(w, tv)
+                else:
+                    adm_finish[row] = finish_time(tv, int(run_ns[w])) if run_ns is not None else NEVER
                 verdicts["ready"] += 1
                 continue
             if chk_fail[w] != ALL_FAIL:
@@ -825,7 +908,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     def resort():
         """rule 6: rebuild the order when a queued or set-aside record carries a key other than the one it was sorted by"""
         nonlocal order, qstart, sort_ts
-        if not checks or not (((state == QUEUED) | (state == SET_ASIDE)) & (qts != sort_ts)).any():
+        if not backoff or not (((state == QUEUED) | (state == SET_ASIDE)) & (qts != sort_ts)).any():
             return
         order, qstart, _, _ = _queue_order(a, Q, qts)
         sort_ts = qts.copy()
@@ -842,21 +925,54 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                                       cursor=cursor.copy(), first_aside=first_aside.copy(), seg_of=seg_of.copy(),
                                       pos_of=pos_of.copy()))
 
+    def apply_timeouts(t_next):
+        """rules 3-4 of WaitForPodsReady: the timeouts due by t_next, after the verdicts and before the completions"""
+        for row in np.flatnonzero((pr_phase == WAIT) & (adm_finish <= t_next)):
+            w, T = int(adm_wl[row]), int(adm_finish[row])
+            if 0 < pr_fail[w] != ALL_FAIL:
+                pr_fail[w] -= 1
+            if pr_limit >= 0 and pr_count[w] + 1 > pr_limit:  # RequeuingLimitExceeded: deactivated, RequeueState cleared
+                pr_count[w] = 0
+                deactivated[w] = 1
+                timeouts["deactivated"].append(w)
+            else:
+                pr_count[w] = min(int(pr_count[w]) + 1, ALL_FAIL)
+                requeue_at[w] = min(T + pods_ready_wait_ns(int(pr_count[w]), pr_base, pr_max), NEVER)
+                if not pr_creation:
+                    qts[w] = T
+                timeouts["timeout"].append(w)
+                timeouts["at"].append((T, int(requeue_at[w])))
+            pr_phase[row] = TIMED_OUT
+            if lat is not None:  # the pods terminate: an evicting row until T + latency
+                evicting[row] = True
+                adm["adm_evicted"][row] = 1
+                adm_finish[row] = min(T + int(lat[w]), NEVER)
+
     def apply_events(t_next, notified):
         """steps 5 and 6 at t_next; returns (finished records, arrived records, records whose eviction completed)"""
         nonlocal arr_next
         if checks:
             apply_verdicts(t_next, notified)
+        if pr:
+            apply_timeouts(t_next)
         done = np.flatnonzero(adm_finish <= t_next)
         gone = evicting[done] if evicting is not None else np.zeros(len(done), bool)
-        fin, released = adm_wl[done[~gone]].copy(), adm_wl[done[gone]].copy()
+        to = pr_phase[done] == TIMED_OUT if pr else np.zeros(len(done), bool)
+        fin, released = adm_wl[done[~gone & ~to]].copy(), adm_wl[done[gone & ~to]].copy()
         for row in done:
             notified.add(int(adm["adm_cq"][row]))
             if decay and adm_lq[row] >= 0 and afs_cq[int(adm["adm_cq"][row])]:  # rule 5
                 for k in range(int(adm["adm_use_start"][row]), int(adm["adm_use_start"][row + 1])):
                     ladm[adm_lq[row], int(adm["adm_use_fr"][k]) % R] -= int(adm["adm_use_qty"][k])
             w = int(adm_wl[row])
-            if evicting is not None and evicting[row]:
+            if pr and pr_phase[row] == TIMED_OUT:  # rule 4: the record waits for RequeueAt, or is deactivated
+                state[w] = DEACTIVATED if deactivated[w] else BACKOFF
+                last_gen[w] = -1
+                last_tried[int(ps_start[w]):int(ps_start[w + 1])] = -1
+                if has_qr is not None:
+                    has_qr[w] = 0
+                admit_cycle[w] = -1
+            elif evicting is not None and evicting[row]:
                 release(w)
             elif w >= 0:
                 state[w] = FINISHED
@@ -869,7 +985,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             w = int(arr_order[arr_next]); arr_next += 1
             enqueue(w)
             arr.append(w)
-        if checks:  # rule 3: the records whose RequeueAt has come
+        if backoff:  # rule 3: the records whose RequeueAt has come
             for w in np.flatnonzero((state == BACKOFF) & (requeue_at <= t_next)):
                 requeue_at[w] = UNSET
                 enqueue(int(w))
@@ -903,6 +1019,15 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 res.check_retry[-1] = np.concatenate([res.check_retry[-1], ret])
                 res.check_rejected[-1] = np.concatenate([res.check_rejected[-1], rej])
             verdicts.update(ready=0, retry=[], rejected=[])
+        if pr:
+            to, de = np.asarray(timeouts["timeout"], np.int64), np.asarray(timeouts["deactivated"], np.int64)
+            res.n_pods_ready_timeout += len(to); res.n_pods_ready_deactivated += len(de)
+            if res.cycles:
+                res.pods_ready_timeout[-1] = np.concatenate([res.pods_ready_timeout[-1], to])
+                res.pods_ready_timeout_at[-1] = np.concatenate([res.pods_ready_timeout_at[-1],
+                                                                np.asarray(timeouts["at"], np.int64).reshape(-1, 2)])
+                res.pods_ready_deactivated[-1] = np.concatenate([res.pods_ready_deactivated[-1], de])
+            timeouts.update(timeout=[], at=[], deactivated=[])
 
     t = int(snap.now_ns)
     cyc = 0
@@ -966,6 +1091,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         res.cycle_start_ns.append(t)
         res.finished.append(np.zeros(0, np.int64)); res.arrived.append(np.zeros(0, np.int64)); res.evict_done.append(np.zeros(0, np.int64))
         res.check_retry.append(np.zeros(0, np.int64)); res.check_rejected.append(np.zeros(0, np.int64))
+        res.pods_ready_timeout.append(np.zeros(0, np.int64)); res.pods_ready_deactivated.append(np.zeros(0, np.int64))
+        res.pods_ready_timeout_at.append(np.zeros((0, 2), np.int64))
         ok = dec == abi.DEC_ASSUMED
         res.admitted.append(heads[ok])
         # ---- apply the admissions: Assignment.Usage (flavorassigner.go:198-218) with the admitted counts
@@ -1028,8 +1155,9 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 adm_wl = np.concatenate([adm_wl, g])
             if decay:
                 adm_lq = np.concatenate([adm_lq, a["wl_lq"][g].astype(np.int64)])
-            if checks:  # rules 1 and 4: a check delay starts an attempt, a delay of 0 is Ready at once
+            if backoff:  # rule 4 of the checks, 6 of PodsReady: the reservation resets Evicted
                 qts[g] = a["wl_ts"][g]
+            if checks:  # rule 1: a check delay starts an attempt, a delay of 0 is Ready at once
                 chk = chk_ns[g] > 0
                 checking = np.concatenate([checking, chk])
                 ready_ns[g[~chk]] = t
@@ -1037,6 +1165,12 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 fin_new = [finish_time(t, int(run_ns[w])) if run_ns is not None else NEVER for w in g]
                 if checks:
                     fin_new = [min(t + int(chk_ns[w]), NEVER) if chk_ns[w] > 0 else f for w, f in zip(g, fin_new)]
+                if pr:  # rule 1: Admitted now unless the checks run
+                    ph_new = np.full(n_new, RUN, np.int64)
+                    for i, w in enumerate(g):
+                        if not (checks and chk_ns[w] > 0):
+                            fin_new[i], ph_new[i] = pr_attempt(int(w), t)
+                    pr_phase = np.concatenate([pr_phase, ph_new])
                 adm_finish = np.concatenate([adm_finish, np.asarray(fin_new, np.int64)])
             if evicting is not None:
                 evicting = np.concatenate([evicting, np.zeros(n_new, bool)])
@@ -1100,11 +1234,17 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 if checking is not None and checking[row]:  # rule 5: no pods, released at the next boundary
                     checking[row] = False
                     adm_finish[row] = t
+                if pr:  # rule 5 of PodsReady: a waiting attempt is dropped
+                    pr_phase[row] = RUN
+                    if pr_at[w] > t:
+                        pr_at[w] = pr_prev[w]
                 evictions[w] += 1
         elif victims:
             for row in victims:
                 w = int(adm_wl[row])
                 release(w)
+                if pr and pr_at[w] > t:  # rule 5 of PodsReady: dropped before PodsReady
+                    pr_at[w] = pr_prev[w]
                 evictions[w] += 1
                 notified.add(int(adm["adm_cq"][row]))
             remove_rows(victims)
@@ -1144,10 +1284,14 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     res.wl_finish_ns = finish_ns
     res.end_ns = t
     res.cq_sticky = sticky
+    if backoff:
+        res.wl_deactivated, res.wl_queue_ts = deactivated, qts
     if checks:
-        res.wl_ready_ns, res.wl_check_retries, res.wl_deactivated = ready_ns, retries, deactivated
-        res.wl_queue_ts = qts
+        res.wl_ready_ns, res.wl_check_retries = ready_ns, retries
         res.adm["adm_checking"] = checking
+    if pr:
+        res.wl_pods_ready_at, res.wl_pods_ready_count = pr_at, pr_count
+        res.adm["adm_pods_ready_phase"] = pr_phase
     if decay:
         res.lq_consumed = consumed.astype(np.int64)
         res.lq_consumed_scale = cscale.astype(np.int32)

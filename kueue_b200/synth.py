@@ -319,6 +319,21 @@ def add_admission_checks(snap: abi.FlatSnapshot, seed: int = 0, delay_ns=(1_000,
     return snap
 
 
+def add_pods_ready(snap: abi.FlatSnapshot, seed: int = 0, delay_ns=(0, 2_000), fail_share: float = 0.1,
+                   timeout_ns: int = 5_000, base_s: int = 1, max_s: int = 8, limit: int = 2, creation: int = 0) -> abi.FlatSnapshot:
+    """WaitForPodsReady of an event drain (include/kueue_b200.h) on a snapshot with `adm_wl`, seeded: every workload
+    gets an Admitted -> PodsReady delay uniform in `delay_ns` (inclusive), and a share `fail_share` of them never
+    becomes ready (wl_pods_ready_fail = INT32_MAX).  timeout_ns, base_s, max_s, limit (-1 = nil) and creation are the
+    waitForPodsReady settings."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    W = snap.n_wl
+    snap.set("wl_pods_ready_ns", rng.integers(int(delay_ns[0]), int(delay_ns[1]) + 1, W))
+    snap.set("wl_pods_ready_fail", np.where(rng.random(W) < fail_share, np.iinfo(np.int32).max, 0))
+    snap.pods_ready_timeout_ns, snap.pods_ready_backoff_base_s, snap.pods_ready_backoff_max_s = int(timeout_ns), int(base_s), int(max_s)
+    snap.pods_ready_backoff_limit, snap.pods_ready_requeue_creation = int(limit), int(creation)
+    return snap
+
+
 # The reference's scheduler performance scenario (test/performance/scheduler/configs/baseline/generator.yaml, generated
 # by runner/generator/generator.go): 5 cohorts of 6 ClusterQueues, one flavor, cpu only; per ClusterQueue, workload k of
 # a class is created at (k + 1) * interval and runs `run` once admitted (runner/controller/controller.go).
@@ -332,7 +347,8 @@ PERF_NOMINAL_CPU, PERF_BORROW_CPU = 20, 100
 _MS = 1_000_000
 
 
-def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None = None, checks: int | None = None) -> abi.FlatSnapshot:
+def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None = None, checks: int | None = None,
+                  pods_ready: int | None = None) -> abi.FlatSnapshot:
     """The baseline scenario as numbers (15,000 workloads at scale 1; `scale` multiplies the count of every class):
     nominal 20 cpu and borrowingLimit 100 cpu per ClusterQueue, preemption reclaimWithinCohort Any and
     withinClusterQueue LowerPriority, BestEffortFIFO.  cpu is in milli-units.  wl_ts is the creation time, an empty
@@ -340,7 +356,9 @@ def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None 
     evict_ns: the termination latency of every workload (wl_evict_ns: an eviction releases its quota that long after it
     is issued); None = every eviction completes before the next cycle.
     checks: a seed: every other ClusterQueue of each cohort gets an admission check (add_admission_checks: a
-    ProvisioningRequest-like delay of 20-200 ms, a share of failing attempts, backoff base 1 s, max 8 s, limit 3)."""
+    ProvisioningRequest-like delay of 20-200 ms, a share of failing attempts, backoff base 1 s, max 8 s, limit 3).
+    pods_ready: a seed: WaitForPodsReady on every workload (add_pods_ready: a PodsReady delay of 0-50 ms, 10% of the
+    workloads never ready, timeout 100 ms, backoff base 1 s, max 8 s, limit 2)."""
     Q = PERF_COHORTS * PERF_CQS_PER_COHORT
     snap = abi.FlatSnapshot(n_cq=Q, n_cohort=PERF_COHORTS, n_flavor=1, n_resource=1)
     snap.set("parent", np.concatenate([Q + np.arange(Q) // PERF_CQS_PER_COHORT, np.full(PERF_COHORTS, -1)]))
@@ -372,6 +390,8 @@ def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None 
     snap.drain_cycle_ns = cycle_ns
     if checks is not None:
         add_admission_checks(snap, checks, delay_ns=(20 * _MS, 200 * _MS), cqs=np.arange(0, Q, 2))
+    if pods_ready is not None:
+        add_pods_ready(snap, pods_ready, delay_ns=(0, 50 * _MS), timeout_ns=100 * _MS)
     snap.finalize()
     snap.__dict__["perf_class"] = np.asarray(cls, np.int64)
     return snap
