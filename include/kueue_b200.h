@@ -398,6 +398,23 @@ typedef struct kb_snapshot {
   int32_t pods_ready_backoff_max_s;      /* requeuingStrategy.backoffMaxSeconds (>= 0; 0 = no cap)                       */
   int32_t pods_ready_backoff_limit;      /* requeuingStrategy.backoffLimitCount; -1 = nil (requeue forever)              */
   int32_t pods_ready_requeue_creation;   /* requeuingStrategy.timestamp: 0 = Eviction (default), 1 = Creation            */
+
+  /* ---- MaximumExecutionTimeSeconds (optional; read by kb_run_drain only, kb_run_cycle ignores them) ----
+     In the reference a workload that has spent spec.maximumExecutionTimeSeconds in the Admitted state, summed over its
+     admissions in status.accumulatedPastExecutionTimeSeconds, is deactivated with reason MaximumExecutionTimeExceeded
+     and never requeued (workload_types.go:71-77,658-662; reconcileMaxExecutionTime workload_controller.go:619-646;
+     SyncAdmittedCondition admissionchecks.go:36-86).  wl_max_exec_s == NULL: off, and every launch, copy and result of
+     the drain stays as without this block.  A non-NULL wl_max_exec_s turns on event mode and needs adm_wl.  The block
+     composes with admission checks (the clock starts at the Ready verdict), WaitForPodsReady, eviction latency, the
+     sticky table and AFS.  See kb_run_drain.  Errors: KB_ERR_INVALID for any table of this block without
+     wl_max_exec_s or without adm_wl, wl_max_exec_s[w] < 0, wl_exec_acc_s[w] < -1, adm_exec_since_ns NULL while
+     n_adm > 0, adm_exec_since_ns[a] > now_ns, INT64_MIN on a row whose checks do not run or another value on one whose
+     checks run (adm_check_end_ns), a value other than adm_admitted_ns[a] where that is set; KB_ERR_UNSUPPORTED when an
+     attempt's seconds or the accumulated sum leaves int32 (the reference's int32 conversion is then undefined). */
+  const int32_t *wl_max_exec_s;     /* [n_wl] spec.maximumExecutionTimeSeconds; 0 = nil (no limit)                      */
+  const int32_t *wl_exec_acc_s;     /* [n_wl] status.accumulatedPastExecutionTimeSeconds at the start; -1 = nil; NULL =
+                                       every value nil                                                                  */
+  const int64_t *adm_exec_since_ns; /* [n_adm] Admitted LastTransitionTime of each row; INT64_MIN = its checks run     */
 } kb_snapshot;
 
 /* ------------------------------------------------------------------------
@@ -667,7 +684,43 @@ int32_t kb_download(kb_handle *h, kb_cycle_out *out);
  * Timeouts applied between the start of cycle c and of c+1 count in cycle_pods_ready_timeout / _deactivated[c].
  * Not modelled: waitForPodsReady.blockAdmission (the reference stops the admit loop mid-cycle until every admitted
  * workload is ready, scheduler.go:361-373, which a cycle evaluated at one instant cannot express) and recoveryTimeout
- * (the drain models no pod failure after PodsReady). */
+ * (the drain models no pod failure after PodsReady).
+ *
+ * MaximumExecutionTimeSeconds (kb_snapshot.wl_max_exec_s != NULL, with adm_wl; event mode).  Every record has a limit
+ * max (wl_max_exec_s, 0 = nil) and an accumulated time acc (wl_exec_acc_s, -1 = nil, read as 0 below).  Additions:
+ *   1. every row has an Admitted time A: the reservation t_c when the workload has no check delay, else its Ready
+ *      verdict time; a row whose checks run has none (SyncAdmittedCondition admissionchecks.go:36-70: Admitted is
+ *      QuotaReserved with every check Ready).  A row of a record with a limit has the deadline D = A + (max - acc) * 1e9
+ *      (saturating) and the effective deadline max(D, A, now_ns): a negative max - acc, or a snapshot row already past
+ *      its limit, expires at the first boundary that can apply it (reconcileMaxExecutionTime workload_controller.go:
+ *      619-646 computes remaining = (max - acc) s - (now - A) and acts on remaining <= 0);
+ *   2. the expiry is an event: the finish column holds the earlier of the row's own next event (its finish, or the
+ *      PodsReady timeout T of a failing attempt) and the effective deadline, and a row whose deadline came first is
+ *      marked (kb_drain.cuh KB_PH_EXPIRE).  Ties go to the own event: a finish at the deadline finishes, a PodsReady
+ *      timeout at the deadline is a timeout (rule 4 then deactivates the workload at its release).  Expiries are applied
+ *      in step 5 after the check verdicts and the PodsReady timeouts, before the completions;
+ *   3. at its expiry the workload is deactivated (reason MaximumExecutionTimeExceeded, SetDeactivationTarget
+ *      :619-646; the inactive branch :316-321,386-420 evicts it and clears RequeueState: Count 0, no RequeueAt) and acc
+ *      becomes nil.  A WaitForPodsReady attempt still waiting is dropped (not counted, no failure used,
+ *      wl_pods_ready_at_ns keeps its previous value).  The row is evicted at the effective deadline: with wl_evict_ns it
+ *      holds its cells as an evicting row until deadline + latency (a preemptor that targets it is ongoing); without, it
+ *      is released at the boundary that applies the deadline.  At release the record is DEACTIVATED;
+ *   4. every release of a row that has an Admitted time (a completed preemption, a PodsReady-timeout release, an expiry
+ *      release) adds d = int32(Duration(t - A).Seconds()) to acc, or sets acc = d when nil (the Admitted true -> false
+ *      transition happens when the quota reservation is removed, UnsetQuotaReservationWithCondition workload.go:684-704,
+ *      so termination latency counts).  t is the end of the eviction: T or the effective deadline without latency, t_c
+ *      for a preemption without latency.  Completions and rows whose checks run add nothing.  Truncation is per
+ *      attempt: Seconds() is float64(sec) + float64(nsec) / 1e9, which from about 2^24 s can round up to sec + 1
+ *      (kb_drain.cuh kb_exec_seconds).  If a row's deadline D is at or before its release t and the workload was not
+ *      deactivated already (RequeuingLimitExceeded sets DeactivationTarget first, :840-851, and reconcileMaxExecutionTime
+ *      then leaves it), rule 3 applies at that release in place of the requeue or the backoff: a deadline that passes
+ *      while an eviction is under way (both reconcilers run while the reservation is held, :509-536).  It leaves acc =
+ *      d of that last attempt (the nil reset, then the addition) and counts at the boundary of the release;
+ *   5. condition times keep nanoseconds (the API server stores seconds).  With every limit nil and no start state the
+ *      drain equals the drain without the block in heads, decisions, evictions, usage and per-workload results; only
+ *      wl_exec_acc_s_out is new.
+ * Deactivations (at an expiry or a release) between the start of cycle c and of c+1 count in
+ * cycle_max_exec_deactivated[c].  Not modelled: reactivation (a user action), MultiKueue's handling of the field. */
 typedef struct kb_drain_out {
   int32_t max_cycles;        /* in */
   int32_t n_cycles;          /* out: cycles run */
@@ -719,8 +772,9 @@ typedef struct kb_drain_out {
   int32_t *cycle_check_rejected; /* [max_cycles] Rejected verdicts, likewise */
   int64_t *wl_ready_ns;          /* [n_wl] time of the last Admitted in the drain, INT64_MIN if none */
   int32_t *wl_check_retries_out; /* [n_wl] final RetryCount */
-  uint8_t *wl_deactivated;       /* [n_wl] 1 if the workload was deactivated (Rejected, or RequeuingLimitExceeded with
-                                    kb_snapshot.wl_pods_ready_ns, which also writes it and the two fields below) */
+  uint8_t *wl_deactivated;       /* [n_wl] 1 if the workload was deactivated (Rejected, RequeuingLimitExceeded with
+                                    kb_snapshot.wl_pods_ready_ns or MaximumExecutionTimeExceeded with
+                                    kb_snapshot.wl_max_exec_s, which also write it and the two fields below) */
   int64_t n_resorts;             /* out: queue re-sorts (a record entered its queue with a new queue-order timestamp) */
   double resort_ms;              /* out: device time of those re-sorts (part of gpu_ms) */
   /* WaitForPodsReady (kb_snapshot.wl_pods_ready_ns != NULL; zero / untouched otherwise; each pointer may be NULL).
@@ -732,6 +786,12 @@ typedef struct kb_drain_out {
   int64_t *wl_pods_ready_at_ns;          /* [n_wl] PodsReady time of the last attempt that reached it, or will (a row still
                                             waiting at the end of the drain); INT64_MIN if none */
   int32_t *wl_pods_ready_count_out;      /* [n_wl] final RequeueState.Count */
+  /* MaximumExecutionTimeSeconds (kb_snapshot.wl_max_exec_s != NULL; zero / untouched otherwise; each pointer may be
+     NULL).  wl_deactivation_reason is written whenever wl_deactivated is. */
+  int64_t n_max_exec_deactivated;        /* out: deactivations for MaximumExecutionTimeExceeded, those before cycle 0 included */
+  int32_t *cycle_max_exec_deactivated;   /* [max_cycles] deactivations from the start of cycle c to the start of c+1 */
+  int32_t *wl_exec_acc_s_out;            /* [n_wl] final accumulatedPastExecutionTimeSeconds, -1 = nil */
+  uint8_t *wl_deactivation_reason;       /* [n_wl] 0 none, 1 Rejected, 2 RequeuingLimitExceeded, 3 MaximumExecutionTimeExceeded */
 } kb_drain_out;
 int32_t kb_run_drain(kb_handle *h, const kb_snapshot *s, kb_drain_out *out);
 

@@ -381,6 +381,10 @@ func (s *Scheduler) flatten(snap *schdcache.Snapshot, heads []workload.Info, gen
 	//   c.wl_pods_ready_evict_ns, c.adm_admitted_ns = cp64(timeoutEvictedAt), cp64(admittedNotReadyAt)
 	//   c.pods_ready_timeout_ns, c.pods_ready_backoff_base_s, c.pods_ready_backoff_max_s = timeout, base, max
 	//   c.pods_ready_backoff_limit, c.pods_ready_requeue_creation = limitOrMinus1, creation
+	// MaximumExecutionTimeSeconds (INTEGRATION.md): the limit from Spec.MaximumExecutionTimeSeconds (nil = 0), the
+	// accumulated time from Status.AccumulatedPastExecutionTimeSeconds (nil = -1), and each admitted row's Admitted time
+	// from the Admitted condition's LastTransitionTime (math.MinInt64 while its checks are not all Ready):
+	//   c.wl_max_exec_s, c.wl_exec_acc_s, c.adm_exec_since_ns = cp32(maxExecS), cp32(accS), cp64(admittedAt)
 	// They stay nil here: a single cycle ignores them.
 	if anyGroup { // optional table: NULL when no podset is grouped
 		c.ps_group = cp32(psGroup)

@@ -91,6 +91,7 @@ class kb_snapshot(C.Structure):
         ("wl_pods_ready_evict_ns", _P(C.c_int64)), ("adm_admitted_ns", _P(C.c_int64)),
         ("pods_ready_timeout_ns", C.c_int64), ("pods_ready_backoff_base_s", C.c_int32), ("pods_ready_backoff_max_s", C.c_int32),
         ("pods_ready_backoff_limit", C.c_int32), ("pods_ready_requeue_creation", C.c_int32),
+        ("wl_max_exec_s", _P(C.c_int32)), ("wl_exec_acc_s", _P(C.c_int32)), ("adm_exec_since_ns", _P(C.c_int64)),
     ]
 
 
@@ -149,6 +150,8 @@ class kb_drain_out(C.Structure):
         ("n_pods_ready_timeout", C.c_int64), ("n_pods_ready_deactivated", C.c_int64),
         ("cycle_pods_ready_timeout", _P(C.c_int32)), ("cycle_pods_ready_deactivated", _P(C.c_int32)),
         ("wl_pods_ready_at_ns", _P(C.c_int64)), ("wl_pods_ready_count_out", _P(C.c_int32)),
+        ("n_max_exec_deactivated", C.c_int64), ("cycle_max_exec_deactivated", _P(C.c_int32)),
+        ("wl_exec_acc_s_out", _P(C.c_int32)), ("wl_deactivation_reason", _P(C.c_uint8)),
     ]
 
 
@@ -209,12 +212,13 @@ _DT = {
     "wl_requeue_at_ns": np.int64, "adm_check_end_ns": np.int64,
     "wl_pods_ready_ns": np.int64, "wl_pods_ready_fail": np.int32, "wl_pods_ready_count": np.int32,
     "wl_pods_ready_evict_ns": np.int64, "adm_admitted_ns": np.int64,
+    "wl_max_exec_s": np.int32, "wl_exec_acc_s": np.int32, "adm_exec_since_ns": np.int64,
 }
 # AdmissionFairSharing tables (include/kueue_b200.h): wl_lq absent = AFS off
 AFS_FIELDS = ("wl_lq", "lq_cq", "cq_afs", "lq_weight", "lq_consumed", "lq_consumed_scale", "lq_penalty", "afs_res_weight",
               "afs_milli_mul")
 # arrivals and completions of kb_run_drain's event mode (include/kueue_b200.h): all absent = event mode off
-EVENT_FIELDS = ("wl_create_ns", "wl_run_ns", "adm_finish_ns", "wl_evict_ns", "wl_check_ns", "wl_pods_ready_ns")
+EVENT_FIELDS = ("wl_create_ns", "wl_run_ns", "adm_finish_ns", "wl_evict_ns", "wl_check_ns", "wl_pods_ready_ns", "wl_max_exec_s")
 # decay of the AdmissionFairSharing consumed usage in event mode (include/kueue_b200.h): lq_last_update_ns absent = off
 AFS_DECAY_FIELDS = ("lq_last_update_ns", "adm_lq")
 # end times of the evictions under way before an event drain with wl_evict_ns (include/kueue_b200.h): absent = none known
@@ -225,9 +229,11 @@ STICKY_FIELDS = ("cq_sticky",)
 CHECK_FIELDS = ("wl_check_ns", "wl_check_fail", "wl_check_retries", "wl_check_evict_ns", "wl_requeue_at_ns", "adm_check_end_ns")
 # WaitForPodsReady in event mode (include/kueue_b200.h): wl_pods_ready_ns absent = off; the others need it
 PODS_READY_FIELDS = ("wl_pods_ready_ns", "wl_pods_ready_fail", "wl_pods_ready_count", "wl_pods_ready_evict_ns", "adm_admitted_ns")
+# MaximumExecutionTimeSeconds in event mode (include/kueue_b200.h): wl_max_exec_s absent = off; the others need it
+MAX_EXEC_FIELDS = ("wl_max_exec_s", "wl_exec_acc_s", "adm_exec_since_ns")
 OPTIONAL_FIELDS = (("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows", "adm_wl") + AFS_FIELDS +
                    EVENT_FIELDS + AFS_DECAY_FIELDS + EVICT_END_FIELDS + STICKY_FIELDS + CHECK_FIELDS +
-                   PODS_READY_FIELDS)  # NULL in kb_snapshot when absent
+                   PODS_READY_FIELDS + MAX_EXEC_FIELDS)  # NULL in kb_snapshot when absent
 ARRAY_FIELDS = list(_DT.keys())
 # tables the library keeps resident while kb_snapshot.static_generation is unchanged (include/kueue_b200.h)
 STATIC_FIELDS = ("parent", "fair_weight", "nominal", "borrow_limit", "lend_limit", "cq_within_cq", "cq_reclaim_within",
@@ -488,6 +494,9 @@ class DrainOut:
         self.cycle_pods_ready_deactivated = np.zeros(max_cycles, np.int32)
         self.wl_pods_ready_at_ns = np.full(W, KB_TS_UNSET, np.int64)
         self.wl_pods_ready_count_out = np.zeros(W, np.int32)
+        self.cycle_max_exec_deactivated = np.zeros(max_cycles, np.int32)  # MaximumExecutionTimeSeconds (kb_snapshot.wl_max_exec_s)
+        self.wl_exec_acc_s_out = np.full(W, -1, np.int32)
+        self.wl_deactivation_reason = np.zeros(W, np.uint8)
         cap = (min(W * 4 + Q, min(Q, W) * max_cycles) if trace_capacity is None else trace_capacity) if trace else 0
         self.trace_wl = np.zeros(max(1, cap), np.int32)
         self.trace_decision = np.zeros(max(1, cap), np.uint8)
@@ -515,6 +524,9 @@ class DrainOut:
         s.cycle_pods_ready_deactivated = _ptr(self.cycle_pods_ready_deactivated, C.c_int32)
         s.wl_pods_ready_at_ns = _ptr(self.wl_pods_ready_at_ns, C.c_int64)
         s.wl_pods_ready_count_out = _ptr(self.wl_pods_ready_count_out, C.c_int32)
+        s.cycle_max_exec_deactivated = _ptr(self.cycle_max_exec_deactivated, C.c_int32)
+        s.wl_exec_acc_s_out = _ptr(self.wl_exec_acc_s_out, C.c_int32)
+        s.wl_deactivation_reason = _ptr(self.wl_deactivation_reason, C.c_uint8)
         if trace:
             s.trace_wl = _ptr(self.trace_wl, C.c_int32); s.trace_decision = _ptr(self.trace_decision, C.c_uint8)
         s.trace_capacity = cap
@@ -554,6 +566,8 @@ class DrainOut:
     def n_pods_ready_timeout(self): return int(self.struct.n_pods_ready_timeout)
     @property
     def n_pods_ready_deactivated(self): return int(self.struct.n_pods_ready_deactivated)
+    @property
+    def n_max_exec_deactivated(self): return int(self.struct.n_max_exec_deactivated)
 
     def cycles(self):
         """[(heads, decisions)] per cycle from the trace."""

@@ -1356,7 +1356,7 @@ extern "C" int32_t kb_run_cycle(kb_handle *h, const kb_snapshot *s, kb_cycle_out
 // ---------------------------------------------------------------------------
 // what a boundary of kb_run_drain reads back, in the pinned host words [8, 24)
 struct DrainWords {
-  uint32_t counters[KB_DC_PR_DEACTIVATED + 1];  // DrainDev::counters; [0] = heads of the next cycle
+  uint32_t counters[KB_DC_EXEC_STATUS + 1];  // DrainDev::counters; [0] = heads of the next cycle
   uint32_t n_new, n_cells;              // this cycle's admissions and their usage cells (the admit scans' totals)
   uint32_t status;                      // the cycle's status word (KBS_AFS_OVERFLOW)
   i64 t_next;                           // event mode: t_{c+1}
@@ -1370,7 +1370,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   out->n_cycles = 0; out->n_decisions = 0; out->n_admitted = 0; out->gpu_ms = 0; out->n_evicted = 0;
   out->n_finished = 0; out->n_arrived = 0; out->end_ns = s->now_ns; out->n_evict_done = 0;
   out->n_check_ready = 0; out->n_check_retry = 0; out->n_check_rejected = 0; out->n_resorts = 0; out->resort_ms = 0;
-  out->n_pods_ready_timeout = 0; out->n_pods_ready_deactivated = 0;
+  out->n_pods_ready_timeout = 0; out->n_pods_ready_deactivated = 0; out->n_max_exec_deactivated = 0;
   // ---- eviction replay: host-side checks of adm_wl (include/kueue_b200.h)
   const bool replay = s->adm_wl != nullptr;
   if (replay) {
@@ -1386,7 +1386,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     }
   }
   // ---- event mode: host-side checks of the arrival and completion tables (include/kueue_b200.h)
-  const bool events = s->wl_create_ns || s->wl_run_ns || s->adm_finish_ns || s->wl_evict_ns || s->wl_check_ns || s->wl_pods_ready_ns;
+  const bool events = s->wl_create_ns || s->wl_run_ns || s->adm_finish_ns || s->wl_evict_ns || s->wl_check_ns || s->wl_pods_ready_ns ||
+                      s->wl_max_exec_s;
   if (events) {
     if (s->adm_finish_ns)
       for (int a = 0; a < s->n_adm; a++)
@@ -1510,6 +1511,26 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
           return fail(h, KB_ERR_INVALID, "pods ready: adm_admitted_ns on a row whose eviction is under way (adm_evict_end_ns)");
       }
   }
+  // ---- MaximumExecutionTimeSeconds: host-side checks (include/kueue_b200.h)
+  const bool mx = s->wl_max_exec_s != nullptr;
+  if (mx || s->wl_exec_acc_s || s->adm_exec_since_ns) {
+    if (!mx) return fail(h, KB_ERR_INVALID, "max exec: the tables need wl_max_exec_s");
+    if (!replay) return fail(h, KB_ERR_INVALID, "max exec: the tables need adm_wl");
+    for (int w = 0; w < W; w++) {
+      if (s->wl_max_exec_s[w] < 0) return fail(h, KB_ERR_INVALID, "max exec: wl_max_exec_s < 0");
+      if (s->wl_exec_acc_s && s->wl_exec_acc_s[w] < -1) return fail(h, KB_ERR_INVALID, "max exec: wl_exec_acc_s < -1");
+    }
+    if (s->n_adm > 0 && !s->adm_exec_since_ns) return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns is NULL while n_adm > 0");
+    for (int a = 0; a < s->n_adm; a++) {
+      const i64 A = s->adm_exec_since_ns[a];
+      const bool chk = checks && s->adm_check_end_ns && s->adm_check_end_ns[a] != INT64_MIN;
+      if (A == INT64_MIN && !chk) return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns missing on a row whose checks do not run");
+      if (A != INT64_MIN && chk) return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns set on a row whose checks run (adm_check_end_ns)");
+      if (A > s->now_ns) return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns after now_ns");
+      if (pr && s->adm_admitted_ns && s->adm_admitted_ns[a] != INT64_MIN && s->adm_admitted_ns[a] != A)
+        return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns differs from adm_admitted_ns");
+    }
+  }
   out->n_afs_samples = 0;
   if (Hcap == 0 || max_cycles == 0) return KB_OK;
   size_t extra = (size_t)std::min<long long>((long long)W, (long long)Hcap * max_cycles);
@@ -1588,6 +1609,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   int32_t *vals[2], *arr_vals[2] = {nullptr, nullptr}, *q_count, *d_wl_class = nullptr, *d_cq_class_start = nullptr;
   char *sort_tmp, *scan_tmp = nullptr;
   i64 *run = nullptr, *create = nullptr, *evict_ns = nullptr, *check_ns = nullptr, *pr_ns = nullptr;
+  int32_t *max_exec = nullptr;
   DrainDev X{};
   AdmTabs other{};  // compaction: the other half of the admitted tables' double buffer
   auto layout = [&](Arena &a) {
@@ -1600,7 +1622,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     X.flag = a.take<int32_t>((size_t)Q + 2); X.pos = a.take<int32_t>((size_t)Q + 2);
     X.e_assumed = a.take<int32_t>(Hz + 2); X.e_ncells = a.take<int32_t>(Hz + 2);
     X.e_adm_off = a.take<int32_t>(Hz + 2); X.e_cell_off = a.take<int32_t>(Hz + 2);
-    X.counters = a.take<int32_t>(KB_DC_PR_DEACTIVATED + 1);
+    X.counters = a.take<int32_t>(KB_DC_EXEC_STATUS + 1);
     X.wl_admit_cycle = a.take<int32_t>(Wz); X.wl_evals = a.take<int32_t>(Wz); X.wl_last_decision = a.take<uint8_t>(Wz);
     if (trace_cap) { X.trace_wl = a.take<int32_t>(trace_cap); X.trace_dec = a.take<uint8_t>(trace_cap); }
     if (replay || events) {
@@ -1642,10 +1664,17 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       pr_ns = a.take<i64>(Wz); X.wl_pr_fail = a.take<int32_t>(Wz); X.wl_pr_count = a.take<int32_t>(Wz);
       X.wl_pr_at = a.take<i64>(Wz); X.wl_pr_prev = a.take<i64>(Wz);
     }
-    if (requeue) {  // timestamps, requeue state and the phase byte of both halves
+    if (requeue) {  // timestamps and requeue state
       X.wl_ts0 = a.take<i64>(Wz); X.wl_sort_ts = a.take<i64>(Wz); X.wl_requeue_at = a.take<i64>(Wz);
-      X.wl_ready_ns = a.take<i64>(Wz); X.wl_deactivated = a.take<uint8_t>(Wz);
+      X.wl_ready_ns = a.take<i64>(Wz);
+    }
+    if (requeue || mx) {  // deactivation reasons and the phase byte of both halves
+      X.wl_deactivated = a.take<uint8_t>(Wz);
       X.adm_phase = a.take<uint8_t>(Acap); other.phase = a.take<uint8_t>(Acap);
+    }
+    if (mx) {  // limits, accumulated times and the Admitted time of both halves
+      max_exec = a.take<int32_t>(Wz); X.wl_exec_acc = a.take<int32_t>(Wz);
+      X.adm_exec_since = a.take<i64>(Acap); other.since = a.take<i64>(Acap);
     }
     if (afs) {
       X.seg_start = a.take<int32_t>(seg_start.size()); X.lq_seg = a.take<int32_t>(lq_seg.size());
@@ -1693,26 +1722,32 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       never.swap(fin);
       finish = never.data();
     }
-    if ((checks && s->adm_check_end_ns) || (pr && s->adm_admitted_ns)) {  // rows whose checks run: the verdict time in the
-      // finish column; rows whose pods are not ready: their attempt from Admitted (drain_pr_attempt; no failure is used
-      // until a timeout is applied), T in the finish column of a failing one
+    if ((checks && s->adm_check_end_ns) || (pr && s->adm_admitted_ns) || (mx && s->n_adm > 0)) {  // rows whose checks run:
+      // the verdict time in the finish column; rows whose pods are not ready: their attempt from Admitted
+      // (drain_pr_attempt; no failure is used until a timeout is applied), T in the finish column of a failing one; rows
+      // with an Admitted time and a limit, not evicting: the effective deadline max(D, A, now_ns) where it comes first
       std::vector<i64> fin((size_t)s->n_adm);
       std::vector<uint8_t> ph((size_t)s->n_adm, KB_PH_RUN);
       memcpy(fin.data(), finish, (size_t)s->n_adm * 8);
       for (int a = 0; a < s->n_adm; a++) {
         if (checks && s->adm_check_end_ns && s->adm_check_end_ns[a] != INT64_MIN) { fin[a] = s->adm_check_end_ns[a]; ph[a] = KB_PH_CHECK; }
-        if (!pr || !s->adm_admitted_ns || s->adm_admitted_ns[a] == INT64_MIN) continue;
-        const int w = s->adm_wl[a];
-        const i64 t0 = s->adm_admitted_ns[a], d = s->wl_pods_ready_ns[w], to = s->pods_ready_timeout_ns;
-        const i64 run = s->wl_run_ns ? s->wl_run_ns[w] : -1;
-        if ((s->wl_pods_ready_fail && s->wl_pods_ready_fail[w] > 0) || d > to) { fin[a] = t0 > INT64_MAX - to ? INT64_MAX : t0 + to; ph[a] = KB_PH_WAIT; }
-        else { const i64 at = t0 > INT64_MAX - d ? INT64_MAX : t0 + d; fin[a] = run < 0 ? INT64_MAX : (at > INT64_MAX - run ? INT64_MAX : at + run); }
+        const int w = replay ? s->adm_wl[a] : -1;
+        if (pr && s->adm_admitted_ns && s->adm_admitted_ns[a] != INT64_MIN) {
+          const i64 t0 = s->adm_admitted_ns[a], d = s->wl_pods_ready_ns[w], to = s->pods_ready_timeout_ns;
+          const i64 run = s->wl_run_ns ? s->wl_run_ns[w] : -1;
+          if ((s->wl_pods_ready_fail && s->wl_pods_ready_fail[w] > 0) || d > to) { fin[a] = t0 > INT64_MAX - to ? INT64_MAX : t0 + to; ph[a] = KB_PH_WAIT; }
+          else { const i64 at = t0 > INT64_MAX - d ? INT64_MAX : t0 + d; fin[a] = run < 0 ? INT64_MAX : (at > INT64_MAX - run ? INT64_MAX : at + run); }
+        }
+        if (!mx || s->adm_exec_since_ns[a] == INT64_MIN || s->wl_max_exec_s[w] <= 0 || (!evicting.empty() && evicting[a])) continue;
+        const i64 A = s->adm_exec_since_ns[a];
+        const i64 dl = std::max({kb_exec_deadline(A, s->wl_max_exec_s[w], s->wl_exec_acc_s ? s->wl_exec_acc_s[w] : -1), A, (i64)s->now_ns});
+        if (dl < fin[a]) { fin[a] = dl; ph[a] = KB_PH_EXPIRE; }
       }
       never.swap(fin);
       finish = never.data();
       CUDA_TRY(h, h2d(h, X.adm_phase, ph.data(), ph.size()));
       CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // ph is a local
-    } else if (requeue) {
+    } else if (requeue || mx) {
       CUDA_TRY(h, cudaMemsetAsync(X.adm_phase, KB_PH_RUN, (size_t)s->n_adm, h->stream));
     }
     CUDA_TRY(h, h2d(h, X.adm_finish, finish, (size_t)s->n_adm * 8));
@@ -1796,6 +1831,16 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     CUDA_TRY(h, h2d(h, X.wl_pr_prev, pr_none.data(), Wz * 8));  // no PodsReady before the attempts under way
     X.pr_timeout = s->pods_ready_timeout_ns; X.pr_base_s = s->pods_ready_backoff_base_s; X.pr_max_s = s->pods_ready_backoff_max_s;
     X.pr_limit = s->pods_ready_backoff_limit; X.pr_creation = s->pods_ready_requeue_creation;
+  }
+  std::vector<int32_t> exec_acc;  // MaximumExecutionTimeSeconds: the accumulated times at the start
+  if (mx) {
+    exec_acc.assign(Wz, -1);
+    if (s->wl_exec_acc_s) exec_acc.assign(s->wl_exec_acc_s, s->wl_exec_acc_s + W);
+    X.wl_max_exec = max_exec;
+    CUDA_TRY(h, h2d(h, max_exec, s->wl_max_exec_s, Wz * 4));
+    CUDA_TRY(h, h2d(h, X.wl_exec_acc, exec_acc.data(), Wz * 4));
+    if (s->n_adm) CUDA_TRY(h, h2d(h, X.adm_exec_since, s->adm_exec_since_ns, (size_t)s->n_adm * 8));
+    if (!requeue) CUDA_TRY(h, cudaMemsetAsync(X.wl_deactivated, 0, Wz, h->stream));  // (k_drain_init_checks clears it otherwise)
   }
   std::vector<i64> lq_adm;  // decay: the initial admitted usage of every LocalQueue (live rows of the snapshot)
   if (decay) {
@@ -1883,6 +1928,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     CUDA_TRY(h, cudaEventCreate(&ev_r[1]));
     CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_RESORT, 0, (pr ? 6 : 4) * 4, h->stream));  // once: the boundaries never clear them
   }
+  uint32_t exec_seen = 0;  // cumulative MaximumExecutionTimeExceeded deactivations at the previous boundary
+  if (mx) CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_EXEC_DEACTIVATED, 0, 2 * 4, h->stream));  // once, likewise
   // ---- one boundary per iteration, one synchronisation each (kueue_b200/drain.py): cycle c at t (in event mode, a
   // jump to the next event when there are no heads), its decisions and admissions, the evictions; in event mode E,
   // t_{c+1}, the decay samples, completions and arrivals; where rows can die (compact) the inadmissible requeue and the
@@ -1946,7 +1993,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (!jump) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_new, n_new_d, 4, cudaMemcpyDeviceToHost, h->stream));
     if (!compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_cells, X.e_cell_off + n_live, 4, cudaMemcpyDeviceToHost, h->stream));
     if (afs && (!jump || decay)) CUDA_TRY(h, cudaMemcpyAsync(&hw.status, D.status, 4, cudaMemcpyDeviceToHost, h->stream));
-    if (compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[1], X.counters + 1, (pr ? KB_DC_PR_DEACTIVATED : checks ? KB_DC_CHECK_REJECTED : events ? KB_DC_ARR_HI : KB_DC_FULL) * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[1], X.counters + 1, (mx ? KB_DC_EXEC_STATUS : pr ? KB_DC_PR_DEACTIVATED : checks ? KB_DC_CHECK_REJECTED : events ? KB_DC_ARR_HI : KB_DC_FULL) * 4, cudaMemcpyDeviceToHost, h->stream));
     if (events) CUDA_TRY(h, cudaMemcpyAsync(&hw.t_next, X.clock, 8, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     if (!jump) {
@@ -1971,6 +2018,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       if (checks && out->cycle_check_rejected) out->cycle_check_rejected[cyc] = 0;
       if (pr && out->cycle_pods_ready_timeout) out->cycle_pods_ready_timeout[cyc] = 0;
       if (pr && out->cycle_pods_ready_deactivated) out->cycle_pods_ready_deactivated[cyc] = 0;
+      if (mx && out->cycle_max_exec_deactivated) out->cycle_max_exec_deactivated[cyc] = 0;
       out->n_decisions += n_live; out->n_admitted += n_new; out->n_evicted += n_ev;
       out->n_cycles = ++cyc;
     } else {
@@ -2004,6 +2052,14 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
         if (out->cycle_pods_ready_deactivated) out->cycle_pods_ready_deactivated[cyc - 1] += de;
       }
     }
+    if (mx) {  // MaximumExecutionTimeExceeded deactivations of this boundary, and the overflow bit
+      if (hw.counters[KB_DC_EXEC_STATUS] & KBS_EXEC_OVERFLOW)
+        return fail(h, KB_ERR_UNSUPPORTED, "max exec: an accumulated execution time leaves int32");
+      const int de = (int)(hw.counters[KB_DC_EXEC_DEACTIVATED] - exec_seen);
+      exec_seen = hw.counters[KB_DC_EXEC_DEACTIVATED];
+      out->n_max_exec_deactivated += de;
+      if (cyc > 0 && out->cycle_max_exec_deactivated) out->cycle_max_exec_deactivated[cyc - 1] += de;
+    }
     if (lat) {  // evictions completed at this boundary (counter slot 4, inside the events copy)
       const int done = (int)hw.counters[KB_DC_EVICT_DONE];
       out->n_evict_done += done;
@@ -2012,10 +2068,11 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (compact) {  // the compacted half becomes the admitted tables of the next boundary
       A_cur = (int)hw.counters[KB_DC_ROWS]; AU_cur = (int)hw.counters[KB_DC_CELLS];
       AdmTabs cur{X.adm_cq, X.adm_priority, X.adm_ts, X.adm_qr_ts, X.adm_uid, X.adm_evicted, X.adm_use_start, X.adm_use_fr, X.adm_use_qty, X.adm_wl, X.adm_finish, X.adm_lq,
-                  X.adm_evicting, X.adm_phase};
+                  X.adm_evicting, X.adm_phase, X.adm_exec_since};
       X.adm_cq = other.cq; X.adm_priority = other.priority; X.adm_ts = other.ts; X.adm_qr_ts = other.qr_ts; X.adm_uid = other.uid;
       X.adm_evicted = other.evicted; X.adm_use_start = other.use_start; X.adm_use_fr = other.use_fr; X.adm_use_qty = other.use_qty; X.adm_wl = other.wl;
       X.adm_finish = other.finish; X.adm_lq = other.lq; X.adm_evicting = other.evicting; X.adm_phase = other.phase;
+      X.adm_exec_since = other.since;
       D.adm_cq = X.adm_cq; D.adm_priority = X.adm_priority; D.adm_ts = X.adm_ts; D.adm_qr_ts = X.adm_qr_ts; D.adm_uid = X.adm_uid;
       D.adm_evicted = X.adm_evicted; D.adm_use_start = X.adm_use_start; D.adm_use_fr = X.adm_use_fr; D.adm_use_qty = X.adm_use_qty;
       other = cur;
@@ -2072,7 +2129,10 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (out->wl_ready_ns) CUDA_TRY(h, cudaMemcpyAsync(out->wl_ready_ns, X.wl_ready_ns, Wz * 8, cudaMemcpyDeviceToHost, h->stream));
     if (out->wl_check_retries_out) CUDA_TRY(h, cudaMemcpyAsync(out->wl_check_retries_out, X.wl_retries, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
   }
-  if (requeue && out->wl_deactivated) CUDA_TRY(h, cudaMemcpyAsync(out->wl_deactivated, X.wl_deactivated, Wz, cudaMemcpyDeviceToHost, h->stream));
+  if ((requeue || mx) && out->wl_deactivated) CUDA_TRY(h, cudaMemcpyAsync(out->wl_deactivated, X.wl_deactivated, Wz, cudaMemcpyDeviceToHost, h->stream));
+  if ((requeue || mx) && out->wl_deactivation_reason)
+    CUDA_TRY(h, cudaMemcpyAsync(out->wl_deactivation_reason, X.wl_deactivated, Wz, cudaMemcpyDeviceToHost, h->stream));
+  if (mx && out->wl_exec_acc_s_out) CUDA_TRY(h, cudaMemcpyAsync(out->wl_exec_acc_s_out, X.wl_exec_acc, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
   if (pr) {
     if (out->wl_pods_ready_at_ns) CUDA_TRY(h, cudaMemcpyAsync(out->wl_pods_ready_at_ns, X.wl_pr_at, Wz * 8, cudaMemcpyDeviceToHost, h->stream));
     if (out->wl_pods_ready_count_out) CUDA_TRY(h, cudaMemcpyAsync(out->wl_pods_ready_count_out, X.wl_pr_count, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
@@ -2086,6 +2146,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     CUDA_TRY(h, cudaMemcpyAsync(out->trace_decision, X.trace_dec, nt, cudaMemcpyDeviceToHost, h->stream));
   }
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  if ((requeue || mx) && out->wl_deactivated)  // the device byte holds the reason (KB_DR_*)
+    for (int w = 0; w < W; w++) out->wl_deactivated[w] = out->wl_deactivated[w] != 0;
   return KB_OK;
 }
 

@@ -19,7 +19,8 @@ typedef unsigned long long u64;
 
 // Status word bits written by kernels (checked by the host after a cycle).
 enum { KBS_UNSUPPORTED_PREEMPTION = 1u << 0, KBS_TARGET_OVERFLOW = 1u << 1, KBS_PATH_TOO_DEEP = 1u << 2, KBS_INTERNAL_LOOP = 1u << 3,
-       KBS_AFS_OVERFLOW = 1u << 4 /* kb_run_drain: an AdmissionFairSharing quantity left int64 */ };
+       KBS_AFS_OVERFLOW = 1u << 4 /* kb_run_drain: an AdmissionFairSharing quantity left int64 */,
+       KBS_EXEC_OVERFLOW = 1u << 5 /* kb_run_drain: an accumulated execution time left int32 */ };
 
 // Static + per-cycle state of one (node, flavor-resource) cell, transposed per root (kb_search.cuh): everything the
 // column arithmetic of a target search reads besides the usage itself.  32 B, loaded as two 16 B words.

@@ -66,6 +66,14 @@
 // RequeueAt and the queue timestamp on the record, and the row is KB_PH_TIMED_OUT, released at once or, with latency, at
 // T + latency as an evicting row; its release sends the record to BACKOFF (k_drain_backoff queues it) or DEACTIVATED.
 // k_drain_evict drops a waiting attempt.
+//
+// MaximumExecutionTimeSeconds (kb_snapshot.wl_max_exec_s) adds one int64 row column, adm_exec_since (the Admitted time;
+// both halves, carried by the compaction), and the per-record limit and accumulated time.  drain_exec_clip puts the
+// effective deadline into the finish column where it comes before the row's own event (KB_PH_EXPIRE): in k_drain_admit
+// and on a Ready verdict, after drain_pr_attempt.  k_drain_finish applies an expiry after the timeouts: the record is
+// deactivated and the row becomes KB_PH_TIMED_OUT, whose release sends a deactivated record to DEACTIVATED.
+// drain_exec_release adds an attempt's seconds at every release of a row with an Admitted time (k_drain_finish, and
+// k_drain_evict without latency) and deactivates a record whose deadline passed before the release.
 #pragma once
 
 #include <cub/device/device_scan.cuh>
@@ -101,6 +109,21 @@ __host__ __device__ inline i64 kb_check_wait_ns(int k, i64 base_s, i64 max_s) {
 // without jitter, in nanoseconds (RequeueAt = T + it).  Restated by kueue_b200/drain.py pods_ready_wait_ns.
 __host__ __device__ inline i64 kb_pods_ready_wait_ns(int k, i64 base_s, i64 max_s) {
   return kb_backoff_wait(base_s * 1000000000ll, max_s * 1000000000ll, 2.0, k);
+}
+// Seconds of an Admitted span of d >= 0 ns as SyncAdmittedCondition adds them (admissionchecks.go:73-80):
+// int32(Duration.Seconds()) with Seconds() = float64(d / 1e9) + float64(d % 1e9) / 1e9, so from about 2^24 s the sum can
+// round up to the next second.  -1 when the value leaves int32 (Go's conversion is then undefined).  Restated by
+// kueue_b200/drain.py exec_seconds.
+__host__ __device__ inline i64 kb_exec_seconds(i64 d) {
+  const double x = (double)(d / 1000000000ll) + (double)(d % 1000000000ll) / 1e9;
+  return x >= 2147483648.0 ? -1 : (i64)x;
+}
+// the MaximumExecutionTimeSeconds deadline A + (max - acc) s of a row Admitted at A (acc -1 = nil, read as 0), saturating
+// both ways.  Restated by kueue_b200/drain.py exec_deadline.
+__host__ __device__ inline i64 kb_exec_deadline(i64 A, int32_t max_s, int32_t acc_s) {
+  const i64 left = ((i64)max_s - (acc_s < 0 ? 0 : acc_s)) * 1000000000ll;
+  if (left >= 0) return A > INT64_MAX - left ? INT64_MAX : A + left;
+  return A < INT64_MIN - left ? INT64_MIN : A + left;
 }
 
 // ---- resource.Quantity in the int64Amount form (value * 10^scale), as AdmissionFairSharing sums it -----------------
@@ -289,19 +312,28 @@ struct DrainDev {
   int32_t *wl_pr_fail, *wl_pr_count;  // [W] failures left (INT32_MAX = all) / RequeueState.Count
   i64 *wl_pr_at, *wl_pr_prev;      // [W] PodsReady time of the last attempt that reaches it / the value before it
   i64 pr_timeout, pr_base_s, pr_max_s; int pr_limit, pr_creation;
+  // MaximumExecutionTimeSeconds (event mode; adm_phase and wl_deactivated are allocated with it); wl_max_exec == nullptr:
+  // off.  wl_deactivated then holds the reason (KB_DR_*).
+  const int32_t *wl_max_exec;      // [W] limit in seconds, 0 = nil
+  int32_t *wl_exec_acc;            // [W] accumulated seconds, -1 = nil
+  i64 *adm_exec_since;             // [A_cap] Admitted time of each row (current half), INT64_MIN while its checks run
 };
 // adm_phase: what the finish column of a row holds.  RUN: its finish (or its eviction's end when adm_evicting); CHECK: its
-// checks' verdict; WAIT: the timeout T of a PodsReady attempt that fails; TIMED_OUT: the end of its eviction by that timeout
-enum { KB_PH_RUN = 0, KB_PH_CHECK = 1, KB_PH_WAIT = 2, KB_PH_TIMED_OUT = 3 };
+// checks' verdict; WAIT: the timeout T of a PodsReady attempt that fails; TIMED_OUT: the end of its eviction by that
+// timeout or by an expiry; EXPIRE: its effective MaximumExecutionTimeSeconds deadline, which comes before its own event
+enum { KB_PH_RUN = 0, KB_PH_CHECK = 1, KB_PH_WAIT = 2, KB_PH_TIMED_OUT = 3, KB_PH_EXPIRE = 4 };
+// wl_deactivated: 0, or the reason a record was deactivated (kb_drain_out.wl_deactivation_reason)
+enum { KB_DR_REJECTED = 1, KB_DR_REQUEUING_LIMIT = 2, KB_DR_MAX_EXEC = 3 };
 // counters of a boundary: [1] evictions (issued, with latency), [2] / [3] rows / cells after the compaction, [4]
 // evictions completed (latency), [5] capacity flag; event mode: [6] completions, [7] arrivals, [8] end flag, [9] / [10]
 // arrived prefix of arr_order [lo, hi); admission checks: [11] the stamp (cycle + 1) of the last boundary that needs a
 // re-sort, [12] / [13] / [14] Ready / Retry / Rejected verdicts since the start (the host takes differences: no memset);
-// WaitForPodsReady: [15] / [16] timeouts that requeue / deactivate since the start, likewise
+// WaitForPodsReady: [15] / [16] timeouts that requeue / deactivate since the start, likewise; MaximumExecutionTimeSeconds:
+// [17] deactivations since the start, [18] KBS_EXEC_OVERFLOW once an accumulated time leaves int32 (never cleared)
 enum { KB_DC_EVICTED = 1, KB_DC_ROWS = 2, KB_DC_CELLS = 3, KB_DC_EVICT_DONE = 4, KB_DC_FULL = 5,
        KB_DC_FINISHED = 6, KB_DC_ARRIVED = 7, KB_DC_END = 8, KB_DC_ARR_LO = 9, KB_DC_ARR_HI = 10,
        KB_DC_RESORT = 11, KB_DC_CHECK_READY = 12, KB_DC_CHECK_RETRY = 13, KB_DC_CHECK_REJECTED = 14,
-       KB_DC_PR_TIMEOUT = 15, KB_DC_PR_DEACTIVATED = 16 };
+       KB_DC_PR_TIMEOUT = 15, KB_DC_PR_DEACTIVATED = 16, KB_DC_EXEC_DEACTIVATED = 17, KB_DC_EXEC_STATUS = 18 };
 
 __device__ __forceinline__ int drain_seg0(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq] : cq; }
 __device__ __forceinline__ int drain_seg1(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq + 1] : cq + 1; }
@@ -506,6 +538,40 @@ __device__ __forceinline__ i64 drain_pr_attempt(const DrainDev &X, int a, int w,
   X.wl_pr_prev[w] = X.wl_pr_at[w]; X.wl_pr_at[w] = at;
   return run < 0 ? INT64_MAX : drain_sat_add(at, run);
 }
+// MaximumExecutionTimeSeconds: the deadline D = A + (max - acc) s of record w Admitted at A, saturating both ways
+__device__ __forceinline__ i64 drain_exec_deadline(const DrainDev &X, int w, i64 A) {
+  return kb_exec_deadline(A, X.wl_max_exec[w], X.wl_exec_acc[w]);
+}
+// row a (record w) Admitted at A with its own next event at fin: the effective deadline max(D, A) when it comes first,
+// with the row marked KB_PH_EXPIRE (a tie goes to the own event).  The host applies max(., now_ns) to the snapshot's rows.
+__device__ __forceinline__ i64 drain_exec_clip(const DrainDev &X, int a, int w, i64 A, i64 fin) {
+  if (X.wl_max_exec[w] <= 0) return fin;
+  const i64 dl = max(drain_exec_deadline(X, w, A), A);
+  if (dl >= fin) return fin;
+  X.adm_phase[a] = KB_PH_EXPIRE;
+  return dl;
+}
+// deactivation for MaximumExecutionTimeExceeded: acc nil, RequeueState cleared (Count 0; a BACKOFF-bound record is
+// DEACTIVATED at its release instead)
+__device__ __forceinline__ void drain_exec_deactivate(const DrainDev &X, int w) {
+  X.wl_deactivated[w] = KB_DR_MAX_EXEC;
+  X.wl_exec_acc[w] = -1;
+  if (X.wl_pr) X.wl_pr_count[w] = 0;
+  atomicAdd(&X.counters[KB_DC_EXEC_DEACTIVATED], 1);
+}
+// release at t of row a (record w): with an Admitted time, a deadline at or before t deactivates a record not
+// deactivated yet (rule 4), then the attempt's seconds join acc.  Returns whether it deactivated the record.
+__device__ __forceinline__ bool drain_exec_release(const DrainDev &X, int a, int w, i64 t) {
+  const i64 A = X.adm_exec_since[a];
+  if (A == INT64_MIN) return false;
+  const bool deact = X.wl_max_exec[w] > 0 && X.wl_deactivated[w] == 0 && drain_exec_deadline(X, w, A) <= t;
+  if (deact) drain_exec_deactivate(X, w);
+  const i64 d = kb_exec_seconds(t - A), acc = X.wl_exec_acc[w];
+  const i64 sum = acc < 0 ? d : acc + d;
+  if (d < 0 || sum > INT32_MAX) atomicOr((unsigned *)&X.counters[KB_DC_EXEC_STATUS], KBS_EXEC_OVERFLOW);
+  else X.wl_exec_acc[w] = (int32_t)sum;
+  return deact;
+}
 
 // admitted entries join the admitted tables (cache.AssumeWorkload), appended at X.A / X.AU, and the ClusterQueue usage
 __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
@@ -534,6 +600,12 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
         X.wl_ready_ns[wl] = qr_ts;
         if (X.wl_pr) fin = drain_pr_attempt(X, a, wl, qr_ts);  // Admitted now: the PodsReady attempt starts
       }
+    }
+    if (X.wl_max_exec) {  // Admitted now unless the checks run: the deadline may come first
+      const bool checking = X.wl_check && X.wl_check[wl] > 0;
+      if (!X.wl_qts) X.adm_phase[a] = KB_PH_RUN;
+      X.adm_exec_since[a] = checking ? INT64_MIN : qr_ts;
+      if (!checking) fin = drain_exec_clip(X, a, wl, qr_ts, fin);
     }
     X.adm_finish[a] = fin;
     X.wl_admit_ns[wl] = qr_ts;
@@ -643,7 +715,8 @@ __global__ void k_drain_evict(DevSnap D, DrainDev X) {
     for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)  // cache.DeleteWorkload
       atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
     const int w = X.adm_wl[a];
-    drain_release(D, X, w);
+    if (X.wl_max_exec && drain_exec_release(X, a, w, D.now_ns)) { drain_forget(D, X, w); X.wl_state[w] = KB_WS_DEACTIVATED; }
+    else drain_release(D, X, w);
     if (X.wl_pr && X.wl_pr_at[w] > D.now_ns) X.wl_pr_at[w] = X.wl_pr_prev[w];  // dropped before PodsReady
     X.wl_evictions[w]++;  // a workload holds at most one row: one writer
     X.root_mark[D.root_slot[cq]] = stamp;
@@ -672,7 +745,7 @@ __global__ void k_drain_live(DrainDev X, int bound, const int32_t *n_new) {
   X.row_live[a] = live;
   X.row_cells[a] = live ? X.adm_use_start[a + 1] - X.adm_use_start[a] : 0;
 }
-struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; i64 *finish; int32_t *lq; uint8_t *evicting, *phase; };
+struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; i64 *finish; int32_t *lq; uint8_t *evicting, *phase; i64 *since; };
 // live rows of [0, bound), in order, into the other half of the double buffer; thread bound writes the totals
 __global__ void k_drain_compact(DrainDev X, AdmTabs O, int bound) {
   int a = blockIdx.x * blockDim.x + threadIdx.x;
@@ -686,6 +759,7 @@ __global__ void k_drain_compact(DrainDev X, AdmTabs O, int bound) {
   if (X.adm_lq) O.lq[n] = X.adm_lq[a];
   if (X.adm_evicting) O.evicting[n] = X.adm_evicting[a];
   if (X.adm_phase) O.phase[n] = X.adm_phase[a];
+  if (X.adm_exec_since) O.since[n] = X.adm_exec_since[a];
   for (int c = 0; c < nc; c++) { O.use_fr[c0 + c] = X.adm_use_fr[u0 + c]; O.use_qty[c0 + c] = X.adm_use_qty[u0 + c]; }
 }
 
@@ -751,8 +825,9 @@ __global__ void k_drain_ev_next(DrainDev X, i64 t_c, i64 step, int jump, const i
 // completions (thread per row): a live row with finish <= t_{c+1} gets the dead stamp, its cells leave its ClusterQueue's
 // usage (cache.DeleteWorkload, integer atomics), its record becomes FINISHED and its root tree is marked.  An evicting
 // row's finish column holds its end time: it completes the eviction instead, its record returns to its queue.  Rows in
-// [A + *n_new, bound) only pad the compaction's range.  Verdicts (admission checks) and PodsReady timeouts come first; a
-// timed-out row releases its record to BACKOFF or DEACTIVATED, and counts as neither a completion nor an eviction.
+// [A + *n_new, bound) only pad the compaction's range.  Verdicts (admission checks), PodsReady timeouts and
+// MaximumExecutionTimeSeconds expiries come first; a timed-out or expired row releases its record to BACKOFF or
+// DEACTIVATED, and counts as neither a completion nor an eviction.
 __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *n_new) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x;
   if (a >= bound || a >= X.A + (n_new ? *n_new : 0) || X.counters[KB_DC_FULL]) return;
@@ -766,8 +841,9 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
     X.adm_phase[a] = KB_PH_RUN;
     if (X.wl_fail[w] == 0) {  // Ready: Admitted, the run clock (or the PodsReady attempt) starts; it may end in this boundary
       const i64 run = X.wl_run ? X.wl_run[w] : -1;
-      const i64 fin = X.wl_pr ? drain_pr_attempt(X, a, w, tv) : run < 0 ? INT64_MAX : (tv > INT64_MAX - run ? INT64_MAX : tv + run);
+      i64 fin = X.wl_pr ? drain_pr_attempt(X, a, w, tv) : run < 0 ? INT64_MAX : (tv > INT64_MAX - run ? INT64_MAX : tv + run);
       X.wl_ready_ns[w] = tv;
+      if (X.wl_max_exec) { X.adm_exec_since[a] = tv; fin = drain_exec_clip(X, a, w, tv, fin); }
       X.adm_finish[a] = fin;
       atomicAdd(&X.counters[KB_DC_CHECK_READY], 1);
       if (fin > X.clock[0]) return;
@@ -788,7 +864,7 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
         atomicAdd(&X.counters[KB_DC_CHECK_RETRY], 1);
       } else {  // Rejected: deactivated
         X.wl_state[w] = KB_WS_DEACTIVATED;
-        X.wl_deactivated[w] = 1;
+        X.wl_deactivated[w] = KB_DR_REJECTED;
         atomicAdd(&X.counters[KB_DC_CHECK_REJECTED], 1);
       }
       X.root_mark[D.root_slot[cq]] = stamp;
@@ -802,7 +878,7 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
     const int n = X.wl_pr_count[w];
     if (X.pr_limit >= 0 && n >= X.pr_limit) {  // Count + 1 > limit: deactivated, RequeueState cleared
       X.wl_pr_count[w] = 0;
-      X.wl_deactivated[w] = 1;
+      X.wl_deactivated[w] = KB_DR_REQUEUING_LIMIT;
       atomicAdd(&X.counters[KB_DC_PR_DEACTIVATED], 1);
     } else {  // BACKOFF at release: RequeueAt = T + WaitTime(Count); under Eviction the queue timestamp is T
       const int k = n == INT32_MAX ? n : n + 1;
@@ -820,12 +896,26 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
       if (X.adm_finish[a] > X.clock[0]) return;
     }
   }
+  if (ph == KB_PH_EXPIRE) {  // MaximumExecutionTimeExceeded at the effective deadline (workload_controller.go:619-646)
+    const i64 dl = X.adm_finish[a];
+    drain_exec_deactivate(X, w);
+    if (X.wl_pr && X.wl_pr_at[w] > dl) X.wl_pr_at[w] = X.wl_pr_prev[w];  // a PodsReady attempt still waiting is dropped
+    ph = KB_PH_TIMED_OUT;
+    X.adm_phase[a] = ph;
+    if (X.wl_evict) {  // evicted at the deadline: the row holds its cells until deadline + latency, as an evicting row
+      X.adm_evicted[a] = 1;
+      X.adm_evicting[a] = 1;
+      X.adm_finish[a] = drain_sat_add(dl, X.wl_evict[w]);
+      if (X.adm_finish[a] > X.clock[0]) return;
+    }
+  }
   X.adm_dead[a] = stamp;
   for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)
     atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
   const bool timed_out = ph == KB_PH_TIMED_OUT;
   const bool released = X.adm_evicting && X.adm_evicting[a];
-  if (timed_out) { drain_forget(D, X, w); X.wl_state[w] = X.wl_deactivated[w] ? KB_WS_DEACTIVATED : KB_WS_BACKOFF; }
+  const bool expired = X.wl_max_exec && (timed_out || released) && drain_exec_release(X, a, w, X.adm_finish[a]);
+  if (timed_out || expired) { drain_forget(D, X, w); X.wl_state[w] = X.wl_deactivated[w] ? KB_WS_DEACTIVATED : KB_WS_BACKOFF; }
   else if (released) drain_release(D, X, w);
   else if (w >= 0) { X.wl_state[w] = KB_WS_FINISHED; X.wl_admit_cycle[w] = -1; X.wl_finish_ns[w] = X.adm_finish[a]; }
   if (X.lq_last && X.adm_lq[a] >= 0 && X.cq_afs[cq]) {  // several rows of one LocalQueue can finish together

@@ -225,6 +225,37 @@ WaitTime(k) is `pods_ready_wait_ns`: wait.NewBackoff(base, max, 2, 0.0001).WaitT
 (the reference's RequeueAt carries a jitter below wait * 1e-4 at second precision).  Timeouts applied between the start of
 cycle c and of c+1 are cycle c's (`pods_ready_timeout`, `pods_ready_deactivated`).  blockAdmission and recoveryTimeout
 are not modelled.
+
+MaximumExecutionTimeSeconds (event mode, the snapshot carries `wl_max_exec_s` and `adm_wl`, include/kueue_b200.h).  A
+workload that has spent spec.maximumExecutionTimeSeconds (`max`, 0 = nil) in the Admitted state, summed over its
+admissions in status.accumulatedPastExecutionTimeSeconds (`acc`, -1 = nil, read as 0), is deactivated with reason
+MaximumExecutionTimeExceeded and never requeued (workload_types.go:71-77,658-662):
+  1. every row has an Admitted time A (`exec_since`): the reservation t_c without a check delay, else the Ready verdict
+     time; a row whose checks run has none (SyncAdmittedCondition admissionchecks.go:36-70).  A row of a record with a
+     limit has the deadline D = A + (max - acc) * 1e9 (saturating, `exec_deadline`) and the effective deadline
+     max(D, A, now_ns) (reconcileMaxExecutionTime workload_controller.go:619-646: remaining = (max - acc) s - (now - A),
+     acting on remaining <= 0), so a negative max - acc or a snapshot row past its limit expires at the first boundary;
+  2. the finish column holds the earlier of the row's own next event (its finish, or T of a failing PodsReady attempt)
+     and the effective deadline; a row whose deadline came first is EXPIRE.  A tie goes to the own event (a finish at
+     the deadline finishes, a PodsReady timeout at the deadline is a timeout).  `apply_expiries` runs in step 5 after the
+     verdicts and the timeouts, before the completions;
+  3. at expiry (`exec_deactivate`): reason MaximumExecutionTimeExceeded (SetDeactivationTarget; the inactive branch
+     :316-321,386-420 evicts and clears RequeueState: Count 0, no RequeueAt), acc = nil.  A PodsReady attempt still
+     waiting is dropped (not counted, no failure used, wl_pods_ready_at back to its previous value).  The row is evicted at
+     the effective deadline: an evicting row until deadline + latency with wl_evict_ns (a preemptor that targets it is
+     ongoing), else released by the boundary that applies it.  At release the record is DEACTIVATED;
+  4. every release of a row with an Admitted time (a completed preemption, a PodsReady-timeout release, an expiry
+     release; `exec_release`) adds d = `exec_seconds`(t - A) to acc, or sets acc = d when nil (UnsetQuotaReservation
+     workload.go:684-704 turns Admitted false at the release, so termination latency counts).  t is the eviction's end,
+     T or the effective deadline without latency, t_c for a preemption without latency.  Completions and rows whose
+     checks run add nothing.  A release at or after the row's D of a record not deactivated yet (RequeuingLimitExceeded
+     sets DeactivationTarget first, :840-851) applies rule 3 there instead of the requeue or the backoff (both reconcilers
+     run while the reservation is held, :509-536): acc ends as d of that attempt, and it counts at that boundary;
+  5. condition times keep nanoseconds; with every limit nil and no start state the drain equals the drain without the
+     block except for `wl_exec_acc_s`.
+`exec_seconds` is int32(Duration.Seconds()): float64(sec) + float64(nsec) / 1e9, truncated per attempt; from about 2^24 s
+the float sum can round up to sec + 1.  A value or a sum outside int32 raises ExecOverflow (kb_run_drain:
+KB_ERR_UNSUPPORTED).  Deactivations between the start of cycle c and of c+1 are cycle c's (`max_exec_deactivated`).
 """
 from __future__ import annotations
 
@@ -278,7 +309,7 @@ class DrainResult:
     n_check_rejected: int = 0
     wl_ready_ns: np.ndarray | None = None                      # [n_wl] time of the last Admitted, INT64_MIN = none
     wl_check_retries: np.ndarray | None = None                 # [n_wl] final RetryCount
-    wl_deactivated: np.ndarray | None = None                   # [n_wl] 1 = Rejected
+    wl_deactivated: np.ndarray | None = None                   # [n_wl] 1 = deactivated (Rejected, or the blocks below)
     wl_queue_ts: np.ndarray | None = None                      # [n_wl] final queue-order timestamps
     n_resorts: int = 0
     resort_orders: List[dict] = field(default_factory=list)    # the rebuilt queue state after every re-sort
@@ -291,6 +322,13 @@ class DrainResult:
     n_pods_ready_deactivated: int = 0
     wl_pods_ready_at: np.ndarray | None = None                 # [n_wl] last PodsReady time, INT64_MIN = none
     wl_pods_ready_count: np.ndarray | None = None              # [n_wl] final RequeueState.Count
+    # MaximumExecutionTimeSeconds (wl_max_exec_s in the snapshot; None / empty / 0 otherwise); wl_deactivated also marks
+    # its deactivations
+    max_exec_deactivated: List[np.ndarray] = field(default_factory=list)  # per cycle: records deactivated
+    n_max_exec_deactivated: int = 0                            # those before cycle 0 included
+    wl_exec_acc_s: np.ndarray | None = None                    # [n_wl] final accumulated seconds, -1 = nil
+    exec_spans: List[tuple] = field(default_factory=list)      # (record, Admitted time, release time, seconds added)
+    wl_deactivation_reason: np.ndarray | None = None           # [n_wl] 0 none, 1 Rejected, 2 RequeuingLimitExceeded, 3 this
 
     @property
     def n_evicted(self) -> int:
@@ -344,7 +382,12 @@ QUEUED, SET_ASIDE, HELD, ABSENT, FINISHED, BACKOFF, DEACTIVATED = 0, 1, 2, 3, 4,
 NEVER = np.iinfo(np.int64).max  # an event time that never comes
 UNSET = np.iinfo(np.int64).min
 ALL_FAIL = np.iinfo(np.int32).max  # wl_check_fail / wl_pods_ready_fail: every attempt fails
-RUN, WAIT, TIMED_OUT = 0, 2, 3  # PodsReady phase of a row (kb_drain.cuh KB_PH_*): its finish column holds the finish, T, the end
+# phase of a row (kb_drain.cuh KB_PH_*): its finish column holds the finish, T of a PodsReady attempt, the end of an
+# eviction by a timeout or an expiry, the effective MaximumExecutionTimeSeconds deadline
+RUN, WAIT, TIMED_OUT, EXPIRE = 0, 2, 3, 4
+REJECTED, REQUEUING_LIMIT, MAX_EXEC = 1, 2, 3  # deactivation reasons (kb_drain_out.wl_deactivation_reason)
+_S = 1_000_000_000
+_I32_MAX = 2**31 - 1
 MAX_BACKOFF_S = 10_000  # below it the reference's jittered, truncated WaitTime is exact
 
 
@@ -380,6 +423,26 @@ def pods_ready_wait_ns(k: int, base_s: int, max_s: int) -> int:
     """WaitTime of PodsReady requeue k: wait.NewBackoff(base, max, 2, 0.0001).WaitTime(k) without jitter, in
     nanoseconds (kb_drain.cuh kb_pods_ready_wait_ns)"""
     return wait_time(int(base_s) * 1_000_000_000, int(max_s) * 1_000_000_000, 2.0, int(k))
+
+
+class ExecOverflow(ValueError):
+    """An attempt's seconds or the accumulated time leaves int32 (kb_run_drain: KB_ERR_UNSUPPORTED)."""
+
+
+def exec_seconds(d_ns: int) -> int:
+    """int32(time.Duration(d_ns).Seconds()) for d_ns >= 0 (SyncAdmittedCondition admissionchecks.go:73-80; kb_drain.cuh
+    kb_exec_seconds): float64(sec) + float64(nsec) / 1e9, truncated.  ExecOverflow when it leaves int32."""
+    sec, nsec = divmod(int(d_ns), _S)
+    x = float(sec) + float(nsec) / 1e9
+    if x >= 2.0**31:
+        raise ExecOverflow(d_ns)
+    return int(x)
+
+
+def exec_deadline(admitted_ns: int, max_s: int, acc_s: int) -> int:
+    """the MaximumExecutionTimeSeconds deadline A + (max - acc) s (acc -1 = nil, read as 0), saturating both ways
+    (kb_drain.cuh kb_exec_deadline)"""
+    return max(min(int(admitted_ns) + (int(max_s) - max(int(acc_s), 0)) * _S, NEVER), UNSET)
 
 
 def check_wait_bound_s(base_s: int, max_s: int, limit: int) -> int:
@@ -617,6 +680,9 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     checks = "wl_check_ns" in a
     pr = "wl_pods_ready_ns" in a                                  # WaitForPodsReady
     backoff = checks or pr                                        # BACKOFF / DEACTIVATED, RequeueAt, mutable qts
+    mx = "wl_max_exec_s" in a                                     # MaximumExecutionTimeSeconds
+    if mx and "adm_wl" not in a:
+        raise ValueError("wl_max_exec_s needs adm_wl")
     qts = a["wl_ts"].astype(np.int64).copy()                      # queue-order timestamps (checks, PodsReady: mutable)
     if backoff:
         if "adm_wl" not in a:
@@ -667,7 +733,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             ra = a["wl_requeue_at_ns"].astype(np.int64)
             state[ra > snap.now_ns] = BACKOFF
             requeue_at[ra > snap.now_ns] = ra[ra > snap.now_ns]
-        deactivated = np.zeros(snap.n_wl, np.uint8)
+    if backoff or mx:
+        deactivated = np.zeros(snap.n_wl, np.uint8)               # 0, or the reason (REJECTED, REQUEUING_LIMIT, MAX_EXEC)
     if checks:  # rule 1: attempt state; start state of the rows whose checks run
         chk_ns = a["wl_check_ns"].astype(np.int64)
         chk_fail = a["wl_check_fail"].astype(np.int64).copy() if "wl_check_fail" in a else np.zeros(snap.n_wl, np.int64)
@@ -682,7 +749,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         verdicts = {"ready": 0, "retry": [], "rejected": []}
     else:
         checking = None
-    pr_phase = None                                               # [rows] PodsReady phase (RUN / WAIT / TIMED_OUT)
+    phase = None                                                  # [rows] RUN / WAIT / TIMED_OUT / EXPIRE
     if pr:  # rules 2 and 7: attempt state, and the rows whose pods are not ready at the start
         pr_ns = a["wl_pods_ready_ns"].astype(np.int64)
         pr_fail = a["wl_pods_ready_fail"].astype(np.int64).copy() if "wl_pods_ready_fail" in a else np.zeros(snap.n_wl, np.int64)
@@ -702,10 +769,32 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             pr_prev[w] = pr_at[w]
             pr_at[w] = min(t0 + d, NEVER)
             return (finish_time(int(pr_at[w]), int(run_ns[w])) if run_ns is not None else NEVER), RUN
-        pr_phase = np.full(snap.n_adm, RUN, np.int64)
+        phase = np.full(snap.n_adm, RUN, np.int64)
         if "adm_admitted_ns" in a:
             for row in np.flatnonzero(a["adm_admitted_ns"] != UNSET):
-                adm_finish[row], pr_phase[row] = pr_attempt(int(adm_wl[row]), int(a["adm_admitted_ns"][row]))
+                adm_finish[row], phase[row] = pr_attempt(int(adm_wl[row]), int(a["adm_admitted_ns"][row]))
+    if mx:  # rule 1: limits, accumulated times, the Admitted time of every row; the start rows' effective deadlines
+        exec_max = a["wl_max_exec_s"].astype(np.int64)
+        acc = a["wl_exec_acc_s"].astype(np.int64).copy() if "wl_exec_acc_s" in a else np.full(snap.n_wl, -1, np.int64)
+        if snap.n_adm and "adm_exec_since_ns" not in a:
+            raise ValueError("wl_max_exec_s needs adm_exec_since_ns when the snapshot has admitted rows")
+        exec_since = a["adm_exec_since_ns"].astype(np.int64).copy() if snap.n_adm else np.zeros(0, np.int64)
+        exec_events = []                                          # records deactivated since the last boundary
+
+        def exec_clip(w, A, fin, floor=UNSET):
+            """rule 2: (finish column, expires first) of a row of record w Admitted at A whose own next event is fin"""
+            if exec_max[w] <= 0:
+                return fin, False
+            dl = max(exec_deadline(A, int(exec_max[w]), int(acc[w])), A, floor)
+            return (dl, True) if dl < fin else (fin, False)
+        if phase is None:
+            phase = np.full(snap.n_adm, RUN, np.int64)
+        for row in range(snap.n_adm):
+            if exec_since[row] == UNSET or (evicting is not None and evicting[row]):
+                continue
+            adm_finish[row], e = exec_clip(int(adm_wl[row]), int(exec_since[row]), int(adm_finish[row]), int(snap.now_ns))
+            if e:
+                phase[row] = EXPIRE
     sticky = a["cq_sticky"].astype(np.int64).copy() if "cq_sticky" in a else None  # sticky workload per ClusterQueue
     cursor = np.zeros(len(qlen), np.int64)
     first_aside = qlen.copy()                                     # smallest SET_ASIDE position per segment (qlen = none)
@@ -812,7 +901,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
 
     def remove_rows(rows):
         """rows leave the admitted tables (cache.DeleteWorkload: cells out of the usage; the other rows keep their order)"""
-        nonlocal adm_wl, adm_finish, adm_lq, evicting, checking, pr_phase
+        nonlocal adm_wl, adm_finish, adm_lq, evicting, checking, phase, exec_since
         us, uf, uq = adm["adm_use_start"], adm["adm_use_fr"], adm["adm_use_qty"]
         for row in rows:
             cqi = int(adm["adm_cq"][row])
@@ -836,8 +925,45 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             evicting = evicting[keep]
         if checking is not None:
             checking = checking[keep]
-        if pr_phase is not None:
-            pr_phase = pr_phase[keep]
+        if phase is not None:
+            phase = phase[keep]
+        if mx:
+            exec_since = exec_since[keep]
+
+    def forget(w):
+        """a released record: LastAssignment nil, no reservation"""
+        last_gen[w] = -1
+        last_tried[int(ps_start[w]):int(ps_start[w + 1])] = -1
+        if has_qr is not None:
+            has_qr[w] = 0
+        admit_cycle[w] = -1
+
+    def exec_deactivate(w):
+        """rule 3 of MaximumExecutionTimeSeconds: deactivated, acc nil, RequeueState cleared"""
+        deactivated[w] = MAX_EXEC
+        acc[w] = -1
+        if pr:
+            pr_count[w] = 0
+        if backoff:
+            requeue_at[w] = UNSET
+        exec_events.append(int(w))
+
+    def exec_release(row, w, t_rel):
+        """rule 4: the release at t_rel of a row with an Admitted time adds its seconds to acc, after deactivating a
+        record whose deadline has passed; returns whether it deactivated the record"""
+        A = int(exec_since[row])
+        if A == UNSET:
+            return False
+        deact = exec_max[w] > 0 and deactivated[w] == 0 and exec_deadline(A, int(exec_max[w]), int(acc[w])) <= t_rel
+        if deact:
+            exec_deactivate(w)
+        d = exec_seconds(t_rel - A)
+        total = d if acc[w] < 0 else int(acc[w]) + d
+        if total > _I32_MAX:
+            raise ExecOverflow(total)
+        acc[w] = total
+        res.exec_spans.append((int(w), A, int(t_rel), d))
+        return deact
 
     def release(w):
         """the record of an evicted row returns to its queue with LastAssignment nil (workload_controller.go:973-1004);
@@ -877,9 +1003,14 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             if chk_fail[w] == 0:  # Ready: Admitted, the run clock (or the PodsReady attempt) starts
                 ready_ns[w] = tv
                 if pr:
-                    adm_finish[row], pr_phase[row] = pr_attempt(w, tv)
+                    adm_finish[row], phase[row] = pr_attempt(w, tv)
                 else:
                     adm_finish[row] = finish_time(tv, int(run_ns[w])) if run_ns is not None else NEVER
+                if mx:  # rule 1 of MaximumExecutionTimeSeconds: Admitted now
+                    exec_since[row] = tv
+                    adm_finish[row], e = exec_clip(w, tv, int(adm_finish[row]))
+                    if e:
+                        phase[row] = EXPIRE
                 verdicts["ready"] += 1
                 continue
             if chk_fail[w] != ALL_FAIL:
@@ -900,7 +1031,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 verdicts["retry"].append(w)
             else:  # Rejected: deactivated
                 state[w] = DEACTIVATED
-                deactivated[w] = 1
+                deactivated[w] = REJECTED
                 verdicts["rejected"].append(w)
         if gone:
             remove_rows(gone)
@@ -927,13 +1058,13 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
 
     def apply_timeouts(t_next):
         """rules 3-4 of WaitForPodsReady: the timeouts due by t_next, after the verdicts and before the completions"""
-        for row in np.flatnonzero((pr_phase == WAIT) & (adm_finish <= t_next)):
+        for row in np.flatnonzero((phase == WAIT) & (adm_finish <= t_next)):
             w, T = int(adm_wl[row]), int(adm_finish[row])
             if 0 < pr_fail[w] != ALL_FAIL:
                 pr_fail[w] -= 1
             if pr_limit >= 0 and pr_count[w] + 1 > pr_limit:  # RequeuingLimitExceeded: deactivated, RequeueState cleared
                 pr_count[w] = 0
-                deactivated[w] = 1
+                deactivated[w] = REQUEUING_LIMIT
                 timeouts["deactivated"].append(w)
             else:
                 pr_count[w] = min(int(pr_count[w]) + 1, ALL_FAIL)
@@ -942,11 +1073,24 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                     qts[w] = T
                 timeouts["timeout"].append(w)
                 timeouts["at"].append((T, int(requeue_at[w])))
-            pr_phase[row] = TIMED_OUT
+            phase[row] = TIMED_OUT
             if lat is not None:  # the pods terminate: an evicting row until T + latency
                 evicting[row] = True
                 adm["adm_evicted"][row] = 1
                 adm_finish[row] = min(T + int(lat[w]), NEVER)
+
+    def apply_expiries(t_next):
+        """rules 2-3 of MaximumExecutionTimeSeconds: the expiries due by t_next, after the timeouts, before the completions"""
+        for row in np.flatnonzero((phase == EXPIRE) & (adm_finish <= t_next)):
+            w, dl = int(adm_wl[row]), int(adm_finish[row])
+            exec_deactivate(w)
+            if pr and pr_at[w] > dl:  # a PodsReady attempt still waiting is dropped
+                pr_at[w] = pr_prev[w]
+            phase[row] = TIMED_OUT
+            if lat is not None:  # evicted at the deadline: an evicting row until deadline + latency
+                evicting[row] = True
+                adm["adm_evicted"][row] = 1
+                adm_finish[row] = min(dl + int(lat[w]), NEVER)
 
     def apply_events(t_next, notified):
         """steps 5 and 6 at t_next; returns (finished records, arrived records, records whose eviction completed)"""
@@ -955,9 +1099,11 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             apply_verdicts(t_next, notified)
         if pr:
             apply_timeouts(t_next)
+        if mx:
+            apply_expiries(t_next)
         done = np.flatnonzero(adm_finish <= t_next)
         gone = evicting[done] if evicting is not None else np.zeros(len(done), bool)
-        to = pr_phase[done] == TIMED_OUT if pr else np.zeros(len(done), bool)
+        to = phase[done] == TIMED_OUT if phase is not None else np.zeros(len(done), bool)
         fin, released = adm_wl[done[~gone & ~to]].copy(), adm_wl[done[gone & ~to]].copy()
         for row in done:
             notified.add(int(adm["adm_cq"][row]))
@@ -965,14 +1111,13 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 for k in range(int(adm["adm_use_start"][row]), int(adm["adm_use_start"][row + 1])):
                     ladm[adm_lq[row], int(adm["adm_use_fr"][k]) % R] -= int(adm["adm_use_qty"][k])
             w = int(adm_wl[row])
-            if pr and pr_phase[row] == TIMED_OUT:  # rule 4: the record waits for RequeueAt, or is deactivated
+            timed_out = phase is not None and phase[row] == TIMED_OUT
+            rel = evicting is not None and evicting[row]
+            expired = mx and (timed_out or rel) and exec_release(row, w, int(adm_finish[row]))  # rule 4 (max exec)
+            if timed_out or expired:  # rule 4 (PodsReady): the record waits for RequeueAt, or is deactivated
                 state[w] = DEACTIVATED if deactivated[w] else BACKOFF
-                last_gen[w] = -1
-                last_tried[int(ps_start[w]):int(ps_start[w + 1])] = -1
-                if has_qr is not None:
-                    has_qr[w] = 0
-                admit_cycle[w] = -1
-            elif evicting is not None and evicting[row]:
+                forget(w)
+            elif rel:
                 release(w)
             elif w >= 0:
                 state[w] = FINISHED
@@ -1028,6 +1173,12 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                                                                 np.asarray(timeouts["at"], np.int64).reshape(-1, 2)])
                 res.pods_ready_deactivated[-1] = np.concatenate([res.pods_ready_deactivated[-1], de])
             timeouts.update(timeout=[], at=[], deactivated=[])
+        if mx:
+            de = np.asarray(exec_events, np.int64)
+            res.n_max_exec_deactivated += len(de)
+            if res.cycles:
+                res.max_exec_deactivated[-1] = np.concatenate([res.max_exec_deactivated[-1], de])
+            exec_events.clear()
 
     t = int(snap.now_ns)
     cyc = 0
@@ -1093,6 +1244,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         res.check_retry.append(np.zeros(0, np.int64)); res.check_rejected.append(np.zeros(0, np.int64))
         res.pods_ready_timeout.append(np.zeros(0, np.int64)); res.pods_ready_deactivated.append(np.zeros(0, np.int64))
         res.pods_ready_timeout_at.append(np.zeros((0, 2), np.int64))
+        res.max_exec_deactivated.append(np.zeros(0, np.int64))
         ok = dec == abi.DEC_ASSUMED
         res.admitted.append(heads[ok])
         # ---- apply the admissions: Assignment.Usage (flavorassigner.go:198-218) with the admitted counts
@@ -1165,12 +1317,22 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 fin_new = [finish_time(t, int(run_ns[w])) if run_ns is not None else NEVER for w in g]
                 if checks:
                     fin_new = [min(t + int(chk_ns[w]), NEVER) if chk_ns[w] > 0 else f for w, f in zip(g, fin_new)]
-                if pr:  # rule 1: Admitted now unless the checks run
+                if phase is not None:  # rule 1 (PodsReady, max exec): Admitted now unless the checks run
                     ph_new = np.full(n_new, RUN, np.int64)
+                    since_new = np.full(n_new, UNSET, np.int64)
                     for i, w in enumerate(g):
-                        if not (checks and chk_ns[w] > 0):
+                        if checks and chk_ns[w] > 0:
+                            continue
+                        if pr:
                             fin_new[i], ph_new[i] = pr_attempt(int(w), t)
-                    pr_phase = np.concatenate([pr_phase, ph_new])
+                        if mx:
+                            since_new[i] = t
+                            fin_new[i], e = exec_clip(int(w), t, int(fin_new[i]))
+                            if e:
+                                ph_new[i] = EXPIRE
+                    phase = np.concatenate([phase, ph_new])
+                    if mx:
+                        exec_since = np.concatenate([exec_since, since_new])
                 adm_finish = np.concatenate([adm_finish, np.asarray(fin_new, np.int64)])
             if evicting is not None:
                 evicting = np.concatenate([evicting, np.zeros(n_new, bool)])
@@ -1234,15 +1396,19 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 if checking is not None and checking[row]:  # rule 5: no pods, released at the next boundary
                     checking[row] = False
                     adm_finish[row] = t
-                if pr:  # rule 5 of PodsReady: a waiting attempt is dropped
-                    pr_phase[row] = RUN
-                    if pr_at[w] > t:
-                        pr_at[w] = pr_prev[w]
+                if phase is not None:  # an ordinary evicting row (rule 5 of PodsReady: a waiting attempt is dropped)
+                    phase[row] = RUN
+                if pr and pr_at[w] > t:
+                    pr_at[w] = pr_prev[w]
                 evictions[w] += 1
         elif victims:
             for row in victims:
                 w = int(adm_wl[row])
-                release(w)
+                if mx and exec_release(row, w, t):  # rule 4 of max exec: past its deadline, deactivated
+                    state[w] = DEACTIVATED
+                    forget(w)
+                else:
+                    release(w)
                 if pr and pr_at[w] > t:  # rule 5 of PodsReady: dropped before PodsReady
                     pr_at[w] = pr_prev[w]
                 evictions[w] += 1
@@ -1285,13 +1451,18 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     res.end_ns = t
     res.cq_sticky = sticky
     if backoff:
-        res.wl_deactivated, res.wl_queue_ts = deactivated, qts
+        res.wl_queue_ts = qts
+    if backoff or mx:
+        res.wl_deactivated, res.wl_deactivation_reason = (deactivated != 0).astype(np.uint8), deactivated
+    if mx:
+        res.wl_exec_acc_s = acc
+        res.adm["adm_exec_since_ns"] = exec_since
     if checks:
         res.wl_ready_ns, res.wl_check_retries = ready_ns, retries
         res.adm["adm_checking"] = checking
     if pr:
         res.wl_pods_ready_at, res.wl_pods_ready_count = pr_at, pr_count
-        res.adm["adm_pods_ready_phase"] = pr_phase
+        res.adm["adm_pods_ready_phase"] = phase
     if decay:
         res.lq_consumed = consumed.astype(np.int64)
         res.lq_consumed_scale = cscale.astype(np.int32)

@@ -334,6 +334,31 @@ def add_pods_ready(snap: abi.FlatSnapshot, seed: int = 0, delay_ns=(0, 2_000), f
     return snap
 
 
+def add_max_exec(snap: abi.FlatSnapshot, seed: int = 0, share: float = 0.5, limit_s=(1, 3), spent_share: float = 0.1,
+                 since_ns: int = 2_000_000_000) -> abi.FlatSnapshot:
+    """MaximumExecutionTimeSeconds of an event drain (include/kueue_b200.h) on a snapshot with `adm_wl`, seeded: a share
+    `share` of the workloads gets a limit uniform in `limit_s` seconds (inclusive; 0 = nil elsewhere).  A share
+    `spent_share` of those starts with an accumulated time of limit - 1, limit or limit + 1 seconds, so its remaining time
+    is 1 s, 0 or negative: below the run time of most workloads; the others start nil.  Every admitted row of the
+    snapshot gets an Admitted time up to `since_ns` before now_ns (INT64_MIN where its checks run, adm_admitted_ns where
+    that is set)."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    W, A, now = snap.n_wl, snap.n_adm if "adm_cq" in snap.arrays else 0, int(snap.now_ns)
+    limit = np.where(rng.random(W) < share, rng.integers(int(limit_s[0]), int(limit_s[1]) + 1, W), 0)
+    spent = (limit > 0) & (rng.random(W) < spent_share)
+    acc = np.where(spent, np.maximum(limit + rng.integers(-1, 2, W), 0), -1)
+    since = now - rng.integers(0, int(since_ns) + 1, A)
+    a = snap.arrays
+    if "adm_admitted_ns" in a:
+        since = np.where(a["adm_admitted_ns"] != np.iinfo(np.int64).min, a["adm_admitted_ns"], since)
+    if "adm_check_end_ns" in a:
+        since = np.where(a["adm_check_end_ns"] != np.iinfo(np.int64).min, np.iinfo(np.int64).min, since)
+    snap.set("wl_max_exec_s", limit)
+    snap.set("wl_exec_acc_s", acc)
+    snap.set("adm_exec_since_ns", since)
+    return snap
+
+
 # The reference's scheduler performance scenario (test/performance/scheduler/configs/baseline/generator.yaml, generated
 # by runner/generator/generator.go): 5 cohorts of 6 ClusterQueues, one flavor, cpu only; per ClusterQueue, workload k of
 # a class is created at (k + 1) * interval and runs `run` once admitted (runner/controller/controller.go).
@@ -348,7 +373,7 @@ _MS = 1_000_000
 
 
 def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None = None, checks: int | None = None,
-                  pods_ready: int | None = None) -> abi.FlatSnapshot:
+                  pods_ready: int | None = None, max_exec: int | None = None) -> abi.FlatSnapshot:
     """The baseline scenario as numbers (15,000 workloads at scale 1; `scale` multiplies the count of every class):
     nominal 20 cpu and borrowingLimit 100 cpu per ClusterQueue, preemption reclaimWithinCohort Any and
     withinClusterQueue LowerPriority, BestEffortFIFO.  cpu is in milli-units.  wl_ts is the creation time, an empty
@@ -358,7 +383,9 @@ def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None 
     checks: a seed: every other ClusterQueue of each cohort gets an admission check (add_admission_checks: a
     ProvisioningRequest-like delay of 20-200 ms, a share of failing attempts, backoff base 1 s, max 8 s, limit 3).
     pods_ready: a seed: WaitForPodsReady on every workload (add_pods_ready: a PodsReady delay of 0-50 ms, 10% of the
-    workloads never ready, timeout 100 ms, backoff base 1 s, max 8 s, limit 2)."""
+    workloads never ready, timeout 100 ms, backoff base 1 s, max 8 s, limit 2).
+    max_exec: a seed: MaximumExecutionTimeSeconds (add_max_exec: half of the workloads get a limit of 1 s, and 20% of
+    those start with 0, 1 or 2 s accumulated, so they expire at admission or race their run time of up to 1 s)."""
     Q = PERF_COHORTS * PERF_CQS_PER_COHORT
     snap = abi.FlatSnapshot(n_cq=Q, n_cohort=PERF_COHORTS, n_flavor=1, n_resource=1)
     snap.set("parent", np.concatenate([Q + np.arange(Q) // PERF_CQS_PER_COHORT, np.full(PERF_COHORTS, -1)]))
@@ -392,6 +419,8 @@ def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None 
         add_admission_checks(snap, checks, delay_ns=(20 * _MS, 200 * _MS), cqs=np.arange(0, Q, 2))
     if pods_ready is not None:
         add_pods_ready(snap, pods_ready, delay_ns=(0, 50 * _MS), timeout_ns=100 * _MS)
+    if max_exec is not None:
+        add_max_exec(snap, max_exec, share=0.5, limit_s=(1, 1), spent_share=0.2)
     snap.finalize()
     snap.__dict__["perf_class"] = np.asarray(cls, np.int64)
     return snap
