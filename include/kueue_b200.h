@@ -415,6 +415,26 @@ typedef struct kb_snapshot {
   const int32_t *wl_exec_acc_s;     /* [n_wl] status.accumulatedPastExecutionTimeSeconds at the start; -1 = nil; NULL =
                                        every value nil                                                                  */
   const int64_t *adm_exec_since_ns; /* [n_adm] Admitted LastTransitionTime of each row; INT64_MIN = its checks run     */
+
+  /* ---- ClusterQueue and Cohort quota changes (optional; read by kb_run_drain only, kb_run_cycle ignores them) ----
+     Planned edits of the quota rows of one node (a ClusterQueue or a Cohort), applied on the drain's clock.  In the
+     reference a spec update goes through the cache (updateClusterQueue clusterqueue.go:130-145 /
+     updateQuotasAndResourceGroups :199-209, updateCohort cohort.go:44-52 -> updateCohortTreeResources
+     resource_node.go:168-198, which bumps AllocatableResourceGeneration of every ClusterQueue of the root tree,
+     :160-165) and through the queue manager (UpdateClusterQueue with specUpdated, clusterqueue_controller.go:384,
+     AddOrUpdateCohort manager.go:251-262 -> notifyRetryInadmissibleWithoutLock inadmissible_workloads.go:206-223).
+     n_quota_change == 0 or qc_ns == NULL: off, and every launch, copy and result of the drain stays as without this
+     block.  Otherwise the block turns on event mode (adm_wl is not needed).  Resource groups, flavor order, cohort
+     membership and every policy table stay static.  See kb_run_drain.  Errors (KB_ERR_INVALID): a NULL table with
+     n_quota_change > 0, n_quota_change < 0, qc_ns decreasing or <= now_ns (an edit already made belongs in the
+     snapshot's own rows), qc_node outside [0, n_cq + n_cohort), a negative nominal, KB_NO_LIMIT in a nominal row, a
+     negative limit other than KB_NO_LIMIT, and for a ClusterQueue a change to a cell its resource groups do not cover. */
+  int32_t n_quota_change;           /* edits below                                                                    */
+  const int64_t *qc_ns;             /* [n_quota_change] time of the edit, non-decreasing, each > now_ns               */
+  const int32_t *qc_node;           /* [n_quota_change] node in [0, n_cq + n_cohort)                                  */
+  const int64_t *qc_nominal;        /* [n_quota_change][F*R] the node's new nominal row                               */
+  const int64_t *qc_borrow_limit;   /* [n_quota_change][F*R] its new borrowing-limit row (KB_NO_LIMIT = nil)          */
+  const int64_t *qc_lend_limit;     /* [n_quota_change][F*R] its new lending-limit row (KB_NO_LIMIT = nil)            */
 } kb_snapshot;
 
 /* ------------------------------------------------------------------------
@@ -720,7 +740,29 @@ int32_t kb_download(kb_handle *h, kb_cycle_out *out);
  *      drain equals the drain without the block in heads, decisions, evictions, usage and per-workload results; only
  *      wl_exec_acc_s_out is new.
  * Deactivations (at an expiry or a release) between the start of cycle c and of c+1 count in
- * cycle_max_exec_deactivated[c].  Not modelled: reactivation (a user action), MultiKueue's handling of the field. */
+ * cycle_max_exec_deactivated[c].  Not modelled: reactivation (a user action), MultiKueue's handling of the field.
+ *
+ * Quota changes (kb_snapshot.n_quota_change > 0 with every qc_* table; event mode).  Edit i replaces the three quota
+ * rows of node qc_node[i] at qc_ns[i].  Additions to the loop:
+ *   1. every edit time is a pending event: E includes the next edit not applied yet; a quiet cycle waits for it, with no
+ *      head the clock jumps to it; after the last edit the stop rule is as before;
+ *   2. at a boundary t -> t' every edit with qc_ns in (t, t'] is applied in table order, in step 5 before the check
+ *      verdicts: its rows replace the node's (of two edits of one node in one boundary the later wins);
+ *   3. an edit whose three rows equal the node's rows at that point changes nothing (specUpdated is false: no bump, no
+ *      requeue); it still counts in n_quota_changes;
+ *   4. every other edit adds 1 to AllocatableResourceGeneration of every ClusterQueue of the node's root tree (of the
+ *      ClusterQueue alone when it has no cohort), which outdates every remembered LastAssignment there
+ *      (lastAssignmentOutdated flavorassigner.go:533: the next attempt searches flavors from the first), and marks the
+ *      root tree for the inadmissible requeue of step 7 (its NoFit sets are cleared, as in any requeue);
+ *   5. nothing is evicted: admitted rows keep their cells, usage above the new quota stays (as in the reference);
+ *   6. the LastAssignment of an entry that stays pending records the current generation;
+ *   7. the block composes with eviction latency, the sticky table, admission checks, WaitForPodsReady,
+ *      MaximumExecutionTimeSeconds and AFS with or without decay: none of their rules reads quotas.
+ * Edits applied between the start of cycle c and of c+1 count in cycle_quota_changes[c]; cq_generation receives the
+ * generations after the drain, for the caller to write back.  Resident tables: the drain edits the handle's device
+ * copies of nominal / borrow_limit / lend_limit / cq_generation and the tables derived from them, so a kb_run_drain with
+ * the block on resets the handle's static generation: the next kb_run_cycle / kb_upload on the handle uploads its
+ * static tables again whatever its static_generation. */
 typedef struct kb_drain_out {
   int32_t max_cycles;        /* in */
   int32_t n_cycles;          /* out: cycles run */
@@ -792,6 +834,10 @@ typedef struct kb_drain_out {
   int32_t *cycle_max_exec_deactivated;   /* [max_cycles] deactivations from the start of cycle c to the start of c+1 */
   int32_t *wl_exec_acc_s_out;            /* [n_wl] final accumulatedPastExecutionTimeSeconds, -1 = nil */
   uint8_t *wl_deactivation_reason;       /* [n_wl] 0 none, 1 Rejected, 2 RequeuingLimitExceeded, 3 MaximumExecutionTimeExceeded */
+  /* quota changes (kb_snapshot.n_quota_change > 0; zero / untouched otherwise; each pointer may be NULL) */
+  int64_t n_quota_changes;               /* out: edits applied, no-op edits included */
+  int32_t *cycle_quota_changes;          /* [max_cycles] edits applied from the start of cycle c to the start of c+1 */
+  int64_t *cq_generation;                /* [n_cq] AllocatableResourceGeneration after the drain */
 } kb_drain_out;
 int32_t kb_run_drain(kb_handle *h, const kb_snapshot *s, kb_drain_out *out);
 

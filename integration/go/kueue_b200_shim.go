@@ -385,6 +385,10 @@ func (s *Scheduler) flatten(snap *schdcache.Snapshot, heads []workload.Info, gen
 	// accumulated time from Status.AccumulatedPastExecutionTimeSeconds (nil = -1), and each admitted row's Admitted time
 	// from the Admitted condition's LastTransitionTime (math.MinInt64 while its checks are not all Ready):
 	//   c.wl_max_exec_s, c.wl_exec_acc_s, c.adm_exec_since_ns = cp32(maxExecS), cp32(accS), cp64(admittedAt)
+	// Quota changes (INTEGRATION.md): planned ClusterQueue / Cohort edits, one per node and time, sorted by time, each
+	// with the node's full rows after the change; kb_drain_out.cq_generation is written back after the drain:
+	//   c.n_quota_change, c.qc_ns, c.qc_node = C.int32_t(len(editNs)), cp64(editNs), cp32(editNode)
+	//   c.qc_nominal, c.qc_borrow_limit, c.qc_lend_limit = cp64(editNominal), cp64(editBorrow), cp64(editLend)
 	// They stay nil here: a single cycle ignores them.
 	if anyGroup { // optional table: NULL when no podset is grouped
 		c.ps_group = cp32(psGroup)

@@ -92,6 +92,8 @@ class kb_snapshot(C.Structure):
         ("pods_ready_timeout_ns", C.c_int64), ("pods_ready_backoff_base_s", C.c_int32), ("pods_ready_backoff_max_s", C.c_int32),
         ("pods_ready_backoff_limit", C.c_int32), ("pods_ready_requeue_creation", C.c_int32),
         ("wl_max_exec_s", _P(C.c_int32)), ("wl_exec_acc_s", _P(C.c_int32)), ("adm_exec_since_ns", _P(C.c_int64)),
+        ("n_quota_change", C.c_int32), ("qc_ns", _P(C.c_int64)), ("qc_node", _P(C.c_int32)), ("qc_nominal", _P(C.c_int64)),
+        ("qc_borrow_limit", _P(C.c_int64)), ("qc_lend_limit", _P(C.c_int64)),
     ]
 
 
@@ -152,6 +154,7 @@ class kb_drain_out(C.Structure):
         ("wl_pods_ready_at_ns", _P(C.c_int64)), ("wl_pods_ready_count_out", _P(C.c_int32)),
         ("n_max_exec_deactivated", C.c_int64), ("cycle_max_exec_deactivated", _P(C.c_int32)),
         ("wl_exec_acc_s_out", _P(C.c_int32)), ("wl_deactivation_reason", _P(C.c_uint8)),
+        ("n_quota_changes", C.c_int64), ("cycle_quota_changes", _P(C.c_int32)), ("cq_generation", _P(C.c_int64)),
     ]
 
 
@@ -213,6 +216,7 @@ _DT = {
     "wl_pods_ready_ns": np.int64, "wl_pods_ready_fail": np.int32, "wl_pods_ready_count": np.int32,
     "wl_pods_ready_evict_ns": np.int64, "adm_admitted_ns": np.int64,
     "wl_max_exec_s": np.int32, "wl_exec_acc_s": np.int32, "adm_exec_since_ns": np.int64,
+    "qc_ns": np.int64, "qc_node": np.int32, "qc_nominal": np.int64, "qc_borrow_limit": np.int64, "qc_lend_limit": np.int64,
 }
 # AdmissionFairSharing tables (include/kueue_b200.h): wl_lq absent = AFS off
 AFS_FIELDS = ("wl_lq", "lq_cq", "cq_afs", "lq_weight", "lq_consumed", "lq_consumed_scale", "lq_penalty", "afs_res_weight",
@@ -231,9 +235,11 @@ CHECK_FIELDS = ("wl_check_ns", "wl_check_fail", "wl_check_retries", "wl_check_ev
 PODS_READY_FIELDS = ("wl_pods_ready_ns", "wl_pods_ready_fail", "wl_pods_ready_count", "wl_pods_ready_evict_ns", "adm_admitted_ns")
 # MaximumExecutionTimeSeconds in event mode (include/kueue_b200.h): wl_max_exec_s absent = off; the others need it
 MAX_EXEC_FIELDS = ("wl_max_exec_s", "wl_exec_acc_s", "adm_exec_since_ns")
+# ClusterQueue / Cohort quota changes in event mode (include/kueue_b200.h): qc_ns absent = off; n_quota_change = len(qc_ns)
+QUOTA_CHANGE_FIELDS = ("qc_ns", "qc_node", "qc_nominal", "qc_borrow_limit", "qc_lend_limit")
 OPTIONAL_FIELDS = (("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows", "adm_wl") + AFS_FIELDS +
                    EVENT_FIELDS + AFS_DECAY_FIELDS + EVICT_END_FIELDS + STICKY_FIELDS + CHECK_FIELDS +
-                   PODS_READY_FIELDS + MAX_EXEC_FIELDS)  # NULL in kb_snapshot when absent
+                   PODS_READY_FIELDS + MAX_EXEC_FIELDS + QUOTA_CHANGE_FIELDS)  # NULL in kb_snapshot when absent
 ARRAY_FIELDS = list(_DT.keys())
 # tables the library keeps resident while kb_snapshot.static_generation is unchanged (include/kueue_b200.h)
 STATIC_FIELDS = ("parent", "fair_weight", "nominal", "borrow_limit", "lend_limit", "cq_within_cq", "cq_reclaim_within",
@@ -383,6 +389,7 @@ class FlatSnapshot:
         s.n_rg, s.n_wl, s.n_podset, s.n_adm = self.n_rg, self.n_wl, self.n_podset, self.n_adm
         s.n_adm_use = len(self.arrays["adm_use_fr"])
         s.n_usage_delta = len(self.arrays["usage_delta_cq"]) if "usage_delta_cq" in self.arrays else 0
+        s.n_quota_change = len(self.arrays["qc_ns"]) if "qc_ns" in self.arrays else 0
         s.n_heads = self.n_heads
         s.pods_resource, s.flags, s.now_ns = self.pods_resource, self.flags, self.now_ns
         s.static_generation = self.static_generation
@@ -497,6 +504,8 @@ class DrainOut:
         self.cycle_max_exec_deactivated = np.zeros(max_cycles, np.int32)  # MaximumExecutionTimeSeconds (kb_snapshot.wl_max_exec_s)
         self.wl_exec_acc_s_out = np.full(W, -1, np.int32)
         self.wl_deactivation_reason = np.zeros(W, np.uint8)
+        self.cycle_quota_changes = np.zeros(max_cycles, np.int32)  # quota changes (kb_snapshot.qc_*)
+        self.cq_generation = np.zeros(max(1, Q), np.int64)[:Q]
         cap = (min(W * 4 + Q, min(Q, W) * max_cycles) if trace_capacity is None else trace_capacity) if trace else 0
         self.trace_wl = np.zeros(max(1, cap), np.int32)
         self.trace_decision = np.zeros(max(1, cap), np.uint8)
@@ -527,6 +536,8 @@ class DrainOut:
         s.cycle_max_exec_deactivated = _ptr(self.cycle_max_exec_deactivated, C.c_int32)
         s.wl_exec_acc_s_out = _ptr(self.wl_exec_acc_s_out, C.c_int32)
         s.wl_deactivation_reason = _ptr(self.wl_deactivation_reason, C.c_uint8)
+        s.cycle_quota_changes = _ptr(self.cycle_quota_changes, C.c_int32)
+        s.cq_generation = _ptr(self.cq_generation, C.c_int64)
         if trace:
             s.trace_wl = _ptr(self.trace_wl, C.c_int32); s.trace_decision = _ptr(self.trace_decision, C.c_uint8)
         s.trace_capacity = cap
@@ -568,6 +579,8 @@ class DrainOut:
     def n_pods_ready_deactivated(self): return int(self.struct.n_pods_ready_deactivated)
     @property
     def n_max_exec_deactivated(self): return int(self.struct.n_max_exec_deactivated)
+    @property
+    def n_quota_changes(self): return int(self.struct.n_quota_changes)
 
     def cycles(self):
         """[(heads, decisions)] per cycle from the trace."""

@@ -90,7 +90,7 @@ struct kb_handle {
   int kev_n = 0;
   std::string err;
   kb_stats stats{};
-  uint32_t *host_words = nullptr;  // pinned scratch words; [32..63] = copy of the cycle header
+  uint32_t *host_words = nullptr;  // pinned scratch words; [32..63] = copy of the cycle header, [64..] kb_run_drain's
   const uint32_t *hdr_host = nullptr;  // where the last cycle's header landed (host_words or the caller's result block)
   int last_launches = 0;
   int64_t last_d2h_bytes = 0;
@@ -222,7 +222,7 @@ int32_t kb_create(const kb_config *cfg, kb_handle **out) {
   if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) { delete h; return fail(nullptr, KB_ERR_CUDA, "stream"); }
   cudaEventCreate(&h->ev0); cudaEventCreate(&h->ev1); cudaEventCreate(&h->ev2); cudaEventCreate(&h->ev3); cudaEventCreate(&h->ev4); cudaEventCreate(&h->ev5);
   for (int i = 0; i <= KB_N_KERNELS; i++) cudaEventCreate(&h->kev[i]);
-  cudaHostAlloc((void **)&h->host_words, 256, cudaHostAllocDefault);
+  cudaHostAlloc((void **)&h->host_words, 512, cudaHostAllocDefault);
   h->stats.sm_count = h->sm_count;
   *out = h;
   return KB_OK;
@@ -1354,14 +1354,14 @@ extern "C" int32_t kb_run_cycle(kb_handle *h, const kb_snapshot *s, kb_cycle_out
 // ---------------------------------------------------------------------------
 // kb_run_drain: iterated cycles with the queue layer on the device (kb_drain.cuh)
 // ---------------------------------------------------------------------------
-// what a boundary of kb_run_drain reads back, in the pinned host words [8, 24)
+// what a boundary of kb_run_drain reads back, in the pinned host words [64, 128)
 struct DrainWords {
-  uint32_t counters[KB_DC_EXEC_STATUS + 1];  // DrainDev::counters; [0] = heads of the next cycle
+  uint32_t counters[KB_DC_QC_HI + 1];   // DrainDev::counters; [0] = heads of the next cycle
   uint32_t n_new, n_cells;              // this cycle's admissions and their usage cells (the admit scans' totals)
   uint32_t status;                      // the cycle's status word (KBS_AFS_OVERFLOW)
   i64 t_next;                           // event mode: t_{c+1}
 };
-static_assert(8 * 4 + sizeof(DrainWords) <= 32 * 4, "host_words[32..63] hold the cycle header");
+static_assert(sizeof(DrainWords) <= 64 * 4, "host_words[64..127] hold the words of a drain boundary");
 
 static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out) {
   const int Q = s->n_cq, W = s->n_wl, R = s->n_resource, FR = s->n_flavor * s->n_resource;
@@ -1370,7 +1370,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   out->n_cycles = 0; out->n_decisions = 0; out->n_admitted = 0; out->gpu_ms = 0; out->n_evicted = 0;
   out->n_finished = 0; out->n_arrived = 0; out->end_ns = s->now_ns; out->n_evict_done = 0;
   out->n_check_ready = 0; out->n_check_retry = 0; out->n_check_rejected = 0; out->n_resorts = 0; out->resort_ms = 0;
-  out->n_pods_ready_timeout = 0; out->n_pods_ready_deactivated = 0; out->n_max_exec_deactivated = 0;
+  out->n_pods_ready_timeout = 0; out->n_pods_ready_deactivated = 0; out->n_max_exec_deactivated = 0; out->n_quota_changes = 0;
   // ---- eviction replay: host-side checks of adm_wl (include/kueue_b200.h)
   const bool replay = s->adm_wl != nullptr;
   if (replay) {
@@ -1386,8 +1386,9 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     }
   }
   // ---- event mode: host-side checks of the arrival and completion tables (include/kueue_b200.h)
+  const bool quota = s->n_quota_change > 0 && s->qc_ns;  // ClusterQueue / Cohort quota changes
   const bool events = s->wl_create_ns || s->wl_run_ns || s->adm_finish_ns || s->wl_evict_ns || s->wl_check_ns || s->wl_pods_ready_ns ||
-                      s->wl_max_exec_s;
+                      s->wl_max_exec_s || quota;
   if (events) {
     if (s->adm_finish_ns)
       for (int a = 0; a < s->n_adm; a++)
@@ -1531,6 +1532,37 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
         return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns differs from adm_admitted_ns");
     }
   }
+  // ---- quota changes: host-side checks (include/kueue_b200.h), and what the device needs besides the tables: the edits
+  // that change nothing, the root slot and the cohort tree of every other one (the rows change only through the edits, in
+  // table order, so the rows an edit meets are known here), the ClusterQueues of every root, the place of every
+  // ClusterQueue's generation in the static tree blocks
+  const int QN = Q + s->n_cohort, NQC = quota ? s->n_quota_change : 0;
+  std::vector<int32_t> qc_root, qc_tree, qc_tree_next, qc_cq_start, qc_cq, qc_blob_gen;
+  if (s->n_quota_change < 0) return fail(h, KB_ERR_INVALID, "quota changes: n_quota_change < 0");
+  if (s->n_quota_change > 0) {
+    if (!s->qc_ns || !s->qc_node || !s->qc_nominal || !s->qc_borrow_limit || !s->qc_lend_limit)
+      return fail(h, KB_ERR_INVALID, "quota changes: a NULL table with n_quota_change > 0");
+    std::vector<uint8_t> covered((size_t)Q * FR, 0);  // the cells a ClusterQueue's resource groups cover
+    for (int q = 0; q < Q; q++)
+      for (int g = s->cq_rg_start[q]; g < s->cq_rg_start[q + 1]; g++)
+        for (int k = s->rg_flavor_start[g]; k < s->rg_flavor_start[g + 1]; k++)
+          for (int r = 0; r < R; r++)
+            if (s->rg_res_mask[g] & (1u << r)) covered[(size_t)q * FR + (size_t)s->rg_flavors[k] * R + r] = 1;
+    for (int i = 0; i < NQC; i++) {
+      if (s->qc_ns[i] <= s->now_ns) return fail(h, KB_ERR_INVALID, "quota changes: qc_ns at or before now_ns");
+      if (i > 0 && s->qc_ns[i] < s->qc_ns[i - 1]) return fail(h, KB_ERR_INVALID, "quota changes: qc_ns decreasing");
+      const int n = s->qc_node[i];
+      if (n < 0 || n >= QN) return fail(h, KB_ERR_INVALID, "quota changes: qc_node out of range");
+      for (int c = 0; c < FR; c++) {
+        const size_t k = (size_t)i * FR + c;
+        if (s->qc_nominal[k] < 0 || s->qc_nominal[k] == KB_NO_LIMIT) return fail(h, KB_ERR_INVALID, "quota changes: a negative nominal or KB_NO_LIMIT in a nominal row");
+        if (s->qc_borrow_limit[k] < 0 || s->qc_lend_limit[k] < 0) return fail(h, KB_ERR_INVALID, "quota changes: a negative limit");
+        const size_t o = (size_t)n * FR + c;
+        if (n < Q && !covered[o] && (s->qc_nominal[k] != s->nominal[o] || s->qc_borrow_limit[k] != s->borrow_limit[o] || s->qc_lend_limit[k] != s->lend_limit[o]))
+          return fail(h, KB_ERR_INVALID, "quota changes: a ClusterQueue cell its resource groups do not cover");
+      }
+    }
+  }
   out->n_afs_samples = 0;
   if (Hcap == 0 || max_cycles == 0) return KB_OK;
   size_t extra = (size_t)std::min<long long>((long long)W, (long long)Hcap * max_cycles);
@@ -1610,6 +1642,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   char *sort_tmp, *scan_tmp = nullptr;
   i64 *run = nullptr, *create = nullptr, *evict_ns = nullptr, *check_ns = nullptr, *pr_ns = nullptr;
   int32_t *max_exec = nullptr;
+  i64 *qc_ns_d = nullptr, *qc_rows_d[3] = {nullptr, nullptr, nullptr};
+  int32_t *qc_node_d = nullptr, *qc_root_d = nullptr, *qc_tree_d = nullptr, *qc_tree_next_d = nullptr, *qc_cq_start_d = nullptr, *qc_cq_d = nullptr, *qc_blob_gen_d = nullptr;
   DrainDev X{};
   AdmTabs other{};  // compaction: the other half of the admitted tables' double buffer
   auto layout = [&](Arena &a) {
@@ -1622,7 +1656,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     X.flag = a.take<int32_t>((size_t)Q + 2); X.pos = a.take<int32_t>((size_t)Q + 2);
     X.e_assumed = a.take<int32_t>(Hz + 2); X.e_ncells = a.take<int32_t>(Hz + 2);
     X.e_adm_off = a.take<int32_t>(Hz + 2); X.e_cell_off = a.take<int32_t>(Hz + 2);
-    X.counters = a.take<int32_t>(KB_DC_EXEC_STATUS + 1);
+    X.counters = a.take<int32_t>(KB_DC_QC_HI + 1);
     X.wl_admit_cycle = a.take<int32_t>(Wz); X.wl_evals = a.take<int32_t>(Wz); X.wl_last_decision = a.take<uint8_t>(Wz);
     if (trace_cap) { X.trace_wl = a.take<int32_t>(trace_cap); X.trace_dec = a.take<uint8_t>(trace_cap); }
     if (replay || events) {
@@ -1688,6 +1722,12 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       X.lq_last = a.take<i64>(Lz); X.lq_adm = a.take<i64>(LR);
       X.adm_lq = a.take<int32_t>(Acap); other.lq = a.take<int32_t>(Acap);
       X.afs_samples = a.take<unsigned long long>(1);
+    }
+    if (quota) {  // the edits and the host's precomputation (quota_prep below)
+      qc_ns_d = a.take<i64>(NQC); qc_node_d = a.take<int32_t>(NQC);
+      qc_rows_d[0] = a.take<i64>((size_t)NQC * FR); qc_rows_d[1] = a.take<i64>((size_t)NQC * FR); qc_rows_d[2] = a.take<i64>((size_t)NQC * FR);
+      qc_root_d = a.take<int32_t>(NQC); qc_tree_d = a.take<int32_t>(NQC); qc_tree_next_d = a.take<int32_t>(NQC);
+      qc_cq_start_d = a.take<int32_t>(nR + 1); qc_cq_d = a.take<int32_t>((size_t)std::max(1, Q)); qc_blob_gen_d = a.take<int32_t>((size_t)std::max(1, Q));
     }
   };
   if (!h->drain_arena.carve(layout)) return fail(h, KB_ERR_CUDA, "kb_run_drain: cudaMalloc of the drain buffer failed");
@@ -1854,6 +1894,52 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     CUDA_TRY(h, cudaMemsetAsync(X.afs_samples, 0, 8, h->stream));
     X.half_life_ns = s->afs_half_life_ns; X.sampling_ns = s->afs_sampling_ns;
   }
+  if (quota) {  // quota_prep: no-op edits, roots and trees of the others; the ClusterQueues of every root; the blob offsets
+    std::vector<i64> nom(s->nominal, s->nominal + (size_t)QN * FR), bl(s->borrow_limit, s->borrow_limit + (size_t)QN * FR),
+        ll(s->lend_limit, s->lend_limit + (size_t)QN * FR);  // the rows each edit meets
+    qc_root.assign((size_t)NQC, -1); qc_tree.assign((size_t)NQC, -1);
+    for (int i = 0; i < NQC; i++) {
+      const int n = s->qc_node[i];
+      const size_t o = (size_t)n * FR, k = (size_t)i * FR, b = (size_t)FR * 8;
+      if (!memcmp(&nom[o], s->qc_nominal + k, b) && !memcmp(&bl[o], s->qc_borrow_limit + k, b) && !memcmp(&ll[o], s->qc_lend_limit + k, b)) continue;
+      memcpy(&nom[o], s->qc_nominal + k, b); memcpy(&bl[o], s->qc_borrow_limit + k, b); memcpy(&ll[o], s->qc_lend_limit + k, b);
+      qc_root[i] = h->root_slot[n];
+      if (D.tl_subtree && h->root_slot[n] >= D.nLone) qc_tree[i] = h->root_slot[n] - D.nLone;  // lone ClusterQueues come first
+    }
+    qc_tree_next.assign((size_t)NQC, NQC);
+    {
+      std::vector<int32_t> later((size_t)std::max(1, D.nTrees), NQC);
+      for (int i = NQC - 1; i >= 0; i--)
+        if (qc_tree[i] >= 0) { qc_tree_next[i] = later[qc_tree[i]]; later[qc_tree[i]] = i; }
+    }
+    qc_cq_start.assign(h->root_cq_start.begin(), h->root_cq_start.end());
+    qc_cq.assign((size_t)std::max(1, Q), 0);
+    std::vector<int32_t> fill(qc_cq_start.begin(), qc_cq_start.end() - 1);
+    for (int q = 0; q < Q; q++) qc_cq[fill[h->root_slot[q]]++] = q;
+    qc_blob_gen.assign((size_t)std::max(1, Q), -1);
+    for (int q = 0; q < Q; q++) {
+      const int slot = h->root_slot[q];
+      if (slot < D.nLone) continue;
+      const int tr = slot - D.nLone, b0 = h->tree_blob_off[tr];
+      const TreeBlobHdr *BH = (const TreeBlobHdr *)(h->tree_blob.data() + b0);
+      qc_blob_gen[q] = b0 + BH->gen + 8 * h->local_idx[q];
+    }
+    CUDA_TRY(h, h2d(h, qc_ns_d, s->qc_ns, (size_t)NQC * 8));
+    CUDA_TRY(h, h2d(h, qc_node_d, s->qc_node, (size_t)NQC * 4));
+    CUDA_TRY(h, h2d(h, qc_rows_d[0], s->qc_nominal, (size_t)NQC * FR * 8));
+    CUDA_TRY(h, h2d(h, qc_rows_d[1], s->qc_borrow_limit, (size_t)NQC * FR * 8));
+    CUDA_TRY(h, h2d(h, qc_rows_d[2], s->qc_lend_limit, (size_t)NQC * FR * 8));
+    CUDA_TRY(h, h2d(h, qc_root_d, qc_root.data(), (size_t)NQC * 4));
+    CUDA_TRY(h, h2d(h, qc_tree_d, qc_tree.data(), (size_t)NQC * 4));
+    CUDA_TRY(h, h2d(h, qc_tree_next_d, qc_tree_next.data(), (size_t)NQC * 4));
+    CUDA_TRY(h, h2d(h, qc_cq_start_d, qc_cq_start.data(), qc_cq_start.size() * 4));
+    CUDA_TRY(h, h2d(h, qc_cq_d, qc_cq.data(), qc_cq.size() * 4));
+    CUDA_TRY(h, h2d(h, qc_blob_gen_d, qc_blob_gen.data(), qc_blob_gen.size() * 4));
+    CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_QC_LO, 0, 2 * 4, h->stream));  // once: the boundaries never clear them
+    X.qc_ns = qc_ns_d; X.qc_node = qc_node_d; X.qc_nominal = qc_rows_d[0]; X.qc_blimit = qc_rows_d[1]; X.qc_llimit = qc_rows_d[2];
+    X.qc_root = qc_root_d; X.qc_tree = qc_tree_d; X.qc_tree_next = qc_tree_next_d; X.qc_cq_start = qc_cq_start_d; X.qc_cq = qc_cq_d; X.qc_blob_gen = qc_blob_gen_d;
+    X.n_qc = NQC;
+  }
   // ---- per-ClusterQueue order (queueOrderingFunc): stable LSD passes uid -> timestamp -> (ClusterQueue | priority desc)
   const int tb = 256, nbW = (W + tb - 1) / tb, nbQ = (Q + tb - 1) / tb;
   auto sort_queues = [&]() -> cudaError_t {  // also the re-sort of admission checks (same segments, same q_start)
@@ -1900,7 +1986,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     k_scan_i32<<<1, 1024, 0, h->stream>>>(X.flag, X.pos, Q);
     k_drain_heads<<<nbQ, tb, 0, h->stream>>>(D, X, d_heads);
   };
-  DrainWords &hw = *reinterpret_cast<DrainWords *>(&h->host_words[8]);
+  DrainWords &hw = *reinterpret_cast<DrainWords *>(&h->host_words[64]);
   CUDA_TRY(h, cudaMemsetAsync(X.counters + 1, 0, 5 * 4, h->stream));
   enqueue_heads();
   CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[0], X.counters, 4, cudaMemcpyDeviceToHost, h->stream));
@@ -1971,6 +2057,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       const int nbB = std::max(1, (bound + tb - 1) / tb);
       k_drain_ev_min<<<nbB, tb, 0, h->stream>>>(X, bound, n_new_d);
       k_drain_ev_next<<<1, 1, 0, h->stream>>>(X, t, step, jump, n_new_d);
+      if (quota) k_drain_quota<<<1, 1024, 0, h->stream>>>(D, X);  // step 5: the edits, before the verdicts
       if (decay) k_drain_afs_decay<<<nbL, tb, 0, h->stream>>>(D, X, L);  // samples due in (t, t_{c+1}], before the completions
       k_drain_finish<<<nbB, tb, 0, h->stream>>>(D, X, bound, n_new_d);
       if (X.arr_key) k_drain_arrive<<<nbArr, tb, 0, h->stream>>>(X);
@@ -1993,7 +2080,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (!jump) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_new, n_new_d, 4, cudaMemcpyDeviceToHost, h->stream));
     if (!compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_cells, X.e_cell_off + n_live, 4, cudaMemcpyDeviceToHost, h->stream));
     if (afs && (!jump || decay)) CUDA_TRY(h, cudaMemcpyAsync(&hw.status, D.status, 4, cudaMemcpyDeviceToHost, h->stream));
-    if (compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[1], X.counters + 1, (mx ? KB_DC_EXEC_STATUS : pr ? KB_DC_PR_DEACTIVATED : checks ? KB_DC_CHECK_REJECTED : events ? KB_DC_ARR_HI : KB_DC_FULL) * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[1], X.counters + 1, (quota ? KB_DC_QC_HI : mx ? KB_DC_EXEC_STATUS : pr ? KB_DC_PR_DEACTIVATED : checks ? KB_DC_CHECK_REJECTED : events ? KB_DC_ARR_HI : KB_DC_FULL) * 4, cudaMemcpyDeviceToHost, h->stream));
     if (events) CUDA_TRY(h, cudaMemcpyAsync(&hw.t_next, X.clock, 8, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     if (!jump) {
@@ -2019,6 +2106,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       if (pr && out->cycle_pods_ready_timeout) out->cycle_pods_ready_timeout[cyc] = 0;
       if (pr && out->cycle_pods_ready_deactivated) out->cycle_pods_ready_deactivated[cyc] = 0;
       if (mx && out->cycle_max_exec_deactivated) out->cycle_max_exec_deactivated[cyc] = 0;
+      if (quota && out->cycle_quota_changes) out->cycle_quota_changes[cyc] = 0;
       out->n_decisions += n_live; out->n_admitted += n_new; out->n_evicted += n_ev;
       out->n_cycles = ++cyc;
     } else {
@@ -2059,6 +2147,11 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       exec_seen = hw.counters[KB_DC_EXEC_DEACTIVATED];
       out->n_max_exec_deactivated += de;
       if (cyc > 0 && out->cycle_max_exec_deactivated) out->cycle_max_exec_deactivated[cyc - 1] += de;
+    }
+    if (quota) {  // edits applied at this boundary
+      const int qc = (int)(hw.counters[KB_DC_QC_HI] - hw.counters[KB_DC_QC_LO]);
+      out->n_quota_changes += qc;
+      if (cyc > 0 && out->cycle_quota_changes) out->cycle_quota_changes[cyc - 1] += qc;
     }
     if (lat) {  // evictions completed at this boundary (counter slot 4, inside the events copy)
       const int done = (int)hw.counters[KB_DC_EVICT_DONE];
@@ -2140,6 +2233,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   if (out->ps_flavor && PR) CUDA_TRY(h, cudaMemcpyAsync(out->ps_flavor, D.ps_flavor, PR, cudaMemcpyDeviceToHost, h->stream));
   if (out->ps_count && D.P) CUDA_TRY(h, cudaMemcpyAsync(out->ps_count, D.ps_count_out, (size_t)D.P * 4, cudaMemcpyDeviceToHost, h->stream));
   if (out->cq_usage) CUDA_TRY(h, cudaMemcpyAsync(out->cq_usage, D.cq_usage, (size_t)Q * FR * 8, cudaMemcpyDeviceToHost, h->stream));
+  if (quota && out->cq_generation) CUDA_TRY(h, cudaMemcpyAsync(out->cq_generation, D.cq_generation, (size_t)Q * 8, cudaMemcpyDeviceToHost, h->stream));
   size_t nt = std::min<size_t>(trace_cap, (size_t)out->n_decisions);
   if (nt) {
     CUDA_TRY(h, cudaMemcpyAsync(out->trace_wl, X.trace_wl, nt * 4, cudaMemcpyDeviceToHost, h->stream));
@@ -2155,6 +2249,7 @@ extern "C" int32_t kb_run_drain(kb_handle *h, const kb_snapshot *s, kb_drain_out
   if (!h || !s || !out) return KB_ERR_INVALID;
   int32_t rc = drain_impl(h, s, out);
   h->drain_mode = false; h->drain_events = false; h->drain_extra_adm = 0; h->drain_extra_au = 0;
+  if (s->n_quota_change > 0 && s->qc_ns) h->static_gen = 0;  // quota changes edited the resident static tables
   h->uploaded = false;  // the resident snapshot was consumed (queues advanced, admitted tables grown)
   return rc;
 }

@@ -190,6 +190,26 @@ __device__ __forceinline__ i64 local_quota(i64 subtree, i64 lend_limit) {
   return lend_limit != KB_NO_LIMIT ? imax(0, subtree - lend_limit) : 0;
 }
 
+// one cell of the tree-local quota tables (DevSnap::tl_subtree / tl_blimit / tl_lquota), as the static upload builds
+// them (k_tl_static, k_tl_root, kb_flat.cuh) and kb_run_drain's quota changes rebuild them for an edited tree
+// (k_drain_quota, kb_drain.cuh).  Cell i of [tree nodes][FR]: SubtreeQuota (a ClusterQueue's is its nominal quota,
+// resource_node.go:160-166), the borrowing limit and localQuota (:66-71).
+__device__ __forceinline__ void tl_static_cell(const DevSnap &D, i64 *subtree, i64 *blimit, i64 *lquota, int i) {
+  const size_t g = (size_t)D.tree_nodes[i / D.FR] * D.FR + i % D.FR;
+  subtree[i] = D.nominal[g]; blimit[i] = D.blimit[g]; lquota[i] = local_quota(D.nominal[g], D.llimit[g]);
+}
+// the root row of flat tree t in column fr: SubtreeQuota = nominal + sum of (SubtreeQuota - localQuota) over the
+// ClusterQueues (accumulateFromChild resource_node.go:210-217), then its localQuota; after tl_static_cell
+__device__ __forceinline__ void tl_root_cell(const DevSnap &D, i64 *subtree, i64 *lquota, int t, int fr) {
+  if (!D.tree_flat[t]) return;
+  const size_t r0 = (size_t)D.tree_start[t] * D.FR + fr;
+  const int nn = D.tree_start[t + 1] - D.tree_start[t];
+  i64 sub = subtree[r0];
+  for (int h = 1; h < nn; h++) sub += subtree[r0 + (size_t)h * D.FR] - lquota[r0 + (size_t)h * D.FR];
+  subtree[r0] = sub;
+  lquota[r0] = local_quota(sub, D.llimit[(size_t)D.tree_nodes[D.tree_start[t]] * D.FR + fr]);
+}
+
 // FindHeightOfLowestSubtreeThatFits hierarchical_preemption.go:214-227, on the
 // cycle-start usage.  Returns the borrow height; *may_reclaim = second result.
 __device__ __forceinline__ int nix(const DevSnap &D, int node) { return D.tab_local == 1 ? D.local_idx[node] : node; }

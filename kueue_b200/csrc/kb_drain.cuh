@@ -317,6 +317,17 @@ struct DrainDev {
   const int32_t *wl_max_exec;      // [W] limit in seconds, 0 = nil
   int32_t *wl_exec_acc;            // [W] accumulated seconds, -1 = nil
   i64 *adm_exec_since;             // [A_cap] Admitted time of each row (current half), INT64_MIN while its checks run
+  // quota changes (event mode); qc_ns == nullptr: off.  The host works out which edits change nothing, the root and
+  // the tree of every other one (the rows change only through the edits, in table order).
+  const i64 *qc_ns;                // [n_qc] edit times, non-decreasing
+  const int32_t *qc_node;          // [n_qc] edited node
+  const i64 *qc_nominal, *qc_blimit, *qc_llimit;  // [n_qc][FR] the node's new rows
+  const int32_t *qc_root;          // [n_qc] root slot of the node's tree, -1 = the edit changes nothing
+  const int32_t *qc_tree;          // [n_qc] cohort tree of the tree-local tables to refresh, -1 = none
+  const int32_t *qc_tree_next;     // [n_qc] the next edit that refreshes the same tree (n_qc = none): one refresh per tree
+  const int32_t *qc_cq_start, *qc_cq;  // [nRoots+1] / [Q] the ClusterQueues of every root tree
+  const int32_t *qc_blob_gen;      // [Q] byte offset of the ClusterQueue's generation in tree_blob, -1 = not in a tree
+  int n_qc;
 };
 // adm_phase: what the finish column of a row holds.  RUN: its finish (or its eviction's end when adm_evicting); CHECK: its
 // checks' verdict; WAIT: the timeout T of a PodsReady attempt that fails; TIMED_OUT: the end of its eviction by that
@@ -329,11 +340,13 @@ enum { KB_DR_REJECTED = 1, KB_DR_REQUEUING_LIMIT = 2, KB_DR_MAX_EXEC = 3 };
 // arrived prefix of arr_order [lo, hi); admission checks: [11] the stamp (cycle + 1) of the last boundary that needs a
 // re-sort, [12] / [13] / [14] Ready / Retry / Rejected verdicts since the start (the host takes differences: no memset);
 // WaitForPodsReady: [15] / [16] timeouts that requeue / deactivate since the start, likewise; MaximumExecutionTimeSeconds:
-// [17] deactivations since the start, [18] KBS_EXEC_OVERFLOW once an accumulated time leaves int32 (never cleared)
+// [17] deactivations since the start, [18] KBS_EXEC_OVERFLOW once an accumulated time leaves int32 (never cleared);
+// quota changes: [19] / [20] the edits of this boundary [lo, hi) (hi = edits applied since the start)
 enum { KB_DC_EVICTED = 1, KB_DC_ROWS = 2, KB_DC_CELLS = 3, KB_DC_EVICT_DONE = 4, KB_DC_FULL = 5,
        KB_DC_FINISHED = 6, KB_DC_ARRIVED = 7, KB_DC_END = 8, KB_DC_ARR_LO = 9, KB_DC_ARR_HI = 10,
        KB_DC_RESORT = 11, KB_DC_CHECK_READY = 12, KB_DC_CHECK_RETRY = 13, KB_DC_CHECK_REJECTED = 14,
-       KB_DC_PR_TIMEOUT = 15, KB_DC_PR_DEACTIVATED = 16, KB_DC_EXEC_DEACTIVATED = 17, KB_DC_EXEC_STATUS = 18 };
+       KB_DC_PR_TIMEOUT = 15, KB_DC_PR_DEACTIVATED = 16, KB_DC_EXEC_DEACTIVATED = 17, KB_DC_EXEC_STATUS = 18,
+       KB_DC_QC_LO = 19, KB_DC_QC_HI = 20 };
 
 __device__ __forceinline__ int drain_seg0(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq] : cq; }
 __device__ __forceinline__ int drain_seg1(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq + 1] : cq + 1; }
@@ -800,11 +813,13 @@ __global__ void k_drain_ev_min(DrainDev X, int bound, const int32_t *n_new) {
   i64 v = INT64_MAX;
   if (a < bound && a < n_rows && X.adm_dead[a] != X.cycle + 1) v = X.adm_finish[a];
   if (a == 0 && X.counters[KB_DC_ARR_HI] < X.n_arr) v = min(v, ev_time(X.arr_key[X.counters[KB_DC_ARR_HI]]));
+  if (a == 0 && X.qc_ns && X.counters[KB_DC_QC_HI] < X.n_qc) v = min(v, X.qc_ns[X.counters[KB_DC_QC_HI]]);  // the next edit
   for (int o = 16; o > 0; o >>= 1) v = min(v, (i64)__shfl_xor_sync(0xffffffffu, (long long)v, o));
   if ((threadIdx.x & 31) == 0 && v < INT64_MAX) atomicMin((long long *)&X.clock[1], (long long)v);
 }
 // t_{c+1} and the end flag (one thread).  jump: no heads, the clock goes to E.  Otherwise a cycle that admitted or
-// evicted steps, a quiet one waits for E; no E ends the drain.  Then the arrived prefix up to t_{c+1}.
+// evicted steps, a quiet one waits for E; no E ends the drain.  Then the arrived prefix up to t_{c+1}, and the edits
+// with a time in (t_c, t_{c+1}] (k_drain_quota applies them).
 __global__ void k_drain_ev_next(DrainDev X, i64 t_c, i64 step, int jump, const int32_t *n_new) {
   const i64 E = min(X.clock[1], X.clock[2]);  // [2]: the next RequeueAt (admission checks), INT64_MAX otherwise
   X.clock[2] = INT64_MAX;
@@ -821,6 +836,13 @@ __global__ void k_drain_ev_next(DrainDev X, i64 t_c, i64 step, int jump, const i
   const int lo = X.counters[KB_DC_ARR_HI];
   X.counters[KB_DC_ARR_LO] = lo;
   X.counters[KB_DC_ARR_HI] = (end || !X.arr_key) ? lo : ev_upper_bound(X.arr_key, lo, X.n_arr, tn);
+  if (X.qc_ns) {
+    int qlo = X.counters[KB_DC_QC_HI], qhi = X.n_qc;
+    X.counters[KB_DC_QC_LO] = qlo;
+    if (end) qhi = qlo;
+    while (qlo < qhi) { const int m = qlo + (qhi - qlo) / 2; if (X.qc_ns[m] <= tn) qlo = m + 1; else qhi = m; }
+    X.counters[KB_DC_QC_HI] = qlo;
+  }
 }
 // completions (thread per row): a live row with finish <= t_{c+1} gets the dead stamp, its cells leave its ClusterQueue's
 // usage (cache.DeleteWorkload, integer atomics), its record becomes FINISHED and its root tree is marked.  An evicting
@@ -977,6 +999,46 @@ __global__ void k_drain_arrive(DrainDev X) {
       X.wl_state[w] = KB_WS_QUEUED;
       atomicMin(&X.cursor[s], p);
     }
+  }
+}
+
+// ---- quota changes -----------------------------------------------------------------------------------------------------
+// the edits of this boundary (one block, after k_drain_ev_next and before k_drain_finish: step 5 before the verdicts), in
+// table order: the node's three rows, +1 on the generation of every ClusterQueue of its root tree (D.cq_generation and
+// the copy in the tree's static block, TreeBlobHdr.gen), the root marked for k_drain_requeue; then the tree-local quota
+// tables of the edited trees, rebuilt from the new rows as the static upload builds them, once per tree (by the tree's
+// last edit of the boundary).  An edit that changes nothing (qc_root -1) is only counted.
+__global__ void k_drain_quota(DevSnap D, DrainDev X) {
+  const int lo = X.counters[KB_DC_QC_LO], hi = X.counters[KB_DC_QC_HI];
+  if (lo == hi) return;
+  const int FR = D.FR;
+  i64 *nom = const_cast<i64 *>(D.nominal), *bl = const_cast<i64 *>(D.blimit), *ll = const_cast<i64 *>(D.llimit);
+  i64 *gen = const_cast<i64 *>(D.cq_generation);
+  unsigned char *blob = const_cast<unsigned char *>(D.tree_blob);
+  for (int i = lo; i < hi; i++) {
+    const int slot = X.qc_root[i];
+    if (slot < 0) continue;
+    const size_t src = (size_t)i * FR, dst = (size_t)X.qc_node[i] * FR;
+    for (int c = threadIdx.x; c < FR; c += blockDim.x) { nom[dst + c] = X.qc_nominal[src + c]; bl[dst + c] = X.qc_blimit[src + c]; ll[dst + c] = X.qc_llimit[src + c]; }
+    for (int k = X.qc_cq_start[slot] + threadIdx.x; k < X.qc_cq_start[slot + 1]; k += blockDim.x) {
+      const int q = X.qc_cq[k];
+      const i64 g = gen[q] + 1;
+      gen[q] = g;
+      if (X.qc_blob_gen[q] >= 0) *(i64 *)(blob + X.qc_blob_gen[q]) = g;
+    }
+    if (threadIdx.x == 0) X.root_mark[slot] = X.cycle + 1;
+    __syncthreads();  // the next edit may write the same rows and generations
+  }
+  if (!D.tl_subtree) return;
+  i64 *sub = const_cast<i64 *>(D.tl_subtree), *tbl = const_cast<i64 *>(D.tl_blimit), *lq = const_cast<i64 *>(D.tl_lquota);
+  for (int i = lo; i < hi; i++) {
+    const int t = X.qc_tree[i];
+    if (t < 0 || X.qc_tree_next[i] < hi) continue;
+    const int c0 = D.tree_start[t] * FR, c1 = D.tree_start[t + 1] * FR;
+    for (int c = c0 + threadIdx.x; c < c1; c += blockDim.x) tl_static_cell(D, sub, tbl, lq, c);
+    __syncthreads();
+    for (int fr = threadIdx.x; fr < FR; fr += blockDim.x) tl_root_cell(D, sub, lq, t, fr);
+    __syncthreads();
   }
 }
 

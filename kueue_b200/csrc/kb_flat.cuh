@@ -87,28 +87,21 @@ __global__ void k_cq_rec(DevSnap D, int4 *rec, int tl_cells) {
   if (i < tl_cells) tl_usage_write(D, i);
 }
 // static quota tables into tree-local row order (once per static upload), holding the quotas k_cycle_flat derives from
-// them: SubtreeQuota (a ClusterQueue's is its nominal quota, resource_node.go:160-166) and localQuota (:66-71) per cell.
+// them: SubtreeQuota (a ClusterQueue's is its nominal quota, resource_node.go:160-166) and localQuota (:66-71) per cell
+// (tl_static_cell / tl_root_cell, kb_device.cuh).
 // A flat root's SubtreeQuota and localQuota depend on its ClusterQueues' rows and are written by k_tl_root.  Cohort
 // rows of hierarchical trees are left at nominal / local_quota(nominal) and never read: k_cycle_flat needs every tree flat.
 __global__ void k_tl_static(DevSnap D, i64 *subtree, i64 *blimit, i64 *lquota, int tl_cells) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= tl_cells) return;
-  const size_t g = (size_t)D.tree_nodes[i / D.FR] * D.FR + i % D.FR;
-  subtree[i] = D.nominal[g]; blimit[i] = D.blimit[g]; lquota[i] = local_quota(D.nominal[g], D.llimit[g]);
+  tl_static_cell(D, subtree, blimit, lquota, i);
 }
 // the root row of a flat tree: SubtreeQuota = nominal + sum of (SubtreeQuota - localQuota) over the ClusterQueues
 // (accumulateFromChild resource_node.go:210-217), then its localQuota.  One thread per (tree, column), after k_tl_static.
 __global__ void k_tl_root(DevSnap D, i64 *subtree, i64 *lquota) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= D.nTrees * D.FR) return;
-  const int t = k / D.FR, fr = k % D.FR;
-  if (!D.tree_flat[t]) return;
-  const size_t r0 = (size_t)D.tree_start[t] * D.FR + fr;
-  const int nn = D.tree_start[t + 1] - D.tree_start[t];
-  i64 sub = subtree[r0];
-  for (int h = 1; h < nn; h++) sub += subtree[r0 + (size_t)h * D.FR] - lquota[r0 + (size_t)h * D.FR];
-  subtree[r0] = sub;
-  lquota[r0] = local_quota(sub, D.llimit[(size_t)D.tree_nodes[D.tree_start[t]] * D.FR + fr]);
+  tl_root_cell(D, subtree, lquota, k / D.FR, k % D.FR);
 }
 // Everything the cycle needs prepared on the device, in one launch: head records, result rows of workloads that are
 // not heads (-1 / 0), cleared cycle header.

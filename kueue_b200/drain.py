@@ -256,6 +256,30 @@ MaximumExecutionTimeExceeded and never requeued (workload_types.go:71-77,658-662
 `exec_seconds` is int32(Duration.Seconds()): float64(sec) + float64(nsec) / 1e9, truncated per attempt; from about 2^24 s
 the float sum can round up to sec + 1.  A value or a sum outside int32 raises ExecOverflow (kb_run_drain:
 KB_ERR_UNSUPPORTED).  Deactivations between the start of cycle c and of c+1 are cycle c's (`max_exec_deactivated`).
+
+ClusterQueue and Cohort quota changes (event mode, the snapshot carries `qc_ns`, `qc_node`, `qc_nominal`,
+`qc_borrow_limit` and `qc_lend_limit`, include/kueue_b200.h).  Edit i replaces the three quota rows of node qc_node[i]
+at qc_ns[i].  In the reference a spec update reaches the cache (updateClusterQueue clusterqueue.go:130-145 ->
+updateQuotasAndResourceGroups :199-209; updateCohort cohort.go:44-52) and the queue manager (UpdateClusterQueue with
+specUpdated, clusterqueue_controller.go:384; AddOrUpdateCohort manager.go:251-262):
+  1. every edit time is a pending event: E includes the next edit not applied yet, a quiet cycle waits for it, with no
+     head the clock jumps to it; after the last edit the stop rule is as before;
+  2. at a boundary t -> t' every edit with qc_ns in (t, t'] is applied in table order (`apply_quota_changes`), in step
+     5 before the verdicts: its rows replace the node's in the `static` tables the cycles see (of two edits of one node
+     in one boundary the later wins);
+  3. an edit whose three rows equal the node's current rows changes nothing (updateQuotasAndResourceGroups returns
+     false, specUpdated is false): no bump, no requeue.  It still counts in `quota_changes`;
+  4. every other edit adds 1 to the generation (AllocatableResourceGeneration) of every ClusterQueue of the node's root
+     tree, or of the ClusterQueue alone without a cohort (updateCohortTreeResources resource_node.go:168-198 ->
+     updateClusterQueueResourceNode :160-165), so every remembered LastAssignment there is outdated
+     (lastAssignmentOutdated flavorassigner.go:533); and it marks the root tree for the requeue of step 7
+     (notifyRetryInadmissibleWithoutLock inadmissible_workloads.go:206-223), which clears its NoFit sets;
+  5. nothing is evicted: admitted rows keep their cells, usage above the new quota stays;
+  6. the LastAssignment of an entry that stays pending records the current generation (`gen`);
+  7. the block composes with every block above: none of their rules reads quotas.
+Every cycle's snapshot carries a static_generation that changes with the rows (`static_generation_after`; 0 stays
+"none"), so an evaluator that keeps static tables resident never reuses old quotas.  Edits applied between the start
+of cycle c and of c+1 are cycle c's (`quota_changes`); `cq_generation` holds the generations after the drain.
 """
 from __future__ import annotations
 
@@ -329,6 +353,11 @@ class DrainResult:
     wl_exec_acc_s: np.ndarray | None = None                    # [n_wl] final accumulated seconds, -1 = nil
     exec_spans: List[tuple] = field(default_factory=list)      # (record, Admitted time, release time, seconds added)
     wl_deactivation_reason: np.ndarray | None = None           # [n_wl] 0 none, 1 Rejected, 2 RequeuingLimitExceeded, 3 this
+    # quota changes (qc_ns in the snapshot; None / empty / 0 otherwise)
+    quota_changes: List[np.ndarray] = field(default_factory=list)  # per cycle: indices of the edits applied
+    n_quota_changes: int = 0                                   # those before cycle 0 included (no-op edits too)
+    cq_generation: np.ndarray | None = None                    # [n_cq] the generations after the drain
+    static_generations: List[int] = field(default_factory=list)  # per cycle: the static_generation its snapshot carried
 
     @property
     def n_evicted(self) -> int:
@@ -443,6 +472,50 @@ def exec_deadline(admitted_ns: int, max_s: int, acc_s: int) -> int:
     """the MaximumExecutionTimeSeconds deadline A + (max - acc) s (acc -1 = nil, read as 0), saturating both ways
     (kb_drain.cuh kb_exec_deadline)"""
     return max(min(int(admitted_ns) + (int(max_s) - max(int(acc_s), 0)) * _S, NEVER), UNSET)
+
+
+def check_quota_changes(snap) -> None:
+    """the refusals of the quota-change tables (kb_run_drain: KB_ERR_INVALID): ValueError"""
+    a = snap.arrays
+    if not any(k in a for k in abi.QUOTA_CHANGE_FIELDS):
+        return
+    if not all(k in a for k in abi.QUOTA_CHANGE_FIELDS):
+        raise ValueError("quota changes: a NULL table with n_quota_change > 0")
+    N, Q, FR, R = snap.n_nodes, snap.n_cq, snap.n_fr, snap.n_resource
+    ns, node = a["qc_ns"].astype(np.int64), a["qc_node"].astype(np.int64)
+    nom, bl, ll = (a[k].reshape(-1, FR).astype(np.int64) for k in ("qc_nominal", "qc_borrow_limit", "qc_lend_limit"))
+    if (ns <= snap.now_ns).any():
+        raise ValueError("quota changes: qc_ns at or before now_ns")
+    if (np.diff(ns) < 0).any():
+        raise ValueError("quota changes: qc_ns decreasing")
+    if ((node < 0) | (node >= N)).any():
+        raise ValueError("quota changes: qc_node out of range")
+    if ((nom < 0) | (nom == abi.KB_NO_LIMIT)).any():
+        raise ValueError("quota changes: a negative nominal or KB_NO_LIMIT in a nominal row")
+    if ((bl < 0) | (ll < 0)).any():
+        raise ValueError("quota changes: a negative limit")
+    covered = np.zeros((Q, FR), bool)  # the cells a ClusterQueue's resource groups cover
+    for q in range(Q):
+        for g in range(int(a["cq_rg_start"][q]), int(a["cq_rg_start"][q + 1])):
+            for f in a["rg_flavors"][int(a["rg_flavor_start"][g]):int(a["rg_flavor_start"][g + 1])]:
+                for r in range(R):
+                    if int(a["rg_res_mask"][g]) >> r & 1:
+                        covered[q, int(f) * R + r] = True
+    rows = [a[k].reshape(N, FR) for k in ("nominal", "borrow_limit", "lend_limit")]
+    for i in np.flatnonzero(node < Q):
+        q = int(node[i])
+        for new, old in zip((nom[i], bl[i], ll[i]), rows):
+            if (new[~covered[q]] != old[q][~covered[q]]).any():
+                raise ValueError("quota changes: a ClusterQueue cell its resource groups do not cover")
+
+
+def static_generation_after(base: int, changes: int, n_edits: int) -> int:
+    """kb_snapshot.static_generation of a cycle after `changes` row-changing edits of a drain whose snapshot carries
+    `base`: 0 stays none, otherwise one value per state of the rows that is not 0"""
+    if base == 0 or changes == 0:
+        return base
+    g = base + changes
+    return g if g != 0 else base + n_edits + 1
 
 
 def check_wait_bound_s(base_s: int, max_s: int, limit: int) -> int:
@@ -700,7 +773,9 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     qlen = np.diff(qstart)
     afs_cq = a["cq_afs"].astype(bool) if "wl_lq" in a else np.zeros(Q, bool)
     replay = "adm_wl" in a
-    events = any(k in a for k in abi.EVENT_FIELDS)
+    check_quota_changes(snap)
+    quota = "qc_ns" in a and len(a["qc_ns"]) > 0                  # ClusterQueue / Cohort quota changes
+    events = any(k in a for k in abi.EVENT_FIELDS) or quota
     step = max(1, int(snap.drain_cycle_ns)) if events else 1
     create = a.get("wl_create_ns")
     run_ns = a.get("wl_run_ns")
@@ -886,7 +961,15 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     root = root_of(a["parent"])
     static = {k: v for k, v in a.items() if not (k.startswith(("wl_", "ps_", "adm_")) or k in ("heads", "cq_usage") + abi.AFS_FIELDS +
                                                                                                abi.AFS_DECAY_FIELDS +
-                                                                                               abi.STICKY_FIELDS)}
+                                                                                               abi.STICKY_FIELDS +
+                                                                                               abi.QUOTA_CHANGE_FIELDS)}
+    gen = a["cq_generation"].astype(np.int64).copy()             # AllocatableResourceGeneration (rule 4 of quota changes)
+    static_gen, qc_next, qc_rowed, qc_events = int(snap.static_generation), 0, 0, []
+    if quota:
+        N_ = snap.n_nodes
+        qc_ns, qc_node = a["qc_ns"].astype(np.int64), a["qc_node"].astype(np.int64)
+        qc_rows = [a[k].reshape(-1, FR) for k in ("qc_nominal", "qc_borrow_limit", "qc_lend_limit")]
+        static.update({k: a[k].reshape(N_, FR).astype(np.int64).copy() for k in ("nominal", "borrow_limit", "lend_limit")})
     covers_pods = np.zeros(Q, bool)
     if snap.pods_resource >= 0:
         for q in range(Q):
@@ -976,9 +1059,30 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         admit_cycle[w] = -1
         cursor[seg_of[w]] = min(cursor[seg_of[w]], pos_of[w])
 
+    def apply_quota_changes(t_next, notified):
+        """rules 2-4 of quota changes: the edits due by t_next, in table order, before the verdicts"""
+        nonlocal qc_next, qc_rowed, static_gen
+        while qc_next < len(qc_ns) and int(qc_ns[qc_next]) <= t_next:
+            i, n = qc_next, int(qc_node[qc_next])
+            qc_next += 1
+            qc_events.append(i)
+            keys = ("nominal", "borrow_limit", "lend_limit")
+            if all(np.array_equal(static[k][n], rows[i]) for k, rows in zip(keys, qc_rows)):
+                continue  # no-op: specUpdated is false
+            for k, rows in zip(keys, qc_rows):
+                static[k] = static[k].copy()
+                static[k][n] = rows[i]
+            gen[root[:Q] == root[n]] += 1
+            static["cq_generation"] = gen.copy()
+            notified.add(n)  # its root tree is requeued (requeue_inadmissible maps a node to its root)
+            qc_rowed += 1
+            static_gen = static_generation_after(int(snap.static_generation), qc_rowed, len(qc_ns))
+
     def next_event():
         """earliest pending event after the evictions: a live row's finish or an ABSENT workload's creation (None = none)"""
         e = int(adm_finish.min()) if len(adm_finish) else NEVER
+        if quota and qc_next < len(qc_ns):
+            e = min(e, int(qc_ns[qc_next]))
         if arr_next < len(arr_order):
             e = min(e, int(create[arr_order[arr_next]]))
         if backoff and (state == BACKOFF).any():
@@ -1095,6 +1199,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     def apply_events(t_next, notified):
         """steps 5 and 6 at t_next; returns (finished records, arrived records, records whose eviction completed)"""
         nonlocal arr_next
+        if quota:
+            apply_quota_changes(t_next, notified)
         if checks:
             apply_verdicts(t_next, notified)
         if pr:
@@ -1179,6 +1285,12 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             if res.cycles:
                 res.max_exec_deactivated[-1] = np.concatenate([res.max_exec_deactivated[-1], de])
             exec_events.clear()
+        if quota:
+            qe = np.asarray(qc_events, np.int64)
+            res.n_quota_changes += len(qe)
+            if res.cycles:
+                res.quota_changes[-1] = np.concatenate([res.quota_changes[-1], qe])
+            qc_events.clear()
 
     t = int(snap.now_ns)
     cyc = 0
@@ -1214,7 +1326,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                     heads[e] = w
                     chosen.append(w)
         cs = abi.FlatSnapshot(n_cq=Q, n_cohort=snap.n_cohort, n_flavor=snap.n_flavor, n_resource=R, pods_resource=snap.pods_resource,
-                              flags=snap.flags, now_ns=t, static_generation=snap.static_generation)
+                              flags=snap.flags, now_ns=t, static_generation=static_gen)
         cs.arrays.update(static)
         cs.set("cq_usage", usage)
         for k, v in adm.items():
@@ -1245,6 +1357,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         res.pods_ready_timeout.append(np.zeros(0, np.int64)); res.pods_ready_deactivated.append(np.zeros(0, np.int64))
         res.pods_ready_timeout_at.append(np.zeros((0, 2), np.int64))
         res.max_exec_deactivated.append(np.zeros(0, np.int64))
+        res.quota_changes.append(np.zeros(0, np.int64))
+        res.static_generations.append(static_gen)
         ok = dec == abi.DEC_ASSUMED
         res.admitted.append(heads[ok])
         # ---- apply the admissions: Assignment.Usage (flavorassigner.go:198-218) with the admitted counts
@@ -1349,7 +1463,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 last_gen[w] = -1
                 last = None
             else:
-                last_gen[w] = int(a["cq_generation"][int(a["wl_cq"][w])])
+                last_gen[w] = int(gen[int(a["wl_cq"][w])])  # the current generation (rule 6 of quota changes)
                 last_tried[int(ps_start[w]):int(ps_start[w + 1])] = tried[r0:r1]
                 last = tried[r0:r1]
             # ---- queue movement (cluster_queue.go:362-425,609-633); a StrictFIFO queue keeps its head either way
@@ -1450,6 +1564,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     res.wl_finish_ns = finish_ns
     res.end_ns = t
     res.cq_sticky = sticky
+    if quota:
+        res.cq_generation = gen
     if backoff:
         res.wl_queue_ts = qts
     if backoff or mx:

@@ -359,6 +359,72 @@ def add_max_exec(snap: abi.FlatSnapshot, seed: int = 0, share: float = 0.5, limi
     return snap
 
 
+def _covered_cells(snap: abi.FlatSnapshot) -> np.ndarray:
+    """[n_cq][F*R] the cells a ClusterQueue's resource groups cover"""
+    a, R = snap.arrays, snap.n_resource
+    cov = np.zeros((snap.n_cq, snap.n_fr), bool)
+    for q in range(snap.n_cq):
+        for g in range(int(a["cq_rg_start"][q]), int(a["cq_rg_start"][q + 1])):
+            for f in a["rg_flavors"][int(a["rg_flavor_start"][g]):int(a["rg_flavor_start"][g + 1])]:
+                for r in range(R):
+                    if int(a["rg_res_mask"][g]) >> r & 1:
+                        cov[q, int(f) * R + r] = True
+    return cov
+
+
+def add_quota_changes(snap: abi.FlatSnapshot, seed: int = 0, span_ns: int = 50_000, dip: float = 0.5, lend_share: float = 0.2,
+                      noop_share: float = 0.1, start_ns: int | None = None) -> abi.FlatSnapshot:
+    """Planned ClusterQueue / Cohort quota edits of an event drain (kb_snapshot.qc_*, include/kueue_b200.h), seeded, in
+    (start_ns, start_ns + span_ns] (start_ns defaults to now_ns):
+      - a capacity dip per root tree: at a time t1 the nominal row of every node of the tree with some quota is scaled by
+        `dip` (a ClusterQueue's covered cells only), and at a later t2 restored;
+      - a share `lend_share` of the ClusterQueues with quota get a lending limit of half their nominal quota on their
+        covered cells at one time (KB_NO_LIMIT elsewhere stays);
+      - a share `noop_share` of the nodes get an edit at one time that repeats the rows in force then (no change).
+    The edits are sorted by time (ties keep the order above)."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    a = snap.arrays
+    N, Q, FR = snap.n_nodes, snap.n_cq, snap.n_fr
+    t0 = int(snap.now_ns if start_ns is None else start_ns)
+    snap.finalize()  # the default rows of absent tables
+    rows = [a[k].reshape(N, FR).astype(np.int64).copy() for k in ("nominal", "borrow_limit", "lend_limit")]
+    cov = np.ones((N, FR), bool)
+    cov[:Q] = _covered_cells(snap)
+    parent = a["parent"].astype(np.int64)
+    root = np.arange(N)
+    for _ in range(N):
+        root = np.where(parent[root] >= 0, parent[root], root)
+    plan = []  # (time, kind order, node, kind)
+    for r in np.unique(root):
+        t1, t2 = np.sort(rng.integers(1, span_ns + 1, 2))
+        for n in np.flatnonzero(root == r):
+            if (rows[0][n][cov[n]] > 0).any():
+                plan += [(t0 + int(t1), 0, int(n), "dip"), (t0 + int(t2) + (t2 == t1), 0, int(n), "restore")]
+    for q in range(Q):
+        if (rows[0][q][cov[q]] > 0).any() and rng.random() < lend_share:
+            plan.append((t0 + int(rng.integers(1, span_ns + 1)), 1, q, "lend"))
+    for n in range(N):
+        if rng.random() < noop_share:
+            plan.append((t0 + int(rng.integers(1, span_ns + 1)), 2, n, "noop"))
+    plan.sort(key=lambda e: (e[0], e[1]))
+    base = rows[0].copy()
+    ns, node, out = [], [], [[], [], []]
+    for t, _, n, kind in plan:
+        if kind == "dip":
+            rows[0][n] = np.where(cov[n], (base[n] * dip).astype(np.int64), rows[0][n])
+        elif kind == "restore":
+            rows[0][n] = np.where(cov[n], base[n], rows[0][n])
+        elif kind == "lend":
+            rows[2][n] = np.where(cov[n], rows[0][n] // 2, rows[2][n])
+        ns.append(t); node.append(n)
+        for k in range(3):
+            out[k].append(rows[k][n].copy())
+    snap.set("qc_ns", np.asarray(ns, np.int64)); snap.set("qc_node", np.asarray(node, np.int64))
+    for k, nm in enumerate(("qc_nominal", "qc_borrow_limit", "qc_lend_limit")):
+        snap.set(nm, np.asarray(out[k], np.int64).reshape(len(ns), FR))
+    return snap
+
+
 # The reference's scheduler performance scenario (test/performance/scheduler/configs/baseline/generator.yaml, generated
 # by runner/generator/generator.go): 5 cohorts of 6 ClusterQueues, one flavor, cpu only; per ClusterQueue, workload k of
 # a class is created at (k + 1) * interval and runs `run` once admitted (runner/controller/controller.go).
@@ -373,7 +439,7 @@ _MS = 1_000_000
 
 
 def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None = None, checks: int | None = None,
-                  pods_ready: int | None = None, max_exec: int | None = None) -> abi.FlatSnapshot:
+                  pods_ready: int | None = None, max_exec: int | None = None, quota: int | None = None) -> abi.FlatSnapshot:
     """The baseline scenario as numbers (15,000 workloads at scale 1; `scale` multiplies the count of every class):
     nominal 20 cpu and borrowingLimit 100 cpu per ClusterQueue, preemption reclaimWithinCohort Any and
     withinClusterQueue LowerPriority, BestEffortFIFO.  cpu is in milli-units.  wl_ts is the creation time, an empty
@@ -385,7 +451,9 @@ def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None 
     pods_ready: a seed: WaitForPodsReady on every workload (add_pods_ready: a PodsReady delay of 0-50 ms, 10% of the
     workloads never ready, timeout 100 ms, backoff base 1 s, max 8 s, limit 2).
     max_exec: a seed: MaximumExecutionTimeSeconds (add_max_exec: half of the workloads get a limit of 1 s, and 20% of
-    those start with 0, 1 or 2 s accumulated, so they expire at admission or race their run time of up to 1 s)."""
+    those start with 0, 1 or 2 s accumulated, so they expire at admission or race their run time of up to 1 s).
+    quota: a seed: a capacity dip (add_quota_changes over the scenario's 60 s: each cohort's ClusterQueues drop to half
+    their nominal quota at one time and get it back later, some lending limits, some no-op edits)."""
     Q = PERF_COHORTS * PERF_CQS_PER_COHORT
     snap = abi.FlatSnapshot(n_cq=Q, n_cohort=PERF_COHORTS, n_flavor=1, n_resource=1)
     snap.set("parent", np.concatenate([Q + np.arange(Q) // PERF_CQS_PER_COHORT, np.full(PERF_COHORTS, -1)]))
@@ -421,6 +489,8 @@ def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None 
         add_pods_ready(snap, pods_ready, delay_ns=(0, 50 * _MS), timeout_ns=100 * _MS)
     if max_exec is not None:
         add_max_exec(snap, max_exec, share=0.5, limit_s=(1, 1), spent_share=0.2)
+    if quota is not None:
+        add_quota_changes(snap, quota, span_ns=int(60_000 * scale) * _MS)
     snap.finalize()
     snap.__dict__["perf_class"] = np.asarray(cls, np.int64)
     return snap
