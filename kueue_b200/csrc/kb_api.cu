@@ -112,6 +112,7 @@ struct kb_handle {
   // kb_run_drain: capacity reserved beyond the snapshot's admitted tables, heads chosen on the device
   size_t drain_extra_adm = 0, drain_extra_au = 0; bool drain_mode = false; bool preempt_possible = true;
   bool drain_events = false;  // kb_run_drain in event mode: rows admitted during the drain are preemption candidates
+  size_t out_tgt_capacity = 0;  // kb_run_cycle: the caller's target buffer, a lower bound of the device target pool
   Arena drain_arena; cudaEvent_t ev_d = nullptr;  // kb_run_drain's queue tables, double buffer and scratch
   Arena tas_arena;  // kb_tas_find's inputs, lists and outputs
   bool fused_on = false; size_t fused_smem = 0; bool one_head_per_cq = false; int32_t *d_cq_entry = nullptr;
@@ -861,7 +862,9 @@ static int32_t carve_scratch(kb_handle *h, const kb_snapshot *s) {
     cub::DeviceRadixSort::SortPairs(nullptr, b2, (const u64 *)nullptr, (u64 *)nullptr, (const int32_t *)nullptr, (int32_t *)nullptr, (int)A, 0, 32, h->stream);
     h->rk_temp_bytes = std::max(b1, b2) + 256;
   }
-  const size_t G = p.G, acap = p.acap, ncap = p.ncap, pool_cap = A * 4 + 1024;
+  // the entries' target lists may name the same admitted workload many times (one per entry that preempts it), so the
+  // pool is at least as large as the caller's target buffer
+  const size_t G = p.G, acap = p.acap, ncap = p.ncap, pool_cap = std::max(A * 4 + 1024, h->out_tgt_capacity);
   const size_t nbuckets = (size_t)nroots * FR, sNF = A ? NF : 1, sAU = A ? AUc : 1, tl_cells = h->tree_nodes.size() * (size_t)FR;
   const OutLayout L = out_layout(H, P, (size_t)R);
   auto layout = [&](Arena &a) {
@@ -1334,7 +1337,9 @@ extern "C" int32_t kb_run_cycle(kb_handle *h, const kb_snapshot *s, kb_cycle_out
   static const bool trace = getenv("KB_TRACE") != nullptr;  // host-side phase times of the call on stderr
   auto now = [] { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
   double t0 = trace ? now() : 0, t1 = 0, t2 = 0, t3 = 0;
+  if (h && out) h->out_tgt_capacity = (size_t)std::max(0, out->tgt_capacity);
   int32_t rc = upload_impl(h, s, false);
+  if (h) h->out_tgt_capacity = 0;
   if (rc != KB_OK) return rc;
   if (trace) t1 = now();
   rc = cycle_enqueue(h, !out_is_canonical_block(h, out));
