@@ -435,6 +435,19 @@ typedef struct kb_snapshot {
   const int64_t *qc_nominal;        /* [n_quota_change][F*R] the node's new nominal row                               */
   const int64_t *qc_borrow_limit;   /* [n_quota_change][F*R] its new borrowing-limit row (KB_NO_LIMIT = nil)          */
   const int64_t *qc_lend_limit;     /* [n_quota_change][F*R] its new lending-limit row (KB_NO_LIMIT = nil)            */
+
+  /* ---- workload deactivation and reactivation (optional; read by kb_run_drain only, kb_run_cycle ignores them) ----
+     Planned edits of spec.active (kueuectl stop workload / resume workload), applied on the drain's clock.
+     n_active_change == 0 or ac_ns == NULL: no edits.  Edits turn event mode on; the edits and wl_inactive need adm_wl.
+     See kb_run_drain.  Errors (KB_ERR_INVALID): a NULL table with n_active_change > 0, n_active_change < 0, ac_ns
+     decreasing or <= now_ns, ac_wl outside [0, n_wl), ac_active other than 0 or 1, an edit at or before its record's
+     wl_create_ns, wl_inactive above 4, and an inactive start record that adm_wl names or that is created after now_ns. */
+  int32_t n_active_change;          /* edits below                                                                    */
+  const int64_t *ac_ns;             /* [n_active_change] time of the edit, non-decreasing, each > now_ns              */
+  const int32_t *ac_wl;             /* [n_active_change] pending record                                               */
+  const uint8_t *ac_active;         /* [n_active_change] 0 = set spec.active false (stop), 1 = set it true (resume)   */
+  const uint8_t *wl_inactive;       /* [n_wl] start state: 0 = active, 1-4 = inactive with the reason of the
+                                       deactivation in force (kb_drain_out.wl_deactivation_reason codes); NULL = all 0 */
 } kb_snapshot;
 
 /* ------------------------------------------------------------------------
@@ -740,7 +753,7 @@ int32_t kb_download(kb_handle *h, kb_cycle_out *out);
  *      drain equals the drain without the block in heads, decisions, evictions, usage and per-workload results; only
  *      wl_exec_acc_s_out is new.
  * Deactivations (at an expiry or a release) between the start of cycle c and of c+1 count in
- * cycle_max_exec_deactivated[c].  Not modelled: reactivation (a user action), MultiKueue's handling of the field.
+ * cycle_max_exec_deactivated[c].  Not modelled: MultiKueue's handling of the field.  Reactivation: see below.
  *
  * Quota changes (kb_snapshot.n_quota_change > 0 with every qc_* table; event mode).  Edit i replaces the three quota
  * rows of node qc_node[i] at qc_ns[i].  Additions to the loop:
@@ -762,7 +775,48 @@ int32_t kb_download(kb_handle *h, kb_cycle_out *out);
  * generations after the drain, for the caller to write back.  Resident tables: the drain edits the handle's device
  * copies of nominal / borrow_limit / lend_limit / cq_generation and the tables derived from them, so a kb_run_drain with
  * the block on resets the handle's static generation: the next kb_run_cycle / kb_upload on the handle uploads its
- * static tables again whatever its static_generation. */
+ * static tables again whatever its static_generation.
+ *
+ * Deactivation and reactivation (kb_snapshot.n_active_change > 0 with every ac_* table: event mode; and / or
+ * kb_snapshot.wl_inactive; both need adm_wl).  Edit i sets spec.active of record ac_wl[i] to ac_active[i] at ac_ns[i].
+ * In the reference an Update event that leaves a workload inactive takes the `status == Finished || !active` branch
+ * (workload_controller.go:937-952): queues.DeleteWorkload and, inside QueueAssociatedInadmissibleWorkloadsAfter,
+ * cache.DeleteWorkload at once, whatever the status: a deactivated workload leaves the usage and the preemption
+ * candidates when spec.active turns false, not when its pods are gone.  Additions to the loop:
+ *   1. every edit time is a pending event: E includes the next edit not applied yet, a quiet cycle waits for it, with no
+ *      head the clock jumps to it.  At a boundary t -> t' the edits with ac_ns in (t, t'] are applied in table order.
+ *      A record's edits are ordered in time against its own events (arrival, finish, check verdict, PodsReady timeout,
+ *      expiry, eviction end, RequeueAt); an own event at the time of an edit goes first;
+ *   2. stop, record active and holding no row (QUEUED, SET_ASIDE, BACKOFF): it leaves its queue and is DEACTIVATED
+ *      with reason 4 (Deactivated by a user); RequeueState is cleared (Count 0, no RequeueAt; the inactive branch
+ *      :386-420); a sticky workload clears its ClusterQueue's slot (delete, cluster_queue.go:330-340); its root tree is
+ *      marked for the inadmissible requeue (QueueAssociatedInadmissibleWorkloadsAfter, manager.go:676-697);
+ *   3. stop at d, record active and holding a row in any phase (running, checks under way, waiting for PodsReady,
+ *      evicting): the row's cells leave the usage at d and the row is removed; the root tree is marked; RequeueState is
+ *      cleared and a PodsReady attempt still waiting is dropped, as at an expiry; a check attempt under way is dropped
+ *      (not counted, no failure used); the record is DEACTIVATED with reason 4 and LastAssignment nil.  A row with an
+ *      Admitted time adds int32(Seconds) of t - Admitted to acc (rule 4 of MaximumExecutionTimeSeconds), with t the
+ *      QuotaReserved unset, which comes after the pods terminate (jobframework/reconciler.go:576-590): the end of an
+ *      eviction already under way, else d + wl_evict_ns (d without the table).  acc is not reset (only
+ *      MaximumExecutionTimeExceeded resets it, :635);
+ *   4. stop, record already inactive (whatever its state) or FINISHED: nothing changes; the edit still counts as applied;
+ *   5. resume, record DEACTIVATED (any reason): reason 0, and it joins its queue as an arrival does (PushOrUpdate, the
+ *      NoFit rule of a BestEffortFIFO ClusterQueue included; with AFS in its LocalQueue's segment), with LastAssignment
+ *      nil (queues.DeleteWorkload dropped its queue entry) and Count 0.  wl_check_retries is unchanged, as at every
+ *      eviction the drain replays (resetChecksOnEviction admissionchecks.go:88-109 keeps the RetryCount of a Pending
+ *      check).  A resume on any other record changes nothing: an active one, or one still holding a row while the
+ *      eviction of its deactivation (MaximumExecutionTimeExceeded, RequeuingLimitExceeded) is under way;
+ *   6. the queue-order timestamp does not change: a deactivation sets Evicted(reason Deactivated) only on a workload
+ *      that is not evicted, and GetQueueOrderTimestamp (workload.go:1174-1193) reads creation time for that reason; an
+ *      evicted record keeps its Evicted condition and its timestamp.  A record that rejoins its queue with a timestamp
+ *      other than its sort key re-sorts the queues as a requeue after a backoff does;
+ *   7. start state: a record with wl_inactive 1-4 starts DEACTIVATED with that reason, in no queue, without RequeueAt;
+ *   8. the block composes with eviction latency, the sticky table, admission checks, WaitForPodsReady,
+ *      MaximumExecutionTimeSeconds, quota changes and AFS with or without decay; with no edit and every wl_inactive 0
+ *      the drain equals the drain without the block in every output.
+ * n_stopped / n_resumed count the edits that changed the state (rules 2, 3, 5); those applied between the start of
+ * cycle c and of c+1 count in cycle_stopped[c] / cycle_resumed[c].  wl_deactivated / wl_deactivation_reason describe
+ * the state at the end: 1 and the reason while the record is inactive, 0 after a reactivation. */
 typedef struct kb_drain_out {
   int32_t max_cycles;        /* in */
   int32_t n_cycles;          /* out: cycles run */
@@ -833,11 +887,18 @@ typedef struct kb_drain_out {
   int64_t n_max_exec_deactivated;        /* out: deactivations for MaximumExecutionTimeExceeded, those before cycle 0 included */
   int32_t *cycle_max_exec_deactivated;   /* [max_cycles] deactivations from the start of cycle c to the start of c+1 */
   int32_t *wl_exec_acc_s_out;            /* [n_wl] final accumulatedPastExecutionTimeSeconds, -1 = nil */
-  uint8_t *wl_deactivation_reason;       /* [n_wl] 0 none, 1 Rejected, 2 RequeuingLimitExceeded, 3 MaximumExecutionTimeExceeded */
+  uint8_t *wl_deactivation_reason;       /* [n_wl] 0 none, 1 Rejected, 2 RequeuingLimitExceeded, 3 MaximumExecutionTimeExceeded,
+                                            4 Deactivated by a user (kb_snapshot.ac_*, wl_inactive) */
   /* quota changes (kb_snapshot.n_quota_change > 0; zero / untouched otherwise; each pointer may be NULL) */
   int64_t n_quota_changes;               /* out: edits applied, no-op edits included */
   int32_t *cycle_quota_changes;          /* [max_cycles] edits applied from the start of cycle c to the start of c+1 */
   int64_t *cq_generation;                /* [n_cq] AllocatableResourceGeneration after the drain */
+  /* deactivation and reactivation (kb_snapshot.n_active_change > 0 or wl_inactive; zero / untouched otherwise; each
+     pointer may be NULL).  wl_deactivated and wl_deactivation_reason (4 = Deactivated by a user) are written with it. */
+  int64_t n_stopped;                     /* out: stop edits that deactivated a record, those before cycle 0 included */
+  int64_t n_resumed;                     /* out: resume edits that reactivated a record, likewise */
+  int32_t *cycle_stopped;                /* [max_cycles] stops from the start of cycle c to the start of c+1 */
+  int32_t *cycle_resumed;                /* [max_cycles] resumes, likewise */
 } kb_drain_out;
 int32_t kb_run_drain(kb_handle *h, const kb_snapshot *s, kb_drain_out *out);
 

@@ -389,6 +389,11 @@ func (s *Scheduler) flatten(snap *schdcache.Snapshot, heads []workload.Info, gen
 	// with the node's full rows after the change; kb_drain_out.cq_generation is written back after the drain:
 	//   c.n_quota_change, c.qc_ns, c.qc_node = C.int32_t(len(editNs)), cp64(editNs), cp32(editNode)
 	//   c.qc_nominal, c.qc_borrow_limit, c.qc_lend_limit = cp64(editNominal), cp64(editBorrow), cp64(editLend)
+	// Deactivation and reactivation (INTEGRATION.md): the start state from !workload.IsActive (0 when active, else the
+	// reason of the deactivation in force: 1 Rejected, 2 RequeuingLimitExceeded, 3 MaximumExecutionTimeExceeded, 4 a
+	// user's stop, read from the Evicted condition's reason), and planned stop / resume edits sorted by time:
+	//   c.wl_inactive = cpU8(inactiveReason)
+	//   c.n_active_change, c.ac_ns, c.ac_wl, c.ac_active = C.int32_t(len(acNs)), cp64(acNs), cp32(acWl), cpU8(acActive)
 	// They stay nil here: a single cycle ignores them.
 	if anyGroup { // optional table: NULL when no podset is grouped
 		c.ps_group = cp32(psGroup)

@@ -94,6 +94,8 @@ class kb_snapshot(C.Structure):
         ("wl_max_exec_s", _P(C.c_int32)), ("wl_exec_acc_s", _P(C.c_int32)), ("adm_exec_since_ns", _P(C.c_int64)),
         ("n_quota_change", C.c_int32), ("qc_ns", _P(C.c_int64)), ("qc_node", _P(C.c_int32)), ("qc_nominal", _P(C.c_int64)),
         ("qc_borrow_limit", _P(C.c_int64)), ("qc_lend_limit", _P(C.c_int64)),
+        ("n_active_change", C.c_int32), ("ac_ns", _P(C.c_int64)), ("ac_wl", _P(C.c_int32)), ("ac_active", _P(C.c_uint8)),
+        ("wl_inactive", _P(C.c_uint8)),
     ]
 
 
@@ -155,6 +157,7 @@ class kb_drain_out(C.Structure):
         ("n_max_exec_deactivated", C.c_int64), ("cycle_max_exec_deactivated", _P(C.c_int32)),
         ("wl_exec_acc_s_out", _P(C.c_int32)), ("wl_deactivation_reason", _P(C.c_uint8)),
         ("n_quota_changes", C.c_int64), ("cycle_quota_changes", _P(C.c_int32)), ("cq_generation", _P(C.c_int64)),
+        ("n_stopped", C.c_int64), ("n_resumed", C.c_int64), ("cycle_stopped", _P(C.c_int32)), ("cycle_resumed", _P(C.c_int32)),
     ]
 
 
@@ -217,6 +220,7 @@ _DT = {
     "wl_pods_ready_evict_ns": np.int64, "adm_admitted_ns": np.int64,
     "wl_max_exec_s": np.int32, "wl_exec_acc_s": np.int32, "adm_exec_since_ns": np.int64,
     "qc_ns": np.int64, "qc_node": np.int32, "qc_nominal": np.int64, "qc_borrow_limit": np.int64, "qc_lend_limit": np.int64,
+    "ac_ns": np.int64, "ac_wl": np.int32, "ac_active": np.uint8, "wl_inactive": np.uint8,
 }
 # AdmissionFairSharing tables (include/kueue_b200.h): wl_lq absent = AFS off
 AFS_FIELDS = ("wl_lq", "lq_cq", "cq_afs", "lq_weight", "lq_consumed", "lq_consumed_scale", "lq_penalty", "afs_res_weight",
@@ -237,9 +241,12 @@ PODS_READY_FIELDS = ("wl_pods_ready_ns", "wl_pods_ready_fail", "wl_pods_ready_co
 MAX_EXEC_FIELDS = ("wl_max_exec_s", "wl_exec_acc_s", "adm_exec_since_ns")
 # ClusterQueue / Cohort quota changes in event mode (include/kueue_b200.h): qc_ns absent = off; n_quota_change = len(qc_ns)
 QUOTA_CHANGE_FIELDS = ("qc_ns", "qc_node", "qc_nominal", "qc_borrow_limit", "qc_lend_limit")
+# workload deactivation / reactivation (include/kueue_b200.h): ac_ns present = edits (event mode), n_active_change =
+# len(ac_ns); wl_inactive = the start state
+ACTIVE_FIELDS = ("ac_ns", "ac_wl", "ac_active", "wl_inactive")
 OPTIONAL_FIELDS = (("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows", "adm_wl") + AFS_FIELDS +
                    EVENT_FIELDS + AFS_DECAY_FIELDS + EVICT_END_FIELDS + STICKY_FIELDS + CHECK_FIELDS +
-                   PODS_READY_FIELDS + MAX_EXEC_FIELDS + QUOTA_CHANGE_FIELDS)  # NULL in kb_snapshot when absent
+                   PODS_READY_FIELDS + MAX_EXEC_FIELDS + QUOTA_CHANGE_FIELDS + ACTIVE_FIELDS)  # NULL in kb_snapshot when absent
 ARRAY_FIELDS = list(_DT.keys())
 # tables the library keeps resident while kb_snapshot.static_generation is unchanged (include/kueue_b200.h)
 STATIC_FIELDS = ("parent", "fair_weight", "nominal", "borrow_limit", "lend_limit", "cq_within_cq", "cq_reclaim_within",
@@ -390,6 +397,7 @@ class FlatSnapshot:
         s.n_adm_use = len(self.arrays["adm_use_fr"])
         s.n_usage_delta = len(self.arrays["usage_delta_cq"]) if "usage_delta_cq" in self.arrays else 0
         s.n_quota_change = len(self.arrays["qc_ns"]) if "qc_ns" in self.arrays else 0
+        s.n_active_change = len(self.arrays["ac_ns"]) if "ac_ns" in self.arrays else 0
         s.n_heads = self.n_heads
         s.pods_resource, s.flags, s.now_ns = self.pods_resource, self.flags, self.now_ns
         s.static_generation = self.static_generation
@@ -506,6 +514,8 @@ class DrainOut:
         self.wl_deactivation_reason = np.zeros(W, np.uint8)
         self.cycle_quota_changes = np.zeros(max_cycles, np.int32)  # quota changes (kb_snapshot.qc_*)
         self.cq_generation = np.zeros(max(1, Q), np.int64)[:Q]
+        self.cycle_stopped = np.zeros(max_cycles, np.int32)  # deactivation / reactivation (kb_snapshot.ac_*)
+        self.cycle_resumed = np.zeros(max_cycles, np.int32)
         cap = (min(W * 4 + Q, min(Q, W) * max_cycles) if trace_capacity is None else trace_capacity) if trace else 0
         self.trace_wl = np.zeros(max(1, cap), np.int32)
         self.trace_decision = np.zeros(max(1, cap), np.uint8)
@@ -538,6 +548,8 @@ class DrainOut:
         s.wl_deactivation_reason = _ptr(self.wl_deactivation_reason, C.c_uint8)
         s.cycle_quota_changes = _ptr(self.cycle_quota_changes, C.c_int32)
         s.cq_generation = _ptr(self.cq_generation, C.c_int64)
+        s.cycle_stopped = _ptr(self.cycle_stopped, C.c_int32)
+        s.cycle_resumed = _ptr(self.cycle_resumed, C.c_int32)
         if trace:
             s.trace_wl = _ptr(self.trace_wl, C.c_int32); s.trace_decision = _ptr(self.trace_decision, C.c_uint8)
         s.trace_capacity = cap
@@ -581,6 +593,10 @@ class DrainOut:
     def n_max_exec_deactivated(self): return int(self.struct.n_max_exec_deactivated)
     @property
     def n_quota_changes(self): return int(self.struct.n_quota_changes)
+    @property
+    def n_stopped(self): return int(self.struct.n_stopped)
+    @property
+    def n_resumed(self): return int(self.struct.n_resumed)
 
     def cycles(self):
         """[(heads, decisions)] per cycle from the trace."""

@@ -1361,7 +1361,7 @@ extern "C" int32_t kb_run_cycle(kb_handle *h, const kb_snapshot *s, kb_cycle_out
 // ---------------------------------------------------------------------------
 // what a boundary of kb_run_drain reads back, in the pinned host words [64, 128)
 struct DrainWords {
-  uint32_t counters[KB_DC_QC_HI + 1];   // DrainDev::counters; [0] = heads of the next cycle
+  uint32_t counters[KB_DC_AC_HI + 1];   // DrainDev::counters; [0] = heads of the next cycle
   uint32_t n_new, n_cells;              // this cycle's admissions and their usage cells (the admit scans' totals)
   uint32_t status;                      // the cycle's status word (KBS_AFS_OVERFLOW)
   i64 t_next;                           // event mode: t_{c+1}
@@ -1376,6 +1376,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   out->n_finished = 0; out->n_arrived = 0; out->end_ns = s->now_ns; out->n_evict_done = 0;
   out->n_check_ready = 0; out->n_check_retry = 0; out->n_check_rejected = 0; out->n_resorts = 0; out->resort_ms = 0;
   out->n_pods_ready_timeout = 0; out->n_pods_ready_deactivated = 0; out->n_max_exec_deactivated = 0; out->n_quota_changes = 0;
+  out->n_stopped = 0; out->n_resumed = 0;
   // ---- eviction replay: host-side checks of adm_wl (include/kueue_b200.h)
   const bool replay = s->adm_wl != nullptr;
   if (replay) {
@@ -1392,8 +1393,10 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   }
   // ---- event mode: host-side checks of the arrival and completion tables (include/kueue_b200.h)
   const bool quota = s->n_quota_change > 0 && s->qc_ns;  // ClusterQueue / Cohort quota changes
+  const bool act = s->n_active_change > 0 && s->ac_ns;    // deactivation / reactivation edits
+  const bool blk = act || s->wl_inactive;                 // the block (its start state alone needs no events)
   const bool events = s->wl_create_ns || s->wl_run_ns || s->adm_finish_ns || s->wl_evict_ns || s->wl_check_ns || s->wl_pods_ready_ns ||
-                      s->wl_max_exec_s || quota;
+                      s->wl_max_exec_s || quota || act;
   if (events) {
     if (s->adm_finish_ns)
       for (int a = 0; a < s->n_adm; a++)
@@ -1568,6 +1571,40 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       }
     }
   }
+  // ---- deactivation / reactivation: host-side checks (include/kueue_b200.h), and each edit's neighbours of the same record
+  const int NAC = act ? s->n_active_change : 0;
+  std::vector<int32_t> ac_next, ac_prev;
+  if (s->n_active_change < 0) return fail(h, KB_ERR_INVALID, "active changes: n_active_change < 0");
+  if (s->n_active_change > 0 && (!s->ac_ns || !s->ac_wl || !s->ac_active))
+    return fail(h, KB_ERR_INVALID, "active changes: a NULL table with n_active_change > 0");
+  if (blk) {
+    if (!replay) return fail(h, KB_ERR_INVALID, "active changes: the tables need adm_wl");
+    for (int i = 0; i < NAC; i++) {
+      if (s->ac_ns[i] <= s->now_ns) return fail(h, KB_ERR_INVALID, "active changes: ac_ns at or before now_ns");
+      if (i > 0 && s->ac_ns[i] < s->ac_ns[i - 1]) return fail(h, KB_ERR_INVALID, "active changes: ac_ns decreasing");
+      const int w = s->ac_wl[i];
+      if (w < 0 || w >= W) return fail(h, KB_ERR_INVALID, "active changes: ac_wl out of range");
+      if (s->ac_active[i] > 1) return fail(h, KB_ERR_INVALID, "active changes: ac_active neither 0 nor 1");
+      if (s->wl_create_ns && s->ac_ns[i] <= s->wl_create_ns[w]) return fail(h, KB_ERR_INVALID, "active changes: an edit at or before its record's wl_create_ns");
+    }
+    if (s->wl_inactive) {
+      std::vector<uint8_t> held((size_t)std::max(1, W), 0);
+      for (int a = 0; a < s->n_adm; a++) held[s->adm_wl[a]] = 1;
+      for (int w = 0; w < W; w++) {
+        if (s->wl_inactive[w] > KB_DR_USER) return fail(h, KB_ERR_INVALID, "active changes: wl_inactive above 4");
+        if (!s->wl_inactive[w]) continue;
+        if (held[w]) return fail(h, KB_ERR_INVALID, "active changes: an inactive start record that adm_wl names");
+        if (s->wl_create_ns && s->wl_create_ns[w] > s->now_ns) return fail(h, KB_ERR_INVALID, "active changes: an inactive start record created after now_ns");
+      }
+    }
+    ac_next.assign((size_t)std::max(1, NAC), NAC); ac_prev.assign((size_t)std::max(1, NAC), -1);
+    std::vector<int32_t> last((size_t)std::max(1, W), -1);
+    for (int i = 0; i < NAC; i++) {
+      const int w = s->ac_wl[i];
+      if (last[w] >= 0) { ac_prev[i] = last[w]; ac_next[last[w]] = i; }
+      last[w] = i;
+    }
+  }
   out->n_afs_samples = 0;
   if (Hcap == 0 || max_cycles == 0) return KB_OK;
   size_t extra = (size_t)std::min<long long>((long long)W, (long long)Hcap * max_cycles);
@@ -1648,6 +1685,9 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   i64 *run = nullptr, *create = nullptr, *evict_ns = nullptr, *check_ns = nullptr, *pr_ns = nullptr;
   int32_t *max_exec = nullptr;
   i64 *qc_ns_d = nullptr, *qc_rows_d[3] = {nullptr, nullptr, nullptr};
+  i64 *ac_ns_d = nullptr;
+  int32_t *ac_wl_d = nullptr, *ac_next_d = nullptr, *ac_prev_d = nullptr;
+  uint8_t *ac_on_d = nullptr, *inactive_d = nullptr;
   int32_t *qc_node_d = nullptr, *qc_root_d = nullptr, *qc_tree_d = nullptr, *qc_tree_next_d = nullptr, *qc_cq_start_d = nullptr, *qc_cq_d = nullptr, *qc_blob_gen_d = nullptr;
   DrainDev X{};
   AdmTabs other{};  // compaction: the other half of the admitted tables' double buffer
@@ -1661,7 +1701,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     X.flag = a.take<int32_t>((size_t)Q + 2); X.pos = a.take<int32_t>((size_t)Q + 2);
     X.e_assumed = a.take<int32_t>(Hz + 2); X.e_ncells = a.take<int32_t>(Hz + 2);
     X.e_adm_off = a.take<int32_t>(Hz + 2); X.e_cell_off = a.take<int32_t>(Hz + 2);
-    X.counters = a.take<int32_t>(KB_DC_QC_HI + 1);
+    X.counters = a.take<int32_t>(KB_DC_AC_HI + 1);
     X.wl_admit_cycle = a.take<int32_t>(Wz); X.wl_evals = a.take<int32_t>(Wz); X.wl_last_decision = a.take<uint8_t>(Wz);
     if (trace_cap) { X.trace_wl = a.take<int32_t>(trace_cap); X.trace_dec = a.take<uint8_t>(trace_cap); }
     if (replay || events) {
@@ -1707,10 +1747,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       X.wl_ts0 = a.take<i64>(Wz); X.wl_sort_ts = a.take<i64>(Wz); X.wl_requeue_at = a.take<i64>(Wz);
       X.wl_ready_ns = a.take<i64>(Wz);
     }
-    if (requeue || mx) {  // deactivation reasons and the phase byte of both halves
-      X.wl_deactivated = a.take<uint8_t>(Wz);
-      X.adm_phase = a.take<uint8_t>(Acap); other.phase = a.take<uint8_t>(Acap);
-    }
+    if (requeue || mx || blk) X.wl_deactivated = a.take<uint8_t>(Wz);  // deactivation reasons
+    if (requeue || mx) { X.adm_phase = a.take<uint8_t>(Acap); other.phase = a.take<uint8_t>(Acap); }  // the phase byte of both halves
     if (mx) {  // limits, accumulated times and the Admitted time of both halves
       max_exec = a.take<int32_t>(Wz); X.wl_exec_acc = a.take<int32_t>(Wz);
       X.adm_exec_since = a.take<i64>(Acap); other.since = a.take<i64>(Acap);
@@ -1733,6 +1771,12 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       qc_rows_d[0] = a.take<i64>((size_t)NQC * FR); qc_rows_d[1] = a.take<i64>((size_t)NQC * FR); qc_rows_d[2] = a.take<i64>((size_t)NQC * FR);
       qc_root_d = a.take<int32_t>(NQC); qc_tree_d = a.take<int32_t>(NQC); qc_tree_next_d = a.take<int32_t>(NQC);
       qc_cq_start_d = a.take<int32_t>(nR + 1); qc_cq_d = a.take<int32_t>((size_t)std::max(1, Q)); qc_blob_gen_d = a.take<int32_t>((size_t)std::max(1, Q));
+    }
+    if (s->wl_inactive) inactive_d = a.take<uint8_t>(Wz);
+    if (act) {  // the edits, their neighbours, and the per-record state of a boundary
+      ac_ns_d = a.take<i64>(NAC); ac_wl_d = a.take<int32_t>(NAC); ac_on_d = a.take<uint8_t>(NAC);
+      ac_next_d = a.take<int32_t>(NAC); ac_prev_d = a.take<int32_t>(NAC);
+      X.wl_ac_from = a.take<int32_t>(Wz); X.wl_stop = a.take<i64>(Wz); X.wl_gone = a.take<i64>(Wz);
     }
   };
   if (!h->drain_arena.carve(layout)) return fail(h, KB_ERR_CUDA, "kb_run_drain: cudaMalloc of the drain buffer failed");
@@ -1887,6 +1931,19 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (s->n_adm) CUDA_TRY(h, h2d(h, X.adm_exec_since, s->adm_exec_since_ns, (size_t)s->n_adm * 8));
     if (!requeue) CUDA_TRY(h, cudaMemsetAsync(X.wl_deactivated, 0, Wz, h->stream));  // (k_drain_init_checks clears it otherwise)
   }
+  if (blk) {  // deactivation / reactivation: the start state, the edits
+    if (!requeue && !mx) CUDA_TRY(h, cudaMemsetAsync(X.wl_deactivated, 0, Wz, h->stream));
+    if (inactive_d) CUDA_TRY(h, h2d(h, inactive_d, s->wl_inactive, Wz));
+    if (act) {
+      CUDA_TRY(h, h2d(h, ac_ns_d, s->ac_ns, (size_t)NAC * 8));
+      CUDA_TRY(h, h2d(h, ac_wl_d, s->ac_wl, (size_t)NAC * 4));
+      CUDA_TRY(h, h2d(h, ac_on_d, s->ac_active, (size_t)NAC));
+      CUDA_TRY(h, h2d(h, ac_next_d, ac_next.data(), (size_t)NAC * 4));
+      CUDA_TRY(h, h2d(h, ac_prev_d, ac_prev.data(), (size_t)NAC * 4));
+      CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_STOPPED, 0, 4 * 4, h->stream));  // once: the boundaries never clear them
+      X.ac_ns = ac_ns_d; X.ac_wl = ac_wl_d; X.ac_on = ac_on_d; X.ac_next = ac_next_d; X.ac_prev = ac_prev_d; X.n_ac = NAC;
+    }
+  }
   std::vector<i64> lq_adm;  // decay: the initial admitted usage of every LocalQueue (live rows of the snapshot)
   if (decay) {
     lq_adm.assign(LR, 0);
@@ -1974,10 +2031,11 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   k_drain_init<<<std::max(nbW, (S + tb - 1) / tb), tb, 0, h->stream>>>(D, X, S);
   if (events) k_drain_init_events<<<std::max(1, nbW), tb, 0, h->stream>>>(D, X, create, s->now_ns);
   if (replay || events || sticky) k_drain_init_replay<<<std::max(nbW, (s->n_adm + tb - 1) / tb), tb, 0, h->stream>>>(D, X, replay ? s->n_adm : 0);
-  if (requeue) {  // records in backoff, and the first RequeueAt into clock[2] (k_drain_init_events set clock[0] = now_ns)
-    k_drain_init_checks<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W, s->now_ns);
-    k_drain_backoff<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W);
-  }
+  // records in backoff, records inactive at the start, and the first RequeueAt into clock[2] (k_drain_init_events set
+  // clock[0] = now_ns)
+  if (requeue) k_drain_init_checks<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W, s->now_ns);
+  if (blk) k_drain_init_active<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W, inactive_d);
+  if (requeue) k_drain_backoff<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W);
   k_drain_advance<<<(S + tb - 1) / tb, tb, 0, h->stream>>>(X, S);
   const int nbL = std::max(1, (L + tb - 1) / tb);
   if (decay) {  // the samples due at or before now_ns (k_drain_init_events set clock[0] = now_ns), before the first heads
@@ -2020,6 +2078,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_RESORT, 0, (pr ? 6 : 4) * 4, h->stream));  // once: the boundaries never clear them
   }
   uint32_t exec_seen = 0;  // cumulative MaximumExecutionTimeExceeded deactivations at the previous boundary
+  uint32_t active_seen[2] = {0, 0};  // cumulative stops / resumes, likewise
+  const int nbAc = std::max(1, std::min((NAC + tb - 1) / tb, std::max(1, h->sm_count)));  // grid-stride over a boundary's edits
   if (mx) CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_EXEC_DEACTIVATED, 0, 2 * 4, h->stream));  // once, likewise
   // ---- one boundary per iteration, one synchronisation each (kueue_b200/drain.py): cycle c at t (in event mode, a
   // jump to the next event when there are no heads), its decisions and admissions, the evictions; in event mode E,
@@ -2063,13 +2123,18 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       k_drain_ev_min<<<nbB, tb, 0, h->stream>>>(X, bound, n_new_d);
       k_drain_ev_next<<<1, 1, 0, h->stream>>>(X, t, step, jump, n_new_d);
       if (quota) k_drain_quota<<<1, 1024, 0, h->stream>>>(D, X);  // step 5: the edits, before the verdicts
+      if (act) k_drain_active<<<nbAc, tb, 0, h->stream>>>(D, X, 0);  // the edits of records without a row; the stop times
       if (decay) k_drain_afs_decay<<<nbL, tb, 0, h->stream>>>(D, X, L);  // samples due in (t, t_{c+1}], before the completions
       k_drain_finish<<<nbB, tb, 0, h->stream>>>(D, X, bound, n_new_d);
       if (X.arr_key) k_drain_arrive<<<nbArr, tb, 0, h->stream>>>(X);
+      // the edits of records that met their own events first, before k_drain_backoff folds the remaining RequeueAts
+      // into the next E: a record a timeout or a Retry put in BACKOFF and a later stop deactivated has none
+      if (act) k_drain_active<<<nbAc, tb, 0, h->stream>>>(D, X, 1);
       if (requeue) k_drain_backoff<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W);
     }
     if (compact) {
       k_drain_requeue<<<nbQ, tb, 0, h->stream>>>(D, X);
+      if (act) k_drain_advance<<<(S + tb - 1) / tb, tb, 0, h->stream>>>(X, S);  // a deactivated record may sit at a cursor
       const int nbA = (bound + 1 + tb - 1) / tb;
       k_drain_live<<<nbA, tb, 0, h->stream>>>(X, bound, n_new_d);
       size_t sb = scan_bytes;
@@ -2085,7 +2150,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (!jump) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_new, n_new_d, 4, cudaMemcpyDeviceToHost, h->stream));
     if (!compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_cells, X.e_cell_off + n_live, 4, cudaMemcpyDeviceToHost, h->stream));
     if (afs && (!jump || decay)) CUDA_TRY(h, cudaMemcpyAsync(&hw.status, D.status, 4, cudaMemcpyDeviceToHost, h->stream));
-    if (compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[1], X.counters + 1, (quota ? KB_DC_QC_HI : mx ? KB_DC_EXEC_STATUS : pr ? KB_DC_PR_DEACTIVATED : checks ? KB_DC_CHECK_REJECTED : events ? KB_DC_ARR_HI : KB_DC_FULL) * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[1], X.counters + 1, (act ? KB_DC_AC_HI : quota ? KB_DC_QC_HI : mx ? KB_DC_EXEC_STATUS : pr ? KB_DC_PR_DEACTIVATED : checks ? KB_DC_CHECK_REJECTED : events ? KB_DC_ARR_HI : KB_DC_FULL) * 4, cudaMemcpyDeviceToHost, h->stream));
     if (events) CUDA_TRY(h, cudaMemcpyAsync(&hw.t_next, X.clock, 8, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     if (!jump) {
@@ -2112,6 +2177,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       if (pr && out->cycle_pods_ready_deactivated) out->cycle_pods_ready_deactivated[cyc] = 0;
       if (mx && out->cycle_max_exec_deactivated) out->cycle_max_exec_deactivated[cyc] = 0;
       if (quota && out->cycle_quota_changes) out->cycle_quota_changes[cyc] = 0;
+      if (act && out->cycle_stopped) out->cycle_stopped[cyc] = 0;
+      if (act && out->cycle_resumed) out->cycle_resumed[cyc] = 0;
       out->n_decisions += n_live; out->n_admitted += n_new; out->n_evicted += n_ev;
       out->n_cycles = ++cyc;
     } else {
@@ -2157,6 +2224,16 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       const int qc = (int)(hw.counters[KB_DC_QC_HI] - hw.counters[KB_DC_QC_LO]);
       out->n_quota_changes += qc;
       if (cyc > 0 && out->cycle_quota_changes) out->cycle_quota_changes[cyc - 1] += qc;
+    }
+    if (act) {  // stops / resumes that changed the state at this boundary
+      const uint32_t *cum = &hw.counters[KB_DC_STOPPED];
+      const int st = (int)(cum[0] - active_seen[0]), re = (int)(cum[1] - active_seen[1]);
+      memcpy(active_seen, cum, sizeof(active_seen));
+      out->n_stopped += st; out->n_resumed += re;
+      if (cyc > 0) {
+        if (out->cycle_stopped) out->cycle_stopped[cyc - 1] += st;
+        if (out->cycle_resumed) out->cycle_resumed[cyc - 1] += re;
+      }
     }
     if (lat) {  // evictions completed at this boundary (counter slot 4, inside the events copy)
       const int done = (int)hw.counters[KB_DC_EVICT_DONE];
@@ -2227,8 +2304,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (out->wl_ready_ns) CUDA_TRY(h, cudaMemcpyAsync(out->wl_ready_ns, X.wl_ready_ns, Wz * 8, cudaMemcpyDeviceToHost, h->stream));
     if (out->wl_check_retries_out) CUDA_TRY(h, cudaMemcpyAsync(out->wl_check_retries_out, X.wl_retries, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
   }
-  if ((requeue || mx) && out->wl_deactivated) CUDA_TRY(h, cudaMemcpyAsync(out->wl_deactivated, X.wl_deactivated, Wz, cudaMemcpyDeviceToHost, h->stream));
-  if ((requeue || mx) && out->wl_deactivation_reason)
+  if ((requeue || mx || blk) && out->wl_deactivated) CUDA_TRY(h, cudaMemcpyAsync(out->wl_deactivated, X.wl_deactivated, Wz, cudaMemcpyDeviceToHost, h->stream));
+  if ((requeue || mx || blk) && out->wl_deactivation_reason)
     CUDA_TRY(h, cudaMemcpyAsync(out->wl_deactivation_reason, X.wl_deactivated, Wz, cudaMemcpyDeviceToHost, h->stream));
   if (mx && out->wl_exec_acc_s_out) CUDA_TRY(h, cudaMemcpyAsync(out->wl_exec_acc_s_out, X.wl_exec_acc, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
   if (pr) {
@@ -2245,7 +2322,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     CUDA_TRY(h, cudaMemcpyAsync(out->trace_decision, X.trace_dec, nt, cudaMemcpyDeviceToHost, h->stream));
   }
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  if ((requeue || mx) && out->wl_deactivated)  // the device byte holds the reason (KB_DR_*)
+  if ((requeue || mx || blk) && out->wl_deactivated)  // the device byte holds the reason (KB_DR_*)
     for (int w = 0; w < W; w++) out->wl_deactivated[w] = out->wl_deactivated[w] != 0;
   return KB_OK;
 }

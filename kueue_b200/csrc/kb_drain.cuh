@@ -328,25 +328,35 @@ struct DrainDev {
   const int32_t *qc_cq_start, *qc_cq;  // [nRoots+1] / [Q] the ClusterQueues of every root tree
   const int32_t *qc_blob_gen;      // [Q] byte offset of the ClusterQueue's generation in tree_blob, -1 = not in a tree
   int n_qc;
+  // deactivation / reactivation edits (event mode); ac_ns == nullptr: off.  wl_deactivated holds the reason (KB_DR_*).
+  const i64 *ac_ns;                // [n_ac] edit times, non-decreasing
+  const int32_t *ac_wl;            // [n_ac] record
+  const uint8_t *ac_on;            // [n_ac] 0 = stop, 1 = resume
+  const int32_t *ac_next, *ac_prev;  // [n_ac] the record's next / previous edit (n_ac / -1 = none)
+  int32_t *wl_ac_from;             // [W] the edit a deferred record continues from (values before the boundary: none)
+  i64 *wl_stop;                    // [W] stop time of an active row-holding record at this boundary, INT64_MAX = none
+  i64 *wl_gone;                    // [W] time its row went at this boundary, INT64_MIN = none
+  int n_ac;
 };
 // adm_phase: what the finish column of a row holds.  RUN: its finish (or its eviction's end when adm_evicting); CHECK: its
 // checks' verdict; WAIT: the timeout T of a PodsReady attempt that fails; TIMED_OUT: the end of its eviction by that
 // timeout or by an expiry; EXPIRE: its effective MaximumExecutionTimeSeconds deadline, which comes before its own event
 enum { KB_PH_RUN = 0, KB_PH_CHECK = 1, KB_PH_WAIT = 2, KB_PH_TIMED_OUT = 3, KB_PH_EXPIRE = 4 };
 // wl_deactivated: 0, or the reason a record was deactivated (kb_drain_out.wl_deactivation_reason)
-enum { KB_DR_REJECTED = 1, KB_DR_REQUEUING_LIMIT = 2, KB_DR_MAX_EXEC = 3 };
+enum { KB_DR_REJECTED = 1, KB_DR_REQUEUING_LIMIT = 2, KB_DR_MAX_EXEC = 3, KB_DR_USER = 4 };
 // counters of a boundary: [1] evictions (issued, with latency), [2] / [3] rows / cells after the compaction, [4]
 // evictions completed (latency), [5] capacity flag; event mode: [6] completions, [7] arrivals, [8] end flag, [9] / [10]
 // arrived prefix of arr_order [lo, hi); admission checks: [11] the stamp (cycle + 1) of the last boundary that needs a
 // re-sort, [12] / [13] / [14] Ready / Retry / Rejected verdicts since the start (the host takes differences: no memset);
 // WaitForPodsReady: [15] / [16] timeouts that requeue / deactivate since the start, likewise; MaximumExecutionTimeSeconds:
 // [17] deactivations since the start, [18] KBS_EXEC_OVERFLOW once an accumulated time leaves int32 (never cleared);
-// quota changes: [19] / [20] the edits of this boundary [lo, hi) (hi = edits applied since the start)
+// quota changes: [19] / [20] the edits of this boundary [lo, hi) (hi = edits applied since the start); deactivation:
+// [21] / [22] stops / resumes that changed the state since the start, [23] / [24] the edits of this boundary [lo, hi)
 enum { KB_DC_EVICTED = 1, KB_DC_ROWS = 2, KB_DC_CELLS = 3, KB_DC_EVICT_DONE = 4, KB_DC_FULL = 5,
        KB_DC_FINISHED = 6, KB_DC_ARRIVED = 7, KB_DC_END = 8, KB_DC_ARR_LO = 9, KB_DC_ARR_HI = 10,
        KB_DC_RESORT = 11, KB_DC_CHECK_READY = 12, KB_DC_CHECK_RETRY = 13, KB_DC_CHECK_REJECTED = 14,
        KB_DC_PR_TIMEOUT = 15, KB_DC_PR_DEACTIVATED = 16, KB_DC_EXEC_DEACTIVATED = 17, KB_DC_EXEC_STATUS = 18,
-       KB_DC_QC_LO = 19, KB_DC_QC_HI = 20 };
+       KB_DC_QC_LO = 19, KB_DC_QC_HI = 20, KB_DC_STOPPED = 21, KB_DC_RESUMED = 22, KB_DC_AC_LO = 23, KB_DC_AC_HI = 24 };
 
 __device__ __forceinline__ int drain_seg0(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq] : cq; }
 __device__ __forceinline__ int drain_seg1(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq + 1] : cq + 1; }
@@ -814,6 +824,7 @@ __global__ void k_drain_ev_min(DrainDev X, int bound, const int32_t *n_new) {
   if (a < bound && a < n_rows && X.adm_dead[a] != X.cycle + 1) v = X.adm_finish[a];
   if (a == 0 && X.counters[KB_DC_ARR_HI] < X.n_arr) v = min(v, ev_time(X.arr_key[X.counters[KB_DC_ARR_HI]]));
   if (a == 0 && X.qc_ns && X.counters[KB_DC_QC_HI] < X.n_qc) v = min(v, X.qc_ns[X.counters[KB_DC_QC_HI]]);  // the next edit
+  if (a == 0 && X.ac_ns && X.counters[KB_DC_AC_HI] < X.n_ac) v = min(v, X.ac_ns[X.counters[KB_DC_AC_HI]]);
   for (int o = 16; o > 0; o >>= 1) v = min(v, (i64)__shfl_xor_sync(0xffffffffu, (long long)v, o));
   if ((threadIdx.x & 31) == 0 && v < INT64_MAX) atomicMin((long long *)&X.clock[1], (long long)v);
 }
@@ -843,6 +854,30 @@ __global__ void k_drain_ev_next(DrainDev X, i64 t_c, i64 step, int jump, const i
     while (qlo < qhi) { const int m = qlo + (qhi - qlo) / 2; if (X.qc_ns[m] <= tn) qlo = m + 1; else qhi = m; }
     X.counters[KB_DC_QC_HI] = qlo;
   }
+  if (X.ac_ns) {  // the deactivation / reactivation edits (k_drain_active applies them)
+    int alo = X.counters[KB_DC_AC_HI], ahi = X.n_ac;
+    X.counters[KB_DC_AC_LO] = alo;
+    if (end) ahi = alo;
+    while (alo < ahi) { const int m = alo + (ahi - alo) / 2; if (X.ac_ns[m] <= tn) alo = m + 1; else ahi = m; }
+    X.counters[KB_DC_AC_HI] = alo;
+  }
+}
+// a stop at sd (INT64_MAX = none) of row a's record comes before the row's own event at e while the record is active
+__device__ __forceinline__ bool drain_stop_due(const DrainDev &X, int a, i64 sd, i64 e) {
+  return sd < e && X.wl_deactivated[X.adm_wl[a]] == 0;
+}
+// a stop at d of active record w holding row a (before the row leaves): RequeueState cleared, a waiting PodsReady
+// attempt dropped, the Admitted seconds into acc up to the QuotaReserved unset (the end of an eviction under way, else
+// d + latency), reason KB_DR_USER
+__device__ __forceinline__ void drain_stop_row(const DrainDev &X, int a, int w, i64 d) {
+  X.wl_deactivated[w] = KB_DR_USER;
+  if (X.wl_pr) { X.wl_pr_count[w] = 0; if (X.wl_pr_at[w] > d) X.wl_pr_at[w] = X.wl_pr_prev[w]; }
+  if (X.wl_requeue_at) X.wl_requeue_at[w] = INT64_MIN;
+  if (X.wl_max_exec) {
+    const bool rel = X.adm_evicting && X.adm_evicting[a];
+    drain_exec_release(X, a, w, rel ? X.adm_finish[a] : X.wl_evict ? drain_sat_add(d, X.wl_evict[w]) : d);
+  }
+  X.wl_gone[w] = d;
 }
 // completions (thread per row): a live row with finish <= t_{c+1} gets the dead stamp, its cells leave its ClusterQueue's
 // usage (cache.DeleteWorkload, integer atomics), its record becomes FINISHED and its root tree is marked.  An evicting
@@ -854,10 +889,13 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
   const int a = blockIdx.x * blockDim.x + threadIdx.x;
   if (a >= bound || a >= X.A + (n_new ? *n_new : 0) || X.counters[KB_DC_FULL]) return;
   const int stamp = X.cycle + 1;
-  if (X.counters[KB_DC_END] || X.adm_dead[a] == stamp || X.adm_finish[a] > X.clock[0]) return;
+  if (X.counters[KB_DC_END] || X.adm_dead[a] == stamp) return;
+  const i64 sd = X.wl_stop ? X.wl_stop[X.adm_wl[a]] : INT64_MAX;  // a stop edit of the record at this boundary
+  bool stop = drain_stop_due(X, a, sd, X.adm_finish[a]);
+  if (!stop && X.adm_finish[a] > X.clock[0]) return;
   const int cq = X.adm_cq[a];
   int ph = X.adm_phase ? X.adm_phase[a] : KB_PH_RUN;
-  if (ph == KB_PH_CHECK) {  // a verdict (ProvisioningRequest controller.go:536-580)
+  if (!stop && ph == KB_PH_CHECK) {  // a verdict (ProvisioningRequest controller.go:536-580)
     const int w = X.adm_wl[a];
     const i64 tv = X.adm_finish[a];
     X.adm_phase[a] = KB_PH_RUN;
@@ -868,7 +906,8 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
       if (X.wl_max_exec) { X.adm_exec_since[a] = tv; fin = drain_exec_clip(X, a, w, tv, fin); }
       X.adm_finish[a] = fin;
       atomicAdd(&X.counters[KB_DC_CHECK_READY], 1);
-      if (fin > X.clock[0]) return;
+      stop = drain_stop_due(X, a, sd, fin);
+      if (!stop && fin > X.clock[0]) return;
       ph = X.adm_phase[a];
     } else {  // Retry or Rejected: the workload holds no pods, its quota goes at once
       if (X.wl_fail[w] != INT32_MAX) X.wl_fail[w]--;
@@ -894,7 +933,7 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
     }
   }
   const int w = X.adm_wl[a];
-  if (ph == KB_PH_WAIT) {  // PodsReady timeout at T (workload_controller.go:805-855, UpdateRequeueState workload.go:707-722)
+  if (!stop && ph == KB_PH_WAIT) {  // PodsReady timeout at T (workload_controller.go:805-855, UpdateRequeueState workload.go:707-722)
     const i64 T = X.adm_finish[a];
     if (X.wl_pr_fail[w] > 0 && X.wl_pr_fail[w] != INT32_MAX) X.wl_pr_fail[w]--;
     const int n = X.wl_pr_count[w];
@@ -915,10 +954,11 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
       X.adm_evicted[a] = 1;
       X.adm_evicting[a] = 1;
       X.adm_finish[a] = drain_sat_add(T, X.wl_evict[w]);
-      if (X.adm_finish[a] > X.clock[0]) return;
+      stop = drain_stop_due(X, a, sd, X.adm_finish[a]);
+      if (!stop && X.adm_finish[a] > X.clock[0]) return;
     }
   }
-  if (ph == KB_PH_EXPIRE) {  // MaximumExecutionTimeExceeded at the effective deadline (workload_controller.go:619-646)
+  if (!stop && ph == KB_PH_EXPIRE) {  // MaximumExecutionTimeExceeded at the effective deadline (workload_controller.go:619-646)
     const i64 dl = X.adm_finish[a];
     drain_exec_deactivate(X, w);
     if (X.wl_pr && X.wl_pr_at[w] > dl) X.wl_pr_at[w] = X.wl_pr_prev[w];  // a PodsReady attempt still waiting is dropped
@@ -931,13 +971,16 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
       if (X.adm_finish[a] > X.clock[0]) return;
     }
   }
+  if (stop) drain_stop_row(X, a, w, sd);
+  else if (X.wl_gone) X.wl_gone[w] = X.adm_finish[a];
   X.adm_dead[a] = stamp;
   for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)
     atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
-  const bool timed_out = ph == KB_PH_TIMED_OUT;
-  const bool released = X.adm_evicting && X.adm_evicting[a];
+  const bool timed_out = !stop && ph == KB_PH_TIMED_OUT;
+  const bool released = !stop && X.adm_evicting && X.adm_evicting[a];
   const bool expired = X.wl_max_exec && (timed_out || released) && drain_exec_release(X, a, w, X.adm_finish[a]);
-  if (timed_out || expired) { drain_forget(D, X, w); X.wl_state[w] = X.wl_deactivated[w] ? KB_WS_DEACTIVATED : KB_WS_BACKOFF; }
+  if (stop) { drain_forget(D, X, w); X.wl_state[w] = KB_WS_DEACTIVATED; }
+  else if (timed_out || expired) { drain_forget(D, X, w); X.wl_state[w] = X.wl_deactivated[w] ? KB_WS_DEACTIVATED : KB_WS_BACKOFF; }
   else if (released) drain_release(D, X, w);
   else if (w >= 0) { X.wl_state[w] = KB_WS_FINISHED; X.wl_admit_cycle[w] = -1; X.wl_finish_ns[w] = X.adm_finish[a]; }
   if (X.lq_last && X.adm_lq[a] >= 0 && X.cq_afs[cq]) {  // several rows of one LocalQueue can finish together
@@ -946,7 +989,7 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
       atomicAdd((unsigned long long *)&adm[X.adm_use_fr[c] % D.R], (unsigned long long)(-X.adm_use_qty[c]));
   }
   X.root_mark[D.root_slot[cq]] = stamp;
-  if (!timed_out) atomicAdd(&X.counters[released ? KB_DC_EVICT_DONE : KB_DC_FINISHED], 1);
+  if (!timed_out) atomicAdd(&X.counters[stop ? KB_DC_STOPPED : released ? KB_DC_EVICT_DONE : KB_DC_FINISHED], 1);
 }
 // decay samples (thread per LocalQueue of an AFS ClusterQueue): every sample due in (t, t'] with t' = clock[0], in time
 // order, each with alpha = afs_alpha (one interval elapsed), or a reset to empty with half-life 0; LastUpdate moves to
@@ -1040,6 +1083,82 @@ __global__ void k_drain_quota(DevSnap D, DrainDev X) {
     for (int fr = threadIdx.x; fr < FR; fr += blockDim.x) tl_root_cell(D, sub, lq, t, fr);
     __syncthreads();
   }
+}
+
+// ---- deactivation and reactivation --------------------------------------------------------------------------------------
+// edit j on record w (rules 2, 4 and 5 of kb_run_drain); held: the record holds a row at the edit's time (nothing changes).
+// A stop deactivates an active record without a row; a resume returns a DEACTIVATED record to its queue as an arrival
+// does (NoFit rule included), with LastAssignment nil, and raises the re-sort flag when its queue-order timestamp is not
+// its sort key.  One thread per record: no atomics on the record's state.
+__device__ __forceinline__ void drain_active_edit(const DevSnap &D, const DrainDev &X, int j, int w, bool held) {
+  if (held) return;
+  const uint8_t st = X.wl_state[w];
+  if (X.ac_on[j] == 0) {
+    if (X.wl_deactivated[w] != 0 || (st != KB_WS_QUEUED && st != KB_WS_SET_ASIDE && st != KB_WS_BACKOFF)) return;
+    X.wl_state[w] = KB_WS_DEACTIVATED;
+    X.wl_deactivated[w] = KB_DR_USER;
+    if (X.wl_pr) X.wl_pr_count[w] = 0;
+    if (X.wl_requeue_at) X.wl_requeue_at[w] = INT64_MIN;
+    const int cq = D.wl_cq[w];
+    if (X.cq_sticky && X.cq_sticky[cq] == w) X.cq_sticky[cq] = -1;  // delete (cluster_queue.go:330-340)
+    X.root_mark[D.root_slot[cq]] = X.cycle + 1;
+    drain_forget(D, X, w);
+    atomicAdd(&X.counters[KB_DC_STOPPED], 1);
+  } else if (st == KB_WS_DEACTIVATED) {
+    X.wl_deactivated[w] = 0;
+    drain_forget(D, X, w);
+    const int s = X.wl_seg[w], p = X.wl_pos[w];
+    if (X.class_nofit && X.wl_class[w] >= 0 && X.class_nofit[X.wl_class[w]]) {
+      X.wl_state[w] = KB_WS_SET_ASIDE;
+      atomicMin(&X.first_aside[s], p);
+    } else {
+      X.wl_state[w] = KB_WS_QUEUED;
+      atomicMin(&X.cursor[s], p);
+    }
+    if (X.wl_sort_ts && X.wl_sort_ts[w] != X.wl_qts[w]) X.counters[KB_DC_RESORT] = X.cycle + 1;
+    atomicAdd(&X.counters[KB_DC_RESUMED], 1);
+  }
+}
+// the edits of this boundary [lo, hi), one thread per record (grid-stride over the edits; the record's first edit of the
+// boundary walks its edits in table order).  pass 0, after k_drain_ev_next and before k_drain_finish: the edits of records
+// without a row; a record that is ABSENT or holds a row stops at its edit (wl_ac_from) to meet its own events first, and
+// the first stop of an active row-holding record writes its time to wl_stop for k_drain_finish.  pass 1, after the
+// arrivals and before k_drain_backoff (so a record that its own timeout or Retry put in BACKOFF and a stop then
+// deactivated leaves no RequeueAt in the next E): the deferred edits; an edit before the time the record's row went (wl_gone) met a
+// held record.  It clears wl_stop and wl_gone.
+__global__ void k_drain_active(DevSnap D, DrainDev X, int pass) {
+  const int lo = X.counters[KB_DC_AC_LO], hi = X.counters[KB_DC_AC_HI];
+  for (int i = lo + blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += gridDim.x * blockDim.x) {
+    const int w = X.ac_wl[i];
+    if (pass == 0) {
+      if (X.ac_prev[i] >= lo) continue;
+      for (int j = i; j < hi; j = X.ac_next[j]) {
+        const uint8_t st = X.wl_state[w];
+        const bool inactive = X.wl_deactivated[w] != 0;
+        if (st == KB_WS_ABSENT || (st == KB_WS_HELD && (inactive || X.ac_on[j] == 0))) {
+          if (st == KB_WS_HELD && !inactive) X.wl_stop[w] = X.ac_ns[j];
+          X.wl_ac_from[w] = j;
+          break;
+        }
+        drain_active_edit(D, X, j, w, st == KB_WS_HELD);
+      }
+    } else {
+      if (X.wl_ac_from[w] != i) continue;
+      for (int j = i; j < hi; j = X.ac_next[j]) drain_active_edit(D, X, j, w, X.wl_state[w] == KB_WS_HELD || X.wl_gone[w] > X.ac_ns[j]);
+      X.wl_stop[w] = INT64_MAX; X.wl_gone[w] = INT64_MIN;
+    }
+  }
+}
+// start of a drain with the block: no edit deferred, no stop; records with wl_inactive start DEACTIVATED with its reason,
+// in no queue, without RequeueAt (after k_drain_init_checks, before k_drain_backoff)
+__global__ void k_drain_init_active(DrainDev X, int W, const uint8_t *inactive) {
+  const int w = blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= W) return;
+  if (X.wl_ac_from) { X.wl_ac_from[w] = -1; X.wl_stop[w] = INT64_MAX; X.wl_gone[w] = INT64_MIN; }
+  if (!inactive || !inactive[w]) return;
+  X.wl_state[w] = KB_WS_DEACTIVATED;
+  X.wl_deactivated[w] = inactive[w];
+  if (X.wl_requeue_at) X.wl_requeue_at[w] = INT64_MIN;
 }
 
 // ---- admission checks ------------------------------------------------------------------------------------------------

@@ -280,6 +280,44 @@ specUpdated, clusterqueue_controller.go:384; AddOrUpdateCohort manager.go:251-26
 Every cycle's snapshot carries a static_generation that changes with the rows (`static_generation_after`; 0 stays
 "none"), so an evaluator that keeps static tables resident never reuses old quotas.  Edits applied between the start
 of cycle c and of c+1 are cycle c's (`quota_changes`); `cq_generation` holds the generations after the drain.
+
+Deactivation and reactivation (the snapshot carries `ac_ns`, `ac_wl`, `ac_active` (event mode) and / or `wl_inactive`;
+both need `adm_wl`, include/kueue_b200.h).  Edit i sets spec.active of record ac_wl[i] to ac_active[i] at ac_ns[i]
+(kueuectl stop / resume workload).  An Update that leaves a workload inactive takes the `status == Finished || !active`
+branch (workload_controller.go:937-952): queues.DeleteWorkload and cache.DeleteWorkload at once, whatever the status, so
+the quota goes when spec.active turns false, not when the pods are gone.  Reason 4 (USER) is a deactivation without a
+DeactivationTarget.
+  1. edit times are events (E, the quiet wait, the jump).  At a boundary the edits due are applied in table order per
+     record; a record's own events (arrival, finish, verdict, PodsReady timeout, expiry, eviction end, RequeueAt) at or
+     before an edit's time come first.  `apply_active_first` applies the edits of records that hold no row and are
+     present; a record that is ABSENT or holds a row waits at its edit for `apply_active_rest` (after the row events and
+     arrivals), and the first stop of an active row-holding record sets its stop time d for `apply_row_stops`, which runs
+     before each row phase and stops a row whose next own event comes after d (a tie goes to the own event);
+  2. stop of an active record without a row (QUEUED, SET_ASIDE, BACKOFF): DEACTIVATED, reason USER, RequeueState
+     cleared (Count 0, no RequeueAt; the inactive branch :386-420), the sticky slot cleared (delete, cluster_queue.go:
+     330-340), the root tree marked (QueueAssociatedInadmissibleWorkloadsAfter, manager.go:676-697);
+  3. stop at d of an active record holding a row (running, checks under way, waiting for PodsReady, evicting): the cells
+     leave the usage at d, the row goes, the root tree is marked, RequeueState is cleared, a waiting PodsReady attempt is
+     dropped (as at an expiry), a check attempt under way is dropped (not counted, no failure used), LastAssignment nil,
+     DEACTIVATED with reason USER.  A row with an Admitted time adds exec_seconds(t - A) to acc (`exec_release`): t is the
+     QuotaReserved unset, after the pods terminate (jobframework/reconciler.go:576-590): the end of an eviction under way,
+     else d + wl_evict_ns (d without it).  acc is not reset (only MaximumExecutionTimeExceeded resets it, :635);
+  4. stop of an inactive record (any state) or a FINISHED one: nothing; it counts in `active_changes` only;
+  5. resume of a DEACTIVATED record (any reason): reason 0, LastAssignment nil (its queue entry was deleted), Count 0 (as
+     the deactivation left it), and it joins its queue by step 6 (`enqueue`: the NoFit rule, its LocalQueue's segment).
+     wl_check_retries does not change: resetChecksOnEviction (admissionchecks.go:88-109) keeps a Pending check's
+     RetryCount, and the drain keeps it at every eviction it replays.  A resume of any other record changes nothing:
+     an active one, or one holding a row while the eviction of its deactivation (MaximumExecutionTimeExceeded,
+     RequeuingLimitExceeded) is under way (canonical);
+  6. qts does not change: a deactivation sets Evicted(Deactivated) only on a workload that is not evicted, and
+     GetQueueOrderTimestamp (workload.go:1174-1193) reads the creation time for that reason; an evicted record keeps
+     its condition and timestamp.  A resumed record with a qts other than its sort key re-sorts the queues (`resort`);
+  7. `wl_inactive` 1-4: the record starts DEACTIVATED with that reason, in no queue, without RequeueAt;
+  8. after the inadmissible requeue every cursor moves to its first QUEUED workload (a deactivated record may sit at a
+     cursor or at first_aside);
+  9. with no edit and every wl_inactive 0 the drain equals the drain without the block.
+Edits applied between the start of cycle c and of c+1 are cycle c's (`active_changes`, and `stopped` / `resumed` for
+those that changed the state); wl_deactivated / wl_deactivation_reason describe the state at the end.
 """
 from __future__ import annotations
 
@@ -358,6 +396,14 @@ class DrainResult:
     n_quota_changes: int = 0                                   # those before cycle 0 included (no-op edits too)
     cq_generation: np.ndarray | None = None                    # [n_cq] the generations after the drain
     static_generations: List[int] = field(default_factory=list)  # per cycle: the static_generation its snapshot carried
+    # deactivation / reactivation (ac_ns or wl_inactive in the snapshot; empty / 0 otherwise); wl_deactivated and
+    # wl_deactivation_reason describe the state at the end
+    active_changes: List[np.ndarray] = field(default_factory=list)  # per cycle: indices of the edits applied
+    stopped: List[np.ndarray] = field(default_factory=list)    # per cycle: records a stop deactivated
+    resumed: List[np.ndarray] = field(default_factory=list)    # per cycle: records a resume reactivated
+    n_active_changes: int = 0                                  # edits applied, those before cycle 0 and no-op edits included
+    n_stopped: int = 0
+    n_resumed: int = 0
 
     @property
     def n_evicted(self) -> int:
@@ -414,7 +460,7 @@ ALL_FAIL = np.iinfo(np.int32).max  # wl_check_fail / wl_pods_ready_fail: every a
 # phase of a row (kb_drain.cuh KB_PH_*): its finish column holds the finish, T of a PodsReady attempt, the end of an
 # eviction by a timeout or an expiry, the effective MaximumExecutionTimeSeconds deadline
 RUN, WAIT, TIMED_OUT, EXPIRE = 0, 2, 3, 4
-REJECTED, REQUEUING_LIMIT, MAX_EXEC = 1, 2, 3  # deactivation reasons (kb_drain_out.wl_deactivation_reason)
+REJECTED, REQUEUING_LIMIT, MAX_EXEC, USER = 1, 2, 3, 4  # deactivation reasons (kb_drain_out.wl_deactivation_reason)
 _S = 1_000_000_000
 _I32_MAX = 2**31 - 1
 MAX_BACKOFF_S = 10_000  # below it the reference's jittered, truncated WaitTime is exact
@@ -507,6 +553,37 @@ def check_quota_changes(snap) -> None:
         for new, old in zip((nom[i], bl[i], ll[i]), rows):
             if (new[~covered[q]] != old[q][~covered[q]]).any():
                 raise ValueError("quota changes: a ClusterQueue cell its resource groups do not cover")
+
+
+def check_active_changes(snap) -> None:
+    """the refusals of the deactivation / reactivation tables (kb_run_drain: KB_ERR_INVALID): ValueError"""
+    a = snap.arrays
+    if not any(k in a for k in abi.ACTIVE_FIELDS):
+        return
+    if "adm_wl" not in a:
+        raise ValueError("active changes: the tables need adm_wl")
+    if "ac_ns" in a or "ac_wl" in a or "ac_active" in a:
+        if not all(k in a for k in ("ac_ns", "ac_wl", "ac_active")):
+            raise ValueError("active changes: a NULL table with n_active_change > 0")
+        ns, w, act = (a[k].astype(np.int64) for k in ("ac_ns", "ac_wl", "ac_active"))
+        if (ns <= snap.now_ns).any():
+            raise ValueError("active changes: ac_ns at or before now_ns")
+        if (np.diff(ns) < 0).any():
+            raise ValueError("active changes: ac_ns decreasing")
+        if ((w < 0) | (w >= snap.n_wl)).any():
+            raise ValueError("active changes: ac_wl out of range")
+        if ((act != 0) & (act != 1)).any():
+            raise ValueError("active changes: ac_active neither 0 nor 1")
+        if "wl_create_ns" in a and (ns <= a["wl_create_ns"].astype(np.int64)[w]).any():
+            raise ValueError("active changes: an edit at or before its record's wl_create_ns")
+    if "wl_inactive" in a:
+        ina = a["wl_inactive"].astype(np.int64)
+        if (ina > USER).any():
+            raise ValueError("active changes: wl_inactive above 4")
+        if (ina[a["adm_wl"].astype(np.int64)] != 0).any():
+            raise ValueError("active changes: an inactive start record that adm_wl names")
+        if "wl_create_ns" in a and ((ina != 0) & (a["wl_create_ns"].astype(np.int64) > snap.now_ns)).any():
+            raise ValueError("active changes: an inactive start record created after now_ns")
 
 
 def static_generation_after(base: int, changes: int, n_edits: int) -> int:
@@ -775,7 +852,10 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     replay = "adm_wl" in a
     check_quota_changes(snap)
     quota = "qc_ns" in a and len(a["qc_ns"]) > 0                  # ClusterQueue / Cohort quota changes
-    events = any(k in a for k in abi.EVENT_FIELDS) or quota
+    check_active_changes(snap)
+    act = "ac_ns" in a and len(a["ac_ns"]) > 0                    # deactivation / reactivation edits
+    blk = act or "wl_inactive" in a                               # the block (its start state alone needs no events)
+    events = any(k in a for k in abi.EVENT_FIELDS) or quota or act
     step = max(1, int(snap.drain_cycle_ns)) if events else 1
     create = a.get("wl_create_ns")
     run_ns = a.get("wl_run_ns")
@@ -808,8 +888,14 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             ra = a["wl_requeue_at_ns"].astype(np.int64)
             state[ra > snap.now_ns] = BACKOFF
             requeue_at[ra > snap.now_ns] = ra[ra > snap.now_ns]
-    if backoff or mx:
-        deactivated = np.zeros(snap.n_wl, np.uint8)               # 0, or the reason (REJECTED, REQUEUING_LIMIT, MAX_EXEC)
+    if backoff or mx or blk:
+        deactivated = np.zeros(snap.n_wl, np.uint8)               # 0, or the reason (REJECTED, REQUEUING_LIMIT, MAX_EXEC, USER)
+    if "wl_inactive" in a:  # rule 7 of deactivation: inactive records start DEACTIVATED, in no queue, without RequeueAt
+        ina = a["wl_inactive"].astype(np.uint8)
+        deactivated[ina != 0] = ina[ina != 0]
+        state[ina != 0] = DEACTIVATED
+        if backoff:
+            requeue_at[ina != 0] = UNSET
     if checks:  # rule 1: attempt state; start state of the rows whose checks run
         chk_ns = a["wl_check_ns"].astype(np.int64)
         chk_fail = a["wl_check_fail"].astype(np.int64).copy() if "wl_check_fail" in a else np.zeros(snap.n_wl, np.int64)
@@ -962,7 +1048,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
     static = {k: v for k, v in a.items() if not (k.startswith(("wl_", "ps_", "adm_")) or k in ("heads", "cq_usage") + abi.AFS_FIELDS +
                                                                                                abi.AFS_DECAY_FIELDS +
                                                                                                abi.STICKY_FIELDS +
-                                                                                               abi.QUOTA_CHANGE_FIELDS)}
+                                                                                               abi.QUOTA_CHANGE_FIELDS +
+                                                                                               abi.ACTIVE_FIELDS)}
     gen = a["cq_generation"].astype(np.int64).copy()             # AllocatableResourceGeneration (rule 4 of quota changes)
     static_gen, qc_next, qc_rowed, qc_events = int(snap.static_generation), 0, 0, []
     if quota:
@@ -970,6 +1057,11 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         qc_ns, qc_node = a["qc_ns"].astype(np.int64), a["qc_node"].astype(np.int64)
         qc_rows = [a[k].reshape(-1, FR) for k in ("qc_nominal", "qc_borrow_limit", "qc_lend_limit")]
         static.update({k: a[k].reshape(N_, FR).astype(np.int64).copy() for k in ("nominal", "borrow_limit", "lend_limit")})
+    if act:  # deactivation / reactivation edits; per boundary: the stop times of row-holding records, the edits left for
+        # after the row events and arrivals, the time a deferred record's row went
+        ac_ns, ac_wl, ac_on = (a[k].astype(np.int64) for k in ("ac_ns", "ac_wl", "ac_active"))
+    ac_next, ac_events = 0, {"applied": [], "stopped": [], "resumed": []}
+    stop_at, deferred, row_gone = {}, {}, {}
     covers_pods = np.zeros(Q, bool)
     if snap.pods_resource >= 0:
         for q in range(Q):
@@ -1083,6 +1175,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         e = int(adm_finish.min()) if len(adm_finish) else NEVER
         if quota and qc_next < len(qc_ns):
             e = min(e, int(qc_ns[qc_next]))
+        if act and ac_next < len(ac_ns):
+            e = min(e, int(ac_ns[ac_next]))
         if arr_next < len(arr_order):
             e = min(e, int(create[arr_order[arr_next]]))
         if backoff and (state == BACKOFF).any():
@@ -1097,6 +1191,88 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         else:
             state[w] = QUEUED
             cursor[seg_of[w]] = min(cursor[seg_of[w]], pos_of[w])
+
+    def apply_active_edit(j, w, held, notified):
+        """rules 2, 4 and 5 of deactivation on record w; held: it holds a row at the edit's time (nothing changes)"""
+        if held:
+            return
+        if ac_on[j] == 0:
+            if deactivated[w] == 0 and state[w] in (QUEUED, SET_ASIDE, BACKOFF):  # rule 2
+                state[w] = DEACTIVATED
+                deactivated[w] = USER
+                if pr:
+                    pr_count[w] = 0
+                if backoff:
+                    requeue_at[w] = UNSET
+                q = int(a["wl_cq"][w])
+                if sticky is not None and sticky[q] == w:
+                    sticky[q] = -1
+                notified.add(q)
+                forget(w)
+                ac_events["stopped"].append(w)
+        elif state[w] == DEACTIVATED:  # rule 5: LastAssignment nil, Count 0 since the deactivation
+            deactivated[w] = 0
+            forget(w)
+            enqueue(w)
+            ac_events["resumed"].append(w)
+
+    def apply_active_first(t_next, notified):
+        """rule 1: the edits due by t_next, in table order per record, before the row events.  A record that is ABSENT
+        or holds a row meets its own events first: its edits from there wait for apply_active_rest; the first stop of an
+        active row-holding record sets its stop time (apply_row_stops)"""
+        nonlocal ac_next
+        hi = ac_next
+        while hi < len(ac_ns) and int(ac_ns[hi]) <= t_next:
+            hi += 1
+        by_w = {}
+        for j in range(ac_next, hi):
+            by_w.setdefault(int(ac_wl[j]), []).append(j)
+        ac_events["applied"].extend(range(ac_next, hi))
+        ac_next = hi
+        for w, js in by_w.items():
+            for k, j in enumerate(js):
+                if state[w] == ABSENT or (state[w] == HELD and (deactivated[w] != 0 or ac_on[j] == 0)):
+                    if state[w] == HELD and deactivated[w] == 0:
+                        stop_at[w] = int(ac_ns[j])
+                    deferred[w] = js[k:]
+                    break
+                apply_active_edit(j, w, state[w] == HELD, notified)
+
+    def apply_row_stops(notified):
+        """rule 3: every row of an active record whose stop time comes before the row's next own event"""
+        rows = [row for row in range(len(adm_wl)) if int(adm_wl[row]) in stop_at and deactivated[adm_wl[row]] == 0
+                and stop_at[int(adm_wl[row])] < adm_finish[row]]
+        for row in rows:
+            w = int(adm_wl[row]); d = stop_at[w]
+            deactivated[w] = USER
+            if pr:
+                pr_count[w] = 0
+                if pr_at[w] > d:  # a PodsReady attempt still waiting is dropped
+                    pr_at[w] = pr_prev[w]
+            if backoff:
+                requeue_at[w] = UNSET
+            if mx and exec_since[row] != UNSET:  # QuotaReserved unset once the pods are gone
+                rel = evicting is not None and evicting[row]
+                exec_release(row, w, int(adm_finish[row]) if rel else min(d + int(lat[w]), NEVER) if lat is not None else d)
+            cqi = int(adm["adm_cq"][row])
+            notified.add(cqi)
+            if decay and adm_lq[row] >= 0 and afs_cq[cqi]:
+                for k in range(int(adm["adm_use_start"][row]), int(adm["adm_use_start"][row + 1])):
+                    ladm[adm_lq[row], int(adm["adm_use_fr"][k]) % R] -= int(adm["adm_use_qty"][k])
+            state[w] = DEACTIVATED
+            forget(w)
+            row_gone[w] = d
+            ac_events["stopped"].append(w)
+        if rows:
+            remove_rows(rows)
+
+    def apply_active_rest(notified):
+        """rule 1: the deferred edits after the row events and arrivals; a record whose row went at a time after an
+        edit held it then"""
+        for w, js in deferred.items():
+            for j in js:
+                apply_active_edit(j, w, state[w] == HELD or row_gone.get(w, UNSET) > int(ac_ns[j]), notified)
+        deferred.clear(); stop_at.clear(); row_gone.clear()
 
     def apply_verdicts(t_next, notified):
         """rule 2: the verdicts due by t_next, before the completions"""
@@ -1201,10 +1377,17 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         nonlocal arr_next
         if quota:
             apply_quota_changes(t_next, notified)
+        if act:
+            apply_active_first(t_next, notified)
+            apply_row_stops(notified)
         if checks:
             apply_verdicts(t_next, notified)
+            if act:
+                apply_row_stops(notified)
         if pr:
             apply_timeouts(t_next)
+            if act:
+                apply_row_stops(notified)
         if mx:
             apply_expiries(t_next)
         done = np.flatnonzero(adm_finish <= t_next)
@@ -1217,6 +1400,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 for k in range(int(adm["adm_use_start"][row]), int(adm["adm_use_start"][row + 1])):
                     ladm[adm_lq[row], int(adm["adm_use_fr"][k]) % R] -= int(adm["adm_use_qty"][k])
             w = int(adm_wl[row])
+            if act:
+                row_gone[w] = int(adm_finish[row])
             timed_out = phase is not None and phase[row] == TIMED_OUT
             rel = evicting is not None and evicting[row]
             expired = mx and (timed_out or rel) and exec_release(row, w, int(adm_finish[row]))  # rule 4 (max exec)
@@ -1236,6 +1421,8 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             w = int(arr_order[arr_next]); arr_next += 1
             enqueue(w)
             arr.append(w)
+        if act:  # before the requeue after a backoff: a BACKOFF record's stop and its requeue give the same state
+            apply_active_rest(notified)
         if backoff:  # rule 3: the records whose RequeueAt has come
             for w in np.flatnonzero((state == BACKOFF) & (requeue_at <= t_next)):
                 requeue_at[w] = UNSET
@@ -1291,6 +1478,14 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             if res.cycles:
                 res.quota_changes[-1] = np.concatenate([res.quota_changes[-1], qe])
             qc_events.clear()
+        if blk:
+            ap, st_, re_ = (np.asarray(ac_events[k], np.int64) for k in ("applied", "stopped", "resumed"))
+            res.n_active_changes += len(ap); res.n_stopped += len(st_); res.n_resumed += len(re_)
+            if res.cycles:
+                res.active_changes[-1] = np.concatenate([res.active_changes[-1], ap])
+                res.stopped[-1] = np.concatenate([res.stopped[-1], st_]); res.resumed[-1] = np.concatenate([res.resumed[-1], re_])
+            for v in ac_events.values():
+                v.clear()
 
     t = int(snap.now_ns)
     cyc = 0
@@ -1314,6 +1509,9 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
             after(*apply_events(t, notified))
             if notified:
                 requeue(notified)
+            if act:  # a deactivated record may sit at a cursor or at first_aside: every cursor to its first QUEUED
+                for s in range(len(qlen)):
+                    advance(s)
             resort()
             continue
         segs = hseg[live]
@@ -1358,6 +1556,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         res.pods_ready_timeout_at.append(np.zeros((0, 2), np.int64))
         res.max_exec_deactivated.append(np.zeros(0, np.int64))
         res.quota_changes.append(np.zeros(0, np.int64))
+        res.active_changes.append(np.zeros(0, np.int64)); res.stopped.append(np.zeros(0, np.int64)); res.resumed.append(np.zeros(0, np.int64))
         res.static_generations.append(static_gen)
         ok = dec == abi.DEC_ASSUMED
         res.admitted.append(heads[ok])
@@ -1550,6 +1749,9 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         after(*apply_events(t, notified))
         if notified:
             requeue(notified)
+        if act:
+            for s in range(len(qlen)):
+                advance(s)
         resort()
     res.cq_usage = usage
     res.wl_evictions = evictions
@@ -1568,7 +1770,7 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         res.cq_generation = gen
     if backoff:
         res.wl_queue_ts = qts
-    if backoff or mx:
+    if backoff or mx or blk:
         res.wl_deactivated, res.wl_deactivation_reason = (deactivated != 0).astype(np.uint8), deactivated
     if mx:
         res.wl_exec_acc_s = acc

@@ -425,6 +425,40 @@ def add_quota_changes(snap: abi.FlatSnapshot, seed: int = 0, span_ns: int = 50_0
     return snap
 
 
+def add_active_changes(snap: abi.FlatSnapshot, seed: int = 0, span_ns: int = 50_000, stop_share: float = 0.1,
+                       resume_share: float = 0.5, inactive_share: float = 0.0, start_ns: int | None = None) -> abi.FlatSnapshot:
+    """Stop / resume edits of spec.active for an event drain (kb_snapshot.ac_*, wl_inactive, include/kueue_b200.h),
+    seeded: a share `stop_share` of the records get a stop at a time in (t, t + span_ns] with t the later of start_ns
+    (default now_ns) and its creation, and a share `resume_share` of those a resume at or after it, within span_ns;
+    a share `inactive_share` of the records present at the start that adm_wl does not name start inactive (reason 4).
+    The edits are sorted by time (a stop before a resume at the same time).  An empty adm_wl is added when the
+    snapshot has no admitted rows and no adm_wl."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    a = snap.arrays
+    snap.finalize()
+    W = snap.n_wl
+    if "adm_wl" not in a and snap.n_adm == 0:
+        snap.set("adm_wl", np.zeros(0))
+    t0 = int(snap.now_ns if start_ns is None else start_ns)
+    create = a["wl_create_ns"].astype(np.int64) if "wl_create_ns" in a else np.full(W, np.iinfo(np.int64).min)
+    plan = []  # (time, kind, record)
+    for w in np.flatnonzero(rng.random(W) < stop_share):
+        t = max(t0, int(create[w])) + int(rng.integers(1, span_ns + 1))
+        plan.append((t, 0, int(w)))
+        if rng.random() < resume_share:
+            plan.append((t + int(rng.integers(0, span_ns + 1)), 1, int(w)))
+    plan.sort(key=lambda e: (e[0], e[1]))
+    snap.set("ac_ns", np.asarray([p[0] for p in plan], np.int64))
+    snap.set("ac_wl", np.asarray([p[2] for p in plan], np.int64))
+    snap.set("ac_active", np.asarray([p[1] for p in plan], np.int64))
+    if inactive_share > 0:
+        held = np.zeros(W, bool)
+        held[a["adm_wl"].astype(np.int64)] = True
+        ok = ~held & (create <= snap.now_ns)
+        snap.set("wl_inactive", np.where(ok & (rng.random(W) < inactive_share), 4, 0))
+    return snap
+
+
 # The reference's scheduler performance scenario (test/performance/scheduler/configs/baseline/generator.yaml, generated
 # by runner/generator/generator.go): 5 cohorts of 6 ClusterQueues, one flavor, cpu only; per ClusterQueue, workload k of
 # a class is created at (k + 1) * interval and runs `run` once admitted (runner/controller/controller.go).
@@ -439,7 +473,8 @@ _MS = 1_000_000
 
 
 def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None = None, checks: int | None = None,
-                  pods_ready: int | None = None, max_exec: int | None = None, quota: int | None = None) -> abi.FlatSnapshot:
+                  pods_ready: int | None = None, max_exec: int | None = None, quota: int | None = None,
+                  active: int | None = None) -> abi.FlatSnapshot:
     """The baseline scenario as numbers (15,000 workloads at scale 1; `scale` multiplies the count of every class):
     nominal 20 cpu and borrowingLimit 100 cpu per ClusterQueue, preemption reclaimWithinCohort Any and
     withinClusterQueue LowerPriority, BestEffortFIFO.  cpu is in milli-units.  wl_ts is the creation time, an empty
@@ -453,7 +488,9 @@ def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None 
     max_exec: a seed: MaximumExecutionTimeSeconds (add_max_exec: half of the workloads get a limit of 1 s, and 20% of
     those start with 0, 1 or 2 s accumulated, so they expire at admission or race their run time of up to 1 s).
     quota: a seed: a capacity dip (add_quota_changes over the scenario's 60 s: each cohort's ClusterQueues drop to half
-    their nominal quota at one time and get it back later, some lending limits, some no-op edits)."""
+    their nominal quota at one time and get it back later, some lending limits, some no-op edits).
+    active: a seed: stop / resume edits (add_active_changes over the scenario's 60 s: 5% of the workloads are stopped
+    once, half of those resumed later)."""
     Q = PERF_COHORTS * PERF_CQS_PER_COHORT
     snap = abi.FlatSnapshot(n_cq=Q, n_cohort=PERF_COHORTS, n_flavor=1, n_resource=1)
     snap.set("parent", np.concatenate([Q + np.arange(Q) // PERF_CQS_PER_COHORT, np.full(PERF_COHORTS, -1)]))
@@ -491,6 +528,8 @@ def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None 
         add_max_exec(snap, max_exec, share=0.5, limit_s=(1, 1), spent_share=0.2)
     if quota is not None:
         add_quota_changes(snap, quota, span_ns=int(60_000 * scale) * _MS)
+    if active is not None:
+        add_active_changes(snap, active, span_ns=int(60_000 * scale) * _MS, stop_share=0.05)
     snap.finalize()
     snap.__dict__["perf_class"] = np.asarray(cls, np.int64)
     return snap
