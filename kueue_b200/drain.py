@@ -824,201 +824,304 @@ def _queue_order(a, Q, ts=None):
     return order, np.cumsum(start), seg_start, seg_lq
 
 
+_ADM_ROW_KEYS = ("adm_cq", "adm_priority", "adm_ts", "adm_qr_ts", "adm_uid", "adm_evicted")
+_ADM_KEYS = _ADM_ROW_KEYS + ("adm_use_start", "adm_use_fr", "adm_use_qty")
+# DrainResult's per-cycle event lists (`_Drain.log`); each has its total n_<name> but pods_ready_timeout_at, the [n, 2]
+# times beside pods_ready_timeout
+_EVENT_LISTS = ("finished", "arrived", "evict_done", "check_retry", "check_rejected", "pods_ready_timeout",
+                "pods_ready_timeout_at", "pods_ready_deactivated", "max_exec_deactivated", "quota_changes", "active_changes",
+                "stopped", "resumed")
+
+
+class _Rows:
+    """The admitted tables of a drain.  `adm` holds the snapshot's columns (the cells of row i are adm_use_start[i] ..
+    adm_use_start[i + 1]); every block the snapshot carries adds a column (None otherwise), exported under its key:
+      wl        the pending record, -1 = a row of an event snapshot without adm_wl     adm_wl
+      finish    the finish column: the next event of the row (see RUN .. EXPIRE)       adm_finish_ns
+      evicting  an eviction is under way (eviction latency)                            adm_evicting
+      since     the Admitted time, UNSET = none (MaximumExecutionTimeSeconds)          adm_exec_since_ns
+      checking  the admission checks run                                               adm_checking
+      phase     RUN / WAIT / TIMED_OUT / EXPIRE (WaitForPodsReady, max exec)           adm_pods_ready_phase
+      lq        the LocalQueue (decay of consumed usage)                               -
+    Rows join and leave only through `append` and `remove`, which move their cells in and out of the ClusterQueue usage
+    (cache.AddWorkload / DeleteWorkload) and keep every column aligned."""
+    COLUMNS = {"wl": "adm_wl", "finish": "adm_finish_ns", "evicting": "adm_evicting", "since": "adm_exec_since_ns",
+               "checking": "adm_checking", "phase": "adm_pods_ready_phase", "lq": None}
+
+    def __init__(self, a, usage):
+        self.adm = {k: a[k].copy() for k in _ADM_KEYS}
+        self.usage = usage
+        self.wl = self.finish = self.evicting = self.since = self.checking = self.phase = self.lq = None
+
+    def _columns(self):
+        return [c for c in self.COLUMNS if getattr(self, c) is not None]
+
+    def append(self, cells, **cols):
+        """new rows at the end: `cells` holds one {flavor-resource: quantity} per row, `cols` the new rows' values of
+        every snapshot column but the cells and of every block column"""
+        adm, usage = self.adm, self.usage
+        start, fr, qty = [int(adm["adm_use_start"][-1])], [], []
+        for cqi, row_cells in zip(cols["adm_cq"], cells):
+            for f, q in row_cells.items():
+                usage[int(cqi), f] += q
+                fr.append(f); qty.append(q)
+            start.append(start[-1] + len(row_cells))
+        cols.update(adm_use_start=np.asarray(start[1:], np.int32), adm_use_fr=np.asarray(fr, np.int32),
+                    adm_use_qty=np.asarray(qty, np.int64))
+        for k in _ADM_KEYS:
+            adm[k] = np.concatenate([adm[k], cols[k]])
+        for c in self._columns():
+            setattr(self, c, np.concatenate([getattr(self, c), cols[c]]))
+
+    def remove(self, rows):
+        """rows leave the tables; the other rows keep their order"""
+        adm, usage = self.adm, self.usage
+        us, uf, uq = adm["adm_use_start"], adm["adm_use_fr"], adm["adm_use_qty"]
+        for row in rows:
+            cqi = int(adm["adm_cq"][row])
+            for k in range(int(us[row]), int(us[row + 1])):
+                usage[cqi, int(uf[k])] -= int(uq[k])
+        keep = np.ones(len(adm["adm_cq"]), bool)
+        keep[rows] = False
+        cnt = np.diff(us.astype(np.int64))
+        cell_keep = np.repeat(keep, cnt)
+        for k in _ADM_ROW_KEYS:
+            adm[k] = adm[k][keep]
+        adm["adm_use_fr"], adm["adm_use_qty"] = uf[cell_keep], uq[cell_keep]
+        adm["adm_use_start"] = np.concatenate([[0], np.cumsum(cnt[keep])]).astype(np.int32)
+        for c in self._columns():
+            setattr(self, c, getattr(self, c)[keep])
+
+    def export(self, hide=()):
+        """DrainResult.adm: the snapshot's columns, then every block column but those in `hide` under its key"""
+        out = dict(self.adm)
+        for c, key in self.COLUMNS.items():
+            if key is not None and c not in hide and getattr(self, c) is not None:
+                out[key] = getattr(self, c)
+        return out
+
+
 def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.CycleOut], max_cycles: int = 10_000) -> DrainResult:
-    a = snap.arrays
-    Q, R, FR = snap.n_cq, snap.n_resource, snap.n_fr
-    checks = "wl_check_ns" in a
-    pr = "wl_pods_ready_ns" in a                                  # WaitForPodsReady
-    backoff = checks or pr                                        # BACKOFF / DEACTIVATED, RequeueAt, mutable qts
-    mx = "wl_max_exec_s" in a                                     # MaximumExecutionTimeSeconds
-    if mx and "adm_wl" not in a:
-        raise ValueError("wl_max_exec_s needs adm_wl")
-    qts = a["wl_ts"].astype(np.int64).copy()                      # queue-order timestamps (checks, PodsReady: mutable)
-    if backoff:
-        if "adm_wl" not in a:
-            raise ValueError("wl_check_ns / wl_pods_ready_ns need adm_wl")
-        held0 = np.zeros(snap.n_wl, bool)
-        held0[a["adm_wl"].astype(np.int64)] = True
-        if "wl_check_evict_ns" in a:
-            ce = a["wl_check_evict_ns"].astype(np.int64)
-            qts = np.where((ce != UNSET) & ~held0, ce, qts)
-        if pr and "wl_pods_ready_evict_ns" in a and not snap.pods_ready_requeue_creation:  # rule 7 (Eviction timestamp)
-            pe = a["wl_pods_ready_evict_ns"].astype(np.int64)
-            qts = np.where(pe != UNSET, pe, qts)
-    order, qstart, seg_start, seg_lq = _queue_order(a, Q, qts)
-    sort_ts = qts.copy()                                          # the keys the order was built with
-    qlen = np.diff(qstart)
-    afs_cq = a["cq_afs"].astype(bool) if "wl_lq" in a else np.zeros(Q, bool)
-    replay = "adm_wl" in a
-    check_quota_changes(snap)
-    quota = "qc_ns" in a and len(a["qc_ns"]) > 0                  # ClusterQueue / Cohort quota changes
-    check_active_changes(snap)
-    act = "ac_ns" in a and len(a["ac_ns"]) > 0                    # deactivation / reactivation edits
-    blk = act or "wl_inactive" in a                               # the block (its start state alone needs no events)
-    events = any(k in a for k in abi.EVENT_FIELDS) or quota or act
-    step = max(1, int(snap.drain_cycle_ns)) if events else 1
-    create = a.get("wl_create_ns")
-    run_ns = a.get("wl_run_ns")
-    lat = a.get("wl_evict_ns")  # eviction latency: issue at t_c, release at the end time
-    if lat is not None and not replay:
-        raise ValueError("wl_evict_ns needs adm_wl")
-    evicting = None                                               # [rows] the row's eviction is under way (latency)
-    state = np.full(snap.n_wl, QUEUED, np.uint8)
-    seg_of = np.zeros(snap.n_wl, np.int64)                        # segment of every pending workload
-    pos_of = np.zeros(snap.n_wl, np.int64)                        # its position in the segment's static order
-    for s in range(len(qlen)):
-        seg_of[order[qstart[s]:qstart[s + 1]]] = s
-        pos_of[order[qstart[s]:qstart[s + 1]]] = np.arange(qlen[s])
-    adm_wl = a["adm_wl"].astype(np.int64).copy() if replay else None
-    if events:  # the record of every row (-1: a row of the snapshot without adm_wl) and its finish time
-        adm_wl = adm_wl if replay else np.full(snap.n_adm, -1, np.int64)
-        adm_finish = a["adm_finish_ns"].astype(np.int64).copy() if "adm_finish_ns" in a else np.full(snap.n_adm, NEVER, np.int64)
-        if create is not None:
-            state[create > snap.now_ns] = ABSENT
-        if lat is not None:
-            evicting = np.zeros(snap.n_adm, bool)
-            if "adm_evict_end_ns" in a:  # evictions under way before the drain complete at their end time
-                evicting = a["adm_evicted"].astype(bool).copy()
-                adm_finish[evicting] = a["adm_evict_end_ns"][evicting]
-    if replay:
-        state[a["adm_wl"].astype(np.int64)] = HELD  # holds quota: out of every queue
-    if backoff:  # records in backoff at the start
-        requeue_at = np.full(snap.n_wl, UNSET, np.int64)
-        if "wl_requeue_at_ns" in a:
+    return _Drain(snap).run(run_cycle, max_cycles)
+
+
+class _Drain:
+    """The state of one drain: the queues, the records, the admitted tables (`rows`) and the blocks the snapshot
+    carries.  The methods named in the module docstring are its rules; `run` iterates the cycles and the boundaries."""
+
+    def __init__(self, snap: abi.FlatSnapshot):
+        self.snap = snap
+        a = self.a = snap.arrays
+        Q, R, FR = self.Q, self.R, self.FR = snap.n_cq, snap.n_resource, snap.n_fr
+        W = snap.n_wl
+        checks = self.checks = "wl_check_ns" in a
+        pr = self.pr = "wl_pods_ready_ns" in a                         # WaitForPodsReady
+        backoff = self.backoff = checks or pr                          # BACKOFF / DEACTIVATED, RequeueAt, mutable qts
+        mx = self.mx = "wl_max_exec_s" in a                            # MaximumExecutionTimeSeconds
+        if mx and "adm_wl" not in a:
+            raise ValueError("wl_max_exec_s needs adm_wl")
+        qts = self.qts = a["wl_ts"].astype(np.int64).copy()            # queue-order timestamps (checks, PodsReady: mutable)
+        if backoff:
+            if "adm_wl" not in a:
+                raise ValueError("wl_check_ns / wl_pods_ready_ns need adm_wl")
+            held0 = np.zeros(W, bool)
+            held0[a["adm_wl"].astype(np.int64)] = True
+            if "wl_check_evict_ns" in a:
+                ce = a["wl_check_evict_ns"].astype(np.int64)
+                qts[:] = np.where((ce != UNSET) & ~held0, ce, qts)
+            if pr and "wl_pods_ready_evict_ns" in a and not snap.pods_ready_requeue_creation:  # rule 7 (Eviction timestamp)
+                pe = a["wl_pods_ready_evict_ns"].astype(np.int64)
+                qts[:] = np.where(pe != UNSET, pe, qts)
+        self.order, self.qstart, seg_start, self.seg_lq = _queue_order(a, Q, qts)
+        self.seg_start = seg_start
+        self.sort_ts = qts.copy()                                      # the keys the order was built with
+        qlen = self.qlen = np.diff(self.qstart)
+        afs_cq = self.afs_cq = a["cq_afs"].astype(bool) if "wl_lq" in a else np.zeros(Q, bool)
+        replay = self.replay = "adm_wl" in a
+        check_quota_changes(snap)
+        quota = self.quota = "qc_ns" in a and len(a["qc_ns"]) > 0     # ClusterQueue / Cohort quota changes
+        check_active_changes(snap)
+        act = self.act = "ac_ns" in a and len(a["ac_ns"]) > 0         # deactivation / reactivation edits
+        self.blk = act or "wl_inactive" in a                           # the block (its start state alone needs no events)
+        events = self.events = any(k in a for k in abi.EVENT_FIELDS) or quota or act
+        self.step = max(1, int(snap.drain_cycle_ns)) if events else 1
+        create = self.create = a.get("wl_create_ns")
+        self.run_ns = a.get("wl_run_ns")
+        lat = self.lat = a.get("wl_evict_ns")  # eviction latency: issue at t_c, release at the end time
+        if lat is not None and not replay:
+            raise ValueError("wl_evict_ns needs adm_wl")
+        state = self.state = np.full(W, QUEUED, np.uint8)
+        self.seg_of = np.zeros(W, np.int64)                            # segment of every pending workload
+        self.pos_of = np.zeros(W, np.int64)                            # its position in the segment's static order
+        self.index_segments()
+        self.usage = a["cq_usage"].reshape(Q, FR).astype(np.int64).copy()
+        rows = self.rows = _Rows(a, self.usage)
+        self.res = DrainResult()
+        if replay:
+            rows.wl = a["adm_wl"].astype(np.int64).copy()
+        if events:  # the record of every row (-1: a row of the snapshot without adm_wl) and its finish time
+            if not replay:
+                rows.wl = np.full(snap.n_adm, -1, np.int64)
+            rows.finish = a["adm_finish_ns"].astype(np.int64).copy() if "adm_finish_ns" in a else np.full(snap.n_adm, NEVER, np.int64)
+            if create is not None:
+                state[create > snap.now_ns] = ABSENT
+            if lat is not None:
+                rows.evicting = np.zeros(snap.n_adm, bool)
+                if "adm_evict_end_ns" in a:  # evictions under way before the drain complete at their end time
+                    rows.evicting = a["adm_evicted"].astype(bool).copy()
+                    rows.finish[rows.evicting] = a["adm_evict_end_ns"][rows.evicting]
+        if replay:
+            state[a["adm_wl"].astype(np.int64)] = HELD  # holds quota: out of every queue
+        self.requeue_at = np.full(W, UNSET, np.int64)                  # RequeueAt of a BACKOFF record
+        if backoff and "wl_requeue_at_ns" in a:  # records in backoff at the start
             ra = a["wl_requeue_at_ns"].astype(np.int64)
             state[ra > snap.now_ns] = BACKOFF
-            requeue_at[ra > snap.now_ns] = ra[ra > snap.now_ns]
-    if backoff or mx or blk:
-        deactivated = np.zeros(snap.n_wl, np.uint8)               # 0, or the reason (REJECTED, REQUEUING_LIMIT, MAX_EXEC, USER)
-    if "wl_inactive" in a:  # rule 7 of deactivation: inactive records start DEACTIVATED, in no queue, without RequeueAt
-        ina = a["wl_inactive"].astype(np.uint8)
-        deactivated[ina != 0] = ina[ina != 0]
-        state[ina != 0] = DEACTIVATED
-        if backoff:
-            requeue_at[ina != 0] = UNSET
-    if checks:  # rule 1: attempt state; start state of the rows whose checks run
-        chk_ns = a["wl_check_ns"].astype(np.int64)
-        chk_fail = a["wl_check_fail"].astype(np.int64).copy() if "wl_check_fail" in a else np.zeros(snap.n_wl, np.int64)
-        retries = a["wl_check_retries"].astype(np.int64).copy() if "wl_check_retries" in a else np.zeros(snap.n_wl, np.int64)
-        checking = np.zeros(snap.n_adm, bool)
-        if "adm_check_end_ns" in a:
-            ce = a["adm_check_end_ns"].astype(np.int64)
-            checking = ce != UNSET
-            adm_finish[checking] = ce[checking]
-        ready_ns = np.full(snap.n_wl, UNSET, np.int64)
-        base_s, max_s, limit = int(snap.check_backoff_base_s), int(snap.check_backoff_max_s), int(snap.check_backoff_limit)
-        verdicts = {"ready": 0, "retry": [], "rejected": []}
-    else:
-        checking = None
-    phase = None                                                  # [rows] RUN / WAIT / TIMED_OUT / EXPIRE
-    if pr:  # rules 2 and 7: attempt state, and the rows whose pods are not ready at the start
-        pr_ns = a["wl_pods_ready_ns"].astype(np.int64)
-        pr_fail = a["wl_pods_ready_fail"].astype(np.int64).copy() if "wl_pods_ready_fail" in a else np.zeros(snap.n_wl, np.int64)
-        pr_count = a["wl_pods_ready_count"].astype(np.int64).copy() if "wl_pods_ready_count" in a else np.zeros(snap.n_wl, np.int64)
-        pr_at = np.full(snap.n_wl, UNSET, np.int64)               # last PodsReady time
-        pr_prev = pr_at.copy()                                    # its value before the attempt under way
-        pr_timeout = int(snap.pods_ready_timeout_ns)
-        pr_base, pr_max, pr_limit = int(snap.pods_ready_backoff_base_s), int(snap.pods_ready_backoff_max_s), int(snap.pods_ready_backoff_limit)
-        pr_creation = bool(snap.pods_ready_requeue_creation)
-        timeouts = {"timeout": [], "at": [], "deactivated": []}
+            self.requeue_at[ra > snap.now_ns] = ra[ra > snap.now_ns]
+        deactivated = self.deactivated = np.zeros(W, np.uint8)        # 0, or the reason (REJECTED, REQUEUING_LIMIT, MAX_EXEC, USER)
+        if "wl_inactive" in a:  # rule 7 of deactivation: inactive records start DEACTIVATED, in no queue, without RequeueAt
+            ina = a["wl_inactive"].astype(np.uint8)
+            deactivated[ina != 0] = ina[ina != 0]
+            state[ina != 0] = DEACTIVATED
+            self.requeue_at[ina != 0] = UNSET
+        if checks:  # rule 1: attempt state; start state of the rows whose checks run
+            self.chk_ns = a["wl_check_ns"].astype(np.int64)
+            self.chk_fail = a["wl_check_fail"].astype(np.int64).copy() if "wl_check_fail" in a else np.zeros(W, np.int64)
+            self.retries = a["wl_check_retries"].astype(np.int64).copy() if "wl_check_retries" in a else np.zeros(W, np.int64)
+            rows.checking = np.zeros(snap.n_adm, bool)
+            if "adm_check_end_ns" in a:
+                ce = a["adm_check_end_ns"].astype(np.int64)
+                rows.checking = ce != UNSET
+                rows.finish[rows.checking] = ce[rows.checking]
+            self.ready_ns = np.full(W, UNSET, np.int64)
+        if pr or mx:
+            rows.phase = np.full(snap.n_adm, RUN, np.int64)
+        if pr:  # rules 2 and 7: attempt state, and the rows whose pods are not ready at the start
+            self.pr_ns = a["wl_pods_ready_ns"].astype(np.int64)
+            self.pr_fail = a["wl_pods_ready_fail"].astype(np.int64).copy() if "wl_pods_ready_fail" in a else np.zeros(W, np.int64)
+            self.pr_count = a["wl_pods_ready_count"].astype(np.int64).copy() if "wl_pods_ready_count" in a else np.zeros(W, np.int64)
+            self.pr_at = np.full(W, UNSET, np.int64)                   # last PodsReady time
+            self.pr_prev = self.pr_at.copy()                           # its value before the attempt under way
+            if "adm_admitted_ns" in a:
+                for row in np.flatnonzero(a["adm_admitted_ns"] != UNSET):
+                    rows.finish[row], rows.phase[row] = self.pr_attempt(int(rows.wl[row]), int(a["adm_admitted_ns"][row]))
+        if mx:  # rule 1: limits, accumulated times, the Admitted time of every row; the start rows' effective deadlines
+            self.exec_max = a["wl_max_exec_s"].astype(np.int64)
+            self.acc = a["wl_exec_acc_s"].astype(np.int64).copy() if "wl_exec_acc_s" in a else np.full(W, -1, np.int64)
+            if snap.n_adm and "adm_exec_since_ns" not in a:
+                raise ValueError("wl_max_exec_s needs adm_exec_since_ns when the snapshot has admitted rows")
+            rows.since = a["adm_exec_since_ns"].astype(np.int64).copy() if snap.n_adm else np.zeros(0, np.int64)
+            for row in range(snap.n_adm):
+                if rows.since[row] == UNSET or (rows.evicting is not None and rows.evicting[row]):
+                    continue
+                rows.finish[row], e = self.exec_clip(int(rows.wl[row]), int(rows.since[row]), int(rows.finish[row]), int(snap.now_ns))
+                if e:
+                    rows.phase[row] = EXPIRE
+        self.sticky = a["cq_sticky"].astype(np.int64).copy() if "cq_sticky" in a else None  # sticky workload per ClusterQueue
+        self.cursor = np.zeros(len(qlen), np.int64)
+        self.first_aside = qlen.copy()                                 # smallest SET_ASIDE position per segment (qlen = none)
+        self.nofit = NoFitSets()
+        for s in range(len(qlen)):
+            self.advance(s)
+        decay = self.decay = events and "wl_lq" in a and "lq_last_update_ns" in a
+        if afs_cq.any() or decay:
+            L = len(a["lq_cq"])
+            self.penalty = (a["lq_penalty"].reshape(L, R).astype(object) if "lq_penalty" in a else np.zeros((L, R), object))
+            self.consumed, self.cscale = a["lq_consumed"].reshape(L, R), a["lq_consumed_scale"].reshape(L, R)
+            if decay:  # rule 1: mutable consumed usage, LastUpdate and the admitted usage of the snapshot's rows
+                self.consumed, self.cscale = self.consumed.astype(object), self.cscale.astype(np.int64)
+                self.lq_last = a["lq_last_update_ns"].astype(np.int64).copy()
+                self.lq_afs = afs_cq[a["lq_cq"].astype(np.int64)]
+                rows.lq = a["adm_lq"].astype(np.int64).copy() if "adm_lq" in a else np.zeros(0, np.int64)
+                self.ladm = np.zeros((L, R), object)
+                us = a["adm_use_start"]
+                for row in np.flatnonzero(rows.lq >= 0):
+                    for k in range(int(us[row]), int(us[row + 1])):
+                        self.ladm[rows.lq[row], int(a["adm_use_fr"][k]) % R] += int(a["adm_use_qty"][k])
+                self.hl, self.samp = int(snap.afs_half_life_ns), int(snap.afs_sampling_ns)
+                self.n_samples = 0
+            self.lqu = {int(l): self.usage_of(l) for l in self.seg_lq if l >= 0}
+        self.first_seg = seg_start[:-1]
+        self.strict = a["cq_strategy"].astype(bool)  # KB_QUEUE_STRICT_FIFO = 1
+        self.ps_start = a["wl_ps_start"].astype(np.int64)
+        self.ps_req = a["ps_req"].reshape(-1, R)
+        self.last_gen = a["wl_last_gen"].astype(np.int64).copy()       # LastAssignment.ClusterQueueGeneration, -1 = nil
+        self.last_tried = a["ps_last_tried"].reshape(-1, R).copy()     # LastAssignment.LastTriedFlavorIdx
+        self.shash = a.get("wl_sched_hash")
+        self.has_qr = a["wl_has_quota_reservation"].copy() if "wl_has_quota_reservation" in a else None
+        self.admit_cycle = np.full(W, -1, np.int64)
+        self.evictions = np.zeros(W, np.int64)
+        self.admit_ns = np.full(W, np.iinfo(np.int64).min, np.int64)
+        self.finish_ns = np.full(W, NEVER, np.int64)
+        self.root = root_of(a["parent"])
+        self.static = {k: v for k, v in a.items() if not (k.startswith(("wl_", "ps_", "adm_")) or k in ("heads", "cq_usage") +
+                                                          abi.AFS_FIELDS + abi.AFS_DECAY_FIELDS + abi.STICKY_FIELDS +
+                                                          abi.QUOTA_CHANGE_FIELDS + abi.ACTIVE_FIELDS)}
+        self.gen = a["cq_generation"].astype(np.int64).copy()          # AllocatableResourceGeneration (rule 4 of quota changes)
+        self.static_gen, self.qc_next, self.qc_rowed = int(snap.static_generation), 0, 0
+        if quota:
+            self.qc_ns, self.qc_node = a["qc_ns"].astype(np.int64), a["qc_node"].astype(np.int64)
+            self.qc_rows = [a[k].reshape(-1, FR) for k in ("qc_nominal", "qc_borrow_limit", "qc_lend_limit")]
+            self.static.update({k: a[k].reshape(snap.n_nodes, FR).astype(np.int64).copy()
+                                for k in ("nominal", "borrow_limit", "lend_limit")})
+        if act:  # deactivation / reactivation edits
+            self.ac_ns, self.ac_wl, self.ac_on = (a[k].astype(np.int64) for k in ("ac_ns", "ac_wl", "ac_active"))
+        # per boundary: the stop times of row-holding records, the edits left for after the row events and arrivals, the
+        # time a deferred record's row went
+        self.ac_next, self.stop_at, self.deferred, self.row_gone = 0, {}, {}, {}
+        self.covers_pods = np.zeros(Q, bool)
+        if snap.pods_resource >= 0:
+            for q in range(Q):
+                masks = a["rg_res_mask"][a["cq_rg_start"][q]:a["cq_rg_start"][q + 1]]
+                self.covers_pods[q] = bool(np.any(masks & (1 << snap.pods_resource)))
+        if events and create is not None:  # ABSENT workloads in (create, index) order; `arr_next` is the first not arrived
+            arr_order = np.lexsort((np.arange(W), create))
+            self.arr_order = arr_order[create[arr_order] > snap.now_ns]
+        else:
+            self.arr_order = np.zeros(0, np.int64)
+        self.arr_next = 0
+        self.t = int(snap.now_ns)
 
-        def pr_attempt(w, t0):
-            """rules 1-2: the attempt of record w Admitted at t0 -> (finish column, phase)"""
-            d = int(pr_ns[w])
-            if pr_fail[w] > 0 or d > pr_timeout:
-                return min(t0 + pr_timeout, NEVER), WAIT
-            pr_prev[w] = pr_at[w]
-            pr_at[w] = min(t0 + d, NEVER)
-            return (finish_time(int(pr_at[w]), int(run_ns[w])) if run_ns is not None else NEVER), RUN
-        phase = np.full(snap.n_adm, RUN, np.int64)
-        if "adm_admitted_ns" in a:
-            for row in np.flatnonzero(a["adm_admitted_ns"] != UNSET):
-                adm_finish[row], phase[row] = pr_attempt(int(adm_wl[row]), int(a["adm_admitted_ns"][row]))
-    if mx:  # rule 1: limits, accumulated times, the Admitted time of every row; the start rows' effective deadlines
-        exec_max = a["wl_max_exec_s"].astype(np.int64)
-        acc = a["wl_exec_acc_s"].astype(np.int64).copy() if "wl_exec_acc_s" in a else np.full(snap.n_wl, -1, np.int64)
-        if snap.n_adm and "adm_exec_since_ns" not in a:
-            raise ValueError("wl_max_exec_s needs adm_exec_since_ns when the snapshot has admitted rows")
-        exec_since = a["adm_exec_since_ns"].astype(np.int64).copy() if snap.n_adm else np.zeros(0, np.int64)
-        exec_events = []                                          # records deactivated since the last boundary
+    # ---- queues
+    def index_segments(self):
+        """seg_of / pos_of of every pending workload from the order"""
+        order, qstart = self.order, self.qstart
+        for s in range(len(self.qlen)):
+            self.seg_of[order[qstart[s]:qstart[s + 1]]] = s
+            self.pos_of[order[qstart[s]:qstart[s + 1]]] = np.arange(self.qlen[s])
 
-        def exec_clip(w, A, fin, floor=UNSET):
-            """rule 2: (finish column, expires first) of a row of record w Admitted at A whose own next event is fin"""
-            if exec_max[w] <= 0:
-                return fin, False
-            dl = max(exec_deadline(A, int(exec_max[w]), int(acc[w])), A, floor)
-            return (dl, True) if dl < fin else (fin, False)
-        if phase is None:
-            phase = np.full(snap.n_adm, RUN, np.int64)
-        for row in range(snap.n_adm):
-            if exec_since[row] == UNSET or (evicting is not None and evicting[row]):
-                continue
-            adm_finish[row], e = exec_clip(int(adm_wl[row]), int(exec_since[row]), int(adm_finish[row]), int(snap.now_ns))
-            if e:
-                phase[row] = EXPIRE
-    sticky = a["cq_sticky"].astype(np.int64).copy() if "cq_sticky" in a else None  # sticky workload per ClusterQueue
-    cursor = np.zeros(len(qlen), np.int64)
-    first_aside = qlen.copy()                                     # smallest SET_ASIDE position per segment (qlen = none)
-    nofit = NoFitSets()
-
-    def advance(s):
-        while cursor[s] < qlen[s] and state[order[qstart[s] + cursor[s]]] != QUEUED:
+    def advance(self, s):
+        """the cursor of segment s to its first QUEUED workload"""
+        cursor, qlen, state, order, q0 = self.cursor, self.qlen, self.state, self.order, self.qstart[s]
+        while cursor[s] < qlen[s] and state[order[q0 + cursor[s]]] != QUEUED:
             cursor[s] += 1
 
-    def set_aside(w):
-        state[w] = SET_ASIDE
-        first_aside[seg_of[w]] = min(first_aside[seg_of[w]], pos_of[w])
-    for s in range(len(qlen)):
-        advance(s)
-    decay = events and "wl_lq" in a and "lq_last_update_ns" in a
-    if afs_cq.any() or decay:
-        L = len(a["lq_cq"])
-        penalty = (a["lq_penalty"].reshape(L, R).astype(object) if "lq_penalty" in a else np.zeros((L, R), object))
-        consumed, cscale = a["lq_consumed"].reshape(L, R), a["lq_consumed_scale"].reshape(L, R)
-        if decay:  # rule 1: mutable consumed usage, LastUpdate and the admitted usage of the snapshot's rows
-            consumed, cscale = consumed.astype(object), cscale.astype(np.int64)
-            lq_last = a["lq_last_update_ns"].astype(np.int64).copy()
-            lq_afs = afs_cq[a["lq_cq"].astype(np.int64)]
-            adm_lq = a["adm_lq"].astype(np.int64).copy() if "adm_lq" in a else np.zeros(0, np.int64)
-            ladm = np.zeros((L, R), object)
-            us = a["adm_use_start"]
-            for row in np.flatnonzero(adm_lq >= 0):
-                for k in range(int(us[row]), int(us[row + 1])):
-                    ladm[adm_lq[row], int(a["adm_use_fr"][k]) % R] += int(a["adm_use_qty"][k])
-            hl, samp = int(snap.afs_half_life_ns), int(snap.afs_sampling_ns)
-            n_samples = 0
-        usage_of = lambda l: lq_usage(consumed[l], cscale[l], penalty[l], a["afs_res_weight"], a["lq_weight"][l])  # noqa: E731
-        lqu = {int(l): usage_of(l) for l in seg_lq if l >= 0}
+    def set_aside(self, w):
+        self.state[w] = SET_ASIDE
+        s = self.seg_of[w]
+        self.first_aside[s] = min(self.first_aside[s], self.pos_of[w])
 
-    first_seg = seg_start[:-1]
+    def queue(self, w):
+        """w is QUEUED: the cursor of its segment moves back to it if it comes earlier"""
+        self.state[w] = QUEUED
+        s = self.seg_of[w]
+        self.cursor[s] = min(self.cursor[s], self.pos_of[w])
 
-    def sample(t_to):
-        """rule 3: every sample due at or before t_to (nothing is due at or before the previous boundary)"""
-        nonlocal n_samples
-        for l in np.flatnonzero(lq_afs & (lq_last <= t_to - samp)):
-            k = (int(t_to) - int(lq_last[l])) // samp
-            n_samples += k
-            moved = False
-            for _ in range(k):
-                if hl == 0:
-                    vals, sc = [0] * R, 0
-                    changed = any(int(v) != 0 for v in consumed[l]) or bool((cscale[l] != 0).any())
-                else:
-                    (vals, changed), sc = decay_quantities(consumed[l], cscale[l], ladm[l], a["afs_milli_mul"], snap.afs_alpha), -3
-                consumed[l, :] = vals
-                cscale[l, :] = sc
-                if not changed:
-                    break
-                moved = True
-            lq_last[l] += k * samp
-            if moved:
-                lqu[int(l)] = usage_of(l)
+    def enqueue(self, w):
+        """step 6 for one record: PushOrUpdate, with the NoFit rule of a BestEffortFIFO ClusterQueue"""
+        q = int(self.a["wl_cq"][w])
+        if self.shash is not None and self.nofit.arrival_goes_aside(q, bool(self.strict[q]), int(self.shash[w])):
+            self.set_aside(w)
+        else:
+            self.queue(w)
 
-    def afs_head_seg(q):
+    def usage_of(self, l):
+        return lq_usage(self.consumed[l], self.cscale[l], self.penalty[l], self.a["afs_res_weight"], self.a["lq_weight"][l])
+
+    def afs_head_seg(self, q):
         """segment of the head of AFS ClusterQueue q, -1 = nothing queued"""
-        s0, s1 = int(seg_start[q]), int(seg_start[q + 1])
+        a, cursor, qlen, order, qstart, lqu, seg_lq = self.a, self.cursor, self.qlen, self.order, self.qstart, self.lqu, self.seg_lq
         best, bkey = -1, None
-        for s in range(s0, s1):
+        for s in range(int(self.seg_start[q]), int(self.seg_start[q + 1])):
             if cursor[s] >= qlen[s]:
                 continue
             w = order[qstart[s] + cursor[s]]
@@ -1029,493 +1132,453 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                     continue
             best, bkey = s, key
         return best
-    strict = a["cq_strategy"].astype(bool)  # KB_QUEUE_STRICT_FIFO = 1
-    usage = a["cq_usage"].reshape(Q, FR).astype(np.int64).copy()
-    adm = {k: a[k].copy() for k in ("adm_cq", "adm_priority", "adm_ts", "adm_qr_ts", "adm_uid", "adm_evicted", "adm_use_start",
-                                    "adm_use_fr", "adm_use_qty")}
-    ps_start = a["wl_ps_start"].astype(np.int64)
-    ps_req = a["ps_req"].reshape(-1, R)
-    res = DrainResult()
-    last_gen = a["wl_last_gen"].astype(np.int64).copy()          # LastAssignment.ClusterQueueGeneration, -1 = nil
-    last_tried = a["ps_last_tried"].reshape(-1, R).copy()         # LastAssignment.LastTriedFlavorIdx
-    shash = a.get("wl_sched_hash")
-    has_qr = a["wl_has_quota_reservation"].copy() if "wl_has_quota_reservation" in a else None
-    admit_cycle = np.full(snap.n_wl, -1, np.int64)
-    evictions = np.zeros(snap.n_wl, np.int64)
-    admit_ns = np.full(snap.n_wl, np.iinfo(np.int64).min, np.int64)
-    finish_ns = np.full(snap.n_wl, NEVER, np.int64)
-    root = root_of(a["parent"])
-    static = {k: v for k, v in a.items() if not (k.startswith(("wl_", "ps_", "adm_")) or k in ("heads", "cq_usage") + abi.AFS_FIELDS +
-                                                                                               abi.AFS_DECAY_FIELDS +
-                                                                                               abi.STICKY_FIELDS +
-                                                                                               abi.QUOTA_CHANGE_FIELDS +
-                                                                                               abi.ACTIVE_FIELDS)}
-    gen = a["cq_generation"].astype(np.int64).copy()             # AllocatableResourceGeneration (rule 4 of quota changes)
-    static_gen, qc_next, qc_rowed, qc_events = int(snap.static_generation), 0, 0, []
-    if quota:
-        N_ = snap.n_nodes
-        qc_ns, qc_node = a["qc_ns"].astype(np.int64), a["qc_node"].astype(np.int64)
-        qc_rows = [a[k].reshape(-1, FR) for k in ("qc_nominal", "qc_borrow_limit", "qc_lend_limit")]
-        static.update({k: a[k].reshape(N_, FR).astype(np.int64).copy() for k in ("nominal", "borrow_limit", "lend_limit")})
-    if act:  # deactivation / reactivation edits; per boundary: the stop times of row-holding records, the edits left for
-        # after the row events and arrivals, the time a deferred record's row went
-        ac_ns, ac_wl, ac_on = (a[k].astype(np.int64) for k in ("ac_ns", "ac_wl", "ac_active"))
-    ac_next, ac_events = 0, {"applied": [], "stopped": [], "resumed": []}
-    stop_at, deferred, row_gone = {}, {}, {}
-    covers_pods = np.zeros(Q, bool)
-    if snap.pods_resource >= 0:
-        for q in range(Q):
-            masks = a["rg_res_mask"][a["cq_rg_start"][q]:a["cq_rg_start"][q + 1]]
-            covers_pods[q] = bool(np.any(masks & (1 << snap.pods_resource)))
-    if events and create is not None:  # ABSENT workloads in (create, index) order; `arr_next` is the first not arrived
-        arr_order = np.lexsort((np.arange(snap.n_wl), create))
-        arr_order = arr_order[create[arr_order] > snap.now_ns]
-    else:
-        arr_order = np.zeros(0, np.int64)
-    arr_next = 0
 
-    def remove_rows(rows):
-        """rows leave the admitted tables (cache.DeleteWorkload: cells out of the usage; the other rows keep their order)"""
-        nonlocal adm_wl, adm_finish, adm_lq, evicting, checking, phase, exec_since
-        us, uf, uq = adm["adm_use_start"], adm["adm_use_fr"], adm["adm_use_qty"]
-        for row in rows:
-            cqi = int(adm["adm_cq"][row])
-            for k in range(int(us[row]), int(us[row + 1])):
-                usage[cqi, int(uf[k])] -= int(uq[k])
-        keep = np.ones(len(adm["adm_cq"]), bool)
-        keep[rows] = False
-        cnt = np.diff(us.astype(np.int64))
-        cell_keep = np.repeat(keep, cnt)
-        for k in ("adm_cq", "adm_priority", "adm_ts", "adm_qr_ts", "adm_uid", "adm_evicted"):
-            adm[k] = adm[k][keep]
-        adm["adm_use_fr"], adm["adm_use_qty"] = uf[cell_keep], uq[cell_keep]
-        adm["adm_use_start"] = np.concatenate([[0], np.cumsum(cnt[keep])]).astype(np.int32)
-        if adm_wl is not None:
-            adm_wl = adm_wl[keep]
-        if events:
-            adm_finish = adm_finish[keep]
-        if decay:
-            adm_lq = adm_lq[keep]
-        if evicting is not None:
-            evicting = evicting[keep]
-        if checking is not None:
-            checking = checking[keep]
-        if phase is not None:
-            phase = phase[keep]
-        if mx:
-            exec_since = exec_since[keep]
+    def resort(self):
+        """rule 6: rebuild the order when a queued or set-aside record carries a key other than the one it was sorted by"""
+        state, qts, cursor, first_aside, qlen, res = self.state, self.qts, self.cursor, self.first_aside, self.qlen, self.res
+        if not self.backoff or not (((state == QUEUED) | (state == SET_ASIDE)) & (qts != self.sort_ts)).any():
+            return
+        self.order, self.qstart, _, _ = _queue_order(self.a, self.Q, qts)
+        self.sort_ts = qts.copy()
+        self.index_segments()
+        for s in range(len(qlen)):
+            cursor[s] = 0
+            self.advance(s)
+            seg = self.order[self.qstart[s]:self.qstart[s + 1]]
+            aside = np.flatnonzero(state[seg] == SET_ASIDE)
+            first_aside[s] = int(aside[0]) if len(aside) else qlen[s]
+        res.n_resorts += 1
+        res.resort_orders.append(dict(order=self.order.copy(), qstart=self.qstart.copy(), qts=qts.copy(), state=state.copy(),
+                                      cursor=cursor.copy(), first_aside=first_aside.copy(), seg_of=self.seg_of.copy(),
+                                      pos_of=self.pos_of.copy()))
 
-    def forget(w):
+    def requeue(self, notified):
+        """step 7: the inadmissible requeue in the root cohort trees of `notified`"""
+        order, qstart, state, cursor, first_aside = self.order, self.qstart, self.state, self.cursor, self.first_aside
+        seg_start = self.seg_start
+        aside = {}
+        for q in range(self.Q):
+            for s in range(int(seg_start[q]), int(seg_start[q + 1])):
+                seg = order[qstart[s] + first_aside[s]:qstart[s + 1]]
+                aside.setdefault(q, []).extend(int(w) for w in seg[state[seg] == SET_ASIDE])
+        moved, roots = requeue_inadmissible(self.a["parent"], self.Q, sorted(notified), aside)
+        for ws in moved.values():
+            state[np.asarray(ws, np.int64)] = QUEUED
+        for q in np.flatnonzero(np.isin(self.root[:self.Q], roots)):
+            self.nofit.clear(q)
+            for s in range(int(seg_start[q]), int(seg_start[q + 1])):
+                cursor[s] = min(cursor[s], first_aside[s])
+                first_aside[s] = self.qlen[s]
+
+    # ---- records and rows
+    def log(self, name, vals):
+        """files events of the boundary under way in DrainResult: into the list of the last cycle (the events between
+        the start of cycle c and of c+1 are cycle c's) and into the total, or into the total only before cycle 0"""
+        res = self.res
+        if name != "pods_ready_timeout_at":
+            setattr(res, "n_" + name, getattr(res, "n_" + name) + len(vals))
+        if res.cycles and len(vals):
+            lst = getattr(res, name)
+            lst[-1] = np.concatenate([lst[-1], np.asarray(vals, np.int64)])
+
+    def forget(self, w):
         """a released record: LastAssignment nil, no reservation"""
-        last_gen[w] = -1
-        last_tried[int(ps_start[w]):int(ps_start[w + 1])] = -1
-        if has_qr is not None:
-            has_qr[w] = 0
-        admit_cycle[w] = -1
+        self.last_gen[w] = -1
+        self.last_tried[int(self.ps_start[w]):int(self.ps_start[w + 1])] = -1
+        if self.has_qr is not None:
+            self.has_qr[w] = 0
+        self.admit_cycle[w] = -1
 
-    def exec_deactivate(w):
+    def release(self, w):
+        """the record of an evicted row returns to its queue with LastAssignment nil (workload_controller.go:973-1004);
+        preemption sets no RequeueState, so the requeue is immediate"""
+        self.forget(w)
+        self.queue(w)
+
+    def clear_requeue(self, w):
+        """RequeueState cleared: Count 0, no RequeueAt"""
+        if self.pr:
+            self.pr_count[w] = 0
+        self.requeue_at[w] = UNSET
+
+    def drop_attempt(self, w, t):
+        """a PodsReady attempt still waiting at t is dropped: not counted, no failure used"""
+        if self.pr and self.pr_at[w] > t:
+            self.pr_at[w] = self.pr_prev[w]
+
+    def evict_row(self, row, w, t0):
+        """an eviction issued at t0 on a row (eviction latency): evicting until t0 + latency"""
+        rows = self.rows
+        rows.evicting[row] = True
+        rows.adm["adm_evicted"][row] = 1
+        rows.finish[row] = min(t0 + int(self.lat[w]), NEVER)
+
+    def lq_release(self, row):
+        """rule 5 of decay: a row's cells leave its LocalQueue's admitted usage"""
+        rows = self.rows
+        if self.decay and rows.lq[row] >= 0 and self.afs_cq[int(rows.adm["adm_cq"][row])]:
+            us = rows.adm["adm_use_start"]
+            for k in range(int(us[row]), int(us[row + 1])):
+                self.ladm[rows.lq[row], int(rows.adm["adm_use_fr"][k]) % self.R] -= int(rows.adm["adm_use_qty"][k])
+
+    def pr_attempt(self, w, t0):
+        """rules 1-2 of WaitForPodsReady: the attempt of record w Admitted at t0 -> (finish column, phase)"""
+        d = int(self.pr_ns[w])
+        timeout = int(self.snap.pods_ready_timeout_ns)
+        if self.pr_fail[w] > 0 or d > timeout:
+            return min(t0 + timeout, NEVER), WAIT
+        self.pr_prev[w] = self.pr_at[w]
+        self.pr_at[w] = min(t0 + d, NEVER)
+        return (finish_time(int(self.pr_at[w]), int(self.run_ns[w])) if self.run_ns is not None else NEVER), RUN
+
+    def exec_clip(self, w, A, fin, floor=UNSET):
+        """rule 2 of MaximumExecutionTimeSeconds: (finish column, expires first) of a row of record w Admitted at A
+        whose own next event is fin"""
+        if self.exec_max[w] <= 0:
+            return fin, False
+        dl = max(exec_deadline(A, int(self.exec_max[w]), int(self.acc[w])), A, floor)
+        return (dl, True) if dl < fin else (fin, False)
+
+    def admitted(self, row, w, t):
+        """row of record w is Admitted at t: the run clock or the PodsReady attempt starts, and the
+        MaximumExecutionTimeSeconds deadline with it (rule 1 of each; the reservation without a check delay, or a Ready
+        verdict)"""
+        rows = self.rows
+        if self.checks:
+            self.ready_ns[w] = t
+        if self.pr:
+            rows.finish[row], rows.phase[row] = self.pr_attempt(w, t)
+        else:
+            rows.finish[row] = finish_time(t, int(self.run_ns[w])) if self.run_ns is not None else NEVER
+        if self.mx:
+            rows.since[row] = t
+            rows.finish[row], e = self.exec_clip(w, t, int(rows.finish[row]))
+            if e:
+                rows.phase[row] = EXPIRE
+
+    def exec_deactivate(self, w):
         """rule 3 of MaximumExecutionTimeSeconds: deactivated, acc nil, RequeueState cleared"""
-        deactivated[w] = MAX_EXEC
-        acc[w] = -1
-        if pr:
-            pr_count[w] = 0
-        if backoff:
-            requeue_at[w] = UNSET
-        exec_events.append(int(w))
+        self.deactivated[w] = MAX_EXEC
+        self.acc[w] = -1
+        self.clear_requeue(w)
+        self.log("max_exec_deactivated", [w])
 
-    def exec_release(row, w, t_rel):
+    def exec_release(self, row, w, t_rel):
         """rule 4: the release at t_rel of a row with an Admitted time adds its seconds to acc, after deactivating a
         record whose deadline has passed; returns whether it deactivated the record"""
-        A = int(exec_since[row])
+        A = int(self.rows.since[row])
         if A == UNSET:
             return False
-        deact = exec_max[w] > 0 and deactivated[w] == 0 and exec_deadline(A, int(exec_max[w]), int(acc[w])) <= t_rel
+        acc, lim = self.acc, self.exec_max
+        deact = lim[w] > 0 and self.deactivated[w] == 0 and exec_deadline(A, int(lim[w]), int(acc[w])) <= t_rel
         if deact:
-            exec_deactivate(w)
+            self.exec_deactivate(w)
         d = exec_seconds(t_rel - A)
         total = d if acc[w] < 0 else int(acc[w]) + d
         if total > _I32_MAX:
             raise ExecOverflow(total)
         acc[w] = total
-        res.exec_spans.append((int(w), A, int(t_rel), d))
+        self.res.exec_spans.append((int(w), A, int(t_rel), d))
         return deact
 
-    def release(w):
-        """the record of an evicted row returns to its queue with LastAssignment nil (workload_controller.go:973-1004);
-        preemption sets no RequeueState, so the requeue is immediate"""
-        state[w] = QUEUED
-        last_gen[w] = -1
-        last_tried[int(ps_start[w]):int(ps_start[w + 1])] = -1
-        if has_qr is not None:
-            has_qr[w] = 0
-        admit_cycle[w] = -1
-        cursor[seg_of[w]] = min(cursor[seg_of[w]], pos_of[w])
-
-    def apply_quota_changes(t_next, notified):
-        """rules 2-4 of quota changes: the edits due by t_next, in table order, before the verdicts"""
-        nonlocal qc_next, qc_rowed, static_gen
-        while qc_next < len(qc_ns) and int(qc_ns[qc_next]) <= t_next:
-            i, n = qc_next, int(qc_node[qc_next])
-            qc_next += 1
-            qc_events.append(i)
-            keys = ("nominal", "borrow_limit", "lend_limit")
-            if all(np.array_equal(static[k][n], rows[i]) for k, rows in zip(keys, qc_rows)):
-                continue  # no-op: specUpdated is false
-            for k, rows in zip(keys, qc_rows):
-                static[k] = static[k].copy()
-                static[k][n] = rows[i]
-            gen[root[:Q] == root[n]] += 1
-            static["cq_generation"] = gen.copy()
-            notified.add(n)  # its root tree is requeued (requeue_inadmissible maps a node to its root)
-            qc_rowed += 1
-            static_gen = static_generation_after(int(snap.static_generation), qc_rowed, len(qc_ns))
-
-    def next_event():
+    # ---- the boundary: steps 5-8
+    def next_event(self):
         """earliest pending event after the evictions: a live row's finish or an ABSENT workload's creation (None = none)"""
-        e = int(adm_finish.min()) if len(adm_finish) else NEVER
-        if quota and qc_next < len(qc_ns):
-            e = min(e, int(qc_ns[qc_next]))
-        if act and ac_next < len(ac_ns):
-            e = min(e, int(ac_ns[ac_next]))
-        if arr_next < len(arr_order):
-            e = min(e, int(create[arr_order[arr_next]]))
-        if backoff and (state == BACKOFF).any():
-            e = min(e, int(requeue_at[state == BACKOFF].min()))
+        fin = self.rows.finish
+        e = int(fin.min()) if len(fin) else NEVER
+        if self.quota and self.qc_next < len(self.qc_ns):
+            e = min(e, int(self.qc_ns[self.qc_next]))
+        if self.act and self.ac_next < len(self.ac_ns):
+            e = min(e, int(self.ac_ns[self.ac_next]))
+        if self.arr_next < len(self.arr_order):
+            e = min(e, int(self.create[self.arr_order[self.arr_next]]))
+        if self.backoff and (self.state == BACKOFF).any():
+            e = min(e, int(self.requeue_at[self.state == BACKOFF].min()))
         return None if e >= NEVER else e
 
-    def enqueue(w):
-        """step 6 for one record: PushOrUpdate, with the NoFit rule of a BestEffortFIFO ClusterQueue"""
-        q = int(a["wl_cq"][w])
-        if shash is not None and nofit.arrival_goes_aside(q, bool(strict[q]), int(shash[w])):
-            set_aside(w)
-        else:
-            state[w] = QUEUED
-            cursor[seg_of[w]] = min(cursor[seg_of[w]], pos_of[w])
+    def sample(self, t_to):
+        """rule 3 of decay: every sample due at or before t_to (nothing is due at or before the previous boundary)"""
+        consumed, cscale, lq_last, samp, R = self.consumed, self.cscale, self.lq_last, self.samp, self.R
+        for l in np.flatnonzero(self.lq_afs & (lq_last <= t_to - samp)):
+            k = (int(t_to) - int(lq_last[l])) // samp
+            self.n_samples += k
+            moved = False
+            for _ in range(k):
+                if self.hl == 0:
+                    vals, sc = [0] * R, 0
+                    changed = any(int(v) != 0 for v in consumed[l]) or bool((cscale[l] != 0).any())
+                else:
+                    (vals, changed), sc = decay_quantities(consumed[l], cscale[l], self.ladm[l], self.a["afs_milli_mul"],
+                                                           self.snap.afs_alpha), -3
+                consumed[l, :] = vals
+                cscale[l, :] = sc
+                if not changed:
+                    break
+                moved = True
+            lq_last[l] += k * samp
+            if moved:
+                self.lqu[int(l)] = self.usage_of(l)
 
-    def apply_active_edit(j, w, held, notified):
+    def apply_quota_changes(self, t_next, notified):
+        """rules 2-4 of quota changes: the edits due by t_next, in table order, before the verdicts"""
+        static, keys = self.static, ("nominal", "borrow_limit", "lend_limit")
+        while self.qc_next < len(self.qc_ns) and int(self.qc_ns[self.qc_next]) <= t_next:
+            i, n = self.qc_next, int(self.qc_node[self.qc_next])
+            self.qc_next += 1
+            self.log("quota_changes", [i])
+            if all(np.array_equal(static[k][n], new[i]) for k, new in zip(keys, self.qc_rows)):
+                continue  # no-op: specUpdated is false
+            for k, new in zip(keys, self.qc_rows):
+                static[k] = static[k].copy()
+                static[k][n] = new[i]
+            self.gen[self.root[:self.Q] == self.root[n]] += 1
+            static["cq_generation"] = self.gen.copy()
+            notified.add(n)  # its root tree is requeued (requeue_inadmissible maps a node to its root)
+            self.qc_rowed += 1
+            self.static_gen = static_generation_after(int(self.snap.static_generation), self.qc_rowed, len(self.qc_ns))
+
+    def apply_active_edit(self, j, w, held, notified):
         """rules 2, 4 and 5 of deactivation on record w; held: it holds a row at the edit's time (nothing changes)"""
+        state, deactivated = self.state, self.deactivated
         if held:
             return
-        if ac_on[j] == 0:
+        if self.ac_on[j] == 0:
             if deactivated[w] == 0 and state[w] in (QUEUED, SET_ASIDE, BACKOFF):  # rule 2
                 state[w] = DEACTIVATED
                 deactivated[w] = USER
-                if pr:
-                    pr_count[w] = 0
-                if backoff:
-                    requeue_at[w] = UNSET
-                q = int(a["wl_cq"][w])
-                if sticky is not None and sticky[q] == w:
-                    sticky[q] = -1
+                self.clear_requeue(w)
+                q = int(self.a["wl_cq"][w])
+                if self.sticky is not None and self.sticky[q] == w:
+                    self.sticky[q] = -1
                 notified.add(q)
-                forget(w)
-                ac_events["stopped"].append(w)
+                self.forget(w)
+                self.log("stopped", [w])
         elif state[w] == DEACTIVATED:  # rule 5: LastAssignment nil, Count 0 since the deactivation
             deactivated[w] = 0
-            forget(w)
-            enqueue(w)
-            ac_events["resumed"].append(w)
+            self.forget(w)
+            self.enqueue(w)
+            self.log("resumed", [w])
 
-    def apply_active_first(t_next, notified):
+    def apply_active_first(self, t_next, notified):
         """rule 1: the edits due by t_next, in table order per record, before the row events.  A record that is ABSENT
         or holds a row meets its own events first: its edits from there wait for apply_active_rest; the first stop of an
         active row-holding record sets its stop time (apply_row_stops)"""
-        nonlocal ac_next
-        hi = ac_next
+        state, deactivated, ac_ns = self.state, self.deactivated, self.ac_ns
+        hi = self.ac_next
         while hi < len(ac_ns) and int(ac_ns[hi]) <= t_next:
             hi += 1
         by_w = {}
-        for j in range(ac_next, hi):
-            by_w.setdefault(int(ac_wl[j]), []).append(j)
-        ac_events["applied"].extend(range(ac_next, hi))
-        ac_next = hi
+        for j in range(self.ac_next, hi):
+            by_w.setdefault(int(self.ac_wl[j]), []).append(j)
+        self.log("active_changes", range(self.ac_next, hi))
+        self.ac_next = hi
         for w, js in by_w.items():
             for k, j in enumerate(js):
-                if state[w] == ABSENT or (state[w] == HELD and (deactivated[w] != 0 or ac_on[j] == 0)):
+                if state[w] == ABSENT or (state[w] == HELD and (deactivated[w] != 0 or self.ac_on[j] == 0)):
                     if state[w] == HELD and deactivated[w] == 0:
-                        stop_at[w] = int(ac_ns[j])
-                    deferred[w] = js[k:]
+                        self.stop_at[w] = int(ac_ns[j])
+                    self.deferred[w] = js[k:]
                     break
-                apply_active_edit(j, w, state[w] == HELD, notified)
+                self.apply_active_edit(j, w, state[w] == HELD, notified)
 
-    def apply_row_stops(notified):
+    def apply_row_stops(self, notified):
         """rule 3: every row of an active record whose stop time comes before the row's next own event"""
-        rows = [row for row in range(len(adm_wl)) if int(adm_wl[row]) in stop_at and deactivated[adm_wl[row]] == 0
-                and stop_at[int(adm_wl[row])] < adm_finish[row]]
-        for row in rows:
-            w = int(adm_wl[row]); d = stop_at[w]
+        rows, stop_at, deactivated = self.rows, self.stop_at, self.deactivated
+        if not stop_at:
+            return
+        gone = [row for row in range(len(rows.wl)) if int(rows.wl[row]) in stop_at and deactivated[rows.wl[row]] == 0
+                and stop_at[int(rows.wl[row])] < rows.finish[row]]
+        for row in gone:
+            w = int(rows.wl[row]); d = stop_at[w]
             deactivated[w] = USER
-            if pr:
-                pr_count[w] = 0
-                if pr_at[w] > d:  # a PodsReady attempt still waiting is dropped
-                    pr_at[w] = pr_prev[w]
-            if backoff:
-                requeue_at[w] = UNSET
-            if mx and exec_since[row] != UNSET:  # QuotaReserved unset once the pods are gone
-                rel = evicting is not None and evicting[row]
-                exec_release(row, w, int(adm_finish[row]) if rel else min(d + int(lat[w]), NEVER) if lat is not None else d)
-            cqi = int(adm["adm_cq"][row])
-            notified.add(cqi)
-            if decay and adm_lq[row] >= 0 and afs_cq[cqi]:
-                for k in range(int(adm["adm_use_start"][row]), int(adm["adm_use_start"][row + 1])):
-                    ladm[adm_lq[row], int(adm["adm_use_fr"][k]) % R] -= int(adm["adm_use_qty"][k])
-            state[w] = DEACTIVATED
-            forget(w)
-            row_gone[w] = d
-            ac_events["stopped"].append(w)
-        if rows:
-            remove_rows(rows)
+            self.clear_requeue(w)
+            self.drop_attempt(w, d)
+            if self.mx:  # QuotaReserved unset once the pods are gone
+                rel = rows.evicting is not None and rows.evicting[row]
+                t_rel = int(rows.finish[row]) if rel else min(d + int(self.lat[w]), NEVER) if self.lat is not None else d
+                self.exec_release(row, w, t_rel)
+            notified.add(int(rows.adm["adm_cq"][row]))
+            self.lq_release(row)
+            self.state[w] = DEACTIVATED
+            self.forget(w)
+            self.row_gone[w] = d
+            self.log("stopped", [w])
+        if gone:
+            rows.remove(gone)
 
-    def apply_active_rest(notified):
+    def apply_active_rest(self, notified):
         """rule 1: the deferred edits after the row events and arrivals; a record whose row went at a time after an
         edit held it then"""
-        for w, js in deferred.items():
+        for w, js in self.deferred.items():
             for j in js:
-                apply_active_edit(j, w, state[w] == HELD or row_gone.get(w, UNSET) > int(ac_ns[j]), notified)
-        deferred.clear(); stop_at.clear(); row_gone.clear()
+                self.apply_active_edit(j, w, self.state[w] == HELD or self.row_gone.get(w, UNSET) > int(self.ac_ns[j]), notified)
+        self.deferred.clear(); self.stop_at.clear(); self.row_gone.clear()
 
-    def apply_verdicts(t_next, notified):
-        """rule 2: the verdicts due by t_next, before the completions"""
+    def apply_verdicts(self, t_next, notified):
+        """rule 2 of the checks: the verdicts due by t_next, before the completions"""
+        rows, chk_fail, state = self.rows, self.chk_fail, self.state
         gone = []
-        for row in np.flatnonzero(checking & (adm_finish <= t_next)):
-            w, tv = int(adm_wl[row]), int(adm_finish[row])
-            checking[row] = False
+        for row in np.flatnonzero(rows.checking & (rows.finish <= t_next)):
+            w, tv = int(rows.wl[row]), int(rows.finish[row])
+            rows.checking[row] = False
             if chk_fail[w] == 0:  # Ready: Admitted, the run clock (or the PodsReady attempt) starts
-                ready_ns[w] = tv
-                if pr:
-                    adm_finish[row], phase[row] = pr_attempt(w, tv)
-                else:
-                    adm_finish[row] = finish_time(tv, int(run_ns[w])) if run_ns is not None else NEVER
-                if mx:  # rule 1 of MaximumExecutionTimeSeconds: Admitted now
-                    exec_since[row] = tv
-                    adm_finish[row], e = exec_clip(w, tv, int(adm_finish[row]))
-                    if e:
-                        phase[row] = EXPIRE
-                verdicts["ready"] += 1
+                self.admitted(row, w, tv)
+                self.res.n_check_ready += 1
                 continue
             if chk_fail[w] != ALL_FAIL:
                 chk_fail[w] -= 1
-            k = int(retries[w]) + 1
+            k = int(self.retries[w]) + 1
             gone.append(row)
-            notified.add(int(adm["adm_cq"][row]))
-            last_gen[w] = -1
-            last_tried[int(ps_start[w]):int(ps_start[w + 1])] = -1
-            if has_qr is not None:
-                has_qr[w] = 0
-            admit_cycle[w] = -1
-            if k <= limit:  # Retry: backoff, then requeued with the eviction time as its queue-order timestamp
-                retries[w] = k
+            notified.add(int(rows.adm["adm_cq"][row]))
+            self.forget(w)
+            if k <= self.snap.check_backoff_limit:  # Retry: backoff, then requeued with the eviction time as its queue-order timestamp
+                self.retries[w] = k
                 state[w] = BACKOFF
-                requeue_at[w] = min(tv + check_wait_s(k, base_s, max_s) * 1_000_000_000, NEVER)
-                qts[w] = tv
-                verdicts["retry"].append(w)
+                wait_s = check_wait_s(k, self.snap.check_backoff_base_s, self.snap.check_backoff_max_s)
+                self.requeue_at[w] = min(tv + wait_s * 1_000_000_000, NEVER)
+                self.qts[w] = tv
+                self.log("check_retry", [w])
             else:  # Rejected: deactivated
                 state[w] = DEACTIVATED
-                deactivated[w] = REJECTED
-                verdicts["rejected"].append(w)
+                self.deactivated[w] = REJECTED
+                self.log("check_rejected", [w])
         if gone:
-            remove_rows(gone)
+            rows.remove(gone)
 
-    def resort():
-        """rule 6: rebuild the order when a queued or set-aside record carries a key other than the one it was sorted by"""
-        nonlocal order, qstart, sort_ts
-        if not backoff or not (((state == QUEUED) | (state == SET_ASIDE)) & (qts != sort_ts)).any():
-            return
-        order, qstart, _, _ = _queue_order(a, Q, qts)
-        sort_ts = qts.copy()
-        for s in range(len(qlen)):
-            seg_of[order[qstart[s]:qstart[s + 1]]] = s
-            pos_of[order[qstart[s]:qstart[s + 1]]] = np.arange(qlen[s])
-            cursor[s] = 0
-            advance(s)
-            seg = order[qstart[s]:qstart[s + 1]]
-            aside = np.flatnonzero(state[seg] == SET_ASIDE)
-            first_aside[s] = int(aside[0]) if len(aside) else qlen[s]
-        res.n_resorts += 1
-        res.resort_orders.append(dict(order=order.copy(), qstart=qstart.copy(), qts=qts.copy(), state=state.copy(),
-                                      cursor=cursor.copy(), first_aside=first_aside.copy(), seg_of=seg_of.copy(),
-                                      pos_of=pos_of.copy()))
-
-    def apply_timeouts(t_next):
+    def apply_timeouts(self, t_next):
         """rules 3-4 of WaitForPodsReady: the timeouts due by t_next, after the verdicts and before the completions"""
-        for row in np.flatnonzero((phase == WAIT) & (adm_finish <= t_next)):
-            w, T = int(adm_wl[row]), int(adm_finish[row])
-            if 0 < pr_fail[w] != ALL_FAIL:
-                pr_fail[w] -= 1
-            if pr_limit >= 0 and pr_count[w] + 1 > pr_limit:  # RequeuingLimitExceeded: deactivated, RequeueState cleared
+        rows, snap, pr_count = self.rows, self.snap, self.pr_count
+        limit = int(snap.pods_ready_backoff_limit)
+        for row in np.flatnonzero((rows.phase == WAIT) & (rows.finish <= t_next)):
+            w, T = int(rows.wl[row]), int(rows.finish[row])
+            if 0 < self.pr_fail[w] != ALL_FAIL:
+                self.pr_fail[w] -= 1
+            if limit >= 0 and pr_count[w] + 1 > limit:  # RequeuingLimitExceeded: deactivated, RequeueState cleared
                 pr_count[w] = 0
-                deactivated[w] = REQUEUING_LIMIT
-                timeouts["deactivated"].append(w)
+                self.deactivated[w] = REQUEUING_LIMIT
+                self.log("pods_ready_deactivated", [w])
             else:
                 pr_count[w] = min(int(pr_count[w]) + 1, ALL_FAIL)
-                requeue_at[w] = min(T + pods_ready_wait_ns(int(pr_count[w]), pr_base, pr_max), NEVER)
-                if not pr_creation:
-                    qts[w] = T
-                timeouts["timeout"].append(w)
-                timeouts["at"].append((T, int(requeue_at[w])))
-            phase[row] = TIMED_OUT
-            if lat is not None:  # the pods terminate: an evicting row until T + latency
-                evicting[row] = True
-                adm["adm_evicted"][row] = 1
-                adm_finish[row] = min(T + int(lat[w]), NEVER)
+                self.requeue_at[w] = min(T + pods_ready_wait_ns(int(pr_count[w]), snap.pods_ready_backoff_base_s,
+                                                                snap.pods_ready_backoff_max_s), NEVER)
+                if not snap.pods_ready_requeue_creation:
+                    self.qts[w] = T
+                self.log("pods_ready_timeout", [w])
+                self.log("pods_ready_timeout_at", [(T, int(self.requeue_at[w]))])
+            rows.phase[row] = TIMED_OUT
+            if self.lat is not None:  # the pods terminate: an evicting row until T + latency
+                self.evict_row(row, w, T)
 
-    def apply_expiries(t_next):
+    def apply_expiries(self, t_next):
         """rules 2-3 of MaximumExecutionTimeSeconds: the expiries due by t_next, after the timeouts, before the completions"""
-        for row in np.flatnonzero((phase == EXPIRE) & (adm_finish <= t_next)):
-            w, dl = int(adm_wl[row]), int(adm_finish[row])
-            exec_deactivate(w)
-            if pr and pr_at[w] > dl:  # a PodsReady attempt still waiting is dropped
-                pr_at[w] = pr_prev[w]
-            phase[row] = TIMED_OUT
-            if lat is not None:  # evicted at the deadline: an evicting row until deadline + latency
-                evicting[row] = True
-                adm["adm_evicted"][row] = 1
-                adm_finish[row] = min(dl + int(lat[w]), NEVER)
+        rows = self.rows
+        for row in np.flatnonzero((rows.phase == EXPIRE) & (rows.finish <= t_next)):
+            w, dl = int(rows.wl[row]), int(rows.finish[row])
+            self.exec_deactivate(w)
+            self.drop_attempt(w, dl)
+            rows.phase[row] = TIMED_OUT
+            if self.lat is not None:  # evicted at the deadline: an evicting row until deadline + latency
+                self.evict_row(row, w, dl)
 
-    def apply_events(t_next, notified):
-        """steps 5 and 6 at t_next; returns (finished records, arrived records, records whose eviction completed)"""
-        nonlocal arr_next
-        if quota:
-            apply_quota_changes(t_next, notified)
-        if act:
-            apply_active_first(t_next, notified)
-            apply_row_stops(notified)
-        if checks:
-            apply_verdicts(t_next, notified)
-            if act:
-                apply_row_stops(notified)
-        if pr:
-            apply_timeouts(t_next)
-            if act:
-                apply_row_stops(notified)
-        if mx:
-            apply_expiries(t_next)
-        done = np.flatnonzero(adm_finish <= t_next)
-        gone = evicting[done] if evicting is not None else np.zeros(len(done), bool)
-        to = phase[done] == TIMED_OUT if phase is not None else np.zeros(len(done), bool)
-        fin, released = adm_wl[done[~gone & ~to]].copy(), adm_wl[done[gone & ~to]].copy()
+    def apply_events(self, t_next, notified):
+        """steps 5 and 6 at t_next: the row events, the completions and the arrivals"""
+        rows, state = self.rows, self.state
+        if self.quota:
+            self.apply_quota_changes(t_next, notified)
+        if self.act:
+            self.apply_active_first(t_next, notified)
+            self.apply_row_stops(notified)
+        if self.checks:
+            self.apply_verdicts(t_next, notified)
+            if self.act:
+                self.apply_row_stops(notified)
+        if self.pr:
+            self.apply_timeouts(t_next)
+            if self.act:
+                self.apply_row_stops(notified)
+        if self.mx:
+            self.apply_expiries(t_next)
+        done = np.flatnonzero(rows.finish <= t_next)
+        gone = rows.evicting[done] if rows.evicting is not None else np.zeros(len(done), bool)
+        to = rows.phase[done] == TIMED_OUT if rows.phase is not None else np.zeros(len(done), bool)
+        self.log("finished", rows.wl[done[~gone & ~to]].copy())
+        self.log("evict_done", rows.wl[done[gone & ~to]].copy())
         for row in done:
-            notified.add(int(adm["adm_cq"][row]))
-            if decay and adm_lq[row] >= 0 and afs_cq[int(adm["adm_cq"][row])]:  # rule 5
-                for k in range(int(adm["adm_use_start"][row]), int(adm["adm_use_start"][row + 1])):
-                    ladm[adm_lq[row], int(adm["adm_use_fr"][k]) % R] -= int(adm["adm_use_qty"][k])
-            w = int(adm_wl[row])
-            if act:
-                row_gone[w] = int(adm_finish[row])
-            timed_out = phase is not None and phase[row] == TIMED_OUT
-            rel = evicting is not None and evicting[row]
-            expired = mx and (timed_out or rel) and exec_release(row, w, int(adm_finish[row]))  # rule 4 (max exec)
+            notified.add(int(rows.adm["adm_cq"][row]))
+            self.lq_release(row)
+            w = int(rows.wl[row])
+            if self.act:
+                self.row_gone[w] = int(rows.finish[row])
+            timed_out = rows.phase is not None and rows.phase[row] == TIMED_OUT
+            rel = rows.evicting is not None and rows.evicting[row]
+            expired = self.mx and (timed_out or rel) and self.exec_release(row, w, int(rows.finish[row]))  # rule 4 (max exec)
             if timed_out or expired:  # rule 4 (PodsReady): the record waits for RequeueAt, or is deactivated
-                state[w] = DEACTIVATED if deactivated[w] else BACKOFF
-                forget(w)
+                state[w] = DEACTIVATED if self.deactivated[w] else BACKOFF
+                self.forget(w)
             elif rel:
-                release(w)
+                self.release(w)
             elif w >= 0:
                 state[w] = FINISHED
-                admit_cycle[w] = -1
-                finish_ns[w] = int(adm_finish[row])
+                self.admit_cycle[w] = -1
+                self.finish_ns[w] = int(rows.finish[row])
         if len(done):
-            remove_rows(done)
+            rows.remove(done)
         arr = []
-        while arr_next < len(arr_order) and int(create[arr_order[arr_next]]) <= t_next:
-            w = int(arr_order[arr_next]); arr_next += 1
-            enqueue(w)
+        while self.arr_next < len(self.arr_order) and int(self.create[self.arr_order[self.arr_next]]) <= t_next:
+            w = int(self.arr_order[self.arr_next]); self.arr_next += 1
+            self.enqueue(w)
             arr.append(w)
-        if act:  # before the requeue after a backoff: a BACKOFF record's stop and its requeue give the same state
-            apply_active_rest(notified)
-        if backoff:  # rule 3: the records whose RequeueAt has come
-            for w in np.flatnonzero((state == BACKOFF) & (requeue_at <= t_next)):
-                requeue_at[w] = UNSET
-                enqueue(int(w))
-        return fin, np.asarray(arr, np.int64), released
+        self.log("arrived", arr)
+        if self.act:  # before the requeue after a backoff: a BACKOFF record's stop and its requeue give the same state
+            self.apply_active_rest(notified)
+        if self.backoff:  # rule 3 of the checks: the records whose RequeueAt has come
+            for w in np.flatnonzero((state == BACKOFF) & (self.requeue_at <= t_next)):
+                self.requeue_at[w] = UNSET
+                self.enqueue(int(w))
 
-    def requeue(notified):
-        """step 7: the inadmissible requeue in the root cohort trees of `notified`"""
-        aside = {}
-        for q in range(Q):
-            for s in range(int(seg_start[q]), int(seg_start[q + 1])):
-                seg = order[qstart[s] + first_aside[s]:qstart[s + 1]]
-                aside.setdefault(q, []).extend(int(w) for w in seg[state[seg] == SET_ASIDE])
-        moved, roots = requeue_inadmissible(a["parent"], Q, sorted(notified), aside)
-        for ws in moved.values():
-            state[np.asarray(ws, np.int64)] = QUEUED
-        for q in np.flatnonzero(np.isin(root[:Q], roots)):
-            nofit.clear(q)
-            for s in range(int(seg_start[q]), int(seg_start[q + 1])):
-                cursor[s] = min(cursor[s], first_aside[s])
-                first_aside[s] = qlen[s]
+    def boundary(self, t_next, notified):
+        """the clock moves to t_next: samples, steps 5-7, and the cursors and the order of step 8; `notified`: the
+        ClusterQueues whose root trees the cycle's evictions marked"""
+        if self.decay:
+            self.sample(t_next)
+        self.t = t_next
+        self.apply_events(t_next, notified)
+        if notified:
+            self.requeue(notified)
+        if self.act:  # a deactivated record may sit at a cursor or at first_aside: every cursor to its first QUEUED
+            for s in range(len(self.qlen)):
+                self.advance(s)
+        self.resort()
 
-    def after(fin, arr, released):  # events applied between the start of the last cycle and the next one
-        res.n_finished += len(fin); res.n_arrived += len(arr); res.n_evict_done += len(released)
-        if res.cycles:
-            res.finished[-1] = np.concatenate([res.finished[-1], fin]); res.arrived[-1] = np.concatenate([res.arrived[-1], arr])
-            res.evict_done[-1] = np.concatenate([res.evict_done[-1], released])
-        if checks:
-            ret, rej = np.asarray(verdicts["retry"], np.int64), np.asarray(verdicts["rejected"], np.int64)
-            res.n_check_ready += verdicts["ready"]; res.n_check_retry += len(ret); res.n_check_rejected += len(rej)
-            if res.cycles:
-                res.check_retry[-1] = np.concatenate([res.check_retry[-1], ret])
-                res.check_rejected[-1] = np.concatenate([res.check_rejected[-1], rej])
-            verdicts.update(ready=0, retry=[], rejected=[])
-        if pr:
-            to, de = np.asarray(timeouts["timeout"], np.int64), np.asarray(timeouts["deactivated"], np.int64)
-            res.n_pods_ready_timeout += len(to); res.n_pods_ready_deactivated += len(de)
-            if res.cycles:
-                res.pods_ready_timeout[-1] = np.concatenate([res.pods_ready_timeout[-1], to])
-                res.pods_ready_timeout_at[-1] = np.concatenate([res.pods_ready_timeout_at[-1],
-                                                                np.asarray(timeouts["at"], np.int64).reshape(-1, 2)])
-                res.pods_ready_deactivated[-1] = np.concatenate([res.pods_ready_deactivated[-1], de])
-            timeouts.update(timeout=[], at=[], deactivated=[])
-        if mx:
-            de = np.asarray(exec_events, np.int64)
-            res.n_max_exec_deactivated += len(de)
-            if res.cycles:
-                res.max_exec_deactivated[-1] = np.concatenate([res.max_exec_deactivated[-1], de])
-            exec_events.clear()
-        if quota:
-            qe = np.asarray(qc_events, np.int64)
-            res.n_quota_changes += len(qe)
-            if res.cycles:
-                res.quota_changes[-1] = np.concatenate([res.quota_changes[-1], qe])
-            qc_events.clear()
-        if blk:
-            ap, st_, re_ = (np.asarray(ac_events[k], np.int64) for k in ("applied", "stopped", "resumed"))
-            res.n_active_changes += len(ap); res.n_stopped += len(st_); res.n_resumed += len(re_)
-            if res.cycles:
-                res.active_changes[-1] = np.concatenate([res.active_changes[-1], ap])
-                res.stopped[-1] = np.concatenate([res.stopped[-1], st_]); res.resumed[-1] = np.concatenate([res.resumed[-1], re_])
-            for v in ac_events.values():
-                v.clear()
-
-    t = int(snap.now_ns)
-    cyc = 0
-    if decay and len(qlen) and snap.n_wl and max_cycles > 0:
-        sample(t)
-    while len(qlen) and cyc < max_cycles:
-        hseg = np.where(cursor[np.minimum(first_seg, len(qlen) - 1)] < qlen[np.minimum(first_seg, len(qlen) - 1)], first_seg, -1)
-        for q in np.flatnonzero(afs_cq):
-            hseg[q] = afs_head_seg(q)
-        live = np.flatnonzero(hseg >= 0)
-        if len(live) == 0:
-            if not events:
+    # ---- the loop
+    def run(self, run_cycle, max_cycles):
+        res, qlen, cursor, first_seg = self.res, self.qlen, self.cursor, self.first_seg
+        if self.decay and len(qlen) and self.snap.n_wl and max_cycles > 0:
+            self.sample(self.t)
+        while len(qlen) and res.cycles < max_cycles:
+            hseg = np.where(cursor[np.minimum(first_seg, len(qlen) - 1)] < qlen[np.minimum(first_seg, len(qlen) - 1)], first_seg, -1)
+            for q in np.flatnonzero(self.afs_cq):
+                hseg[q] = self.afs_head_seg(q)
+            live = np.flatnonzero(hseg >= 0)
+            if len(live) == 0:
+                if not self.events:
+                    break
+                e = self.next_event()  # step 1: the clock jumps to the next event
+                if e is None:
+                    break
+                self.boundary(e, set())
+                continue
+            if not self.cycle(run_cycle, live, hseg[live]):
                 break
-            e = next_event()  # step 1: the clock jumps to the next event
-            if e is None:
-                break
-            if decay:
-                sample(e)
-            t = e
-            notified = set()
-            after(*apply_events(t, notified))
-            if notified:
-                requeue(notified)
-            if act:  # a deactivated record may sit at a cursor or at first_aside: every cursor to its first QUEUED
-                for s in range(len(qlen)):
-                    advance(s)
-            resort()
-            continue
-        segs = hseg[live]
-        heads = order[qstart[segs] + cursor[segs]]  # global pending indices, one per ClusterQueue with work left
+        return self.result()
+
+    def cycle(self, run_cycle, live, segs):
+        """steps 2-4 at t for the ClusterQueues `live` with heads in segments `segs`, then the boundary; False when the
+        drain ends"""
+        a, snap, res, rows, R, t = self.a, self.snap, self.res, self.rows, self.R, self.t
+        state, sticky, strict, seg_start, ps_start = self.state, self.sticky, self.strict, self.seg_start, self.ps_start
+        c = res.cycles
+        heads = self.order[self.qstart[segs] + self.cursor[segs]]  # global pending indices, one per ClusterQueue with work left
         chosen = []
         if sticky is not None:  # a queued sticky workload is its ClusterQueue's head
             for e, q in enumerate(live):
@@ -1523,25 +1586,25 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 if w >= 0 and state[w] == QUEUED and w != heads[e]:
                     heads[e] = w
                     chosen.append(w)
-        cs = abi.FlatSnapshot(n_cq=Q, n_cohort=snap.n_cohort, n_flavor=snap.n_flavor, n_resource=R, pods_resource=snap.pods_resource,
-                              flags=snap.flags, now_ns=t, static_generation=static_gen)
-        cs.arrays.update(static)
-        cs.set("cq_usage", usage)
-        for k, v in adm.items():
+        cs = abi.FlatSnapshot(n_cq=self.Q, n_cohort=snap.n_cohort, n_flavor=snap.n_flavor, n_resource=R,
+                              pods_resource=snap.pods_resource, flags=snap.flags, now_ns=t, static_generation=self.static_gen)
+        cs.arrays.update(self.static)
+        cs.set("cq_usage", self.usage)
+        for k, v in rows.adm.items():
             cs.set(k, v)
         for nm in ("wl_cq", "wl_priority", "wl_uid"):
             cs.set(nm, a[nm][heads])
-        cs.set("wl_ts", qts[heads])  # the queue-order timestamp (rule 6)
-        cs.set("wl_last_gen", last_gen[heads])
-        if has_qr is not None:
-            cs.set("wl_has_quota_reservation", has_qr[heads])
-        st, rows = _csr_take(ps_start, heads)
+        cs.set("wl_ts", self.qts[heads])  # the queue-order timestamp (rule 6)
+        cs.set("wl_last_gen", self.last_gen[heads])
+        if self.has_qr is not None:
+            cs.set("wl_has_quota_reservation", self.has_qr[heads])
+        st, psr = _csr_take(ps_start, heads)
         cs.set("wl_ps_start", st)
-        cs.set("ps_req", ps_req[rows]); cs.set("ps_last_tried", last_tried[rows])
+        cs.set("ps_req", self.ps_req[psr]); cs.set("ps_last_tried", self.last_tried[psr])
         for nm in ("ps_req_mask", "ps_count", "ps_min_count", "ps_flavor_ok"):
-            cs.set(nm, a[nm][rows])
+            cs.set(nm, a[nm][psr])
         if "ps_group" in a:  # optional tables (kb_snapshot: NULL when absent)
-            cs.set("ps_group", a["ps_group"][rows])
+            cs.set("ps_group", a["ps_group"][psr])
         cs.set("heads", np.arange(len(heads)))
         cs.finalize()
         out = run_cycle(cs)
@@ -1550,18 +1613,13 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
         res.heads.append(heads); res.decisions.append(dec)
         res.sticky_heads.append(np.asarray(chosen, np.int64))
         res.cycle_start_ns.append(t)
-        res.finished.append(np.zeros(0, np.int64)); res.arrived.append(np.zeros(0, np.int64)); res.evict_done.append(np.zeros(0, np.int64))
-        res.check_retry.append(np.zeros(0, np.int64)); res.check_rejected.append(np.zeros(0, np.int64))
-        res.pods_ready_timeout.append(np.zeros(0, np.int64)); res.pods_ready_deactivated.append(np.zeros(0, np.int64))
-        res.pods_ready_timeout_at.append(np.zeros((0, 2), np.int64))
-        res.max_exec_deactivated.append(np.zeros(0, np.int64))
-        res.quota_changes.append(np.zeros(0, np.int64))
-        res.active_changes.append(np.zeros(0, np.int64)); res.stopped.append(np.zeros(0, np.int64)); res.resumed.append(np.zeros(0, np.int64))
-        res.static_generations.append(static_gen)
+        for k in _EVENT_LISTS:
+            getattr(res, k).append(np.zeros((0, 2) if k == "pods_ready_timeout_at" else 0, np.int64))
+        res.static_generations.append(self.static_gen)
         ok = dec == abi.DEC_ASSUMED
         res.admitted.append(heads[ok])
         # ---- apply the admissions: Assignment.Usage (flavorassigner.go:198-218) with the admitted counts
-        new_fr, new_qty, new_start = [], [], [int(adm["adm_use_start"][-1])]
+        new_cells = []
         for e in np.flatnonzero(ok):
             cqi = int(cs.arrays["wl_cq"][e])
             cells = {}
@@ -1571,88 +1629,41 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                     f = int(out.ps_flavor[row, r])
                     if f < 0:
                         continue
-                    if covers_pods[cqi] and r == snap.pods_resource:
+                    if self.covers_pods[cqi] and r == snap.pods_resource:
                         q = cnt
                     else:
                         q = int(cs.arrays["ps_req"].reshape(-1, R)[row, r])
                         if full != 0 and full != cnt:
                             q = q // full * cnt  # ScaledTo workload.go:258-275
                     cells[f * R + r] = cells.get(f * R + r, 0) + q
-            for fr, q in cells.items():
-                usage[cqi, fr] += q
-                new_fr.append(fr); new_qty.append(q)
-            new_start.append(new_start[-1] + len(cells))
-            if afs_cq[cqi]:  # AfsEntryPenalties.Push of the entry penalty, then the LocalQueue's usage again
+            new_cells.append(cells)
+            if self.afs_cq[cqi]:  # AfsEntryPenalties.Push of the entry penalty, then the LocalQueue's usage again
                 w, lq = int(heads[e]), int(a["wl_lq"][heads[e]])
-                rows = slice(int(ps_start[w]), int(ps_start[w + 1]))
-                pen = entry_penalty(ps_req[rows], a["ps_req_mask"][rows], a["afs_milli_mul"], snap.afs_alpha)
-                if decay:  # rule 4: admitted usage, decay to t, LastUpdate = t, the penalty into consumed
+                wrows = slice(int(ps_start[w]), int(ps_start[w + 1]))
+                pen = entry_penalty(self.ps_req[wrows], a["ps_req_mask"][wrows], a["afs_milli_mul"], snap.afs_alpha)
+                if self.decay:  # rule 4: admitted usage, decay to t, LastUpdate = t, the penalty into consumed
+                    consumed, cscale, ladm = self.consumed, self.cscale, self.ladm
                     for fr, q in cells.items():
                         ladm[lq, fr % R] += q
-                    vals, _ = decay_quantities(consumed[lq], cscale[lq], ladm[lq], a["afs_milli_mul"], alpha_of(t - int(lq_last[lq]), hl))
+                    alpha = alpha_of(t - int(self.lq_last[lq]), self.hl)
+                    vals, _ = decay_quantities(consumed[lq], cscale[lq], ladm[lq], a["afs_milli_mul"], alpha)
                     consumed[lq, :] = vals
                     cscale[lq, :] = -3
-                    lq_last[lq] = t
+                    self.lq_last[lq] = t
                     for r, d in enumerate(pen):
                         consumed[lq, r], cscale[lq, r] = quantity_add((int(consumed[lq, r]), int(cscale[lq, r])), (d, -3))
                 else:
                     for r, d in enumerate(pen):
-                        penalty[lq, r] = _int64(int(penalty[lq, r]) + d)
-                lqu[lq] = usage_of(lq)
-        n_new = int(ok.sum())
+                        self.penalty[lq, r] = _int64(int(self.penalty[lq, r]) + d)
+                self.lqu[lq] = self.usage_of(lq)
+        g = heads[ok]
+        n_new = len(g)
         if n_new:
-            g = heads[ok]
-            admit_cycle[g] = cyc
-            admit_ns[g] = t
-            state[g] = HELD
-        if n_new:
-            g = heads[ok]
-            adm["adm_cq"] = np.concatenate([adm["adm_cq"], a["wl_cq"][g]])
-            adm["adm_priority"] = np.concatenate([adm["adm_priority"], a["wl_priority"][g]])
-            adm["adm_ts"] = np.concatenate([adm["adm_ts"], a["wl_ts"][g]])
-            adm["adm_qr_ts"] = np.concatenate([adm["adm_qr_ts"], np.full(n_new, t, np.int64)])
-            adm["adm_uid"] = np.concatenate([adm["adm_uid"], a["wl_uid"][g]])
-            adm["adm_evicted"] = np.concatenate([adm["adm_evicted"], np.zeros(n_new, np.uint8)])
-            adm["adm_use_start"] = np.concatenate([adm["adm_use_start"], np.asarray(new_start[1:], np.int32)])
-            adm["adm_use_fr"] = np.concatenate([adm["adm_use_fr"], np.asarray(new_fr, np.int32)])
-            adm["adm_use_qty"] = np.concatenate([adm["adm_use_qty"], np.asarray(new_qty, np.int64)])
-            if adm_wl is not None:
-                adm_wl = np.concatenate([adm_wl, g])
-            if decay:
-                adm_lq = np.concatenate([adm_lq, a["wl_lq"][g].astype(np.int64)])
-            if backoff:  # rule 4 of the checks, 6 of PodsReady: the reservation resets Evicted
-                qts[g] = a["wl_ts"][g]
-            if checks:  # rule 1: a check delay starts an attempt, a delay of 0 is Ready at once
-                chk = chk_ns[g] > 0
-                checking = np.concatenate([checking, chk])
-                ready_ns[g[~chk]] = t
-            if events:
-                fin_new = [finish_time(t, int(run_ns[w])) if run_ns is not None else NEVER for w in g]
-                if checks:
-                    fin_new = [min(t + int(chk_ns[w]), NEVER) if chk_ns[w] > 0 else f for w, f in zip(g, fin_new)]
-                if phase is not None:  # rule 1 (PodsReady, max exec): Admitted now unless the checks run
-                    ph_new = np.full(n_new, RUN, np.int64)
-                    since_new = np.full(n_new, UNSET, np.int64)
-                    for i, w in enumerate(g):
-                        if checks and chk_ns[w] > 0:
-                            continue
-                        if pr:
-                            fin_new[i], ph_new[i] = pr_attempt(int(w), t)
-                        if mx:
-                            since_new[i] = t
-                            fin_new[i], e = exec_clip(int(w), t, int(fin_new[i]))
-                            if e:
-                                ph_new[i] = EXPIRE
-                    phase = np.concatenate([phase, ph_new])
-                    if mx:
-                        exec_since = np.concatenate([exec_since, since_new])
-                adm_finish = np.concatenate([adm_finish, np.asarray(fin_new, np.int64)])
-            if evicting is not None:
-                evicting = np.concatenate([evicting, np.zeros(n_new, bool)])
+            self.admit(g, new_cells, c)
         # ---- LastAssignment of the entries that stay pending (scheduler.go:345,494)
         tried = np.asarray(out.ps_tried_idx).reshape(-1, R)
         cqs = live
-        inadmissible = np.zeros(len(heads), bool)
+        last_gen, last_tried = self.last_gen, self.last_tried
         for e in range(len(heads)):
             if ok[e]:
                 continue
@@ -1662,13 +1673,12 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                 last_gen[w] = -1
                 last = None
             else:
-                last_gen[w] = int(gen[int(a["wl_cq"][w])])  # the current generation (rule 6 of quota changes)
+                last_gen[w] = int(self.gen[int(a["wl_cq"][w])])  # the current generation (rule 6 of quota changes)
                 last_tried[int(ps_start[w]):int(ps_start[w + 1])] = tried[r0:r1]
                 last = tried[r0:r1]
             # ---- queue movement (cluster_queue.go:362-425,609-633); a StrictFIFO queue keeps its head either way
-            inadmissible[e] = requeue_goes_inadmissible(False, requeue_reason(int(dec[e])), last)
-            if inadmissible[e] and not strict[cqs[e]]:
-                set_aside(w)
+            if requeue_goes_inadmissible(False, requeue_reason(int(dec[e])), last) and not strict[cqs[e]]:
+                self.set_aside(w)
         if sticky is not None:  # admission deletes the sticky workload, a BestEffortFIFO preemptor becomes it
             for e in range(len(heads)):
                 q, w = int(cqs[e]), int(heads[e])
@@ -1676,114 +1686,118 @@ def drain(snap: abi.FlatSnapshot, run_cycle: Callable[[abi.FlatSnapshot], abi.Cy
                     sticky[q] = -1
                 elif dec[e] == abi.DEC_PREEMPTING and not strict[q]:
                     sticky[q] = w
-        if shash is not None:
+        if self.shash is not None:
+            order, qstart, cursor, shash = self.order, self.qstart, self.cursor, self.shash
             for e in np.flatnonzero((dec == abi.DEC_NOFIT) & ~strict[cqs]):
                 hsh = int(shash[heads[e]])
                 if hsh == 0:
                     continue
                 q = int(cqs[e])
-                nofit.insert(q, hsh)
+                self.nofit.insert(q, hsh)
                 for s in range(int(seg_start[q]), int(seg_start[q + 1])):  # every queued workload of the class but the head
                     rest = order[qstart[s] + cursor[s]:qstart[s + 1]]
                     for w in rest[(shash[rest] == hsh) & (state[rest] == QUEUED) & (rest != heads[e])]:
-                        set_aside(int(w))
+                        self.set_aside(int(w))
+        advance = self.advance
         for q in cqs:  # the next head is the first queued workload
             for s in range(int(seg_start[q]), int(seg_start[q + 1])):
                 advance(s)
         # ---- evictions (replay): every target of every Preempting entry, as rows of the tables the cycle saw
         victims = []
-        if replay:
+        if self.replay:
             for e in np.flatnonzero(dec == abi.DEC_PREEMPTING):
                 victims.extend(int(out.tgt_adm[k]) for k in range(int(out.tgt_start[e]), int(out.tgt_start[e + 1])))
             victims = sorted(set(victims))
-        if evicting is not None:  # latency: issue the evictions not under way yet; the rows stay until their end time
-            victims = [row for row in victims if not evicting[row]]
-        res.evicted.append(np.sort(adm_wl[victims]) if victims else np.zeros(0, np.int64))
+        if rows.evicting is not None:  # latency: issue the evictions not under way yet; the rows stay until their end time
+            victims = [row for row in victims if not rows.evicting[row]]
+        res.evicted.append(np.sort(rows.wl[victims]) if victims else np.zeros(0, np.int64))
         notified = set()
-        if victims and evicting is not None:
-            for row in victims:
-                w = int(adm_wl[row])
-                evicting[row] = True
-                adm["adm_evicted"][row] = 1
-                adm_finish[row] = min(t + int(lat[w]), NEVER)
-                if checking is not None and checking[row]:  # rule 5: no pods, released at the next boundary
-                    checking[row] = False
-                    adm_finish[row] = t
-                if phase is not None:  # an ordinary evicting row (rule 5 of PodsReady: a waiting attempt is dropped)
-                    phase[row] = RUN
-                if pr and pr_at[w] > t:
-                    pr_at[w] = pr_prev[w]
-                evictions[w] += 1
-        elif victims:
-            for row in victims:
-                w = int(adm_wl[row])
-                if mx and exec_release(row, w, t):  # rule 4 of max exec: past its deadline, deactivated
+        for row in victims:
+            w = int(rows.wl[row])
+            if rows.evicting is not None:
+                self.evict_row(row, w, t)
+                if rows.checking is not None and rows.checking[row]:  # rule 5 of the checks: no pods, released at the next boundary
+                    rows.checking[row] = False
+                    rows.finish[row] = t
+                if rows.phase is not None:  # an ordinary evicting row (rule 5 of PodsReady: a waiting attempt is dropped)
+                    rows.phase[row] = RUN
+            else:
+                if self.mx and self.exec_release(row, w, t):  # rule 4 of max exec: past its deadline, deactivated
                     state[w] = DEACTIVATED
-                    forget(w)
+                    self.forget(w)
                 else:
-                    release(w)
-                if pr and pr_at[w] > t:  # rule 5 of PodsReady: dropped before PodsReady
-                    pr_at[w] = pr_prev[w]
-                evictions[w] += 1
-                notified.add(int(adm["adm_cq"][row]))
-            remove_rows(victims)
-        cyc += 1
-        if not events:
+                    self.release(w)
+                notified.add(int(rows.adm["adm_cq"][row]))
+            self.drop_attempt(w, t)  # rule 5 of PodsReady: dropped before PodsReady
+            self.evictions[w] += 1
+        if victims and rows.evicting is None:
+            rows.remove(victims)
+        if not self.events:
             if notified:  # ---- inadmissible requeue in the root cohort trees of the victims
-                requeue(notified)
+                self.requeue(notified)
             if n_new == 0 and not victims:
-                break
-            t += 1
-            continue
+                return False
+            self.t += 1
+            return True
         # ---- the next time, then the completions and arrivals up to it
         if n_new or victims:
-            t_next = min(t + step, NEVER)
+            t_next = min(t + self.step, NEVER)
         else:
-            e = next_event()
+            e = self.next_event()
             if e is None:
-                break  # quiet, and nothing will ever happen again
-            t_next = max(min(t + step, NEVER), e)
-        if decay:
-            sample(t_next)
-        t = t_next
-        after(*apply_events(t, notified))
-        if notified:
-            requeue(notified)
-        if act:
-            for s in range(len(qlen)):
-                advance(s)
-        resort()
-    res.cq_usage = usage
-    res.wl_evictions = evictions
-    res.wl_admit_cycle = admit_cycle
-    res.state = state
-    res.adm = dict(adm, **({"adm_wl": adm_wl} if replay else {}))
-    if events:
-        res.adm["adm_finish_ns"] = adm_finish
-    if evicting is not None:
-        res.adm["adm_evicting"] = evicting
-    res.wl_admit_ns = admit_ns
-    res.wl_finish_ns = finish_ns
-    res.end_ns = t
-    res.cq_sticky = sticky
-    if quota:
-        res.cq_generation = gen
-    if backoff:
-        res.wl_queue_ts = qts
-    if backoff or mx or blk:
-        res.wl_deactivated, res.wl_deactivation_reason = (deactivated != 0).astype(np.uint8), deactivated
-    if mx:
-        res.wl_exec_acc_s = acc
-        res.adm["adm_exec_since_ns"] = exec_since
-    if checks:
-        res.wl_ready_ns, res.wl_check_retries = ready_ns, retries
-        res.adm["adm_checking"] = checking
-    if pr:
-        res.wl_pods_ready_at, res.wl_pods_ready_count = pr_at, pr_count
-        res.adm["adm_pods_ready_phase"] = phase
-    if decay:
-        res.lq_consumed = consumed.astype(np.int64)
-        res.lq_consumed_scale = cscale.astype(np.int32)
-        res.lq_last_update_ns = lq_last
-        res.n_afs_samples = n_samples
-    return res
+                return False  # quiet, and nothing will ever happen again
+            t_next = max(min(t + self.step, NEVER), e)
+        self.boundary(t_next, notified)
+        return True
+
+    def admit(self, g, cells, c):
+        """the workloads g admitted in cycle c at t join the tables with their cells: HELD, a reservation with a check
+        delay starts an attempt (rule 1 of the checks), every other one is Admitted at once"""
+        a, t, rows = self.a, self.t, self.rows
+        self.admit_cycle[g] = c
+        self.admit_ns[g] = t
+        self.state[g] = HELD
+        if self.backoff:  # rule 4 of the checks, 6 of PodsReady: the reservation resets Evicted
+            self.qts[g] = a["wl_ts"][g]
+        n = len(g)
+        chk = self.chk_ns[g] > 0 if self.checks else np.zeros(n, bool)
+        fin = [min(t + int(self.chk_ns[w]), NEVER) if k else NEVER for w, k in zip(g, chk)]  # a verdict comes at t + delay
+        first = len(rows.adm["adm_cq"])
+        rows.append(cells, adm_cq=a["wl_cq"][g], adm_priority=a["wl_priority"][g], adm_ts=a["wl_ts"][g],
+                    adm_qr_ts=np.full(n, t, np.int64), adm_uid=a["wl_uid"][g], adm_evicted=np.zeros(n, np.uint8), wl=g,
+                    finish=np.asarray(fin, np.int64), evicting=np.zeros(n, bool), since=np.full(n, UNSET, np.int64),
+                    checking=chk, phase=np.full(n, RUN, np.int64),
+                    lq=a["wl_lq"][g].astype(np.int64) if self.decay else None)
+        if self.events:
+            for i in np.flatnonzero(~chk):
+                self.admitted(first + int(i), int(g[i]), t)
+
+    def result(self):
+        res = self.res
+        res.cq_usage = self.usage
+        res.wl_evictions = self.evictions
+        res.wl_admit_cycle = self.admit_cycle
+        res.state = self.state
+        res.adm = self.rows.export(hide=[c for c, on in (("wl", self.replay), ("phase", self.pr)) if not on])
+        res.wl_admit_ns = self.admit_ns
+        res.wl_finish_ns = self.finish_ns
+        res.end_ns = self.t
+        res.cq_sticky = self.sticky
+        if self.quota:
+            res.cq_generation = self.gen
+        if self.backoff:
+            res.wl_queue_ts = self.qts
+        if self.backoff or self.mx or self.blk:
+            res.wl_deactivated, res.wl_deactivation_reason = (self.deactivated != 0).astype(np.uint8), self.deactivated
+        if self.mx:
+            res.wl_exec_acc_s = self.acc
+        if self.checks:
+            res.wl_ready_ns, res.wl_check_retries = self.ready_ns, self.retries
+        if self.pr:
+            res.wl_pods_ready_at, res.wl_pods_ready_count = self.pr_at, self.pr_count
+        if self.decay:
+            res.lq_consumed = self.consumed.astype(np.int64)
+            res.lq_consumed_scale = self.cscale.astype(np.int32)
+            res.lq_last_update_ns = self.lq_last
+            res.n_afs_samples = self.n_samples
+        return res
