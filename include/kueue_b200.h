@@ -36,7 +36,9 @@ extern "C" {
 #define KB_NO_LIMIT INT64_MAX
 #define KB_MAX_RESOURCES 16   /* n_resource <= 16  */
 #define KB_MAX_FLAVORS   64   /* n_flavor   <= 64 (eligibility bitmask is u64) */
-#define KB_MAX_DEPTH     16   /* CQ -> root path length <= 16 */
+#define KB_MAX_DEPTH     16   /* parent hops from a ClusterQueue to its root <= 16: paths of <= 17 nodes */
+#define KB_MAX_WL_PODSETS 8   /* podsets per workload <= 8 (Workload spec.podSets MaxItems=8,
+                                 apis/kueue/v1beta2/workload_types.go) */
 #define KB_N_KERNELS     20
 
 typedef enum kb_status {

@@ -496,6 +496,7 @@ static int32_t build_dynamic(kb_handle *h, const kb_snapshot *s) {
   for (int w = 0; w < s->n_wl; w++) {
     if (s->wl_cq[w] < 0 || s->wl_cq[w] >= Q) return fail(h, KB_ERR_INVALID, "wl_cq out of range");
     if (s->wl_ps_start[w + 1] < s->wl_ps_start[w]) return fail(h, KB_ERR_INVALID, "wl_ps_start not monotone");
+    if (s->wl_ps_start[w + 1] - s->wl_ps_start[w] > KB_MAX_WL_PODSETS) return fail(h, KB_ERR_INVALID, "a workload with more than KB_MAX_WL_PODSETS podsets");
   }
   if (s->n_wl && (s->wl_ps_start[0] != 0 || s->wl_ps_start[s->n_wl] != s->n_podset)) return fail(h, KB_ERR_INVALID, "wl_ps_start must run from 0 to n_podset");
   // heads: range, most podsets of one entry, one head per ClusterQueue? (fairSharingIterator keeps one entry per CQ,
@@ -1009,34 +1010,35 @@ static int32_t launch_tree(kb_handle *h, int *launches) {
 
 // admit kernel launches: lone-CQ roots (slots [0, nLone)) and cohort-tree roots
 // (slots [nLone, nRoots)) separately so each class gets the shared memory it needs.
-static size_t admit_smem(int nn_tables, int FR, int sort_cap, int nn_stage = 0) {
+// k_admit's shared memory: quota tables of nn_tables nodes, a request tile of `tile` entries x FR, tile metadata, path
+static size_t admit_smem(int nn_tables, int FR, int tile, int nn_stage = 0) {
   size_t tb = (size_t)nn_tables * FR * 32;
-  size_t mid = (size_t)KB_TILE * FR * 8; (void)sort_cap;
+  size_t mid = (size_t)tile * FR * 8;
   // global-table mode: staging buffers of the commit pipeline (k_admit: cells, path table, target ids, scratch)
   size_t staging = nn_stage ? sizeof(TgCell) * 2 * KB_SUB * KB_ECAP + 4 * (size_t)nn_stage * KB_PF + 4 * 2 * KB_SUB * KB_TCAP +
                                   4 * KB_SUB * (KB_TCAP + 1) + 4 * KB_SUB * 32 + 2 * 2 * KB_SUB * 34 + (size_t)nn_stage + 2 * KB_SUB + 64
                             : 0;
   return tb + mid + 16 + (size_t)nn_tables * 4 + KB_TILE * 28 + (KB_MAX_DEPTH + 2) * 4 + 64 + staging;
 }
+// the longest request tile (<= KB_TILE entries) that fits `budget` next to the rest of k_admit's shared memory; 0 when
+// not even one entry does.  KB_TILE entries of 1,024 cells take 1 MiB: wide snapshots commit in shorter tiles.
+static int admit_tile(size_t budget, int nn_tables, int FR, int nn_stage = 0) {
+  size_t fixed = admit_smem(nn_tables, FR, 0, nn_stage), row = (size_t)FR * 8;
+  return fixed + row > budget ? 0 : (int)std::min<size_t>(KB_TILE, (budget - fixed) / row);
+}
 static int32_t launch_admit(kb_handle *h, int *launches) {
   DevSnap &D = h->D;
   const size_t kMaxSmem = 200 * 1024;
-  // sort capacity: entries per root are at most H; cap by what shared memory allows
-  auto pick_cap = [&](int nn_tables) {
-    int cap = 64;
-    while (cap < KB_SORT_CAP && cap < D.H && admit_smem(nn_tables, D.FR, cap * 2) <= kMaxSmem) cap *= 2;
-    return cap;
-  };
   if (D.nLone && D.lone_fast) {
     size_t sm = (size_t)KB_LONE_WARPS * 32 * D.FR * 8;
     CUDA_TRY(h, cudaFuncSetAttribute(k_admit_lone, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem));
     k_admit_lone<<<(D.nLone + KB_LONE_WARPS - 1) / KB_LONE_WARPS, KB_LONE_WARPS * 32, sm, h->stream>>>(D); (*launches)++;
   }
   if (D.nLone) {
-    int cap = pick_cap(1);
-    size_t sm = admit_smem(1, D.FR, cap);
+    int tile = admit_tile(kMaxSmem, 1, D.FR);
+    if (!tile) return fail(h, KB_ERR_INVALID, "k_admit: one ClusterQueue's quota tables exceed shared memory");
     CUDA_TRY(h, cudaFuncSetAttribute(k_admit<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem));
-    k_admit<true><<<D.nLone, KB_ADMIT_THREADS, sm, h->stream>>>(D, 0, cap, 0); (*launches)++;
+    k_admit<true><<<D.nLone, KB_ADMIT_THREADS, admit_smem(1, D.FR, tile), h->stream>>>(D, 0, tile, 0); (*launches)++;
   }
   bool fair_trees = D.nTrees && (D.flags & KB_F_FAIR_SHARING);
   bool any_deep = false;
@@ -1057,19 +1059,19 @@ static int32_t launch_admit(kb_handle *h, int *launches) {
     }
   }
   if (D.nTrees) {  // classical order, and fair sharing in flat cohorts (static key order)
-    bool fits = admit_smem(h->max_tree_nodes, D.FR, 64) <= kMaxSmem;
-    if (fits) {
-      int cap = pick_cap(h->max_tree_nodes);
-      size_t sm = admit_smem(h->max_tree_nodes, D.FR, cap);
+    // quota tables in shared memory when they fit next to a full tile, in global memory otherwise, with the staged
+    // commit pipeline when its buffers fit next to a tile of at least one entry
+    if (admit_smem(h->max_tree_nodes, D.FR, KB_TILE) <= kMaxSmem) {
+      int tile = admit_tile(kMaxSmem, h->max_tree_nodes, D.FR);
       CUDA_TRY(h, cudaFuncSetAttribute(k_admit<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem));
-      k_admit<true><<<D.nTrees, KB_ADMIT_THREADS, sm, h->stream>>>(D, D.nLone, cap, 0); (*launches)++;
+      k_admit<true><<<D.nTrees, KB_ADMIT_THREADS, admit_smem(h->max_tree_nodes, D.FR, tile), h->stream>>>(D, D.nLone, tile, 0); (*launches)++;
     } else {
-      int cap = pick_cap(0);
-      size_t sm = admit_smem(0, D.FR, cap, h->max_tree_nodes);
-      int staged = sm <= kMaxSmem;
-      if (!staged) sm = admit_smem(0, D.FR, cap);
+      int tile = admit_tile(kMaxSmem, 0, D.FR, h->max_tree_nodes), staged = tile > 0;
+      if (!staged) tile = admit_tile(kMaxSmem, 0, D.FR);
+      if (!tile) return fail(h, KB_ERR_INVALID, "k_admit: no request tile fits shared memory");
+      size_t sm = admit_smem(0, D.FR, tile, staged ? h->max_tree_nodes : 0);
       CUDA_TRY(h, cudaFuncSetAttribute(k_admit<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem));
-      k_admit<false><<<D.nTrees, KB_ADMIT_THREADS, sm, h->stream>>>(D, D.nLone, cap, staged); (*launches)++;
+      k_admit<false><<<D.nTrees, KB_ADMIT_THREADS, sm, h->stream>>>(D, D.nLone, tile, staged); (*launches)++;
     }
   }
   return KB_OK;

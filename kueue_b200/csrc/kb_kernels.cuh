@@ -371,6 +371,8 @@ __device__ inline int assign_workload(const DevSnap &D, Oracle &orc, int wl, con
 }
 
 #define KB_MAX_PODSETS 16
+static_assert(KB_MAX_WL_PODSETS <= KB_MAX_PODSETS, "the PodSetReducer must hold every podset of an accepted workload");
+static_assert(KB_MAX_CELLS >= KB_MAX_WL_PODSETS * KB_MAX_RESOURCES, "GetTargets must hold every cell of an accepted workload");
 
 // getInitialAssignments scheduler.go:584-625 incl. PodSetReducer.Search podset_reducer.go:56-86.
 // Leaves the final PodSetAssignment rows in the output tables; returns the representative
@@ -1855,7 +1857,8 @@ __device__ inline void expand_entry(const DevSnap &D, int e, i64 *qrow) {
 }
 
 template <bool kSmemTables>
-__global__ void __launch_bounds__(KB_ADMIT_THREADS) k_admit(DevSnap D, int slot_base, int sort_cap, int stage_buffers) {
+// tile: entries per request tile (1..KB_TILE), as many as the launch's shared memory holds (admit_tile, kb_api.cu)
+__global__ void __launch_bounds__(KB_ADMIT_THREADS) k_admit(DevSnap D, int slot_base, int tile, int stage_buffers) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int FR = D.FR;
 #ifdef KB_ADMIT_PROBE
@@ -1875,8 +1878,7 @@ __global__ void __launch_bounds__(KB_ADMIT_THREADS) k_admit(DevSnap D, int slot_
   Tab<kSmemTables> T;
   unsigned char *p = stage_tables<kSmemTables>(D, T, smem_raw, nodes, nn);
   i64 *s_q = (i64 *)p;
-  p += (size_t)KB_TILE * FR * 8;
-  (void)sort_cap;
+  p += (size_t)tile * FR * 8;
   p = (unsigned char *)(((uintptr_t)p + 7) & ~(uintptr_t)7);
   int *t_e = (int *)p, *t_node = t_e + KB_TILE, *t_mode = t_node + KB_TILE, *t_borrow = t_mode + KB_TILE;
   int *t_cq = t_borrow + KB_TILE, *t_ntg = t_cq + KB_TILE, *t_toff = t_ntg + KB_TILE;
@@ -1993,8 +1995,8 @@ __global__ void __launch_bounds__(KB_ADMIT_THREADS) k_admit(DevSnap D, int slot_
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   // flat cohort (every ClusterQueue directly under the root), tables in shared memory, at most two columns per lane
   const bool flat = kSmemTables && FR <= 64 && slot >= D.nLone && D.tree_flat[slot - D.nLone];
-  for (int base = 0; base < n; base += KB_TILE) {
-    int tn = min(KB_TILE, n - base);
+  for (int base = 0; base < n; base += tile) {
+    int tn = min(tile, n - base);
     for (int i = threadIdx.x; i < tn; i += blockDim.x) {
       int e = ent[base + i];
       int cqn = D.wl_cq[D.heads[e]];

@@ -10,6 +10,13 @@ import numpy as np
 
 from . import abi
 
+# mean request per resource; resources past the eighth repeat the row (np.resize), so R <= 8 keeps its old snapshots
+_SCALE = np.array([2_000, 2**31, 4, 100_000, 50, 10, 1000, 64], np.int64)
+
+
+def _scale(R: int) -> np.ndarray:
+    return np.resize(_SCALE, R)
+
 
 def _cohort_forest(n_root: int, fanouts, cqs_per_leaf: int):
     """Cohort forest: n_root roots, then `fanouts` children per level; CQs hang off
@@ -67,7 +74,7 @@ def make_snapshot(config: int = 2, W: int | None = None, Q: int | None = None, F
         fw[:Q] = rng.choice([0.5, 1.0, 2.0], Q)
     snap.set("fair_weight", fw)
     # ---- quotas ----
-    scale = np.array([2_000, 2**31, 4, 100_000, 50, 10, 1000, 64][:R], np.int64)  # mean request per resource
+    scale = _scale(R)
     per_cq = max(1, W // Q)
     k = rng.uniform(4, 16, (Q, F, 1))
     nominal = np.zeros((N, FR), np.int64)
@@ -206,7 +213,7 @@ def add_afs(snap: abi.FlatSnapshot, k: int, seed: int = 0, half_life_s: float = 
     snap.set("wl_lq", snap.arrays["wl_cq"].astype(np.int64) * k + rng.integers(0, k, W))
     snap.set("cq_afs", np.ones(Q))
     snap.set("lq_weight", rng.choice([0.5, 1.0, 1.5, 2.0], L))
-    scale = np.array([2_000, 2**31, 4, 100_000, 50, 10, 1000, 64][:R], np.int64)
+    scale = _scale(R)
     val = (rng.uniform(0, 8, (L, R)) * scale[None, :]).astype(np.int64)
     sc = np.zeros((L, R), np.int64)
     whole = rng.random(L) < 0.5  # cpu as "3" (scale 0) or "3500m" (scale -3)
