@@ -450,6 +450,24 @@ typedef struct kb_snapshot {
   const uint8_t *ac_active;         /* [n_active_change] 0 = set spec.active false (stop), 1 = set it true (resume)   */
   const uint8_t *wl_inactive;       /* [n_wl] start state: 0 = active, 1-4 = inactive with the reason of the
                                        deactivation in force (kb_drain_out.wl_deactivation_reason codes); NULL = all 0 */
+
+  /* ---- reclaim steps (optional; read by kb_run_drain only, kb_run_cycle ignores them) ----
+     Status.ReclaimablePods over a workload's run: step i lowers the Count of podset rc_ps[i] to rc_remaining[i] (spec
+     Count - reclaimable pods) rc_after_ns[i] after the run starts.  wl_rc_start == NULL: the block is off.  The tables
+     turn event mode on and need adm_wl.  See kb_run_drain for the definition and the errors. */
+  int32_t n_reclaim;                /* steps below (= wl_rc_start[n_wl])                                              */
+  const int32_t *wl_rc_start;       /* [n_wl+1] CSR: the steps of record w are [wl_rc_start[w], wl_rc_start[w+1])     */
+  const int64_t *rc_after_ns;       /* [n_reclaim] time of the step after the run starts; > 0, non-decreasing per record */
+  const int32_t *rc_ps;             /* [n_reclaim] podset row, inside the record's wl_ps_start range                  */
+  const int32_t *rc_remaining;      /* [n_reclaim] the podset's Count after the step; >= 0, non-increasing per podset */
+  const int64_t *rc_sched_hash;     /* [n_reclaim] the record's wl_sched_hash after the step; NULL = 0 (unknown)      */
+  /* start state of the snapshot's rows, read for rows whose record (adm_wl) has steps: the Admission's
+     PodSetAssignments, indexed like the podset tables */
+  const int8_t *ps_adm_flavor;      /* [n_podset][R] PodSetAssignment.Flavors, -1 = none                              */
+  const int32_t *ps_adm_count;      /* [n_podset] PodSetAssignment.Count                                              */
+  const int64_t *ps_adm_usage;      /* [n_podset][R] PodSetAssignment.ResourceUsage in library units                  */
+  const int64_t *adm_run_start_ns;  /* [n_adm] run start of a running row; INT64_MIN while its checks run, its
+                                       PodsReady attempt waits or its eviction is under way; NULL = all INT64_MIN     */
 } kb_snapshot;
 
 /* ------------------------------------------------------------------------
@@ -818,7 +836,47 @@ int32_t kb_download(kb_handle *h, kb_cycle_out *out);
  *      the drain equals the drain without the block in every output.
  * n_stopped / n_resumed count the edits that changed the state (rules 2, 3, 5); those applied between the start of
  * cycle c and of c+1 count in cycle_stopped[c] / cycle_resumed[c].  wl_deactivated / wl_deactivation_reason describe
- * the state at the end: 1 and the reason while the record is inactive, 0 after a reactivation. */
+ * the state at the end: 1 and the reason while the record is inactive, 0 after a reactivation.
+ *
+ * Reclaim steps (kb_snapshot.wl_rc_start != NULL: event mode; needs adm_wl).  ReclaimablePods, a feature gate on by
+ * default: the Job, JobSet, TrainJob and Pod integrations write Status.ReclaimablePods as pods succeed (a Job with
+ * completions > parallelism reports parallelism - remaining once remaining < parallelism, job_controller.go:213-227), and
+ * the cache counts only the pods still needed.  Step i of record w lowers podset rc_ps[i] to rc_remaining[i] pods.
+ *   1. run start S: the reservation t_c without a check delay, else the Ready verdict; with WaitForPodsReady the
+ *      PodsReady time of a ready attempt (a failing attempt has no run and takes no steps).  A snapshot row starts at
+ *      adm_run_start_ns, or at the PodsReady time of a ready attempt under way (adm_admitted_ns).  A readmission
+ *      starts a new run that replays the steps from the first;
+ *   2. step i is an event at S + rc_after_ns[i] (E includes it while it can apply).  It applies while the row runs:
+ *      phase running, not evicting, strictly before the row's finish and its effective MaximumExecutionTimeSeconds
+ *      deadline; a step at the finish time is dropped, and a row whose preemption is issued takes no more steps.
+ *      Against a stop (spec.active) of the record at the same time the step goes first.  A step whose rc_remaining is
+ *      not below the podset's current Count changes nothing and is not counted;
+ *   3. in a boundary the steps apply after the quota edits, the check verdicts (a run a Ready verdict starts takes its
+ *      steps in that boundary), the AFS samples, and before the completions; a record's steps go in time order, and
+ *      its steps at one instant are one status update.  Their effects do not depend on the order of the rows;
+ *   4. a step that lowers podset p from Count c to r (totalRequestsFromAdmission workload.go:600-645): the record's
+ *      ps_count[p] = r and ps_req[p][.] = ps_req[p][.] / c * r (the requests of a requeued record,
+ *      totalRequestsFromPodSets :567-598 via podSetsCountsAfterReclaim :547-559; the pods resource, which the caller
+ *      sets to the Count, stays equal to it, and the AFS entry penalty of a later admission reads these requests).  The
+ *      row's usage of p becomes U0 / n * min(r, n) per resource on its assigned flavor, U0 and n the admission's
+ *      ResourceUsage and Count (from the drain's own admission, or ps_adm_*); the difference leaves the row's cells,
+ *      its ClusterQueue's usage and, under AFS decay, its LocalQueue's admitted usage (consumed changes at the next
+ *      sample).  Once per update (workload_controller.go:1005-1014): the ClusterQueue's AllocatableResourceGeneration +1
+ *      (deleteWorkload, clusterqueue.go:477-491), its root tree marked for the inadmissible requeue, and the record's
+ *      scheduling hash set to rc_sched_hash of the step (0 without the table; workload.go:317 hashes the counts);
+ *   5. finishes and releases still leave the generation alone;
+ *   6. the block composes with every block above; stopped and resumed records keep their reduced counts.  With no step
+ *      that lowers a count the drain equals the drain without the block in every output but ps_remaining_out.
+ * A partially admitted snapshot row (ps_adm_count below its Count) follows rule 4's min(r, n).  Steps applied between the
+ * start of cycle c and of c+1 count in cycle_reclaims[c].  The generations go where the quota-change block writes them,
+ * and a kb_run_drain with the block on resets the handle's static generation.  Errors (KB_ERR_INVALID): a table of the
+ * block without adm_wl or without wl_rc_start / rc_after_ns / rc_ps / rc_remaining, wl_rc_start not a CSR of n_reclaim
+ * steps, rc_ps outside its record, rc_after_ns <= 0 or decreasing within a record, rc_remaining negative or increasing
+ * within a podset, ps_req of a podset with steps not divisible by its ps_count, adm_run_start_ns after now_ns or set on
+ * a row that is not running, ps_adm_* missing or out of range for a snapshot row whose record has steps, and such a row
+ * whose ps_adm_* at the current counts do not add up to its adm_use_* cells.  KB_ERR_UNSUPPORTED: steps on a record
+ * that can be partially admitted (KB_F_PARTIAL_ADMISSION and some ps_min_count >= 0): the reference's PodSetReducer
+ * starts from the spec counts (scheduler.go:605), the library's from ps_count. */
 typedef struct kb_drain_out {
   int32_t max_cycles;        /* in */
   int32_t n_cycles;          /* out: cycles run */
@@ -901,6 +959,11 @@ typedef struct kb_drain_out {
   int64_t n_resumed;                     /* out: resume edits that reactivated a record, likewise */
   int32_t *cycle_stopped;                /* [max_cycles] stops from the start of cycle c to the start of c+1 */
   int32_t *cycle_resumed;                /* [max_cycles] resumes, likewise */
+  /* reclaim steps (kb_snapshot.wl_rc_start != NULL; zero / untouched otherwise; each pointer may be NULL).
+     cq_generation is written with it. */
+  int64_t n_reclaims;                    /* out: steps that lowered a count, those before cycle 0 included */
+  int32_t *cycle_reclaims;               /* [max_cycles] such steps from the start of cycle c to the start of c+1 */
+  int32_t *ps_remaining_out;             /* [n_podset] each podset's Count after reclaim at the end of the drain */
 } kb_drain_out;
 int32_t kb_run_drain(kb_handle *h, const kb_snapshot *s, kb_drain_out *out);
 

@@ -394,6 +394,13 @@ func (s *Scheduler) flatten(snap *schdcache.Snapshot, heads []workload.Info, gen
 	// user's stop, read from the Evicted condition's reason), and planned stop / resume edits sorted by time:
 	//   c.wl_inactive = cpU8(inactiveReason)
 	//   c.n_active_change, c.ac_ns, c.ac_wl, c.ac_active = C.int32_t(len(acNs)), cp64(acNs), cp32(acWl), cpU8(acActive)
+	// Reclaim steps (INTEGRATION.md): ps_count / ps_req after Status.ReclaimablePods (spec Count - reclaimable), planned
+	// steps per record (the podset's count after each step, relative to the run start), each admitted row's
+	// Admission.PodSetAssignments[].Flavors / Count / ResourceUsage, and its run start from the Admitted condition's
+	// LastTransitionTime (the PodsReady condition's with waitForPodsReady; math.MinInt64 while the row does not run);
+	// Status.ReclaimablePods = spec Count - kb_drain_out.ps_remaining_out is written back after the drain:
+	//   c.n_reclaim, c.wl_rc_start, c.rc_after_ns, c.rc_ps, c.rc_remaining = C.int32_t(len(rcAfter)), cp32(rcStart), cp64(rcAfter), cp32(rcPs), cp32(rcRemaining)
+	//   c.ps_adm_flavor, c.ps_adm_count, c.ps_adm_usage, c.adm_run_start_ns = cp8(admFlavor), cp32(admCount), cp64(admUsage), cp64(runStart)
 	// They stay nil here: a single cycle ignores them.
 	if anyGroup { // optional table: NULL when no podset is grouped
 		c.ps_group = cp32(psGroup)

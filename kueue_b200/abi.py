@@ -96,6 +96,10 @@ class kb_snapshot(C.Structure):
         ("qc_borrow_limit", _P(C.c_int64)), ("qc_lend_limit", _P(C.c_int64)),
         ("n_active_change", C.c_int32), ("ac_ns", _P(C.c_int64)), ("ac_wl", _P(C.c_int32)), ("ac_active", _P(C.c_uint8)),
         ("wl_inactive", _P(C.c_uint8)),
+        ("n_reclaim", C.c_int32), ("wl_rc_start", _P(C.c_int32)), ("rc_after_ns", _P(C.c_int64)), ("rc_ps", _P(C.c_int32)),
+        ("rc_remaining", _P(C.c_int32)), ("rc_sched_hash", _P(C.c_int64)),
+        ("ps_adm_flavor", _P(C.c_int8)), ("ps_adm_count", _P(C.c_int32)), ("ps_adm_usage", _P(C.c_int64)),
+        ("adm_run_start_ns", _P(C.c_int64)),
     ]
 
 
@@ -158,6 +162,7 @@ class kb_drain_out(C.Structure):
         ("wl_exec_acc_s_out", _P(C.c_int32)), ("wl_deactivation_reason", _P(C.c_uint8)),
         ("n_quota_changes", C.c_int64), ("cycle_quota_changes", _P(C.c_int32)), ("cq_generation", _P(C.c_int64)),
         ("n_stopped", C.c_int64), ("n_resumed", C.c_int64), ("cycle_stopped", _P(C.c_int32)), ("cycle_resumed", _P(C.c_int32)),
+        ("n_reclaims", C.c_int64), ("cycle_reclaims", _P(C.c_int32)), ("ps_remaining_out", _P(C.c_int32)),
     ]
 
 
@@ -221,6 +226,8 @@ _DT = {
     "wl_max_exec_s": np.int32, "wl_exec_acc_s": np.int32, "adm_exec_since_ns": np.int64,
     "qc_ns": np.int64, "qc_node": np.int32, "qc_nominal": np.int64, "qc_borrow_limit": np.int64, "qc_lend_limit": np.int64,
     "ac_ns": np.int64, "ac_wl": np.int32, "ac_active": np.uint8, "wl_inactive": np.uint8,
+    "wl_rc_start": np.int32, "rc_after_ns": np.int64, "rc_ps": np.int32, "rc_remaining": np.int32, "rc_sched_hash": np.int64,
+    "ps_adm_flavor": np.int8, "ps_adm_count": np.int32, "ps_adm_usage": np.int64, "adm_run_start_ns": np.int64,
 }
 # AdmissionFairSharing tables (include/kueue_b200.h): wl_lq absent = AFS off
 AFS_FIELDS = ("wl_lq", "lq_cq", "cq_afs", "lq_weight", "lq_consumed", "lq_consumed_scale", "lq_penalty", "afs_res_weight",
@@ -244,9 +251,13 @@ QUOTA_CHANGE_FIELDS = ("qc_ns", "qc_node", "qc_nominal", "qc_borrow_limit", "qc_
 # workload deactivation / reactivation (include/kueue_b200.h): ac_ns present = edits (event mode), n_active_change =
 # len(ac_ns); wl_inactive = the start state
 ACTIVE_FIELDS = ("ac_ns", "ac_wl", "ac_active", "wl_inactive")
+# reclaim steps (include/kueue_b200.h): wl_rc_start present = the block on (event mode), n_reclaim = wl_rc_start[-1]; the
+# start state of the snapshot's rows (ps_adm_*, adm_run_start_ns) is read for rows whose record has steps
+RECLAIM_FIELDS = ("wl_rc_start", "rc_after_ns", "rc_ps", "rc_remaining", "rc_sched_hash", "ps_adm_flavor", "ps_adm_count",
+                  "ps_adm_usage", "adm_run_start_ns")
 OPTIONAL_FIELDS = (("wl_has_quota_reservation", "wl_sched_hash", "ps_group", "usage_delta_cq", "usage_delta_rows", "adm_wl") + AFS_FIELDS +
                    EVENT_FIELDS + AFS_DECAY_FIELDS + EVICT_END_FIELDS + STICKY_FIELDS + CHECK_FIELDS +
-                   PODS_READY_FIELDS + MAX_EXEC_FIELDS + QUOTA_CHANGE_FIELDS + ACTIVE_FIELDS)  # NULL in kb_snapshot when absent
+                   PODS_READY_FIELDS + MAX_EXEC_FIELDS + QUOTA_CHANGE_FIELDS + ACTIVE_FIELDS + RECLAIM_FIELDS)  # NULL in kb_snapshot when absent
 ARRAY_FIELDS = list(_DT.keys())
 # tables the library keeps resident while kb_snapshot.static_generation is unchanged (include/kueue_b200.h)
 STATIC_FIELDS = ("parent", "fair_weight", "nominal", "borrow_limit", "lend_limit", "cq_within_cq", "cq_reclaim_within",
@@ -398,6 +409,7 @@ class FlatSnapshot:
         s.n_usage_delta = len(self.arrays["usage_delta_cq"]) if "usage_delta_cq" in self.arrays else 0
         s.n_quota_change = len(self.arrays["qc_ns"]) if "qc_ns" in self.arrays else 0
         s.n_active_change = len(self.arrays["ac_ns"]) if "ac_ns" in self.arrays else 0
+        s.n_reclaim = len(self.arrays["rc_after_ns"]) if "rc_after_ns" in self.arrays else 0
         s.n_heads = self.n_heads
         s.pods_resource, s.flags, s.now_ns = self.pods_resource, self.flags, self.now_ns
         s.static_generation = self.static_generation
@@ -516,6 +528,8 @@ class DrainOut:
         self.cq_generation = np.zeros(max(1, Q), np.int64)[:Q]
         self.cycle_stopped = np.zeros(max_cycles, np.int32)  # deactivation / reactivation (kb_snapshot.ac_*)
         self.cycle_resumed = np.zeros(max_cycles, np.int32)
+        self.cycle_reclaims = np.zeros(max_cycles, np.int32)  # reclaim steps (kb_snapshot.wl_rc_start)
+        self.ps_remaining_out = np.zeros(max(1, snap.n_podset), np.int32)[:snap.n_podset]
         cap = (min(W * 4 + Q, min(Q, W) * max_cycles) if trace_capacity is None else trace_capacity) if trace else 0
         self.trace_wl = np.zeros(max(1, cap), np.int32)
         self.trace_decision = np.zeros(max(1, cap), np.uint8)
@@ -550,6 +564,8 @@ class DrainOut:
         s.cq_generation = _ptr(self.cq_generation, C.c_int64)
         s.cycle_stopped = _ptr(self.cycle_stopped, C.c_int32)
         s.cycle_resumed = _ptr(self.cycle_resumed, C.c_int32)
+        s.cycle_reclaims = _ptr(self.cycle_reclaims, C.c_int32)
+        s.ps_remaining_out = _ptr(self.ps_remaining_out, C.c_int32)
         if trace:
             s.trace_wl = _ptr(self.trace_wl, C.c_int32); s.trace_decision = _ptr(self.trace_decision, C.c_uint8)
         s.trace_capacity = cap
@@ -597,6 +613,8 @@ class DrainOut:
     def n_stopped(self): return int(self.struct.n_stopped)
     @property
     def n_resumed(self): return int(self.struct.n_resumed)
+    @property
+    def n_reclaims(self): return int(self.struct.n_reclaims)
 
     def cycles(self):
         """[(heads, decisions)] per cycle from the trace."""

@@ -1363,7 +1363,7 @@ extern "C" int32_t kb_run_cycle(kb_handle *h, const kb_snapshot *s, kb_cycle_out
 // ---------------------------------------------------------------------------
 // what a boundary of kb_run_drain reads back, in the pinned host words [64, 128)
 struct DrainWords {
-  uint32_t counters[KB_DC_AC_HI + 1];   // DrainDev::counters; [0] = heads of the next cycle
+  uint32_t counters[KB_DC_RECLAIMS + 1];  // DrainDev::counters; [0] = heads of the next cycle
   uint32_t n_new, n_cells;              // this cycle's admissions and their usage cells (the admit scans' totals)
   uint32_t status;                      // the cycle's status word (KBS_AFS_OVERFLOW)
   i64 t_next;                           // event mode: t_{c+1}
@@ -1378,7 +1378,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   out->n_finished = 0; out->n_arrived = 0; out->end_ns = s->now_ns; out->n_evict_done = 0;
   out->n_check_ready = 0; out->n_check_retry = 0; out->n_check_rejected = 0; out->n_resorts = 0; out->resort_ms = 0;
   out->n_pods_ready_timeout = 0; out->n_pods_ready_deactivated = 0; out->n_max_exec_deactivated = 0; out->n_quota_changes = 0;
-  out->n_stopped = 0; out->n_resumed = 0;
+  out->n_stopped = 0; out->n_resumed = 0; out->n_reclaims = 0;
   // ---- eviction replay: host-side checks of adm_wl (include/kueue_b200.h)
   const bool replay = s->adm_wl != nullptr;
   if (replay) {
@@ -1397,8 +1397,9 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   const bool quota = s->n_quota_change > 0 && s->qc_ns;  // ClusterQueue / Cohort quota changes
   const bool act = s->n_active_change > 0 && s->ac_ns;    // deactivation / reactivation edits
   const bool blk = act || s->wl_inactive;                 // the block (its start state alone needs no events)
+  const bool rcl = s->wl_rc_start != nullptr;              // reclaim steps
   const bool events = s->wl_create_ns || s->wl_run_ns || s->adm_finish_ns || s->wl_evict_ns || s->wl_check_ns || s->wl_pods_ready_ns ||
-                      s->wl_max_exec_s || quota || act;
+                      s->wl_max_exec_s || quota || act || rcl;
   if (events) {
     if (s->adm_finish_ns)
       for (int a = 0; a < s->n_adm; a++)
@@ -1607,8 +1608,77 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       last[w] = i;
     }
   }
+  // ---- reclaim steps: host-side checks (include/kueue_b200.h), restated by kueue_b200/drain.py check_reclaims
+  const int NRC = rcl ? s->n_reclaim : 0;
+  if (rcl || s->rc_after_ns || s->rc_ps || s->rc_remaining || s->rc_sched_hash || s->ps_adm_flavor || s->ps_adm_count || s->ps_adm_usage ||
+      s->adm_run_start_ns) {
+    if (!replay) return fail(h, KB_ERR_INVALID, "reclaim steps: the tables need adm_wl");
+    if (!rcl || (s->n_reclaim > 0 && (!s->rc_after_ns || !s->rc_ps || !s->rc_remaining)))
+      return fail(h, KB_ERR_INVALID, "reclaim steps: a NULL table (wl_rc_start, rc_after_ns, rc_ps, rc_remaining)");
+    if (s->n_reclaim < 0 || s->wl_rc_start[0] != 0 || s->wl_rc_start[W] != s->n_reclaim)
+      return fail(h, KB_ERR_INVALID, "reclaim steps: wl_rc_start is not a CSR of the steps");
+    for (int w = 0; w < W; w++)
+      if (s->wl_rc_start[w + 1] < s->wl_rc_start[w]) return fail(h, KB_ERR_INVALID, "reclaim steps: wl_rc_start is not a CSR of the steps");
+    for (int w = 0; w < W; w++)
+      for (int i = s->wl_rc_start[w]; i < s->wl_rc_start[w + 1]; i++)
+        if (s->rc_ps[i] < s->wl_ps_start[w] || s->rc_ps[i] >= s->wl_ps_start[w + 1]) return fail(h, KB_ERR_INVALID, "reclaim steps: rc_ps outside its record");
+    for (int w = 0; w < W; w++)
+      for (int i = s->wl_rc_start[w]; i < s->wl_rc_start[w + 1]; i++)
+        if (s->rc_after_ns[i] <= 0 || (i > s->wl_rc_start[w] && s->rc_after_ns[i] < s->rc_after_ns[i - 1]))
+          return fail(h, KB_ERR_INVALID, "reclaim steps: rc_after_ns <= 0 or decreasing within a record");
+    std::vector<int32_t> last((size_t)std::max(1, s->n_podset), INT32_MAX);
+    for (int i = 0; i < NRC; i++) {
+      const int p = s->rc_ps[i];
+      if (s->rc_remaining[i] < 0 || s->rc_remaining[i] > last[p]) return fail(h, KB_ERR_INVALID, "reclaim steps: rc_remaining negative or increasing within a podset");
+      last[p] = s->rc_remaining[i];
+    }
+    for (int p = 0; p < s->n_podset; p++)
+      if (last[p] != INT32_MAX && s->ps_count[p] > 0)
+        for (int r = 0; r < R; r++)
+          if (s->ps_req[(size_t)p * R + r] % s->ps_count[p] != 0) return fail(h, KB_ERR_INVALID, "reclaim steps: ps_req of a podset with steps not divisible by its ps_count");
+    if (s->flags & KB_F_PARTIAL_ADMISSION)
+      for (int w = 0; w < W; w++)
+        if (s->wl_rc_start[w + 1] > s->wl_rc_start[w])
+          for (int p = s->wl_ps_start[w]; p < s->wl_ps_start[w + 1]; p++)
+            if (s->ps_min_count[p] >= 0) return fail(h, KB_ERR_UNSUPPORTED, "reclaim steps: steps on a record that can be partially admitted");
+    if (s->adm_run_start_ns)
+      for (int a = 0; a < s->n_adm; a++) {
+        const i64 S = s->adm_run_start_ns[a];
+        if (S != INT64_MIN && S > s->now_ns) return fail(h, KB_ERR_INVALID, "reclaim steps: adm_run_start_ns after now_ns");
+      }
+    if (s->adm_run_start_ns)
+      for (int a = 0; a < s->n_adm; a++) {
+        const bool idle = (s->adm_evicted && s->adm_evicted[a]) || (s->adm_check_end_ns && s->adm_check_end_ns[a] != INT64_MIN) ||
+                          (s->adm_admitted_ns && s->adm_admitted_ns[a] != INT64_MIN);
+        if (s->adm_run_start_ns[a] != INT64_MIN && idle) return fail(h, KB_ERR_INVALID, "reclaim steps: adm_run_start_ns on a row that is not running");
+      }
+    bool any_row = false;
+    for (int a = 0; a < s->n_adm; a++) any_row |= s->wl_rc_start[s->adm_wl[a] + 1] > s->wl_rc_start[s->adm_wl[a]];
+    if (any_row && (!s->ps_adm_flavor || !s->ps_adm_count || !s->ps_adm_usage))
+      return fail(h, KB_ERR_INVALID, "reclaim steps: ps_adm_* missing for a row whose record has steps");
+    for (int a = 0; a < s->n_adm && any_row; a++) {
+      const int w = s->adm_wl[a];
+      if (s->wl_rc_start[w + 1] == s->wl_rc_start[w]) continue;
+      std::map<int, i64> want, have;
+      for (int p = s->wl_ps_start[w]; p < s->wl_ps_start[w + 1]; p++)
+        for (int r = 0; r < R; r++) {
+          const int f = s->ps_adm_flavor[(size_t)p * R + r];
+          const i64 u = s->ps_adm_usage[(size_t)p * R + r];
+          const int n = s->ps_adm_count[p];
+          if (f < -1 || f >= s->n_flavor || n < 0 || u < 0) return fail(h, KB_ERR_INVALID, "reclaim steps: ps_adm_* out of range");
+          if (f >= 0 && n > 0) want[f * R + r] += u / n * std::min(s->ps_count[p], n);
+        }
+      for (int c = s->adm_use_start[a]; c < s->adm_use_start[a + 1]; c++) have[s->adm_use_fr[c]] += s->adm_use_qty[c];
+      for (auto *m : {&want, &have})
+        for (auto it = m->begin(); it != m->end();) it = it->second == 0 ? m->erase(it) : std::next(it);
+      if (want != have) return fail(h, KB_ERR_INVALID, "reclaim steps: a row's ps_adm_* do not add up to its adm_use cells");
+    }
+  }
   out->n_afs_samples = 0;
-  if (Hcap == 0 || max_cycles == 0) return KB_OK;
+  if (Hcap == 0 || max_cycles == 0) {
+    if (rcl && out->ps_remaining_out && s->n_podset) memcpy(out->ps_remaining_out, s->ps_count, (size_t)s->n_podset * 4);
+    return KB_OK;
+  }
   size_t extra = (size_t)std::min<long long>((long long)W, (long long)Hcap * max_cycles);
   h->drain_extra_adm = extra;
   h->drain_extra_au = std::min<size_t>((size_t)s->n_podset * R, extra * (size_t)FR);
@@ -1664,17 +1734,23 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   size_t scan_bytes = 0;
   if (compact) cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (int32_t *)nullptr, (int32_t *)nullptr, (int)Acap + 1, h->stream);
   const size_t nR = (size_t)std::max(1, D.nRoots);
-  std::vector<int32_t> wl_class, cq_class_start;
+  std::vector<int32_t> wl_class, cq_class_start, rc_class;
   int n_class = 0;
-  if (events && s->wl_create_ns && s->wl_sched_hash) {  // dense class id per (BestEffortFIFO ClusterQueue, known hash)
+  if (events && s->wl_create_ns && s->wl_sched_hash) {  // dense class id per (BestEffortFIFO ClusterQueue, known hash),
+    // the hashes reclaim steps set included (a value >= W names step value - W)
     std::vector<std::pair<std::pair<int32_t, int64_t>, int32_t>> cls;
     for (int w = 0; w < W; w++)
       if (s->wl_sched_hash[w] != 0 && s->cq_strategy[s->wl_cq[w]] != KB_QUEUE_STRICT_FIFO) cls.push_back({{s->wl_cq[w], s->wl_sched_hash[w]}, w});
+    if (rcl && s->rc_sched_hash)
+      for (int w = 0; w < W; w++)
+        for (int i = s->wl_rc_start[w]; i < s->wl_rc_start[w + 1]; i++)
+          if (s->rc_sched_hash[i] != 0 && s->cq_strategy[s->wl_cq[w]] != KB_QUEUE_STRICT_FIFO) cls.push_back({{s->wl_cq[w], s->rc_sched_hash[i]}, W + i});
     std::sort(cls.begin(), cls.end());
-    wl_class.assign(Wz, -1); cq_class_start.assign((size_t)Q + 1, 0);
+    wl_class.assign(Wz, -1); cq_class_start.assign((size_t)Q + 1, 0); rc_class.assign((size_t)std::max(1, NRC), -1);
     for (size_t i = 0; i < cls.size(); i++) {
       if (i > 0 && cls[i].first != cls[i - 1].first) n_class++;
-      wl_class[cls[i].second] = n_class;
+      if (cls[i].second < W) wl_class[cls[i].second] = n_class;
+      else rc_class[cls[i].second - W] = n_class;
       cq_class_start[cls[i].first.first + 1] = n_class + 1;
     }
     if (!cls.empty()) n_class++;
@@ -1690,6 +1766,9 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   i64 *ac_ns_d = nullptr;
   int32_t *ac_wl_d = nullptr, *ac_next_d = nullptr, *ac_prev_d = nullptr;
   uint8_t *ac_on_d = nullptr, *inactive_d = nullptr;
+  int32_t *rc_start_d = nullptr, *rc_ps_d = nullptr, *rc_rem_d = nullptr, *rc_class_d = nullptr, *rc_blob_gen_d = nullptr;
+  i64 *rc_after_d = nullptr, *rc_hash_d = nullptr;
+  const size_t Pz = (size_t)std::max(1, s->n_podset), NRCz = (size_t)std::max(1, NRC);
   int32_t *qc_node_d = nullptr, *qc_root_d = nullptr, *qc_tree_d = nullptr, *qc_tree_next_d = nullptr, *qc_cq_start_d = nullptr, *qc_cq_d = nullptr, *qc_blob_gen_d = nullptr;
   DrainDev X{};
   AdmTabs other{};  // compaction: the other half of the admitted tables' double buffer
@@ -1703,7 +1782,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     X.flag = a.take<int32_t>((size_t)Q + 2); X.pos = a.take<int32_t>((size_t)Q + 2);
     X.e_assumed = a.take<int32_t>(Hz + 2); X.e_ncells = a.take<int32_t>(Hz + 2);
     X.e_adm_off = a.take<int32_t>(Hz + 2); X.e_cell_off = a.take<int32_t>(Hz + 2);
-    X.counters = a.take<int32_t>(KB_DC_AC_HI + 1);
+    X.counters = a.take<int32_t>(KB_DC_RECLAIMS + 1);
     X.wl_admit_cycle = a.take<int32_t>(Wz); X.wl_evals = a.take<int32_t>(Wz); X.wl_last_decision = a.take<uint8_t>(Wz);
     if (trace_cap) { X.trace_wl = a.take<int32_t>(trace_cap); X.trace_dec = a.take<uint8_t>(trace_cap); }
     if (replay || events) {
@@ -1779,6 +1858,15 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       ac_ns_d = a.take<i64>(NAC); ac_wl_d = a.take<int32_t>(NAC); ac_on_d = a.take<uint8_t>(NAC);
       ac_next_d = a.take<int32_t>(NAC); ac_prev_d = a.take<int32_t>(NAC);
       X.wl_ac_from = a.take<int32_t>(Wz); X.wl_stop = a.take<i64>(Wz); X.wl_gone = a.take<i64>(Wz);
+    }
+    if (rcl) {  // the steps, the records' assignments, the two row columns of both halves, the generations' blob offsets
+      rc_start_d = a.take<int32_t>(Wz + 1); rc_after_d = a.take<i64>(NRCz); rc_ps_d = a.take<int32_t>(NRCz); rc_rem_d = a.take<int32_t>(NRCz);
+      if (s->rc_sched_hash) rc_hash_d = a.take<i64>(NRCz);
+      if (n_class) rc_class_d = a.take<int32_t>(NRCz);
+      X.ps_adm_cnt = a.take<int32_t>(Pz); X.ps_adm_fl = a.take<int8_t>(Pz * R); X.ps_adm_use = a.take<i64>(Pz * R);
+      X.adm_rc_next = a.take<i64>(Acap); other.rc_next = a.take<i64>(Acap);
+      X.adm_rc_cur = a.take<int32_t>(Acap); other.rc_cur = a.take<int32_t>(Acap);
+      rc_blob_gen_d = a.take<int32_t>((size_t)std::max(1, Q));
     }
   };
   if (!h->drain_arena.carve(layout)) return fail(h, KB_ERR_CUDA, "kb_run_drain: cudaMalloc of the drain buffer failed");
@@ -1958,6 +2046,17 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     CUDA_TRY(h, cudaMemsetAsync(X.afs_samples, 0, 8, h->stream));
     X.half_life_ns = s->afs_half_life_ns; X.sampling_ns = s->afs_sampling_ns;
   }
+  auto blob_gen = [&]() {  // byte offset of every ClusterQueue's generation in the static tree blocks, -1 = not in a tree
+    std::vector<int32_t> off((size_t)std::max(1, Q), -1);
+    for (int q = 0; q < Q; q++) {
+      const int slot = h->root_slot[q];
+      if (slot < D.nLone) continue;
+      const int tr = slot - D.nLone, b0 = h->tree_blob_off[tr];
+      const TreeBlobHdr *BH = (const TreeBlobHdr *)(h->tree_blob.data() + b0);
+      off[q] = b0 + BH->gen + 8 * h->local_idx[q];
+    }
+    return off;
+  };
   if (quota) {  // quota_prep: no-op edits, roots and trees of the others; the ClusterQueues of every root; the blob offsets
     std::vector<i64> nom(s->nominal, s->nominal + (size_t)QN * FR), bl(s->borrow_limit, s->borrow_limit + (size_t)QN * FR),
         ll(s->lend_limit, s->lend_limit + (size_t)QN * FR);  // the rows each edit meets
@@ -1980,14 +2079,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     qc_cq.assign((size_t)std::max(1, Q), 0);
     std::vector<int32_t> fill(qc_cq_start.begin(), qc_cq_start.end() - 1);
     for (int q = 0; q < Q; q++) qc_cq[fill[h->root_slot[q]]++] = q;
-    qc_blob_gen.assign((size_t)std::max(1, Q), -1);
-    for (int q = 0; q < Q; q++) {
-      const int slot = h->root_slot[q];
-      if (slot < D.nLone) continue;
-      const int tr = slot - D.nLone, b0 = h->tree_blob_off[tr];
-      const TreeBlobHdr *BH = (const TreeBlobHdr *)(h->tree_blob.data() + b0);
-      qc_blob_gen[q] = b0 + BH->gen + 8 * h->local_idx[q];
-    }
+    qc_blob_gen = blob_gen();
     CUDA_TRY(h, h2d(h, qc_ns_d, s->qc_ns, (size_t)NQC * 8));
     CUDA_TRY(h, h2d(h, qc_node_d, s->qc_node, (size_t)NQC * 4));
     CUDA_TRY(h, h2d(h, qc_rows_d[0], s->qc_nominal, (size_t)NQC * FR * 8));
@@ -2003,6 +2095,48 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     X.qc_ns = qc_ns_d; X.qc_node = qc_node_d; X.qc_nominal = qc_rows_d[0]; X.qc_blimit = qc_rows_d[1]; X.qc_llimit = qc_rows_d[2];
     X.qc_root = qc_root_d; X.qc_tree = qc_tree_d; X.qc_tree_next = qc_tree_next_d; X.qc_cq_start = qc_cq_start_d; X.qc_cq = qc_cq_d; X.qc_blob_gen = qc_blob_gen_d;
     X.n_qc = NQC;
+  }
+  std::vector<i64> rc_next;  // reclaim steps: the snapshot's running rows with steps start at their run start
+  std::vector<int32_t> rc_cur, rc_blob_gen;
+  std::vector<int8_t> adm_fl;
+  std::vector<int32_t> adm_cnt;
+  std::vector<i64> adm_use;
+  if (rcl) {
+    rc_next.assign((size_t)std::max(1, s->n_adm), INT64_MAX); rc_cur.assign((size_t)std::max(1, s->n_adm), 0);
+    adm_fl.assign(Pz * R, -1); adm_cnt.assign(Pz, 0); adm_use.assign(Pz * R, 0);
+    for (int a = 0; a < s->n_adm; a++) {
+      const int w = s->adm_wl[a], i = s->wl_rc_start[w];
+      if (i == s->wl_rc_start[w + 1]) continue;
+      const size_t p0 = s->wl_ps_start[w], p1 = s->wl_ps_start[w + 1];
+      memcpy(&adm_fl[p0 * R], s->ps_adm_flavor + p0 * R, (p1 - p0) * R);
+      memcpy(&adm_cnt[p0], s->ps_adm_count + p0, (p1 - p0) * 4);
+      memcpy(&adm_use[p0 * R], s->ps_adm_usage + p0 * R, (p1 - p0) * R * 8);
+      i64 S = s->adm_run_start_ns ? s->adm_run_start_ns[a] : INT64_MIN;
+      if (S == INT64_MIN && pr && s->adm_admitted_ns && s->adm_admitted_ns[a] != INT64_MIN) S = pr_at[w];  // a ready attempt under way
+      if (S == INT64_MIN) continue;
+      rc_cur[a] = i;
+      rc_next[a] = S > INT64_MAX - s->rc_after_ns[i] ? INT64_MAX : S + s->rc_after_ns[i];
+    }
+    rc_blob_gen = blob_gen();
+    CUDA_TRY(h, h2d(h, rc_start_d, s->wl_rc_start, (Wz + 1) * 4));
+    if (NRC) {
+      CUDA_TRY(h, h2d(h, rc_after_d, s->rc_after_ns, (size_t)NRC * 8));
+      CUDA_TRY(h, h2d(h, rc_ps_d, s->rc_ps, (size_t)NRC * 4));
+      CUDA_TRY(h, h2d(h, rc_rem_d, s->rc_remaining, (size_t)NRC * 4));
+      if (rc_hash_d) CUDA_TRY(h, h2d(h, rc_hash_d, s->rc_sched_hash, (size_t)NRC * 8));
+      if (rc_class_d) CUDA_TRY(h, h2d(h, rc_class_d, rc_class.data(), (size_t)NRC * 4));
+    }
+    CUDA_TRY(h, h2d(h, X.ps_adm_fl, adm_fl.data(), adm_fl.size()));
+    CUDA_TRY(h, h2d(h, X.ps_adm_cnt, adm_cnt.data(), adm_cnt.size() * 4));
+    CUDA_TRY(h, h2d(h, X.ps_adm_use, adm_use.data(), adm_use.size() * 8));
+    if (s->n_adm) {
+      CUDA_TRY(h, h2d(h, X.adm_rc_next, rc_next.data(), (size_t)s->n_adm * 8));
+      CUDA_TRY(h, h2d(h, X.adm_rc_cur, rc_cur.data(), (size_t)s->n_adm * 4));
+    }
+    CUDA_TRY(h, h2d(h, rc_blob_gen_d, rc_blob_gen.data(), rc_blob_gen.size() * 4));
+    CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_RECLAIMS, 0, 4, h->stream));  // once: the boundaries never clear it
+    X.wl_rc_start = rc_start_d; X.rc_after = rc_after_d; X.rc_ps = rc_ps_d; X.rc_remaining = rc_rem_d; X.rc_hash = rc_hash_d;
+    X.rc_class = rc_class_d; X.rc_blob_gen = rc_blob_gen_d;
   }
   // ---- per-ClusterQueue order (queueOrderingFunc): stable LSD passes uid -> timestamp -> (ClusterQueue | priority desc)
   const int tb = 256, nbW = (W + tb - 1) / tb, nbQ = (Q + tb - 1) / tb;
@@ -2081,6 +2215,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   }
   uint32_t exec_seen = 0;  // cumulative MaximumExecutionTimeExceeded deactivations at the previous boundary
   uint32_t active_seen[2] = {0, 0};  // cumulative stops / resumes, likewise
+  uint32_t reclaims_seen = 0;        // cumulative reclaim steps, likewise
   const int nbAc = std::max(1, std::min((NAC + tb - 1) / tb, std::max(1, h->sm_count)));  // grid-stride over a boundary's edits
   if (mx) CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_EXEC_DEACTIVATED, 0, 2 * 4, h->stream));  // once, likewise
   // ---- one boundary per iteration, one synchronisation each (kueue_b200/drain.py): cycle c at t (in event mode, a
@@ -2152,7 +2287,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (!jump) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_new, n_new_d, 4, cudaMemcpyDeviceToHost, h->stream));
     if (!compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_cells, X.e_cell_off + n_live, 4, cudaMemcpyDeviceToHost, h->stream));
     if (afs && (!jump || decay)) CUDA_TRY(h, cudaMemcpyAsync(&hw.status, D.status, 4, cudaMemcpyDeviceToHost, h->stream));
-    if (compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[1], X.counters + 1, (act ? KB_DC_AC_HI : quota ? KB_DC_QC_HI : mx ? KB_DC_EXEC_STATUS : pr ? KB_DC_PR_DEACTIVATED : checks ? KB_DC_CHECK_REJECTED : events ? KB_DC_ARR_HI : KB_DC_FULL) * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[1], X.counters + 1, (rcl ? KB_DC_RECLAIMS : act ? KB_DC_AC_HI : quota ? KB_DC_QC_HI : mx ? KB_DC_EXEC_STATUS : pr ? KB_DC_PR_DEACTIVATED : checks ? KB_DC_CHECK_REJECTED : events ? KB_DC_ARR_HI : KB_DC_FULL) * 4, cudaMemcpyDeviceToHost, h->stream));
     if (events) CUDA_TRY(h, cudaMemcpyAsync(&hw.t_next, X.clock, 8, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     if (!jump) {
@@ -2181,6 +2316,7 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
       if (quota && out->cycle_quota_changes) out->cycle_quota_changes[cyc] = 0;
       if (act && out->cycle_stopped) out->cycle_stopped[cyc] = 0;
       if (act && out->cycle_resumed) out->cycle_resumed[cyc] = 0;
+      if (rcl && out->cycle_reclaims) out->cycle_reclaims[cyc] = 0;
       out->n_decisions += n_live; out->n_admitted += n_new; out->n_evicted += n_ev;
       out->n_cycles = ++cyc;
     } else {
@@ -2237,6 +2373,12 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
         if (out->cycle_resumed) out->cycle_resumed[cyc - 1] += re;
       }
     }
+    if (rcl) {  // reclaim steps that lowered a count at this boundary
+      const int n = (int)(hw.counters[KB_DC_RECLAIMS] - reclaims_seen);
+      reclaims_seen = hw.counters[KB_DC_RECLAIMS];
+      out->n_reclaims += n;
+      if (cyc > 0 && out->cycle_reclaims) out->cycle_reclaims[cyc - 1] += n;
+    }
     if (lat) {  // evictions completed at this boundary (counter slot 4, inside the events copy)
       const int done = (int)hw.counters[KB_DC_EVICT_DONE];
       out->n_evict_done += done;
@@ -2245,11 +2387,11 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     if (compact) {  // the compacted half becomes the admitted tables of the next boundary
       A_cur = (int)hw.counters[KB_DC_ROWS]; AU_cur = (int)hw.counters[KB_DC_CELLS];
       AdmTabs cur{X.adm_cq, X.adm_priority, X.adm_ts, X.adm_qr_ts, X.adm_uid, X.adm_evicted, X.adm_use_start, X.adm_use_fr, X.adm_use_qty, X.adm_wl, X.adm_finish, X.adm_lq,
-                  X.adm_evicting, X.adm_phase, X.adm_exec_since};
+                  X.adm_evicting, X.adm_phase, X.adm_exec_since, X.adm_rc_next, X.adm_rc_cur};
       X.adm_cq = other.cq; X.adm_priority = other.priority; X.adm_ts = other.ts; X.adm_qr_ts = other.qr_ts; X.adm_uid = other.uid;
       X.adm_evicted = other.evicted; X.adm_use_start = other.use_start; X.adm_use_fr = other.use_fr; X.adm_use_qty = other.use_qty; X.adm_wl = other.wl;
       X.adm_finish = other.finish; X.adm_lq = other.lq; X.adm_evicting = other.evicting; X.adm_phase = other.phase;
-      X.adm_exec_since = other.since;
+      X.adm_exec_since = other.since; X.adm_rc_next = other.rc_next; X.adm_rc_cur = other.rc_cur;
       D.adm_cq = X.adm_cq; D.adm_priority = X.adm_priority; D.adm_ts = X.adm_ts; D.adm_qr_ts = X.adm_qr_ts; D.adm_uid = X.adm_uid;
       D.adm_evicted = X.adm_evicted; D.adm_use_start = X.adm_use_start; D.adm_use_fr = X.adm_use_fr; D.adm_use_qty = X.adm_use_qty;
       other = cur;
@@ -2317,7 +2459,8 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
   if (out->ps_flavor && PR) CUDA_TRY(h, cudaMemcpyAsync(out->ps_flavor, D.ps_flavor, PR, cudaMemcpyDeviceToHost, h->stream));
   if (out->ps_count && D.P) CUDA_TRY(h, cudaMemcpyAsync(out->ps_count, D.ps_count_out, (size_t)D.P * 4, cudaMemcpyDeviceToHost, h->stream));
   if (out->cq_usage) CUDA_TRY(h, cudaMemcpyAsync(out->cq_usage, D.cq_usage, (size_t)Q * FR * 8, cudaMemcpyDeviceToHost, h->stream));
-  if (quota && out->cq_generation) CUDA_TRY(h, cudaMemcpyAsync(out->cq_generation, D.cq_generation, (size_t)Q * 8, cudaMemcpyDeviceToHost, h->stream));
+  if (rcl && out->ps_remaining_out && D.P) CUDA_TRY(h, cudaMemcpyAsync(out->ps_remaining_out, D.ps_count, (size_t)D.P * 4, cudaMemcpyDeviceToHost, h->stream));
+  if ((quota || rcl) && out->cq_generation) CUDA_TRY(h, cudaMemcpyAsync(out->cq_generation, D.cq_generation, (size_t)Q * 8, cudaMemcpyDeviceToHost, h->stream));
   size_t nt = std::min<size_t>(trace_cap, (size_t)out->n_decisions);
   if (nt) {
     CUDA_TRY(h, cudaMemcpyAsync(out->trace_wl, X.trace_wl, nt * 4, cudaMemcpyDeviceToHost, h->stream));
@@ -2333,7 +2476,7 @@ extern "C" int32_t kb_run_drain(kb_handle *h, const kb_snapshot *s, kb_drain_out
   if (!h || !s || !out) return KB_ERR_INVALID;
   int32_t rc = drain_impl(h, s, out);
   h->drain_mode = false; h->drain_events = false; h->drain_extra_adm = 0; h->drain_extra_au = 0;
-  if (s->n_quota_change > 0 && s->qc_ns) h->static_gen = 0;  // quota changes edited the resident static tables
+  if ((s->n_quota_change > 0 && s->qc_ns) || s->wl_rc_start) h->static_gen = 0;  // quota changes or reclaim steps edited the resident static tables
   h->uploaded = false;  // the resident snapshot was consumed (queues advanced, admitted tables grown)
   return rc;
 }

@@ -74,6 +74,13 @@
 // deactivated and the row becomes KB_PH_TIMED_OUT, whose release sends a deactivated record to DEACTIVATED.
 // drain_exec_release adds an attempt's seconds at every release of a row with an Admitted time (k_drain_finish, and
 // k_drain_evict without latency) and deactivates a record whose deadline passed before the release.
+//
+// Reclaim steps (kb_snapshot.wl_rc_start) add two row columns (both halves, carried by the compaction): adm_rc_next, the
+// time of the row's next step, and adm_rc_cur, its index.  drain_rc_begin starts a run (k_drain_admit, and a Ready
+// verdict in k_drain_finish), which also records the admission's PodSetAssignment per podset (ps_adm_*; the snapshot's
+// rows bring theirs).  k_drain_ev_min folds the next step of a running row into E, and k_drain_finish applies the steps
+// due (drain_reclaim) before a row's completion, its stop or its expiry: a thread per row, integer atomics on the usage
+// tables, one writer for the record's ps_count / ps_req / wl_sched_hash (a record holds at most one row).
 #pragma once
 
 #include <cub/device/device_scan.cuh>
@@ -289,7 +296,7 @@ struct DrainDev {
   const u64 *arr_key;              // [n_arr] creation times (sign flipped) of the ABSENT workloads, ascending
   const int32_t *arr_order;        // [n_arr] their indices, ties by index
   int n_arr;
-  const int32_t *wl_class;         // [W] (ClusterQueue, hash) class of a BestEffortFIFO workload with a known hash, -1
+  int32_t *wl_class;               // [W] (ClusterQueue, hash) class of a BestEffortFIFO workload with a known hash, -1
   const int32_t *cq_class_start;   // [Q+1] classes of a ClusterQueue
   uint8_t *class_nofit;            // [classes] in the ClusterQueue's NoFit set; null = no arrivals or no hashes
   // eviction latency (event mode); wl_evict == nullptr: off
@@ -337,6 +344,19 @@ struct DrainDev {
   i64 *wl_stop;                    // [W] stop time of an active row-holding record at this boundary, INT64_MAX = none
   i64 *wl_gone;                    // [W] time its row went at this boundary, INT64_MIN = none
   int n_ac;
+  // reclaim steps (event mode); wl_rc_start == nullptr: off.  D.ps_count / ps_req / wl_sched_hash are the records'
+  // mutable counts and requests after reclaim.
+  const int32_t *wl_rc_start;      // [W+1] CSR of each record's steps
+  const i64 *rc_after;             // [n_rc] time of the step after the run starts
+  const int32_t *rc_ps, *rc_remaining;  // [n_rc] podset row / its count after the step
+  const i64 *rc_hash;              // [n_rc] the record's scheduling hash after the step; null = 0
+  const int32_t *rc_class;         // [n_rc] NoFit class of that hash (wl_class), -1 = none
+  int32_t *ps_adm_cnt;             // [P] the held row's PodSetAssignment.Count
+  int8_t *ps_adm_fl;               // [P][R] its flavors, -1 = none
+  i64 *ps_adm_use;                 // [P][R] its ResourceUsage
+  i64 *adm_rc_next;                // [A_cap] time of each row's next step (current half), INT64_MAX = none
+  int32_t *adm_rc_cur;             // [A_cap] index of that step (current half)
+  const int32_t *rc_blob_gen;      // [Q] byte offset of the ClusterQueue's generation in tree_blob, -1 = not in a tree
 };
 // adm_phase: what the finish column of a row holds.  RUN: its finish (or its eviction's end when adm_evicting); CHECK: its
 // checks' verdict; WAIT: the timeout T of a PodsReady attempt that fails; TIMED_OUT: the end of its eviction by that
@@ -351,12 +371,14 @@ enum { KB_DR_REJECTED = 1, KB_DR_REQUEUING_LIMIT = 2, KB_DR_MAX_EXEC = 3, KB_DR_
 // WaitForPodsReady: [15] / [16] timeouts that requeue / deactivate since the start, likewise; MaximumExecutionTimeSeconds:
 // [17] deactivations since the start, [18] KBS_EXEC_OVERFLOW once an accumulated time leaves int32 (never cleared);
 // quota changes: [19] / [20] the edits of this boundary [lo, hi) (hi = edits applied since the start); deactivation:
-// [21] / [22] stops / resumes that changed the state since the start, [23] / [24] the edits of this boundary [lo, hi)
+// [21] / [22] stops / resumes that changed the state since the start, [23] / [24] the edits of this boundary [lo, hi);
+// reclaim steps: [25] steps that lowered a count since the start
 enum { KB_DC_EVICTED = 1, KB_DC_ROWS = 2, KB_DC_CELLS = 3, KB_DC_EVICT_DONE = 4, KB_DC_FULL = 5,
        KB_DC_FINISHED = 6, KB_DC_ARRIVED = 7, KB_DC_END = 8, KB_DC_ARR_LO = 9, KB_DC_ARR_HI = 10,
        KB_DC_RESORT = 11, KB_DC_CHECK_READY = 12, KB_DC_CHECK_RETRY = 13, KB_DC_CHECK_REJECTED = 14,
        KB_DC_PR_TIMEOUT = 15, KB_DC_PR_DEACTIVATED = 16, KB_DC_EXEC_DEACTIVATED = 17, KB_DC_EXEC_STATUS = 18,
-       KB_DC_QC_LO = 19, KB_DC_QC_HI = 20, KB_DC_STOPPED = 21, KB_DC_RESUMED = 22, KB_DC_AC_LO = 23, KB_DC_AC_HI = 24 };
+       KB_DC_QC_LO = 19, KB_DC_QC_HI = 20, KB_DC_STOPPED = 21, KB_DC_RESUMED = 22, KB_DC_AC_LO = 23, KB_DC_AC_HI = 24,
+       KB_DC_RECLAIMS = 25 };
 
 __device__ __forceinline__ int drain_seg0(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq] : cq; }
 __device__ __forceinline__ int drain_seg1(const DrainDev &X, int cq) { return X.seg_start ? X.seg_start[cq + 1] : cq + 1; }
@@ -596,6 +618,65 @@ __device__ __forceinline__ bool drain_exec_release(const DrainDev &X, int a, int
   return deact;
 }
 
+// ---- reclaim steps ------------------------------------------------------------------------------------------------
+// the run of row a (record w) starts at S: its steps replay from the first
+__device__ __forceinline__ void drain_rc_begin(const DrainDev &X, int a, int w, i64 S) {
+  const int i = X.wl_rc_start[w];
+  X.adm_rc_cur[a] = i;
+  X.adm_rc_next[a] = i < X.wl_rc_start[w + 1] ? drain_sat_add(S, X.rc_after[i]) : INT64_MAX;
+}
+// row a can take a step: not evicting, phase running (its run started: adm_rc_next is INT64_MAX otherwise)
+__device__ __forceinline__ bool drain_rc_live(const DrainDev &X, int a) {
+  if (X.adm_evicting && X.adm_evicting[a]) return false;
+  return !X.adm_phase || X.adm_phase[a] == KB_PH_RUN || X.adm_phase[a] == KB_PH_EXPIRE;
+}
+// the steps of running row a due at or before lim, in time order (rule 4 of kb_run_drain): a step that lowers podset p
+// from c to r scales the record's requests to r pods and the row's usage of p to U0 / n * min(r, n) per resource; the
+// difference leaves the row's cells, the ClusterQueue usage and the LocalQueue's admitted usage (integer atomics).  The
+// steps of one instant are one update: generation + 1 (the cycle's copy and the tree block's), root tree marked.
+__device__ void drain_reclaim(const DevSnap &D, const DrainDev &X, int a, i64 lim) {
+  i64 t = X.adm_rc_next[a];
+  if (t > lim) return;
+  const int w = X.adm_wl[a], cq = X.adm_cq[a], R = D.R, i1 = X.wl_rc_start[w + 1];
+  int i = X.adm_rc_cur[a], n = 0;
+  const i64 S = t - X.rc_after[i];  // t <= lim < INT64_MAX: not saturated
+  int32_t *cnt = const_cast<int32_t *>(D.ps_count);
+  i64 *req = const_cast<i64 *>(D.ps_req), *hash = const_cast<i64 *>(D.wl_sched_hash);
+  while (i < i1 && t <= lim) {
+    bool lowered = false;
+    for (; i < i1 && drain_sat_add(S, X.rc_after[i]) == t; i++) {
+      const int p = X.rc_ps[i], rem = X.rc_remaining[i], c = cnt[p];
+      if (rem >= c) continue;  // counts only go down
+      for (int r = 0; r < R; r++) req[(size_t)p * R + r] = req[(size_t)p * R + r] / c * rem;
+      const int na = X.ps_adm_cnt[p];
+      for (int r = 0; r < R && na > 0; r++) {
+        const int f = X.ps_adm_fl[(size_t)p * R + r];
+        if (f < 0) continue;
+        const i64 u = X.ps_adm_use[(size_t)p * R + r] / na, d = u * min(rem, na) - u * min(c, na);
+        if (d == 0) continue;
+        const int fr = f * R + r;
+        for (int k = X.adm_use_start[a]; k < X.adm_use_start[a + 1]; k++)
+          if (X.adm_use_fr[k] == fr) { X.adm_use_qty[k] += d; break; }
+        atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + fr], (unsigned long long)d);
+        if (X.lq_last && X.adm_lq[a] >= 0 && X.cq_afs[cq])
+          atomicAdd((unsigned long long *)&X.lq_adm[(size_t)X.adm_lq[a] * R + r], (unsigned long long)d);
+      }
+      cnt[p] = rem;
+      if (hash) { hash[w] = X.rc_hash ? X.rc_hash[i] : 0; if (X.wl_class) X.wl_class[w] = X.rc_class[i]; }
+      lowered = true;
+      n++;
+    }
+    if (lowered) {  // AddOrUpdateWorkload -> deleteWorkload: AllocatableResourceGeneration + 1; the root tree requeued
+      atomicAdd((unsigned long long *)&D.cq_generation[cq], 1ull);
+      if (X.rc_blob_gen[cq] >= 0) atomicAdd((unsigned long long *)(D.tree_blob + X.rc_blob_gen[cq]), 1ull);
+      X.root_mark[D.root_slot[cq]] = X.cycle + 1;
+    }
+    t = i < i1 ? drain_sat_add(S, X.rc_after[i]) : INT64_MAX;
+  }
+  X.adm_rc_cur[a] = i; X.adm_rc_next[a] = t;
+  if (n) atomicAdd(&X.counters[KB_DC_RECLAIMS], n);
+}
+
 // admitted entries join the admitted tables (cache.AssumeWorkload), appended at X.A / X.AU, and the ClusterQueue usage
 __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
   int e = blockIdx.x * blockDim.x + threadIdx.x;
@@ -624,6 +705,11 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
         if (X.wl_pr) fin = drain_pr_attempt(X, a, wl, qr_ts);  // Admitted now: the PodsReady attempt starts
       }
     }
+    if (X.wl_rc_start) {  // the run starts now, or at PodsReady of a ready attempt; not while the checks run
+      const bool run = !(X.wl_check && X.wl_check[wl] > 0) && (!X.wl_pr || X.adm_phase[a] == KB_PH_RUN);
+      if (run) drain_rc_begin(X, a, wl, X.wl_pr ? X.wl_pr_at[wl] : qr_ts);
+      else X.adm_rc_next[a] = INT64_MAX;
+    }
     if (X.wl_max_exec) {  // Admitted now unless the checks run: the deadline may come first
       const bool checking = X.wl_check && X.wl_check[wl] > 0;
       if (!X.wl_qts) X.adm_phase[a] = KB_PH_RUN;
@@ -639,6 +725,11 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
   for (int row = ps0; row < ps1; row++)
     for (int r = 0; r < R; r++) {
       int f = D.ps_flavor[(size_t)row * R + r];
+      if (X.wl_rc_start) {  // the admission's PodSetAssignment, read by the reclaim steps
+        if (r == 0) X.ps_adm_cnt[row] = D.ps_count_out[row];
+        X.ps_adm_fl[(size_t)row * R + r] = (int8_t)f;
+        X.ps_adm_use[(size_t)row * R + r] = f < 0 ? 0 : drain_request(D, row, r, D.ps_count_out[row], covers_pods);
+      }
       if (f < 0) continue;
       int fr = f * R + r;
       i64 q = drain_request(D, row, r, D.ps_count_out[row], covers_pods);
@@ -768,7 +859,7 @@ __global__ void k_drain_live(DrainDev X, int bound, const int32_t *n_new) {
   X.row_live[a] = live;
   X.row_cells[a] = live ? X.adm_use_start[a + 1] - X.adm_use_start[a] : 0;
 }
-struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; i64 *finish; int32_t *lq; uint8_t *evicting, *phase; i64 *since; };
+struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; i64 *finish; int32_t *lq; uint8_t *evicting, *phase; i64 *since, *rc_next; int32_t *rc_cur; };
 // live rows of [0, bound), in order, into the other half of the double buffer; thread bound writes the totals
 __global__ void k_drain_compact(DrainDev X, AdmTabs O, int bound) {
   int a = blockIdx.x * blockDim.x + threadIdx.x;
@@ -783,6 +874,7 @@ __global__ void k_drain_compact(DrainDev X, AdmTabs O, int bound) {
   if (X.adm_evicting) O.evicting[n] = X.adm_evicting[a];
   if (X.adm_phase) O.phase[n] = X.adm_phase[a];
   if (X.adm_exec_since) O.since[n] = X.adm_exec_since[a];
+  if (X.adm_rc_next) { O.rc_next[n] = X.adm_rc_next[a]; O.rc_cur[n] = X.adm_rc_cur[a]; }
   for (int c = 0; c < nc; c++) { O.use_fr[c0 + c] = X.adm_use_fr[u0 + c]; O.use_qty[c0 + c] = X.adm_use_qty[u0 + c]; }
 }
 
@@ -821,7 +913,10 @@ __global__ void k_drain_ev_min(DrainDev X, int bound, const int32_t *n_new) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x;
   const int n_rows = X.A + (n_new ? *n_new : 0);
   i64 v = INT64_MAX;
-  if (a < bound && a < n_rows && X.adm_dead[a] != X.cycle + 1) v = X.adm_finish[a];
+  if (a < bound && a < n_rows && X.adm_dead[a] != X.cycle + 1) {
+    v = X.adm_finish[a];
+    if (X.adm_rc_next && drain_rc_live(X, a)) v = min(v, X.adm_rc_next[a]);  // the row's next reclaim step
+  }
   if (a == 0 && X.counters[KB_DC_ARR_HI] < X.n_arr) v = min(v, ev_time(X.arr_key[X.counters[KB_DC_ARR_HI]]));
   if (a == 0 && X.qc_ns && X.counters[KB_DC_QC_HI] < X.n_qc) v = min(v, X.qc_ns[X.counters[KB_DC_QC_HI]]);  // the next edit
   if (a == 0 && X.ac_ns && X.counters[KB_DC_AC_HI] < X.n_ac) v = min(v, X.ac_ns[X.counters[KB_DC_AC_HI]]);
@@ -892,6 +987,8 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
   if (X.counters[KB_DC_END] || X.adm_dead[a] == stamp) return;
   const i64 sd = X.wl_stop ? X.wl_stop[X.adm_wl[a]] : INT64_MAX;  // a stop edit of the record at this boundary
   bool stop = drain_stop_due(X, a, sd, X.adm_finish[a]);
+  // reclaim steps of a running row: strictly before its finish column, and at or before a stop (an own event first)
+  if (X.wl_rc_start && drain_rc_live(X, a)) drain_reclaim(D, X, a, stop ? sd : min(X.clock[0], X.adm_finish[a] - 1));
   if (!stop && X.adm_finish[a] > X.clock[0]) return;
   const int cq = X.adm_cq[a];
   int ph = X.adm_phase ? X.adm_phase[a] : KB_PH_RUN;
@@ -903,10 +1000,13 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
       const i64 run = X.wl_run ? X.wl_run[w] : -1;
       i64 fin = X.wl_pr ? drain_pr_attempt(X, a, w, tv) : run < 0 ? INT64_MAX : (tv > INT64_MAX - run ? INT64_MAX : tv + run);
       X.wl_ready_ns[w] = tv;
+      const bool rc_run = X.wl_rc_start && (!X.wl_pr || X.adm_phase[a] == KB_PH_RUN);  // the run starts (a ready attempt)
+      if (rc_run) drain_rc_begin(X, a, w, X.wl_pr ? X.wl_pr_at[w] : tv);
       if (X.wl_max_exec) { X.adm_exec_since[a] = tv; fin = drain_exec_clip(X, a, w, tv, fin); }
       X.adm_finish[a] = fin;
       atomicAdd(&X.counters[KB_DC_CHECK_READY], 1);
       stop = drain_stop_due(X, a, sd, fin);
+      if (rc_run) drain_reclaim(D, X, a, stop ? sd : min(X.clock[0], fin - 1));
       if (!stop && fin > X.clock[0]) return;
       ph = X.adm_phase[a];
     } else {  // Retry or Rejected: the workload holds no pods, its quota goes at once

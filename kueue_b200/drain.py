@@ -318,6 +318,33 @@ DeactivationTarget.
   9. with no edit and every wl_inactive 0 the drain equals the drain without the block.
 Edits applied between the start of cycle c and of c+1 are cycle c's (`active_changes`, and `stopped` / `resumed` for
 those that changed the state); wl_deactivated / wl_deactivation_reason describe the state at the end.
+
+Reclaim steps (event mode, the snapshot carries `wl_rc_start`, `rc_after_ns`, `rc_ps`, `rc_remaining` and `adm_wl`,
+include/kueue_b200.h).  ReclaimablePods: the Job, JobSet, TrainJob and Pod integrations write Status.ReclaimablePods as
+pods succeed (job_controller.go:213-227) and the cache counts only the pods still needed.  Step i of record w lowers
+podset rc_ps[i] to rc_remaining[i] pods rc_after_ns[i] after the run starts:
+  1. the run start S (`rc_begin`): the reservation t_c without a check delay, else the Ready verdict; with
+     WaitForPodsReady the PodsReady time of a ready attempt (a failing attempt has no run).  A snapshot row starts at
+     adm_run_start_ns, or at the PodsReady time of a ready attempt under way.  A readmission replays from the first step;
+  2. step i is an event at S + rc_after_ns[i] (saturating; `next_event` includes it while the row can take it).  It
+     applies while the row runs (`rc_live`): not checking, not evicting, phase RUN or EXPIRE, strictly before the
+     finish column (its finish or its effective MaximumExecutionTimeSeconds deadline); a step at the finish is dropped,
+     a row whose preemption is issued takes none.  A stop of the record at d takes the steps at or before d first
+     (`apply_row_stops`: the step is an own event).  A step whose rc_remaining is not below the podset's count changes
+     nothing and is not counted;
+  3. `apply_reclaims` runs in step 5 after the quota edits, the verdicts and the stops they allow, the AFS samples, and
+     before the timeouts, expiries and completions: none of those changes a running row before its finish column, so
+     the steps it applies are those the order of the issue names.  A record's steps at one instant are one update;
+  4. a step that lowers podset p from c to r (`reclaim_row`; totalRequestsFromAdmission workload.go:600-645): the
+     record's ps_count[p] = r and ps_req[p] = ps_req[p] // c * r (totalRequestsFromPodSets :567-598); the row's usage of
+     p becomes U0 // n * min(r, n) per resource on its flavor, U0 and n the admission's ResourceUsage and Count (`adm_use`,
+     `adm_cnt`, `adm_fl`: the drain's admission, or ps_adm_*); the difference leaves the row's cells, the ClusterQueue
+     usage and, under decay, the LocalQueue's admitted usage.  Once per update (workload_controller.go:1005-1014): the
+     ClusterQueue's generation + 1 (deleteWorkload clusterqueue.go:477-491), its root tree marked for step 7, the
+     record's scheduling hash = rc_sched_hash of the step (0 without the table);
+  5. finishes and releases leave the generation alone; the block composes with every block above.
+With no step that lowers a count the drain equals the drain without the block but for `ps_remaining`.  Steps applied
+between the start of cycle c and of c+1 are cycle c's (`reclaims`, indices of the steps).
 """
 from __future__ import annotations
 
@@ -404,6 +431,10 @@ class DrainResult:
     n_active_changes: int = 0                                  # edits applied, those before cycle 0 and no-op edits included
     n_stopped: int = 0
     n_resumed: int = 0
+    # reclaim steps (wl_rc_start in the snapshot; None / empty / 0 otherwise); cq_generation is written with it
+    reclaims: List[np.ndarray] = field(default_factory=list)  # per cycle: indices of the steps that lowered a count
+    n_reclaims: int = 0                                        # those before cycle 0 included
+    ps_remaining: np.ndarray | None = None                     # [n_podset] the counts after reclaim at the end
 
     @property
     def n_evicted(self) -> int:
@@ -584,6 +615,82 @@ def check_active_changes(snap) -> None:
             raise ValueError("active changes: an inactive start record that adm_wl names")
         if "wl_create_ns" in a and ((ina != 0) & (a["wl_create_ns"].astype(np.int64) > snap.now_ns)).any():
             raise ValueError("active changes: an inactive start record created after now_ns")
+
+
+class ReclaimUnsupported(ValueError):
+    """Steps on a record that can be partially admitted (kb_run_drain: KB_ERR_UNSUPPORTED)."""
+
+
+def check_reclaims(snap) -> None:
+    """the refusals of the reclaim-step tables (kb_run_drain: KB_ERR_INVALID): ValueError; ReclaimUnsupported"""
+    a = snap.arrays
+    if not any(k in a for k in abi.RECLAIM_FIELDS):
+        return
+    if "adm_wl" not in a:
+        raise ValueError("reclaim steps: the tables need adm_wl")
+    if not all(k in a for k in ("wl_rc_start", "rc_after_ns", "rc_ps", "rc_remaining")):
+        raise ValueError("reclaim steps: a NULL table (wl_rc_start, rc_after_ns, rc_ps, rc_remaining)")
+    W, R, F = snap.n_wl, snap.n_resource, snap.n_flavor
+    st = a["wl_rc_start"].astype(np.int64)
+    n = len(a["rc_after_ns"])
+    if (len(st) != W + 1 or st[0] != 0 or (np.diff(st) < 0).any() or st[-1] != n or len(a["rc_ps"]) != n
+            or len(a["rc_remaining"]) != n or ("rc_sched_hash" in a and len(a["rc_sched_hash"]) != n)):
+        raise ValueError("reclaim steps: wl_rc_start is not a CSR of the steps")
+    ps_start = a["wl_ps_start"].astype(np.int64)
+    after, ps, rem = (a[k].astype(np.int64) for k in ("rc_after_ns", "rc_ps", "rc_remaining"))
+    rec = np.repeat(np.arange(W), np.diff(st))
+    if ((ps < ps_start[rec]) | (ps >= ps_start[rec + 1])).any():
+        raise ValueError("reclaim steps: rc_ps outside its record")
+    if (after <= 0).any() or ((np.diff(after) < 0) & (rec[1:] == rec[:-1])).any():
+        raise ValueError("reclaim steps: rc_after_ns <= 0 or decreasing within a record")
+    last = {}
+    for i in range(n):
+        if rem[i] < 0 or rem[i] > last.get(int(ps[i]), rem[i]):
+            raise ValueError("reclaim steps: rc_remaining negative or increasing within a podset")
+        last[int(ps[i])] = int(rem[i])
+    cnt, req = a["ps_count"].astype(np.int64), a["ps_req"].reshape(-1, R).astype(np.int64)
+    for p in last:
+        if cnt[p] > 0 and (req[p] % cnt[p] != 0).any():
+            raise ValueError("reclaim steps: ps_req of a podset with steps not divisible by its ps_count")
+    has = np.diff(st) > 0
+    if snap.flags & abi.F_PARTIAL_ADMISSION:
+        for w in np.flatnonzero(has):
+            if (a["ps_min_count"][ps_start[w]:ps_start[w + 1]] >= 0).any():
+                raise ReclaimUnsupported("reclaim steps: steps on a record that can be partially admitted")
+    adm_wl = a["adm_wl"].astype(np.int64)
+    if "adm_run_start_ns" in a:
+        rs = a["adm_run_start_ns"].astype(np.int64)
+        if ((rs != UNSET) & (rs > snap.now_ns)).any():
+            raise ValueError("reclaim steps: adm_run_start_ns after now_ns")
+        idle = a["adm_evicted"].astype(bool).copy()
+        for k in ("adm_check_end_ns", "adm_admitted_ns"):
+            if k in a:
+                idle |= a[k].astype(np.int64) != UNSET
+        if ((rs != UNSET) & idle).any():
+            raise ValueError("reclaim steps: adm_run_start_ns on a row that is not running")
+    rows = [row for row in range(snap.n_adm) if has[adm_wl[row]]]
+    if not rows:
+        return
+    if not all(k in a for k in ("ps_adm_flavor", "ps_adm_count", "ps_adm_usage")):
+        raise ValueError("reclaim steps: ps_adm_* missing for a row whose record has steps")
+    fl, acnt, use = a["ps_adm_flavor"].reshape(-1, R).astype(np.int64), a["ps_adm_count"].astype(np.int64), a["ps_adm_usage"].reshape(-1, R).astype(np.int64)
+    us = a["adm_use_start"]
+    for row in rows:
+        w = adm_wl[row]
+        p0, p1 = ps_start[w], ps_start[w + 1]
+        if (fl[p0:p1] < -1).any() or (fl[p0:p1] >= F).any() or (acnt[p0:p1] < 0).any() or (use[p0:p1] < 0).any():
+            raise ValueError("reclaim steps: ps_adm_* out of range")
+        want = {}
+        for p in range(p0, p1):
+            for r in range(R):
+                if fl[p, r] >= 0 and acnt[p] > 0:
+                    fr = int(fl[p, r]) * R + r
+                    want[fr] = want.get(fr, 0) + int(use[p, r]) // int(acnt[p]) * min(int(cnt[p]), int(acnt[p]))
+        have = {}
+        for k in range(int(us[row]), int(us[row + 1])):
+            have[int(a["adm_use_fr"][k])] = have.get(int(a["adm_use_fr"][k]), 0) + int(a["adm_use_qty"][k])
+        if {f: q for f, q in want.items() if q} != {f: q for f, q in have.items() if q}:
+            raise ValueError("reclaim steps: a row's ps_adm_* do not add up to its adm_use cells")
 
 
 def static_generation_after(base: int, changes: int, n_edits: int) -> int:
@@ -830,7 +937,7 @@ _ADM_KEYS = _ADM_ROW_KEYS + ("adm_use_start", "adm_use_fr", "adm_use_qty")
 # times beside pods_ready_timeout
 _EVENT_LISTS = ("finished", "arrived", "evict_done", "check_retry", "check_rejected", "pods_ready_timeout",
                 "pods_ready_timeout_at", "pods_ready_deactivated", "max_exec_deactivated", "quota_changes", "active_changes",
-                "stopped", "resumed")
+                "stopped", "resumed", "reclaims")
 
 
 class _Rows:
@@ -843,15 +950,18 @@ class _Rows:
       checking  the admission checks run                                               adm_checking
       phase     RUN / WAIT / TIMED_OUT / EXPIRE (WaitForPodsReady, max exec)           adm_pods_ready_phase
       lq        the LocalQueue (decay of consumed usage)                               -
+      rc_next   the time of the row's next reclaim step, NEVER = none                  -
+      rc_cur    the index of that step                                                 -
     Rows join and leave only through `append` and `remove`, which move their cells in and out of the ClusterQueue usage
     (cache.AddWorkload / DeleteWorkload) and keep every column aligned."""
     COLUMNS = {"wl": "adm_wl", "finish": "adm_finish_ns", "evicting": "adm_evicting", "since": "adm_exec_since_ns",
-               "checking": "adm_checking", "phase": "adm_pods_ready_phase", "lq": None}
+               "checking": "adm_checking", "phase": "adm_pods_ready_phase", "lq": None, "rc_next": None, "rc_cur": None}
 
     def __init__(self, a, usage):
         self.adm = {k: a[k].copy() for k in _ADM_KEYS}
         self.usage = usage
         self.wl = self.finish = self.evicting = self.since = self.checking = self.phase = self.lq = None
+        self.rc_next = self.rc_cur = None
 
     def _columns(self):
         return [c for c in self.COLUMNS if getattr(self, c) is not None]
@@ -943,7 +1053,9 @@ class _Drain:
         check_active_changes(snap)
         act = self.act = "ac_ns" in a and len(a["ac_ns"]) > 0         # deactivation / reactivation edits
         self.blk = act or "wl_inactive" in a                           # the block (its start state alone needs no events)
-        events = self.events = any(k in a for k in abi.EVENT_FIELDS) or quota or act
+        check_reclaims(snap)
+        rc = self.rc = "wl_rc_start" in a                              # reclaim steps
+        events = self.events = any(k in a for k in abi.EVENT_FIELDS) or quota or act or rc
         self.step = max(1, int(snap.drain_cycle_ns)) if events else 1
         create = self.create = a.get("wl_create_ns")
         self.run_ns = a.get("wl_run_ns")
@@ -1016,6 +1128,33 @@ class _Drain:
                 rows.finish[row], e = self.exec_clip(int(rows.wl[row]), int(rows.since[row]), int(rows.finish[row]), int(snap.now_ns))
                 if e:
                     rows.phase[row] = EXPIRE
+        self.ps_start = a["wl_ps_start"].astype(np.int64)
+        self.ps_req = a["ps_req"].reshape(-1, R)
+        self.ps_cnt = a["ps_count"]                                    # the counts after reclaim (reclaim steps: mutable)
+        self.shash = a.get("wl_sched_hash")
+        if rc:  # rule 1 of reclaim steps: the steps, the admissions' assignments, the running rows of the snapshot
+            self.ps_req, self.ps_cnt = self.ps_req.astype(np.int64).copy(), self.ps_cnt.astype(np.int64).copy()
+            self.shash = self.shash.astype(np.int64).copy() if self.shash is not None else None
+            self.rc_start, self.rc_after, self.rc_ps, self.rc_rem = (a[k].astype(np.int64) for k in (
+                "wl_rc_start", "rc_after_ns", "rc_ps", "rc_remaining"))
+            self.rc_hash = a["rc_sched_hash"].astype(np.int64) if "rc_sched_hash" in a else None
+            P = len(self.ps_cnt)
+            self.adm_fl, self.adm_cnt, self.adm_use = np.full((P, R), -1, np.int64), np.zeros(P, np.int64), np.zeros((P, R), np.int64)
+            rows.rc_next, rows.rc_cur = np.full(snap.n_adm, NEVER, np.int64), np.zeros(snap.n_adm, np.int64)
+            rs = a["adm_run_start_ns"].astype(np.int64) if "adm_run_start_ns" in a else np.full(snap.n_adm, UNSET, np.int64)
+            for row in range(snap.n_adm):
+                w = int(rows.wl[row])
+                if self.rc_start[w] == self.rc_start[w + 1]:
+                    continue
+                p = slice(int(self.ps_start[w]), int(self.ps_start[w + 1]))
+                self.adm_fl[p] = a["ps_adm_flavor"].reshape(-1, R)[p]
+                self.adm_cnt[p] = a["ps_adm_count"][p]
+                self.adm_use[p] = a["ps_adm_usage"].reshape(-1, R)[p]
+                S = int(rs[row])
+                if S == UNSET and pr and "adm_admitted_ns" in a and a["adm_admitted_ns"][row] != UNSET:
+                    S = int(self.pr_at[w])  # a ready attempt under way: its PodsReady time (UNSET for a failing one)
+                if S != UNSET:
+                    self.rc_begin(row, w, S)
         self.sticky = a["cq_sticky"].astype(np.int64).copy() if "cq_sticky" in a else None  # sticky workload per ClusterQueue
         self.cursor = np.zeros(len(qlen), np.int64)
         self.first_aside = qlen.copy()                                 # smallest SET_ASIDE position per segment (qlen = none)
@@ -1042,11 +1181,8 @@ class _Drain:
             self.lqu = {int(l): self.usage_of(l) for l in self.seg_lq if l >= 0}
         self.first_seg = seg_start[:-1]
         self.strict = a["cq_strategy"].astype(bool)  # KB_QUEUE_STRICT_FIFO = 1
-        self.ps_start = a["wl_ps_start"].astype(np.int64)
-        self.ps_req = a["ps_req"].reshape(-1, R)
         self.last_gen = a["wl_last_gen"].astype(np.int64).copy()       # LastAssignment.ClusterQueueGeneration, -1 = nil
         self.last_tried = a["ps_last_tried"].reshape(-1, R).copy()     # LastAssignment.LastTriedFlavorIdx
-        self.shash = a.get("wl_sched_hash")
         self.has_qr = a["wl_has_quota_reservation"].copy() if "wl_has_quota_reservation" in a else None
         self.admit_cycle = np.full(W, -1, np.int64)
         self.evictions = np.zeros(W, np.int64)
@@ -1055,9 +1191,11 @@ class _Drain:
         self.root = root_of(a["parent"])
         self.static = {k: v for k, v in a.items() if not (k.startswith(("wl_", "ps_", "adm_")) or k in ("heads", "cq_usage") +
                                                           abi.AFS_FIELDS + abi.AFS_DECAY_FIELDS + abi.STICKY_FIELDS +
-                                                          abi.QUOTA_CHANGE_FIELDS + abi.ACTIVE_FIELDS)}
+                                                          abi.QUOTA_CHANGE_FIELDS + abi.ACTIVE_FIELDS + abi.RECLAIM_FIELDS)}
         self.gen = a["cq_generation"].astype(np.int64).copy()          # AllocatableResourceGeneration (rule 4 of quota changes)
         self.static_gen, self.qc_next, self.qc_rowed = int(snap.static_generation), 0, 0
+        # edits that can change the static tables: quota changes, and reclaim updates (the generations)
+        self.n_gen_edits = (len(a["qc_ns"]) if quota else 0) + (len(a["rc_after_ns"]) if rc else 0)
         if quota:
             self.qc_ns, self.qc_node = a["qc_ns"].astype(np.int64), a["qc_node"].astype(np.int64)
             self.qc_rows = [a[k].reshape(-1, FR) for k in ("qc_nominal", "qc_borrow_limit", "qc_lend_limit")]
@@ -1250,6 +1388,11 @@ class _Drain:
             rows.finish[row], rows.phase[row] = self.pr_attempt(w, t)
         else:
             rows.finish[row] = finish_time(t, int(self.run_ns[w])) if self.run_ns is not None else NEVER
+        if self.rc:  # rule 1 of reclaim steps: the run starts at Admitted, or at PodsReady of a ready attempt
+            if not self.pr or rows.phase[row] == RUN:
+                self.rc_begin(row, w, int(self.pr_at[w]) if self.pr else t)
+            else:
+                rows.rc_next[row] = NEVER
         if self.mx:
             rows.since[row] = t
             rows.finish[row], e = self.exec_clip(w, t, int(rows.finish[row]))
@@ -1281,6 +1424,80 @@ class _Drain:
         self.res.exec_spans.append((int(w), A, int(t_rel), d))
         return deact
 
+    # ---- reclaim steps
+    def rc_begin(self, row, w, S):
+        """rule 1: the run of row (record w) starts at S; its steps replay from the first"""
+        i = int(self.rc_start[w])
+        self.rows.rc_cur[row] = i
+        self.rows.rc_next[row] = min(S + int(self.rc_after[i]), NEVER) if i < self.rc_start[w + 1] else NEVER
+
+    def rc_live(self):
+        """rule 2: the rows that can take a step (their run started, not checking, not evicting, RUN or EXPIRE)"""
+        rows = self.rows
+        live = rows.rc_next < NEVER
+        if rows.checking is not None:
+            live &= ~rows.checking
+        if rows.evicting is not None:
+            live &= ~rows.evicting
+        if rows.phase is not None:
+            live &= (rows.phase == RUN) | (rows.phase == EXPIRE)
+        return live
+
+    def reclaim_row(self, row, lim, notified):
+        """rules 2 and 4: the steps of a running row due at or before lim, in time order; a record's steps at one instant
+        are one update"""
+        rows, R, a = self.rows, self.R, self.a
+        t, i, w = int(rows.rc_next[row]), int(rows.rc_cur[row]), int(rows.wl[row])
+        if t > lim:
+            return
+        i1, S = int(self.rc_start[w + 1]), t - int(self.rc_after[i])
+        cq = int(rows.adm["adm_cq"][row])
+        us = rows.adm["adm_use_start"]
+        while i < i1 and t <= lim:
+            lowered = False
+            while i < i1 and min(S + int(self.rc_after[i]), NEVER) == t:
+                p, rem = int(self.rc_ps[i]), int(self.rc_rem[i])
+                c = int(self.ps_cnt[p])
+                if rem < c:
+                    self.ps_req[p] = self.ps_req[p] // c * rem
+                    n = int(self.adm_cnt[p])
+                    for r in range(R):
+                        f = int(self.adm_fl[p, r])
+                        if f < 0 or n <= 0:
+                            continue
+                        u = int(self.adm_use[p, r]) // n
+                        d = u * min(rem, n) - u * min(c, n)
+                        if d == 0:
+                            continue
+                        fr = f * R + r
+                        for k in range(int(us[row]), int(us[row + 1])):
+                            if int(rows.adm["adm_use_fr"][k]) == fr:
+                                rows.adm["adm_use_qty"][k] += d
+                                break
+                        self.usage[cq, fr] += d
+                        if self.decay and rows.lq[row] >= 0 and self.afs_cq[cq]:
+                            self.ladm[rows.lq[row], r] += d
+                    self.ps_cnt[p] = rem
+                    if self.shash is not None:
+                        self.shash[w] = int(self.rc_hash[i]) if self.rc_hash is not None else 0
+                    lowered = True
+                    self.log("reclaims", [i])
+                i += 1
+            if lowered:  # AllocatableResourceGeneration + 1, the root tree requeued
+                self.gen[cq] += 1
+                self.static["cq_generation"] = self.gen.copy()
+                notified.add(cq)
+                self.qc_rowed += 1
+                self.static_gen = static_generation_after(int(self.snap.static_generation), self.qc_rowed, self.n_gen_edits)
+            t = min(S + int(self.rc_after[i]), NEVER) if i < i1 else NEVER
+        rows.rc_cur[row], rows.rc_next[row] = i, t
+
+    def apply_reclaims(self, t_next, notified):
+        """rule 3: the steps due by t_next of every running row, strictly before its finish column"""
+        rows = self.rows
+        for row in np.flatnonzero(self.rc_live() & (rows.rc_next <= t_next)):
+            self.reclaim_row(row, min(int(t_next), int(rows.finish[row]) - 1), notified)
+
     # ---- the boundary: steps 5-8
     def next_event(self):
         """earliest pending event after the evictions: a live row's finish or an ABSENT workload's creation (None = none)"""
@@ -1294,6 +1511,8 @@ class _Drain:
             e = min(e, int(self.create[self.arr_order[self.arr_next]]))
         if self.backoff and (self.state == BACKOFF).any():
             e = min(e, int(self.requeue_at[self.state == BACKOFF].min()))
+        if self.rc and len(fin):
+            e = min(e, int(np.where(self.rc_live(), self.rows.rc_next, NEVER).min()))
         return None if e >= NEVER else e
 
     def sample(self, t_to):
@@ -1335,7 +1554,7 @@ class _Drain:
             static["cq_generation"] = self.gen.copy()
             notified.add(n)  # its root tree is requeued (requeue_inadmissible maps a node to its root)
             self.qc_rowed += 1
-            self.static_gen = static_generation_after(int(self.snap.static_generation), self.qc_rowed, len(self.qc_ns))
+            self.static_gen = static_generation_after(int(self.snap.static_generation), self.qc_rowed, self.n_gen_edits)
 
     def apply_active_edit(self, j, w, held, notified):
         """rules 2, 4 and 5 of deactivation on record w; held: it holds a row at the edit's time (nothing changes)"""
@@ -1388,6 +1607,11 @@ class _Drain:
             return
         gone = [row for row in range(len(rows.wl)) if int(rows.wl[row]) in stop_at and deactivated[rows.wl[row]] == 0
                 and stop_at[int(rows.wl[row])] < rows.finish[row]]
+        if self.rc:  # a step at or before the stop goes first
+            live = self.rc_live()
+            for row in gone:
+                if live[row]:
+                    self.reclaim_row(row, stop_at[int(rows.wl[row])], notified)
         for row in gone:
             w = int(rows.wl[row]); d = stop_at[w]
             deactivated[w] = USER
@@ -1492,6 +1716,8 @@ class _Drain:
             self.apply_verdicts(t_next, notified)
             if self.act:
                 self.apply_row_stops(notified)
+        if self.rc:
+            self.apply_reclaims(t_next, notified)
         if self.pr:
             self.apply_timeouts(t_next)
             if self.act:
@@ -1601,7 +1827,8 @@ class _Drain:
         st, psr = _csr_take(ps_start, heads)
         cs.set("wl_ps_start", st)
         cs.set("ps_req", self.ps_req[psr]); cs.set("ps_last_tried", self.last_tried[psr])
-        for nm in ("ps_req_mask", "ps_count", "ps_min_count", "ps_flavor_ok"):
+        cs.set("ps_count", self.ps_cnt[psr])  # the counts after reclaim
+        for nm in ("ps_req_mask", "ps_min_count", "ps_flavor_ok"):
             cs.set(nm, a[nm][psr])
         if "ps_group" in a:  # optional tables (kb_snapshot: NULL when absent)
             cs.set("ps_group", a["ps_group"][psr])
@@ -1625,6 +1852,9 @@ class _Drain:
             cells = {}
             for row in range(int(st[e]), int(st[e + 1])):
                 full, cnt = int(cs.arrays["ps_count"][row]), int(out.ps_count[row])
+                if self.rc:  # the admission's PodSetAssignment (rule 4 of reclaim steps)
+                    g_row = int(ps_start[heads[e]]) + row - int(st[e])
+                    self.adm_fl[g_row], self.adm_cnt[g_row], self.adm_use[g_row] = -1, cnt, 0
                 for r in range(R):
                     f = int(out.ps_flavor[row, r])
                     if f < 0:
@@ -1636,6 +1866,8 @@ class _Drain:
                         if full != 0 and full != cnt:
                             q = q // full * cnt  # ScaledTo workload.go:258-275
                     cells[f * R + r] = cells.get(f * R + r, 0) + q
+                    if self.rc:
+                        self.adm_fl[g_row, r], self.adm_use[g_row, r] = f, q
             new_cells.append(cells)
             if self.afs_cq[cqi]:  # AfsEntryPenalties.Push of the entry penalty, then the LocalQueue's usage again
                 w, lq = int(heads[e]), int(a["wl_lq"][heads[e]])
@@ -1767,7 +1999,8 @@ class _Drain:
                     adm_qr_ts=np.full(n, t, np.int64), adm_uid=a["wl_uid"][g], adm_evicted=np.zeros(n, np.uint8), wl=g,
                     finish=np.asarray(fin, np.int64), evicting=np.zeros(n, bool), since=np.full(n, UNSET, np.int64),
                     checking=chk, phase=np.full(n, RUN, np.int64),
-                    lq=a["wl_lq"][g].astype(np.int64) if self.decay else None)
+                    lq=a["wl_lq"][g].astype(np.int64) if self.decay else None,
+                    rc_next=np.full(n, NEVER, np.int64), rc_cur=np.zeros(n, np.int64))
         if self.events:
             for i in np.flatnonzero(~chk):
                 self.admitted(first + int(i), int(g[i]), t)
@@ -1783,8 +2016,10 @@ class _Drain:
         res.wl_finish_ns = self.finish_ns
         res.end_ns = self.t
         res.cq_sticky = self.sticky
-        if self.quota:
+        if self.quota or self.rc:
             res.cq_generation = self.gen
+        if self.rc:
+            res.ps_remaining = self.ps_cnt
         if self.backoff:
             res.wl_queue_ts = self.qts
         if self.backoff or self.mx or self.blk:

@@ -466,6 +466,42 @@ def add_active_changes(snap: abi.FlatSnapshot, seed: int = 0, span_ns: int = 50_
     return snap
 
 
+def add_reclaims(snap: abi.FlatSnapshot, seed: int = 0, share: float = 0.3, steps: int = 3,
+                 span_ns: int = 50_000) -> abi.FlatSnapshot:
+    """Reclaim steps for an event drain (kb_snapshot.wl_rc_start, rc_*, include/kueue_b200.h), seeded: a share `share` of
+    the multi-pod records (a podset with Count >= 2 whose requests divide by it) that adm_wl does not name and that
+    cannot be partially admitted get 1..`steps` steps on one such podset, at times in (0, run) after the run starts
+    (wl_run_ns, or span_ns for a record without one), each leaving fewer pods than the one before.  An empty adm_wl is
+    added when the snapshot has no admitted rows and no adm_wl."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    a = snap.arrays
+    snap.finalize()
+    W, R = snap.n_wl, snap.n_resource
+    if "adm_wl" not in a and snap.n_adm == 0:
+        snap.set("adm_wl", np.zeros(0))
+    held = np.zeros(W, bool)
+    held[a["adm_wl"].astype(np.int64)] = True
+    ps_start, cnt = a["wl_ps_start"].astype(np.int64), a["ps_count"].astype(np.int64)
+    req = a["ps_req"].reshape(-1, R).astype(np.int64)
+    run = a["wl_run_ns"].astype(np.int64) if "wl_run_ns" in a else np.full(W, span_ns, np.int64)
+    partial = bool(snap.flags & abi.F_PARTIAL_ADMISSION)
+    start, after, ps, rem = [0], [], [], []
+    for w in range(W):
+        p0, p1 = int(ps_start[w]), int(ps_start[w + 1])
+        ok = [p for p in range(p0, p1) if cnt[p] >= 2 and not (req[p] % cnt[p]).any()]
+        if (ok and not held[w] and not (partial and (a["ps_min_count"][p0:p1] >= 0).any())
+                and rng.random() < share):
+            p = ok[int(rng.integers(0, len(ok)))]
+            k = int(rng.integers(1, steps + 1))
+            horizon = int(run[w]) if run[w] > 1 else span_ns
+            after += sorted(int(x) for x in rng.integers(1, max(2, horizon), size=k))
+            rem += sorted((int(x) for x in rng.integers(0, int(cnt[p]), size=k)), reverse=True)
+            ps += [p] * k
+        start.append(len(after))
+    snap.set("wl_rc_start", start); snap.set("rc_after_ns", after); snap.set("rc_ps", ps); snap.set("rc_remaining", rem)
+    return snap
+
+
 # The reference's scheduler performance scenario (test/performance/scheduler/configs/baseline/generator.yaml, generated
 # by runner/generator/generator.go): 5 cohorts of 6 ClusterQueues, one flavor, cpu only; per ClusterQueue, workload k of
 # a class is created at (k + 1) * interval and runs `run` once admitted (runner/controller/controller.go).
@@ -481,7 +517,7 @@ _MS = 1_000_000
 
 def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None = None, checks: int | None = None,
                   pods_ready: int | None = None, max_exec: int | None = None, quota: int | None = None,
-                  active: int | None = None) -> abi.FlatSnapshot:
+                  active: int | None = None, reclaim: int | None = None) -> abi.FlatSnapshot:
     """The baseline scenario as numbers (15,000 workloads at scale 1; `scale` multiplies the count of every class):
     nominal 20 cpu and borrowingLimit 100 cpu per ClusterQueue, preemption reclaimWithinCohort Any and
     withinClusterQueue LowerPriority, BestEffortFIFO.  cpu is in milli-units.  wl_ts is the creation time, an empty
@@ -497,7 +533,9 @@ def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None 
     quota: a seed: a capacity dip (add_quota_changes over the scenario's 60 s: each cohort's ClusterQueues drop to half
     their nominal quota at one time and get it back later, some lending limits, some no-op edits).
     active: a seed: stop / resume edits (add_active_changes over the scenario's 60 s: 5% of the workloads are stopped
-    once, half of those resumed later)."""
+    once, half of those resumed later).
+    reclaim: a seed: every workload runs one pod per cpu (the medium and large classes become 5- and 20-pod Jobs with the
+    same total requests), and add_reclaims gives a third of the multi-pod ones up to 3 steps within their run time."""
     Q = PERF_COHORTS * PERF_CQS_PER_COHORT
     snap = abi.FlatSnapshot(n_cq=Q, n_cohort=PERF_COHORTS, n_flavor=1, n_resource=1)
     snap.set("parent", np.concatenate([Q + np.arange(Q) // PERF_CQS_PER_COHORT, np.full(PERF_COHORTS, -1)]))
@@ -537,6 +575,9 @@ def perf_scenario(scale: float = 1.0, cycle_ns: int = _MS, evict_ns: int | None 
         add_quota_changes(snap, quota, span_ns=int(60_000 * scale) * _MS)
     if active is not None:
         add_active_changes(snap, active, span_ns=int(60_000 * scale) * _MS, stop_share=0.05)
+    if reclaim is not None:
+        snap.set("ps_count", np.asarray(cpu, np.int64) // 1000)
+        add_reclaims(snap, reclaim, share=1 / 3, steps=3)
     snap.finalize()
     snap.__dict__["perf_class"] = np.asarray(cls, np.int64)
     return snap
