@@ -1370,413 +1370,648 @@ struct DrainWords {
 };
 static_assert(sizeof(DrainWords) <= 64 * 4, "host_words[64..127] hold the words of a drain boundary");
 
-static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out) {
-  const int Q = s->n_cq, W = s->n_wl, R = s->n_resource, FR = s->n_flavor * s->n_resource;
-  const int Hcap = std::min(Q, W);
-  const int max_cycles = std::max(0, out->max_cycles);
-  out->n_cycles = 0; out->n_decisions = 0; out->n_admitted = 0; out->gpu_ms = 0; out->n_evicted = 0;
-  out->n_finished = 0; out->n_arrived = 0; out->end_ns = s->now_ns; out->n_evict_done = 0;
-  out->n_check_ready = 0; out->n_check_retry = 0; out->n_check_rejected = 0; out->n_resorts = 0; out->resort_ms = 0;
-  out->n_pods_ready_timeout = 0; out->n_pods_ready_deactivated = 0; out->n_max_exec_deactivated = 0; out->n_quota_changes = 0;
-  out->n_stopped = 0; out->n_resumed = 0; out->n_reclaims = 0;
-  // ---- eviction replay: host-side checks of adm_wl (include/kueue_b200.h)
-  const bool replay = s->adm_wl != nullptr;
-  if (replay) {
-    if (!(s->flags & KB_F_PRIORITY_SORTING_WITHIN_COHORT))
-      return fail(h, KB_ERR_UNSUPPORTED, "adm_wl: eviction replay needs KB_F_PRIORITY_SORTING_WITHIN_COHORT (a preempted workload's queue-order timestamp would be its eviction time)");
-    std::vector<uint8_t> named((size_t)std::max(1, W), 0);
+// The blocks a drain runs (include/kueue_b200.h), worked out once from the snapshot by drain_mode.  evict and compact
+// also depend on whether any ClusterQueue can preempt, which upload_impl works out: drain_plan sets them.
+struct DrainMode {
+  bool replay;   // adm_wl: the admitted rows name their pending records (eviction replay)
+  bool events;   // event mode: a clock replays arrivals, completions and the event blocks below
+  bool lat;      // eviction latency
+  bool decay;    // decay of AdmissionFairSharing consumed usage
+  bool sticky;   // sticky workload
+  bool checks;   // admission checks
+  bool pr;       // WaitForPodsReady
+  bool requeue;  // checks or pr: BACKOFF / DEACTIVATED, RequeueAt, queue-order timestamps, re-sorts
+  bool mx;       // MaximumExecutionTimeSeconds
+  bool quota;    // ClusterQueue / Cohort quota changes
+  bool act;      // deactivation / reactivation edits
+  bool blk;      // the edits, or their start state (wl_inactive) alone
+  bool deact;    // requeue, mx or blk: records carry a deactivation reason
+  bool rcl;      // reclaim steps
+  bool afs;      // AdmissionFairSharing queues (wl_lq)
+  bool evict;    // a preemption can evict a row
+  bool compact;  // rows can die: the admitted tables are compacted after every boundary
+  int n_qc, n_ac, n_rc;  // quota changes, active changes and reclaim steps the drain replays
+};
+static DrainMode drain_mode(const kb_snapshot *s) {
+  DrainMode m{};
+  m.replay = s->adm_wl != nullptr;
+  m.quota = s->n_quota_change > 0 && s->qc_ns;
+  m.act = s->n_active_change > 0 && s->ac_ns;
+  m.blk = m.act || s->wl_inactive;
+  m.rcl = s->wl_rc_start != nullptr;
+  m.events = s->wl_create_ns || s->wl_run_ns || s->adm_finish_ns || s->wl_evict_ns || s->wl_check_ns || s->wl_pods_ready_ns ||
+             s->wl_max_exec_s || m.quota || m.act || m.rcl;
+  m.lat = s->wl_evict_ns != nullptr;
+  m.decay = s->lq_last_update_ns != nullptr;
+  m.sticky = s->cq_sticky != nullptr;
+  m.checks = s->wl_check_ns != nullptr;
+  m.pr = s->wl_pods_ready_ns != nullptr;
+  m.requeue = m.checks || m.pr;
+  m.mx = s->wl_max_exec_s != nullptr;
+  m.deact = m.requeue || m.mx || m.blk;
+  m.afs = s->wl_lq != nullptr;
+  m.n_qc = m.quota ? s->n_quota_change : 0;
+  m.n_ac = m.act ? s->n_active_change : 0;
+  m.n_rc = m.rcl ? s->n_reclaim : 0;
+  return m;
+}
+
+// ---- input checks of kb_run_drain (include/kueue_b200.h), one per block, run in this order by drain_validate: a
+// snapshot that breaks two rules fails the first.  held[w]: an admitted row names record w (filled by check_replay).
+using HeldRecords = std::vector<uint8_t>;
+static int32_t check_replay(kb_handle *h, const kb_snapshot *s, const DrainMode &m, HeldRecords &held) {
+  if (!m.replay) return KB_OK;
+  if (!(s->flags & KB_F_PRIORITY_SORTING_WITHIN_COHORT))
+    return fail(h, KB_ERR_UNSUPPORTED, "adm_wl: eviction replay needs KB_F_PRIORITY_SORTING_WITHIN_COHORT (a preempted workload's queue-order timestamp would be its eviction time)");
+  for (int a = 0; a < s->n_adm; a++) {
+    const int w = s->adm_wl[a];
+    if (w < 0 || w >= s->n_wl) return fail(h, KB_ERR_INVALID, "adm_wl out of range");
+    if (held[w]) return fail(h, KB_ERR_INVALID, "adm_wl names a pending record twice");
+    held[w] = 1;
+    if (s->adm_cq[a] < 0 || s->adm_cq[a] >= s->n_cq || s->wl_cq[w] != s->adm_cq[a]) return fail(h, KB_ERR_INVALID, "adm_wl: the record's ClusterQueue is not the admitted workload's");
+  }
+  return KB_OK;
+}
+static int32_t check_events(kb_handle *h, const kb_snapshot *s, const DrainMode &m, HeldRecords &) {
+  if (!m.events) return KB_OK;
+  if (s->adm_finish_ns)
+    for (int a = 0; a < s->n_adm; a++)
+      if (s->adm_finish_ns[a] <= s->now_ns) return fail(h, KB_ERR_INVALID, "adm_finish_ns: a row admitted before the drain finishes at or before now_ns");
+  if (m.replay && s->wl_create_ns)
+    for (int a = 0; a < s->n_adm; a++)
+      if (s->wl_create_ns[s->adm_wl[a]] > s->now_ns) return fail(h, KB_ERR_INVALID, "adm_wl names a record created after now_ns");
+  return KB_OK;
+}
+static int32_t check_latency(kb_handle *h, const kb_snapshot *s, const DrainMode &m, HeldRecords &) {
+  if (!m.lat && !s->adm_evict_end_ns) return KB_OK;
+  if (!m.replay) return fail(h, KB_ERR_INVALID, "eviction latency: wl_evict_ns / adm_evict_end_ns need adm_wl");
+  if (!m.lat) return fail(h, KB_ERR_INVALID, "eviction latency: adm_evict_end_ns needs wl_evict_ns");
+  for (int w = 0; w < s->n_wl; w++)
+    if (s->wl_evict_ns[w] < 0) return fail(h, KB_ERR_INVALID, "eviction latency: wl_evict_ns < 0");
+  if (s->adm_evict_end_ns && s->adm_evicted)
+    for (int a = 0; a < s->n_adm; a++)
+      if (s->adm_evicted[a] && s->adm_evict_end_ns[a] <= s->now_ns)
+        return fail(h, KB_ERR_INVALID, "eviction latency: an eviction under way before the drain ends at or before now_ns");
+  return KB_OK;
+}
+static int32_t check_decay(kb_handle *h, const kb_snapshot *s, const DrainMode &m, HeldRecords &) {
+  if (!m.decay) return KB_OK;
+  if (!s->wl_lq || !s->lq_cq || !m.events) return fail(h, KB_ERR_INVALID, "afs decay: lq_last_update_ns needs wl_lq and event mode");
+  if (s->afs_half_life_ns < 0 || s->afs_sampling_ns <= 0) return fail(h, KB_ERR_INVALID, "afs decay: half-life < 0 or sampling interval <= 0");
+  if (!(s->afs_alpha >= 0.0 && s->afs_alpha < 1.0) || (s->afs_half_life_ns == 0 && s->afs_alpha != 0.0))
+    return fail(h, KB_ERR_INVALID, "afs decay: afs_alpha outside [0, 1), or non-zero with half-life 0");
+  for (int l = 0; l < s->n_lq; l++)
+    if (s->lq_last_update_ns[l] > s->now_ns) return fail(h, KB_ERR_INVALID, "afs decay: lq_last_update_ns after now_ns");
+  if (s->n_adm > 0 && !s->adm_lq) return fail(h, KB_ERR_INVALID, "afs decay: adm_lq is NULL while n_adm > 0");
+  for (int a = 0; a < s->n_adm; a++) {
+    const int l = s->adm_lq[a];
+    if (l < -1 || l >= s->n_lq) return fail(h, KB_ERR_INVALID, "afs decay: adm_lq out of range");
+    if (l >= 0 && s->lq_cq[l] != s->adm_cq[a]) return fail(h, KB_ERR_INVALID, "afs decay: the LocalQueue of an admitted row feeds another ClusterQueue");
+  }
+  return KB_OK;
+}
+static int32_t check_sticky(kb_handle *h, const kb_snapshot *s, const DrainMode &m, HeldRecords &held) {
+  if (!m.sticky) return KB_OK;
+  for (int q = 0; q < s->n_cq; q++) {
+    const int w = s->cq_sticky[q];
+    if (w < -1 || w >= s->n_wl) return fail(h, KB_ERR_INVALID, "cq_sticky out of range");
+    if (w < 0) continue;
+    if (s->wl_cq[w] != q) return fail(h, KB_ERR_INVALID, "cq_sticky: the workload is not in the ClusterQueue's queue");
+    if (held[w]) return fail(h, KB_ERR_INVALID, "cq_sticky names a record that holds quota (adm_wl): admission deleted it from its queue");
+    if (s->wl_create_ns && s->wl_create_ns[w] > s->now_ns) return fail(h, KB_ERR_INVALID, "cq_sticky names a record created after now_ns");
+    if (s->wl_lq && s->cq_afs && s->cq_afs[q])
+      return fail(h, KB_ERR_UNSUPPORTED, "cq_sticky: a sticky workload on a ClusterQueue with AdmissionFairSharing");
+  }
+  return KB_OK;
+}
+// wl_requeue_at_ns of record w (admission checks, PodsReady): a record in backoff holds no quota and exists at now_ns
+static int32_t check_requeue_at(kb_handle *h, const kb_snapshot *s, const HeldRecords &held, int w, const std::string &block) {
+  if (!s->wl_requeue_at_ns || s->wl_requeue_at_ns[w] == INT64_MIN) return KB_OK;
+  if (held[w]) return fail(h, KB_ERR_INVALID, block + ": wl_requeue_at_ns on a record that holds quota (adm_wl)");
+  if (s->wl_create_ns && s->wl_create_ns[w] > s->now_ns) return fail(h, KB_ERR_INVALID, block + ": wl_requeue_at_ns on a record created after now_ns");
+  return KB_OK;
+}
+static int32_t check_checks(kb_handle *h, const kb_snapshot *s, const DrainMode &m, HeldRecords &held) {
+  if (!m.checks && !s->wl_check_fail && !s->wl_check_retries && !s->wl_check_evict_ns && !(s->wl_requeue_at_ns && !m.pr) && !s->adm_check_end_ns)
+    return KB_OK;
+  if (!m.checks) return fail(h, KB_ERR_INVALID, "admission checks: the tables need wl_check_ns");
+  if (!m.replay) return fail(h, KB_ERR_INVALID, "admission checks: the tables need adm_wl");
+  if (m.decay) return fail(h, KB_ERR_UNSUPPORTED, "admission checks with afs decay: a workload with checks never makes the Pending -> Admitted transition that updates consumed usage");
+  if (s->check_backoff_base_s <= 0 || s->check_backoff_max_s < 0 || s->check_backoff_limit < 0)
+    return fail(h, KB_ERR_INVALID, "admission checks: backoff base <= 0, max < 0 or limit < 0");
+  i64 longest = 0;  // the longest WaitTime of attempts 1..limit (constant once capped: a base of >= 1 s gets there in < 64 doublings)
+  for (int k = 1; k <= std::min(s->check_backoff_limit, 64); k++)
+    longest = std::max(longest, kb_check_wait_ns(k, s->check_backoff_base_s, s->check_backoff_max_s));
+  if (longest >= 10000ll * 1000000000ll)
+    return fail(h, KB_ERR_UNSUPPORTED, "admission checks: a reachable backoff of 10,000 s or more is random in the reference (jitter)");
+  for (int w = 0; w < s->n_wl; w++) {
+    if (s->wl_check_ns[w] < 0 || (s->wl_check_fail && s->wl_check_fail[w] < 0) || (s->wl_check_retries && s->wl_check_retries[w] < 0))
+      return fail(h, KB_ERR_INVALID, "admission checks: a negative delay, fail count or retry count");
+    if (int32_t rc = check_requeue_at(h, s, held, w, "admission checks")) return rc;
+  }
+  if (s->adm_check_end_ns)
     for (int a = 0; a < s->n_adm; a++) {
-      const int w = s->adm_wl[a];
-      if (w < 0 || w >= W) return fail(h, KB_ERR_INVALID, "adm_wl out of range");
-      if (named[w]) return fail(h, KB_ERR_INVALID, "adm_wl names a pending record twice");
-      named[w] = 1;
-      if (s->adm_cq[a] < 0 || s->adm_cq[a] >= Q || s->wl_cq[w] != s->adm_cq[a]) return fail(h, KB_ERR_INVALID, "adm_wl: the record's ClusterQueue is not the admitted workload's");
+      if (s->adm_check_end_ns[a] == INT64_MIN) continue;
+      if (s->adm_check_end_ns[a] <= s->now_ns) return fail(h, KB_ERR_INVALID, "admission checks: adm_check_end_ns at or before now_ns");
+      if (m.lat && s->adm_evict_end_ns && s->adm_evicted && s->adm_evicted[a])  // one end time per row
+        return fail(h, KB_ERR_INVALID, "admission checks: a row with both an eviction under way (adm_evict_end_ns) and a check under way");
     }
+  return KB_OK;
+}
+static int32_t check_pods_ready(kb_handle *h, const kb_snapshot *s, const DrainMode &m, HeldRecords &held) {
+  if (!m.pr && !s->wl_pods_ready_fail && !s->wl_pods_ready_count && !s->wl_pods_ready_evict_ns && !s->adm_admitted_ns) return KB_OK;
+  if (!m.pr) return fail(h, KB_ERR_INVALID, "pods ready: the tables need wl_pods_ready_ns");
+  if (!m.replay) return fail(h, KB_ERR_INVALID, "pods ready: the tables need adm_wl");
+  if (s->pods_ready_timeout_ns <= 0) return fail(h, KB_ERR_INVALID, "pods ready: timeout <= 0");
+  if (s->pods_ready_backoff_base_s < 0 || s->pods_ready_backoff_max_s < 0 || s->pods_ready_backoff_limit < -1)
+    return fail(h, KB_ERR_INVALID, "pods ready: backoff base < 0, max < 0 or limit < -1");
+  if (s->pods_ready_requeue_creation != 0 && s->pods_ready_requeue_creation != 1)
+    return fail(h, KB_ERR_INVALID, "pods ready: pods_ready_requeue_creation is neither 0 (Eviction) nor 1 (Creation)");
+  for (int w = 0; w < s->n_wl; w++) {
+    if (s->wl_pods_ready_ns[w] < 0 || (s->wl_pods_ready_fail && s->wl_pods_ready_fail[w] < 0) ||
+        (s->wl_pods_ready_count && s->wl_pods_ready_count[w] < 0))
+      return fail(h, KB_ERR_INVALID, "pods ready: a negative delay, fail count or requeue count");
+    if (s->wl_pods_ready_evict_ns && s->wl_pods_ready_evict_ns[w] != INT64_MIN) {
+      if (held[w]) return fail(h, KB_ERR_INVALID, "pods ready: wl_pods_ready_evict_ns on a record that holds quota (adm_wl)");
+      if (s->wl_check_evict_ns && s->wl_check_evict_ns[w] != INT64_MIN)
+        return fail(h, KB_ERR_INVALID, "pods ready: a record with both wl_pods_ready_evict_ns and wl_check_evict_ns (one Evicted condition)");
+    }
+    if (!m.checks)  // the admission checks check it otherwise
+      if (int32_t rc = check_requeue_at(h, s, held, w, "pods ready")) return rc;
   }
-  // ---- event mode: host-side checks of the arrival and completion tables (include/kueue_b200.h)
-  const bool quota = s->n_quota_change > 0 && s->qc_ns;  // ClusterQueue / Cohort quota changes
-  const bool act = s->n_active_change > 0 && s->ac_ns;    // deactivation / reactivation edits
-  const bool blk = act || s->wl_inactive;                 // the block (its start state alone needs no events)
-  const bool rcl = s->wl_rc_start != nullptr;              // reclaim steps
-  const bool events = s->wl_create_ns || s->wl_run_ns || s->adm_finish_ns || s->wl_evict_ns || s->wl_check_ns || s->wl_pods_ready_ns ||
-                      s->wl_max_exec_s || quota || act || rcl;
-  if (events) {
-    if (s->adm_finish_ns)
-      for (int a = 0; a < s->n_adm; a++)
-        if (s->adm_finish_ns[a] <= s->now_ns) return fail(h, KB_ERR_INVALID, "adm_finish_ns: a row admitted before the drain finishes at or before now_ns");
-    if (replay && s->wl_create_ns)
-      for (int a = 0; a < s->n_adm; a++)
-        if (s->wl_create_ns[s->adm_wl[a]] > s->now_ns) return fail(h, KB_ERR_INVALID, "adm_wl names a record created after now_ns");
-  }
-  // ---- eviction latency: host-side checks (include/kueue_b200.h)
-  const bool lat = s->wl_evict_ns != nullptr;
-  if (lat || s->adm_evict_end_ns) {
-    if (!replay) return fail(h, KB_ERR_INVALID, "eviction latency: wl_evict_ns / adm_evict_end_ns need adm_wl");
-    if (!lat) return fail(h, KB_ERR_INVALID, "eviction latency: adm_evict_end_ns needs wl_evict_ns");
-    for (int w = 0; w < W; w++)
-      if (s->wl_evict_ns[w] < 0) return fail(h, KB_ERR_INVALID, "eviction latency: wl_evict_ns < 0");
-    if (s->adm_evict_end_ns && s->adm_evicted)
-      for (int a = 0; a < s->n_adm; a++)
-        if (s->adm_evicted[a] && s->adm_evict_end_ns[a] <= s->now_ns)
-          return fail(h, KB_ERR_INVALID, "eviction latency: an eviction under way before the drain ends at or before now_ns");
-  }
-  // ---- decay of AdmissionFairSharing consumed usage: host-side checks (include/kueue_b200.h)
-  const bool decay = s->lq_last_update_ns != nullptr;
-  if (decay) {
-    if (!s->wl_lq || !s->lq_cq || !events) return fail(h, KB_ERR_INVALID, "afs decay: lq_last_update_ns needs wl_lq and event mode");
-    if (s->afs_half_life_ns < 0 || s->afs_sampling_ns <= 0) return fail(h, KB_ERR_INVALID, "afs decay: half-life < 0 or sampling interval <= 0");
-    if (!(s->afs_alpha >= 0.0 && s->afs_alpha < 1.0) || (s->afs_half_life_ns == 0 && s->afs_alpha != 0.0))
-      return fail(h, KB_ERR_INVALID, "afs decay: afs_alpha outside [0, 1), or non-zero with half-life 0");
-    for (int l = 0; l < s->n_lq; l++)
-      if (s->lq_last_update_ns[l] > s->now_ns) return fail(h, KB_ERR_INVALID, "afs decay: lq_last_update_ns after now_ns");
-    if (s->n_adm > 0 && !s->adm_lq) return fail(h, KB_ERR_INVALID, "afs decay: adm_lq is NULL while n_adm > 0");
+  if (s->adm_admitted_ns)
     for (int a = 0; a < s->n_adm; a++) {
-      const int l = s->adm_lq[a];
-      if (l < -1 || l >= s->n_lq) return fail(h, KB_ERR_INVALID, "afs decay: adm_lq out of range");
-      if (l >= 0 && s->lq_cq[l] != s->adm_cq[a]) return fail(h, KB_ERR_INVALID, "afs decay: the LocalQueue of an admitted row feeds another ClusterQueue");
+      if (s->adm_admitted_ns[a] == INT64_MIN) continue;
+      if (s->adm_admitted_ns[a] > s->now_ns) return fail(h, KB_ERR_INVALID, "pods ready: adm_admitted_ns after now_ns");
+      if (s->adm_check_end_ns && s->adm_check_end_ns[a] != INT64_MIN)
+        return fail(h, KB_ERR_INVALID, "pods ready: adm_admitted_ns on a row whose checks run (adm_check_end_ns)");
+      if (m.lat && s->adm_evict_end_ns && s->adm_evicted && s->adm_evicted[a])
+        return fail(h, KB_ERR_INVALID, "pods ready: adm_admitted_ns on a row whose eviction is under way (adm_evict_end_ns)");
     }
+  return KB_OK;
+}
+static int32_t check_max_exec(kb_handle *h, const kb_snapshot *s, const DrainMode &m, HeldRecords &) {
+  if (!m.mx && !s->wl_exec_acc_s && !s->adm_exec_since_ns) return KB_OK;
+  if (!m.mx) return fail(h, KB_ERR_INVALID, "max exec: the tables need wl_max_exec_s");
+  if (!m.replay) return fail(h, KB_ERR_INVALID, "max exec: the tables need adm_wl");
+  for (int w = 0; w < s->n_wl; w++) {
+    if (s->wl_max_exec_s[w] < 0) return fail(h, KB_ERR_INVALID, "max exec: wl_max_exec_s < 0");
+    if (s->wl_exec_acc_s && s->wl_exec_acc_s[w] < -1) return fail(h, KB_ERR_INVALID, "max exec: wl_exec_acc_s < -1");
   }
-  // ---- sticky workload: host-side checks of cq_sticky (include/kueue_b200.h)
-  const bool sticky = s->cq_sticky != nullptr;
-  if (sticky) {
-    std::vector<uint8_t> held((size_t)std::max(1, W), 0);
-    if (replay) for (int a = 0; a < s->n_adm; a++) held[s->adm_wl[a]] = 1;
-    for (int q = 0; q < Q; q++) {
-      const int w = s->cq_sticky[q];
-      if (w < -1 || w >= W) return fail(h, KB_ERR_INVALID, "cq_sticky out of range");
-      if (w < 0) continue;
-      if (s->wl_cq[w] != q) return fail(h, KB_ERR_INVALID, "cq_sticky: the workload is not in the ClusterQueue's queue");
-      if (held[w]) return fail(h, KB_ERR_INVALID, "cq_sticky names a record that holds quota (adm_wl): admission deleted it from its queue");
-      if (s->wl_create_ns && s->wl_create_ns[w] > s->now_ns) return fail(h, KB_ERR_INVALID, "cq_sticky names a record created after now_ns");
-      if (s->wl_lq && s->cq_afs && s->cq_afs[q])
-        return fail(h, KB_ERR_UNSUPPORTED, "cq_sticky: a sticky workload on a ClusterQueue with AdmissionFairSharing");
-    }
-    if (out->cq_sticky) memcpy(out->cq_sticky, s->cq_sticky, (size_t)Q * 4);  // the slots of a drain that runs no cycle
+  if (s->n_adm > 0 && !s->adm_exec_since_ns) return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns is NULL while n_adm > 0");
+  for (int a = 0; a < s->n_adm; a++) {
+    const i64 A = s->adm_exec_since_ns[a];
+    const bool chk = m.checks && s->adm_check_end_ns && s->adm_check_end_ns[a] != INT64_MIN;
+    if (A == INT64_MIN && !chk) return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns missing on a row whose checks do not run");
+    if (A != INT64_MIN && chk) return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns set on a row whose checks run (adm_check_end_ns)");
+    if (A > s->now_ns) return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns after now_ns");
+    if (m.pr && s->adm_admitted_ns && s->adm_admitted_ns[a] != INT64_MIN && s->adm_admitted_ns[a] != A)
+      return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns differs from adm_admitted_ns");
   }
-  // ---- admission checks: host-side checks (include/kueue_b200.h)
-  const bool checks = s->wl_check_ns != nullptr;
-  const bool pr = s->wl_pods_ready_ns != nullptr;  // WaitForPodsReady
-  const bool requeue = checks || pr;               // BACKOFF / DEACTIVATED, RequeueAt, queue-order timestamps, re-sorts
-  if (checks || s->wl_check_fail || s->wl_check_retries || s->wl_check_evict_ns || (s->wl_requeue_at_ns && !pr) || s->adm_check_end_ns) {
-    if (!checks) return fail(h, KB_ERR_INVALID, "admission checks: the tables need wl_check_ns");
-    if (!replay) return fail(h, KB_ERR_INVALID, "admission checks: the tables need adm_wl");
-    if (decay) return fail(h, KB_ERR_UNSUPPORTED, "admission checks with afs decay: a workload with checks never makes the Pending -> Admitted transition that updates consumed usage");
-    if (s->check_backoff_base_s <= 0 || s->check_backoff_max_s < 0 || s->check_backoff_limit < 0)
-      return fail(h, KB_ERR_INVALID, "admission checks: backoff base <= 0, max < 0 or limit < 0");
-    {  // the longest WaitTime of attempts 1..limit (constant once capped: a base of >= 1 s gets there in < 64 doublings)
-      i64 longest = 0;
-      for (int k = 1; k <= std::min(s->check_backoff_limit, 64); k++)
-        longest = std::max(longest, kb_check_wait_ns(k, s->check_backoff_base_s, s->check_backoff_max_s));
-      if (longest >= 10000ll * 1000000000ll)
-        return fail(h, KB_ERR_UNSUPPORTED, "admission checks: a reachable backoff of 10,000 s or more is random in the reference (jitter)");
-    }
-    std::vector<uint8_t> held((size_t)std::max(1, W), 0);
-    for (int a = 0; a < s->n_adm; a++) held[s->adm_wl[a]] = 1;
-    for (int w = 0; w < W; w++) {
-      if (s->wl_check_ns[w] < 0 || (s->wl_check_fail && s->wl_check_fail[w] < 0) || (s->wl_check_retries && s->wl_check_retries[w] < 0))
-        return fail(h, KB_ERR_INVALID, "admission checks: a negative delay, fail count or retry count");
-      if (s->wl_requeue_at_ns && s->wl_requeue_at_ns[w] != INT64_MIN) {
-        if (held[w]) return fail(h, KB_ERR_INVALID, "admission checks: wl_requeue_at_ns on a record that holds quota (adm_wl)");
-        if (s->wl_create_ns && s->wl_create_ns[w] > s->now_ns) return fail(h, KB_ERR_INVALID, "admission checks: wl_requeue_at_ns on a record created after now_ns");
-      }
-    }
-    if (s->adm_check_end_ns)
-      for (int a = 0; a < s->n_adm; a++) {
-        if (s->adm_check_end_ns[a] == INT64_MIN) continue;
-        if (s->adm_check_end_ns[a] <= s->now_ns) return fail(h, KB_ERR_INVALID, "admission checks: adm_check_end_ns at or before now_ns");
-        if (lat && s->adm_evict_end_ns && s->adm_evicted && s->adm_evicted[a])  // one end time per row
-          return fail(h, KB_ERR_INVALID, "admission checks: a row with both an eviction under way (adm_evict_end_ns) and a check under way");
-      }
-  }
-  // ---- WaitForPodsReady: host-side checks (include/kueue_b200.h)
-  if (pr || s->wl_pods_ready_fail || s->wl_pods_ready_count || s->wl_pods_ready_evict_ns || s->adm_admitted_ns) {
-    if (!pr) return fail(h, KB_ERR_INVALID, "pods ready: the tables need wl_pods_ready_ns");
-    if (!replay) return fail(h, KB_ERR_INVALID, "pods ready: the tables need adm_wl");
-    if (s->pods_ready_timeout_ns <= 0) return fail(h, KB_ERR_INVALID, "pods ready: timeout <= 0");
-    if (s->pods_ready_backoff_base_s < 0 || s->pods_ready_backoff_max_s < 0 || s->pods_ready_backoff_limit < -1)
-      return fail(h, KB_ERR_INVALID, "pods ready: backoff base < 0, max < 0 or limit < -1");
-    if (s->pods_ready_requeue_creation != 0 && s->pods_ready_requeue_creation != 1)
-      return fail(h, KB_ERR_INVALID, "pods ready: pods_ready_requeue_creation is neither 0 (Eviction) nor 1 (Creation)");
-    std::vector<uint8_t> held((size_t)std::max(1, W), 0);
-    for (int a = 0; a < s->n_adm; a++) held[s->adm_wl[a]] = 1;
-    for (int w = 0; w < W; w++) {
-      if (s->wl_pods_ready_ns[w] < 0 || (s->wl_pods_ready_fail && s->wl_pods_ready_fail[w] < 0) ||
-          (s->wl_pods_ready_count && s->wl_pods_ready_count[w] < 0))
-        return fail(h, KB_ERR_INVALID, "pods ready: a negative delay, fail count or requeue count");
-      if (s->wl_pods_ready_evict_ns && s->wl_pods_ready_evict_ns[w] != INT64_MIN) {
-        if (held[w]) return fail(h, KB_ERR_INVALID, "pods ready: wl_pods_ready_evict_ns on a record that holds quota (adm_wl)");
-        if (s->wl_check_evict_ns && s->wl_check_evict_ns[w] != INT64_MIN)
-          return fail(h, KB_ERR_INVALID, "pods ready: a record with both wl_pods_ready_evict_ns and wl_check_evict_ns (one Evicted condition)");
-      }
-      if (!checks && s->wl_requeue_at_ns && s->wl_requeue_at_ns[w] != INT64_MIN) {  // as the admission checks require
-        if (held[w]) return fail(h, KB_ERR_INVALID, "pods ready: wl_requeue_at_ns on a record that holds quota (adm_wl)");
-        if (s->wl_create_ns && s->wl_create_ns[w] > s->now_ns) return fail(h, KB_ERR_INVALID, "pods ready: wl_requeue_at_ns on a record created after now_ns");
-      }
-    }
-    if (s->adm_admitted_ns)
-      for (int a = 0; a < s->n_adm; a++) {
-        if (s->adm_admitted_ns[a] == INT64_MIN) continue;
-        if (s->adm_admitted_ns[a] > s->now_ns) return fail(h, KB_ERR_INVALID, "pods ready: adm_admitted_ns after now_ns");
-        if (s->adm_check_end_ns && s->adm_check_end_ns[a] != INT64_MIN)
-          return fail(h, KB_ERR_INVALID, "pods ready: adm_admitted_ns on a row whose checks run (adm_check_end_ns)");
-        if (lat && s->adm_evict_end_ns && s->adm_evicted && s->adm_evicted[a])
-          return fail(h, KB_ERR_INVALID, "pods ready: adm_admitted_ns on a row whose eviction is under way (adm_evict_end_ns)");
-      }
-  }
-  // ---- MaximumExecutionTimeSeconds: host-side checks (include/kueue_b200.h)
-  const bool mx = s->wl_max_exec_s != nullptr;
-  if (mx || s->wl_exec_acc_s || s->adm_exec_since_ns) {
-    if (!mx) return fail(h, KB_ERR_INVALID, "max exec: the tables need wl_max_exec_s");
-    if (!replay) return fail(h, KB_ERR_INVALID, "max exec: the tables need adm_wl");
-    for (int w = 0; w < W; w++) {
-      if (s->wl_max_exec_s[w] < 0) return fail(h, KB_ERR_INVALID, "max exec: wl_max_exec_s < 0");
-      if (s->wl_exec_acc_s && s->wl_exec_acc_s[w] < -1) return fail(h, KB_ERR_INVALID, "max exec: wl_exec_acc_s < -1");
-    }
-    if (s->n_adm > 0 && !s->adm_exec_since_ns) return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns is NULL while n_adm > 0");
-    for (int a = 0; a < s->n_adm; a++) {
-      const i64 A = s->adm_exec_since_ns[a];
-      const bool chk = checks && s->adm_check_end_ns && s->adm_check_end_ns[a] != INT64_MIN;
-      if (A == INT64_MIN && !chk) return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns missing on a row whose checks do not run");
-      if (A != INT64_MIN && chk) return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns set on a row whose checks run (adm_check_end_ns)");
-      if (A > s->now_ns) return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns after now_ns");
-      if (pr && s->adm_admitted_ns && s->adm_admitted_ns[a] != INT64_MIN && s->adm_admitted_ns[a] != A)
-        return fail(h, KB_ERR_INVALID, "max exec: adm_exec_since_ns differs from adm_admitted_ns");
-    }
-  }
-  // ---- quota changes: host-side checks (include/kueue_b200.h), and what the device needs besides the tables: the edits
-  // that change nothing, the root slot and the cohort tree of every other one (the rows change only through the edits, in
-  // table order, so the rows an edit meets are known here), the ClusterQueues of every root, the place of every
-  // ClusterQueue's generation in the static tree blocks
-  const int QN = Q + s->n_cohort, NQC = quota ? s->n_quota_change : 0;
-  std::vector<int32_t> qc_root, qc_tree, qc_tree_next, qc_cq_start, qc_cq, qc_blob_gen;
+  return KB_OK;
+}
+static int32_t check_quota(kb_handle *h, const kb_snapshot *s, const DrainMode &m, HeldRecords &) {
   if (s->n_quota_change < 0) return fail(h, KB_ERR_INVALID, "quota changes: n_quota_change < 0");
-  if (s->n_quota_change > 0) {
-    if (!s->qc_ns || !s->qc_node || !s->qc_nominal || !s->qc_borrow_limit || !s->qc_lend_limit)
-      return fail(h, KB_ERR_INVALID, "quota changes: a NULL table with n_quota_change > 0");
-    std::vector<uint8_t> covered((size_t)Q * FR, 0);  // the cells a ClusterQueue's resource groups cover
-    for (int q = 0; q < Q; q++)
-      for (int g = s->cq_rg_start[q]; g < s->cq_rg_start[q + 1]; g++)
-        for (int k = s->rg_flavor_start[g]; k < s->rg_flavor_start[g + 1]; k++)
-          for (int r = 0; r < R; r++)
-            if (s->rg_res_mask[g] & (1u << r)) covered[(size_t)q * FR + (size_t)s->rg_flavors[k] * R + r] = 1;
-    for (int i = 0; i < NQC; i++) {
-      if (s->qc_ns[i] <= s->now_ns) return fail(h, KB_ERR_INVALID, "quota changes: qc_ns at or before now_ns");
-      if (i > 0 && s->qc_ns[i] < s->qc_ns[i - 1]) return fail(h, KB_ERR_INVALID, "quota changes: qc_ns decreasing");
-      const int n = s->qc_node[i];
-      if (n < 0 || n >= QN) return fail(h, KB_ERR_INVALID, "quota changes: qc_node out of range");
-      for (int c = 0; c < FR; c++) {
-        const size_t k = (size_t)i * FR + c;
-        if (s->qc_nominal[k] < 0 || s->qc_nominal[k] == KB_NO_LIMIT) return fail(h, KB_ERR_INVALID, "quota changes: a negative nominal or KB_NO_LIMIT in a nominal row");
-        if (s->qc_borrow_limit[k] < 0 || s->qc_lend_limit[k] < 0) return fail(h, KB_ERR_INVALID, "quota changes: a negative limit");
-        const size_t o = (size_t)n * FR + c;
-        if (n < Q && !covered[o] && (s->qc_nominal[k] != s->nominal[o] || s->qc_borrow_limit[k] != s->borrow_limit[o] || s->qc_lend_limit[k] != s->lend_limit[o]))
-          return fail(h, KB_ERR_INVALID, "quota changes: a ClusterQueue cell its resource groups do not cover");
-      }
+  if (s->n_quota_change == 0) return KB_OK;
+  if (!s->qc_ns || !s->qc_node || !s->qc_nominal || !s->qc_borrow_limit || !s->qc_lend_limit)
+    return fail(h, KB_ERR_INVALID, "quota changes: a NULL table with n_quota_change > 0");
+  const int Q = s->n_cq, R = s->n_resource, FR = s->n_flavor * R;
+  std::vector<uint8_t> covered((size_t)Q * FR, 0);  // the cells a ClusterQueue's resource groups cover
+  for (int q = 0; q < Q; q++)
+    for (int g = s->cq_rg_start[q]; g < s->cq_rg_start[q + 1]; g++)
+      for (int k = s->rg_flavor_start[g]; k < s->rg_flavor_start[g + 1]; k++)
+        for (int r = 0; r < R; r++)
+          if (s->rg_res_mask[g] & (1u << r)) covered[(size_t)q * FR + (size_t)s->rg_flavors[k] * R + r] = 1;
+  for (int i = 0; i < m.n_qc; i++) {
+    if (s->qc_ns[i] <= s->now_ns) return fail(h, KB_ERR_INVALID, "quota changes: qc_ns at or before now_ns");
+    if (i > 0 && s->qc_ns[i] < s->qc_ns[i - 1]) return fail(h, KB_ERR_INVALID, "quota changes: qc_ns decreasing");
+    const int n = s->qc_node[i];
+    if (n < 0 || n >= Q + s->n_cohort) return fail(h, KB_ERR_INVALID, "quota changes: qc_node out of range");
+    for (int c = 0; c < FR; c++) {
+      const size_t k = (size_t)i * FR + c;
+      if (s->qc_nominal[k] < 0 || s->qc_nominal[k] == KB_NO_LIMIT) return fail(h, KB_ERR_INVALID, "quota changes: a negative nominal or KB_NO_LIMIT in a nominal row");
+      if (s->qc_borrow_limit[k] < 0 || s->qc_lend_limit[k] < 0) return fail(h, KB_ERR_INVALID, "quota changes: a negative limit");
+      const size_t o = (size_t)n * FR + c;
+      if (n < Q && !covered[o] && (s->qc_nominal[k] != s->nominal[o] || s->qc_borrow_limit[k] != s->borrow_limit[o] || s->qc_lend_limit[k] != s->lend_limit[o]))
+        return fail(h, KB_ERR_INVALID, "quota changes: a ClusterQueue cell its resource groups do not cover");
     }
   }
-  // ---- deactivation / reactivation: host-side checks (include/kueue_b200.h), and each edit's neighbours of the same record
-  const int NAC = act ? s->n_active_change : 0;
-  std::vector<int32_t> ac_next, ac_prev;
+  return KB_OK;
+}
+static int32_t check_active(kb_handle *h, const kb_snapshot *s, const DrainMode &m, HeldRecords &held) {
   if (s->n_active_change < 0) return fail(h, KB_ERR_INVALID, "active changes: n_active_change < 0");
   if (s->n_active_change > 0 && (!s->ac_ns || !s->ac_wl || !s->ac_active))
     return fail(h, KB_ERR_INVALID, "active changes: a NULL table with n_active_change > 0");
-  if (blk) {
-    if (!replay) return fail(h, KB_ERR_INVALID, "active changes: the tables need adm_wl");
-    for (int i = 0; i < NAC; i++) {
-      if (s->ac_ns[i] <= s->now_ns) return fail(h, KB_ERR_INVALID, "active changes: ac_ns at or before now_ns");
-      if (i > 0 && s->ac_ns[i] < s->ac_ns[i - 1]) return fail(h, KB_ERR_INVALID, "active changes: ac_ns decreasing");
-      const int w = s->ac_wl[i];
-      if (w < 0 || w >= W) return fail(h, KB_ERR_INVALID, "active changes: ac_wl out of range");
-      if (s->ac_active[i] > 1) return fail(h, KB_ERR_INVALID, "active changes: ac_active neither 0 nor 1");
-      if (s->wl_create_ns && s->ac_ns[i] <= s->wl_create_ns[w]) return fail(h, KB_ERR_INVALID, "active changes: an edit at or before its record's wl_create_ns");
-    }
-    if (s->wl_inactive) {
-      std::vector<uint8_t> held((size_t)std::max(1, W), 0);
-      for (int a = 0; a < s->n_adm; a++) held[s->adm_wl[a]] = 1;
-      for (int w = 0; w < W; w++) {
-        if (s->wl_inactive[w] > KB_DR_USER) return fail(h, KB_ERR_INVALID, "active changes: wl_inactive above 4");
-        if (!s->wl_inactive[w]) continue;
-        if (held[w]) return fail(h, KB_ERR_INVALID, "active changes: an inactive start record that adm_wl names");
-        if (s->wl_create_ns && s->wl_create_ns[w] > s->now_ns) return fail(h, KB_ERR_INVALID, "active changes: an inactive start record created after now_ns");
-      }
-    }
-    ac_next.assign((size_t)std::max(1, NAC), NAC); ac_prev.assign((size_t)std::max(1, NAC), -1);
-    std::vector<int32_t> last((size_t)std::max(1, W), -1);
-    for (int i = 0; i < NAC; i++) {
-      const int w = s->ac_wl[i];
-      if (last[w] >= 0) { ac_prev[i] = last[w]; ac_next[last[w]] = i; }
-      last[w] = i;
-    }
+  if (!m.blk) return KB_OK;
+  if (!m.replay) return fail(h, KB_ERR_INVALID, "active changes: the tables need adm_wl");
+  for (int i = 0; i < m.n_ac; i++) {
+    if (s->ac_ns[i] <= s->now_ns) return fail(h, KB_ERR_INVALID, "active changes: ac_ns at or before now_ns");
+    if (i > 0 && s->ac_ns[i] < s->ac_ns[i - 1]) return fail(h, KB_ERR_INVALID, "active changes: ac_ns decreasing");
+    const int w = s->ac_wl[i];
+    if (w < 0 || w >= s->n_wl) return fail(h, KB_ERR_INVALID, "active changes: ac_wl out of range");
+    if (s->ac_active[i] > 1) return fail(h, KB_ERR_INVALID, "active changes: ac_active neither 0 nor 1");
+    if (s->wl_create_ns && s->ac_ns[i] <= s->wl_create_ns[w]) return fail(h, KB_ERR_INVALID, "active changes: an edit at or before its record's wl_create_ns");
   }
-  // ---- reclaim steps: host-side checks (include/kueue_b200.h), restated by kueue_b200/drain.py check_reclaims
-  const int NRC = rcl ? s->n_reclaim : 0;
-  if (rcl || s->rc_after_ns || s->rc_ps || s->rc_remaining || s->rc_sched_hash || s->ps_adm_flavor || s->ps_adm_count || s->ps_adm_usage ||
-      s->adm_run_start_ns) {
-    if (!replay) return fail(h, KB_ERR_INVALID, "reclaim steps: the tables need adm_wl");
-    if (!rcl || (s->n_reclaim > 0 && (!s->rc_after_ns || !s->rc_ps || !s->rc_remaining)))
-      return fail(h, KB_ERR_INVALID, "reclaim steps: a NULL table (wl_rc_start, rc_after_ns, rc_ps, rc_remaining)");
-    if (s->n_reclaim < 0 || s->wl_rc_start[0] != 0 || s->wl_rc_start[W] != s->n_reclaim)
-      return fail(h, KB_ERR_INVALID, "reclaim steps: wl_rc_start is not a CSR of the steps");
-    for (int w = 0; w < W; w++)
-      if (s->wl_rc_start[w + 1] < s->wl_rc_start[w]) return fail(h, KB_ERR_INVALID, "reclaim steps: wl_rc_start is not a CSR of the steps");
-    for (int w = 0; w < W; w++)
-      for (int i = s->wl_rc_start[w]; i < s->wl_rc_start[w + 1]; i++)
-        if (s->rc_ps[i] < s->wl_ps_start[w] || s->rc_ps[i] >= s->wl_ps_start[w + 1]) return fail(h, KB_ERR_INVALID, "reclaim steps: rc_ps outside its record");
-    for (int w = 0; w < W; w++)
-      for (int i = s->wl_rc_start[w]; i < s->wl_rc_start[w + 1]; i++)
-        if (s->rc_after_ns[i] <= 0 || (i > s->wl_rc_start[w] && s->rc_after_ns[i] < s->rc_after_ns[i - 1]))
-          return fail(h, KB_ERR_INVALID, "reclaim steps: rc_after_ns <= 0 or decreasing within a record");
-    std::vector<int32_t> last((size_t)std::max(1, s->n_podset), INT32_MAX);
-    for (int i = 0; i < NRC; i++) {
-      const int p = s->rc_ps[i];
-      if (s->rc_remaining[i] < 0 || s->rc_remaining[i] > last[p]) return fail(h, KB_ERR_INVALID, "reclaim steps: rc_remaining negative or increasing within a podset");
-      last[p] = s->rc_remaining[i];
+  if (s->wl_inactive)
+    for (int w = 0; w < s->n_wl; w++) {
+      if (s->wl_inactive[w] > KB_DR_USER) return fail(h, KB_ERR_INVALID, "active changes: wl_inactive above 4");
+      if (!s->wl_inactive[w]) continue;
+      if (held[w]) return fail(h, KB_ERR_INVALID, "active changes: an inactive start record that adm_wl names");
+      if (s->wl_create_ns && s->wl_create_ns[w] > s->now_ns) return fail(h, KB_ERR_INVALID, "active changes: an inactive start record created after now_ns");
     }
-    for (int p = 0; p < s->n_podset; p++)
-      if (last[p] != INT32_MAX && s->ps_count[p] > 0)
-        for (int r = 0; r < R; r++)
-          if (s->ps_req[(size_t)p * R + r] % s->ps_count[p] != 0) return fail(h, KB_ERR_INVALID, "reclaim steps: ps_req of a podset with steps not divisible by its ps_count");
-    if (s->flags & KB_F_PARTIAL_ADMISSION)
-      for (int w = 0; w < W; w++)
-        if (s->wl_rc_start[w + 1] > s->wl_rc_start[w])
-          for (int p = s->wl_ps_start[w]; p < s->wl_ps_start[w + 1]; p++)
-            if (s->ps_min_count[p] >= 0) return fail(h, KB_ERR_UNSUPPORTED, "reclaim steps: steps on a record that can be partially admitted");
-    if (s->adm_run_start_ns)
-      for (int a = 0; a < s->n_adm; a++) {
-        const i64 S = s->adm_run_start_ns[a];
-        if (S != INT64_MIN && S > s->now_ns) return fail(h, KB_ERR_INVALID, "reclaim steps: adm_run_start_ns after now_ns");
-      }
-    if (s->adm_run_start_ns)
-      for (int a = 0; a < s->n_adm; a++) {
-        const bool idle = (s->adm_evicted && s->adm_evicted[a]) || (s->adm_check_end_ns && s->adm_check_end_ns[a] != INT64_MIN) ||
-                          (s->adm_admitted_ns && s->adm_admitted_ns[a] != INT64_MIN);
-        if (s->adm_run_start_ns[a] != INT64_MIN && idle) return fail(h, KB_ERR_INVALID, "reclaim steps: adm_run_start_ns on a row that is not running");
-      }
-    bool any_row = false;
-    for (int a = 0; a < s->n_adm; a++) any_row |= s->wl_rc_start[s->adm_wl[a] + 1] > s->wl_rc_start[s->adm_wl[a]];
-    if (any_row && (!s->ps_adm_flavor || !s->ps_adm_count || !s->ps_adm_usage))
-      return fail(h, KB_ERR_INVALID, "reclaim steps: ps_adm_* missing for a row whose record has steps");
-    for (int a = 0; a < s->n_adm && any_row; a++) {
-      const int w = s->adm_wl[a];
-      if (s->wl_rc_start[w + 1] == s->wl_rc_start[w]) continue;
-      std::map<int, i64> want, have;
-      for (int p = s->wl_ps_start[w]; p < s->wl_ps_start[w + 1]; p++)
-        for (int r = 0; r < R; r++) {
-          const int f = s->ps_adm_flavor[(size_t)p * R + r];
-          const i64 u = s->ps_adm_usage[(size_t)p * R + r];
-          const int n = s->ps_adm_count[p];
-          if (f < -1 || f >= s->n_flavor || n < 0 || u < 0) return fail(h, KB_ERR_INVALID, "reclaim steps: ps_adm_* out of range");
-          if (f >= 0 && n > 0) want[f * R + r] += u / n * std::min(s->ps_count[p], n);
-        }
-      for (int c = s->adm_use_start[a]; c < s->adm_use_start[a + 1]; c++) have[s->adm_use_fr[c]] += s->adm_use_qty[c];
-      for (auto *m : {&want, &have})
-        for (auto it = m->begin(); it != m->end();) it = it->second == 0 ? m->erase(it) : std::next(it);
-      if (want != have) return fail(h, KB_ERR_INVALID, "reclaim steps: a row's ps_adm_* do not add up to its adm_use cells");
-    }
-  }
-  out->n_afs_samples = 0;
-  if (Hcap == 0 || max_cycles == 0) {
-    if (rcl && out->ps_remaining_out && s->n_podset) memcpy(out->ps_remaining_out, s->ps_count, (size_t)s->n_podset * 4);
+  return KB_OK;
+}
+// restated by kueue_b200/drain.py check_reclaims
+static int32_t check_reclaim(kb_handle *h, const kb_snapshot *s, const DrainMode &m, HeldRecords &) {
+  if (!m.rcl && !s->rc_after_ns && !s->rc_ps && !s->rc_remaining && !s->rc_sched_hash && !s->ps_adm_flavor && !s->ps_adm_count && !s->ps_adm_usage &&
+      !s->adm_run_start_ns)
     return KB_OK;
+  const int W = s->n_wl, R = s->n_resource;
+  if (!m.replay) return fail(h, KB_ERR_INVALID, "reclaim steps: the tables need adm_wl");
+  if (!m.rcl || (s->n_reclaim > 0 && (!s->rc_after_ns || !s->rc_ps || !s->rc_remaining)))
+    return fail(h, KB_ERR_INVALID, "reclaim steps: a NULL table (wl_rc_start, rc_after_ns, rc_ps, rc_remaining)");
+  if (s->n_reclaim < 0 || s->wl_rc_start[0] != 0 || s->wl_rc_start[W] != s->n_reclaim)
+    return fail(h, KB_ERR_INVALID, "reclaim steps: wl_rc_start is not a CSR of the steps");
+  for (int w = 0; w < W; w++)
+    if (s->wl_rc_start[w + 1] < s->wl_rc_start[w]) return fail(h, KB_ERR_INVALID, "reclaim steps: wl_rc_start is not a CSR of the steps");
+  for (int w = 0; w < W; w++)
+    for (int i = s->wl_rc_start[w]; i < s->wl_rc_start[w + 1]; i++)
+      if (s->rc_ps[i] < s->wl_ps_start[w] || s->rc_ps[i] >= s->wl_ps_start[w + 1]) return fail(h, KB_ERR_INVALID, "reclaim steps: rc_ps outside its record");
+  for (int w = 0; w < W; w++)
+    for (int i = s->wl_rc_start[w]; i < s->wl_rc_start[w + 1]; i++)
+      if (s->rc_after_ns[i] <= 0 || (i > s->wl_rc_start[w] && s->rc_after_ns[i] < s->rc_after_ns[i - 1]))
+        return fail(h, KB_ERR_INVALID, "reclaim steps: rc_after_ns <= 0 or decreasing within a record");
+  std::vector<int32_t> last((size_t)std::max(1, s->n_podset), INT32_MAX);
+  for (int i = 0; i < m.n_rc; i++) {
+    const int p = s->rc_ps[i];
+    if (s->rc_remaining[i] < 0 || s->rc_remaining[i] > last[p]) return fail(h, KB_ERR_INVALID, "reclaim steps: rc_remaining negative or increasing within a podset");
+    last[p] = s->rc_remaining[i];
   }
-  size_t extra = (size_t)std::min<long long>((long long)W, (long long)Hcap * max_cycles);
-  h->drain_extra_adm = extra;
-  h->drain_extra_au = std::min<size_t>((size_t)s->n_podset * R, extra * (size_t)FR);
-  h->drain_mode = true;
-  h->drain_events = events;
-  kb_snapshot s2 = *s;
-  s2.n_heads = Hcap; s2.heads = nullptr;
-  int32_t rc = upload_impl(h, &s2, false);
-  if (rc != KB_OK) return rc;
-  DevSnap &D = h->D;
-  if (!h->ev_d) cudaEventCreate(&h->ev_d);
-  // ---- AdmissionFairSharing: queue segments, one per LocalQueue of a ClusterQueue with cq_afs set and one per other
-  // ClusterQueue, numbered ClusterQueue-major; the initial LocalQueue usage (kb_drain.cuh afs_lq_usage)
-  const bool afs = s->wl_lq != nullptr;
-  const int L = afs ? s->n_lq : 0;
-  // evictions happen only where a target search can: without a preemption policy adm_wl only keeps its records queued-out
-  const bool evict = replay && h->preempt_possible;
-  const bool compact = evict || events;  // rows can die: the admitted tables are compacted after every boundary
-  std::vector<int32_t> seg_start, lq_seg, seg_lq, afs_cqs;
-  std::vector<double> lq_usage;
-  int S = Q;
-  if (afs) {
-    std::vector<int32_t> lq_first((size_t)Q + 1, 0);
-    for (int l = 0; l < L; l++) lq_first[s->lq_cq[l] + 1]++;
-    for (int q = 0; q < Q; q++) lq_first[q + 1] += lq_first[q];
-    seg_start.resize((size_t)Q + 1); lq_seg.assign((size_t)std::max(1, L), -1); lq_usage.assign((size_t)std::max(1, L), 0.0);
-    for (int q = 0; q < Q; q++) {
-      seg_start[q] = (int32_t)seg_lq.size();
-      if (!s->cq_afs[q]) { seg_lq.push_back(-1); continue; }
-      afs_cqs.push_back(q);
-      for (int l = lq_first[q]; l < lq_first[q + 1]; l++) {
-        lq_seg[l] = (int32_t)seg_lq.size(); seg_lq.push_back(l);
-        const size_t o = (size_t)l * R;
-        if (!afs_lq_usage((const i64 *)s->lq_consumed + o, s->lq_consumed_scale + o, s->lq_penalty ? (const i64 *)s->lq_penalty + o : nullptr, s->afs_res_weight,
-                          s->lq_weight[l], R, &lq_usage[l]))
-          return fail(h, KB_ERR_UNSUPPORTED, "afs: consumed usage + entry penalty of a LocalQueue overflows int64");
-      }
-    }
-    seg_start[Q] = (int32_t)seg_lq.size();
-    S = seg_start[Q];
-    if (seg_lq.empty()) seg_lq.push_back(-1);
-  }
-  // ---- drain-only device buffers
-  const size_t Wz = (size_t)W, Hz = (size_t)Hcap, Sz = (size_t)S, Lz = (size_t)std::max(1, L), LR = Lz * R;
-  size_t sort_bytes = 0;
-  {
-    cub::DoubleBuffer<u64> dk(nullptr, nullptr); cub::DoubleBuffer<int32_t> dv(nullptr, nullptr);
-    cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, dk, dv, W, 0, 64, h->stream);
-    sort_bytes += 256;
-  }
-  const size_t trace_cap = out->trace_wl && out->trace_decision ? (size_t)std::max<int64_t>(0, out->trace_capacity) : 0;
-  const size_t Acap = (size_t)s->n_adm + h->drain_extra_adm, AUcap = (size_t)s->n_adm_use + h->drain_extra_au;  // see the boundary loop
-  size_t scan_bytes = 0;
-  if (compact) cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (int32_t *)nullptr, (int32_t *)nullptr, (int)Acap + 1, h->stream);
-  const size_t nR = (size_t)std::max(1, D.nRoots);
-  std::vector<int32_t> wl_class, cq_class_start, rc_class;
-  int n_class = 0;
-  if (events && s->wl_create_ns && s->wl_sched_hash) {  // dense class id per (BestEffortFIFO ClusterQueue, known hash),
-    // the hashes reclaim steps set included (a value >= W names step value - W)
-    std::vector<std::pair<std::pair<int32_t, int64_t>, int32_t>> cls;
+  for (int p = 0; p < s->n_podset; p++)
+    if (last[p] != INT32_MAX && s->ps_count[p] > 0)
+      for (int r = 0; r < R; r++)
+        if (s->ps_req[(size_t)p * R + r] % s->ps_count[p] != 0) return fail(h, KB_ERR_INVALID, "reclaim steps: ps_req of a podset with steps not divisible by its ps_count");
+  if (s->flags & KB_F_PARTIAL_ADMISSION)
     for (int w = 0; w < W; w++)
-      if (s->wl_sched_hash[w] != 0 && s->cq_strategy[s->wl_cq[w]] != KB_QUEUE_STRICT_FIFO) cls.push_back({{s->wl_cq[w], s->wl_sched_hash[w]}, w});
-    if (rcl && s->rc_sched_hash)
-      for (int w = 0; w < W; w++)
-        for (int i = s->wl_rc_start[w]; i < s->wl_rc_start[w + 1]; i++)
-          if (s->rc_sched_hash[i] != 0 && s->cq_strategy[s->wl_cq[w]] != KB_QUEUE_STRICT_FIFO) cls.push_back({{s->wl_cq[w], s->rc_sched_hash[i]}, W + i});
-    std::sort(cls.begin(), cls.end());
-    wl_class.assign(Wz, -1); cq_class_start.assign((size_t)Q + 1, 0); rc_class.assign((size_t)std::max(1, NRC), -1);
-    for (size_t i = 0; i < cls.size(); i++) {
-      if (i > 0 && cls[i].first != cls[i - 1].first) n_class++;
-      if (cls[i].second < W) wl_class[cls[i].second] = n_class;
-      else rc_class[cls[i].second - W] = n_class;
-      cq_class_start[cls[i].first.first + 1] = n_class + 1;
+      if (s->wl_rc_start[w + 1] > s->wl_rc_start[w])
+        for (int p = s->wl_ps_start[w]; p < s->wl_ps_start[w + 1]; p++)
+          if (s->ps_min_count[p] >= 0) return fail(h, KB_ERR_UNSUPPORTED, "reclaim steps: steps on a record that can be partially admitted");
+  if (s->adm_run_start_ns)
+    for (int a = 0; a < s->n_adm; a++) {
+      const i64 S = s->adm_run_start_ns[a];
+      if (S != INT64_MIN && S > s->now_ns) return fail(h, KB_ERR_INVALID, "reclaim steps: adm_run_start_ns after now_ns");
     }
-    if (!cls.empty()) n_class++;
-    for (int q = 0; q < Q; q++) cq_class_start[q + 1] = std::max(cq_class_start[q + 1], cq_class_start[q]);
+  if (s->adm_run_start_ns)
+    for (int a = 0; a < s->n_adm; a++) {
+      const bool idle = (s->adm_evicted && s->adm_evicted[a]) || (s->adm_check_end_ns && s->adm_check_end_ns[a] != INT64_MIN) ||
+                        (s->adm_admitted_ns && s->adm_admitted_ns[a] != INT64_MIN);
+      if (s->adm_run_start_ns[a] != INT64_MIN && idle) return fail(h, KB_ERR_INVALID, "reclaim steps: adm_run_start_ns on a row that is not running");
+    }
+  bool any_row = false;
+  for (int a = 0; a < s->n_adm; a++) any_row |= s->wl_rc_start[s->adm_wl[a] + 1] > s->wl_rc_start[s->adm_wl[a]];
+  if (any_row && (!s->ps_adm_flavor || !s->ps_adm_count || !s->ps_adm_usage))
+    return fail(h, KB_ERR_INVALID, "reclaim steps: ps_adm_* missing for a row whose record has steps");
+  for (int a = 0; a < s->n_adm && any_row; a++) {
+    const int w = s->adm_wl[a];
+    if (s->wl_rc_start[w + 1] == s->wl_rc_start[w]) continue;
+    std::map<int, i64> want, have;
+    for (int p = s->wl_ps_start[w]; p < s->wl_ps_start[w + 1]; p++)
+      for (int r = 0; r < R; r++) {
+        const int f = s->ps_adm_flavor[(size_t)p * R + r];
+        const i64 u = s->ps_adm_usage[(size_t)p * R + r];
+        const int n = s->ps_adm_count[p];
+        if (f < -1 || f >= s->n_flavor || n < 0 || u < 0) return fail(h, KB_ERR_INVALID, "reclaim steps: ps_adm_* out of range");
+        if (f >= 0 && n > 0) want[f * R + r] += u / n * std::min(s->ps_count[p], n);
+      }
+    for (int c = s->adm_use_start[a]; c < s->adm_use_start[a + 1]; c++) have[s->adm_use_fr[c]] += s->adm_use_qty[c];
+    for (auto *mp : {&want, &have})
+      for (auto it = mp->begin(); it != mp->end();) it = it->second == 0 ? mp->erase(it) : std::next(it);
+    if (want != have) return fail(h, KB_ERR_INVALID, "reclaim steps: a row's ps_adm_* do not add up to its adm_use cells");
   }
-  // every buffer of the drain, described once (Arena::carve)
-  u64 *keys[2], *arr_keys[2] = {nullptr, nullptr};
-  int32_t *vals[2], *arr_vals[2] = {nullptr, nullptr}, *q_count, *d_wl_class = nullptr, *d_cq_class_start = nullptr;
-  char *sort_tmp, *scan_tmp = nullptr;
-  i64 *run = nullptr, *create = nullptr, *evict_ns = nullptr, *check_ns = nullptr, *pr_ns = nullptr;
-  int32_t *max_exec = nullptr;
-  i64 *qc_ns_d = nullptr, *qc_rows_d[3] = {nullptr, nullptr, nullptr};
-  i64 *ac_ns_d = nullptr;
-  int32_t *ac_wl_d = nullptr, *ac_next_d = nullptr, *ac_prev_d = nullptr;
-  uint8_t *ac_on_d = nullptr, *inactive_d = nullptr;
-  int32_t *rc_start_d = nullptr, *rc_ps_d = nullptr, *rc_rem_d = nullptr, *rc_class_d = nullptr, *rc_blob_gen_d = nullptr;
-  i64 *rc_after_d = nullptr, *rc_hash_d = nullptr;
-  const size_t Pz = (size_t)std::max(1, s->n_podset), NRCz = (size_t)std::max(1, NRC);
-  int32_t *qc_node_d = nullptr, *qc_root_d = nullptr, *qc_tree_d = nullptr, *qc_tree_next_d = nullptr, *qc_cq_start_d = nullptr, *qc_cq_d = nullptr, *qc_blob_gen_d = nullptr;
+  return KB_OK;
+}
+static int32_t drain_validate(kb_handle *h, const kb_snapshot *s, const DrainMode &m, HeldRecords &held) {
+  using Check = int32_t (*)(kb_handle *, const kb_snapshot *, const DrainMode &, HeldRecords &);
+  held.assign((size_t)std::max(1, s->n_wl), 0);
+  for (Check c : {check_replay, check_events, check_latency, check_decay, check_sticky, check_checks, check_pods_ready, check_max_exec,
+                  check_quota, check_active, check_reclaim})
+    if (int32_t rc = c(h, s, m, held)) return rc;
+  return KB_OK;
+}
+
+// ---- host precomputation: the tables the device starts from
+// n values of a caller's table, or n times v where it passes none
+template <class T, class S> static std::vector<T> drain_table_or(const S *src, size_t n, T v) {
+  return src ? std::vector<T>(src, src + n) : std::vector<T>(n, v);
+}
+// the snapshot's rows at the start of an event drain (kb_drain.cuh DrainFin): finish column, phase, evicting byte, and
+// per record the PodsReady time of a ready attempt under way.  An eviction under way holds its end time (an evicted
+// workload never finishes); a row whose checks run, its verdict time; a row Admitted without PodsReady, its attempt
+// (kb_pr_attempt; no failure is used until a timeout is applied); a row with an Admitted time and a limit, not evicting,
+// the effective deadline max(D, A, now_ns) where it comes first (kb_exec_clip).
+struct DrainRowStart {
+  std::vector<i64> finish, pr_at;
+  std::vector<uint8_t> phase, evicting;  // evicting: empty unless eviction latency with adm_evict_end_ns
+  bool phased;                           // some row starts in another phase than KB_PH_RUN, or may
+};
+static DrainRowStart drain_row_start(const kb_snapshot *s, const DrainMode &m) {
+  const int n = s->n_adm;
+  DrainRowStart o;
+  o.finish = drain_table_or<i64>(s->adm_finish_ns, (size_t)n, INT64_MAX);
+  o.phase.assign((size_t)n, KB_PH_RUN);
+  if (m.pr) o.pr_at.assign((size_t)s->n_wl, INT64_MIN);
+  if (m.lat && s->adm_evict_end_ns) {
+    o.evicting.assign((size_t)n, 0);
+    for (int a = 0; a < n; a++)
+      if (s->adm_evicted[a]) { o.finish[a] = s->adm_evict_end_ns[a]; o.evicting[a] = 1; }
+  }
+  o.phased = (m.checks && s->adm_check_end_ns) || (m.pr && s->adm_admitted_ns) || (m.mx && n > 0);
+  for (int a = 0; a < n && o.phased; a++) {
+    DrainFin f{o.finish[a], KB_PH_RUN};
+    if (m.checks && s->adm_check_end_ns && s->adm_check_end_ns[a] != INT64_MIN) f = {s->adm_check_end_ns[a], KB_PH_CHECK};
+    const int w = m.replay ? s->adm_wl[a] : -1;
+    if (m.pr && s->adm_admitted_ns && s->adm_admitted_ns[a] != INT64_MIN) {
+      const i64 t0 = s->adm_admitted_ns[a], d = s->wl_pods_ready_ns[w];
+      f = kb_pr_attempt(t0, d, s->wl_pods_ready_fail && s->wl_pods_ready_fail[w] > 0, s->pods_ready_timeout_ns, s->wl_run_ns ? s->wl_run_ns[w] : -1);
+      if (f.ph == KB_PH_RUN) o.pr_at[w] = drain_sat_add(t0, d);
+    }
+    if (m.mx && s->adm_exec_since_ns[a] != INT64_MIN && (o.evicting.empty() || !o.evicting[a]))
+      f = kb_exec_clip(f, s->adm_exec_since_ns[a], s->wl_max_exec_s[w], s->wl_exec_acc_s ? s->wl_exec_acc_s[w] : -1, s->now_ns);
+    o.finish[a] = f.fin; o.phase[a] = f.ph;
+  }
+  return o;
+}
+
+// reclaim steps: the snapshot's running rows with steps start at their run start (a ready PodsReady attempt under way:
+// at its PodsReady time), and their records' PodSetAssignments
+struct DrainRcStart { std::vector<i64> next, use; std::vector<int32_t> cur, cnt; std::vector<int8_t> fl; };
+static DrainRcStart drain_reclaim_start(const kb_snapshot *s, const DrainMode &m, const std::vector<i64> &pr_at) {
+  const int R = s->n_resource;
+  const size_t Pz = (size_t)std::max(1, s->n_podset), An = (size_t)std::max(1, s->n_adm);
+  DrainRcStart o;
+  o.next.assign(An, INT64_MAX); o.cur.assign(An, 0);
+  o.fl.assign(Pz * R, -1); o.cnt.assign(Pz, 0); o.use.assign(Pz * R, 0);
+  for (int a = 0; a < s->n_adm; a++) {
+    const int w = s->adm_wl[a], i = s->wl_rc_start[w];
+    if (i == s->wl_rc_start[w + 1]) continue;
+    const size_t p0 = s->wl_ps_start[w], p1 = s->wl_ps_start[w + 1];
+    memcpy(&o.fl[p0 * R], s->ps_adm_flavor + p0 * R, (p1 - p0) * R);
+    memcpy(&o.cnt[p0], s->ps_adm_count + p0, (p1 - p0) * 4);
+    memcpy(&o.use[p0 * R], s->ps_adm_usage + p0 * R, (p1 - p0) * R * 8);
+    i64 S = s->adm_run_start_ns ? s->adm_run_start_ns[a] : INT64_MIN;
+    if (S == INT64_MIN && m.pr && s->adm_admitted_ns && s->adm_admitted_ns[a] != INT64_MIN) S = pr_at[w];
+    if (S == INT64_MIN) continue;
+    o.cur[a] = i;
+    o.next[a] = drain_sat_add(S, s->rc_after_ns[i]);
+  }
+  return o;
+}
+
+// AdmissionFairSharing: queue segments, one per LocalQueue of a ClusterQueue with cq_afs set and one per other
+// ClusterQueue, numbered ClusterQueue-major; the initial usage of every LocalQueue (kb_drain.cuh afs_lq_usage); with
+// decay, the initial admitted usage of every LocalQueue (the cells of the snapshot's rows)
+struct DrainAfs { std::vector<int32_t> seg_start, lq_seg, seg_lq, afs_cqs; std::vector<double> lq_usage; std::vector<i64> lq_adm; };
+static int32_t drain_afs_queues(kb_handle *h, const kb_snapshot *s, const DrainMode &m, DrainAfs &o) {
+  const int Q = s->n_cq, R = s->n_resource, L = s->n_lq;
+  std::vector<int32_t> lq_first((size_t)Q + 1, 0);
+  for (int l = 0; l < L; l++) lq_first[s->lq_cq[l] + 1]++;
+  for (int q = 0; q < Q; q++) lq_first[q + 1] += lq_first[q];
+  o.seg_start.resize((size_t)Q + 1); o.lq_seg.assign((size_t)std::max(1, L), -1); o.lq_usage.assign((size_t)std::max(1, L), 0.0);
+  for (int q = 0; q < Q; q++) {
+    o.seg_start[q] = (int32_t)o.seg_lq.size();
+    if (!s->cq_afs[q]) { o.seg_lq.push_back(-1); continue; }
+    o.afs_cqs.push_back(q);
+    for (int l = lq_first[q]; l < lq_first[q + 1]; l++) {
+      o.lq_seg[l] = (int32_t)o.seg_lq.size(); o.seg_lq.push_back(l);
+      const size_t k = (size_t)l * R;
+      if (!afs_lq_usage((const i64 *)s->lq_consumed + k, s->lq_consumed_scale + k, s->lq_penalty ? (const i64 *)s->lq_penalty + k : nullptr, s->afs_res_weight,
+                        s->lq_weight[l], R, &o.lq_usage[l]))
+        return fail(h, KB_ERR_UNSUPPORTED, "afs: consumed usage + entry penalty of a LocalQueue overflows int64");
+    }
+  }
+  o.seg_start[Q] = (int32_t)o.seg_lq.size();
+  if (o.seg_lq.empty()) o.seg_lq.push_back(-1);
+  if (m.decay) {
+    o.lq_adm.assign((size_t)std::max(1, L) * R, 0);
+    for (int a = 0; a < s->n_adm; a++)
+      if (s->adm_lq[a] >= 0)
+        for (int c = s->adm_use_start[a]; c < s->adm_use_start[a + 1]; c++) o.lq_adm[(size_t)s->adm_lq[a] * R + s->adm_use_fr[c] % R] += s->adm_use_qty[c];
+  }
+  return KB_OK;
+}
+
+// NoFit classes (event mode with arrivals and hashes): a dense id per (BestEffortFIFO ClusterQueue, known hash), the
+// hashes reclaim steps set included; n = 0: none
+struct DrainClasses { int n = 0; std::vector<int32_t> wl_class, cq_class_start, rc_class; };
+static DrainClasses drain_nofit_classes(const kb_snapshot *s, const DrainMode &m) {
+  const int W = s->n_wl, Q = s->n_cq;
+  DrainClasses o;
+  if (!m.events || !s->wl_create_ns || !s->wl_sched_hash) return o;
+  std::vector<std::pair<std::pair<int32_t, int64_t>, int32_t>> cls;  // a value >= W names step value - W
+  for (int w = 0; w < W; w++)
+    if (s->wl_sched_hash[w] != 0 && s->cq_strategy[s->wl_cq[w]] != KB_QUEUE_STRICT_FIFO) cls.push_back({{s->wl_cq[w], s->wl_sched_hash[w]}, w});
+  if (m.rcl && s->rc_sched_hash)
+    for (int w = 0; w < W; w++)
+      for (int i = s->wl_rc_start[w]; i < s->wl_rc_start[w + 1]; i++)
+        if (s->rc_sched_hash[i] != 0 && s->cq_strategy[s->wl_cq[w]] != KB_QUEUE_STRICT_FIFO) cls.push_back({{s->wl_cq[w], s->rc_sched_hash[i]}, W + i});
+  std::sort(cls.begin(), cls.end());
+  o.wl_class.assign((size_t)W, -1); o.cq_class_start.assign((size_t)Q + 1, 0); o.rc_class.assign((size_t)std::max(1, m.n_rc), -1);
+  for (size_t i = 0; i < cls.size(); i++) {
+    if (i > 0 && cls[i].first != cls[i - 1].first) o.n++;
+    if (cls[i].second < W) o.wl_class[cls[i].second] = o.n;
+    else o.rc_class[cls[i].second - W] = o.n;
+    o.cq_class_start[cls[i].first.first + 1] = o.n + 1;
+  }
+  if (!cls.empty()) o.n++;
+  for (int q = 0; q < Q; q++) o.cq_class_start[q + 1] = std::max(o.cq_class_start[q + 1], o.cq_class_start[q]);
+  return o;
+}
+
+// byte offset of every ClusterQueue's generation in the static tree blocks, -1 = not in a tree
+static std::vector<int32_t> drain_blob_gen(const kb_handle *h, int Q) {
+  std::vector<int32_t> off((size_t)std::max(1, Q), -1);
+  for (int q = 0; q < Q; q++) {
+    const int slot = h->root_slot[q];
+    if (slot < h->D.nLone) continue;
+    const int tr = slot - h->D.nLone, b0 = h->tree_blob_off[tr];
+    const TreeBlobHdr *BH = (const TreeBlobHdr *)(h->tree_blob.data() + b0);
+    off[q] = b0 + BH->gen + 8 * h->local_idx[q];
+  }
+  return off;
+}
+
+// quota changes: the edits that change nothing (root -1), the root slot and the cohort tree of every other one (the rows
+// change only through the edits, in table order, so the rows an edit meets are known here), the next edit of the same
+// tree, the ClusterQueues of every root, the place of every ClusterQueue's generation in the static tree blocks
+struct DrainQuota { std::vector<int32_t> root, tree, tree_next, cq_start, cq, blob_gen; };
+static DrainQuota drain_quota_prep(const kb_handle *h, const kb_snapshot *s, const DrainMode &m) {
+  const int Q = s->n_cq, FR = s->n_flavor * s->n_resource, QN = Q + s->n_cohort, NQC = m.n_qc;
+  const DevSnap &D = h->D;
+  DrainQuota o;
+  std::vector<i64> nom(s->nominal, s->nominal + (size_t)QN * FR), bl(s->borrow_limit, s->borrow_limit + (size_t)QN * FR),
+      ll(s->lend_limit, s->lend_limit + (size_t)QN * FR);  // the rows each edit meets
+  o.root.assign((size_t)NQC, -1); o.tree.assign((size_t)NQC, -1);
+  for (int i = 0; i < NQC; i++) {
+    const int n = s->qc_node[i];
+    const size_t r = (size_t)n * FR, k = (size_t)i * FR, b = (size_t)FR * 8;
+    if (!memcmp(&nom[r], s->qc_nominal + k, b) && !memcmp(&bl[r], s->qc_borrow_limit + k, b) && !memcmp(&ll[r], s->qc_lend_limit + k, b)) continue;
+    memcpy(&nom[r], s->qc_nominal + k, b); memcpy(&bl[r], s->qc_borrow_limit + k, b); memcpy(&ll[r], s->qc_lend_limit + k, b);
+    o.root[i] = h->root_slot[n];
+    if (D.tl_subtree && h->root_slot[n] >= D.nLone) o.tree[i] = h->root_slot[n] - D.nLone;  // lone ClusterQueues come first
+  }
+  o.tree_next.assign((size_t)NQC, NQC);
+  std::vector<int32_t> later((size_t)std::max(1, D.nTrees), NQC);
+  for (int i = NQC - 1; i >= 0; i--)
+    if (o.tree[i] >= 0) { o.tree_next[i] = later[o.tree[i]]; later[o.tree[i]] = i; }
+  o.cq_start.assign(h->root_cq_start.begin(), h->root_cq_start.end());
+  o.cq.assign((size_t)std::max(1, Q), 0);
+  std::vector<int32_t> fill(o.cq_start.begin(), o.cq_start.end() - 1);
+  for (int q = 0; q < Q; q++) o.cq[fill[h->root_slot[q]]++] = q;
+  o.blob_gen = drain_blob_gen(h, Q);
+  return o;
+}
+
+// deactivation / reactivation: each edit's previous and next edit of the same record (-1 / n_ac = none)
+static void drain_active_links(const kb_snapshot *s, const DrainMode &m, std::vector<int32_t> &next, std::vector<int32_t> &prev) {
+  const int NAC = m.n_ac;
+  next.assign((size_t)std::max(1, NAC), NAC); prev.assign((size_t)std::max(1, NAC), -1);
+  std::vector<int32_t> last((size_t)std::max(1, s->n_wl), -1);
+  for (int i = 0; i < NAC; i++) {
+    const int w = s->ac_wl[i];
+    if (last[w] >= 0) { prev[i] = last[w]; next[last[w]] = i; }
+    last[w] = i;
+  }
+}
+
+// ---- the boundary counters kb_drain_out reports: each row names its slot in DrainDev::counters, how the slot counts,
+// the drain's total and per-cycle array, and whether the drain's blocks write it.  A cleared slot is zeroed every
+// boundary (kb_run_drain's memsets), a cumulative one counts since the start of the drain (the host differences it), a
+// range is the [lo, hi) pair of slots idx, idx + 1 of the edits a boundary applied.
+enum { DC_CLEARED, DC_CUMULATIVE, DC_RANGE };
+struct DrainCounter { int idx, kind; int64_t *total; int32_t *cycle; bool on; uint32_t seen; };
+static std::vector<DrainCounter> drain_counters(kb_drain_out *out, const DrainMode &m) {
+  return {{KB_DC_FINISHED, DC_CLEARED, &out->n_finished, out->cycle_finished, m.events, 0},
+          {KB_DC_ARRIVED, DC_CLEARED, &out->n_arrived, out->cycle_arrived, m.events, 0},
+          {KB_DC_EVICT_DONE, DC_CLEARED, &out->n_evict_done, out->cycle_evict_done, m.lat, 0},
+          {KB_DC_CHECK_READY, DC_CUMULATIVE, &out->n_check_ready, nullptr, m.checks, 0},
+          {KB_DC_CHECK_RETRY, DC_CUMULATIVE, &out->n_check_retry, out->cycle_check_retry, m.checks, 0},
+          {KB_DC_CHECK_REJECTED, DC_CUMULATIVE, &out->n_check_rejected, out->cycle_check_rejected, m.checks, 0},
+          {KB_DC_PR_TIMEOUT, DC_CUMULATIVE, &out->n_pods_ready_timeout, out->cycle_pods_ready_timeout, m.pr, 0},
+          {KB_DC_PR_DEACTIVATED, DC_CUMULATIVE, &out->n_pods_ready_deactivated, out->cycle_pods_ready_deactivated, m.pr, 0},
+          {KB_DC_EXEC_DEACTIVATED, DC_CUMULATIVE, &out->n_max_exec_deactivated, out->cycle_max_exec_deactivated, m.mx, 0},
+          {KB_DC_QC_LO, DC_RANGE, &out->n_quota_changes, out->cycle_quota_changes, m.quota, 0},
+          {KB_DC_STOPPED, DC_CUMULATIVE, &out->n_stopped, out->cycle_stopped, m.act, 0},
+          {KB_DC_RESUMED, DC_CUMULATIVE, &out->n_resumed, out->cycle_resumed, m.act, 0},
+          {KB_DC_RECLAIMS, DC_CUMULATIVE, &out->n_reclaims, out->cycle_reclaims, m.rcl, 0}};
+}
+
+// ---- one kb_run_drain call (the counterpart of kueue_b200/drain.py _Drain): the mode, the host tables of the plan,
+// the device buffers, and the state of the boundary loop
+struct DrainRun {
+  kb_handle *h; const kb_snapshot *s; kb_drain_out *out;
+  DrainMode m;
+  std::vector<DrainCounter> counters;
+  HeldRecords held;  // held[w]: an admitted row names record w (drain_validate)
+  int Q, W, R, FR, Hcap, max_cycles;
+  // plan
+  int S = 0, L = 0;  // queue segments, LocalQueues
+  DrainAfs afs; DrainClasses cls; DrainQuota qc; DrainRowStart rows; DrainRcStart rc;
+  std::vector<int32_t> ac_next, ac_prev, rc_blob_gen;
+  std::vector<i64> qts, requeue_at, pr_none; std::vector<int32_t> fails, retries, pr_fails, pr_counts, exec_acc;  // records at the start
+  size_t Acap = 0, AUcap = 0, sort_bytes = 0, scan_bytes = 0, trace_cap = 0, nR = 1;
+  // device buffers
   DrainDev X{};
-  AdmTabs other{};  // compaction: the other half of the admitted tables' double buffer
+  AdmRows other{};  // compaction: the other half of the admitted rows' double buffer
+  u64 *keys[2] = {}, *arr_keys[2] = {}; int32_t *vals[2] = {}, *arr_vals[2] = {}, *q_count = nullptr;
+  char *sort_tmp = nullptr, *scan_tmp = nullptr;
+  i64 *create = nullptr; uint8_t *inactive = nullptr;
+  // boundary loop
+  int n_used = 1, n_live = 0, A_cur = 0, AU_cur = 0, cyc = 0, jumps = 0;
+  i64 t = 0, step = 1;
+  double gpu_ms = 0;
+  float kms[KB_N_KERNELS] = {};  // per-kernel times summed over the cycles (kb_set_profile)
+  cudaEvent_t ev_r[2] = {nullptr, nullptr};  // around a re-sort (admission checks, PodsReady)
+  bool resort_timed = false;
+  ~DrainRun() { for (cudaEvent_t e : ev_r) if (e) cudaEventDestroy(e); }
+};
+static constexpr int DRAIN_TB = 256;
+static int drain_blocks(long long n) { return (int)((n + DRAIN_TB - 1) / DRAIN_TB); }
+
+// the DevSnap's admitted tables are the first nine columns of the current half
+static AdmRows drain_snap_rows(const DevSnap &D) {
+  AdmRows r{};
+  r.cq = const_cast<int32_t *>(D.adm_cq); r.priority = const_cast<int32_t *>(D.adm_priority); r.ts = const_cast<i64 *>(D.adm_ts);
+  r.qr_ts = const_cast<i64 *>(D.adm_qr_ts); r.uid = const_cast<i64 *>(D.adm_uid); r.evicted = const_cast<uint8_t *>(D.adm_evicted);
+  r.use_start = const_cast<int32_t *>(D.adm_use_start); r.use_fr = const_cast<int32_t *>(D.adm_use_fr); r.use_qty = const_cast<i64 *>(D.adm_use_qty);
+  return r;
+}
+static void drain_point_snap(DevSnap &D, const AdmRows &r) {
+  D.adm_cq = r.cq; D.adm_priority = r.priority; D.adm_ts = r.ts; D.adm_qr_ts = r.qr_ts; D.adm_uid = r.uid;
+  D.adm_evicted = r.evicted; D.adm_use_start = r.use_start; D.adm_use_fr = r.use_fr; D.adm_use_qty = r.use_qty;
+}
+// the columns of one half of the admitted rows its blocks need; base: the nine the first half borrows from the DevSnap
+static void drain_carve_rows(Arena &a, AdmRows &r, const DrainMode &m, size_t Acap, size_t AUcap, bool base) {
+  if (base) {
+    r.cq = a.take<int32_t>(Acap); r.priority = a.take<int32_t>(Acap); r.ts = a.take<i64>(Acap);
+    r.qr_ts = a.take<i64>(Acap); r.uid = a.take<i64>(Acap); r.evicted = a.take<uint8_t>(Acap);
+    r.use_start = a.take<int32_t>(Acap + 1); r.use_fr = a.take<int32_t>(AUcap); r.use_qty = a.take<i64>(AUcap);
+  }
+  if (m.replay || m.events) r.wl = a.take<int32_t>(Acap);
+  if (m.events) r.finish = a.take<i64>(Acap);
+  if (m.decay) r.lq = a.take<int32_t>(Acap);
+  if (m.lat) r.evicting = a.take<uint8_t>(Acap);
+  if (m.requeue || m.mx) r.phase = a.take<uint8_t>(Acap);
+  if (m.mx) r.since = a.take<i64>(Acap);
+  if (m.rcl) { r.rc_next = a.take<i64>(Acap); r.rc_cur = a.take<int32_t>(Acap); }
+}
+
+// after upload_impl: whether rows can die, the host tables, the sizes of the buffers
+static int32_t drain_plan(DrainRun &r) {
+  kb_handle *h = r.h; const kb_snapshot *s = r.s; DrainMode &m = r.m;
+  // evictions happen only where a target search can: without a preemption policy adm_wl only keeps its records queued-out
+  m.evict = m.replay && h->preempt_possible;
+  m.compact = m.evict || m.events;
+  r.S = r.Q;
+  if (m.afs) {
+    r.L = s->n_lq;
+    if (int32_t rc = drain_afs_queues(h, s, m, r.afs)) return rc;
+    r.S = r.afs.seg_start[r.Q];
+  }
+  cub::DoubleBuffer<u64> dk(nullptr, nullptr); cub::DoubleBuffer<int32_t> dv(nullptr, nullptr);
+  cub::DeviceRadixSort::SortPairs(nullptr, r.sort_bytes, dk, dv, r.W, 0, 64, h->stream);
+  r.sort_bytes += 256;
+  r.trace_cap = r.out->trace_wl && r.out->trace_decision ? (size_t)std::max<int64_t>(0, r.out->trace_capacity) : 0;
+  r.Acap = (size_t)s->n_adm + h->drain_extra_adm; r.AUcap = (size_t)s->n_adm_use + h->drain_extra_au;  // see drain_boundary
+  if (m.compact) cub::DeviceScan::ExclusiveSum(nullptr, r.scan_bytes, (int32_t *)nullptr, (int32_t *)nullptr, (int)r.Acap + 1, h->stream);
+  r.nR = (size_t)std::max(1, h->D.nRoots);
+  r.cls = drain_nofit_classes(s, m);
+  if (m.events) r.rows = drain_row_start(s, m);
+  if (m.quota) r.qc = drain_quota_prep(h, s, m);
+  if (m.act) drain_active_links(s, m, r.ac_next, r.ac_prev);
+  if (m.rcl) { r.rc = drain_reclaim_start(s, m, r.rows.pr_at); r.rc_blob_gen = drain_blob_gen(h, r.Q); }
+  // the counter slots [0, n_used) a boundary reads back: the heads; with compaction the evictions, rows, cells and
+  // capacity flag; the end flag, re-sort stamp and execution-time status of their blocks; every reported counter
+  r.n_used = m.compact ? KB_DC_FULL + 1 : 1;
+  if (m.events) r.n_used = std::max(r.n_used, KB_DC_END + 1);
+  if (m.requeue) r.n_used = std::max(r.n_used, KB_DC_RESORT + 1);
+  if (m.mx) r.n_used = std::max(r.n_used, KB_DC_EXEC_STATUS + 1);
+  for (const DrainCounter &c : r.counters)
+    if (c.on) r.n_used = std::max(r.n_used, c.idx + (c.kind == DC_RANGE ? 2 : 1));
+  return KB_OK;
+}
+
+// every buffer of the drain, described once (Arena::carve)
+static bool drain_carve(DrainRun &r) {
+  const DrainMode &m = r.m;
+  DrainDev &X = r.X;
+  const int Q = r.Q, R = r.R, FR = r.FR, L = r.L;
+  const size_t Wz = (size_t)r.W, Hz = (size_t)r.Hcap, Sz = (size_t)r.S, Lz = (size_t)std::max(1, L), LR = Lz * R, Acap = r.Acap;
+  const size_t Pz = (size_t)std::max(1, r.s->n_podset), NQC = (size_t)m.n_qc, NAC = (size_t)m.n_ac, NRCz = (size_t)std::max(1, m.n_rc);
   auto layout = [&](Arena &a) {
-    keys[0] = a.take<u64>(Wz); keys[1] = a.take<u64>(Wz);
-    vals[0] = a.take<int32_t>(Wz); vals[1] = a.take<int32_t>(Wz);
-    sort_tmp = a.take<char>(sort_bytes);
-    q_count = a.take<int32_t>(Sz + 2);
+    r.keys[0] = a.take<u64>(Wz); r.keys[1] = a.take<u64>(Wz);
+    r.vals[0] = a.take<int32_t>(Wz); r.vals[1] = a.take<int32_t>(Wz);
+    r.sort_tmp = a.take<char>(r.sort_bytes);
+    r.q_count = a.take<int32_t>(Sz + 2);
     X.q_start = a.take<int32_t>(Sz + 2); X.cursor = a.take<int32_t>(Sz); X.wl_state = a.take<uint8_t>(Wz);
     X.first_aside = a.take<int32_t>(Sz);
     X.flag = a.take<int32_t>((size_t)Q + 2); X.pos = a.take<int32_t>((size_t)Q + 2);
@@ -1784,172 +2019,113 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     X.e_adm_off = a.take<int32_t>(Hz + 2); X.e_cell_off = a.take<int32_t>(Hz + 2);
     X.counters = a.take<int32_t>(KB_DC_RECLAIMS + 1);
     X.wl_admit_cycle = a.take<int32_t>(Wz); X.wl_evals = a.take<int32_t>(Wz); X.wl_last_decision = a.take<uint8_t>(Wz);
-    if (trace_cap) { X.trace_wl = a.take<int32_t>(trace_cap); X.trace_dec = a.take<uint8_t>(trace_cap); }
-    if (replay || events) {
-      X.adm_wl = a.take<int32_t>(Acap);
-      X.wl_seg = a.take<int32_t>(Wz); X.wl_pos = a.take<int32_t>(Wz); X.wl_evictions = a.take<int32_t>(Wz);
-    } else if (sticky) {  // the sticky head's position
-      X.wl_seg = a.take<int32_t>(Wz); X.wl_pos = a.take<int32_t>(Wz);
-    }
-    if (sticky) X.cq_sticky = a.take<int32_t>((size_t)Q);
-    if (compact) {
-      X.adm_dead = a.take<int32_t>(Acap); other.wl = a.take<int32_t>(Acap); X.root_mark = a.take<int32_t>(nR);
+    if (r.trace_cap) { X.trace_wl = a.take<int32_t>(r.trace_cap); X.trace_dec = a.take<uint8_t>(r.trace_cap); }
+    if (m.replay || m.events || m.sticky) { X.wl_seg = a.take<int32_t>(Wz); X.wl_pos = a.take<int32_t>(Wz); }  // sticky: the head's position
+    if (m.replay || m.events) X.wl_evictions = a.take<int32_t>(Wz);
+    if (m.sticky) X.cq_sticky = a.take<int32_t>((size_t)Q);
+    drain_carve_rows(a, X.adm, m, Acap, r.AUcap, false);
+    if (m.compact) {
+      drain_carve_rows(a, r.other, m, Acap, r.AUcap, true);
+      X.adm_dead = a.take<int32_t>(Acap); X.root_mark = a.take<int32_t>(r.nR);
       X.row_live = a.take<int32_t>(Acap + 1); X.row_cells = a.take<int32_t>(Acap + 1);
       X.row_new = a.take<int32_t>(Acap + 1); X.cell_new = a.take<int32_t>(Acap + 1);
-      scan_tmp = a.take<char>(scan_bytes + 256);
-      other.cq = a.take<int32_t>(Acap); other.priority = a.take<int32_t>(Acap); other.ts = a.take<i64>(Acap);
-      other.qr_ts = a.take<i64>(Acap); other.uid = a.take<i64>(Acap); other.evicted = a.take<uint8_t>(Acap);
-      other.use_start = a.take<int32_t>(Acap + 1); other.use_fr = a.take<int32_t>(AUcap); other.use_qty = a.take<i64>(AUcap);
+      r.scan_tmp = a.take<char>(r.scan_bytes + 256);
     }
-    if (events) {  // finish columns of both halves, run times, admit / finish times, the clock, the arrival order (sorted
-                   // pairs and their double buffers) and the NoFit classes
-      X.adm_finish = a.take<i64>(Acap); other.finish = a.take<i64>(Acap);
-      run = a.take<i64>(Wz);
+    if (m.events) {  // run times, admit / finish times, the clock, the arrival order (sorted pairs and their double
+                     // buffers) and the NoFit classes
+      if (r.s->wl_run_ns) X.wl_run = a.take<i64>(Wz);
       X.wl_admit_ns = a.take<i64>(Wz); X.wl_finish_ns = a.take<i64>(Wz); X.clock = a.take<i64>(4);
-      if (s->wl_create_ns) {
-        arr_keys[0] = a.take<u64>(Wz); arr_keys[1] = a.take<u64>(Wz);
-        arr_vals[0] = a.take<int32_t>(Wz); arr_vals[1] = a.take<int32_t>(Wz);
-        create = a.take<i64>(Wz);
+      if (r.s->wl_create_ns) {
+        r.arr_keys[0] = a.take<u64>(Wz); r.arr_keys[1] = a.take<u64>(Wz);
+        r.arr_vals[0] = a.take<int32_t>(Wz); r.arr_vals[1] = a.take<int32_t>(Wz);
+        r.create = a.take<i64>(Wz);
       }
-      if (n_class) { d_wl_class = a.take<int32_t>(Wz); d_cq_class_start = a.take<int32_t>((size_t)Q + 1); X.class_nofit = a.take<uint8_t>(n_class); }
+      if (r.cls.n) { X.wl_class = a.take<int32_t>(Wz); X.cq_class_start = a.take<int32_t>((size_t)Q + 1); X.class_nofit = a.take<uint8_t>(r.cls.n); }
     }
-    if (lat) {  // latencies and the evicting byte of both halves
-      evict_ns = a.take<i64>(Wz);
-      X.adm_evicting = a.take<uint8_t>(Acap); other.evicting = a.take<uint8_t>(Acap);
-    }
-    if (checks) {  // check delays and attempt state
-      check_ns = a.take<i64>(Wz); X.wl_fail = a.take<int32_t>(Wz); X.wl_retries = a.take<int32_t>(Wz);
-    }
-    if (pr) {  // PodsReady delays and attempt state
-      pr_ns = a.take<i64>(Wz); X.wl_pr_fail = a.take<int32_t>(Wz); X.wl_pr_count = a.take<int32_t>(Wz);
+    if (m.lat) X.wl_evict = a.take<i64>(Wz);
+    if (m.checks) { X.wl_check = a.take<i64>(Wz); X.wl_fail = a.take<int32_t>(Wz); X.wl_retries = a.take<int32_t>(Wz); }
+    if (m.pr) {
+      X.wl_pr = a.take<i64>(Wz); X.wl_pr_fail = a.take<int32_t>(Wz); X.wl_pr_count = a.take<int32_t>(Wz);
       X.wl_pr_at = a.take<i64>(Wz); X.wl_pr_prev = a.take<i64>(Wz);
     }
-    if (requeue) {  // timestamps and requeue state
-      X.wl_ts0 = a.take<i64>(Wz); X.wl_sort_ts = a.take<i64>(Wz); X.wl_requeue_at = a.take<i64>(Wz);
-      X.wl_ready_ns = a.take<i64>(Wz);
-    }
-    if (requeue || mx || blk) X.wl_deactivated = a.take<uint8_t>(Wz);  // deactivation reasons
-    if (requeue || mx) { X.adm_phase = a.take<uint8_t>(Acap); other.phase = a.take<uint8_t>(Acap); }  // the phase byte of both halves
-    if (mx) {  // limits, accumulated times and the Admitted time of both halves
-      max_exec = a.take<int32_t>(Wz); X.wl_exec_acc = a.take<int32_t>(Wz);
-      X.adm_exec_since = a.take<i64>(Acap); other.since = a.take<i64>(Acap);
-    }
-    if (afs) {
-      X.seg_start = a.take<int32_t>(seg_start.size()); X.lq_seg = a.take<int32_t>(lq_seg.size());
-      X.seg_lq = a.take<int32_t>(seg_lq.size()); X.afs_cqs = a.take<int32_t>(afs_cqs.size());
+    if (m.requeue) { X.wl_ts0 = a.take<i64>(Wz); X.wl_sort_ts = a.take<i64>(Wz); X.wl_requeue_at = a.take<i64>(Wz); X.wl_ready_ns = a.take<i64>(Wz); }
+    if (m.deact) X.wl_deactivated = a.take<uint8_t>(Wz);
+    if (m.mx) { X.wl_max_exec = a.take<int32_t>(Wz); X.wl_exec_acc = a.take<int32_t>(Wz); }
+    if (m.afs) {
+      X.seg_start = a.take<int32_t>(r.afs.seg_start.size()); X.lq_seg = a.take<int32_t>(r.afs.lq_seg.size());
+      X.seg_lq = a.take<int32_t>(r.afs.seg_lq.size()); X.afs_cqs = a.take<int32_t>(r.afs.afs_cqs.size());
       X.head_seg = a.take<int32_t>(Q); X.wl_lq = a.take<int32_t>(Wz); X.cq_afs = a.take<uint8_t>(Q);
       X.lq_weight = a.take<double>(L); X.lq_consumed = a.take<i64>((size_t)L * R); X.lq_consumed_scale = a.take<int32_t>((size_t)L * R);
       X.lq_penalty = a.take<i64>(LR); X.lq_usage = a.take<double>(Lz);
       X.res_weight = a.take<double>(R); X.milli_mul = a.take<i64>(R);
     }
-    if (decay) {
-      X.lq_last = a.take<i64>(Lz); X.lq_adm = a.take<i64>(LR);
-      X.adm_lq = a.take<int32_t>(Acap); other.lq = a.take<int32_t>(Acap);
-      X.afs_samples = a.take<unsigned long long>(1);
+    if (m.decay) { X.lq_last = a.take<i64>(Lz); X.lq_adm = a.take<i64>(LR); X.afs_samples = a.take<unsigned long long>(1); }
+    if (m.quota) {  // the edits and drain_quota_prep's tables
+      X.qc_ns = a.take<i64>(NQC); X.qc_node = a.take<int32_t>(NQC);
+      X.qc_nominal = a.take<i64>(NQC * FR); X.qc_blimit = a.take<i64>(NQC * FR); X.qc_llimit = a.take<i64>(NQC * FR);
+      X.qc_root = a.take<int32_t>(NQC); X.qc_tree = a.take<int32_t>(NQC); X.qc_tree_next = a.take<int32_t>(NQC);
+      X.qc_cq_start = a.take<int32_t>(r.nR + 1); X.qc_cq = a.take<int32_t>((size_t)std::max(1, Q)); X.qc_blob_gen = a.take<int32_t>((size_t)std::max(1, Q));
     }
-    if (quota) {  // the edits and the host's precomputation (quota_prep below)
-      qc_ns_d = a.take<i64>(NQC); qc_node_d = a.take<int32_t>(NQC);
-      qc_rows_d[0] = a.take<i64>((size_t)NQC * FR); qc_rows_d[1] = a.take<i64>((size_t)NQC * FR); qc_rows_d[2] = a.take<i64>((size_t)NQC * FR);
-      qc_root_d = a.take<int32_t>(NQC); qc_tree_d = a.take<int32_t>(NQC); qc_tree_next_d = a.take<int32_t>(NQC);
-      qc_cq_start_d = a.take<int32_t>(nR + 1); qc_cq_d = a.take<int32_t>((size_t)std::max(1, Q)); qc_blob_gen_d = a.take<int32_t>((size_t)std::max(1, Q));
-    }
-    if (s->wl_inactive) inactive_d = a.take<uint8_t>(Wz);
-    if (act) {  // the edits, their neighbours, and the per-record state of a boundary
-      ac_ns_d = a.take<i64>(NAC); ac_wl_d = a.take<int32_t>(NAC); ac_on_d = a.take<uint8_t>(NAC);
-      ac_next_d = a.take<int32_t>(NAC); ac_prev_d = a.take<int32_t>(NAC);
+    if (r.s->wl_inactive) r.inactive = a.take<uint8_t>(Wz);
+    if (m.act) {  // the edits, their neighbours, and the per-record state of a boundary
+      X.ac_ns = a.take<i64>(NAC); X.ac_wl = a.take<int32_t>(NAC); X.ac_on = a.take<uint8_t>(NAC);
+      X.ac_next = a.take<int32_t>(NAC); X.ac_prev = a.take<int32_t>(NAC);
       X.wl_ac_from = a.take<int32_t>(Wz); X.wl_stop = a.take<i64>(Wz); X.wl_gone = a.take<i64>(Wz);
     }
-    if (rcl) {  // the steps, the records' assignments, the two row columns of both halves, the generations' blob offsets
-      rc_start_d = a.take<int32_t>(Wz + 1); rc_after_d = a.take<i64>(NRCz); rc_ps_d = a.take<int32_t>(NRCz); rc_rem_d = a.take<int32_t>(NRCz);
-      if (s->rc_sched_hash) rc_hash_d = a.take<i64>(NRCz);
-      if (n_class) rc_class_d = a.take<int32_t>(NRCz);
+    if (m.rcl) {  // the steps, the records' assignments, the generations' blob offsets
+      X.wl_rc_start = a.take<int32_t>(Wz + 1); X.rc_after = a.take<i64>(NRCz); X.rc_ps = a.take<int32_t>(NRCz); X.rc_remaining = a.take<int32_t>(NRCz);
+      if (r.s->rc_sched_hash) X.rc_hash = a.take<i64>(NRCz);
+      if (r.cls.n) X.rc_class = a.take<int32_t>(NRCz);
       X.ps_adm_cnt = a.take<int32_t>(Pz); X.ps_adm_fl = a.take<int8_t>(Pz * R); X.ps_adm_use = a.take<i64>(Pz * R);
-      X.adm_rc_next = a.take<i64>(Acap); other.rc_next = a.take<i64>(Acap);
-      X.adm_rc_cur = a.take<int32_t>(Acap); other.rc_cur = a.take<int32_t>(Acap);
-      rc_blob_gen_d = a.take<int32_t>((size_t)std::max(1, Q));
+      X.rc_blob_gen = a.take<int32_t>((size_t)std::max(1, Q));
     }
   };
-  if (!h->drain_arena.carve(layout)) return fail(h, KB_ERR_CUDA, "kb_run_drain: cudaMalloc of the drain buffer failed");
-  X.trace_cap = (long long)trace_cap;
+  return r.h->drain_arena.carve(layout);
+}
+
+// uploads and initial values of the drain's tables
+static int32_t drain_upload(DrainRun &r) {
+  kb_handle *h = r.h; const kb_snapshot *s = r.s; const DrainMode &m = r.m;
+  DrainDev &X = r.X; DevSnap &D = h->D;
+  const int W = r.W, Q = r.Q, R = r.R, L = r.L;
+  const size_t Wz = (size_t)W, n_adm = (size_t)s->n_adm, LR = (size_t)std::max(1, L) * R;
+  X.trace_cap = (long long)r.trace_cap;
   X.cq_usage = const_cast<i64 *>(D.cq_usage); X.wl_last_gen = const_cast<i64 *>(D.wl_last_gen); X.ps_last_tried = const_cast<int8_t *>(D.ps_last_tried);
-  X.adm_cq = const_cast<int32_t *>(D.adm_cq); X.adm_priority = const_cast<int32_t *>(D.adm_priority);
-  X.adm_ts = const_cast<i64 *>(D.adm_ts); X.adm_qr_ts = const_cast<i64 *>(D.adm_qr_ts); X.adm_uid = const_cast<i64 *>(D.adm_uid);
-  X.adm_evicted = const_cast<uint8_t *>(D.adm_evicted); X.adm_use_start = const_cast<int32_t *>(D.adm_use_start);
-  X.adm_use_fr = const_cast<int32_t *>(D.adm_use_fr); X.adm_use_qty = const_cast<i64 *>(D.adm_use_qty);
-  X.A_cap = (int)Acap; X.AU_cap = (int)AUcap;
-  // ---- uploads and initial values
-  if (replay || events) {  // event mode without adm_wl: the rows of the snapshot have no record (-1)
-    if (replay) CUDA_TRY(h, h2d(h, X.adm_wl, s->adm_wl, (size_t)s->n_adm * 4));
-    else CUDA_TRY(h, cudaMemsetAsync(X.adm_wl, 0xff, (size_t)s->n_adm * 4, h->stream));
+  X.A_cap = (int)r.Acap; X.AU_cap = (int)r.AUcap;
+  // every counter starts at 0, once: the cumulative ones are never cleared, and no kernel before the first boundary
+  // writes a counter but k_drain_init_events (the arrived prefix) and k_drain_heads
+  CUDA_TRY(h, cudaMemsetAsync(X.counters, 0, (KB_DC_RECLAIMS + 1) * 4, h->stream));
+  if (m.replay || m.events) {  // event mode without adm_wl: the rows of the snapshot have no record (-1)
+    if (m.replay) CUDA_TRY(h, h2d(h, X.adm.wl, s->adm_wl, n_adm * 4));
+    else CUDA_TRY(h, cudaMemsetAsync(X.adm.wl, 0xff, n_adm * 4, h->stream));
     X.wl_has_qr = const_cast<uint8_t *>(D.wl_has_qr);
   }
-  if (compact) {
-    CUDA_TRY(h, cudaMemsetAsync(X.adm_dead, 0, Acap * 4, h->stream));
-    CUDA_TRY(h, cudaMemsetAsync(X.root_mark, 0, nR * 4, h->stream));
+  if (m.compact) {
+    CUDA_TRY(h, cudaMemsetAsync(X.adm_dead, 0, r.Acap * 4, h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(X.root_mark, 0, r.nR * 4, h->stream));
   }
-  std::vector<i64> never;  // event mode without adm_finish_ns: the rows of the snapshot never finish
-  std::vector<uint8_t> evicting;  // latency with adm_evict_end_ns: the rows whose eviction is under way
-  if (events) {
-    const void *finish = s->adm_finish_ns;
-    if (!finish) { never.assign((size_t)s->n_adm, INT64_MAX); finish = never.data(); }
-    if (lat && s->adm_evict_end_ns) {  // their end time replaces their finish time (an evicted workload never finishes)
-      std::vector<i64> fin((size_t)s->n_adm);
-      memcpy(fin.data(), finish, (size_t)s->n_adm * 8);
-      evicting.assign((size_t)s->n_adm, 0);
-      for (int a = 0; a < s->n_adm; a++)
-        if (s->adm_evicted[a]) { fin[a] = s->adm_evict_end_ns[a]; evicting[a] = 1; }
-      never.swap(fin);
-      finish = never.data();
+  if (m.events) {  // drain_row_start's columns
+    if (r.rows.phased) CUDA_TRY(h, h2d(h, X.adm.phase, r.rows.phase.data(), n_adm));
+    else if (m.requeue || m.mx) CUDA_TRY(h, cudaMemsetAsync(X.adm.phase, KB_PH_RUN, n_adm, h->stream));
+    CUDA_TRY(h, h2d(h, X.adm.finish, r.rows.finish.data(), n_adm * 8));
+    if (s->wl_run_ns) CUDA_TRY(h, h2d(h, X.wl_run, s->wl_run_ns, Wz * 8));
+    if (r.create) { CUDA_TRY(h, h2d(h, r.create, s->wl_create_ns, Wz * 8)); X.n_arr = W; }
+    if (r.cls.n) {
+      CUDA_TRY(h, h2d(h, X.wl_class, r.cls.wl_class.data(), Wz * 4));
+      CUDA_TRY(h, h2d(h, X.cq_class_start, r.cls.cq_class_start.data(), ((size_t)Q + 1) * 4));
+      CUDA_TRY(h, cudaMemsetAsync(X.class_nofit, 0, (size_t)r.cls.n, h->stream));
     }
-    if ((checks && s->adm_check_end_ns) || (pr && s->adm_admitted_ns) || (mx && s->n_adm > 0)) {  // rows whose checks run:
-      // the verdict time in the finish column; rows whose pods are not ready: their attempt from Admitted
-      // (drain_pr_attempt; no failure is used until a timeout is applied), T in the finish column of a failing one; rows
-      // with an Admitted time and a limit, not evicting: the effective deadline max(D, A, now_ns) where it comes first
-      std::vector<i64> fin((size_t)s->n_adm);
-      std::vector<uint8_t> ph((size_t)s->n_adm, KB_PH_RUN);
-      memcpy(fin.data(), finish, (size_t)s->n_adm * 8);
-      for (int a = 0; a < s->n_adm; a++) {
-        if (checks && s->adm_check_end_ns && s->adm_check_end_ns[a] != INT64_MIN) { fin[a] = s->adm_check_end_ns[a]; ph[a] = KB_PH_CHECK; }
-        const int w = replay ? s->adm_wl[a] : -1;
-        if (pr && s->adm_admitted_ns && s->adm_admitted_ns[a] != INT64_MIN) {
-          const i64 t0 = s->adm_admitted_ns[a], d = s->wl_pods_ready_ns[w], to = s->pods_ready_timeout_ns;
-          const i64 run = s->wl_run_ns ? s->wl_run_ns[w] : -1;
-          if ((s->wl_pods_ready_fail && s->wl_pods_ready_fail[w] > 0) || d > to) { fin[a] = t0 > INT64_MAX - to ? INT64_MAX : t0 + to; ph[a] = KB_PH_WAIT; }
-          else { const i64 at = t0 > INT64_MAX - d ? INT64_MAX : t0 + d; fin[a] = run < 0 ? INT64_MAX : (at > INT64_MAX - run ? INT64_MAX : at + run); }
-        }
-        if (!mx || s->adm_exec_since_ns[a] == INT64_MIN || s->wl_max_exec_s[w] <= 0 || (!evicting.empty() && evicting[a])) continue;
-        const i64 A = s->adm_exec_since_ns[a];
-        const i64 dl = std::max({kb_exec_deadline(A, s->wl_max_exec_s[w], s->wl_exec_acc_s ? s->wl_exec_acc_s[w] : -1), A, (i64)s->now_ns});
-        if (dl < fin[a]) { fin[a] = dl; ph[a] = KB_PH_EXPIRE; }
-      }
-      never.swap(fin);
-      finish = never.data();
-      CUDA_TRY(h, h2d(h, X.adm_phase, ph.data(), ph.size()));
-      CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // ph is a local
-    } else if (requeue || mx) {
-      CUDA_TRY(h, cudaMemsetAsync(X.adm_phase, KB_PH_RUN, (size_t)s->n_adm, h->stream));
-    }
-    CUDA_TRY(h, h2d(h, X.adm_finish, finish, (size_t)s->n_adm * 8));
-    if (s->wl_run_ns) { CUDA_TRY(h, h2d(h, run, s->wl_run_ns, Wz * 8)); X.wl_run = run; }
-    if (create) { CUDA_TRY(h, h2d(h, create, s->wl_create_ns, Wz * 8)); X.n_arr = W; }
-    if (n_class) {
-      CUDA_TRY(h, h2d(h, d_wl_class, wl_class.data(), Wz * 4));
-      CUDA_TRY(h, h2d(h, d_cq_class_start, cq_class_start.data(), ((size_t)Q + 1) * 4));
-      CUDA_TRY(h, cudaMemsetAsync(X.class_nofit, 0, (size_t)n_class, h->stream));
-      X.wl_class = d_wl_class; X.cq_class_start = d_cq_class_start;
-    }
-    if (lat) {
-      CUDA_TRY(h, h2d(h, evict_ns, s->wl_evict_ns, Wz * 8));
-      X.wl_evict = evict_ns;
-      if (!evicting.empty()) CUDA_TRY(h, h2d(h, X.adm_evicting, evicting.data(), evicting.size()));
-      else CUDA_TRY(h, cudaMemsetAsync(X.adm_evicting, 0, (size_t)s->n_adm, h->stream));
+    if (m.lat) {
+      CUDA_TRY(h, h2d(h, X.wl_evict, s->wl_evict_ns, Wz * 8));
+      if (!r.rows.evicting.empty()) CUDA_TRY(h, h2d(h, X.adm.evicting, r.rows.evicting.data(), n_adm));
+      else CUDA_TRY(h, cudaMemsetAsync(X.adm.evicting, 0, n_adm, h->stream));
     }
   }
-  if (afs) {
-    CUDA_TRY(h, h2d(h, X.seg_start, seg_start.data(), seg_start.size() * 4));
-    CUDA_TRY(h, h2d(h, X.lq_seg, lq_seg.data(), lq_seg.size() * 4));
-    CUDA_TRY(h, h2d(h, X.seg_lq, seg_lq.data(), seg_lq.size() * 4));
-    CUDA_TRY(h, h2d(h, X.afs_cqs, afs_cqs.data(), afs_cqs.size() * 4));
+  if (m.afs) {
+    CUDA_TRY(h, h2d(h, X.seg_start, r.afs.seg_start.data(), r.afs.seg_start.size() * 4));
+    CUDA_TRY(h, h2d(h, X.lq_seg, r.afs.lq_seg.data(), r.afs.lq_seg.size() * 4));
+    CUDA_TRY(h, h2d(h, X.seg_lq, r.afs.seg_lq.data(), r.afs.seg_lq.size() * 4));
+    CUDA_TRY(h, h2d(h, X.afs_cqs, r.afs.afs_cqs.data(), r.afs.afs_cqs.size() * 4));
     CUDA_TRY(h, h2d(h, X.wl_lq, s->wl_lq, Wz * 4));
     CUDA_TRY(h, h2d(h, X.cq_afs, s->cq_afs, (size_t)Q));
     CUDA_TRY(h, h2d(h, X.lq_weight, s->lq_weight, (size_t)L * 8));
@@ -1957,519 +2133,411 @@ static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out)
     CUDA_TRY(h, h2d(h, X.lq_consumed_scale, s->lq_consumed_scale, (size_t)L * R * 4));
     if (s->lq_penalty) CUDA_TRY(h, h2d(h, X.lq_penalty, s->lq_penalty, (size_t)L * R * 8));
     else CUDA_TRY(h, cudaMemsetAsync(X.lq_penalty, 0, LR * 8, h->stream));
-    CUDA_TRY(h, h2d(h, X.lq_usage, lq_usage.data(), Lz * 8));
+    CUDA_TRY(h, h2d(h, X.lq_usage, r.afs.lq_usage.data(), (size_t)std::max(1, L) * 8));
     CUDA_TRY(h, h2d(h, X.res_weight, s->afs_res_weight, (size_t)R * 8));
     CUDA_TRY(h, h2d(h, X.milli_mul, s->afs_milli_mul, (size_t)R * 8));
     X.alpha = s->afs_alpha;
-    X.n_afs_cq = (int)afs_cqs.size();
+    X.n_afs_cq = (int)r.afs.afs_cqs.size();
   }
-  if (sticky) CUDA_TRY(h, h2d(h, X.cq_sticky, s->cq_sticky, (size_t)Q * 4));
-  std::vector<i64> qts, requeue_at, pr_at, pr_none;  // checks / PodsReady: queue-order timestamps, RequeueAt, PodsReady at the start
-  std::vector<int32_t> fails, retries, pr_fails, pr_counts;
-  if (requeue) {
-    std::vector<uint8_t> held(Wz, 0);
-    for (int a = 0; a < s->n_adm; a++) held[s->adm_wl[a]] = 1;
-    qts.assign(s->wl_ts, s->wl_ts + W);
+  if (m.sticky) CUDA_TRY(h, h2d(h, X.cq_sticky, s->cq_sticky, (size_t)Q * 4));
+  if (m.requeue) {  // checks / PodsReady: queue-order timestamps (the Evicted time of a record requeued by a check or a
+                    // PodsReady timeout), RequeueAt
+    r.qts.assign(s->wl_ts, s->wl_ts + W);
     if (s->wl_check_evict_ns)
-      for (int w = 0; w < W; w++) if (s->wl_check_evict_ns[w] != INT64_MIN && !held[w]) qts[w] = s->wl_check_evict_ns[w];
-    if (pr && s->wl_pods_ready_evict_ns && !s->pods_ready_requeue_creation)  // the Eviction timestamp of a timed-out record
-      for (int w = 0; w < W; w++) if (s->wl_pods_ready_evict_ns[w] != INT64_MIN) qts[w] = s->wl_pods_ready_evict_ns[w];
-    requeue_at.assign(Wz, INT64_MIN);
-    if (s->wl_requeue_at_ns) requeue_at.assign(s->wl_requeue_at_ns, s->wl_requeue_at_ns + W);
+      for (int w = 0; w < W; w++) if (s->wl_check_evict_ns[w] != INT64_MIN && !r.held[w]) r.qts[w] = s->wl_check_evict_ns[w];
+    if (m.pr && s->wl_pods_ready_evict_ns && !s->pods_ready_requeue_creation)
+      for (int w = 0; w < W; w++) if (s->wl_pods_ready_evict_ns[w] != INT64_MIN) r.qts[w] = s->wl_pods_ready_evict_ns[w];
+    r.requeue_at = drain_table_or<i64>(s->wl_requeue_at_ns, Wz, INT64_MIN);
     X.wl_qts = const_cast<i64 *>(D.wl_ts);
     CUDA_TRY(h, h2d(h, X.wl_ts0, s->wl_ts, Wz * 8));
-    CUDA_TRY(h, h2d(h, X.wl_qts, qts.data(), Wz * 8));       // the cycle kernels read the queue-order timestamp
-    CUDA_TRY(h, h2d(h, X.wl_sort_ts, qts.data(), Wz * 8));
-    CUDA_TRY(h, h2d(h, X.wl_requeue_at, requeue_at.data(), Wz * 8));
+    CUDA_TRY(h, h2d(h, X.wl_qts, r.qts.data(), Wz * 8));  // the cycle kernels read the queue-order timestamp
+    CUDA_TRY(h, h2d(h, X.wl_sort_ts, r.qts.data(), Wz * 8));
+    CUDA_TRY(h, h2d(h, X.wl_requeue_at, r.requeue_at.data(), Wz * 8));
   }
-  if (checks) {
-    fails.assign(Wz, 0); retries.assign(Wz, 0);
-    if (s->wl_check_fail) fails.assign(s->wl_check_fail, s->wl_check_fail + W);
-    if (s->wl_check_retries) retries.assign(s->wl_check_retries, s->wl_check_retries + W);
-    X.wl_check = check_ns;
-    CUDA_TRY(h, h2d(h, check_ns, s->wl_check_ns, Wz * 8));
-    CUDA_TRY(h, h2d(h, X.wl_fail, fails.data(), Wz * 4));
-    CUDA_TRY(h, h2d(h, X.wl_retries, retries.data(), Wz * 4));
+  if (m.checks) {
+    r.fails = drain_table_or<int32_t>(s->wl_check_fail, Wz, 0);
+    r.retries = drain_table_or<int32_t>(s->wl_check_retries, Wz, 0);
+    CUDA_TRY(h, h2d(h, X.wl_check, s->wl_check_ns, Wz * 8));
+    CUDA_TRY(h, h2d(h, X.wl_fail, r.fails.data(), Wz * 4));
+    CUDA_TRY(h, h2d(h, X.wl_retries, r.retries.data(), Wz * 4));
     X.check_base_s = s->check_backoff_base_s; X.check_max_s = s->check_backoff_max_s; X.check_limit = s->check_backoff_limit;
   }
-  if (pr) {
-    pr_fails.assign(Wz, 0); pr_counts.assign(Wz, 0); pr_at.assign(Wz, INT64_MIN); pr_none.assign(Wz, INT64_MIN);
-    if (s->wl_pods_ready_fail) pr_fails.assign(s->wl_pods_ready_fail, s->wl_pods_ready_fail + W);
-    if (s->wl_pods_ready_count) pr_counts.assign(s->wl_pods_ready_count, s->wl_pods_ready_count + W);
-    if (s->adm_admitted_ns)  // a ready attempt under way reaches PodsReady at Admitted + delay
-      for (int a = 0; a < s->n_adm; a++) {
-        const int w = s->adm_wl[a];
-        const i64 t0 = s->adm_admitted_ns[a], d = s->wl_pods_ready_ns[w];
-        if (t0 != INT64_MIN && pr_fails[w] == 0 && d <= s->pods_ready_timeout_ns) pr_at[w] = t0 > INT64_MAX - d ? INT64_MAX : t0 + d;
-      }
-    X.wl_pr = pr_ns;
-    CUDA_TRY(h, h2d(h, pr_ns, s->wl_pods_ready_ns, Wz * 8));
-    CUDA_TRY(h, h2d(h, X.wl_pr_fail, pr_fails.data(), Wz * 4));
-    CUDA_TRY(h, h2d(h, X.wl_pr_count, pr_counts.data(), Wz * 4));
-    CUDA_TRY(h, h2d(h, X.wl_pr_at, pr_at.data(), Wz * 8));
-    CUDA_TRY(h, h2d(h, X.wl_pr_prev, pr_none.data(), Wz * 8));  // no PodsReady before the attempts under way
+  if (m.pr) {
+    r.pr_fails = drain_table_or<int32_t>(s->wl_pods_ready_fail, Wz, 0);
+    r.pr_counts = drain_table_or<int32_t>(s->wl_pods_ready_count, Wz, 0);
+    r.pr_none.assign(Wz, INT64_MIN);
+    CUDA_TRY(h, h2d(h, X.wl_pr, s->wl_pods_ready_ns, Wz * 8));
+    CUDA_TRY(h, h2d(h, X.wl_pr_fail, r.pr_fails.data(), Wz * 4));
+    CUDA_TRY(h, h2d(h, X.wl_pr_count, r.pr_counts.data(), Wz * 4));
+    CUDA_TRY(h, h2d(h, X.wl_pr_at, r.rows.pr_at.data(), Wz * 8));  // a ready attempt under way reaches PodsReady at Admitted + delay
+    CUDA_TRY(h, h2d(h, X.wl_pr_prev, r.pr_none.data(), Wz * 8));   // no PodsReady before the attempts under way
     X.pr_timeout = s->pods_ready_timeout_ns; X.pr_base_s = s->pods_ready_backoff_base_s; X.pr_max_s = s->pods_ready_backoff_max_s;
     X.pr_limit = s->pods_ready_backoff_limit; X.pr_creation = s->pods_ready_requeue_creation;
   }
-  std::vector<int32_t> exec_acc;  // MaximumExecutionTimeSeconds: the accumulated times at the start
-  if (mx) {
-    exec_acc.assign(Wz, -1);
-    if (s->wl_exec_acc_s) exec_acc.assign(s->wl_exec_acc_s, s->wl_exec_acc_s + W);
-    X.wl_max_exec = max_exec;
-    CUDA_TRY(h, h2d(h, max_exec, s->wl_max_exec_s, Wz * 4));
-    CUDA_TRY(h, h2d(h, X.wl_exec_acc, exec_acc.data(), Wz * 4));
-    if (s->n_adm) CUDA_TRY(h, h2d(h, X.adm_exec_since, s->adm_exec_since_ns, (size_t)s->n_adm * 8));
-    if (!requeue) CUDA_TRY(h, cudaMemsetAsync(X.wl_deactivated, 0, Wz, h->stream));  // (k_drain_init_checks clears it otherwise)
+  if (m.mx) {  // the limits, the accumulated times at the start, the Admitted times of the snapshot's rows
+    r.exec_acc = drain_table_or<int32_t>(s->wl_exec_acc_s, Wz, -1);
+    CUDA_TRY(h, h2d(h, X.wl_max_exec, s->wl_max_exec_s, Wz * 4));
+    CUDA_TRY(h, h2d(h, X.wl_exec_acc, r.exec_acc.data(), Wz * 4));
+    if (n_adm) CUDA_TRY(h, h2d(h, X.adm.since, s->adm_exec_since_ns, n_adm * 8));
   }
-  if (blk) {  // deactivation / reactivation: the start state, the edits
-    if (!requeue && !mx) CUDA_TRY(h, cudaMemsetAsync(X.wl_deactivated, 0, Wz, h->stream));
-    if (inactive_d) CUDA_TRY(h, h2d(h, inactive_d, s->wl_inactive, Wz));
-    if (act) {
-      CUDA_TRY(h, h2d(h, ac_ns_d, s->ac_ns, (size_t)NAC * 8));
-      CUDA_TRY(h, h2d(h, ac_wl_d, s->ac_wl, (size_t)NAC * 4));
-      CUDA_TRY(h, h2d(h, ac_on_d, s->ac_active, (size_t)NAC));
-      CUDA_TRY(h, h2d(h, ac_next_d, ac_next.data(), (size_t)NAC * 4));
-      CUDA_TRY(h, h2d(h, ac_prev_d, ac_prev.data(), (size_t)NAC * 4));
-      CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_STOPPED, 0, 4 * 4, h->stream));  // once: the boundaries never clear them
-      X.ac_ns = ac_ns_d; X.ac_wl = ac_wl_d; X.ac_on = ac_on_d; X.ac_next = ac_next_d; X.ac_prev = ac_prev_d; X.n_ac = NAC;
-    }
+  if ((m.mx || m.blk) && !m.requeue) CUDA_TRY(h, cudaMemsetAsync(X.wl_deactivated, 0, Wz, h->stream));  // (k_drain_init_checks clears it otherwise)
+  if (r.inactive) CUDA_TRY(h, h2d(h, r.inactive, s->wl_inactive, Wz));
+  if (m.act) {
+    const size_t NAC = (size_t)m.n_ac;
+    CUDA_TRY(h, h2d(h, X.ac_ns, s->ac_ns, NAC * 8));
+    CUDA_TRY(h, h2d(h, X.ac_wl, s->ac_wl, NAC * 4));
+    CUDA_TRY(h, h2d(h, X.ac_on, s->ac_active, NAC));
+    CUDA_TRY(h, h2d(h, X.ac_next, r.ac_next.data(), NAC * 4));
+    CUDA_TRY(h, h2d(h, X.ac_prev, r.ac_prev.data(), NAC * 4));
+    X.n_ac = m.n_ac;
   }
-  std::vector<i64> lq_adm;  // decay: the initial admitted usage of every LocalQueue (live rows of the snapshot)
-  if (decay) {
-    lq_adm.assign(LR, 0);
-    for (int a = 0; a < s->n_adm; a++)
-      if (s->adm_lq[a] >= 0)
-        for (int c = s->adm_use_start[a]; c < s->adm_use_start[a + 1]; c++) lq_adm[(size_t)s->adm_lq[a] * R + s->adm_use_fr[c] % R] += s->adm_use_qty[c];
+  if (m.decay) {
     CUDA_TRY(h, h2d(h, X.lq_last, s->lq_last_update_ns, (size_t)L * 8));
-    CUDA_TRY(h, h2d(h, X.lq_adm, lq_adm.data(), LR * 8));
-    CUDA_TRY(h, h2d(h, X.adm_lq, s->adm_lq, (size_t)s->n_adm * 4));
+    CUDA_TRY(h, h2d(h, X.lq_adm, r.afs.lq_adm.data(), LR * 8));
+    CUDA_TRY(h, h2d(h, X.adm.lq, s->adm_lq, n_adm * 4));
     CUDA_TRY(h, cudaMemsetAsync(X.afs_samples, 0, 8, h->stream));
     X.half_life_ns = s->afs_half_life_ns; X.sampling_ns = s->afs_sampling_ns;
   }
-  auto blob_gen = [&]() {  // byte offset of every ClusterQueue's generation in the static tree blocks, -1 = not in a tree
-    std::vector<int32_t> off((size_t)std::max(1, Q), -1);
-    for (int q = 0; q < Q; q++) {
-      const int slot = h->root_slot[q];
-      if (slot < D.nLone) continue;
-      const int tr = slot - D.nLone, b0 = h->tree_blob_off[tr];
-      const TreeBlobHdr *BH = (const TreeBlobHdr *)(h->tree_blob.data() + b0);
-      off[q] = b0 + BH->gen + 8 * h->local_idx[q];
-    }
-    return off;
-  };
-  if (quota) {  // quota_prep: no-op edits, roots and trees of the others; the ClusterQueues of every root; the blob offsets
-    std::vector<i64> nom(s->nominal, s->nominal + (size_t)QN * FR), bl(s->borrow_limit, s->borrow_limit + (size_t)QN * FR),
-        ll(s->lend_limit, s->lend_limit + (size_t)QN * FR);  // the rows each edit meets
-    qc_root.assign((size_t)NQC, -1); qc_tree.assign((size_t)NQC, -1);
-    for (int i = 0; i < NQC; i++) {
-      const int n = s->qc_node[i];
-      const size_t o = (size_t)n * FR, k = (size_t)i * FR, b = (size_t)FR * 8;
-      if (!memcmp(&nom[o], s->qc_nominal + k, b) && !memcmp(&bl[o], s->qc_borrow_limit + k, b) && !memcmp(&ll[o], s->qc_lend_limit + k, b)) continue;
-      memcpy(&nom[o], s->qc_nominal + k, b); memcpy(&bl[o], s->qc_borrow_limit + k, b); memcpy(&ll[o], s->qc_lend_limit + k, b);
-      qc_root[i] = h->root_slot[n];
-      if (D.tl_subtree && h->root_slot[n] >= D.nLone) qc_tree[i] = h->root_slot[n] - D.nLone;  // lone ClusterQueues come first
-    }
-    qc_tree_next.assign((size_t)NQC, NQC);
-    {
-      std::vector<int32_t> later((size_t)std::max(1, D.nTrees), NQC);
-      for (int i = NQC - 1; i >= 0; i--)
-        if (qc_tree[i] >= 0) { qc_tree_next[i] = later[qc_tree[i]]; later[qc_tree[i]] = i; }
-    }
-    qc_cq_start.assign(h->root_cq_start.begin(), h->root_cq_start.end());
-    qc_cq.assign((size_t)std::max(1, Q), 0);
-    std::vector<int32_t> fill(qc_cq_start.begin(), qc_cq_start.end() - 1);
-    for (int q = 0; q < Q; q++) qc_cq[fill[h->root_slot[q]]++] = q;
-    qc_blob_gen = blob_gen();
-    CUDA_TRY(h, h2d(h, qc_ns_d, s->qc_ns, (size_t)NQC * 8));
-    CUDA_TRY(h, h2d(h, qc_node_d, s->qc_node, (size_t)NQC * 4));
-    CUDA_TRY(h, h2d(h, qc_rows_d[0], s->qc_nominal, (size_t)NQC * FR * 8));
-    CUDA_TRY(h, h2d(h, qc_rows_d[1], s->qc_borrow_limit, (size_t)NQC * FR * 8));
-    CUDA_TRY(h, h2d(h, qc_rows_d[2], s->qc_lend_limit, (size_t)NQC * FR * 8));
-    CUDA_TRY(h, h2d(h, qc_root_d, qc_root.data(), (size_t)NQC * 4));
-    CUDA_TRY(h, h2d(h, qc_tree_d, qc_tree.data(), (size_t)NQC * 4));
-    CUDA_TRY(h, h2d(h, qc_tree_next_d, qc_tree_next.data(), (size_t)NQC * 4));
-    CUDA_TRY(h, h2d(h, qc_cq_start_d, qc_cq_start.data(), qc_cq_start.size() * 4));
-    CUDA_TRY(h, h2d(h, qc_cq_d, qc_cq.data(), qc_cq.size() * 4));
-    CUDA_TRY(h, h2d(h, qc_blob_gen_d, qc_blob_gen.data(), qc_blob_gen.size() * 4));
-    CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_QC_LO, 0, 2 * 4, h->stream));  // once: the boundaries never clear them
-    X.qc_ns = qc_ns_d; X.qc_node = qc_node_d; X.qc_nominal = qc_rows_d[0]; X.qc_blimit = qc_rows_d[1]; X.qc_llimit = qc_rows_d[2];
-    X.qc_root = qc_root_d; X.qc_tree = qc_tree_d; X.qc_tree_next = qc_tree_next_d; X.qc_cq_start = qc_cq_start_d; X.qc_cq = qc_cq_d; X.qc_blob_gen = qc_blob_gen_d;
-    X.n_qc = NQC;
+  if (m.quota) {
+    const size_t NQC = (size_t)m.n_qc, FRz = (size_t)r.FR;
+    CUDA_TRY(h, h2d(h, X.qc_ns, s->qc_ns, NQC * 8));
+    CUDA_TRY(h, h2d(h, X.qc_node, s->qc_node, NQC * 4));
+    CUDA_TRY(h, h2d(h, X.qc_nominal, s->qc_nominal, NQC * FRz * 8));
+    CUDA_TRY(h, h2d(h, X.qc_blimit, s->qc_borrow_limit, NQC * FRz * 8));
+    CUDA_TRY(h, h2d(h, X.qc_llimit, s->qc_lend_limit, NQC * FRz * 8));
+    CUDA_TRY(h, h2d(h, X.qc_root, r.qc.root.data(), NQC * 4));
+    CUDA_TRY(h, h2d(h, X.qc_tree, r.qc.tree.data(), NQC * 4));
+    CUDA_TRY(h, h2d(h, X.qc_tree_next, r.qc.tree_next.data(), NQC * 4));
+    CUDA_TRY(h, h2d(h, X.qc_cq_start, r.qc.cq_start.data(), r.qc.cq_start.size() * 4));
+    CUDA_TRY(h, h2d(h, X.qc_cq, r.qc.cq.data(), r.qc.cq.size() * 4));
+    CUDA_TRY(h, h2d(h, X.qc_blob_gen, r.qc.blob_gen.data(), r.qc.blob_gen.size() * 4));
+    X.n_qc = m.n_qc;
   }
-  std::vector<i64> rc_next;  // reclaim steps: the snapshot's running rows with steps start at their run start
-  std::vector<int32_t> rc_cur, rc_blob_gen;
-  std::vector<int8_t> adm_fl;
-  std::vector<int32_t> adm_cnt;
-  std::vector<i64> adm_use;
-  if (rcl) {
-    rc_next.assign((size_t)std::max(1, s->n_adm), INT64_MAX); rc_cur.assign((size_t)std::max(1, s->n_adm), 0);
-    adm_fl.assign(Pz * R, -1); adm_cnt.assign(Pz, 0); adm_use.assign(Pz * R, 0);
-    for (int a = 0; a < s->n_adm; a++) {
-      const int w = s->adm_wl[a], i = s->wl_rc_start[w];
-      if (i == s->wl_rc_start[w + 1]) continue;
-      const size_t p0 = s->wl_ps_start[w], p1 = s->wl_ps_start[w + 1];
-      memcpy(&adm_fl[p0 * R], s->ps_adm_flavor + p0 * R, (p1 - p0) * R);
-      memcpy(&adm_cnt[p0], s->ps_adm_count + p0, (p1 - p0) * 4);
-      memcpy(&adm_use[p0 * R], s->ps_adm_usage + p0 * R, (p1 - p0) * R * 8);
-      i64 S = s->adm_run_start_ns ? s->adm_run_start_ns[a] : INT64_MIN;
-      if (S == INT64_MIN && pr && s->adm_admitted_ns && s->adm_admitted_ns[a] != INT64_MIN) S = pr_at[w];  // a ready attempt under way
-      if (S == INT64_MIN) continue;
-      rc_cur[a] = i;
-      rc_next[a] = S > INT64_MAX - s->rc_after_ns[i] ? INT64_MAX : S + s->rc_after_ns[i];
-    }
-    rc_blob_gen = blob_gen();
-    CUDA_TRY(h, h2d(h, rc_start_d, s->wl_rc_start, (Wz + 1) * 4));
+  if (m.rcl) {
+    const size_t NRC = (size_t)m.n_rc;
+    CUDA_TRY(h, h2d(h, X.wl_rc_start, s->wl_rc_start, (Wz + 1) * 4));
     if (NRC) {
-      CUDA_TRY(h, h2d(h, rc_after_d, s->rc_after_ns, (size_t)NRC * 8));
-      CUDA_TRY(h, h2d(h, rc_ps_d, s->rc_ps, (size_t)NRC * 4));
-      CUDA_TRY(h, h2d(h, rc_rem_d, s->rc_remaining, (size_t)NRC * 4));
-      if (rc_hash_d) CUDA_TRY(h, h2d(h, rc_hash_d, s->rc_sched_hash, (size_t)NRC * 8));
-      if (rc_class_d) CUDA_TRY(h, h2d(h, rc_class_d, rc_class.data(), (size_t)NRC * 4));
+      CUDA_TRY(h, h2d(h, X.rc_after, s->rc_after_ns, NRC * 8));
+      CUDA_TRY(h, h2d(h, X.rc_ps, s->rc_ps, NRC * 4));
+      CUDA_TRY(h, h2d(h, X.rc_remaining, s->rc_remaining, NRC * 4));
+      if (X.rc_hash) CUDA_TRY(h, h2d(h, X.rc_hash, s->rc_sched_hash, NRC * 8));
+      if (X.rc_class) CUDA_TRY(h, h2d(h, X.rc_class, r.cls.rc_class.data(), NRC * 4));
     }
-    CUDA_TRY(h, h2d(h, X.ps_adm_fl, adm_fl.data(), adm_fl.size()));
-    CUDA_TRY(h, h2d(h, X.ps_adm_cnt, adm_cnt.data(), adm_cnt.size() * 4));
-    CUDA_TRY(h, h2d(h, X.ps_adm_use, adm_use.data(), adm_use.size() * 8));
-    if (s->n_adm) {
-      CUDA_TRY(h, h2d(h, X.adm_rc_next, rc_next.data(), (size_t)s->n_adm * 8));
-      CUDA_TRY(h, h2d(h, X.adm_rc_cur, rc_cur.data(), (size_t)s->n_adm * 4));
+    CUDA_TRY(h, h2d(h, X.ps_adm_fl, r.rc.fl.data(), r.rc.fl.size()));
+    CUDA_TRY(h, h2d(h, X.ps_adm_cnt, r.rc.cnt.data(), r.rc.cnt.size() * 4));
+    CUDA_TRY(h, h2d(h, X.ps_adm_use, r.rc.use.data(), r.rc.use.size() * 8));
+    if (n_adm) {
+      CUDA_TRY(h, h2d(h, X.adm.rc_next, r.rc.next.data(), n_adm * 8));
+      CUDA_TRY(h, h2d(h, X.adm.rc_cur, r.rc.cur.data(), n_adm * 4));
     }
-    CUDA_TRY(h, h2d(h, rc_blob_gen_d, rc_blob_gen.data(), rc_blob_gen.size() * 4));
-    CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_RECLAIMS, 0, 4, h->stream));  // once: the boundaries never clear it
-    X.wl_rc_start = rc_start_d; X.rc_after = rc_after_d; X.rc_ps = rc_ps_d; X.rc_remaining = rc_rem_d; X.rc_hash = rc_hash_d;
-    X.rc_class = rc_class_d; X.rc_blob_gen = rc_blob_gen_d;
+    CUDA_TRY(h, h2d(h, X.rc_blob_gen, r.rc_blob_gen.data(), r.rc_blob_gen.size() * 4));
   }
-  // ---- per-ClusterQueue order (queueOrderingFunc): stable LSD passes uid -> timestamp -> (ClusterQueue | priority desc)
-  const int tb = 256, nbW = (W + tb - 1) / tb, nbQ = (Q + tb - 1) / tb;
-  auto sort_queues = [&]() -> cudaError_t {  // also the re-sort of admission checks (same segments, same q_start)
-    cudaError_t e = cudaMemsetAsync(q_count, 0, sizeof(int32_t) * (Sz + 2), h->stream);
-    if (e != cudaSuccess) return e;
-    cub::DoubleBuffer<u64> dk(keys[0], keys[1]); cub::DoubleBuffer<int32_t> dv(vals[0], vals[1]);
-    size_t bytes = sort_bytes;
-    k_drain_keys_uid<<<nbW, tb, 0, h->stream>>>(D, dk.Current(), dv.Current());
-    if ((e = cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 64, h->stream)) != cudaSuccess) return e;
-    k_drain_keys_ts<<<nbW, tb, 0, h->stream>>>(D, dv.Current(), dk.Current());
-    if ((e = cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 64, h->stream)) != cudaSuccess) return e;
-    k_drain_keys_cq<<<nbW, tb, 0, h->stream>>>(D, X, dv.Current(), dk.Current(), q_count);
-    int cq_bits = 1; while ((1ll << cq_bits) < (long long)S) cq_bits++;
-    if ((e = cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 32 + cq_bits, h->stream)) != cudaSuccess) return e;
-    X.q_order = dv.Current();
-    return cudaSuccess;
-  };
-  CUDA_TRY(h, sort_queues());
-  if (create) {  // arrival order: (creation time, index); the workloads present at the start are its first k_drain_init_events prefix
-    cub::DoubleBuffer<u64> dk(arr_keys[0], arr_keys[1]); cub::DoubleBuffer<int32_t> dv(arr_vals[0], arr_vals[1]);
-    size_t bytes = sort_bytes;
-    k_drain_keys_create<<<nbW, tb, 0, h->stream>>>(W, create, dk.Current(), dv.Current());
-    CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(sort_tmp, bytes, dk, dv, W, 0, 64, h->stream));
+  return KB_OK;
+}
+
+// per-segment queue order (queueOrderingFunc): stable LSD passes uid -> timestamp -> (segment | priority desc); also
+// the re-sort of admission checks and PodsReady (same segments, same q_start)
+static cudaError_t drain_sort_queues(DrainRun &r) {
+  kb_handle *h = r.h; const DevSnap &D = h->D; DrainDev &X = r.X;
+  cudaError_t e = cudaMemsetAsync(r.q_count, 0, sizeof(int32_t) * ((size_t)r.S + 2), h->stream);
+  if (e != cudaSuccess) return e;
+  cub::DoubleBuffer<u64> dk(r.keys[0], r.keys[1]); cub::DoubleBuffer<int32_t> dv(r.vals[0], r.vals[1]);
+  size_t bytes = r.sort_bytes;
+  k_drain_keys_uid<<<drain_blocks(r.W), DRAIN_TB, 0, h->stream>>>(D, dk.Current(), dv.Current());
+  if ((e = cub::DeviceRadixSort::SortPairs(r.sort_tmp, bytes, dk, dv, r.W, 0, 64, h->stream)) != cudaSuccess) return e;
+  k_drain_keys_ts<<<drain_blocks(r.W), DRAIN_TB, 0, h->stream>>>(D, dv.Current(), dk.Current());
+  if ((e = cub::DeviceRadixSort::SortPairs(r.sort_tmp, bytes, dk, dv, r.W, 0, 64, h->stream)) != cudaSuccess) return e;
+  k_drain_keys_cq<<<drain_blocks(r.W), DRAIN_TB, 0, h->stream>>>(D, X, dv.Current(), dk.Current(), r.q_count);
+  int cq_bits = 1; while ((1ll << cq_bits) < (long long)r.S) cq_bits++;
+  if ((e = cub::DeviceRadixSort::SortPairs(r.sort_tmp, bytes, dk, dv, r.W, 0, 32 + cq_bits, h->stream)) != cudaSuccess) return e;
+  X.q_order = dv.Current();
+  return cudaSuccess;
+}
+// the heads of the next cycle
+static void drain_heads(DrainRun &r) {
+  kb_handle *h = r.h; const DevSnap &D = h->D; const DrainDev &X = r.X;
+  k_drain_flag<<<drain_blocks(r.Q), DRAIN_TB, 0, h->stream>>>(D, X);
+  if (X.n_afs_cq) k_drain_afs_heads<<<(X.n_afs_cq + 7) / 8, DRAIN_TB, 0, h->stream>>>(D, X);
+  k_scan_i32<<<1, 1024, 0, h->stream>>>(X.flag, X.pos, r.Q);
+  k_drain_heads<<<drain_blocks(r.Q), DRAIN_TB, 0, h->stream>>>(D, X, const_cast<int32_t *>(D.heads));
+}
+
+// the start of the drain: the queues, the arrival order, every record's state at now_ns, the first heads; one
+// synchronisation
+static int32_t drain_start(DrainRun &r) {
+  kb_handle *h = r.h; const kb_snapshot *s = r.s; const DrainMode &m = r.m;
+  DevSnap &D = h->D; DrainDev &X = r.X;
+  DrainWords &hw = *reinterpret_cast<DrainWords *>(&h->host_words[64]);
+  const int W = r.W, S = r.S, tb = DRAIN_TB;
+  CUDA_TRY(h, drain_sort_queues(r));
+  if (r.create) {  // arrival order: (creation time, index); the workloads present at the start are its first k_drain_init_events prefix
+    cub::DoubleBuffer<u64> dk(r.arr_keys[0], r.arr_keys[1]); cub::DoubleBuffer<int32_t> dv(r.arr_vals[0], r.arr_vals[1]);
+    size_t bytes = r.sort_bytes;
+    k_drain_keys_create<<<drain_blocks(r.W), tb, 0, h->stream>>>(W, r.create, dk.Current(), dv.Current());
+    CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(r.sort_tmp, bytes, dk, dv, W, 0, 64, h->stream));
     X.arr_key = dk.Current(); X.arr_order = dv.Current();
   }
-  k_scan_i32<<<1, 1024, 0, h->stream>>>(q_count, X.q_start, S);
-  k_drain_init<<<std::max(nbW, (S + tb - 1) / tb), tb, 0, h->stream>>>(D, X, S);
-  if (events) k_drain_init_events<<<std::max(1, nbW), tb, 0, h->stream>>>(D, X, create, s->now_ns);
-  if (replay || events || sticky) k_drain_init_replay<<<std::max(nbW, (s->n_adm + tb - 1) / tb), tb, 0, h->stream>>>(D, X, replay ? s->n_adm : 0);
+  k_scan_i32<<<1, 1024, 0, h->stream>>>(r.q_count, X.q_start, S);
+  k_drain_init<<<std::max(drain_blocks(r.W), drain_blocks(S)), tb, 0, h->stream>>>(D, X, S);
+  if (m.events) k_drain_init_events<<<std::max(1, drain_blocks(r.W)), tb, 0, h->stream>>>(D, X, r.create, s->now_ns);
+  if (m.replay || m.events || m.sticky) k_drain_init_replay<<<std::max(drain_blocks(r.W), drain_blocks(s->n_adm)), tb, 0, h->stream>>>(D, X, m.replay ? s->n_adm : 0);
   // records in backoff, records inactive at the start, and the first RequeueAt into clock[2] (k_drain_init_events set
   // clock[0] = now_ns)
-  if (requeue) k_drain_init_checks<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W, s->now_ns);
-  if (blk) k_drain_init_active<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W, inactive_d);
-  if (requeue) k_drain_backoff<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W);
-  k_drain_advance<<<(S + tb - 1) / tb, tb, 0, h->stream>>>(X, S);
-  const int nbL = std::max(1, (L + tb - 1) / tb);
-  if (decay) {  // the samples due at or before now_ns (k_drain_init_events set clock[0] = now_ns), before the first heads
+  if (m.requeue) k_drain_init_checks<<<std::max(1, drain_blocks(r.W)), tb, 0, h->stream>>>(X, W, s->now_ns);
+  if (m.blk) k_drain_init_active<<<std::max(1, drain_blocks(r.W)), tb, 0, h->stream>>>(X, W, r.inactive);
+  if (m.requeue) k_drain_backoff<<<std::max(1, drain_blocks(r.W)), tb, 0, h->stream>>>(X, W);
+  k_drain_advance<<<drain_blocks(S), tb, 0, h->stream>>>(X, S);
+  if (m.decay) {  // the samples due at or before now_ns (k_drain_init_events set clock[0] = now_ns), before the first heads
     CUDA_TRY(h, cudaMemsetAsync(D.status, 0, 4, h->stream));
-    k_drain_afs_decay<<<nbL, tb, 0, h->stream>>>(D, X, L);
+    k_drain_afs_decay<<<std::max(1, drain_blocks(r.L)), tb, 0, h->stream>>>(D, X, r.L);
   }
-  int32_t *d_heads = const_cast<int32_t *>(D.heads);
-  auto enqueue_heads = [&]() {
-    k_drain_flag<<<nbQ, tb, 0, h->stream>>>(D, X);
-    if (X.n_afs_cq) k_drain_afs_heads<<<(X.n_afs_cq + 7) / 8, tb, 0, h->stream>>>(D, X);
-    k_scan_i32<<<1, 1024, 0, h->stream>>>(X.flag, X.pos, Q);
-    k_drain_heads<<<nbQ, tb, 0, h->stream>>>(D, X, d_heads);
-  };
-  DrainWords &hw = *reinterpret_cast<DrainWords *>(&h->host_words[64]);
-  CUDA_TRY(h, cudaMemsetAsync(X.counters + 1, 0, 5 * 4, h->stream));
-  enqueue_heads();
+  drain_heads(r);
   CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[0], X.counters, 4, cudaMemcpyDeviceToHost, h->stream));
-  if (decay) CUDA_TRY(h, cudaMemcpyAsync(&hw.status, D.status, 4, cudaMemcpyDeviceToHost, h->stream));
+  if (m.decay) CUDA_TRY(h, cudaMemcpyAsync(&hw.status, D.status, 4, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  if (decay && (hw.status & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: a decayed consumed quantity overflows int64");
-  int n_live = (int)hw.counters[0];
-  int A_cur = s->n_adm, AU_cur = s->n_adm_use;
-  const bool pre = h->preempt_possible;
-  double gpu_ms = 0;
-  float kms[KB_N_KERNELS] = {};  // per-kernel times summed over the cycles (kb_set_profile)
-  i64 t = s->now_ns;  // the clock: the plain drain steps it by one per cycle
-  const i64 step = s->drain_cycle_ns > 0 ? s->drain_cycle_ns : 1;
-  const int nbArr = std::max(1, std::min(nbW, 8 * std::max(1, h->sm_count)));
-  struct EventPair {  // around a re-sort (admission checks, PodsReady); destroyed on every return
-    cudaEvent_t e[2] = {nullptr, nullptr};
-    ~EventPair() { for (cudaEvent_t x : e) if (x) cudaEventDestroy(x); }
-  } resort_ev;
-  cudaEvent_t *ev_r = resort_ev.e;
-  bool resort_timed = false;
-  uint32_t verdicts_seen[3] = {0, 0, 0};  // cumulative Ready / Retry / Rejected counters at the previous boundary
-  uint32_t timeouts_seen[2] = {0, 0};     // cumulative PodsReady timeout / deactivation counters, likewise
-  if (requeue) {
-    CUDA_TRY(h, cudaEventCreate(&ev_r[0]));
-    CUDA_TRY(h, cudaEventCreate(&ev_r[1]));
-    CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_RESORT, 0, (pr ? 6 : 4) * 4, h->stream));  // once: the boundaries never clear them
+  if (m.decay && (hw.status & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: a decayed consumed quantity overflows int64");
+  r.n_live = (int)hw.counters[0];
+  r.A_cur = s->n_adm; r.AU_cur = s->n_adm_use;
+  r.t = s->now_ns;  // the clock: the plain drain steps it by one per cycle
+  r.step = s->drain_cycle_ns > 0 ? s->drain_cycle_ns : 1;
+  if (m.requeue) {
+    CUDA_TRY(h, cudaEventCreate(&r.ev_r[0]));
+    CUDA_TRY(h, cudaEventCreate(&r.ev_r[1]));
   }
-  uint32_t exec_seen = 0;  // cumulative MaximumExecutionTimeExceeded deactivations at the previous boundary
-  uint32_t active_seen[2] = {0, 0};  // cumulative stops / resumes, likewise
-  uint32_t reclaims_seen = 0;        // cumulative reclaim steps, likewise
-  const int nbAc = std::max(1, std::min((NAC + tb - 1) / tb, std::max(1, h->sm_count)));  // grid-stride over a boundary's edits
-  if (mx) CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_EXEC_DEACTIVATED, 0, 2 * 4, h->stream));  // once, likewise
-  // ---- one boundary per iteration, one synchronisation each (kueue_b200/drain.py): cycle c at t (in event mode, a
-  // jump to the next event when there are no heads), its decisions and admissions, the evictions; in event mode E,
-  // t_{c+1}, the decay samples, completions and arrivals; where rows can die (compact) the inadmissible requeue and the
-  // compaction over [0, bound); then the heads of the next cycle.  A plain drain ends at a cycle without heads or one
-  // that neither admits nor evicts (the next cycle would see the same snapshot); an event drain when no event is left.
-  // Capacity: before the compaction the tables hold the live rows plus this cycle's admissions, and every admitted head
-  // is a workload that holds no row, so the rows stay within A_in + min(W, Hcap * max_cycles) and the cells within
-  // AU_in + min(P * R, that bound * FR) (a readmitted victim's old cells left with its old row): what upload_impl
-  // reserved.  An admission past the end is not written and the call fails.
-  for (int cyc = 0, jumps = 0; cyc < max_cycles;) {
-    const bool jump = n_live == 0;
-    if (jump && !events) break;
-    const int32_t *n_new_d = jump ? nullptr : X.e_adm_off + n_live;
-    if (!jump) {
-      D.H = n_live; D.now_ns = t;
-      D.A = pre ? A_cur : 0; D.AU = pre ? AU_cur : 0;  // without preemption policies the cycle never looks at the admitted tables
-      rc = cycle_enqueue(h);
-      if (rc != KB_OK) return rc;
-      X.cycle = cyc;
-    } else {
-      CUDA_TRY(h, cudaEventRecord(h->ev2, h->stream));
-      X.cycle = -2 - jumps;  // stamps of a jump (cycle + 1 < 0) never meet those of a cycle
-    }
-    X.A = A_cur; X.AU = AU_cur; X.trace_off = (long long)out->n_decisions;
-    kmark(h, KB_K_DRAIN);
-    if (compact) CUDA_TRY(h, cudaMemsetAsync(X.counters + 1, 0, 4 * 4, h->stream));
-    if (events) CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_FINISHED, 0, 3 * 4, h->stream));
-    int bound = A_cur;  // rows the boundary looks at: the tables plus room for this cycle's admissions
-    if (!jump) {
-      const int nbH = (n_live + tb - 1) / tb;
-      k_drain_apply<<<nbH, tb, 0, h->stream>>>(D, X);
-      k_scan_i32<<<1, 1024, 0, h->stream>>>(X.e_assumed, X.e_adm_off, n_live);
-      k_scan_i32<<<1, 1024, 0, h->stream>>>(X.e_ncells, X.e_cell_off, n_live);
-      k_drain_admit<<<nbH, tb, 0, h->stream>>>(D, X, t);
-      if (evict) k_drain_evict<<<nbH, tb, 0, h->stream>>>(D, X);
-      bound = (int)std::min<size_t>((size_t)A_cur + n_live, Acap);
-    }
-    if (events) {
-      const int nbB = std::max(1, (bound + tb - 1) / tb);
-      k_drain_ev_min<<<nbB, tb, 0, h->stream>>>(X, bound, n_new_d);
-      k_drain_ev_next<<<1, 1, 0, h->stream>>>(X, t, step, jump, n_new_d);
-      if (quota) k_drain_quota<<<1, 1024, 0, h->stream>>>(D, X);  // step 5: the edits, before the verdicts
-      if (act) k_drain_active<<<nbAc, tb, 0, h->stream>>>(D, X, 0);  // the edits of records without a row; the stop times
-      if (decay) k_drain_afs_decay<<<nbL, tb, 0, h->stream>>>(D, X, L);  // samples due in (t, t_{c+1}], before the completions
-      k_drain_finish<<<nbB, tb, 0, h->stream>>>(D, X, bound, n_new_d);
-      if (X.arr_key) k_drain_arrive<<<nbArr, tb, 0, h->stream>>>(X);
-      // the edits of records that met their own events first, before k_drain_backoff folds the remaining RequeueAts
-      // into the next E: a record a timeout or a Retry put in BACKOFF and a later stop deactivated has none
-      if (act) k_drain_active<<<nbAc, tb, 0, h->stream>>>(D, X, 1);
-      if (requeue) k_drain_backoff<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W);
-    }
-    if (compact) {
-      k_drain_requeue<<<nbQ, tb, 0, h->stream>>>(D, X);
-      if (act) k_drain_advance<<<(S + tb - 1) / tb, tb, 0, h->stream>>>(X, S);  // a deactivated record may sit at a cursor
-      const int nbA = (bound + 1 + tb - 1) / tb;
-      k_drain_live<<<nbA, tb, 0, h->stream>>>(X, bound, n_new_d);
-      size_t sb = scan_bytes;
-      CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(scan_tmp, sb, X.row_live, X.row_new, bound + 1, h->stream));
-      sb = scan_bytes;
-      CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(scan_tmp, sb, X.row_cells, X.cell_new, bound + 1, h->stream));
-      k_drain_compact<<<nbA, tb, 0, h->stream>>>(X, other, bound);
-    }
-    enqueue_heads();
-    kmark(h, -1);
-    CUDA_TRY(h, cudaEventRecord(h->ev_d, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[0], X.counters, 4, cudaMemcpyDeviceToHost, h->stream));
-    if (!jump) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_new, n_new_d, 4, cudaMemcpyDeviceToHost, h->stream));
-    if (!compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_cells, X.e_cell_off + n_live, 4, cudaMemcpyDeviceToHost, h->stream));
-    if (afs && (!jump || decay)) CUDA_TRY(h, cudaMemcpyAsync(&hw.status, D.status, 4, cudaMemcpyDeviceToHost, h->stream));
-    if (compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[1], X.counters + 1, (rcl ? KB_DC_RECLAIMS : act ? KB_DC_AC_HI : quota ? KB_DC_QC_HI : mx ? KB_DC_EXEC_STATUS : pr ? KB_DC_PR_DEACTIVATED : checks ? KB_DC_CHECK_REJECTED : events ? KB_DC_ARR_HI : KB_DC_FULL) * 4, cudaMemcpyDeviceToHost, h->stream));
-    if (events) CUDA_TRY(h, cudaMemcpyAsync(&hw.t_next, X.clock, 8, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    if (!jump) {
-      rc = cycle_finish(h);
-      if (rc != KB_OK) return rc;
-      if (afs && (hw.status & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: an entry penalty overflows int64");
-      for (int i = 0; i < KB_N_KERNELS; i++) kms[i] += h->stats.kernel_ms[i];
-    }
-    if (decay && (hw.status & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: a decayed consumed quantity overflows int64");
-    { float ms = 0; cudaEventElapsedTime(&ms, h->ev2, h->ev_d); gpu_ms += ms; }
-    if (compact && hw.counters[KB_DC_FULL]) return fail(h, KB_ERR_CAPACITY, "kb_run_drain: the admitted tables are full");
-    const int n_new = jump ? 0 : (int)hw.n_new, n_ev = evict ? (int)hw.counters[KB_DC_EVICTED] : 0;
-    if (!jump) {
-      if (out->cycle_heads) out->cycle_heads[cyc] = n_live;
-      if (out->cycle_admitted) out->cycle_admitted[cyc] = n_new;
-      if (out->cycle_evicted) out->cycle_evicted[cyc] = n_ev;
-      if (events && out->cycle_start_ns) out->cycle_start_ns[cyc] = t;
-      if (events && out->cycle_finished) out->cycle_finished[cyc] = 0;
-      if (events && out->cycle_arrived) out->cycle_arrived[cyc] = 0;
-      if (lat && out->cycle_evict_done) out->cycle_evict_done[cyc] = 0;
-      if (checks && out->cycle_check_retry) out->cycle_check_retry[cyc] = 0;
-      if (checks && out->cycle_check_rejected) out->cycle_check_rejected[cyc] = 0;
-      if (pr && out->cycle_pods_ready_timeout) out->cycle_pods_ready_timeout[cyc] = 0;
-      if (pr && out->cycle_pods_ready_deactivated) out->cycle_pods_ready_deactivated[cyc] = 0;
-      if (mx && out->cycle_max_exec_deactivated) out->cycle_max_exec_deactivated[cyc] = 0;
-      if (quota && out->cycle_quota_changes) out->cycle_quota_changes[cyc] = 0;
-      if (act && out->cycle_stopped) out->cycle_stopped[cyc] = 0;
-      if (act && out->cycle_resumed) out->cycle_resumed[cyc] = 0;
-      if (rcl && out->cycle_reclaims) out->cycle_reclaims[cyc] = 0;
-      out->n_decisions += n_live; out->n_admitted += n_new; out->n_evicted += n_ev;
-      out->n_cycles = ++cyc;
-    } else {
-      jumps++;
-    }
-    if (events) {
-      const int fin = (int)hw.counters[KB_DC_FINISHED], arr = (int)hw.counters[KB_DC_ARRIVED];
-      out->n_finished += fin; out->n_arrived += arr;
-      if (cyc > 0) {  // events between the start of the last cycle and the next one are that cycle's
-        if (out->cycle_finished) out->cycle_finished[cyc - 1] += fin;
-        if (out->cycle_arrived) out->cycle_arrived[cyc - 1] += arr;
-      }
-    }
-    if (checks) {  // verdicts of this boundary; a record that entered its queue with a new timestamp re-sorts the queues
-      const uint32_t *cum = &hw.counters[KB_DC_CHECK_READY];
-      const int ready = (int)(cum[0] - verdicts_seen[0]), ret = (int)(cum[1] - verdicts_seen[1]), rej = (int)(cum[2] - verdicts_seen[2]);
-      memcpy(verdicts_seen, cum, sizeof(verdicts_seen));
-      out->n_check_ready += ready; out->n_check_retry += ret; out->n_check_rejected += rej;
-      if (cyc > 0) {
-        if (out->cycle_check_retry) out->cycle_check_retry[cyc - 1] += ret;
-        if (out->cycle_check_rejected) out->cycle_check_rejected[cyc - 1] += rej;
-      }
-    }
-    if (pr) {  // PodsReady timeouts of this boundary
-      const uint32_t *cum = &hw.counters[KB_DC_PR_TIMEOUT];
-      const int to = (int)(cum[0] - timeouts_seen[0]), de = (int)(cum[1] - timeouts_seen[1]);
-      memcpy(timeouts_seen, cum, sizeof(timeouts_seen));
-      out->n_pods_ready_timeout += to; out->n_pods_ready_deactivated += de;
-      if (cyc > 0) {
-        if (out->cycle_pods_ready_timeout) out->cycle_pods_ready_timeout[cyc - 1] += to;
-        if (out->cycle_pods_ready_deactivated) out->cycle_pods_ready_deactivated[cyc - 1] += de;
-      }
-    }
-    if (mx) {  // MaximumExecutionTimeExceeded deactivations of this boundary, and the overflow bit
-      if (hw.counters[KB_DC_EXEC_STATUS] & KBS_EXEC_OVERFLOW)
-        return fail(h, KB_ERR_UNSUPPORTED, "max exec: an accumulated execution time leaves int32");
-      const int de = (int)(hw.counters[KB_DC_EXEC_DEACTIVATED] - exec_seen);
-      exec_seen = hw.counters[KB_DC_EXEC_DEACTIVATED];
-      out->n_max_exec_deactivated += de;
-      if (cyc > 0 && out->cycle_max_exec_deactivated) out->cycle_max_exec_deactivated[cyc - 1] += de;
-    }
-    if (quota) {  // edits applied at this boundary
-      const int qc = (int)(hw.counters[KB_DC_QC_HI] - hw.counters[KB_DC_QC_LO]);
-      out->n_quota_changes += qc;
-      if (cyc > 0 && out->cycle_quota_changes) out->cycle_quota_changes[cyc - 1] += qc;
-    }
-    if (act) {  // stops / resumes that changed the state at this boundary
-      const uint32_t *cum = &hw.counters[KB_DC_STOPPED];
-      const int st = (int)(cum[0] - active_seen[0]), re = (int)(cum[1] - active_seen[1]);
-      memcpy(active_seen, cum, sizeof(active_seen));
-      out->n_stopped += st; out->n_resumed += re;
-      if (cyc > 0) {
-        if (out->cycle_stopped) out->cycle_stopped[cyc - 1] += st;
-        if (out->cycle_resumed) out->cycle_resumed[cyc - 1] += re;
-      }
-    }
-    if (rcl) {  // reclaim steps that lowered a count at this boundary
-      const int n = (int)(hw.counters[KB_DC_RECLAIMS] - reclaims_seen);
-      reclaims_seen = hw.counters[KB_DC_RECLAIMS];
-      out->n_reclaims += n;
-      if (cyc > 0 && out->cycle_reclaims) out->cycle_reclaims[cyc - 1] += n;
-    }
-    if (lat) {  // evictions completed at this boundary (counter slot 4, inside the events copy)
-      const int done = (int)hw.counters[KB_DC_EVICT_DONE];
-      out->n_evict_done += done;
-      if (cyc > 0 && out->cycle_evict_done) out->cycle_evict_done[cyc - 1] += done;
-    }
-    if (compact) {  // the compacted half becomes the admitted tables of the next boundary
-      A_cur = (int)hw.counters[KB_DC_ROWS]; AU_cur = (int)hw.counters[KB_DC_CELLS];
-      AdmTabs cur{X.adm_cq, X.adm_priority, X.adm_ts, X.adm_qr_ts, X.adm_uid, X.adm_evicted, X.adm_use_start, X.adm_use_fr, X.adm_use_qty, X.adm_wl, X.adm_finish, X.adm_lq,
-                  X.adm_evicting, X.adm_phase, X.adm_exec_since, X.adm_rc_next, X.adm_rc_cur};
-      X.adm_cq = other.cq; X.adm_priority = other.priority; X.adm_ts = other.ts; X.adm_qr_ts = other.qr_ts; X.adm_uid = other.uid;
-      X.adm_evicted = other.evicted; X.adm_use_start = other.use_start; X.adm_use_fr = other.use_fr; X.adm_use_qty = other.use_qty; X.adm_wl = other.wl;
-      X.adm_finish = other.finish; X.adm_lq = other.lq; X.adm_evicting = other.evicting; X.adm_phase = other.phase;
-      X.adm_exec_since = other.since; X.adm_rc_next = other.rc_next; X.adm_rc_cur = other.rc_cur;
-      D.adm_cq = X.adm_cq; D.adm_priority = X.adm_priority; D.adm_ts = X.adm_ts; D.adm_qr_ts = X.adm_qr_ts; D.adm_uid = X.adm_uid;
-      D.adm_evicted = X.adm_evicted; D.adm_use_start = X.adm_use_start; D.adm_use_fr = X.adm_use_fr; D.adm_use_qty = X.adm_use_qty;
-      other = cur;
-    } else {
-      A_cur += n_new; AU_cur += (int)hw.n_cells;
-    }
-    n_live = (int)hw.counters[0];
-    if (events ? hw.counters[KB_DC_END] != 0 : n_new == 0 && n_ev == 0) break;
-    if (requeue && (int32_t)hw.counters[KB_DC_RESORT] == X.cycle + 1) {  // re-sort: the three passes over the queue-order timestamps, positions,
-      // cursors from 0, first_aside from the SET_ASIDE positions, then the heads again.  The segments and their
-      // lengths do not change, so n_live holds and no synchronisation is added; the events are read at the next one.
-      if (resort_timed) { float ms = 0; cudaEventElapsedTime(&ms, ev_r[0], ev_r[1]); out->resort_ms += ms; gpu_ms += ms; }
-      CUDA_TRY(h, cudaEventRecord(ev_r[0], h->stream));
-      CUDA_TRY(h, sort_queues());
-      k_drain_init_replay<<<std::max(1, nbW), tb, 0, h->stream>>>(D, X, 0);
-      k_drain_resort_reset<<<(S + tb - 1) / tb, tb, 0, h->stream>>>(X, S);
-      k_drain_resort_aside<<<std::max(1, nbW), tb, 0, h->stream>>>(X, W);
-      k_drain_advance<<<(S + tb - 1) / tb, tb, 0, h->stream>>>(X, S);
-      CUDA_TRY(h, cudaMemcpyAsync(X.wl_sort_ts, X.wl_qts, Wz * 8, cudaMemcpyDeviceToDevice, h->stream));
-      enqueue_heads();
-      CUDA_TRY(h, cudaEventRecord(ev_r[1], h->stream));
-      resort_timed = true;
-      out->n_resorts++;
-    }
-    t = events ? hw.t_next : t + 1;
+  return KB_OK;
+}
+
+// One boundary, one synchronisation (kueue_b200/drain.py _Drain.boundary): cycle c at t (in event mode, a jump to the
+// next event when there are no heads), its decisions and admissions, the evictions; in event mode E, t_{c+1}, the decay
+// samples, completions and arrivals; where rows can die (compact) the inadmissible requeue and the compaction over
+// [0, bound); then the heads of the next cycle.  A plain drain ends at a cycle without heads or one that neither admits
+// nor evicts (the next cycle would see the same snapshot); an event drain when no event is left (*done).
+// Capacity: before the compaction the tables hold the live rows plus this cycle's admissions, and every admitted head
+// is a workload that holds no row, so the rows stay within A_in + min(W, Hcap * max_cycles) and the cells within
+// AU_in + min(P * R, that bound * FR) (a readmitted victim's old cells left with its old row): what upload_impl
+// reserved.  An admission past the end is not written and the call fails.
+static int32_t drain_boundary(DrainRun &r, bool *done) {
+  kb_handle *h = r.h; const DrainMode &m = r.m; kb_drain_out *out = r.out;
+  DevSnap &D = h->D; DrainDev &X = r.X;
+  DrainWords &hw = *reinterpret_cast<DrainWords *>(&h->host_words[64]);
+  const int tb = DRAIN_TB, n_live = r.n_live, sms = std::max(1, h->sm_count);
+  const bool jump = n_live == 0;
+  *done = jump && !m.events;
+  if (*done) return KB_OK;
+  const int32_t *n_new_d = jump ? nullptr : X.e_adm_off + n_live;
+  if (!jump) {
+    D.H = n_live; D.now_ns = r.t;
+    D.A = h->preempt_possible ? r.A_cur : 0; D.AU = h->preempt_possible ? r.AU_cur : 0;  // without preemption policies the cycle never looks at the admitted tables
+    if (int32_t rc = cycle_enqueue(h)) return rc;
+    X.cycle = r.cyc;
+  } else {
+    CUDA_TRY(h, cudaEventRecord(h->ev2, h->stream));
+    X.cycle = -2 - r.jumps;  // stamps of a jump (cycle + 1 < 0) never meet those of a cycle
   }
-  if (events) out->end_ns = t;
-  if (resort_timed) {
-    CUDA_TRY(h, cudaEventSynchronize(ev_r[1]));
-    float ms = 0; cudaEventElapsedTime(&ms, ev_r[0], ev_r[1]); out->resort_ms += ms; gpu_ms += ms;
+  X.A = r.A_cur; X.AU = r.AU_cur; X.trace_off = (long long)out->n_decisions;
+  kmark(h, KB_K_DRAIN);
+  if (m.compact) CUDA_TRY(h, cudaMemsetAsync(X.counters + 1, 0, 4 * 4, h->stream));
+  if (m.events) CUDA_TRY(h, cudaMemsetAsync(X.counters + KB_DC_FINISHED, 0, 3 * 4, h->stream));
+  int bound = r.A_cur;  // rows the boundary looks at: the tables plus room for this cycle's admissions
+  if (!jump) {
+    const int nbH = drain_blocks(n_live);
+    k_drain_apply<<<nbH, tb, 0, h->stream>>>(D, X);
+    k_scan_i32<<<1, 1024, 0, h->stream>>>(X.e_assumed, X.e_adm_off, n_live);
+    k_scan_i32<<<1, 1024, 0, h->stream>>>(X.e_ncells, X.e_cell_off, n_live);
+    k_drain_admit<<<nbH, tb, 0, h->stream>>>(D, X, r.t);
+    if (m.evict) k_drain_evict<<<nbH, tb, 0, h->stream>>>(D, X);
+    bound = (int)std::min<size_t>((size_t)r.A_cur + n_live, r.Acap);
   }
-  out->gpu_ms = gpu_ms;
-  h->stats.last_cycle_gpu_ms = gpu_ms;
-  memcpy(h->stats.kernel_ms, kms, sizeof(kms));
-  // ---- results
-  size_t PR = (size_t)D.P * D.R;
-  if (out->wl_admit_cycle) CUDA_TRY(h, cudaMemcpyAsync(out->wl_admit_cycle, X.wl_admit_cycle, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
-  if (out->wl_last_decision) CUDA_TRY(h, cudaMemcpyAsync(out->wl_last_decision, X.wl_last_decision, Wz, cudaMemcpyDeviceToHost, h->stream));
-  if (out->wl_evals) CUDA_TRY(h, cudaMemcpyAsync(out->wl_evals, X.wl_evals, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
-  if (events && out->wl_admit_ns) CUDA_TRY(h, cudaMemcpyAsync(out->wl_admit_ns, X.wl_admit_ns, Wz * 8, cudaMemcpyDeviceToHost, h->stream));
-  if (events && out->wl_finish_ns) CUDA_TRY(h, cudaMemcpyAsync(out->wl_finish_ns, X.wl_finish_ns, Wz * 8, cudaMemcpyDeviceToHost, h->stream));
-  if (decay) {
-    if (out->lq_consumed && L) CUDA_TRY(h, cudaMemcpyAsync(out->lq_consumed, X.lq_consumed, (size_t)L * R * 8, cudaMemcpyDeviceToHost, h->stream));
-    if (out->lq_consumed_scale && L) CUDA_TRY(h, cudaMemcpyAsync(out->lq_consumed_scale, X.lq_consumed_scale, (size_t)L * R * 4, cudaMemcpyDeviceToHost, h->stream));
-    if (out->lq_last_update_ns && L) CUDA_TRY(h, cudaMemcpyAsync(out->lq_last_update_ns, X.lq_last, (size_t)L * 8, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(&out->n_afs_samples, X.afs_samples, 8, cudaMemcpyDeviceToHost, h->stream));
+  if (m.events) {
+    const int nbB = std::max(1, drain_blocks(bound)), nbAc = std::max(1, std::min(drain_blocks(m.n_ac), sms));  // grid-stride over the edits
+    k_drain_ev_min<<<nbB, tb, 0, h->stream>>>(X, bound, n_new_d);
+    k_drain_ev_next<<<1, 1, 0, h->stream>>>(X, r.t, r.step, jump, n_new_d);
+    if (m.quota) k_drain_quota<<<1, 1024, 0, h->stream>>>(D, X);  // step 5: the edits, before the verdicts
+    if (m.act) k_drain_active<<<nbAc, tb, 0, h->stream>>>(D, X, 0);  // the edits of records without a row; the stop times
+    if (m.decay) k_drain_afs_decay<<<std::max(1, drain_blocks(r.L)), tb, 0, h->stream>>>(D, X, r.L);  // samples due in (t, t_{c+1}], before the completions
+    k_drain_finish<<<nbB, tb, 0, h->stream>>>(D, X, bound, n_new_d);
+    if (X.arr_key) k_drain_arrive<<<std::max(1, std::min(drain_blocks(r.W), 8 * sms)), tb, 0, h->stream>>>(X);
+    // the edits of records that met their own events first, before k_drain_backoff folds the remaining RequeueAts
+    // into the next E: a record a timeout or a Retry put in BACKOFF and a later stop deactivated has none
+    if (m.act) k_drain_active<<<nbAc, tb, 0, h->stream>>>(D, X, 1);
+    if (m.requeue) k_drain_backoff<<<std::max(1, drain_blocks(r.W)), tb, 0, h->stream>>>(X, r.W);
+  }
+  if (m.compact) {
+    k_drain_requeue<<<drain_blocks(r.Q), tb, 0, h->stream>>>(D, X);
+    if (m.act) k_drain_advance<<<drain_blocks(r.S), tb, 0, h->stream>>>(X, r.S);  // a deactivated record may sit at a cursor
+    const int nbA = drain_blocks(bound + 1);
+    k_drain_live<<<nbA, tb, 0, h->stream>>>(X, bound, n_new_d);
+    size_t sb = r.scan_bytes;
+    CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(r.scan_tmp, sb, X.row_live, X.row_new, bound + 1, h->stream));
+    sb = r.scan_bytes;
+    CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(r.scan_tmp, sb, X.row_cells, X.cell_new, bound + 1, h->stream));
+    k_drain_compact<<<nbA, tb, 0, h->stream>>>(X, r.other, bound);
+  }
+  drain_heads(r);
+  kmark(h, -1);
+  CUDA_TRY(h, cudaEventRecord(h->ev_d, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(&hw.counters[0], X.counters, (size_t)r.n_used * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (!jump) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_new, n_new_d, 4, cudaMemcpyDeviceToHost, h->stream));
+  if (!m.compact) CUDA_TRY(h, cudaMemcpyAsync(&hw.n_cells, X.e_cell_off + n_live, 4, cudaMemcpyDeviceToHost, h->stream));
+  if (m.afs && (!jump || m.decay)) CUDA_TRY(h, cudaMemcpyAsync(&hw.status, D.status, 4, cudaMemcpyDeviceToHost, h->stream));
+  if (m.events) CUDA_TRY(h, cudaMemcpyAsync(&hw.t_next, X.clock, 8, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  if (!jump) {
+    if (int32_t rc = cycle_finish(h)) return rc;
+    if (m.afs && (hw.status & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: an entry penalty overflows int64");
+    for (int i = 0; i < KB_N_KERNELS; i++) r.kms[i] += h->stats.kernel_ms[i];
+  }
+  if (m.decay && (hw.status & KBS_AFS_OVERFLOW)) return fail(h, KB_ERR_UNSUPPORTED, "afs: a decayed consumed quantity overflows int64");
+  { float ms = 0; cudaEventElapsedTime(&ms, h->ev2, h->ev_d); r.gpu_ms += ms; }
+  if (m.compact && hw.counters[KB_DC_FULL]) return fail(h, KB_ERR_CAPACITY, "kb_run_drain: the admitted tables are full");
+  if (m.mx && (hw.counters[KB_DC_EXEC_STATUS] & KBS_EXEC_OVERFLOW))
+    return fail(h, KB_ERR_UNSUPPORTED, "max exec: an accumulated execution time leaves int32");
+  const int n_new = jump ? 0 : (int)hw.n_new, n_ev = m.evict ? (int)hw.counters[KB_DC_EVICTED] : 0;
+  if (!jump) {
+    const int cyc = r.cyc;
+    if (out->cycle_heads) out->cycle_heads[cyc] = n_live;
+    if (out->cycle_admitted) out->cycle_admitted[cyc] = n_new;
+    if (out->cycle_evicted) out->cycle_evicted[cyc] = n_ev;
+    if (m.events && out->cycle_start_ns) out->cycle_start_ns[cyc] = r.t;
+    for (const DrainCounter &c : r.counters)
+      if (c.on && c.cycle) c.cycle[cyc] = 0;
+    out->n_decisions += n_live; out->n_admitted += n_new; out->n_evicted += n_ev;
+    out->n_cycles = ++r.cyc;
+  } else {
+    r.jumps++;
+  }
+  for (DrainCounter &c : r.counters) {  // the events of this boundary; those between the start of the last cycle and the next one are that cycle's
+    if (!c.on) continue;
+    const uint32_t *v = &hw.counters[c.idx];
+    int n = (int)v[0];
+    if (c.kind == DC_CUMULATIVE) { n = (int)(v[0] - c.seen); c.seen = v[0]; }
+    else if (c.kind == DC_RANGE) n = (int)(v[1] - v[0]);
+    *c.total += n;
+    if (r.cyc > 0 && c.cycle) c.cycle[r.cyc - 1] += n;
+  }
+  if (m.compact) {  // the compacted half becomes the admitted tables of the next boundary
+    r.A_cur = (int)hw.counters[KB_DC_ROWS]; r.AU_cur = (int)hw.counters[KB_DC_CELLS];
+    std::swap(X.adm, r.other);
+    drain_point_snap(D, X.adm);
+  } else {
+    r.A_cur += n_new; r.AU_cur += (int)hw.n_cells;
+  }
+  r.n_live = (int)hw.counters[0];
+  *done = m.events ? hw.counters[KB_DC_END] != 0 : n_new == 0 && n_ev == 0;
+  if (*done) return KB_OK;
+  if (m.requeue && (int32_t)hw.counters[KB_DC_RESORT] == X.cycle + 1) {  // re-sort: the three passes over the queue-order
+    // timestamps, positions, cursors from 0, first_aside from the SET_ASIDE positions, then the heads again.  The segments
+    // and their lengths do not change, so n_live holds and no synchronisation is added; the events are read at the next one.
+    if (r.resort_timed) { float ms = 0; cudaEventElapsedTime(&ms, r.ev_r[0], r.ev_r[1]); out->resort_ms += ms; r.gpu_ms += ms; }
+    CUDA_TRY(h, cudaEventRecord(r.ev_r[0], h->stream));
+    CUDA_TRY(h, drain_sort_queues(r));
+    k_drain_init_replay<<<std::max(1, drain_blocks(r.W)), tb, 0, h->stream>>>(D, X, 0);
+    k_drain_resort_reset<<<drain_blocks(r.S), tb, 0, h->stream>>>(X, r.S);
+    k_drain_resort_aside<<<std::max(1, drain_blocks(r.W)), tb, 0, h->stream>>>(X, r.W);
+    k_drain_advance<<<drain_blocks(r.S), tb, 0, h->stream>>>(X, r.S);
+    CUDA_TRY(h, cudaMemcpyAsync(X.wl_sort_ts, X.wl_qts, (size_t)r.W * 8, cudaMemcpyDeviceToDevice, h->stream));
+    drain_heads(r);
+    CUDA_TRY(h, cudaEventRecord(r.ev_r[1], h->stream));
+    r.resort_timed = true;
+    out->n_resorts++;
+  }
+  r.t = m.events ? hw.t_next : r.t + 1;
+  return KB_OK;
+}
+
+// the end of the drain: the clock, the device time, the tables kb_drain_out asks for
+static int32_t drain_results(DrainRun &r) {
+  kb_handle *h = r.h; const DrainMode &m = r.m; kb_drain_out *out = r.out;
+  const DevSnap &D = h->D; const DrainDev &X = r.X;
+  const size_t Wz = (size_t)r.W, L = (size_t)r.L, R = (size_t)r.R, PR = (size_t)D.P * D.R;
+  if (m.events) out->end_ns = r.t;
+  if (r.resort_timed) {
+    CUDA_TRY(h, cudaEventSynchronize(r.ev_r[1]));
+    float ms = 0; cudaEventElapsedTime(&ms, r.ev_r[0], r.ev_r[1]); out->resort_ms += ms; r.gpu_ms += ms;
+  }
+  out->gpu_ms = r.gpu_ms;
+  h->stats.last_cycle_gpu_ms = r.gpu_ms;
+  memcpy(h->stats.kernel_ms, r.kms, sizeof(r.kms));
+  auto d2h = [&](void *dst, const void *src, size_t bytes) { return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, h->stream); };
+  if (out->wl_admit_cycle) CUDA_TRY(h, d2h(out->wl_admit_cycle, X.wl_admit_cycle, Wz * 4));
+  if (out->wl_last_decision) CUDA_TRY(h, d2h(out->wl_last_decision, X.wl_last_decision, Wz));
+  if (out->wl_evals) CUDA_TRY(h, d2h(out->wl_evals, X.wl_evals, Wz * 4));
+  if (m.events && out->wl_admit_ns) CUDA_TRY(h, d2h(out->wl_admit_ns, X.wl_admit_ns, Wz * 8));
+  if (m.events && out->wl_finish_ns) CUDA_TRY(h, d2h(out->wl_finish_ns, X.wl_finish_ns, Wz * 8));
+  if (m.decay) {
+    if (out->lq_consumed && L) CUDA_TRY(h, d2h(out->lq_consumed, X.lq_consumed, L * R * 8));
+    if (out->lq_consumed_scale && L) CUDA_TRY(h, d2h(out->lq_consumed_scale, X.lq_consumed_scale, L * R * 4));
+    if (out->lq_last_update_ns && L) CUDA_TRY(h, d2h(out->lq_last_update_ns, X.lq_last, L * 8));
+    CUDA_TRY(h, d2h(&out->n_afs_samples, X.afs_samples, 8));
   }
   if (out->wl_evictions) {
-    if (replay) CUDA_TRY(h, cudaMemcpyAsync(out->wl_evictions, X.wl_evictions, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (m.replay) CUDA_TRY(h, d2h(out->wl_evictions, X.wl_evictions, Wz * 4));
     else memset(out->wl_evictions, 0, Wz * 4);
   }
-  if (sticky && out->cq_sticky) CUDA_TRY(h, cudaMemcpyAsync(out->cq_sticky, X.cq_sticky, (size_t)Q * 4, cudaMemcpyDeviceToHost, h->stream));
-  if (checks) {
-    if (out->wl_ready_ns) CUDA_TRY(h, cudaMemcpyAsync(out->wl_ready_ns, X.wl_ready_ns, Wz * 8, cudaMemcpyDeviceToHost, h->stream));
-    if (out->wl_check_retries_out) CUDA_TRY(h, cudaMemcpyAsync(out->wl_check_retries_out, X.wl_retries, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (m.sticky && out->cq_sticky) CUDA_TRY(h, d2h(out->cq_sticky, X.cq_sticky, (size_t)r.Q * 4));
+  if (m.checks) {
+    if (out->wl_ready_ns) CUDA_TRY(h, d2h(out->wl_ready_ns, X.wl_ready_ns, Wz * 8));
+    if (out->wl_check_retries_out) CUDA_TRY(h, d2h(out->wl_check_retries_out, X.wl_retries, Wz * 4));
   }
-  if ((requeue || mx || blk) && out->wl_deactivated) CUDA_TRY(h, cudaMemcpyAsync(out->wl_deactivated, X.wl_deactivated, Wz, cudaMemcpyDeviceToHost, h->stream));
-  if ((requeue || mx || blk) && out->wl_deactivation_reason)
-    CUDA_TRY(h, cudaMemcpyAsync(out->wl_deactivation_reason, X.wl_deactivated, Wz, cudaMemcpyDeviceToHost, h->stream));
-  if (mx && out->wl_exec_acc_s_out) CUDA_TRY(h, cudaMemcpyAsync(out->wl_exec_acc_s_out, X.wl_exec_acc, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
-  if (pr) {
-    if (out->wl_pods_ready_at_ns) CUDA_TRY(h, cudaMemcpyAsync(out->wl_pods_ready_at_ns, X.wl_pr_at, Wz * 8, cudaMemcpyDeviceToHost, h->stream));
-    if (out->wl_pods_ready_count_out) CUDA_TRY(h, cudaMemcpyAsync(out->wl_pods_ready_count_out, X.wl_pr_count, Wz * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (m.deact && out->wl_deactivated) CUDA_TRY(h, d2h(out->wl_deactivated, X.wl_deactivated, Wz));
+  if (m.deact && out->wl_deactivation_reason) CUDA_TRY(h, d2h(out->wl_deactivation_reason, X.wl_deactivated, Wz));
+  if (m.mx && out->wl_exec_acc_s_out) CUDA_TRY(h, d2h(out->wl_exec_acc_s_out, X.wl_exec_acc, Wz * 4));
+  if (m.pr) {
+    if (out->wl_pods_ready_at_ns) CUDA_TRY(h, d2h(out->wl_pods_ready_at_ns, X.wl_pr_at, Wz * 8));
+    if (out->wl_pods_ready_count_out) CUDA_TRY(h, d2h(out->wl_pods_ready_count_out, X.wl_pr_count, Wz * 4));
   }
-  if (out->ps_flavor && PR) CUDA_TRY(h, cudaMemcpyAsync(out->ps_flavor, D.ps_flavor, PR, cudaMemcpyDeviceToHost, h->stream));
-  if (out->ps_count && D.P) CUDA_TRY(h, cudaMemcpyAsync(out->ps_count, D.ps_count_out, (size_t)D.P * 4, cudaMemcpyDeviceToHost, h->stream));
-  if (out->cq_usage) CUDA_TRY(h, cudaMemcpyAsync(out->cq_usage, D.cq_usage, (size_t)Q * FR * 8, cudaMemcpyDeviceToHost, h->stream));
-  if (rcl && out->ps_remaining_out && D.P) CUDA_TRY(h, cudaMemcpyAsync(out->ps_remaining_out, D.ps_count, (size_t)D.P * 4, cudaMemcpyDeviceToHost, h->stream));
-  if ((quota || rcl) && out->cq_generation) CUDA_TRY(h, cudaMemcpyAsync(out->cq_generation, D.cq_generation, (size_t)Q * 8, cudaMemcpyDeviceToHost, h->stream));
-  size_t nt = std::min<size_t>(trace_cap, (size_t)out->n_decisions);
+  if (out->ps_flavor && PR) CUDA_TRY(h, d2h(out->ps_flavor, D.ps_flavor, PR));
+  if (out->ps_count && D.P) CUDA_TRY(h, d2h(out->ps_count, D.ps_count_out, (size_t)D.P * 4));
+  if (out->cq_usage) CUDA_TRY(h, d2h(out->cq_usage, D.cq_usage, (size_t)r.Q * r.FR * 8));
+  if (m.rcl && out->ps_remaining_out && D.P) CUDA_TRY(h, d2h(out->ps_remaining_out, D.ps_count, (size_t)D.P * 4));
+  if ((m.quota || m.rcl) && out->cq_generation) CUDA_TRY(h, d2h(out->cq_generation, D.cq_generation, (size_t)r.Q * 8));
+  const size_t nt = std::min<size_t>(r.trace_cap, (size_t)out->n_decisions);
   if (nt) {
-    CUDA_TRY(h, cudaMemcpyAsync(out->trace_wl, X.trace_wl, nt * 4, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(out->trace_decision, X.trace_dec, nt, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, d2h(out->trace_wl, X.trace_wl, nt * 4));
+    CUDA_TRY(h, d2h(out->trace_decision, X.trace_dec, nt));
   }
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  if ((requeue || mx || blk) && out->wl_deactivated)  // the device byte holds the reason (KB_DR_*)
-    for (int w = 0; w < W; w++) out->wl_deactivated[w] = out->wl_deactivated[w] != 0;
+  if (m.deact && out->wl_deactivated)  // the device byte holds the reason (KB_DR_*)
+    for (int w = 0; w < r.W; w++) out->wl_deactivated[w] = out->wl_deactivated[w] != 0;
   return KB_OK;
+}
+
+// the stages of kb_run_drain: mode, input checks, plan, buffers, uploads and the start, the boundaries, the results
+static int32_t drain_impl(kb_handle *h, const kb_snapshot *s, kb_drain_out *out) {
+  DrainRun r;
+  r.h = h; r.s = s; r.out = out;
+  r.m = drain_mode(s);
+  r.counters = drain_counters(out, r.m);
+  r.Q = s->n_cq; r.W = s->n_wl; r.R = s->n_resource; r.FR = s->n_flavor * s->n_resource;
+  r.Hcap = std::min(r.Q, r.W);
+  r.max_cycles = std::max(0, out->max_cycles);
+  out->n_cycles = 0; out->n_decisions = 0; out->n_admitted = 0; out->gpu_ms = 0; out->n_evicted = 0;
+  out->end_ns = s->now_ns; out->n_resorts = 0; out->resort_ms = 0;
+  for (const DrainCounter &c : r.counters) *c.total = 0;
+  if (int32_t rc = drain_validate(h, s, r.m, r.held)) return rc;
+  if (r.m.sticky && out->cq_sticky) memcpy(out->cq_sticky, s->cq_sticky, (size_t)r.Q * 4);  // the slots of a drain that runs no cycle
+  out->n_afs_samples = 0;
+  if (r.Hcap == 0 || r.max_cycles == 0) {
+    if (r.m.rcl && out->ps_remaining_out && s->n_podset) memcpy(out->ps_remaining_out, s->ps_count, (size_t)s->n_podset * 4);
+    return KB_OK;
+  }
+  size_t extra = (size_t)std::min<long long>((long long)r.W, (long long)r.Hcap * r.max_cycles);
+  h->drain_extra_adm = extra;
+  h->drain_extra_au = std::min<size_t>((size_t)s->n_podset * r.R, extra * (size_t)r.FR);
+  h->drain_mode = true;
+  h->drain_events = r.m.events;
+  kb_snapshot s2 = *s;
+  s2.n_heads = r.Hcap; s2.heads = nullptr;
+  if (int32_t rc = upload_impl(h, &s2, false)) return rc;
+  if (!h->ev_d) cudaEventCreate(&h->ev_d);
+  if (int32_t rc = drain_plan(r)) return rc;
+  r.X.adm = drain_snap_rows(h->D);  // the first half borrows the DevSnap's columns; drain_carve adds the others
+  if (!drain_carve(r)) return fail(h, KB_ERR_CUDA, "kb_run_drain: cudaMalloc of the drain buffer failed");
+  if (int32_t rc = drain_upload(r)) return rc;
+  if (int32_t rc = drain_start(r)) return rc;
+  for (bool done = false; !done && r.cyc < r.max_cycles;)
+    if (int32_t rc = drain_boundary(r, &done)) return rc;
+  return drain_results(r);
 }
 
 extern "C" int32_t kb_run_drain(kb_handle *h, const kb_snapshot *s, kb_drain_out *out) {

@@ -28,11 +28,11 @@
 // an admission adds its entry penalty to its LocalQueue and recomputes that LocalQueue's usage (k_drain_admit).  In event
 // mode with lq_last_update_ns the consumed usage decays (include/kueue_b200.h): k_drain_afs_decay takes the samples due
 // at the start and at every boundary, k_drain_admit decays to t_c and puts the penalty into consumed, k_drain_finish
-// takes finished rows out of the LocalQueue's admitted usage (adm_lq, carried by the compaction).
+// takes finished rows out of the LocalQueue's admitted usage (adm.lq, carried by the compaction).
 //
 // Event mode (kb_snapshot.wl_create_ns / wl_run_ns / adm_finish_ns / wl_evict_ns; include/kueue_b200.h): two more states,
-// KB_WS_ABSENT (not created yet) and KB_WS_FINISHED.  Every admitted row carries its finish time (adm_finish, written by
-// k_drain_admit, carried by the compaction) and its record (adm_wl, -1 for a row of the snapshot without one).  The
+// KB_WS_ABSENT (not created yet) and KB_WS_FINISHED.  Every admitted row carries its finish time (adm.finish, written by
+// k_drain_admit, carried by the compaction) and its record (adm.wl, -1 for a row of the snapshot without one).  The
 // boundary is the replay's, with the clock between the evictions and the requeue: k_drain_ev_min reduces E (the
 // earliest finish of a live row and the next creation), k_drain_ev_next (one thread) computes t_{c+1} and the end
 // flag, k_drain_finish stamps the finished rows dead with the eviction stamp and takes their cells out (a row admitted
@@ -41,7 +41,7 @@
 // is replaced by the same boundary with t_{c+1} = E and a negative stamp (no cycle is counted).  The NoFit set of a
 // ClusterQueue is one byte per (ClusterQueue, scheduling hash) class: k_drain_apply sets it, k_drain_requeue clears the
 // bytes of the queues it visits.  With eviction latency (wl_evict_ns) k_drain_evict only issues: it sets adm_evicted and
-// the byte column adm_evicting (carried by the compaction) and writes the end time into the finish column, so E and the
+// the byte column adm.evicting (carried by the compaction) and writes the end time into the finish column, so E and the
 // compaction see it unchanged; k_drain_finish releases the row at its end time through the replay's requeue path.
 //
 // Sticky workload (kb_snapshot.cq_sticky; include/kueue_b200.h): one slot per ClusterQueue.  k_drain_heads takes a QUEUED
@@ -51,7 +51,7 @@
 // cycle: one writer per slot.  Never set on an AFS ClusterQueue (refused, and no preemption there), so k_drain_afs_heads
 // does not read it.
 //
-// Admission checks (kb_snapshot.wl_check_ns; include/kueue_b200.h): the row-phase byte column adm_phase (both halves,
+// Admission checks (kb_snapshot.wl_check_ns; include/kueue_b200.h): the row-phase byte column adm.phase (both halves,
 // carried by the compaction) marks a row whose checks run (KB_PH_CHECK); its verdict time lives in the finish column, so
 // k_drain_ev_min sees it unchanged.  k_drain_admit starts the attempt, k_drain_evict drops it (a preempted row without pods is released at the
 // next boundary), k_drain_finish applies the verdicts before the completions.  The DevSnap's wl_ts is the mutable
@@ -60,23 +60,23 @@
 // clock[2], which k_drain_ev_next folds into E.  A record that enters its queue with a timestamp other than the key the
 // order was built with (wl_sort_ts) stamps KB_DC_RESORT with the boundary; the host then rebuilds the order (kb_api.cu).
 //
-// WaitForPodsReady (kb_snapshot.wl_pods_ready_ns) runs on the same machinery.  drain_pr_attempt starts an attempt at
-// Admitted (k_drain_admit, or a Ready verdict in k_drain_finish): a ready one only moves the finish column, a failing one
+// WaitForPodsReady (kb_snapshot.wl_pods_ready_ns) runs on the same machinery.  drain_admitted starts an attempt
+// (kb_pr_attempt) at Admitted (k_drain_admit, or a Ready verdict in k_drain_finish): a ready one only moves the finish column, a failing one
 // is KB_PH_WAIT with its timeout T in the finish column.  k_drain_finish applies the timeout after the verdicts: Count,
 // RequeueAt and the queue timestamp on the record, and the row is KB_PH_TIMED_OUT, released at once or, with latency, at
 // T + latency as an evicting row; its release sends the record to BACKOFF (k_drain_backoff queues it) or DEACTIVATED.
 // k_drain_evict drops a waiting attempt.
 //
-// MaximumExecutionTimeSeconds (kb_snapshot.wl_max_exec_s) adds one int64 row column, adm_exec_since (the Admitted time;
-// both halves, carried by the compaction), and the per-record limit and accumulated time.  drain_exec_clip puts the
-// effective deadline into the finish column where it comes before the row's own event (KB_PH_EXPIRE): in k_drain_admit
-// and on a Ready verdict, after drain_pr_attempt.  k_drain_finish applies an expiry after the timeouts: the record is
+// MaximumExecutionTimeSeconds (kb_snapshot.wl_max_exec_s) adds one int64 row column, adm.since (the Admitted time;
+// both halves, carried by the compaction), and the per-record limit and accumulated time.  kb_exec_clip puts the
+// effective deadline into the finish column where it comes before the row's own event (KB_PH_EXPIRE): in drain_admitted,
+// after the PodsReady attempt.  k_drain_finish applies an expiry after the timeouts: the record is
 // deactivated and the row becomes KB_PH_TIMED_OUT, whose release sends a deactivated record to DEACTIVATED.
 // drain_exec_release adds an attempt's seconds at every release of a row with an Admitted time (k_drain_finish, and
 // k_drain_evict without latency) and deactivates a record whose deadline passed before the release.
 //
-// Reclaim steps (kb_snapshot.wl_rc_start) add two row columns (both halves, carried by the compaction): adm_rc_next, the
-// time of the row's next step, and adm_rc_cur, its index.  drain_rc_begin starts a run (k_drain_admit, and a Ready
+// Reclaim steps (kb_snapshot.wl_rc_start) add two row columns (both halves, carried by the compaction): adm.rc_next, the
+// time of the row's next step, and adm.rc_cur, its index.  drain_rc_begin starts a run (k_drain_admit, and a Ready
 // verdict in k_drain_finish), which also records the admission's PodSetAssignment per podset (ps_adm_*; the snapshot's
 // rows bring theirs).  k_drain_ev_min folds the next step of a running row into E, and k_drain_finish applies the steps
 // due (drain_reclaim) before a row's completion, its stop or its expiry: a thread per row, integer atomics on the usage
@@ -125,12 +125,34 @@ __host__ __device__ inline i64 kb_exec_seconds(i64 d) {
   const double x = (double)(d / 1000000000ll) + (double)(d % 1000000000ll) / 1e9;
   return x >= 2147483648.0 ? -1 : (i64)x;
 }
+__host__ __device__ inline i64 drain_sat_add(i64 t, i64 d) { return t > INT64_MAX - d ? INT64_MAX : t + d; }  // d >= 0
 // the MaximumExecutionTimeSeconds deadline A + (max - acc) s of a row Admitted at A (acc -1 = nil, read as 0), saturating
 // both ways.  Restated by kueue_b200/drain.py exec_deadline.
 __host__ __device__ inline i64 kb_exec_deadline(i64 A, int32_t max_s, int32_t acc_s) {
   const i64 left = ((i64)max_s - (acc_s < 0 ? 0 : acc_s)) * 1000000000ll;
   if (left >= 0) return A > INT64_MAX - left ? INT64_MAX : A + left;
   return A < INT64_MIN - left ? INT64_MIN : A + left;
+}
+// adm.phase: what the finish column of a row holds.  RUN: its finish (or its eviction's end when adm.evicting); CHECK: its
+// checks' verdict; WAIT: the timeout T of a PodsReady attempt that fails; TIMED_OUT: the end of its eviction by that
+// timeout or by an expiry; EXPIRE: its effective MaximumExecutionTimeSeconds deadline, which comes before its own event
+enum { KB_PH_RUN = 0, KB_PH_CHECK = 1, KB_PH_WAIT = 2, KB_PH_TIMED_OUT = 3, KB_PH_EXPIRE = 4 };
+struct DrainFin { i64 fin; uint8_t ph; };  // a row's finish column and phase
+// WaitForPodsReady: the attempt of a row Admitted at t.  A failing one (failures left, or a delay d past the timeout)
+// waits for its timeout T = t + timeout; a ready one reaches PodsReady at t + d, and its finish is PodsReady + run (run
+// < 0 never finishes).
+__host__ __device__ inline DrainFin kb_pr_attempt(i64 t, i64 d, bool failing, i64 timeout, i64 run) {
+  if (failing || d > timeout) return {drain_sat_add(t, timeout), KB_PH_WAIT};
+  return {run < 0 ? INT64_MAX : drain_sat_add(drain_sat_add(t, d), run), KB_PH_RUN};
+}
+// MaximumExecutionTimeSeconds of a row Admitted at A whose own next event is f: the effective deadline max(D, A, floor)
+// when it comes first, as KB_PH_EXPIRE (a tie goes to the own event).  floor: now_ns for the snapshot's rows.
+__host__ __device__ inline DrainFin kb_exec_clip(DrainFin f, i64 A, int32_t max_s, int32_t acc_s, i64 floor) {
+  if (max_s <= 0) return f;
+  i64 dl = kb_exec_deadline(A, max_s, acc_s);
+  dl = dl < A ? A : dl;
+  dl = dl < floor ? floor : dl;
+  return dl < f.fin ? DrainFin{dl, KB_PH_EXPIRE} : f;
 }
 
 // ---- resource.Quantity in the int64Amount form (value * 10^scale), as AdmissionFairSharing sums it -----------------
@@ -247,6 +269,21 @@ __host__ __device__ inline bool afs_decay(i64 *cons, int32_t *scale, const i64 *
   return ok;
 }
 
+// The admitted-row columns: one half of the double buffer k_drain_compact copies the live rows between ([A_cap] each).
+// The first nine are the DevSnap's admitted tables (the first half borrows those upload_impl laid out); every other
+// column exists with its block and is null otherwise.
+struct AdmRows {
+  int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty;
+  int32_t *wl;        // pending record of the row, -1 = none (eviction replay or event mode)
+  i64 *finish;        // finish time, INT64_MAX = never (event mode); phase says what it holds
+  int32_t *lq;        // LocalQueue, -1 = none (decay)
+  uint8_t *evicting;  // 1 while the row's eviction is under way, its end in finish (eviction latency)
+  uint8_t *phase;     // KB_PH_*: what finish holds (admission checks, WaitForPodsReady, MaximumExecutionTimeSeconds)
+  i64 *since;         // Admitted time, INT64_MIN while the checks run (MaximumExecutionTimeSeconds)
+  i64 *rc_next;       // time of the row's next reclaim step, INT64_MAX = none (reclaim steps)
+  int32_t *rc_cur;    // index of that step
+};
+
 struct DrainDev {
   // queues
   int32_t *q_order, *q_start, *cursor; uint8_t *wl_state;  // wl_state: KB_WS_* per pending workload
@@ -259,11 +296,10 @@ struct DrainDev {
   int32_t *trace_wl; uint8_t *trace_dec; long long trace_off, trace_cap;
   // mutable views of the snapshot tables
   i64 *cq_usage, *wl_last_gen; int8_t *ps_last_tried;
-  int32_t *adm_cq, *adm_priority; i64 *adm_ts, *adm_qr_ts, *adm_uid; uint8_t *adm_evicted; int32_t *adm_use_start, *adm_use_fr; i64 *adm_use_qty;
+  AdmRows adm;       // the admitted rows (current half)
   int A, AU, cycle;  // admitted workloads / usage cells before this cycle's admissions
   int A_cap, AU_cap; // capacity of the admitted tables (rows / usage cells)
-  // eviction replay; adm_wl == nullptr: off
-  int32_t *adm_wl;                 // [A_cap] pending record of each admitted row (current half)
+  // eviction replay; adm.wl == nullptr: off
   int32_t *wl_seg, *wl_pos;        // [W] segment of a pending workload / its position in the segment
   int32_t *adm_dead;               // [A_cap] cycle + 1 when the row was evicted in that cycle
   int32_t *root_mark;              // [nRoots] cycle + 1 when the root cohort tree had a victim in that cycle
@@ -285,11 +321,9 @@ struct DrainDev {
   // decay of consumed usage (event mode); lq_last == nullptr: off
   i64 *lq_last;               // [n_lq] LastUpdate of the consumed usage
   i64 *lq_adm;                // [n_lq][R] admitted usage in library units: cells of the LocalQueue's live rows
-  int32_t *adm_lq;            // [A_cap] LocalQueue of each admitted row (current half), -1 = none
   unsigned long long *afs_samples;  // [1] samples taken
   i64 half_life_ns, sampling_ns;
-  // event mode; adm_finish == nullptr: off
-  i64 *adm_finish;                 // [A_cap] finish time of each admitted row (current half), INT64_MAX = never
+  // event mode; adm.finish == nullptr: off
   const i64 *wl_run;               // [W] run time once admitted (< 0 never finishes); null = none finishes
   i64 *wl_admit_ns, *wl_finish_ns; // [W]
   i64 *clock;                      // [0] t_{c+1} of the boundary, [1] E (INT64_MAX = none; reset by k_drain_ev_next)
@@ -301,7 +335,6 @@ struct DrainDev {
   uint8_t *class_nofit;            // [classes] in the ClusterQueue's NoFit set; null = no arrivals or no hashes
   // eviction latency (event mode); wl_evict == nullptr: off
   const i64 *wl_evict;             // [W] time from a workload's eviction until its quota is released
-  uint8_t *adm_evicting;           // [A_cap] 1 while the row's eviction is under way (current half); its end is adm_finish
   // sticky workload; cq_sticky == nullptr: off
   int32_t *cq_sticky;              // [Q] pending index of each ClusterQueue's sticky workload, -1 = none
   // admission checks (event mode); wl_check == nullptr: off
@@ -312,18 +345,16 @@ struct DrainDev {
   i64 *wl_sort_ts;                 // [W] the keys the current order was built with
   i64 *wl_requeue_at;              // [W] RequeueAt of a BACKOFF record
   i64 *wl_ready_ns; uint8_t *wl_deactivated;  // [W]
-  uint8_t *adm_phase;              // [A_cap] KB_PH_* of each row (current half); also with WaitForPodsReady
   i64 check_base_s, check_max_s; int check_limit;
   // WaitForPodsReady (event mode; the requeue state above is allocated with it); wl_pr == nullptr: off
   const i64 *wl_pr;                // [W] Admitted -> PodsReady delay of a ready attempt
   int32_t *wl_pr_fail, *wl_pr_count;  // [W] failures left (INT32_MAX = all) / RequeueState.Count
   i64 *wl_pr_at, *wl_pr_prev;      // [W] PodsReady time of the last attempt that reaches it / the value before it
   i64 pr_timeout, pr_base_s, pr_max_s; int pr_limit, pr_creation;
-  // MaximumExecutionTimeSeconds (event mode; adm_phase and wl_deactivated are allocated with it); wl_max_exec == nullptr:
+  // MaximumExecutionTimeSeconds (event mode; adm.phase and wl_deactivated are allocated with it); wl_max_exec == nullptr:
   // off.  wl_deactivated then holds the reason (KB_DR_*).
   const int32_t *wl_max_exec;      // [W] limit in seconds, 0 = nil
   int32_t *wl_exec_acc;            // [W] accumulated seconds, -1 = nil
-  i64 *adm_exec_since;             // [A_cap] Admitted time of each row (current half), INT64_MIN while its checks run
   // quota changes (event mode); qc_ns == nullptr: off.  The host works out which edits change nothing, the root and
   // the tree of every other one (the rows change only through the edits, in table order).
   const i64 *qc_ns;                // [n_qc] edit times, non-decreasing
@@ -354,14 +385,8 @@ struct DrainDev {
   int32_t *ps_adm_cnt;             // [P] the held row's PodSetAssignment.Count
   int8_t *ps_adm_fl;               // [P][R] its flavors, -1 = none
   i64 *ps_adm_use;                 // [P][R] its ResourceUsage
-  i64 *adm_rc_next;                // [A_cap] time of each row's next step (current half), INT64_MAX = none
-  int32_t *adm_rc_cur;             // [A_cap] index of that step (current half)
   const int32_t *rc_blob_gen;      // [Q] byte offset of the ClusterQueue's generation in tree_blob, -1 = not in a tree
 };
-// adm_phase: what the finish column of a row holds.  RUN: its finish (or its eviction's end when adm_evicting); CHECK: its
-// checks' verdict; WAIT: the timeout T of a PodsReady attempt that fails; TIMED_OUT: the end of its eviction by that
-// timeout or by an expiry; EXPIRE: its effective MaximumExecutionTimeSeconds deadline, which comes before its own event
-enum { KB_PH_RUN = 0, KB_PH_CHECK = 1, KB_PH_WAIT = 2, KB_PH_TIMED_OUT = 3, KB_PH_EXPIRE = 4 };
 // wl_deactivated: 0, or the reason a record was deactivated (kb_drain_out.wl_deactivation_reason)
 enum { KB_DR_REJECTED = 1, KB_DR_REQUEUING_LIMIT = 2, KB_DR_MAX_EXEC = 3, KB_DR_USER = 4 };
 // counters of a boundary: [1] evictions (issued, with latency), [2] / [3] rows / cells after the compaction, [4]
@@ -395,13 +420,16 @@ __global__ void k_drain_keys_ts(DevSnap D, const int32_t *vals, u64 *keys) {
   if (i >= D.W) return;
   keys[i] = (u64)D.wl_ts[vals[i]] ^ 0x8000000000000000ull;
 }
-// third pass: (segment | priority desc); the segment is the ClusterQueue unless its queue is split by LocalQueue
+// the segment of workload w: its ClusterQueue's, or its LocalQueue's where the ClusterQueue's queue is split by LocalQueue
+__device__ __forceinline__ int drain_wl_seg(const DevSnap &D, const DrainDev &X, int w) {
+  const int cq = D.wl_cq[w];
+  return (X.seg_start && X.cq_afs[cq]) ? X.lq_seg[X.wl_lq[w]] : drain_seg0(X, cq);
+}
+// third pass: (segment | priority desc)
 __global__ void k_drain_keys_cq(DevSnap D, DrainDev X, const int32_t *vals, u64 *keys, int32_t *q_count) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= D.W) return;
-  int w = vals[i];
-  int cq = D.wl_cq[w];
-  int seg = (X.seg_start && X.cq_afs[cq]) ? X.lq_seg[X.wl_lq[w]] : drain_seg0(X, cq);
+  const int w = vals[i], seg = drain_wl_seg(D, X, w);
   keys[i] = ((u64)seg << 32) | (u64)(~((unsigned)D.wl_priority[w] ^ 0x80000000u));  // higher priority first
   atomicAdd(&q_count[seg], 1);
 }
@@ -416,22 +444,23 @@ __global__ void k_drain_init(DevSnap D, DrainDev X, int S) {
 // replay: the records named by adm_wl hold quota (out of every queue); segment and position of every workload
 __global__ void k_drain_init_replay(DevSnap D, DrainDev X, int n_adm) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n_adm) X.wl_state[X.adm_wl[i]] = KB_WS_HELD;
+  if (i < n_adm) X.wl_state[X.adm.wl[i]] = KB_WS_HELD;
   if (i < D.W) {
-    const int w = X.q_order[i];
-    const int cq = D.wl_cq[w];
-    const int seg = (X.seg_start && X.cq_afs[cq]) ? X.lq_seg[X.wl_lq[w]] : drain_seg0(X, cq);
+    const int w = X.q_order[i], seg = drain_wl_seg(D, X, w);
     X.wl_seg[w] = seg; X.wl_pos[w] = i - X.q_start[seg];
   }
 }
-// the cursor of every segment at its first QUEUED workload (the start of a drain)
-__global__ void k_drain_advance(DrainDev X, int S) {
-  int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s >= S) return;
+// the cursor of segment s past the workloads that left the queue, at its first QUEUED one
+__device__ __forceinline__ void drain_advance(const DrainDev &X, int s) {
   const int qs = X.q_start[s], qn = X.q_start[s + 1] - qs;
   int cur = X.cursor[s];
   while (cur < qn && X.wl_state[X.q_order[qs + cur]] != KB_WS_QUEUED) cur++;
   X.cursor[s] = cur;
+}
+// every segment's cursor (the start of a drain, after a re-sort or the edits of a boundary)
+__global__ void k_drain_advance(DrainDev X, int S) {
+  int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s < S) drain_advance(X, s);
 }
 
 // heads of the next cycle (queues.Heads manager.go:770-794): one per ClusterQueue with work left, in ClusterQueue order.
@@ -562,54 +591,33 @@ __global__ void k_drain_apply(DevSnap D, DrainDev X) {
     }
   }
   if (inadmissible && !strict) { X.wl_state[wl] = KB_WS_SET_ASIDE; X.first_aside[hs] = min(X.first_aside[hs], hp); }
-  for (int s = s0; s < s1; s++) {  // the cursor past the workloads that left the queue, the head among them
-    if (s != hs && !bulk) continue;
-    const int qs = X.q_start[s], qn = X.q_start[s + 1] - qs;
-    int cur = X.cursor[s];
-    while (cur < qn && X.wl_state[X.q_order[qs + cur]] != KB_WS_QUEUED) cur++;
-    X.cursor[s] = cur;
-  }
+  for (int s = s0; s < s1; s++)  // the cursor past the workloads that left the queue, the head among them
+    if (s == hs || bulk) drain_advance(X, s);
 }
 
-__device__ __forceinline__ i64 drain_sat_add(i64 t, i64 d) { return t > INT64_MAX - d ? INT64_MAX : t + d; }  // d >= 0
-// WaitForPodsReady: the attempt of row a (record w) Admitted at t.  A failing one (failures left, or a delay past the
-// timeout) waits for its timeout T = t + timeout in the finish column; a ready one reaches PodsReady at t + delay, and
-// its finish is PodsReady + run (run < 0 never finishes).  Returns the finish column's value.
-__device__ __forceinline__ i64 drain_pr_attempt(const DrainDev &X, int a, int w, i64 t) {
-  const i64 d = X.wl_pr[w];
-  if (X.wl_pr_fail[w] > 0 || d > X.pr_timeout) { X.adm_phase[a] = KB_PH_WAIT; return drain_sat_add(t, X.pr_timeout); }
-  const i64 at = drain_sat_add(t, d), run = X.wl_run ? X.wl_run[w] : -1;
-  X.adm_phase[a] = KB_PH_RUN;
-  X.wl_pr_prev[w] = X.wl_pr_at[w]; X.wl_pr_at[w] = at;
-  return run < 0 ? INT64_MAX : drain_sat_add(at, run);
+// RequeueState cleared: Count 0, no RequeueAt
+__device__ __forceinline__ void drain_clear_requeue(const DrainDev &X, int w) {
+  if (X.wl_pr) X.wl_pr_count[w] = 0;
+  if (X.wl_requeue_at) X.wl_requeue_at[w] = INT64_MIN;
 }
-// MaximumExecutionTimeSeconds: the deadline D = A + (max - acc) s of record w Admitted at A, saturating both ways
-__device__ __forceinline__ i64 drain_exec_deadline(const DrainDev &X, int w, i64 A) {
-  return kb_exec_deadline(A, X.wl_max_exec[w], X.wl_exec_acc[w]);
+// a PodsReady attempt of record w still waiting at t is dropped: not counted, no failure used
+__device__ __forceinline__ void drain_drop_attempt(const DrainDev &X, int w, i64 t) {
+  if (X.wl_pr && X.wl_pr_at[w] > t) X.wl_pr_at[w] = X.wl_pr_prev[w];
 }
-// row a (record w) Admitted at A with its own next event at fin: the effective deadline max(D, A) when it comes first,
-// with the row marked KB_PH_EXPIRE (a tie goes to the own event).  The host applies max(., now_ns) to the snapshot's rows.
-__device__ __forceinline__ i64 drain_exec_clip(const DrainDev &X, int a, int w, i64 A, i64 fin) {
-  if (X.wl_max_exec[w] <= 0) return fin;
-  const i64 dl = max(drain_exec_deadline(X, w, A), A);
-  if (dl >= fin) return fin;
-  X.adm_phase[a] = KB_PH_EXPIRE;
-  return dl;
-}
-// deactivation for MaximumExecutionTimeExceeded: acc nil, RequeueState cleared (Count 0; a BACKOFF-bound record is
-// DEACTIVATED at its release instead)
+// deactivation for MaximumExecutionTimeExceeded: acc nil, RequeueState cleared (a BACKOFF-bound record is DEACTIVATED
+// at its release instead)
 __device__ __forceinline__ void drain_exec_deactivate(const DrainDev &X, int w) {
   X.wl_deactivated[w] = KB_DR_MAX_EXEC;
   X.wl_exec_acc[w] = -1;
-  if (X.wl_pr) X.wl_pr_count[w] = 0;
+  drain_clear_requeue(X, w);
   atomicAdd(&X.counters[KB_DC_EXEC_DEACTIVATED], 1);
 }
 // release at t of row a (record w): with an Admitted time, a deadline at or before t deactivates a record not
 // deactivated yet (rule 4), then the attempt's seconds join acc.  Returns whether it deactivated the record.
 __device__ __forceinline__ bool drain_exec_release(const DrainDev &X, int a, int w, i64 t) {
-  const i64 A = X.adm_exec_since[a];
+  const i64 A = X.adm.since[a];
   if (A == INT64_MIN) return false;
-  const bool deact = X.wl_max_exec[w] > 0 && X.wl_deactivated[w] == 0 && drain_exec_deadline(X, w, A) <= t;
+  const bool deact = X.wl_max_exec[w] > 0 && X.wl_deactivated[w] == 0 && kb_exec_deadline(A, X.wl_max_exec[w], X.wl_exec_acc[w]) <= t;
   if (deact) drain_exec_deactivate(X, w);
   const i64 d = kb_exec_seconds(t - A), acc = X.wl_exec_acc[w];
   const i64 sum = acc < 0 ? d : acc + d;
@@ -622,23 +630,23 @@ __device__ __forceinline__ bool drain_exec_release(const DrainDev &X, int a, int
 // the run of row a (record w) starts at S: its steps replay from the first
 __device__ __forceinline__ void drain_rc_begin(const DrainDev &X, int a, int w, i64 S) {
   const int i = X.wl_rc_start[w];
-  X.adm_rc_cur[a] = i;
-  X.adm_rc_next[a] = i < X.wl_rc_start[w + 1] ? drain_sat_add(S, X.rc_after[i]) : INT64_MAX;
+  X.adm.rc_cur[a] = i;
+  X.adm.rc_next[a] = i < X.wl_rc_start[w + 1] ? drain_sat_add(S, X.rc_after[i]) : INT64_MAX;
 }
-// row a can take a step: not evicting, phase running (its run started: adm_rc_next is INT64_MAX otherwise)
+// row a can take a step: not evicting, phase running (its run started: adm.rc_next is INT64_MAX otherwise)
 __device__ __forceinline__ bool drain_rc_live(const DrainDev &X, int a) {
-  if (X.adm_evicting && X.adm_evicting[a]) return false;
-  return !X.adm_phase || X.adm_phase[a] == KB_PH_RUN || X.adm_phase[a] == KB_PH_EXPIRE;
+  if (X.adm.evicting && X.adm.evicting[a]) return false;
+  return !X.adm.phase || X.adm.phase[a] == KB_PH_RUN || X.adm.phase[a] == KB_PH_EXPIRE;
 }
 // the steps of running row a due at or before lim, in time order (rule 4 of kb_run_drain): a step that lowers podset p
 // from c to r scales the record's requests to r pods and the row's usage of p to U0 / n * min(r, n) per resource; the
 // difference leaves the row's cells, the ClusterQueue usage and the LocalQueue's admitted usage (integer atomics).  The
 // steps of one instant are one update: generation + 1 (the cycle's copy and the tree block's), root tree marked.
 __device__ void drain_reclaim(const DevSnap &D, const DrainDev &X, int a, i64 lim) {
-  i64 t = X.adm_rc_next[a];
+  i64 t = X.adm.rc_next[a];
   if (t > lim) return;
-  const int w = X.adm_wl[a], cq = X.adm_cq[a], R = D.R, i1 = X.wl_rc_start[w + 1];
-  int i = X.adm_rc_cur[a], n = 0;
+  const int w = X.adm.wl[a], cq = X.adm.cq[a], R = D.R, i1 = X.wl_rc_start[w + 1];
+  int i = X.adm.rc_cur[a], n = 0;
   const i64 S = t - X.rc_after[i];  // t <= lim < INT64_MAX: not saturated
   int32_t *cnt = const_cast<int32_t *>(D.ps_count);
   i64 *req = const_cast<i64 *>(D.ps_req), *hash = const_cast<i64 *>(D.wl_sched_hash);
@@ -655,11 +663,11 @@ __device__ void drain_reclaim(const DevSnap &D, const DrainDev &X, int a, i64 li
         const i64 u = X.ps_adm_use[(size_t)p * R + r] / na, d = u * min(rem, na) - u * min(c, na);
         if (d == 0) continue;
         const int fr = f * R + r;
-        for (int k = X.adm_use_start[a]; k < X.adm_use_start[a + 1]; k++)
-          if (X.adm_use_fr[k] == fr) { X.adm_use_qty[k] += d; break; }
+        for (int k = X.adm.use_start[a]; k < X.adm.use_start[a + 1]; k++)
+          if (X.adm.use_fr[k] == fr) { X.adm.use_qty[k] += d; break; }
         atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + fr], (unsigned long long)d);
-        if (X.lq_last && X.adm_lq[a] >= 0 && X.cq_afs[cq])
-          atomicAdd((unsigned long long *)&X.lq_adm[(size_t)X.adm_lq[a] * R + r], (unsigned long long)d);
+        if (X.lq_last && X.adm.lq[a] >= 0 && X.cq_afs[cq])
+          atomicAdd((unsigned long long *)&X.lq_adm[(size_t)X.adm.lq[a] * R + r], (unsigned long long)d);
       }
       cnt[p] = rem;
       if (hash) { hash[w] = X.rc_hash ? X.rc_hash[i] : 0; if (X.wl_class) X.wl_class[w] = X.rc_class[i]; }
@@ -673,10 +681,33 @@ __device__ void drain_reclaim(const DevSnap &D, const DrainDev &X, int a, i64 li
     }
     t = i < i1 ? drain_sat_add(S, X.rc_after[i]) : INT64_MAX;
   }
-  X.adm_rc_cur[a] = i; X.adm_rc_next[a] = t;
+  X.adm.rc_cur[a] = i; X.adm.rc_next[a] = t;
   if (n) atomicAdd(&X.counters[KB_DC_RECLAIMS], n);
 }
 
+// row a (record w) is Admitted at t (the reservation without a check delay, or a Ready verdict): the run clock or the
+// PodsReady attempt starts (kb_pr_attempt; a ready one moves the PodsReady time), the reclaim steps with the run (at
+// PodsReady of a ready attempt), and the MaximumExecutionTimeSeconds deadline may come first
+__device__ __forceinline__ void drain_admitted(const DrainDev &X, int a, int w, i64 t) {
+  if (X.wl_ready_ns) X.wl_ready_ns[w] = t;
+  const i64 run = X.wl_run ? X.wl_run[w] : -1;
+  DrainFin f{run < 0 ? INT64_MAX : drain_sat_add(t, run), KB_PH_RUN};
+  if (X.wl_pr) {
+    const i64 d = X.wl_pr[w];
+    f = kb_pr_attempt(t, d, X.wl_pr_fail[w] > 0, X.pr_timeout, run);
+    if (f.ph == KB_PH_RUN) { X.wl_pr_prev[w] = X.wl_pr_at[w]; X.wl_pr_at[w] = drain_sat_add(t, d); }
+  }
+  if (X.wl_rc_start) {
+    if (f.ph == KB_PH_RUN) drain_rc_begin(X, a, w, X.wl_pr ? X.wl_pr_at[w] : t);
+    else X.adm.rc_next[a] = INT64_MAX;
+  }
+  if (X.wl_max_exec) {
+    X.adm.since[a] = t;
+    f = kb_exec_clip(f, t, X.wl_max_exec[w], X.wl_exec_acc[w], INT64_MIN);
+  }
+  if (X.adm.phase) X.adm.phase[a] = f.ph;
+  X.adm.finish[a] = f.fin;
+}
 // admitted entries join the admitted tables (cache.AssumeWorkload), appended at X.A / X.AU, and the ClusterQueue usage
 __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
   int e = blockIdx.x * blockDim.x + threadIdx.x;
@@ -686,37 +717,23 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
   int a = X.A + X.e_adm_off[e];
   int c0 = X.AU + X.e_cell_off[e];
   if (a >= X.A_cap || c0 + X.e_ncells[e] > X.AU_cap) { atomicOr(&X.counters[KB_DC_FULL], 1); return; }  // nothing past the end
-  if (X.adm_wl) X.adm_wl[a] = wl;
-  if (X.adm_lq) X.adm_lq[a] = X.wl_lq[wl];
-  X.adm_cq[a] = cq; X.adm_priority[a] = D.wl_priority[wl]; X.adm_ts[a] = X.wl_ts0 ? X.wl_ts0[wl] : D.wl_ts[wl]; X.adm_qr_ts[a] = qr_ts;
-  X.adm_uid[a] = D.wl_uid[wl]; X.adm_evicted[a] = 0;
-  if (X.adm_evicting) X.adm_evicting[a] = 0;
-  X.adm_use_start[a] = c0;
-  if (X.adm_finish) {  // finish = QuotaReserved time + run time, saturating; run < 0 never finishes
-    const i64 run = X.wl_run ? X.wl_run[wl] : -1;
-    i64 fin = run < 0 ? INT64_MAX : (qr_ts > INT64_MAX - run ? INT64_MAX : qr_ts + run);
-    if (X.wl_qts) {  // checks or PodsReady: the reservation resets Evicted; a check delay starts an attempt, 0 is Ready at once
-      X.wl_qts[wl] = X.wl_ts0[wl];
-      const i64 chk = X.wl_check ? X.wl_check[wl] : 0;
-      X.adm_phase[a] = chk > 0 ? KB_PH_CHECK : KB_PH_RUN;
-      if (chk > 0) fin = qr_ts > INT64_MAX - chk ? INT64_MAX : qr_ts + chk;
-      else {
-        X.wl_ready_ns[wl] = qr_ts;
-        if (X.wl_pr) fin = drain_pr_attempt(X, a, wl, qr_ts);  // Admitted now: the PodsReady attempt starts
-      }
+  if (X.adm.wl) X.adm.wl[a] = wl;
+  if (X.adm.lq) X.adm.lq[a] = X.wl_lq[wl];
+  X.adm.cq[a] = cq; X.adm.priority[a] = D.wl_priority[wl]; X.adm.ts[a] = X.wl_ts0 ? X.wl_ts0[wl] : D.wl_ts[wl]; X.adm.qr_ts[a] = qr_ts;
+  X.adm.uid[a] = D.wl_uid[wl]; X.adm.evicted[a] = 0;
+  if (X.adm.evicting) X.adm.evicting[a] = 0;
+  X.adm.use_start[a] = c0;
+  if (X.adm.finish) {  // checks or PodsReady: the reservation resets Evicted; a check delay starts an attempt, 0 is Ready at once
+    if (X.wl_qts) X.wl_qts[wl] = X.wl_ts0[wl];
+    const i64 chk = X.wl_check ? X.wl_check[wl] : 0;
+    if (chk > 0) {  // not Admitted while the checks run: the verdict time in the finish column
+      X.adm.phase[a] = KB_PH_CHECK;
+      X.adm.finish[a] = drain_sat_add(qr_ts, chk);
+      if (X.wl_rc_start) X.adm.rc_next[a] = INT64_MAX;
+      if (X.wl_max_exec) X.adm.since[a] = INT64_MIN;
+    } else {
+      drain_admitted(X, a, wl, qr_ts);
     }
-    if (X.wl_rc_start) {  // the run starts now, or at PodsReady of a ready attempt; not while the checks run
-      const bool run = !(X.wl_check && X.wl_check[wl] > 0) && (!X.wl_pr || X.adm_phase[a] == KB_PH_RUN);
-      if (run) drain_rc_begin(X, a, wl, X.wl_pr ? X.wl_pr_at[wl] : qr_ts);
-      else X.adm_rc_next[a] = INT64_MAX;
-    }
-    if (X.wl_max_exec) {  // Admitted now unless the checks run: the deadline may come first
-      const bool checking = X.wl_check && X.wl_check[wl] > 0;
-      if (!X.wl_qts) X.adm_phase[a] = KB_PH_RUN;
-      X.adm_exec_since[a] = checking ? INT64_MIN : qr_ts;
-      if (!checking) fin = drain_exec_clip(X, a, wl, qr_ts, fin);
-    }
-    X.adm_finish[a] = fin;
     X.wl_admit_ns[wl] = qr_ts;
   }
   const bool covers_pods = drain_covers_pods(D, cq);
@@ -734,12 +751,12 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
       int fr = f * R + r;
       i64 q = drain_request(D, row, r, D.ps_count_out[row], covers_pods);
       int j = 0;
-      while (j < n && X.adm_use_fr[c0 + j] != fr) j++;
-      if (j == n) { X.adm_use_fr[c0 + n] = fr; X.adm_use_qty[c0 + n] = 0; n++; }
-      X.adm_use_qty[c0 + j] += q;
+      while (j < n && X.adm.use_fr[c0 + j] != fr) j++;
+      if (j == n) { X.adm.use_fr[c0 + n] = fr; X.adm.use_qty[c0 + n] = 0; n++; }
+      X.adm.use_qty[c0 + j] += q;
     }
-  X.adm_use_start[a + 1] = c0 + n;
-  for (int j = 0; j < n; j++) X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c0 + j]] += X.adm_use_qty[c0 + j];  // one entry per ClusterQueue
+  X.adm.use_start[a + 1] = c0 + n;
+  for (int j = 0; j < n; j++) X.cq_usage[(size_t)cq * D.FR + X.adm.use_fr[c0 + j]] += X.adm.use_qty[c0 + j];  // one entry per ClusterQueue
   if (X.seg_start && X.cq_afs[cq]) {
     // entry penalty (scheduler.go:727-742,946-960; CalculateEntryPenalty + MulByFloat): per resource of SumTotalRequests
     // (the full TotalRequests, partial admission does not reduce it), int64(float64(MilliValue) * alpha) milli-units,
@@ -754,7 +771,7 @@ __global__ void k_drain_admit(DevSnap D, DrainDev X, i64 qr_ts) {
     bool bad = false;
     if (X.lq_last) {
       i64 *adm = X.lq_adm + (size_t)lq * R;
-      for (int j = 0; j < n; j++) adm[X.adm_use_fr[c0 + j] % R] += X.adm_use_qty[c0 + j];
+      for (int j = 0; j < n; j++) adm[X.adm.use_fr[c0 + j] % R] += X.adm.use_qty[c0 + j];
       bool changed = false;
       bad |= !afs_decay(cons, csc, adm, X.milli_mul, afs_alpha_of(qr_ts - X.lq_last[lq], X.half_life_ns), R, &changed);
       X.lq_last[lq] = qr_ts;
@@ -786,11 +803,46 @@ __device__ __forceinline__ void drain_forget(const DevSnap &D, const DrainDev &X
   if (X.wl_has_qr) X.wl_has_qr[w] = 0;
   X.wl_admit_cycle[w] = -1;
 }
+// a record entering its queue with a queue-order timestamp other than the key its position was sorted by stamps the
+// boundary for a re-sort
+__device__ __forceinline__ void drain_mark_resort(const DrainDev &X, int w) {
+  if (X.wl_sort_ts && X.wl_sort_ts[w] != X.wl_qts[w]) X.counters[KB_DC_RESORT] = X.cycle + 1;
+}
 __device__ __forceinline__ void drain_release(const DevSnap &D, const DrainDev &X, int w) {
   X.wl_state[w] = KB_WS_QUEUED;
   drain_forget(D, X, w);
   atomicMin(&X.cursor[X.wl_seg[w]], X.wl_pos[w]);
-  if (X.wl_sort_ts && X.wl_sort_ts[w] != X.wl_qts[w]) X.counters[KB_DC_RESORT] = X.cycle + 1;
+  drain_mark_resort(X, w);
+}
+// record w joins its queue (PushOrUpdate, cluster_queue.go:288-293): the cursor moves back to it, or in a BestEffortFIFO
+// ClusterQueue a known hash in the NoFit set sets it aside
+__device__ __forceinline__ void drain_enqueue(const DrainDev &X, int w) {
+  const int s = X.wl_seg[w], p = X.wl_pos[w];
+  if (X.class_nofit && X.wl_class[w] >= 0 && X.class_nofit[X.wl_class[w]]) {
+    X.wl_state[w] = KB_WS_SET_ASIDE;
+    atomicMin(&X.first_aside[s], p);
+  } else {
+    X.wl_state[w] = KB_WS_QUEUED;
+    atomicMin(&X.cursor[s], p);
+  }
+}
+// the cells of row a leave its ClusterQueue's usage (cache.DeleteWorkload) and, with lq and decay, its LocalQueue's
+// admitted usage: integer atomics, the order does not matter (several rows of one LocalQueue can go together).  lq is
+// false where no AFS row can be: evictions (AFS drains cannot preempt) and check verdicts (checks exclude decay).
+__device__ __forceinline__ void drain_uncharge(const DevSnap &D, const DrainDev &X, int a, bool lq) {
+  const int cq = X.adm.cq[a], c0 = X.adm.use_start[a], c1 = X.adm.use_start[a + 1];
+  for (int c = c0; c < c1; c++)
+    atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm.use_fr[c]], (unsigned long long)(-X.adm.use_qty[c]));
+  if (lq && X.lq_last && X.adm.lq[a] >= 0 && X.cq_afs[cq]) {
+    i64 *adm = X.lq_adm + (size_t)X.adm.lq[a] * D.R;
+    for (int c = c0; c < c1; c++) atomicAdd((unsigned long long *)&adm[X.adm.use_fr[c] % D.R], (unsigned long long)(-X.adm.use_qty[c]));
+  }
+}
+// row a (record w) becomes an evicting row at t0: it holds its cells until t0 + latency
+__device__ __forceinline__ void drain_evict_row(const DrainDev &X, int a, int w, i64 t0) {
+  X.adm.evicted[a] = 1;
+  X.adm.evicting[a] = 1;
+  X.adm.finish[a] = drain_sat_add(t0, X.wl_evict[w]);
 }
 // sets byte i of a byte column (256-byte aligned, padded) and returns whether it was set: atomicOr on its aligned word
 __device__ __forceinline__ bool drain_claim_byte(uint8_t *col, int i) {
@@ -798,8 +850,7 @@ __device__ __forceinline__ bool drain_claim_byte(uint8_t *col, int i) {
   const unsigned bit = 1u << (8 * (unsigned)(p & 3));
   return (atomicOr((unsigned *)(p & ~(uintptr_t)3), bit) & bit) != 0;
 }
-// every target of every Preempting entry (thread per entry): cells out of its ClusterQueue's usage (integer atomics:
-// the order does not matter), row dead, pending record QUEUED with LastAssignment nil, its root tree marked.  With
+// every target of every Preempting entry (thread per entry): cells out of its ClusterQueue's usage, row dead, pending record QUEUED with LastAssignment nil, its root tree marked.  With
 // latency (wl_evict) the eviction is only issued: a row not evicting yet is claimed once, gets adm_evicted and its end
 // time t_c + latency (saturating) in its finish column, and keeps its cells and its record; k_drain_finish releases it.
 __global__ void k_drain_evict(DevSnap D, DrainDev X) {
@@ -808,32 +859,24 @@ __global__ void k_drain_evict(DevSnap D, DrainDev X) {
   const int stamp = X.cycle + 1;
   const int off = D.tgt_off[e], n = D.tgt_cnt[e];
   for (int k = 0; k < n; k++) {
-    const int a = D.tgt_pool_adm[off + k];
+    const int a = D.tgt_pool_adm[off + k], w = X.adm.wl[a];
     if (X.wl_evict) {
-      if (drain_claim_byte(X.adm_evicting, a)) continue;  // under way: "Preemption ongoing" (preemption.go:183-186)
-      const int w = X.adm_wl[a];
-      const i64 lat = X.wl_evict[w];
-      X.adm_evicted[a] = 1;
-      X.adm_finish[a] = D.now_ns > INT64_MAX - lat ? INT64_MAX : D.now_ns + lat;
-      if (X.adm_phase) {  // checks running: no pods, the next boundary; a PodsReady attempt waiting for T is dropped
-        if (X.adm_phase[a] == KB_PH_CHECK) X.adm_finish[a] = D.now_ns;
-        X.adm_phase[a] = KB_PH_RUN;
+      if (drain_claim_byte(X.adm.evicting, a)) continue;  // under way: "Preemption ongoing" (preemption.go:183-186)
+      X.adm.evicted[a] = 1;
+      X.adm.finish[a] = drain_sat_add(D.now_ns, X.wl_evict[w]);
+      if (X.adm.phase) {  // checks running: no pods, the next boundary; a PodsReady attempt waiting for T is dropped
+        if (X.adm.phase[a] == KB_PH_CHECK) X.adm.finish[a] = D.now_ns;
+        X.adm.phase[a] = KB_PH_RUN;
       }
-      if (X.wl_pr && X.wl_pr_at[w] > D.now_ns) X.wl_pr_at[w] = X.wl_pr_prev[w];  // dropped before PodsReady
-      X.wl_evictions[w]++;
-      atomicAdd(&X.counters[KB_DC_EVICTED], 1);
-      continue;
+    } else {
+      if (atomicExch(&X.adm_dead[a], stamp) == stamp) continue;  // one eviction per row
+      drain_uncharge(D, X, a, false);
+      if (X.wl_max_exec && drain_exec_release(X, a, w, D.now_ns)) { drain_forget(D, X, w); X.wl_state[w] = KB_WS_DEACTIVATED; }
+      else drain_release(D, X, w);
+      X.root_mark[D.root_slot[X.adm.cq[a]]] = stamp;
     }
-    if (atomicExch(&X.adm_dead[a], stamp) == stamp) continue;  // one eviction per row
-    const int cq = X.adm_cq[a];
-    for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)  // cache.DeleteWorkload
-      atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
-    const int w = X.adm_wl[a];
-    if (X.wl_max_exec && drain_exec_release(X, a, w, D.now_ns)) { drain_forget(D, X, w); X.wl_state[w] = KB_WS_DEACTIVATED; }
-    else drain_release(D, X, w);
-    if (X.wl_pr && X.wl_pr_at[w] > D.now_ns) X.wl_pr_at[w] = X.wl_pr_prev[w];  // dropped before PodsReady
+    drain_drop_attempt(X, w, D.now_ns);  // dropped before PodsReady
     X.wl_evictions[w]++;  // a workload holds at most one row: one writer
-    X.root_mark[D.root_slot[cq]] = stamp;
     atomicAdd(&X.counters[KB_DC_EVICTED], 1);
   }
 }
@@ -857,35 +900,40 @@ __global__ void k_drain_live(DrainDev X, int bound, const int32_t *n_new) {
   if (a > bound) return;
   const bool live = a < bound && a < X.A + (n_new ? *n_new : 0) && !X.counters[KB_DC_FULL] && X.adm_dead[a] != X.cycle + 1;
   X.row_live[a] = live;
-  X.row_cells[a] = live ? X.adm_use_start[a + 1] - X.adm_use_start[a] : 0;
+  X.row_cells[a] = live ? X.adm.use_start[a + 1] - X.adm.use_start[a] : 0;
 }
-struct AdmTabs { int32_t *cq, *priority; i64 *ts, *qr_ts, *uid; uint8_t *evicted; int32_t *use_start, *use_fr; i64 *use_qty; int32_t *wl; i64 *finish; int32_t *lq; uint8_t *evicting, *phase; i64 *since, *rc_next; int32_t *rc_cur; };
-// live rows of [0, bound), in order, into the other half of the double buffer; thread bound writes the totals
-__global__ void k_drain_compact(DrainDev X, AdmTabs O, int bound) {
+// row a of I into row n of O, its cells excepted (the caller moves them and writes O.use_start)
+__device__ __forceinline__ void drain_copy_row(const AdmRows &I, int a, const AdmRows &O, int n) {
+  O.cq[n] = I.cq[a]; O.priority[n] = I.priority[a]; O.ts[n] = I.ts[a]; O.qr_ts[n] = I.qr_ts[a];
+  O.uid[n] = I.uid[a]; O.evicted[n] = I.evicted[a]; O.wl[n] = I.wl[a];
+  if (I.finish) O.finish[n] = I.finish[a];
+  if (I.lq) O.lq[n] = I.lq[a];
+  if (I.evicting) O.evicting[n] = I.evicting[a];
+  if (I.phase) O.phase[n] = I.phase[a];
+  if (I.since) O.since[n] = I.since[a];
+  if (I.rc_next) { O.rc_next[n] = I.rc_next[a]; O.rc_cur[n] = I.rc_cur[a]; }
+}
+// live rows of [0, bound), in order, into the other half O of the double buffer; thread bound writes the totals
+__global__ void k_drain_compact(DrainDev X, AdmRows O, int bound) {
   int a = blockIdx.x * blockDim.x + threadIdx.x;
   if (a > bound) return;
   if (a == bound) { O.use_start[X.row_new[a]] = X.cell_new[a]; X.counters[KB_DC_ROWS] = X.row_new[a]; X.counters[KB_DC_CELLS] = X.cell_new[a]; return; }
   if (!X.row_live[a]) return;
-  const int n = X.row_new[a], c0 = X.cell_new[a], u0 = X.adm_use_start[a], nc = X.adm_use_start[a + 1] - u0;
-  O.cq[n] = X.adm_cq[a]; O.priority[n] = X.adm_priority[a]; O.ts[n] = X.adm_ts[a]; O.qr_ts[n] = X.adm_qr_ts[a];
-  O.uid[n] = X.adm_uid[a]; O.evicted[n] = X.adm_evicted[a]; O.wl[n] = X.adm_wl[a]; O.use_start[n] = c0;
-  if (X.adm_finish) O.finish[n] = X.adm_finish[a];
-  if (X.adm_lq) O.lq[n] = X.adm_lq[a];
-  if (X.adm_evicting) O.evicting[n] = X.adm_evicting[a];
-  if (X.adm_phase) O.phase[n] = X.adm_phase[a];
-  if (X.adm_exec_since) O.since[n] = X.adm_exec_since[a];
-  if (X.adm_rc_next) { O.rc_next[n] = X.adm_rc_next[a]; O.rc_cur[n] = X.adm_rc_cur[a]; }
-  for (int c = 0; c < nc; c++) { O.use_fr[c0 + c] = X.adm_use_fr[u0 + c]; O.use_qty[c0 + c] = X.adm_use_qty[u0 + c]; }
+  const int n = X.row_new[a], c0 = X.cell_new[a], u0 = X.adm.use_start[a], nc = X.adm.use_start[a + 1] - u0;
+  drain_copy_row(X.adm, a, O, n);
+  O.use_start[n] = c0;
+  for (int c = 0; c < nc; c++) { O.use_fr[c0 + c] = X.adm.use_fr[u0 + c]; O.use_qty[c0 + c] = X.adm.use_qty[u0 + c]; }
 }
 
 // ---- event mode ---------------------------------------------------------------------------------------------------
 __device__ __forceinline__ i64 ev_time(u64 key) { return (i64)(key ^ 0x8000000000000000ull); }
-// first i in [lo, n) with arr_key[i] > t (the creations up to t are [.., i))
-__device__ __forceinline__ int ev_upper_bound(const u64 *key, int lo, int n, i64 t) {
-  const u64 k = (u64)t ^ 0x8000000000000000ull;
-  int hi = n;
+// first i in [lo, hi) with key[i] > k (the keys up to k are [.., i)); key ascending
+template <class K> __device__ __forceinline__ int drain_upper_bound(const K *key, int lo, int hi, K k) {
   while (lo < hi) { const int m = lo + (hi - lo) / 2; if (key[m] <= k) lo = m + 1; else hi = m; }
   return lo;
+}
+__device__ __forceinline__ int ev_upper_bound(const u64 *key, int lo, int n, i64 t) {  // the creations up to t
+  return drain_upper_bound(key, lo, n, (u64)t ^ 0x8000000000000000ull);
 }
 // sort keys of the arrival order: creation time, then index (the radix sort is stable)
 __global__ void k_drain_keys_create(int W, const i64 *create, u64 *keys, int32_t *vals) {
@@ -914,8 +962,8 @@ __global__ void k_drain_ev_min(DrainDev X, int bound, const int32_t *n_new) {
   const int n_rows = X.A + (n_new ? *n_new : 0);
   i64 v = INT64_MAX;
   if (a < bound && a < n_rows && X.adm_dead[a] != X.cycle + 1) {
-    v = X.adm_finish[a];
-    if (X.adm_rc_next && drain_rc_live(X, a)) v = min(v, X.adm_rc_next[a]);  // the row's next reclaim step
+    v = X.adm.finish[a];
+    if (X.adm.rc_next && drain_rc_live(X, a)) v = min(v, X.adm.rc_next[a]);  // the row's next reclaim step
   }
   if (a == 0 && X.counters[KB_DC_ARR_HI] < X.n_arr) v = min(v, ev_time(X.arr_key[X.counters[KB_DC_ARR_HI]]));
   if (a == 0 && X.qc_ns && X.counters[KB_DC_QC_HI] < X.n_qc) v = min(v, X.qc_ns[X.counters[KB_DC_QC_HI]]);  // the next edit
@@ -929,7 +977,7 @@ __global__ void k_drain_ev_min(DrainDev X, int bound, const int32_t *n_new) {
 __global__ void k_drain_ev_next(DrainDev X, i64 t_c, i64 step, int jump, const int32_t *n_new) {
   const i64 E = min(X.clock[1], X.clock[2]);  // [2]: the next RequeueAt (admission checks), INT64_MAX otherwise
   X.clock[2] = INT64_MAX;
-  const i64 stepped = t_c > INT64_MAX - step ? INT64_MAX : t_c + step;
+  const i64 stepped = drain_sat_add(t_c, step);
   const bool active = !jump && ((n_new && *n_new > 0) || X.counters[KB_DC_EVICTED] > 0);
   i64 tn;
   bool end = false;
@@ -943,36 +991,39 @@ __global__ void k_drain_ev_next(DrainDev X, i64 t_c, i64 step, int jump, const i
   X.counters[KB_DC_ARR_LO] = lo;
   X.counters[KB_DC_ARR_HI] = (end || !X.arr_key) ? lo : ev_upper_bound(X.arr_key, lo, X.n_arr, tn);
   if (X.qc_ns) {
-    int qlo = X.counters[KB_DC_QC_HI], qhi = X.n_qc;
+    const int qlo = X.counters[KB_DC_QC_HI];
     X.counters[KB_DC_QC_LO] = qlo;
-    if (end) qhi = qlo;
-    while (qlo < qhi) { const int m = qlo + (qhi - qlo) / 2; if (X.qc_ns[m] <= tn) qlo = m + 1; else qhi = m; }
-    X.counters[KB_DC_QC_HI] = qlo;
+    X.counters[KB_DC_QC_HI] = drain_upper_bound(X.qc_ns, qlo, end ? qlo : X.n_qc, tn);
   }
   if (X.ac_ns) {  // the deactivation / reactivation edits (k_drain_active applies them)
-    int alo = X.counters[KB_DC_AC_HI], ahi = X.n_ac;
+    const int alo = X.counters[KB_DC_AC_HI];
     X.counters[KB_DC_AC_LO] = alo;
-    if (end) ahi = alo;
-    while (alo < ahi) { const int m = alo + (ahi - alo) / 2; if (X.ac_ns[m] <= tn) alo = m + 1; else ahi = m; }
-    X.counters[KB_DC_AC_HI] = alo;
+    X.counters[KB_DC_AC_HI] = drain_upper_bound(X.ac_ns, alo, end ? alo : X.n_ac, tn);
   }
-}
-// a stop at sd (INT64_MAX = none) of row a's record comes before the row's own event at e while the record is active
-__device__ __forceinline__ bool drain_stop_due(const DrainDev &X, int a, i64 sd, i64 e) {
-  return sd < e && X.wl_deactivated[X.adm_wl[a]] == 0;
 }
 // a stop at d of active record w holding row a (before the row leaves): RequeueState cleared, a waiting PodsReady
 // attempt dropped, the Admitted seconds into acc up to the QuotaReserved unset (the end of an eviction under way, else
 // d + latency), reason KB_DR_USER
 __device__ __forceinline__ void drain_stop_row(const DrainDev &X, int a, int w, i64 d) {
   X.wl_deactivated[w] = KB_DR_USER;
-  if (X.wl_pr) { X.wl_pr_count[w] = 0; if (X.wl_pr_at[w] > d) X.wl_pr_at[w] = X.wl_pr_prev[w]; }
-  if (X.wl_requeue_at) X.wl_requeue_at[w] = INT64_MIN;
+  drain_clear_requeue(X, w);
+  drain_drop_attempt(X, w, d);
   if (X.wl_max_exec) {
-    const bool rel = X.adm_evicting && X.adm_evicting[a];
-    drain_exec_release(X, a, w, rel ? X.adm_finish[a] : X.wl_evict ? drain_sat_add(d, X.wl_evict[w]) : d);
+    const bool rel = X.adm.evicting && X.adm.evicting[a];
+    drain_exec_release(X, a, w, rel ? X.adm.finish[a] : X.wl_evict ? drain_sat_add(d, X.wl_evict[w]) : d);
   }
   X.wl_gone[w] = d;
+}
+// a stop at sd (INT64_MAX = none) of row a's record comes before the row's own event while the record is active
+__device__ __forceinline__ bool drain_stop_due(const DrainDev &X, int a, i64 sd) {
+  return sd < X.adm.finish[a] && X.wl_deactivated[X.adm.wl[a]] == 0;
+}
+// whether a stop at sd or the own event of running row a is due at this boundary (stop: the stop), after the reclaim
+// steps before it: strictly before its finish column, at or before a stop (an own event first)
+__device__ __forceinline__ bool drain_row_due(const DevSnap &D, const DrainDev &X, int a, i64 sd, bool &stop) {
+  stop = drain_stop_due(X, a, sd);
+  if (X.wl_rc_start && drain_rc_live(X, a)) drain_reclaim(D, X, a, stop ? sd : min(X.clock[0], X.adm.finish[a] - 1));
+  return stop || X.adm.finish[a] <= X.clock[0];
 }
 // completions (thread per row): a live row with finish <= t_{c+1} gets the dead stamp, its cells leave its ClusterQueue's
 // usage (cache.DeleteWorkload, integer atomics), its record becomes FINISHED and its root tree is marked.  An evicting
@@ -985,41 +1036,27 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
   if (a >= bound || a >= X.A + (n_new ? *n_new : 0) || X.counters[KB_DC_FULL]) return;
   const int stamp = X.cycle + 1;
   if (X.counters[KB_DC_END] || X.adm_dead[a] == stamp) return;
-  const i64 sd = X.wl_stop ? X.wl_stop[X.adm_wl[a]] : INT64_MAX;  // a stop edit of the record at this boundary
-  bool stop = drain_stop_due(X, a, sd, X.adm_finish[a]);
-  // reclaim steps of a running row: strictly before its finish column, and at or before a stop (an own event first)
-  if (X.wl_rc_start && drain_rc_live(X, a)) drain_reclaim(D, X, a, stop ? sd : min(X.clock[0], X.adm_finish[a] - 1));
-  if (!stop && X.adm_finish[a] > X.clock[0]) return;
-  const int cq = X.adm_cq[a];
-  int ph = X.adm_phase ? X.adm_phase[a] : KB_PH_RUN;
+  const i64 sd = X.wl_stop ? X.wl_stop[X.adm.wl[a]] : INT64_MAX;  // a stop edit of the record at this boundary
+  bool stop;
+  if (!drain_row_due(D, X, a, sd, stop)) return;
+  const int cq = X.adm.cq[a], w = X.adm.wl[a];
+  int ph = X.adm.phase ? X.adm.phase[a] : KB_PH_RUN;
   if (!stop && ph == KB_PH_CHECK) {  // a verdict (ProvisioningRequest controller.go:536-580)
-    const int w = X.adm_wl[a];
-    const i64 tv = X.adm_finish[a];
-    X.adm_phase[a] = KB_PH_RUN;
+    const i64 tv = X.adm.finish[a];
     if (X.wl_fail[w] == 0) {  // Ready: Admitted, the run clock (or the PodsReady attempt) starts; it may end in this boundary
-      const i64 run = X.wl_run ? X.wl_run[w] : -1;
-      i64 fin = X.wl_pr ? drain_pr_attempt(X, a, w, tv) : run < 0 ? INT64_MAX : (tv > INT64_MAX - run ? INT64_MAX : tv + run);
-      X.wl_ready_ns[w] = tv;
-      const bool rc_run = X.wl_rc_start && (!X.wl_pr || X.adm_phase[a] == KB_PH_RUN);  // the run starts (a ready attempt)
-      if (rc_run) drain_rc_begin(X, a, w, X.wl_pr ? X.wl_pr_at[w] : tv);
-      if (X.wl_max_exec) { X.adm_exec_since[a] = tv; fin = drain_exec_clip(X, a, w, tv, fin); }
-      X.adm_finish[a] = fin;
+      drain_admitted(X, a, w, tv);
       atomicAdd(&X.counters[KB_DC_CHECK_READY], 1);
-      stop = drain_stop_due(X, a, sd, fin);
-      if (rc_run) drain_reclaim(D, X, a, stop ? sd : min(X.clock[0], fin - 1));
-      if (!stop && fin > X.clock[0]) return;
-      ph = X.adm_phase[a];
+      if (!drain_row_due(D, X, a, sd, stop)) return;
+      ph = X.adm.phase[a];
     } else {  // Retry or Rejected: the workload holds no pods, its quota goes at once
       if (X.wl_fail[w] != INT32_MAX) X.wl_fail[w]--;
       const int k = X.wl_retries[w] + 1;
       X.adm_dead[a] = stamp;
-      for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)
-        atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
+      drain_uncharge(D, X, a, false);
       drain_forget(D, X, w);
       if (k <= X.check_limit) {  // Retry: RequeueAt = verdict + WaitTime(k), queue-order timestamp = the eviction time
-        const i64 wait = kb_check_wait_ns(k, X.check_base_s, X.check_max_s);
         X.wl_retries[w] = k;
-        X.wl_requeue_at[w] = tv > INT64_MAX - wait ? INT64_MAX : tv + wait;
+        X.wl_requeue_at[w] = drain_sat_add(tv, kb_check_wait_ns(k, X.check_base_s, X.check_max_s));
         X.wl_qts[w] = tv;
         X.wl_state[w] = KB_WS_BACKOFF;
         atomicAdd(&X.counters[KB_DC_CHECK_RETRY], 1);
@@ -1032,9 +1069,8 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
       return;
     }
   }
-  const int w = X.adm_wl[a];
+  const i64 T = X.adm.finish[a];  // the time of a timeout or an expiry
   if (!stop && ph == KB_PH_WAIT) {  // PodsReady timeout at T (workload_controller.go:805-855, UpdateRequeueState workload.go:707-722)
-    const i64 T = X.adm_finish[a];
     if (X.wl_pr_fail[w] > 0 && X.wl_pr_fail[w] != INT32_MAX) X.wl_pr_fail[w]--;
     const int n = X.wl_pr_count[w];
     if (X.pr_limit >= 0 && n >= X.pr_limit) {  // Count + 1 > limit: deactivated, RequeueState cleared
@@ -1048,46 +1084,29 @@ __global__ void k_drain_finish(DevSnap D, DrainDev X, int bound, const int32_t *
       if (!X.pr_creation) X.wl_qts[w] = T;
       atomicAdd(&X.counters[KB_DC_PR_TIMEOUT], 1);
     }
-    ph = KB_PH_TIMED_OUT;
-    X.adm_phase[a] = ph;
-    if (X.wl_evict) {  // the pods terminate: the row holds its cells until T + latency, as an evicting row
-      X.adm_evicted[a] = 1;
-      X.adm_evicting[a] = 1;
-      X.adm_finish[a] = drain_sat_add(T, X.wl_evict[w]);
-      stop = drain_stop_due(X, a, sd, X.adm_finish[a]);
-      if (!stop && X.adm_finish[a] > X.clock[0]) return;
-    }
-  }
-  if (!stop && ph == KB_PH_EXPIRE) {  // MaximumExecutionTimeExceeded at the effective deadline (workload_controller.go:619-646)
-    const i64 dl = X.adm_finish[a];
+  } else if (!stop && ph == KB_PH_EXPIRE) {  // MaximumExecutionTimeExceeded at the effective deadline T (workload_controller.go:619-646)
     drain_exec_deactivate(X, w);
-    if (X.wl_pr && X.wl_pr_at[w] > dl) X.wl_pr_at[w] = X.wl_pr_prev[w];  // a PodsReady attempt still waiting is dropped
+    drain_drop_attempt(X, w, T);  // a PodsReady attempt still waiting is dropped
+  }
+  if (!stop && (ph == KB_PH_WAIT || ph == KB_PH_EXPIRE)) {
     ph = KB_PH_TIMED_OUT;
-    X.adm_phase[a] = ph;
-    if (X.wl_evict) {  // evicted at the deadline: the row holds its cells until deadline + latency, as an evicting row
-      X.adm_evicted[a] = 1;
-      X.adm_evicting[a] = 1;
-      X.adm_finish[a] = drain_sat_add(dl, X.wl_evict[w]);
-      if (X.adm_finish[a] > X.clock[0]) return;
+    X.adm.phase[a] = ph;
+    if (X.wl_evict) {  // the pods terminate: the row holds its cells until T + latency, as an evicting row (no steps)
+      drain_evict_row(X, a, w, T);
+      stop = drain_stop_due(X, a, sd);  // an expiry deactivated the record: no stop is due
+      if (!stop && X.adm.finish[a] > X.clock[0]) return;
     }
   }
   if (stop) drain_stop_row(X, a, w, sd);
-  else if (X.wl_gone) X.wl_gone[w] = X.adm_finish[a];
+  else if (X.wl_gone) X.wl_gone[w] = X.adm.finish[a];
   X.adm_dead[a] = stamp;
-  for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)
-    atomicAdd((unsigned long long *)&X.cq_usage[(size_t)cq * D.FR + X.adm_use_fr[c]], (unsigned long long)(-X.adm_use_qty[c]));
+  drain_uncharge(D, X, a, true);
   const bool timed_out = !stop && ph == KB_PH_TIMED_OUT;
-  const bool released = !stop && X.adm_evicting && X.adm_evicting[a];
-  const bool expired = X.wl_max_exec && (timed_out || released) && drain_exec_release(X, a, w, X.adm_finish[a]);
-  if (stop) { drain_forget(D, X, w); X.wl_state[w] = KB_WS_DEACTIVATED; }
-  else if (timed_out || expired) { drain_forget(D, X, w); X.wl_state[w] = X.wl_deactivated[w] ? KB_WS_DEACTIVATED : KB_WS_BACKOFF; }
+  const bool released = !stop && X.adm.evicting && X.adm.evicting[a];
+  const bool expired = X.wl_max_exec && (timed_out || released) && drain_exec_release(X, a, w, X.adm.finish[a]);
+  if (stop || timed_out || expired) { drain_forget(D, X, w); X.wl_state[w] = X.wl_deactivated[w] ? KB_WS_DEACTIVATED : KB_WS_BACKOFF; }
   else if (released) drain_release(D, X, w);
-  else if (w >= 0) { X.wl_state[w] = KB_WS_FINISHED; X.wl_admit_cycle[w] = -1; X.wl_finish_ns[w] = X.adm_finish[a]; }
-  if (X.lq_last && X.adm_lq[a] >= 0 && X.cq_afs[cq]) {  // several rows of one LocalQueue can finish together
-    i64 *adm = X.lq_adm + (size_t)X.adm_lq[a] * D.R;
-    for (int c = X.adm_use_start[a]; c < X.adm_use_start[a + 1]; c++)
-      atomicAdd((unsigned long long *)&adm[X.adm_use_fr[c] % D.R], (unsigned long long)(-X.adm_use_qty[c]));
-  }
+  else if (w >= 0) { X.wl_state[w] = KB_WS_FINISHED; X.wl_admit_cycle[w] = -1; X.wl_finish_ns[w] = X.adm.finish[a]; }
   X.root_mark[D.root_slot[cq]] = stamp;
   if (!timed_out) atomicAdd(&X.counters[stop ? KB_DC_STOPPED : released ? KB_DC_EVICT_DONE : KB_DC_FINISHED], 1);
 }
@@ -1128,21 +1147,11 @@ __global__ void k_drain_afs_decay(DevSnap D, DrainDev X, int L) {
   }
   if (bad) atomicOr(D.status, KBS_AFS_OVERFLOW);
 }
-// arrivals (grid-stride over the arrived prefix [lo, hi)): the workload joins its queue and the cursor moves back to it;
-// in a BestEffortFIFO ClusterQueue a known hash in the NoFit set sets it aside (PushOrUpdate, cluster_queue.go:288-293)
+// arrivals (grid-stride over the arrived prefix [lo, hi)): each workload joins its queue (drain_enqueue)
 __global__ void k_drain_arrive(DrainDev X) {
   const int lo = X.counters[KB_DC_ARR_LO], hi = X.counters[KB_DC_ARR_HI];
   if (blockIdx.x == 0 && threadIdx.x == 0) X.counters[KB_DC_ARRIVED] = hi - lo;
-  for (int i = lo + blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += gridDim.x * blockDim.x) {
-    const int w = X.arr_order[i], s = X.wl_seg[w], p = X.wl_pos[w];
-    if (X.class_nofit && X.wl_class[w] >= 0 && X.class_nofit[X.wl_class[w]]) {
-      X.wl_state[w] = KB_WS_SET_ASIDE;
-      atomicMin(&X.first_aside[s], p);
-    } else {
-      X.wl_state[w] = KB_WS_QUEUED;
-      atomicMin(&X.cursor[s], p);
-    }
-  }
+  for (int i = lo + blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += gridDim.x * blockDim.x) drain_enqueue(X, X.arr_order[i]);
 }
 
 // ---- quota changes -----------------------------------------------------------------------------------------------------
@@ -1197,8 +1206,7 @@ __device__ __forceinline__ void drain_active_edit(const DevSnap &D, const DrainD
     if (X.wl_deactivated[w] != 0 || (st != KB_WS_QUEUED && st != KB_WS_SET_ASIDE && st != KB_WS_BACKOFF)) return;
     X.wl_state[w] = KB_WS_DEACTIVATED;
     X.wl_deactivated[w] = KB_DR_USER;
-    if (X.wl_pr) X.wl_pr_count[w] = 0;
-    if (X.wl_requeue_at) X.wl_requeue_at[w] = INT64_MIN;
+    drain_clear_requeue(X, w);
     const int cq = D.wl_cq[w];
     if (X.cq_sticky && X.cq_sticky[cq] == w) X.cq_sticky[cq] = -1;  // delete (cluster_queue.go:330-340)
     X.root_mark[D.root_slot[cq]] = X.cycle + 1;
@@ -1207,15 +1215,8 @@ __device__ __forceinline__ void drain_active_edit(const DevSnap &D, const DrainD
   } else if (st == KB_WS_DEACTIVATED) {
     X.wl_deactivated[w] = 0;
     drain_forget(D, X, w);
-    const int s = X.wl_seg[w], p = X.wl_pos[w];
-    if (X.class_nofit && X.wl_class[w] >= 0 && X.class_nofit[X.wl_class[w]]) {
-      X.wl_state[w] = KB_WS_SET_ASIDE;
-      atomicMin(&X.first_aside[s], p);
-    } else {
-      X.wl_state[w] = KB_WS_QUEUED;
-      atomicMin(&X.cursor[s], p);
-    }
-    if (X.wl_sort_ts && X.wl_sort_ts[w] != X.wl_qts[w]) X.counters[KB_DC_RESORT] = X.cycle + 1;
+    drain_enqueue(X, w);
+    drain_mark_resort(X, w);
     atomicAdd(&X.counters[KB_DC_RESUMED], 1);
   }
 }
@@ -1271,15 +1272,8 @@ __global__ void k_drain_backoff(DrainDev X, int W) {
   if (w >= W || X.wl_state[w] != KB_WS_BACKOFF) return;
   const i64 at = X.wl_requeue_at[w];
   if (at > X.clock[0]) { atomicMin((long long *)&X.clock[2], (long long)at); return; }
-  const int s = X.wl_seg[w], p = X.wl_pos[w];
-  if (X.class_nofit && X.wl_class[w] >= 0 && X.class_nofit[X.wl_class[w]]) {
-    X.wl_state[w] = KB_WS_SET_ASIDE;
-    atomicMin(&X.first_aside[s], p);
-  } else {
-    X.wl_state[w] = KB_WS_QUEUED;
-    atomicMin(&X.cursor[s], p);
-  }
-  if (X.wl_sort_ts[w] != X.wl_qts[w]) X.counters[KB_DC_RESORT] = X.cycle + 1;
+  drain_enqueue(X, w);
+  drain_mark_resort(X, w);
 }
 // re-sort: every cursor back to 0 and no set-aside position, then the SET_ASIDE positions of the new order
 __global__ void k_drain_resort_reset(DrainDev X, int S) {
